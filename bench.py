@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- pgvector's distance hot path on B200, one JSON line per run (BASELINE.json metric and configs).
+"""bench.py -- pgvector's distance hot path on H100, one JSON line per run (BASELINE.json metric and configs).
 
   python bench.py [--config B] [--gpus N --steps K --warmup W] [--impl reference]
 
@@ -8,7 +8,7 @@
   A  exact L2 <-> scan, 10k x 128 fp32, k = 10                      (no index; the CPU-runnable parity case)
   B  IVFFlat L2 1M x 1536 fp32, lists = 1000, probes = 10, k = 10   (HEADLINE: queries/s, 2048-query batches)
   C  HNSW cosine 1M x 768 halfvec, ef_search = 100                  (graph built on the GPU by vb_hnsw_build)
-  D  IVFFlat k-means build 10M x 1536, lists = 4096                 (rows sharded over the ranks; k-means++ + Lloyd + assign)
+  D  IVFFlat k-means build 4M x 1536 per GPU (at most 10M), lists = 4096   (rows sharded over the ranks; k-means++ + Lloyd + assign)
   E  HNSW Hamming 10M x bit(1024), ef_search = 200
 
 A "step" is one pass of the hot path over one batch of synthetic input (D: one complete build).
@@ -25,8 +25,12 @@ vb_ivf_scan_lists + vb_ivf_scan_items (`batch_sweep`), and the per-query fused-s
 (`north_star_kernel`, scan_impl 1) with its own roofline.  Under torchrun the lists are sharded over the ranks
 (`scaling: strong`, exchanges inside the library over NCCL) and the replica mode is measured beside it.
 
-Both arms share ONE index: whichever arm runs first writes centres + assignment to a cache under /tmp; the other
-loads it (`config.index_build` says which happened)."""
+Both arms share ONE index: whichever arm runs first writes centres + assignment to a cache in the temporary directory;
+the other loads it (`config.index_build` says which happened).
+
+--dump-outputs DIR (config B) writes what the last timed step returned to its caller: DIR/ids.npy (float64 heap ids)
+and DIR/distances.npy (float32), one row per query of the batch.  Inputs are seeded, so two builds of the project run
+with the same arguments can be compared output for output."""
 from __future__ import annotations
 
 import argparse
@@ -35,6 +39,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -49,7 +54,7 @@ try:    # the metric is BASELINE.json's, verbatim
 except Exception:
     METRIC = "IVFFlat 1M×1536d queries/sec at 1/2/4/8 GPU; recall@10; HBM GB/s vs roofline"
 
-CACHE_DIR = os.environ.get("VB_BENCH_CACHE", "/tmp/pgvector_b200_bench")
+CACHE_DIR = os.environ.get("VB_BENCH_CACHE", os.path.join(tempfile.gettempdir(), "pgvector_b200_bench"))
 D_METRIC = "IVFFlat k-means build (BASELINE.json configs[3]): rows indexed per second (k-means++ seeding + k-means on the samples + assign of all rows)"
 
 
@@ -78,14 +83,21 @@ def parse_args():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-recall", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="config B: skip batch sweep / north-star kernel / second law")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="config B: write the last timed step's results (ids, distances) as .npy files into DIR")
     ap.add_argument("--scan-impl", type=int, default=int(os.environ.get("VB_SCAN_IMPL", "2")),
                     help="0 = per-query LDG.128 scan, 1 = per-query cp.async.bulk (TMA) scan, 2 = library default "
                          "(query batches: tensor-core filter + exact re-score), 3 = list-major fp32, 4 = tensor-core filter")
     a = ap.parse_args()
+    if a.dump_outputs is not None and (a.config != "B" or a.impl != "ours"):
+        ap.error("--dump-outputs is implemented for --config B --impl ours")
     d = {"A": dict(rows=10_000, dim=128, lists=0, batch=1000, steps=100, warmup=3),
          "B": dict(rows=1_000_000, dim=1536, lists=1000, batch=2048, steps=100, warmup=3),
          "C": dict(rows=1_000_000, dim=768, lists=0, batch=10_000, steps=20, warmup=3),
-         "D": dict(rows=10_000_000, dim=1536, lists=4096, batch=0, steps=3, warmup=1),
+         # D keeps two device copies of a rank's rows while they load (the caller's tensor and the library's table):
+         # 4M x 1536 fp32 per 80 GB H100 (2 x 24.6 GB), at most the 10M of the sharded configuration
+         "D": dict(rows=min(10_000_000, 4_000_000 * int(os.environ.get("WORLD_SIZE", "1"))), dim=1536, lists=4096, batch=0, steps=3,
+                   warmup=1),
          "E": dict(rows=10_000_000, dim=1024, lists=0, batch=10_000, steps=20, warmup=3)}[a.config]
     for key, v in d.items():
         if getattr(a, key) is None:
@@ -145,7 +157,7 @@ class near_gpu:
 class ClockSampler:
     # Sampled every 200 ms (the period of the profiling recipe).  A query is not free: with `-lms 20` and power.draw in
     # the list the end-to-end step of config B measured 1.69 ms under the sampler against 0.98 ms without it
-    # (profiles/r2_diag_e2e.json) -- the driver serialises the query with the process's copies and synchronisations.
+    # -- the driver serialises the query with the process's copies and synchronisations.
     # power.draw (the slow sensor read) is not used by the line, so it is not queried; the placeholder keeps the columns.
     FIELDS = ("clocks.sm,clocks.max.sm,clocks.mem,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -193,8 +205,8 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", 1417.3)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1417.3, "fallback (B200_PROFILING.md)"
+        return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", 989.0)), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, 989.0, "fallback (H100 SXM data sheet: HBM3, dense BF16)"
 
 
 class Env:
@@ -511,7 +523,7 @@ def measure_ivf(env, args, law, centers, offsets, grouped, order, full, queries)
     env.barrier()
     # The timed region carries the per-kernel event brackets (the roofline's kernel time is measured over it); the
     # traffic accounting -- an extra kernel per filter launch that walks the launch's job list -- runs over two
-    # identical steps AFTER it (it cost 4-7 % of `value` inside, profiles/r2_diag_e2e_v2.json).
+    # identical steps AFTER it (inside, it cost a few % of `value`).
     pv.prof_enable(True)
     for p in (pv.PROF_SCAN_ITEMS, pv.PROF_SCAN_LISTS, pv.PROF_TOPK, pv.PROF_LIST_TC, pv.PROF_CENTRE_TC):
         pv.prof_read(p)
@@ -524,6 +536,7 @@ def measure_ivf(env, args, law, centers, offsets, grouped, order, full, queries)
     env.barrier()
     ms = env.max_over_ranks(e0.elapsed_time(e1))
     launches = pv.launch_count() - l0
+    last_out = (ids_dev.cpu().numpy(), dist_dev.cpu().numpy()) if args.dump_outputs is not None and full else None
     prof = {name: pv.prof_read(p) for name, p in (("scan_items", pv.PROF_SCAN_ITEMS), ("scan_lists", pv.PROF_SCAN_LISTS),
                                                    ("topk", pv.PROF_TOPK), ("list_tc", pv.PROF_LIST_TC), ("centre_tc", pv.PROF_CENTRE_TC))}
     pv.prof_enable(False)
@@ -590,7 +603,7 @@ def measure_ivf(env, args, law, centers, offsets, grouped, order, full, queries)
     # ---- roofline of the dominant kernel, from live CUDA events and the launch's own job list
     peak, _, peak_src = measured_peaks()
     roofline = roofline_ivf(args, ix, prof, traffic, cand_last, cand_all, B, ms, peak, peak_src, world)
-    return dict(ix=ix, qps=qps, ms=ms, launches=int(launches), e2e=e2e, roofline=roofline, clocks=clocks, upload_s=upload_s,
+    return dict(ix=ix, qps=qps, ms=ms, last_out=last_out, launches=int(launches), e2e=e2e, roofline=roofline, clocks=clocks, upload_s=upload_s,
                 cand_all=cand_all, qbatches=qbatches)
 
 
@@ -607,7 +620,7 @@ def roofline_ivf(args, ix, prof, traffic, cand_last, cand_all, B, ms, peak, peak
         moved = a_once + b_once + out_bytes
         level = 1 if ix.tc_level1_fallbacks() == 0 else 2
         achieved = moved / (kern_ms / 1000.0) / 1e9
-        r = {"bound": "hbm", "kernel": "list_tc_kernel (GetScanItems list scan, tcgen05 filter level %d)" % level,
+        r = {"bound": "hbm", "kernel": "list_tc_kernel (GetScanItems list scan, wgmma filter level %d)" % level,
              "achieved": achieved, "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": achieved / peak,
              "traffic": moved, "traffic_source": "computed live from the launch's job list (vb_ivf_tc_traffic): distinct "
                         "row-plane tiles + distinct query tiles + candidate distances written; the ncu capture is the cross-check",
@@ -795,11 +808,12 @@ def run_b_ours(args):
         del rows
         torch.cuda.empty_cache()
         full = li == 0
-        saved_steps = args.steps
-        if not full:
-            args.steps = max(10, args.steps // 4)
         m = measure_ivf(env, args, law, centers, offsets, grouped, order, full, queries)
-        args.steps = saved_steps
+        if m.get("last_out") is not None and env.rank == 0:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            ids, dist = m["last_out"]
+            np.save(os.path.join(args.dump_outputs, "ids.npy"), ids.astype(np.float64))
+            np.save(os.path.join(args.dump_outputs, "distances.npy"), dist.astype(np.float32))
         extras = {}
         oix = None
         if env.world == 1 and env.rank == 0 and not args.no_cpu:
@@ -820,7 +834,7 @@ def run_b_ours(args):
             primary = dict(m=m, law=law, how=how, extras=extras, replica=replica)
         else:
             second[law] = {"data_law": law_name(args, law), "index_build": how, "value": m["qps"], "unit": "queries/s",
-                           "ms_per_step": m["ms"] / max(10, saved_steps // 4), "steps": max(10, saved_steps // 4),
+                           "ms_per_step": m["ms"] / args.steps, "steps": args.steps,
                            "e2e": m["e2e"], "roofline": m["roofline"], "candidates_per_query": m["cand_all"] / min(args.batch, args.queries),
                            **extras}
         m["ix"].free()
@@ -833,8 +847,8 @@ def run_b_ours(args):
             index_upload_s=m["upload_s"], candidates_per_query=m["cand_all"] / B,
             l2_policy="inputs larger than L2: every step reads the probed lists of a %d MB table once" % (args.rows * args.dim * 4 // env.world // 2**20),
             scan_kernel={0: "per-query LDG.128 streaming (all scans)", 1: "per-query cp.async.bulk + mbarrier staged (all scans)",
-                         3: "list-major fp32x2 register tiles (rows read once per batch)"}.get(
-                args.scan_impl, "query batches: tcgen05 split-bf16 filter over packed row planes (each probed list read once per batch; level 1 = "
+                         3: "list-major fp32 register tiles (rows read once per batch)"}.get(
+                args.scan_impl, "query batches: wgmma split-bf16 filter over packed row planes (each probed list read once per batch; level 1 = "
                                 "hi plane, level 2 = both planes on certificate failure) + exact fp32 re-score + certificate; exact kernel last"),
             parallelism=("lists sharded l % N; probe selection sharded over the queries; two NCCL all-gathers inside libvecb200 "
                          "(probe lists, per-rank top-k) + k-way merge kernel" if env.world > 1 else "single GPU")))
@@ -1254,7 +1268,7 @@ def run_d(args):
         lens = counts.cpu().numpy()
         line = {"metric": D_METRIC,
                 "value": args.rows / step_s, "unit": "rows/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
-                "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32 (assign: split-bf16 tcgen05 products, exact fp32 re-check)",
+                "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32 (assign: split-bf16 wgmma products, exact fp32 re-check)",
                 "data": "synthetic",
                 "config": {"workload": f"IVFFlat k-means build {args.rows}x{args.dim} fp32, lists={args.lists}, samples={ns_local * world} (BASELINE.json configs[3])",
                            "data_law": f"mixture of {args.lists} Gaussians (sigma 0.3), seeds 3 / 1000 + rank", "parallelism":
@@ -1283,7 +1297,7 @@ def roofline_d(args, world, ns_local, a_ms, a_n, builds, tf_peak, peak_src, res)
     rows_scored = (per_build - 1) * ns_local + args.rows / world          # per build, per rank
     issued = 3.0 * 2.0 * rows_scored * args.lists * args.dim * builds
     tf = issued / (a_ms / 1000.0) / 1e12
-    return {"bound": "tensor", "kernel": "assign_tc_kernel (tcgen05 split-bf16 GEMM + fused argmin) + exact re-check of flagged rows",
+    return {"bound": "tensor", "kernel": "assign_tc_kernel (wgmma split-bf16 GEMM + fused argmin) + exact re-check of flagged rows",
             "achieved": tf, "peak": tf_peak, "peak_source": peak_src, "unit": "TFLOP/s", "frac": tf / tf_peak, "traffic": None,
             "useful_tflops": tf / 3.0, "assign_launches_per_build": per_build, "ms_per_build_in_assign": a_ms / builds,
             "note": "issued bf16 MMA flops (3 products per fp32-accurate term) over the CUDA-event time of every assign call of a build "

@@ -1,5 +1,5 @@
 /*
- * vecb200.h -- C ABI of libvecb200.so: the B200 (sm_100a) implementation of
+ * vecb200.h -- C ABI of libvecb200.so: the H100 (sm_90a) implementation of
  * pgvector's batched-distance hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  Every entry point takes plain
@@ -15,7 +15,7 @@
  *     backend) turns it into ereport(ERROR) AFTER the call returns, so no device
  *     state is held across a longjmp.
  *   - there is NO CPU fallback: every call fails with VB_ENODEVICE when no
- *     sm_100 device is usable.
+ *     sm_90 device is usable.
  *   - "host" pointers are ordinary process memory; "_dev" variants take device
  *     pointers valid on the library's current device.  Work is enqueued on the
  *     library stream (vb_stream()); host-buffer variants synchronise before
@@ -46,7 +46,7 @@ extern "C" {
 /* status codes */
 #define VB_OK 0
 #define VB_EINVAL (-1)			/* bad argument (dimension mismatch, unsupported metric for type, ...) */
-#define VB_ENODEVICE (-2)		/* no usable sm_100 device / CUDA failure at init */
+#define VB_ENODEVICE (-2)		/* no usable sm_90 device / CUDA failure at init */
 #define VB_ECUDA (-3)			/* CUDA runtime error */
 #define VB_ENOMEM (-4)			/* device or host allocation failed */
 #define VB_ESTATE (-5)			/* call sequence error (index not loaded, ...) */
@@ -111,7 +111,7 @@ int			vb_prof_read(int kernel, double *total_ms, int64_t *launches);
  * float8 the fmgr wrapper returns.  Replaces n calls of
  * FunctionCall2Coll(procinfo, collation, row, q) -> l2_distance / ... / jaccard_distance
  * (src/vector.c:576-750, src/halfvec.c:557-686, src/bitvec.c:33-70).
- * dim is elements (bits for VB_BIT).  q == NULL gives all zeros (ZeroDistance, src/ivfscan.c:192-196).
+ * dim is elements (bits for VB_BIT; 0 is a valid bit length).  q == NULL gives all zeros (ZeroDistance, src/ivfscan.c:192-196).
  */
 int			vb_distance_batch(int elem, int metric, int dim, const void *q,
 							  const void *rows, int64_t n, double *out);
@@ -370,7 +370,7 @@ int			vb_kmeans_pp_init_draws(vb_table *samples, int kmeans_metric, void *center
 int			vb_assign(vb_table *rows, int metric, const void *centers, int k, int32_t *out_list);
 int			vb_assign_dev(vb_table *rows, int metric, const void *centers_dev, int k, int32_t *out_list_dev);
 /*
- * The assign step runs on the tensor cores (tcgen05, split-bf16 GEMM with a fused row argmin)
+ * The assign step runs on the tensor cores (wgmma, split-bf16 GEMM with a fused row argmin)
  * and re-checks rows whose best/second-best margin is inside the error bound with the exact
  * fp32 kernel.  vb_set_tensor_cores(0) forces the exact CUDA-core kernel for everything
  * (used by the parity tests); vb_last_assign_rechecked() = rows the last assign re-checked
@@ -383,7 +383,7 @@ int64_t		vb_last_assign_rechecked(void);
  * 1 = per-query cp.async.bulk (TMA) + mbarrier staged kernel for rows of at least 512 bytes, 2 (default) =
  * automatic (query batches are scanned list-major: each probed list read once per batch, fp32x2 register
  * tiles; single queries stream), 3 = list-major wherever it applies, 4 = tensor-core filter (split-bf16
- * tcgen05 distances, exact fp32 re-score of k' candidates, certificate, exact fallback) wherever it applies.
+ * tensor-core distances, exact fp32 re-score of k' candidates, certificate, exact fallback) wherever it applies.
  * Every setting returns the same neighbours.  "tc_level1" (default 1): the tensor-core filter first reads only the
  * hi plane of the rows (half the HBM traffic, 2^-7 relative error bound) and repeats a batch with both planes when a
  * certificate fails.  "tensor_cores" as vb_set_tensor_cores.  "one_query" (default 1): calls with at most 16 queries --

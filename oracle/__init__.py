@@ -36,8 +36,8 @@ def _cpu_stamp() -> str:
 
 def build(force: bool = False) -> None:
     """(Re)build liboracle.so for THIS host's CPU (-march=native, the reference's
-    flag) and, when /root/reference is present, oracle/_ref/ from the reference's
-    own sources.  On the GPU box the prebuilt _ref/ is used as shipped."""
+    flag) and, when a pgvector source tree is present, oracle/_ref/ from the reference's
+    own sources.  Elsewhere an existing _ref/ is used as it is."""
     so = os.path.join(HERE, "liboracle.so")
     stamp_path = os.path.join(HERE, ".built_for")
     stamp = _cpu_stamp()

@@ -1,5 +1,5 @@
 """pgvector_b200 -- host-side mirror of pgvector's distance / index-scan interface
-over libvecb200.so (hand-written sm_100a CUDA behind the C ABI of include/vecb200.h).
+over libvecb200.so (hand-written sm_90a CUDA behind the C ABI of include/vecb200.h).
 
 PostgreSQL is not available in this image, so the reference's C host code
 (index AM callbacks) cannot be linked here; the extension-side glue is under
@@ -663,7 +663,7 @@ def tc_traffic(on=True, read=False):
 
 
 def set_tensor_cores(on: bool):
-    """False forces the exact fp32 CUDA-core assign kernel (parity tests); True (default) uses tcgen05."""
+    """False forces the exact fp32 CUDA-core assign kernel (parity tests); True (default) uses the tensor cores (wgmma)."""
     _lib.check(load().vb_set_tensor_cores(1 if on else 0))
 
 

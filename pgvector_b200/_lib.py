@@ -2,7 +2,7 @@
 
 The library is the product; this module only binds it.  There is no Python or
 CPU implementation behind any call: if the shared object is missing or no
-sm_100 device is usable every entry point raises.
+sm_90 device is usable every entry point raises.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-// vb_assign_tc.cu -- nearest-centre assign on the 5th-generation tensor cores (tcgen05 + TMEM).
+// vb_assign_tc.cu -- nearest-centre assign on the Hopper tensor cores (wgmma).
 //
 // The assign pass (AddTupleToSort, src/ivfbuild.c:161-219) and the Lloyd assign step of
 // k-means are the one GEMM-shaped part of the hot path: X[n x d] . C^T[d x k] followed by a
@@ -6,17 +6,17 @@
 //
 // Precision.  The reference evaluates fp32 distances.  Tensor cores take bf16 operands, so
 // both operands are split x = hi + lo (two bf16 planes, |lo| <= 2^-8 |hi|) and three MMAs per
-// K step accumulate hi.hi + hi.lo + lo.hi in fp32 TMEM (the dropped lo.lo term is <= 2^-16 of
+// K step accumulate hi.hi + hi.lo + lo.hi in fp32 registers (the dropped lo.lo term is <= 2^-16 of
 // |x||c|).  The epilogue keeps the best AND the second-best value of every row; rows whose
 // margin is below a rigorous error bound are re-evaluated by the exact fp32 kernel
 // (assign_exact_kernel), so the final list numbers equal the fp32 argmin.  halfvec rows are
 // represented exactly by hi + lo (11-bit significand = 8 + 3).
 //
-// Kernel shape (cta_group::1): CTA tile 128 rows x 256 centres, K step 64 (one 128-byte swizzle
-// atom of bf16), UMMA 128x256x16, two TMEM accumulator stages (2 x 256 columns = the whole TMEM)
-// so the row-argmin epilogue of tile j overlaps the MMAs of tile j+1.  Warp roles: warp 0 lane 0
-// = bulk-copy producer, warp 1 lane 0 = MMA issuer, warp 2 = TMEM allocator, warps 4-7 =
-// epilogue (one TMEM lane = one row per thread: the argmin needs no cross-thread reduction).
+// Kernel shape: CTA tile 128 rows x 256 centres, K step 64 (one 128-byte swizzle atom of bf16).
+// Warps 0-7 are two consumer warpgroups, each issuing wgmma m64n256k16 for 64 rows of the tile
+// (128 fp32 accumulators per thread) and then reducing its fragment to the row-argmin (each row is
+// spread over the 4 lanes of a quad: one xor-shuffle merge at the end of the row tile); warp 8 is
+// the bulk-copy producer feeding a 2 x 96 KB stage ring.
 // Operands live in HBM already in the tiled, 128B-swizzled shared-memory image
 // (pack_planes_kernel), so a stage is filled by two contiguous cp.async.bulk copies (A: 32 KB,
 // B: 64 KB) that complete on an mbarrier -- TMA without tensor maps.
@@ -31,10 +31,11 @@
 
 namespace vb {
 
-constexpr int TC_M = 128;       // rows per CTA tile (= TMEM lanes)
-constexpr int TC_N = 256;       // centres per tile (= UMMA_N, TMEM columns per accumulator stage)
+constexpr int TC_M = 128;       // rows per CTA tile (two warpgroups of 64)
+constexpr int TC_N = 256;       // centres per tile (= wgmma N: 128 fp32 accumulator registers per thread)
 constexpr int TC_STAGES = 2;
-constexpr int TC_THREADS = 256;
+constexpr int TC_CONSUMERS = 256;
+constexpr int TC_THREADS = TC_CONSUMERS + 32;   // + the producer warp
 constexpr uint32_t A_PLANE_BYTES = TC_M * TC_K * 2;   // 16 KB
 constexpr uint32_t B_PLANE_BYTES = TC_N * TC_K * 2;   // 32 KB
 constexpr uint32_t A_STAGE_BYTES = 2 * A_PLANE_BYTES; // hi + lo
@@ -62,6 +63,21 @@ struct TcArgs {
     int* n_flagged;
 };
 
+// (best, index, second best) of a row, merged across the lanes that hold other columns of it: the smaller value wins,
+// the smaller centre number on equal values (the first minimum in centre order, src/ivfbuild.c:186-190)
+__device__ __forceinline__ void merge_best(float& best, int& best_i, float& second, int lane_mask) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, lane_mask);
+    const int oi = __shfl_xor_sync(0xffffffffu, best_i, lane_mask);
+    const float os = __shfl_xor_sync(0xffffffffu, second, lane_mask);
+    if (ob < best || (ob == best && oi < best_i)) {
+        second = fminf(best, os);
+        best = ob;
+        best_i = oi;
+    } else {
+        second = fminf(second, ob);
+    }
+}
+
 __global__ void __launch_bounds__(TC_THREADS, 1) assign_tc_kernel(TcArgs a) {
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment for the 128B swizzle atoms
@@ -69,37 +85,23 @@ __global__ void __launch_bounds__(TC_THREADS, 1) assign_tc_kernel(TcArgs a) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)TC_STAGES * STAGE_BYTES);
     uint64_t* full_bar = bars;                    // [TC_STAGES]
     uint64_t* empty_bar = bars + TC_STAGES;       // [TC_STAGES]
-    uint64_t* tfull_bar = bars + 2 * TC_STAGES;   // [2]
-    uint64_t* tempty_bar = bars + 2 * TC_STAGES + 2;  // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * TC_STAGES + 4);
 
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
 
-    if (warp == 1 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int s = 0; s < TC_STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&tfull_bar[s], 1);
-            mbar_init(&tempty_bar[s], 4);   // one arrive per epilogue warp
+            mbar_init(&empty_bar[s], TC_CONSUMERS / 32);   // one arrive per consumer warp
         }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const size_t a_tile_bytes = (size_t)a.n_kblocks * A_STAGE_BYTES;   // per m tile
     const size_t b_tile_bytes = (size_t)a.n_kblocks * B_STAGE_BYTES;   // per n tile
 
-    // The producer and the MMA warp run CONVERGED and one lane elected with elect.sync issues the uniform-datapath
-    // instructions: under "lane == 0" the compiler wraps each of them in an ELECT / BRA.U.ANY loop, and the lone
-    // thread's scalar code becomes a bottleneck of its own (measured on list_tc_kernel, profiles/r1_listtc_ncu.md).
-    if (warp == 0) {
-        // ===== producer: two bulk copies per stage =====
+    if (warp == TC_CONSUMERS / 32) {
+        // ===== producer: two bulk copies per stage; the warp runs converged and one elected lane issues =====
         const bool leader = elect_one();
         uint32_t it = 0;
         for (int mt = blockIdx.x; mt < a.n_mtiles; mt += gridDim.x)
@@ -117,92 +119,73 @@ __global__ void __launch_bounds__(TC_THREADS, 1) assign_tc_kernel(TcArgs a) {
                     }
                     __syncwarp();
                 }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        const bool leader = elect_one();
-        constexpr uint32_t idesc = make_idesc_bf16(TC_M, TC_N);
-        uint32_t it = 0, tile = 0;
-        for (int mt = blockIdx.x; mt < a.n_mtiles; mt += gridDim.x)
-            for (int nt = 0; nt < a.n_ntiles; ++nt, ++tile) {
-                const int as = tile & 1;
-                const uint32_t aph = (tile >> 1) & 1;
-                mbar_wait(&tempty_bar[as], aph ^ 1);      // epilogue has drained this accumulator stage
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)as * TC_N;
+    } else {
+        // ===== consumers: warpgroup wg multiplies rows 64 wg .. 64 wg + 63 of the tile by all 256 centres, then keeps
+        // the running best / second best of its two fragment rows over the centres it holds =====
+        const int wg = warp / 4, t = threadIdx.x % 128;
+        const int frag_row = 16 * (t / 32) + (t % 32) / 4;   // and frag_row + 8
+        const int frag_col = 2 * (t % 4);
+        uint32_t it = 0;
+        for (int mt = blockIdx.x; mt < a.n_mtiles; mt += gridDim.x) {
+            float best[2] = {INFINITY, INFINITY}, second[2] = {INFINITY, INFINITY};
+            int best_i[2] = {0x7fffffff, 0x7fffffff};
+            for (int nt = 0; nt < a.n_ntiles; ++nt) {
+                float acc[TC_N / 2];
                 for (int kb = 0; kb < a.n_kblocks; ++kb, ++it) {
                     const int s = it % TC_STAGES;
                     const uint32_t ph = (it / TC_STAGES) & 1;
                     mbar_wait(&full_bar[s], ph);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + (size_t)s * STAGE_BYTES);
-                    const uint32_t sb = sa + A_STAGE_BYTES;
+                    const uint32_t sa = smem_u32(smem + (size_t)s * STAGE_BYTES) + (uint32_t)wg * (64 * 128);
+                    const uint32_t sb = smem_u32(smem + (size_t)s * STAGE_BYTES) + A_STAGE_BYTES;
                     const uint64_t da_hi = make_sw128_desc(sa), da_lo = make_sw128_desc(sa + A_PLANE_BYTES);
                     const uint64_t db_hi = make_sw128_desc(sb), db_lo = make_sw128_desc(sb + B_PLANE_BYTES);
-                    if (leader) {
+                    wgmma_fence();
 #pragma unroll
-                        for (int k = 0; k < TC_K / 16; ++k) {
-                            const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);   // 32 bytes per UMMA_K step inside the atom
-                            umma_bf16(tmem_d, da_hi + adv, db_hi + adv, idesc, (kb | k) != 0);
-                            umma_bf16(tmem_d, da_hi + adv, db_lo + adv, idesc, 1);
-                            umma_bf16(tmem_d, da_lo + adv, db_hi + adv, idesc, 1);
-                        }
-                        umma_commit(&empty_bar[s]);           // smem stage reusable once these MMAs retire
+                    for (int k = 0; k < TC_K / 16; ++k) {
+                        const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);   // 32 bytes per K step inside the atom
+                        wgmma_bf16_n256(acc, da_hi + adv, db_hi + adv, (kb | k) != 0);
+                        wgmma_bf16_n256(acc, da_hi + adv, db_lo + adv, 1);
+                        wgmma_bf16_n256(acc, da_lo + adv, db_hi + adv, 1);
                     }
+                    wgmma_commit();
+                    wgmma_wait<0>();
                     __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[s]);   // smem stage reusable: this warp's MMAs have retired
                 }
-                if (leader) umma_commit(&tfull_bar[as]);  // accumulator complete -> epilogue
-                __syncwarp();
-            }
-    } else if (warp >= 4) {
-        // ===== epilogue: thread = one row; running best / second best over all centres =====
-        const int q = warp - 4;                           // TMEM lane quarter of this warp (warp % 4)
-        uint32_t tile = 0;
-        for (int mt = blockIdx.x; mt < a.n_mtiles; mt += gridDim.x) {
-            const int64_t r_slab = (int64_t)mt * TC_M + q * 32 + lane;
-            float best = INFINITY, second = INFINITY;
-            int best_i = 0x7fffffff;
-            for (int nt = 0; nt < a.n_ntiles; ++nt, ++tile) {
-                const int as = tile & 1;
-                const uint32_t aph = (tile >> 1) & 1;
-                mbar_wait(&tfull_bar[as], aph);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)as * TC_N;
-                for (int c0 = 0; c0 < TC_N; c0 += 32) {
-                    uint32_t acc[32];
-                    tmem_ld32(taddr + c0, acc);
-                    const int cbase = nt * TC_N + c0;
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const float dot = __uint_as_float(acc[j]);
-                        const float v = a.is_l2 ? fmaf(-2.f, dot, __ldg(a.cn + cbase + j)) : (cbase + j < a.k ? -dot : INFINITY);
-                        if (v < best) {            // strict <: first minimum wins (src/ivfbuild.c:186-190)
-                            second = best;
-                            best = v;
-                            best_i = cbase + j;
-                        } else if (v < second) {
-                            second = v;
-                        }
+                for (int i = 0; i < TC_N / 2; ++i) {
+                    const int h = (i / 2) % 2;
+                    const int col = nt * TC_N + 8 * (i / 4) + frag_col + (i % 2);
+                    const float dot = acc[i];
+                    const float v = a.is_l2 ? fmaf(-2.f, dot, __ldg(a.cn + col)) : (col < a.k ? -dot : INFINITY);
+                    if (v < best[h]) {            // strict <: first minimum wins (src/ivfbuild.c:186-190)
+                        second[h] = best[h];
+                        best[h] = v;
+                        best_i[h] = col;
+                    } else if (v < second[h]) {
+                        second[h] = v;
                     }
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty_bar[as]);
             }
-            if (r_slab < a.n_rows) {
-                const int64_t row = a.row0 + r_slab;
-                a.out_idx[row] = best_i == 0x7fffffff ? 0 : best_i;
-                // error bound of the split product: |err(x.c)| <= tol |x| |c|  (both compared values carry it)
-                const float xnorm = sqrtf(a.xn[r_slab]);
-                const float eps = (a.is_l2 ? 4.f : 2.f) * a.tol * xnorm * a.cmax + (a.is_l2 ? a.sum_tol * (a.cmax * a.cmax + xnorm * xnorm) : 0.f);
-                if (!(second - best > eps)) {      // also catches NaN / Inf rows
-                    int p = atomicAdd(a.n_flagged, 1);
-                    a.flagged[p] = (int32_t)row;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                merge_best(best[h], best_i[h], second[h], 1);
+                merge_best(best[h], best_i[h], second[h], 2);
+                const int64_t r_slab = (int64_t)mt * TC_M + wg * 64 + frag_row + 8 * h;
+                if (t % 4 == 0 && r_slab < a.n_rows) {
+                    const int64_t row = a.row0 + r_slab;
+                    a.out_idx[row] = best_i[h] == 0x7fffffff ? 0 : best_i[h];
+                    // error bound of the split product: |err(x.c)| <= tol |x| |c|  (both compared values carry it)
+                    const float xnorm = sqrtf(a.xn[r_slab]);
+                    const float eps = (a.is_l2 ? 4.f : 2.f) * a.tol * xnorm * a.cmax + (a.is_l2 ? a.sum_tol * (a.cmax * a.cmax + xnorm * xnorm) : 0.f);
+                    if (!(second[h] - best[h] > eps)) {      // also catches NaN / Inf rows
+                        int p = atomicAdd(a.n_flagged, 1);
+                        a.flagged[p] = (int32_t)row;
+                    }
                 }
             }
         }
     }
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 512);
 }
 
 // ----------------------------------------------------------------------------- host side
@@ -293,8 +276,8 @@ int launch_assign_tc(const Table& X, int metric, const Table& Cn, int k, int32_t
         a.cmax = std::sqrt(cmax2);
         // |err(x.c)| <= tol |x||c| for the split product (same derivation as launch_list_tc_refine, vb_list_tc.cu):
         //   representation: hi.hi + hi.lo + lo.hi drops lo.lo and the two bf16 residuals: 3 * 2^-16;
-        //   accumulation: one fp32 rounding of the TMEM accumulator per UMMA, 3 UMMAs per 16-element K step, 2^-23 each
-        //     (truncation), doubled for the alignment of the 16 products inside an UMMA -> 6 * (dim / 16) * 2^-23.
+        //   accumulation: one fp32 rounding of the accumulator per MMA, 3 MMAs per 16-element K step, 2^-23 each
+        //     (truncation), doubled for the alignment of the 16 products inside an MMA -> 6 * (dim / 16) * 2^-23.
         // 2^-13 covers both up to ~1650 dimensions (the shapes validated in round 1); longer rows (ivfflat allows 2000
         // for vector, 4000 for halfvec) take the formula.  The fp32 norms |x|^2, |c|^2 are sums of dim / 32 terms per
         // lane plus a 5-step shuffle tree: (dim / 32 + 8) * 2^-23 relative, at least 1e-6.

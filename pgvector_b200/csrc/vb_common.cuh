@@ -1,4 +1,4 @@
-// vb_common.cuh -- shared declarations for libvecb200 (sm_100a only).
+// vb_common.cuh -- shared declarations for libvecb200 (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -42,7 +42,7 @@ extern thread_local int g_last_status;
 struct Context {
     bool inited = false;
     int device = -1;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;
     cudaStream_t copy_stream = nullptr;
     int64_t launches = 0;

@@ -32,20 +32,12 @@ __device__ __forceinline__ float key_to_float(uint32_t k) {
     return __uint_as_float(u);
 }
 
-// sm_100 mixed-precision scalar arithmetic (PTX ISA 8.6, FHFMA / FHADD in SASS): an fp16 operand is widened inside the
-// instruction, either half of a 32-bit register is addressable (.H1), so a halfvec element costs no conversion.
-// float(a) * float(b) is exact in fp32 (22-bit product) and the addition rounds once: bit-identical to
-// fmaf(__half2float(a), __half2float(b), c); likewise float(a) - c.
+// halfvec element arithmetic: float(a) * float(b) is exact in fp32 (22-bit product) and the addition rounds once, as in
+// the reference's widen-then-accumulate loop (src/halfutils.c)
 __device__ __forceinline__ float fh_fma(uint16_t a, uint16_t b, float c) {
-    float d;
-    asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(d) : "h"(a), "h"(b), "f"(c));
-    return d;
+    return __fmaf_rn(__half2float(__ushort_as_half(a)), __half2float(__ushort_as_half(b)), c);
 }
-__device__ __forceinline__ float fh_sub(uint16_t a, float c) {
-    float d;
-    asm("sub.rn.f32.f16 %0, %1, %2;" : "=f"(d) : "h"(a), "f"(c));
-    return d;
-}
+__device__ __forceinline__ float fh_sub(uint16_t a, float c) { return __fsub_rn(__half2float(__ushort_as_half(a)), c); }
 
 // the same read marked evict-first in L2 (random row gathers of a graph walk: each row is used once, and the lines it would
 // displace -- the per-query visited tables, the neighbour lists -- are re-used)

@@ -184,7 +184,7 @@ enum { WSH_QIMG = 0, WSH_OUT = 7, WSH_FLAG = 12 };
 
 // The visited tables are the only data of a graph walk that is re-used (32 probes per expansion, every one a random
 // 32-byte sector); rows and neighbour lists stream past once.  Marking the tables' range persisting in L2 keeps the
-// probes out of DRAM (ncu r2_hnsw_E2: L2 hit rate 23 %, 3.4 GB of DRAM write-backs per launch without it).
+// probes out of DRAM.
 static void hnsw_l2_window(cudaStream_t s, void* base, size_t bytes, bool on) {
     static int max_window = -1, max_persist = -1;
     if (max_window < 0) {
@@ -269,8 +269,8 @@ static int hnsw_search_impl(Hnsw& h, const void* queries, int64_t nq, int ef, in
     VB_TRY(hnsw_launch(h, g, qimg, qstride, nq, ef, k, nullptr, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, &resident));
     const int grid = (int)std::min<int64_t>(want_ctas, (int64_t)c.sm_count * std::max(1, resident));
     // layer-0 table: a search visits a few multiples of ef elements (about 20 ef at m = 16), and the table may fill to
-    // three quarters.  It is sized tightly: the tables of all resident warps together should stay in L2 (3552 warps x
-    // 64 KB did not: every visited probe of the 10 M-row bit graph went to DRAM, ncu r2_hnsw_E), and the per-query clear
+    // three quarters.  It is sized tightly: the tables of all resident warps together should stay in L2 (64 KB per
+    // warp did not: every visited probe of a 10 M-row bit graph went to DRAM), and the per-query clear
     // is proportional to it.  It grows on overflow -- the grown size is remembered per ef_search.
     uint32_t cap = 1u << 12;
     while (cap < (uint32_t)(ef * h.m * (VB_AB_VIS ? 2 : 4)) && cap < (1u << 22)) cap <<= 1;

@@ -58,7 +58,7 @@ constexpr int HN_WARPS = 4;             // queries (or inserted elements) per CT
 
 // Resident CTAs per SM the register allocation aims for.  Without the second __launch_bounds__ argument ptxas picks a
 // target of its own per instantiation (56 .. 128 registers, the narrow-row ones with spills); the kernel waits on
-// dependent gathers, so resident warps matter more than a spill-free loop -- measured, see profiles/r2_hnsw_minb.md.
+// dependent gathers, so resident warps matter more than a spill-free loop.
 #ifndef VB_HNSW_MINB
 #define VB_HNSW_MINB 6
 #endif
@@ -205,7 +205,7 @@ __device__ __forceinline__ void load_query_image(const uint4* gq, int qvec, int 
 #ifndef VB_HNSW_EVICT_FIRST
 #define VB_HNSW_EVICT_FIRST 1
 #endif
-// A/B switches of the round-2 changes (tools/gpu_session7.sh measures each against the others; see profiles/r2_hnsw_ab.md)
+// A/B switches of alternative search strategies (compile-time, off by default)
 #ifndef VB_AB_PINGPONG
 #define VB_AB_PINGPONG 1
 #endif
@@ -238,8 +238,8 @@ __device__ __forceinline__ void load_query_image(const uint4* gq, int qvec, int 
 #define VB_AB_RPI_WIDE 4
 #endif
 // narrow rows: score all listed neighbours while their visited probes are in flight (see hnsw_search_layer).  Measured on
-// config E (10M x bit(1024), ef_search 200): 724 k queries/s with it, 758 k without -- the 60 % of wasted scorings cost more
-// than the overlapped round trip saves; kept as a switch (profiles/r2_ab_hnsw_spec.md)
+// config E (10M x bit(1024), ef_search 200) it ran slower with it than without -- the wasted scorings cost more than the
+// overlapped round trip saves; kept as a switch
 #ifndef VB_AB_SPEC
 #define VB_AB_SPEC 0
 #endif

@@ -268,8 +268,8 @@ static int ivf_select_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t 
     }
     prof_begin(VB_PROF_SCAN_LISTS);
     // many queries at once: the query image is itself a row table with the centres' stride (vector, bit), so the
-    // centre scan is computed tile-wise (both operands staged once per 128 x 128 tile).  Measured on B200 for 2048
-    // queries x 1000 centres x 1536-d: 1.31 ms as one-query-at-a-time scans (L2-resident, 12.6 GB of L2 reads).
+    // centre scan is computed tile-wise (both operands staged once per 128 x 128 tile) instead of one-query-at-a-time
+    // scans that re-read the L2-resident centre table per query.
     const bool tiled = nq >= 64 && ix.elem != VB_HALFVEC && qstride == ix.centers.stride && ctx().scan_impl != 0 &&
                        (key_metric(ix.metric) == VB_L2_SQUARED || key_metric(ix.metric) == VB_NEG_IP || key_metric(ix.metric) == VB_HAMMING);
     if (tiled) {
@@ -642,9 +642,19 @@ extern "C" {
 
 int vb_distance_batch(int elem, int metric, int dim, const void* q, const void* rows, int64_t n, double* out) {
     VB_TRY(require_init());
-    VB_REQUIRE(elem >= 0 && elem <= 2 && dim > 0 && metric_valid_for(elem, metric), "bad element type/metric/dim (%d, %d, %d)", elem,
-               metric, dim);
+    VB_REQUIRE(elem >= 0 && elem <= 2 && (dim > 0 || (elem == VB_BIT && dim == 0)) && metric_valid_for(elem, metric),
+               "bad element type/metric/dim (%d, %d, %d)", elem, metric, dim);
     if (n <= 0) return VB_OK;
+    // a zero-length bit string ('' :: bit) has no set bits: Hamming 0 and Jaccard 1 (ab == 0, src/bitvec.c:60-70), the
+    // counts of eight zero bits -- scored as such by the same kernel
+    std::vector<uint8_t> zero_rows, zero_q;
+    if (dim == 0 && q != nullptr) {
+        zero_rows.assign((size_t)n, 0);
+        zero_q.assign(1, 0);
+        rows = zero_rows.data();
+        q = zero_q.data();
+        dim = 8;
+    }
     if (q == nullptr) {  // ZeroDistance (src/ivfscan.c:192-196)
         for (int64_t i = 0; i < n; ++i) out[i] = 0.0;
         return VB_OK;

@@ -1,7 +1,7 @@
 // vb_ivf_one.cu -- the IVFFlat scan of ONE query (or a handful): what a backend issues.  ivfflatgettuple's first call
 // runs GetScanLists and GetScanItems for a single ORDER BY value (src/ivfscan.c:47-118, 123-187, 360-414;
 // amcanparallel = false, src/ivfflat.c:266), so the latency of a scan is launches and round trips, not bandwidth: 60 MB of
-// rows are 10 us of HBM time, the nine launches, three memsets and four copies of the general path were 160 us.
+// rows are ~20 us of HBM time, far less than the nine launches, three memsets and four copies of the general path.
 //
 // Here a scan is TWO kernels, each a fused distance + select (north_star's "one-query-vs-many-candidates distance +
 // top-k select as a fused kernel"):

@@ -6,7 +6,7 @@
 // sum((x - c)^2) / sum(x * c) / popcount(x ^ c) in fp32 / integer, the same arithmetic
 // as the reference's proc-1 functions, so argmin decisions match the CPU path up to
 // fp32 reassociation.  It is compute bound on the CUDA cores (2 ops per element for L2);
-// the tensor-core (tcgen05) assign in vb_assign_tc.cu uses it to re-check near ties.
+// the tensor-core (wgmma) assign in vb_assign_tc.cu uses it to re-check near ties.
 #include "vb_common.cuh"
 #include "vb_distance.cuh"
 #include <cuda_bf16.h>
@@ -589,7 +589,7 @@ static int kmeans_run(const Table& X, int kmeans_metric, void* centers_host, int
     const int64_t n = X.n;
     // The state of a run lives in ONE grow-only arena (slot WSK_STATE; the sharded-scan / sparsevec slots it shares
     // never run beside a k-means): nine cudaMalloc + cudaFree pairs per call cost more than the five Lloyd iterations of
-    // config D on a context that holds a 58 GB table (0.2 s of 0.25 s measured), and cudaFree synchronises the device.
+    // config D on a context that holds a large table, and cudaFree synchronises the device.
     size_t scan_tmp_bytes = 0;
     VB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp_bytes, (int32_t*)nullptr, (int32_t*)nullptr, k, s));
     st.scan_tmp_bytes = scan_tmp_bytes;

@@ -3,10 +3,10 @@
 //
 // GetScanItems (src/ivfscan.c:124-180) needs, per query, the k nearest of ~probes * rows/lists candidates.
 // The list-major formulation (vb_list_tile.cu) already reads every probed list once per batch; what is left
-// is 2 fp32 instructions per (row, query, dimension).  Here that arithmetic moves to tcgen05:
+// is 2 fp32 instructions per (row, query, dimension).  Here that arithmetic moves to the tensor cores (wgmma):
 //
 //   1. approximate pass:  d~ = |x|^2 + |q|^2 - 2 x.q   (or -x.q), x.q from three bf16 MMAs on the hi/lo split of
-//      both operands (hi.hi + hi.lo + lo.hi, fp32 accumulation in TMEM) -- |d~ - d| <= eps(q), a rigorous bound;
+//      both operands (hi.hi + hi.lo + lo.hi, fp32 accumulation in registers) -- |d~ - d| <= eps(q), a rigorous bound;
 //   2. the k' = k + slack smallest d~ of every query are selected (segment_topk_kernel);
 //   3. of those, the candidates with d~ <= (k-th d~) + 2 eps are re-scored with the exact scan arithmetic (Acc<>,
 //      same as scan_kernel) -- nothing above that threshold can be among the k nearest;
@@ -18,11 +18,10 @@
 // image, one 32 KB block per (128-row table tile, 64-dimension block); a unit of work is a (list, table tile)
 // pair (tiles straddling a list boundary are visited by both lists, rows outside the list masked).  The queries
 // of each list's group are gathered and packed per batch into 64-query B tiles (16 KB per dimension block).
-// CTA = persistent, one per SM: warp 0 = bulk-copy producer, warp 1 = MMA issuer, warp 2 = TMEM allocator,
-// warps 4-7 = epilogue (thread = row; two 128-column accumulator stages so the epilogue of one tile overlaps the
-// MMAs of the next).  The query operand of a tile is ONE shared-memory tile [q_hi ; q_lo] of 2n rows (n = 32 or 64):
-// x_hi . [q_hi ; q_lo] is a single UMMA 128 x 2n x 16 per K step whose two column groups the epilogue adds;
-// level 2 adds x_lo . q_hi (128 x n x 16).
+// CTA = persistent, one per SM: warps 0-7 = two consumer warpgroups (64 table rows each: MMAs, then the epilogue
+// on the register accumulators), warp 8 = bulk-copy producer.  The query operand of a tile is ONE shared-memory tile
+// [q_hi ; q_lo] of 2n rows (n = 32 or 64): x_hi . [q_hi ; q_lo] is a single wgmma 64 x 2n x 16 per K step whose two
+// column groups the epilogue adds; level 2 adds x_lo . q_hi (64 x n x 16).
 //
 // Two filter levels.  Level 1 streams only the hi plane of the rows (16 KB + B per stage, 7 stages in flight): half
 // the HBM traffic, error bound 2^-7 |x||q|.  A batch with an uncertified query is repeated at level 2 (both planes,
@@ -46,15 +45,16 @@ constexpr int LC_N = 64;
 constexpr int LC_STAGES = 4;                             // level 2: 4 x 48 KB in flight per SM
 constexpr int LC_STAGES_L1 = 7;                          // level 1: 7 x 32 KB (A hi plane + B)
 constexpr int LC_MAX_STAGES = 8;
-constexpr int LC_THREADS = 256;
+constexpr int LC_CONSUMERS = 256;                       // two warpgroups: rows 0-63 and 64-127 of the table tile
+constexpr int LC_THREADS = LC_CONSUMERS + 32;            // + the producer warp
 constexpr uint32_t LC_A_PLANE = LC_M * TC_K * 2;        // 16 KB
 constexpr uint32_t LC_B_PLANE = LC_N * TC_K * 2;        // 8 KB
 constexpr uint32_t LC_A_STAGE = 2 * LC_A_PLANE;
 constexpr uint32_t LC_B_STAGE = 2 * LC_B_PLANE;
 constexpr uint32_t LC_STAGE = LC_A_STAGE + LC_B_STAGE;  // 48 KB
 constexpr uint32_t LC_STAGE_L1 = LC_A_PLANE + LC_B_STAGE;  // 32 KB
-constexpr size_t LC_SMEM = std::max((size_t)LC_STAGES * LC_STAGE, (size_t)LC_STAGES_L1 * LC_STAGE_L1) + 1024 /*align*/ + 256 /*barriers*/;
-constexpr int LC_ACC = 2 * LC_N;                         // TMEM columns of one accumulator stage: [x.q_hi | x.q_lo]
+constexpr size_t LC_SMEM = std::max((size_t)LC_STAGES * LC_STAGE, (size_t)LC_STAGES_L1 * LC_STAGE_L1) + 1024 /*align*/ + 256 /*barriers*/ +
+                           4 * LC_N * sizeof(float) /*slab minima*/;
 constexpr int LC_MAX_KP = 128;                           // candidates selected per query, at most
 
 struct LcArgs {
@@ -96,6 +96,121 @@ __device__ __forceinline__ bool lc_job(const LcArgs& a, int j, LcJob& jb) {
     return jb.q_lo < jb.q_hi;
 }
 
+// One (unit, query tile) for one consumer warpgroup: the MMAs of all K blocks, then the epilogue.  NQ = queries per
+// column group; the accumulator holds the 64 x 2 NQ product x . [q_hi ; q_lo] (NQ registers), whose column groups
+// [0, NQ) and [NQ, 2 NQ) are added -- register i + NQ / 2 holds column c + NQ of register i's column c.
+template <int NQ>
+__device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_stages, uint32_t stage_bytes, uint32_t a_bytes,
+                                        uint64_t* full_bar, uint64_t* empty_bar, float* slab_buf, uint32_t& it, const LcJob& jb,
+                                        int qt) {
+    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+    const int wg = warp / 4, t = threadIdx.x % 128;
+    float acc[NQ];
+    for (int kb = 0; kb < a.n_kblocks; ++kb, ++it) {
+        const int s = it % n_stages;
+        const uint32_t ph = (it / n_stages) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes) + (uint32_t)wg * (64 * 128);
+        const uint32_t sb = smem_u32(smem + (size_t)s * stage_bytes) + a_bytes;
+        const uint64_t da_hi = make_sw128_desc(sa), da_lo = make_sw128_desc(sa + LC_A_PLANE);
+        const uint64_t db = make_sw128_desc(sb);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TC_K / 16; ++k) {
+            const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);
+            // wgmma of different shapes accumulating into the same registers are ordered by a fence between them
+            if constexpr (NQ == 64) {
+                wgmma_bf16_n128(acc, da_hi + adv, db + adv, (kb | k) != 0);
+                if (!a.hi_only) {
+                    wgmma_fence();
+                    wgmma_bf16_n64(acc, da_lo + adv, db + adv, 1);
+                }
+            } else {
+                wgmma_bf16_n64(acc, da_hi + adv, db + adv, (kb | k) != 0);
+                if (!a.hi_only) {
+                    wgmma_fence();
+                    wgmma_bf16_n32(acc, da_lo + adv, db + adv, 1);
+                }
+            }
+            if (!a.hi_only && k + 1 < TC_K / 16) wgmma_fence();   // the next K step returns to the wider shape
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[s]);
+    }
+
+    // ===== epilogue: rows of the table tile x queries of the group =====
+    const ListUnit un = jb.un;
+    const int cnt = jb.cnt;
+    const int64_t lo = a.list_off[un.list], hi = a.list_off[un.list + 1];
+    const int frag_row = wg * 64 + 16 * (t / 32) + (t % 32) / 4;   // and frag_row + 8
+    const int frag_col = 2 * (t % 4);
+    int64_t r_table[2];
+    bool valid_row[2];
+    float xnr[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        r_table[h] = (int64_t)un.tile * LC_M + frag_row + 8 * h;
+        valid_row[h] = r_table[h] >= lo && r_table[h] < hi;
+        xnr[h] = valid_row[h] && a.is_l2 ? a.xn[r_table[h]] : 0.f;
+    }
+    const int gb = a.grp_begin[un.list];
+    // warps 2p and 2p + 1 hold the 32 rows of table-aligned slab p of the tile (if any of them belongs to the list)
+    const int pair = warp / 2;
+    const int64_t slab_row0 = (int64_t)un.tile * LC_M + pair * 32;
+    const bool slabs = a.smin != nullptr && slab_row0 < hi && slab_row0 + 32 > lo;
+    const int slab_local = (int)((slab_row0 >> 5) - (lo >> 5));
+    float col_min[NQ / 4];
+#pragma unroll
+    for (int cb = 0; cb < NQ / 8; ++cb)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int col = qt * LC_N + 8 * cb + frag_col + e;
+            int64_t po = 0;
+            float qn = 0.f;
+            if (col < cnt) {
+                po = a.pair_out[gb + col];
+                if (a.is_l2) qn = a.qn[a.pair_q[gb + col]];
+            }
+            float m = __int_as_float(0x7F800000);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int i = 4 * cb + 2 * h + e;
+                if (col < cnt && valid_row[h]) {
+                    const float dot = acc[i] + acc[i + NQ / 2];
+                    const float val = a.is_l2 ? fmaf(-2.f, dot, xnr[h] + qn) : -dot;
+                    a.out[po + (r_table[h] - lo)] = val;
+                    m = fminf(m, val);
+                }
+            }
+            col_min[2 * cb + e] = m;
+        }
+    if (slabs) {
+        // minimum of each column over the slab's 32 rows: over the 16 rows of this warp (lanes of equal t % 4), then
+        // the odd warp of the pair hands its minima to the even one
+#pragma unroll
+        for (int j = 0; j < NQ / 4; ++j)
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) col_min[j] = fminf(col_min[j], __shfl_xor_sync(0xffffffffu, col_min[j], o));
+        float* buf = slab_buf + pair * LC_N;
+        if ((warp & 1) && lane < 4) {
+#pragma unroll
+            for (int j = 0; j < NQ / 4; ++j) buf[8 * (j / 2) + frag_col + (j % 2)] = col_min[j];
+        }
+        named_bar_sync(1 + pair, 64);
+        if (!(warp & 1) && lane < 4) {
+#pragma unroll
+            for (int j = 0; j < NQ / 4; ++j) {
+                const int c = 8 * (j / 2) + frag_col + (j % 2);
+                const int col = qt * LC_N + c;
+                if (col < cnt) a.smin[a.pair_sbase[gb + col] + slab_local] = fminf(col_min[j], buf[c]);
+            }
+        }
+        named_bar_sync(1 + pair, 64);   // buf is rewritten by the next tile
+    }
+}
+
 __global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) {
     extern __shared__ uint8_t lc_smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(lc_smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -107,29 +222,19 @@ __global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)n_stages * stage_bytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + LC_MAX_STAGES;
-    uint64_t* tfull_bar = bars + 2 * LC_MAX_STAGES;
-    uint64_t* tempty_bar = bars + 2 * LC_MAX_STAGES + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * LC_MAX_STAGES + 4);
+    float* slab_buf = reinterpret_cast<float*>(bars + 32);   // [4 warp pairs][LC_N]
 
-    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-    if (warp == 1 && lane == 0) {
+    const int warp = threadIdx.x / 32;
+    if (threadIdx.x == 0) {
         for (int s = 0; s < n_stages; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&tfull_bar[s], 1);
-            mbar_init(&tempty_bar[s], 4);
+            mbar_init(&empty_bar[s], LC_CONSUMERS / 32);
         }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, 2 * LC_ACC);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == LC_CONSUMERS / 32) {
         // ===== producer (whole warp converged, one elected lane issues the copies) =====
         const bool leader = elect_one();
         uint32_t it = 0;
@@ -140,7 +245,7 @@ __global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) {
             const int gt0 = a.gt_begin[un.list];
             for (int qt = jb.q_lo; qt < jb.q_hi; ++qt)
             {
-                // a query tile with at most 32 queries is multiplied as N = 32: only the first half of each B plane moves
+                // a query tile with at most 32 queries is multiplied as N = 64: only the first half of each B plane moves
                 const bool n32 = jb.cnt - qt * LC_N <= 32;
                 for (int kb = 0; kb < a.n_kblocks; ++kb, ++it) {
                     const int s = it % n_stages;
@@ -163,124 +268,21 @@ __global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) {
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: the whole warp walks the loop (warp-uniform control flow and operands), one elected lane
-        // issues.  Under "lane == 0" the compiler wraps every tcgen05 instruction in an ELECT / BRA.U.ANY loop and the
-        // lone thread's scalar code (~160 instructions per K block) becomes the bottleneck of the kernel. =====
-        const bool leader = elect_one();
-        // One UMMA costs ~130 cycles here whatever its N (it re-reads the 128 x 16 A tile from shared memory), so the
-        // products are merged along N: B = [q_hi ; q_lo] is ONE operand of 2n rows, and x_hi . [q_hi ; q_lo] lands in the
-        // column groups [0, n) and [n, 2n) of the accumulator with a single instruction per K step; level 2 adds
-        // x_lo . q_hi into [0, n).  The epilogue sums the two groups.
-        constexpr uint32_t idesc128 = make_idesc_bf16(LC_M, 128);
-        constexpr uint32_t idesc64 = make_idesc_bf16(LC_M, 64);
-        constexpr uint32_t idesc32 = make_idesc_bf16(LC_M, 32);
-        uint32_t it = 0, tile = 0;
+    } else {
+        // ===== consumers: warpgroup wg multiplies rows 64 wg .. 64 wg + 63 of the table tile.  The query operand of a
+        // tile is ONE shared-memory tile [q_hi ; q_lo] of 2n rows (n = 32 or 64): x_hi . [q_hi ; q_lo] is a single
+        // wgmma 64 x 2n x 16 per K step whose two column groups the epilogue adds; level 2 adds x_lo . q_hi (64 x n x 16)
+        // into the first group. =====
+        uint32_t it = 0;
         for (int j = blockIdx.x; j < a.n_jobs; j += gridDim.x) {
             LcJob jb;
             if (!lc_job(a, j, jb)) continue;
-            for (int qt = jb.q_lo; qt < jb.q_hi; ++qt, ++tile) {
-                const int as = tile & 1;
-                const uint32_t aph = (tile >> 1) & 1;
-                mbar_wait(&tempty_bar[as], aph ^ 1);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)as * LC_ACC;
-                const bool n32 = jb.cnt - qt * LC_N <= 32;
-                const uint32_t idesc_both = n32 ? idesc64 : idesc128;   // N = 2n
-                const uint32_t idesc_one = n32 ? idesc32 : idesc64;     // N = n
-                for (int kb = 0; kb < a.n_kblocks; ++kb, ++it) {
-                    const int s = it % n_stages;
-                    const uint32_t ph = (it / n_stages) & 1;
-                    mbar_wait(&full_bar[s], ph);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
-                    const uint32_t sb = sa + a_bytes;
-                    const uint64_t da_hi = make_sw128_desc(sa), da_lo = make_sw128_desc(sa + LC_A_PLANE);
-                    const uint64_t db = make_sw128_desc(sb);
-                    if (leader) {
-#pragma unroll
-                        for (int k = 0; k < TC_K / 16; ++k) {
-                            const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);
-                            umma_bf16(tmem_d, da_hi + adv, db + adv, idesc_both, (kb | k) != 0);
-                            if (!a.hi_only) umma_bf16(tmem_d, da_lo + adv, db + adv, idesc_one, 1);
-                        }
-                        umma_commit(&empty_bar[s]);
-                    }
-                    __syncwarp();
-                }
-                if (leader) umma_commit(&tfull_bar[as]);
-                __syncwarp();
-            }
-        }
-    } else if (warp >= 4) {
-        // ===== epilogue: thread = one table row of the tile; columns = queries of the group =====
-        const int qr = warp - 4;
-        uint32_t tile = 0;
-        for (int j = blockIdx.x; j < a.n_jobs; j += gridDim.x) {
-            LcJob jb;
-            if (!lc_job(a, j, jb)) continue;
-            const ListUnit un = jb.un;
-            const int cnt = jb.cnt;
-            const int64_t lo = a.list_off[un.list], hi = a.list_off[un.list + 1];
-            const int64_t r_table = (int64_t)un.tile * LC_M + qr * 32 + lane;
-            const bool valid_row = r_table >= lo && r_table < hi;
-            const float xnr = valid_row && a.is_l2 ? a.xn[r_table] : 0.f;
-            const int gb = a.grp_begin[un.list];
-            // this warp's 32 rows are one table-aligned slab of the list (if any of them belongs to it)
-            const bool slabs = a.smin != nullptr && __ballot_sync(0xffffffffu, valid_row) != 0;
-            const int slab_local = (int)((((int64_t)un.tile * LC_M + qr * 32) >> 5) - (lo >> 5));
-            for (int qt = jb.q_lo; qt < jb.q_hi; ++qt, ++tile) {
-                const int as = tile & 1;
-                const uint32_t aph = (tile >> 1) & 1;
-                mbar_wait(&tfull_bar[as], aph);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(qr * 32) << 16) + (uint32_t)as * LC_ACC;
-                const int n = cnt - qt * LC_N <= 32 ? 32 : LC_N;   // queries per column group of this tile
-#pragma unroll
-                for (int c0 = 0; c0 < LC_N; c0 += 32) {
-                    const int col0 = qt * LC_N + c0;
-                    if (col0 >= cnt) break;   // warp-uniform
-                    uint32_t acc[32], part[32];
-                    tmem_ld32(taddr + c0, acc);          // x_hi . q_hi (+ x_lo . q_hi)
-                    tmem_ld32(taddr + n + c0, part);     // x_hi . q_lo
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) acc[j] = __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(part[j]));
-                    // lane j fetches the bookkeeping of column j once; broadcast in the loop
-                    const int myc = col0 + lane;
-                    int64_t my_out = 0;
-                    float my_qn = 0.f;
-                    if (myc < cnt) {
-                        my_out = a.pair_out[gb + myc];
-                        if (a.is_l2) my_qn = a.qn[a.pair_q[gb + myc]];
-                    }
-                    float my_min = __int_as_float(0x7F800000);
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const int64_t po = __shfl_sync(0xffffffffu, my_out, j);
-                        const float qn = __shfl_sync(0xffffffffu, my_qn, j);
-                        float val = __int_as_float(0x7F800000);
-                        if (col0 + j < cnt && valid_row) {
-                            const float dot = __uint_as_float(acc[j]);
-                            val = a.is_l2 ? fmaf(-2.f, dot, xnr + qn) : -dot;
-                            a.out[po + (r_table - lo)] = val;
-                        }
-                        if (slabs) {
-                            // minimum of column j over the warp's 32 rows (one CREDUX), kept by lane j
-                            float m;
-                            asm volatile("redux.sync.min.f32 %0, %1, 0xffffffff;" : "=f"(m) : "f"(val));
-                            if (lane == j) my_min = m;
-                        }
-                    }
-                    if (slabs && myc < cnt) a.smin[a.pair_sbase[gb + myc] + slab_local] = my_min;
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty_bar[as]);
+            for (int qt = jb.q_lo; qt < jb.q_hi; ++qt) {
+                if (jb.cnt - qt * LC_N <= 32) lc_tile<32>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt);
+                else lc_tile<64>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt);
             }
         }
     }
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 2 * LC_ACC);
 }
 
 // gather + split the queries of every (query, list) pair into the B tiles of its list's group:
@@ -959,8 +961,8 @@ int list_tc_traffic(int on, int64_t* out8) {
 //   representation: bf16 keeps 8 significant bits (unit roundoff 2^-8), so |x - x_hi| <= 2^-8 |x| and
 //     |x - x_hi - x_lo| <= 2^-16 |x|.  Level 2 drops x_lo.q_lo and the two residuals: 3 * 2^-16.  Level 1 also
 //     drops x_lo.q: 2^-8 + 2^-16.
-//   accumulation: one fp32 rounding of the TMEM accumulator per UMMA, (products per K step) * dim / 16 of them,
-//     <= 2^-23 each if the unit truncates; doubled to cover the alignment of the 16 products inside an UMMA.
+//   accumulation: one fp32 rounding of the accumulator per MMA, (products per K step) * dim / 16 of them,
+//     <= 2^-23 each if the unit truncates; doubled to cover the alignment of the 16 products inside an MMA.
 // The constants below are the values the GPU tests and benches of round 1 ran with (dim <= 1536); the formula takes
 // over for longer rows, where the accumulation term grows past them.
 // The fp32 norms, the final sum and the rounding of the exact fp32 distance it is compared with: 2^-16 (|x|^2 +

@@ -15,11 +15,10 @@
 // all queries of the sub-tile; the query loop is compiled for every count of query quads 1..8, so a group
 // of 20 queries costs 20/32 of a full tile and every warp with rows stays busy.  Operands are staged
 // through shared memory in steps of 16 dimensions, k-major, double buffered with register prefetch; the
-// inner loop is packed fp32x2 over two queries: (x, x) + (-q0, -q1) with one FADD2, squared and accumulated
-// with one FFMA2.  fp32x2 results are IEEE-identical to the scalar instructions, and each (row, query)
-// distance is the plain sequential fmaf chain over the dimensions.
+// inner loop works on pairs of queries: (x, x) + (-q0, -q1), squared and accumulated, each lane rounded as
+// the scalar instruction, so each (row, query) distance is the plain sequential fmaf chain over the dimensions.
 //
-// Bound: fp32 issue (2 packed instructions per 2 pairs for L2, 1 for inner product); HBM traffic is
+// Bound: fp32 issue (2 instructions per pair for L2, 1 for inner product); HBM traffic is
 // one pass over the probed lists per batch.
 #include "vb_common.cuh"
 
@@ -56,15 +55,20 @@ __device__ __forceinline__ unsigned long long lt_pack(float lo, float hi) {
 __device__ __forceinline__ void lt_unpack(unsigned long long v, float& lo, float& hi) {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
+// two fp32 lanes of a packed pair, each rounded as the scalar instruction (never contracted: the distance of every
+// (row, query) pair is the plain sequential fmaf chain)
 __device__ __forceinline__ unsigned long long lt_add2(unsigned long long a, unsigned long long b) {
-    unsigned long long r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    lt_unpack(a, a0, a1);
+    lt_unpack(b, b0, b1);
+    return lt_pack(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ unsigned long long lt_fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-    unsigned long long r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    float a0, a1, b0, b1, c0, c1;
+    lt_unpack(a, a0, a1);
+    lt_unpack(b, b0, b1);
+    lt_unpack(c, c0, c1);
+    return lt_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
 // 4 consecutive elements of a row starting at element e (zero past the padded dimension count)

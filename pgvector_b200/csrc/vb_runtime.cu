@@ -319,8 +319,8 @@ int vb_init(int device) {
         return VB_ENODEVICE;
     }
     cudaDeviceProp p;
-    if (cudaGetDeviceProperties(&p, device) != cudaSuccess || p.major != 10) {
-        vb::set_error("device %d is sm_%d%d; libvecb200 is built for sm_100a only", device, p.major, p.minor);
+    if (cudaGetDeviceProperties(&p, device) != cudaSuccess || p.major != 9 || p.minor != 0) {
+        vb::set_error("device %d is sm_%d%d; libvecb200 is built for sm_90a only", device, p.major, p.minor);
         return VB_ENODEVICE;
     }
     if (cudaSetDevice(device) != cudaSuccess) {

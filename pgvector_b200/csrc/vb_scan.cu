@@ -1,5 +1,5 @@
 // vb_scan.cu -- the fused one-query-vs-many-rows distance kernels and the per-query
-// top-k select.  sm_100a only.
+// top-k select.  sm_90a only.
 //
 // Replaces the inner loops of GetScanLists / GetScanItems (src/ivfscan.c:68-107,
 // 150-174), the sequential-scan operator evaluation (src/vector.c:576-750,
@@ -173,15 +173,15 @@ static int scan_rows_per_chunk(size_t stride) {
 
 int scan_chunk_rows(const Table& t) { return scan_rows_per_chunk(t.stride); }
 
-// Which scan kernel?  Measured on B200 (profiles/r1_listscan_*.md): the bulk-copy (TMA) kernel streams HBM at
-// ~6.7 TB/s (82 % DRAM utilisation at 14 % warp occupancy) but, with one CTA per SM, is slower than the
-// LDG kernel when the rows are L2-resident (centre table: 0.76 ms vs 1.39 ms for 2048 queries x 1000 centres).
-// scan_impl: 0 = always LDG, 1 = bulk whenever the shape allows, 2 (default) = bulk for tables larger than L2.
+// Which scan kernel?  The bulk-copy (TMA) kernel streams HBM at low warp occupancy but, with one CTA per SM, is
+// slower than the LDG kernel when the rows are L2-resident (a centre table read by many queries).
+// scan_impl: 0 = always LDG, 1 = bulk whenever the shape allows, 2 (default) = bulk for tables larger than the
+// H100's 50 MB L2.
 static bool use_bulk_scan(const Table& t, int64_t n_rows, size_t qstride) {
     const int impl = ctx().scan_impl;
     if (impl == 0 || !scan_bulk_supported(t.elem, t.stride, qstride)) return false;
     if (impl == 1) return true;
-    return (size_t)n_rows * t.stride > ((size_t)96 << 20);
+    return (size_t)n_rows * t.stride > ((size_t)50 << 20);
 }
 
 static int scan_grid() {

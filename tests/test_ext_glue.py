@@ -7,11 +7,11 @@ import subprocess
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference/src"
+REF = os.path.join(os.environ.get("PGV_REFERENCE", "/root/reference"), "src")
 EXT = os.path.join(ROOT, "pgvector_b200", "ext")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present (GPU box)")
+@pytest.mark.skipif(not os.path.isdir(REF), reason="no pgvector source tree (PGV_REFERENCE) to compile against")
 @pytest.mark.parametrize("src", ["vb_ivfflat_scan.c", "vb_hnsw_scan.c", "vb_ivfflat_build.c", "vb_hnsw_build.c"])
 def test_glue_parses_against_reference_headers(src):
     cmd = ["gcc", "-fsyntax-only", "-std=gnu11", "-Wall", "-Werror", "-Wno-unused-function", "-Wno-comment",

@@ -129,7 +129,7 @@ def test_gpu_and_oracle_agree_on_the_gpu_built_graph(pv, opclass, dim, n, m, efc
         assert same_q.mean() > 0.95
         assert np.array_equal(nd[same_q], wnd[same_q])
     # quality next to the reference's serial build (oracle restatement) on the same rows WITH THE SAME LEVEL DRAWS
-    # (recall moves by a few points between level draws; measured on B200 with shared levels, 8000 x 32, m = 8:
+    # (recall moves by a few points between level draws; measured with shared levels, 8000 x 32, m = 8:
     # serial 0.6945, batches of 1/64 of the graph 0.6955, 1/8 0.6475, one element at a time 0.6945 = the serial build)
     truth = [O.exact_topk(elem, metric, qq, x, k, dim=dim)[0] for qq in q]
     ob = O.Hnsw(elem, metric, x, m=m, ef_construction=efc, seed=7, dim=dim)

@@ -65,7 +65,7 @@ def test_assign_matches_oracle(pv, tensor_cores, elem, metric, n, dim, k):
     agree = _assign_agreement(elem, metric, rows, centers, got, dim=dim)
     assert agree >= (1.0 if elem == O.BIT else 0.9995), agree
     if tensor_cores and elem != O.BIT and n >= 1024 and k >= 16:
-        assert rechecked >= 0            # the tcgen05 path ran
+        assert rechecked >= 0            # the tensor-core path ran
         assert rechecked <= 0.2 * n      # and only a minority of rows needed the exact kernel
     else:
         assert rechecked == -1

@@ -1,7 +1,10 @@
 """CPU tests: the oracle against the reference's own known-answer outputs
 (tests/golden/distance_kat.json, transcribed from test/expected/*.out) and against
-the reference's halfutils.c/bitutils.c compiled verbatim (oracle/_ref)."""
+what the reference's halfutils.c/bitutils.c return on seeded inputs
+(tests/golden/ref_kernels.npz, recorded by tests/golden/make_ref_kernels.py; when
+oracle/_ref is built, that build is checked against the recording too)."""
 import math
+import os
 
 import numpy as np
 import pytest
@@ -15,6 +18,7 @@ METRIC = {"l2_distance": O.L2, "inner_product": O.IP, "negative_inner_product": 
           "jaccard_distance": O.JACCARD}
 
 KAT = load_golden("distance_kat.json")["cases"]
+REF_KERNELS = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_kernels.npz"))
 
 
 def _expect_float(text):
@@ -81,70 +85,64 @@ def test_kat_coverage():
 
 
 def test_half_conversion_matches_reference_and_numpy():
-    rng = np.random.default_rng(0)
-    xs = np.concatenate([
-        rng.standard_normal(2000).astype(np.float32) * 10,
-        np.float32([0, -0.0, 1, -1, 65504, 65520, 65519.99, 1e-8, 5.96e-8, 2.98e-8, 2.9802322e-8, 6.1e-5, 6.0975552e-5,
-                    1e5, -1e5, np.inf, -np.inf, 0.1, 0.33325195, 1.0009766, 1.00048828125, 1.0014648]),
-        (rng.standard_normal(500) * 1e-6).astype(np.float32),
-    ])
+    from tests.golden.make_ref_kernels import conversion_inputs
+    xs = conversion_inputs()
     L = O.lib()
     R = O.ref()
     npbits = f32_to_half_bits(xs)
-    for x, nb in zip(xs, npbits):
+    for x, nb, rb in zip(xs, npbits, REF_KERNELS["f2h"]):
         ob = L.pgv_float_to_half(float(x))
         assert ob == int(nb), (x, ob, nb)
+        assert ob == int(rb), x
         if R is not None:
             assert R.ref_float_to_half(float(x)) == ob, x
     # widening: all 65536 patterns
     allh = np.arange(65536, dtype=np.uint16)
     npf = half_bits_to_f32(allh)
-    for h in range(0, 65536, 7):
+    for h, rf in zip(range(0, 65536, 7), REF_KERNELS["h2f"]):
         f = L.pgv_half_to_float(h)
         if math.isnan(f):
-            assert math.isnan(npf[h])
+            assert math.isnan(npf[h]) and math.isnan(rf)
         else:
             assert f == npf[h]
+            assert np.float32(f) == rf
             if R is not None:
                 assert R.ref_half_to_float(h) == f
 
 
-@pytest.mark.skipif(O.ref() is None, reason="oracle/_ref not built (needs /root/reference)")
 def test_restated_half_and_bit_kernels_match_reference_build():
-    """The restatement vs the reference's own kernels on random inputs: bit kernels
+    """The restatement vs the reference's own kernels on seeded inputs: bit kernels
     exactly; half kernels within fp32 reassociation noise of the fp64 truth."""
+    from tests.golden.make_ref_kernels import kernel_inputs
     R = O.ref()
-    rng = np.random.default_rng(1)
-    for dim in (1, 3, 8, 9, 64, 100, 768, 1537):
-        a = f32_to_half_bits(rng.standard_normal(dim))
-        b = f32_to_half_bits(rng.standard_normal(dim))
-        pa, pb = a.ctypes.data, b.ctypes.data
+    half, bits = kernel_inputs()
+    for dim, (a, b) in half.items():
+        ref_l2, ref_ip, ref_l1, ref_cos = REF_KERNELS[f"half_{dim}"]
+        if R is not None:
+            pa, pb = a.ctypes.data, b.ctypes.data
+            assert [R.ref_half_l2sq(dim, pa, pb), R.ref_half_ip(dim, pa, pb), R.ref_half_l1(dim, pa, pb),
+                    R.ref_half_cos(dim, pa, pb)] == [ref_l2, ref_ip, ref_l1, ref_cos]
         truth = O.distance(O.HALFVEC, O.L2_SQUARED, a, b, f64=True)
-        for got in (R.ref_half_l2sq(dim, pa, pb), O.distance(O.HALFVEC, O.L2_SQUARED, a, b)):
+        for got in (ref_l2, O.distance(O.HALFVEC, O.L2_SQUARED, a, b)):
             assert abs(got - truth) <= 1e-5 * max(1.0, abs(truth))
         truth = O.distance(O.HALFVEC, O.IP, a, b, f64=True)
         scale = float(np.sum(np.abs(half_bits_to_f32(a) * half_bits_to_f32(b)))) + 1.0
-        for got in (R.ref_half_ip(dim, pa, pb), O.distance(O.HALFVEC, O.IP, a, b)):
+        for got in (ref_ip, O.distance(O.HALFVEC, O.IP, a, b)):
             assert abs(got - truth) <= 1e-5 * scale
         truth = O.distance(O.HALFVEC, O.L1, a, b, f64=True)
-        for got in (R.ref_half_l1(dim, pa, pb), O.distance(O.HALFVEC, O.L1, a, b)):
+        for got in (ref_l1, O.distance(O.HALFVEC, O.L1, a, b)):
             assert abs(got - truth) <= 1e-5 * max(1.0, truth)
-        cos_ref = 1.0 - min(1.0, max(-1.0, R.ref_half_cos(dim, pa, pb)))
+        cos_ref = 1.0 - min(1.0, max(-1.0, ref_cos))
         assert abs(cos_ref - O.distance(O.HALFVEC, O.COSINE, a, b)) <= 1e-5
-    for nbits in (0, 1, 7, 8, 52, 63, 64, 65, 513, 1024, 4099):
+    for nbits, (a, b) in bits.items():
+        ref_ham, ref_jac = REF_KERNELS[f"bit_{nbits}"]
         nbytes = (nbits + 7) // 8
-        a = rng.integers(0, 256, size=max(nbytes, 1), dtype=np.uint8)[:nbytes].copy()
-        b = rng.integers(0, 256, size=max(nbytes, 1), dtype=np.uint8)[:nbytes].copy()
-        if nbits % 8 and nbytes:
-            mask = (0xFF << (8 - nbits % 8)) & 0xFF
-            a[-1] &= mask
-            b[-1] &= mask
-        a = np.ascontiguousarray(a)
-        b = np.ascontiguousarray(b)
-        pa = a.ctypes.data if nbytes else None
-        pb = b.ctypes.data if nbytes else None
-        assert R.ref_bit_hamming(nbytes, pa, pb) == O.distance(O.BIT, O.HAMMING, a, b, dim=nbits)
-        assert R.ref_bit_jaccard(nbytes, pa, pb) == O.distance(O.BIT, O.JACCARD, a, b, dim=nbits)
+        if R is not None:
+            pa = a.ctypes.data if nbytes else None
+            pb = b.ctypes.data if nbytes else None
+            assert R.ref_bit_hamming(nbytes, pa, pb) == ref_ham and R.ref_bit_jaccard(nbytes, pa, pb) == ref_jac
+        assert ref_ham == O.distance(O.BIT, O.HAMMING, a, b, dim=nbits)
+        assert ref_jac == O.distance(O.BIT, O.JACCARD, a, b, dim=nbits)
 
 
 def test_cross_type_equality_small_integers():
