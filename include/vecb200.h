@@ -162,6 +162,21 @@ int			vb_exact_topk(vb_table *t, int metric, const void *queries, int64_t nq, in
 int			vb_exact_topk_dev(vb_table *t, int metric, const void *queries_dev, int64_t nq, int k,
 							  int64_t *out_ids_dev, float *out_dist_dev);
 
+/*
+ * Re-rank: for each query, the k nearest of ITS candidate rows of the table, under the SQL operator -- the outer
+ * "ORDER BY v <op> q LIMIT k" over an inner index scan's result (README quantize-then-rerank flow).
+ * cand[q*c + j] = a row number of t (append order); -1 = no candidate.  metric: as vb_exact_topk (VB_L2, VB_L2_SQUARED,
+ * VB_IP, VB_NEG_IP, VB_COSINE, VB_L1 for vector / halfvec; VB_HAMMING, VB_JACCARD for bit).  1 <= k <= 2048, c >= 0.
+ * out_ids = row numbers, -1 padded when a query has fewer than k candidates; out_dist = the operator's float8, as
+ * vb_exact_topk reports it.  Ties: earlier candidate position first.  A row listed twice is scored twice.
+ * Host variant: a candidate outside [-1, n) fails with VB_EINVAL naming query, position and value, nothing written.
+ * _dev variant: asynchronous on vb_stream(), no host read; candidates outside [0, n) are treated as absent (never read).
+ */
+int			vb_table_rerank(vb_table *t, int metric, const void *queries, int64_t nq, const int64_t *cand, int c, int k,
+							int64_t *out_ids, double *out_dist);
+int			vb_table_rerank_dev(vb_table *t, int metric, const void *queries_dev, int64_t nq, const int64_t *cand_dev, int c,
+								int k, int64_t *out_ids_dev, float *out_dist_dev);
+
 /* ---------------------------------------------------------------- sparsevec */
 
 /*

@@ -229,6 +229,45 @@ class Table:
         _lib.check(load().vb_exact_topk(self.h, metric, _ptr(queries), nq, k, _ptr(ids), _ptr(dist)))
         return ids, dist
 
+    def rerank(self, metric, queries, candidates, k):
+        """ORDER BY v <op> q LIMIT k over each query's own candidate rows: candidates[q] = row numbers of this table
+        (-1 = none), typically what an index on a cheaper form of the vector returned (quantize-then-rerank).
+        numpy inputs -> (int64 ids, float64 distances); torch CUDA tensors -> (int64 ids, float32 distances)."""
+        k = int(k)
+        raw = (self.dim + 7) // 8 if self.elem == BIT else self.dim
+        if _is_torch(queries) or _is_torch(candidates):
+            import torch
+            if not (_is_torch(queries) and _is_torch(candidates) and queries.is_cuda and candidates.is_cuda):
+                raise TypeError("rerank: queries and candidates must both be CUDA tensors or both host arrays")
+            if queries.dim() != 2 or queries.shape[1] != raw:
+                raise ValueError(f"rerank: queries must have shape [nq, {raw}], got {tuple(queries.shape)}")
+            nq = queries.shape[0]
+            if candidates.dtype != torch.int64 or candidates.dim() != 2 or candidates.shape[0] != nq:
+                raise ValueError(f"rerank: candidates must be int64 of shape [{nq}, c], got {candidates.dtype} {tuple(candidates.shape)}")
+            queries, candidates = queries.contiguous(), candidates.contiguous()
+            ids = torch.empty((nq, k), dtype=torch.int64, device=queries.device)
+            dist = torch.empty((nq, k), dtype=torch.float32, device=queries.device)
+            _after_torch(queries, candidates)
+            _lib.check(load().vb_table_rerank_dev(self.h, metric, _ptr(queries), nq, _ptr(candidates), candidates.shape[1], k,
+                                                  _ptr(ids), _ptr(dist)))
+            synchronize()   # the library runs on its own stream; results are handed back complete
+            return ids, dist
+        queries = _host(self.elem, queries)
+        if queries.ndim == 1:
+            queries = queries.reshape(1, -1)
+        if queries.ndim != 2 or queries.shape[1] != raw:
+            raise ValueError(f"rerank: queries must have shape [nq, {raw}], got {queries.shape}")
+        nq = queries.shape[0]
+        candidates = np.asarray(candidates)
+        if candidates.dtype != np.int64 or candidates.ndim != 2 or candidates.shape[0] != nq:
+            raise ValueError(f"rerank: candidates must be int64 of shape [{nq}, c], got {candidates.dtype} {candidates.shape}")
+        candidates = np.ascontiguousarray(candidates)
+        ids = np.empty((nq, k), dtype=np.int64)
+        dist = np.empty((nq, k), dtype=np.float64)
+        _lib.check(load().vb_table_rerank(self.h, metric, _ptr(queries), nq, _ptr(candidates), candidates.shape[1], k,
+                                          _ptr(ids), _ptr(dist)))
+        return ids, dist
+
     def exact_topk_sharded(self, metric, queries_dev, k, id_offset):
         """exact top-k over a row-sharded table (collective over the library's communicator); torch CUDA tensors"""
         import torch

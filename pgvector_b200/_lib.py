@@ -52,6 +52,8 @@ SIGNATURES = {
     "vb_table_free": (_i, [_vp]),
     "vb_exact_topk": (_i, [_vp, _i, _vp, _i64, _i, _vp, _vp]),
     "vb_exact_topk_dev": (_i, [_vp, _i, _vp, _i64, _i, _vp, _vp]),
+    "vb_table_rerank": (_i, [_vp, _i, _vp, _i64, _vp, _i, _i, _vp, _vp]),
+    "vb_table_rerank_dev": (_i, [_vp, _i, _vp, _i64, _vp, _i, _i, _vp, _vp]),
     "vb_ivf_create": (_i, [_i, _i, _i, _i, C.POINTER(_vp)]),
     "vb_ivf_load": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "vb_ivf_load_dev": (_i, [_vp, _vp, _vp, _vp, _vp]),

@@ -143,6 +143,9 @@ int launch_scan_regular(const Table& t, int key_metric, const void* q_dev, size_
 // distances of chunk-list work; n_chunks_dev holds the chunk count (device int32)
 int launch_scan_chunks(const Table& t, int key_metric, const void* q_dev, size_t qstride,
                        const Chunk* chunks_dev, const int* n_chunks_dev, int max_chunks, float* out);
+// distances of chunk-list work over gathered rows: row r of a chunk is table row ids_dev[row_begin + r] (LDG kernel)
+int launch_scan_gather(const Table& t, int key_metric, const void* q_dev, size_t qstride, const int64_t* ids_dev,
+                       const Chunk* chunks_dev, const int* n_chunks_dev, int max_chunks, float* out);
 // Jaccard needs the exact float8: out as double
 int launch_scan_regular_f64(const Table& t, int key_metric, const void* q_dev, size_t qstride, int64_t nq,
                             int64_t n_rows, double* out, int64_t out_stride);

@@ -176,6 +176,13 @@ struct Acc {
 };
 
 
+// float key -> the operator's float8 (sqrt for <->, negate for inner_product)
+__device__ __forceinline__ double finish_value(int metric, float key) {
+    if (metric == VB_L2) return sqrt((double)key);
+    if (metric == VB_IP) return -(double)key;
+    return (double)key;
+}
+
 // arguments of the scan kernels (vb_scan.cu: LDG variant, vb_scan_bulk.cu: bulk-copy/TMA variant)
 struct ScanArgs {
     const uint8_t* rows;

@@ -24,13 +24,6 @@ __global__ void regular_segments_kernel(int64_t nseg, int64_t stride, int32_t le
     }
 }
 
-// float key -> the operator's float8 (sqrt for <->, negate for inner_product)
-__device__ __forceinline__ double finish_value(int metric, float key) {
-    if (metric == VB_L2) return sqrt((double)key);
-    if (metric == VB_IP) return -(double)key;
-    return (double)key;
-}
-
 __global__ void finish_exact_kernel(int metric, int64_t n, const int32_t* __restrict__ pos, const float* __restrict__ key,
                                     int64_t* __restrict__ out_ids, float* __restrict__ out_f, double* __restrict__ out_d) {
     int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;

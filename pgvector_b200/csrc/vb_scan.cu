@@ -26,8 +26,10 @@ namespace vb {
 
 constexpr int SCAN_THREADS = 128;
 
-template <int ELEM, int METRIC, int LPR, int RPI, typename OUT>
-__global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(ScanArgs a) {
+// GATHER: row r of a chunk is table row ids[row_begin + r] (the candidate lists of vb_rerank.cu) instead of row
+// row_begin + r; the per-row arithmetic is the same, so gathered distances are bit-identical to the contiguous scan's.
+template <int ELEM, int METRIC, int LPR, int RPI, typename OUT, bool GATHER>
+__device__ __forceinline__ void scan_body(const ScanArgs& a, const int64_t* __restrict__ ids) {
     extern __shared__ uint4 sq[];
     constexpr int G = SCAN_THREADS / LPR;  // row groups per CTA
     const int g = threadIdx.x / LPR;
@@ -78,7 +80,10 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(ScanArgs a) {
             for (int i = 0; i < RPI; ++i) {
                 int r = r0 + i * G;
                 // clamp so out-of-range lanes re-read a valid row (result discarded)
-                rp[i] = reinterpret_cast<const uint4*>(base + (size_t)min(r, n_rows - 1) * a.stride);
+                if constexpr (GATHER)
+                    rp[i] = reinterpret_cast<const uint4*>(a.rows + (size_t)ids[row_begin + min(r, n_rows - 1)] * a.stride);
+                else
+                    rp[i] = reinterpret_cast<const uint4*>(base + (size_t)min(r, n_rows - 1) * a.stride);
             }
             // register double buffering: the loads of step v + LPR are issued before the FMAs of step v,
             // so 2 * RPI independent 128-bit loads per thread stay in flight through the whole row set
@@ -112,17 +117,33 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(ScanArgs a) {
     }
 }
 
+template <int ELEM, int METRIC, int LPR, int RPI, typename OUT>
+__global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(ScanArgs a) {
+    scan_body<ELEM, METRIC, LPR, RPI, OUT, false>(a, nullptr);
+}
+
+template <int ELEM, int METRIC, int LPR, int RPI>
+__global__ void __launch_bounds__(SCAN_THREADS) scan_gather_kernel(ScanArgs a, const int64_t* __restrict__ ids) {
+    scan_body<ELEM, METRIC, LPR, RPI, float, true>(a, ids);
+}
+
 // ----------------------------------------------------------------------------- dispatch
 
-template <int ELEM, int METRIC, typename OUT>
-static int launch_scan_t(const ScanArgs& a, int grid, cudaStream_t s) {
+template <int ELEM, int METRIC, typename OUT, bool GATHER>
+static int launch_scan_t(const ScanArgs& a, const int64_t* ids, int grid, cudaStream_t s) {
     size_t smem = a.qstride;
     int V = a.vec_per_row;
 #define VB_LAUNCH(LPR, RPI)                                                                          \
     do {                                                                                             \
-        auto kern = scan_kernel<ELEM, METRIC, LPR, RPI, OUT>;                                        \
-        if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        kern<<<grid, SCAN_THREADS, smem, s>>>(a);                                                    \
+        if constexpr (GATHER) {                                                                      \
+            auto kern = scan_gather_kernel<ELEM, METRIC, LPR, RPI>;                                  \
+            if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            kern<<<grid, SCAN_THREADS, smem, s>>>(a, ids);                                           \
+        } else {                                                                                     \
+            auto kern = scan_kernel<ELEM, METRIC, LPR, RPI, OUT>;                                    \
+            if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            kern<<<grid, SCAN_THREADS, smem, s>>>(a);                                                \
+        }                                                                                            \
     } while (0)
     if (V >= 32) VB_LAUNCH(32, 4);
     else if (V >= 16) VB_LAUNCH(16, 4);
@@ -136,26 +157,26 @@ static int launch_scan_t(const ScanArgs& a, int grid, cudaStream_t s) {
     return VB_OK;
 }
 
-template <typename OUT>
-static int launch_scan_any(int elem, int metric, const ScanArgs& a, int grid, cudaStream_t s) {
+template <typename OUT, bool GATHER = false>
+static int launch_scan_any(int elem, int metric, const ScanArgs& a, int grid, cudaStream_t s, const int64_t* ids = nullptr) {
     if (elem == VB_VECTOR) {
         switch (metric) {
-            case VB_L2_SQUARED: return launch_scan_t<VB_VECTOR, VB_L2_SQUARED, OUT>(a, grid, s);
-            case VB_NEG_IP: return launch_scan_t<VB_VECTOR, VB_NEG_IP, OUT>(a, grid, s);
-            case VB_COSINE: return launch_scan_t<VB_VECTOR, VB_COSINE, OUT>(a, grid, s);
-            case VB_L1: return launch_scan_t<VB_VECTOR, VB_L1, OUT>(a, grid, s);
+            case VB_L2_SQUARED: return launch_scan_t<VB_VECTOR, VB_L2_SQUARED, OUT, GATHER>(a, ids, grid, s);
+            case VB_NEG_IP: return launch_scan_t<VB_VECTOR, VB_NEG_IP, OUT, GATHER>(a, ids, grid, s);
+            case VB_COSINE: return launch_scan_t<VB_VECTOR, VB_COSINE, OUT, GATHER>(a, ids, grid, s);
+            case VB_L1: return launch_scan_t<VB_VECTOR, VB_L1, OUT, GATHER>(a, ids, grid, s);
         }
     } else if (elem == VB_HALFVEC) {
         switch (metric) {
-            case VB_L2_SQUARED: return launch_scan_t<VB_HALFVEC, VB_L2_SQUARED, OUT>(a, grid, s);
-            case VB_NEG_IP: return launch_scan_t<VB_HALFVEC, VB_NEG_IP, OUT>(a, grid, s);
-            case VB_COSINE: return launch_scan_t<VB_HALFVEC, VB_COSINE, OUT>(a, grid, s);
-            case VB_L1: return launch_scan_t<VB_HALFVEC, VB_L1, OUT>(a, grid, s);
+            case VB_L2_SQUARED: return launch_scan_t<VB_HALFVEC, VB_L2_SQUARED, OUT, GATHER>(a, ids, grid, s);
+            case VB_NEG_IP: return launch_scan_t<VB_HALFVEC, VB_NEG_IP, OUT, GATHER>(a, ids, grid, s);
+            case VB_COSINE: return launch_scan_t<VB_HALFVEC, VB_COSINE, OUT, GATHER>(a, ids, grid, s);
+            case VB_L1: return launch_scan_t<VB_HALFVEC, VB_L1, OUT, GATHER>(a, ids, grid, s);
         }
     } else {
         switch (metric) {
-            case VB_HAMMING: return launch_scan_t<VB_BIT, VB_HAMMING, OUT>(a, grid, s);
-            case VB_JACCARD: return launch_scan_t<VB_BIT, VB_JACCARD, OUT>(a, grid, s);
+            case VB_HAMMING: return launch_scan_t<VB_BIT, VB_HAMMING, OUT, GATHER>(a, ids, grid, s);
+            case VB_JACCARD: return launch_scan_t<VB_BIT, VB_JACCARD, OUT, GATHER>(a, ids, grid, s);
         }
     }
     set_error("unsupported metric %d for element type %d", metric, elem);
@@ -241,6 +262,23 @@ int launch_scan_chunks(const Table& t, int metric, const void* q_dev, size_t qst
         return launch_scan_bulk(t.elem, metric, a, false, max_chunks);
     int grid = std::min(max_chunks, scan_grid());
     return launch_scan_any<float>(t.elem, metric, a, grid, ctx().stream);
+}
+
+int launch_scan_gather(const Table& t, int metric, const void* q_dev, size_t qstride, const int64_t* ids_dev,
+                       const Chunk* chunks_dev, const int* n_chunks_dev, int max_chunks, float* out) {
+    if (max_chunks <= 0) return VB_OK;
+    ScanArgs a{};
+    a.rows = t.d;
+    a.stride = t.stride;
+    a.vec_per_row = (int)(t.stride / 16);
+    a.queries = (const uint8_t*)q_dev;
+    a.qstride = qstride;
+    a.qvec = (int)(qstride / 16);
+    a.chunks = chunks_dev;
+    a.n_chunks_dev = n_chunks_dev;
+    a.out = out;
+    int grid = std::min(max_chunks, scan_grid());
+    return launch_scan_any<float, true>(t.elem, metric, a, grid, ctx().stream, ids_dev);
 }
 
 // ----------------------------------------------------------------------------- per-segment top-k

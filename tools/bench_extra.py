@@ -6,6 +6,7 @@ does not cover: k-means assign on the tensor cores (config D shape, one GPU's sh
     python tools/bench_extra.py assign   [--rows N --dim D --k K]
     python tools/bench_extra.py hnsw     [--elem halfvec|bit --rows N --dim D --ef EF]
     python tools/bench_extra.py exact    [--rows N --dim D]
+    python tools/bench_extra.py rerank   [--rows N --dim D]     (bit HNSW candidates re-ranked on the fp32 rows)
 
 All timing with CUDA events on the library stream; inputs resident in HBM.
 """
@@ -150,6 +151,109 @@ def bench_hnsw(args):
                       "roofline": {"bound": "hbm", "achieved": gbs, "peak": hbm, "unit": "GB/s", "frac": gbs / hbm, "peak_source": src,
                                    "note": "latency-bound random gathers; bytes = n_dist*row + n_expand*lm*4"},
                       "cpu_baseline": {"value": cpu_qps, "unit": "queries/s", "cores": os.cpu_count(), "kind": "port"}}))
+
+
+def card():
+    """name and power limit of the cards, read in the same run as the numbers they qualify (a read-only query)"""
+    import subprocess
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=60)
+        return [line.strip() for line in r.stdout.splitlines() if line.strip()] or r.stderr.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        return f"nvidia-smi failed: {e}"
+
+
+def bench_rerank(args):
+    """pgvector's quantize-then-rerank on config E's law at a reduced row count: a bit(dim) HNSW over binary_quantize(rows)
+    fetches ef_search candidates per query, then the fp32 rows re-rank them under cosine (vb_table_rerank_dev)."""
+    import torch
+    import pgvector_b200 as pv
+    pv.init(0)
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.ExternalStream(pv.stream_handle(), device=dev)
+    n, dim, nq, ef, k = args.rows, args.dim, args.queries, args.ef, 10
+    assert dim % 8 == 0, "--dim must be a multiple of 8"
+    # low intrinsic dimension (the law of bench_hnsw), generated on the device in slices
+    g = torch.Generator(device=dev).manual_seed(6)
+    frame = torch.linalg.qr(torch.randn((dim, 16), generator=g, device=dev))[0]
+    weights = torch.tensor([128, 64, 32, 16, 8, 4, 2, 1], dtype=torch.uint8, device=dev)
+
+    def law(m):
+        return (torch.randn((m, 16), generator=g, device=dev) @ frame.T + 0.02 * torch.randn((m, dim), generator=g, device=dev)).contiguous()
+
+    def quantize(x):   # binary_quantize: a bit per element, set where it is > 0, MSB first
+        return ((x > 0).to(torch.uint8).reshape(x.shape[0], -1, 8) * weights).sum(-1).to(torch.uint8).contiguous()
+
+    table = pv.Table(pv.VECTOR, dim)
+    bits = []
+    for r0 in range(0, n, 1 << 17):
+        x = law(min(1 << 17, n - r0))
+        table.append(x)
+        bits.append(quantize(x))
+        if r0 == 0:
+            sample = x[:1000].cpu().numpy()
+            assert np.array_equal(bits[0][:1000].cpu().numpy(), pv.binary_quantize(sample)), "device quantization != binary_quantize"
+        del x
+    bits = torch.cat(bits)
+    q = law(nq)
+    qbits = quantize(q)
+    torch.cuda.synchronize()
+    ix = pv.HnswIndex("bit_hamming_ops", dim, m=16)
+    t0 = time.perf_counter()
+    ix.build(bits, ef_construction=64, seed=42)
+    pv.synchronize()
+    build_s = time.perf_counter() - t0
+    folded = int((ix.export()["dup_of"] >= 0).sum())
+
+    cids = torch.empty((nq, ef), dtype=torch.int64, device=dev)
+    cdist = torch.empty((nq, ef), dtype=torch.float32, device=dev)
+    rids = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    rdist = torch.empty((nq, k), dtype=torch.float32, device=dev)
+
+    def search():
+        ix.search_into(qbits, ef, ef, cids, cdist)
+
+    def rerank(qq=q, cand=cids, out_i=rids, out_d=rdist):
+        pv._lib.check(pv.load().vb_table_rerank_dev(table.h, pv.COSINE, pv._ptr(qq), qq.shape[0], pv._ptr(cand), cand.shape[1], k,
+                                                    pv._ptr(out_i), pv._ptr(out_d)))
+
+    def both():
+        search()
+        rerank()
+
+    ms_search = timed(pv, torch, stream, search, warmup=2, steps=10)
+    ms_both = timed(pv, torch, stream, both, warmup=2, steps=10)
+    ms_rerank = timed(pv, torch, stream, rerank, warmup=3, steps=20)   # on the candidates of the last search
+    single = {}
+    for c in (20, 200):
+        c1 = cids[:1, :c].contiguous()
+        i1, d1 = rids[:1].clone(), rdist[:1].clone()
+        single[f"c{c}"] = timed(pv, torch, stream, lambda: rerank(q[:1], c1, i1, d1), warmup=10, steps=200)
+
+    # recall@10 against fp32 cosine truth (vb_exact_topk)
+    truth = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    tdist = torch.empty((nq, k), dtype=torch.float32, device=dev)
+    pv._lib.check(pv.load().vb_exact_topk_dev(table.h, pv.COSINE, pv._ptr(q), nq, k, pv._ptr(truth), pv._ptr(tdist)))
+    pv.synchronize()
+    tr, ca, rr = truth.cpu().numpy(), cids.cpu().numpy(), rids.cpu().numpy()
+
+    def recall(got):
+        return sum(len(set(a.tolist()) & set(b.tolist())) for a, b in zip(got, tr)) / (nq * k)
+
+    valid = int((cids >= 0).sum().item())
+    stride = table.device_rows()[1]
+    moved = valid * stride + nq * ef * 8 + nq * dim * 4
+    hbm, _, _, src = peaks()
+    gbs = moved / (ms_rerank / 1000.0) / 1e9
+    print(json.dumps({"bench": "rerank", "workload": f"bit({dim}) HNSW (bit_hamming_ops, m=16, ef_construction=64) over binary_quantize of {n}x{dim} fp32 rows, "
+                                                     f"{nq} queries, ef_search={ef}, candidates c={ef}, re-ranked by cosine on the fp32 rows, k={k}",
+                      "card": card(), "index_build_s": build_s, "rows_folded_as_duplicates": folded,
+                      "ms_per_batch": {"bit_search": ms_search, "rerank": ms_rerank, "search_then_rerank": ms_both},
+                      "single_query_rerank_ms": single,
+                      "recall_at_10": {"bit_top10": recall(ca[:, :k]), "reranked_top10": recall(rr), "candidate_set": recall(ca)},
+                      "roofline": {"bound": "hbm", "kernel": "rerank (prepare + gathered scan + select + finish)", "achieved": gbs, "peak": hbm,
+                                   "unit": "GB/s", "frac": gbs / hbm, "bytes_per_batch": moved, "valid_candidates": valid, "peak_source": src,
+                                   "note": "bytes = valid candidates x row stride + candidate ids + queries"}}))
 
 
 def bench_ivf(args):
@@ -324,7 +428,7 @@ def bench_sparse(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "kmeans", "sparse"])
+    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "kmeans", "sparse", "rerank"])
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--lists", type=int, default=1000)
     ap.add_argument("--probes", type=int, default=10)
@@ -332,10 +436,13 @@ if __name__ == "__main__":
     ap.add_argument("--dim", type=int, default=None)
     ap.add_argument("--k", type=int, default=4096)
     ap.add_argument("--elem", default="halfvec")
-    ap.add_argument("--ef", type=int, default=100)
-    ap.add_argument("--queries", type=int, default=4096)
+    ap.add_argument("--ef", type=int, default=None)
+    ap.add_argument("--queries", type=int, default=None)
     ap.add_argument("--nnz", type=int, default=100)
     a = ap.parse_args()
+    if a.what == "rerank":      # config E's query batch and ef_search
+        a.queries, a.ef = a.queries or 2048, a.ef or 200
+    a.queries, a.ef = a.queries or 4096, a.ef or 100
     if a.what == "sparse":
         a.rows = a.rows or 1_000_000
         a.dim = a.dim or 100_000
@@ -349,6 +456,10 @@ if __name__ == "__main__":
         a.rows = a.rows or 100_000
         a.dim = a.dim or (768 if a.elem == "halfvec" else 1024)
         bench_hnsw(a)
+    elif a.what == "rerank":
+        a.rows = a.rows or 1_000_000
+        a.dim = a.dim or 1024
+        bench_rerank(a)
     elif a.what == "kmeans":
         a.dim = a.dim or 1536
         bench_kmeans(a)
