@@ -281,6 +281,58 @@ int			vb_ivf_search_dev(vb_ivf *ix, const void *queries_dev, int64_t nq, int pro
  */
 int			vb_ivf_prefetch_queries(vb_ivf *ix, const void *queries, int64_t nq, int slot);
 int			vb_ivf_search_prefetched(vb_ivf *ix, int slot, int probes, int k, int64_t *out_ids, double *out_dist);
+/*
+ * ivfflat.iterative_scan (src/ivfscan.c:123-187 GetScanItems, :252-283 ivfflatbeginscan, :400-406 ivfflatgettuple) for
+ * nq queries at once.  The handle owns what IvfflatScanOpaqueData keeps between batches: the probe order, listIndex
+ * and the position in the sorted batch.
+ *
+ * Begin.  p = min(probes, lists) and P = min(max(max_probes, probes), lists), as ivfflatbeginscan clamps them
+ * (:268-277); max_probes = probes is iterative_scan = off.  Probe selection runs for P lists per query: the lists and
+ * their order are what vb_ivf_scan_lists(q, P) returns (ties by list number).  Queries are host memory; begin
+ * returns synchronised.  Cosine opclasses: the caller normalises the queries, as for vb_ivf_search.
+ *
+ * The sequence S_q of a query.  L[0..P) is split into groups of p consecutive lists (the last may be short).  S_q is
+ * the concatenation, over the groups in order, of all rows of the group's lists sorted by (distance, scan position),
+ * the scan position being the position in the concatenation of the group's lists in probe order, rows in stored
+ * order: GetScanItems + tuplesort_performsort + the loop at :400-406.  Distances are the float8 vb_ivf_scan_items
+ * reports; ids are the heap ids given at load, or row positions when those were NULL.
+ *
+ * Next.  Per query, the next <= page elements of S_q go to out_ids / out_dist [nq x page] (-1 / +inf padded) and
+ * their number to out_counts[q].  A page never spans two groups: a query whose group ran dry moves to its next
+ * non-empty group within the same call (empty lists and groups are skipped as the reference's while loop skips
+ * them).  out_counts[q] == 0 if and only if S_q is exhausted, and stays 0.  Queries progress independently: in one
+ * call some may still drain group 0 while others start group 3.  vb_ivf_scan_lists_done writes the reference's
+ * so->listIndex per query [nq]: 0 before the first next, P once the sequence is exhausted.
+ *
+ * Limits.  1 <= page <= 2048 (the selection stays on the device), probes >= 1, max_probes >= 1, nq >= 1, queries not
+ * NULL (NULL-query scans keep vb_ivf_scan_items, as for vb_ivf_search), the index loaded: VB_EINVAL / VB_ESTATE and a
+ * message otherwise.
+ *
+ * State.  Everything a handle keeps between calls lives in device memory it owns, so other searches or handles between
+ * two next calls do not change a sequence.  Begin allocates per query the query image, P probe slots, the group's
+ * candidate distances (as many as the p longest lists hold), group lists and offsets, the cursor and the page staging, plus the scan chunk
+ * descriptors; when that does not fit next to the index it fails with VB_ENOMEM, names the bytes per query and
+ * allocates nothing.  next allocates nothing.  vb_ivf_load*, vb_ivf_begin_load, vb_ivf_end_load and
+ * vb_ivf_replace_list change the image: next on a handle opened before fails with VB_ESTATE ("index changed since the
+ * scan began") and writes nothing.  end always succeeds; end every handle before vb_ivf_free.
+ *
+ * Equivalence with the per-scan path.  For every query, S_q is bit-identical in ids and distances to what successive
+ * vb_ivf_scan_items(q, L[g p ..], cap = all) calls return when those calls score with scan_kernel's per-row arithmetic:
+ * the fused one-query kernels (the default for one query) and option scan_impl = 0.  The handle therefore always
+ * scores with that arithmetic (the LDG chunk scan), whatever scan_impl says.  The bulk-copy scan (scan_bulk_kernel,
+ * scan_impl 1, or 2 on tables above 50 MB) is not bit-identical in general: it splits every row over 32 lanes where
+ * the LDG scan uses fewer for rows narrower than 512 bytes, and it scores halfvec rows against a half-precision query
+ * image; for vector and bit rows of 512 bytes and more the two follow the same per-lane order.  The list-major and
+ * tensor-core formulations of vb_ivf_search are not used here: a filter cannot certify a full order, and list-major
+ * distances differ in the last bits.  This is what lets a caller serve the first pages of a request from a batch and
+ * the rest per scan without a visible difference.
+ */
+typedef struct vb_ivf_scan vb_ivf_scan;
+int			vb_ivf_scan_begin(vb_ivf *ix, const void *queries, int64_t nq, int probes, int max_probes, int page,
+							  vb_ivf_scan **out);
+int			vb_ivf_scan_next(vb_ivf_scan *scan, int64_t *out_ids, double *out_dist, int32_t *out_counts);
+int			vb_ivf_scan_lists_done(vb_ivf_scan *scan, int32_t *out);	/* [nq]: the reference's so->listIndex */
+int			vb_ivf_scan_end(vb_ivf_scan *scan);
 /* algorithmic bytes of the last vb_ivf_search*: sum over queries of (lists + candidates) * dim * elem size (SURVEY 8d) */
 int64_t		vb_ivf_last_scan_bytes(const vb_ivf *ix);
 int64_t		vb_ivf_last_candidates(const vb_ivf *ix);

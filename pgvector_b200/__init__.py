@@ -404,6 +404,14 @@ class IvfflatIndex:
         _lib.check(load().vb_ivf_search(self.h, _ptr(q), nq, p, k, _ptr(ids), _ptr(dist)))
         return ids, dist
 
+    def iterative_scan(self, queries, probes=None, max_probes=None, page=100):
+        """ivfflat.iterative_scan = relaxed_order for a batch of queries: an IvfflatScan whose next_batch() returns the next
+        page of every query's sequence (src/ivfscan.c:400-406).  probes / max_probes mirror ivfflat.probes /
+        ivfflat.max_probes; max_probes defaults to probes (iterative_scan = off).  Cosine opclasses: pass
+        prepare_query(queries)."""
+        p = int(probes or self.probes)
+        return IvfflatScan(self, queries, p, int(max_probes or p), int(page))
+
     def search_into(self, queries_dev, k, probes, ids_dev, dist_dev):
         """asynchronous device-resident search into preallocated torch tensors (bench inner loop): enqueued on the
         library stream after torch's current stream; the caller synchronises (pv.synchronize()) before reading."""
@@ -454,6 +462,63 @@ class IvfflatIndex:
     def __del__(self):
         try:
             self.free()
+        except Exception:
+            pass
+
+
+class IvfflatScan:
+    """One ivfflat iterative index scan per query (src/ivfscan.c:360-414): next_batch() returns (ids, distances, counts) of
+    the next <= page elements of every query, nearest first within a group of `probes` lists; counts == 0 marks an
+    exhausted scan.  Close it (or use it as a context manager) before the index changes or is freed."""
+
+    def __init__(self, index, queries, probes, max_probes, page):
+        q = None if queries is None else _host(index.elem, queries)   # (NULL queries: the library refuses them)
+        if q is not None and q.ndim == 1:
+            q = q.reshape(1, -1)
+        self.index, self.page = index, page
+        self.nq = 0 if q is None else q.shape[0]
+        self.h = None
+        h = C.c_void_p()
+        _lib.check(load().vb_ivf_scan_begin(index.h, _ptr(q), self.nq, probes, max_probes, page, C.byref(h)))
+        self.h = h
+
+    def next_batch(self):
+        ids = np.empty((self.nq, self.page), dtype=np.int64)
+        dist = np.empty((self.nq, self.page), dtype=np.float64)
+        cnt = np.empty(self.nq, dtype=np.int32)
+        _lib.check(load().vb_ivf_scan_next(self.h, _ptr(ids), _ptr(dist), _ptr(cnt)))
+        return ids, dist, cnt
+
+    def lists_done(self):
+        """per query, the lists scanned so far (the reference's listIndex)"""
+        out = np.empty(self.nq, dtype=np.int32)
+        _lib.check(load().vb_ivf_scan_lists_done(self.h, _ptr(out)))
+        return out
+
+    def tuples_of(self, query=0, limit=None):
+        """what ivfflatgettuple hands the executor for one query, in order: (heap id, distance) pairs"""
+        out = []
+        while limit is None or len(out) < limit:
+            ids, dist, cnt = self.next_batch()
+            if cnt[query] == 0:
+                break
+            out.extend((int(ids[query, j]), float(dist[query, j])) for j in range(int(cnt[query])))
+        return out if limit is None else out[:limit]
+
+    def close(self):
+        if self.h:
+            load().vb_ivf_scan_end(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
         except Exception:
             pass
 

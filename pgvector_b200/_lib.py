@@ -67,6 +67,10 @@ SIGNATURES = {
     "vb_ivf_scan_items": (_i, [_vp, _vp, _vp, _i, _i64, _vp, _vp, _vp]),
     "vb_ivf_search": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
     "vb_ivf_search_dev": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
+    "vb_ivf_scan_begin": (_i, [_vp, _vp, _i64, _i, _i, _i, C.POINTER(_vp)]),
+    "vb_ivf_scan_next": (_i, [_vp, _vp, _vp, _vp]),
+    "vb_ivf_scan_lists_done": (_i, [_vp, _vp]),
+    "vb_ivf_scan_end": (_i, [_vp]),
     "vb_ivf_prefetch_queries": (_i, [_vp, _vp, _i64, _i]),
     "vb_ivf_search_prefetched": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "vb_ivf_last_scan_bytes": (_i64, [_vp]),

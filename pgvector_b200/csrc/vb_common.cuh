@@ -140,9 +140,10 @@ struct Chunk {           // one unit of scan work: a run of rows against one que
 // distances of regular work: every query against rows [0, n) ; out[q * out_stride + r]
 int launch_scan_regular(const Table& t, int key_metric, const void* q_dev, size_t qstride, int64_t nq,
                         int64_t n_rows, float* out, int64_t out_stride);
-// distances of chunk-list work; n_chunks_dev holds the chunk count (device int32)
+// distances of chunk-list work; n_chunks_dev holds the chunk count (device int32).  ldg_only: always the LDG kernel
+// (scan_kernel), whose per-row arithmetic the scans of one query share, never the bulk-copy one
 int launch_scan_chunks(const Table& t, int key_metric, const void* q_dev, size_t qstride,
-                       const Chunk* chunks_dev, const int* n_chunks_dev, int max_chunks, float* out);
+                       const Chunk* chunks_dev, const int* n_chunks_dev, int max_chunks, float* out, bool ldg_only = false);
 // distances of chunk-list work over gathered rows: row r of a chunk is table row ids_dev[row_begin + r] (LDG kernel)
 int launch_scan_gather(const Table& t, int key_metric, const void* q_dev, size_t qstride, const int64_t* ids_dev,
                        const Chunk* chunks_dev, const int* n_chunks_dev, int max_chunks, float* out);
@@ -158,6 +159,10 @@ int launch_segment_topk_v(const float* keys, const int64_t* seg_begin_dev, const
                           const int64_t* seg_begin_host, const int32_t* seg_len_host, int64_t nseg, int k,
                           int32_t* out_pos, float* out_key);
 int scan_chunk_rows(const Table& t);
+// the k smallest keys of every segment strictly above floor_key[seg] (once returned[seg] > 0), ascending; then
+// floor_key / returned advance past the page and count[seg] = its size.  k <= 2048 (the paged scan of vb_ivf_iter.cu)
+int launch_segment_topk_floor(const float* keys, const int64_t* seg_begin_dev, const int32_t* seg_len_dev, int64_t nseg, int k,
+                              uint64_t* floor_key, int32_t* returned, int32_t* count, int32_t* out_pos, float* out_key);
 
 // exact fp32 nearest-centre assign (vb_kmeans.cu) and the default assign entry (tensor cores + exact re-check)
 int launch_assign_exact(const Table& X, int metric, const Table& Cn, int k, const int32_t* row_sel_dev, int64_t n_sel,
@@ -249,6 +254,9 @@ int launch_one_scan(const Table& rows, int key_metric, int metric, const int64_t
                     float* dist, unsigned* ticket, int64_t* out_ids, float* out_f, double* out_d, int32_t* out_total,
                     int64_t* cand_sum, bool cand_store);
 constexpr int ONE_MAX_Q = 16;   // queries per call the fused path takes
+// vb_ivf_iter.cu: a query of an iterative scan whose group of lists is used up moves to its next non-empty group
+int launch_ivf_iter_advance(int64_t nq, int probes, int max_probes, const int32_t* probe_lists, const int64_t* list_off,
+                            int32_t* glists, int32_t* list_index, int32_t* returned, int32_t* seg_len, int32_t* active);
 int list_tile_rows();
 bool list_major_supported(int elem, int key_metric);
 int launch_list_major(const Table& rows, int key_metric, const void* qimg, size_t qstride, int64_t nq, const int32_t* d_lists,

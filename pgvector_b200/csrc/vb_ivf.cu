@@ -65,6 +65,7 @@ struct Ivf {
     int l1_cooldown = 0;              // batches left before level 1 is tried again after it failed
     int64_t last_tc_failed = 0, total_tc_failed = 0, total_l1_failed = 0;
     bool loaded = false;
+    uint64_t generation = 0;          // bumped whenever rows or lists change: an iterative scan handle refuses a changed image
     // streaming load (vb_ivf_begin_load / vb_ivf_load_list / vb_ivf_end_load)
     bool loading = false;
     int next_list = 0;
@@ -78,8 +79,10 @@ __global__ void __launch_bounds__(128) ivf_build_chunks_kernel(const int32_t* __
                                                                int64_t cap, int32_t* __restrict__ cand_off /*[nq][probes+1]*/,
                                                                int64_t* __restrict__ seg_begin, int32_t* __restrict__ seg_len,
                                                                Chunk* __restrict__ chunks, int* __restrict__ n_chunks,
-                                                               int64_t* __restrict__ cand_sum) {
+                                                               int64_t* __restrict__ cand_sum, const int32_t* __restrict__ active) {
     const int q = blockIdx.x;
+    // (an iterative scan rebuilds only the queries that moved to a new group; the others keep their runs)
+    if (active != nullptr && active[q] == 0) return;
     const int32_t* pl = probe_lists + (int64_t)q * probes;
     int32_t* co = cand_off + (int64_t)q * (probes + 1);
     __shared__ int s_base;
@@ -356,7 +359,7 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
                                   (c.scan_impl >= 3 || (c.scan_impl == 2 && nq * probes >= 256)));
     ivf_build_chunks_kernel<<<(unsigned)nq, per_query_scan ? 128 : 32, 0, c.stream>>>(d_lists, probes, ix.d_list_off, rpc, cap, cand_off, seg_begin,
                                                                                       seg_len, per_query_scan ? chunks : nullptr, n_chunks,
-                                                                                      ix.d_cand_sum);
+                                                                                      ix.d_cand_sum, nullptr);
     VB_CUDA(cudaGetLastError());
     count_launch();
     VB_TRY(workspace(WS_DIST, sizeof(float) * (size_t)nq * cap, &d_dist));
@@ -629,6 +632,109 @@ struct vb_ivf {
     Ivf ix;
 };
 
+// ivfflat.iterative_scan for a batch of queries (vb_ivf_iter.cu).  Everything kept between calls lives in `mem`, one
+// allocation the handle owns: the shared workspaces only carry data within a call.
+struct vb_ivf_scan {
+    Ivf* ix = nullptr;
+    uint64_t generation = 0;   // ix->generation at begin
+    int64_t nq = 0;
+    int probes = 0, max_probes = 0, page = 0, rpc = 0;
+    int64_t cap = 0, max_chunks = 0;
+    size_t qstride = 0;
+    void* mem = nullptr;
+    uint8_t* qimg = nullptr;       // [nq][qstride] query image
+    int32_t* probe = nullptr;      // [nq][max_probes] lists in probe order
+    int32_t* glists = nullptr;     // [nq][probes] lists of the current group (-1 padded)
+    int32_t* cand_off = nullptr;   // [nq][probes + 1]
+    int64_t* seg_begin = nullptr;  // [nq]
+    int32_t* seg_len = nullptr;    // [nq] candidates of the current group
+    int32_t* list_index = nullptr; // [nq] the reference's listIndex
+    uint64_t* floor_key = nullptr; // [nq] composite key of the last element returned
+    int32_t* returned = nullptr;   // [nq] elements of the current group returned so far
+    int32_t* active = nullptr;     // [nq] moved to a new group in this call
+    float* dist = nullptr;         // [nq][cap] candidate distances of the current group
+    Chunk* chunks = nullptr;       // [max_chunks]
+    int* n_chunks = nullptr;
+    int64_t* cand_sum = nullptr;
+    int32_t* pos = nullptr;        // [nq][page] selected positions
+    float* key = nullptr;          // [nq][page] their distances
+    int64_t* out_ids = nullptr;    // staging, copied back at once: ids [nq][page] | float8 [nq][page] | counts [nq]
+    double* out_d = nullptr;
+    int32_t* counts = nullptr;
+};
+
+namespace vb {
+
+// device bytes of a handle: per query (the rest is a few hundred bytes of alignment)
+static size_t ivf_scan_bytes_per_query(const vb_ivf_scan& s) {
+    return s.qstride + 4 * (size_t)s.max_probes + 4 * (size_t)s.probes + 4 * ((size_t)s.probes + 1) + 8 + 4 + 4 + 8 + 4 + 4 +
+           4 * (size_t)s.cap + sizeof(Chunk) * (size_t)(s.max_chunks / s.nq) + (4 + 4 + 8 + 8) * (size_t)s.page + 4;
+}
+
+// carve the handle's allocation (bytes == 0: only count them)
+static size_t ivf_scan_carve(vb_ivf_scan& s, uint8_t* base) {
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        uint8_t* p = base ? base + off : nullptr;
+        off += (bytes + 255) & ~(size_t)255;
+        return p;
+    };
+    const size_t nq = (size_t)s.nq;
+    s.qimg = take(nq * s.qstride);
+    s.probe = (int32_t*)take(4 * nq * s.max_probes);
+    s.glists = (int32_t*)take(4 * nq * s.probes);
+    s.cand_off = (int32_t*)take(4 * nq * (s.probes + 1));
+    // cursor state, seg_begin .. cand_sum, zeroed at begin: every query starts with an empty group and listIndex 0
+    s.seg_begin = (int64_t*)take(8 * nq);
+    s.floor_key = (uint64_t*)take(8 * nq);
+    s.seg_len = (int32_t*)take(4 * nq);
+    s.list_index = (int32_t*)take(4 * nq);
+    s.returned = (int32_t*)take(4 * nq);
+    s.active = (int32_t*)take(4 * nq);
+    s.n_chunks = (int*)take(8);
+    s.cand_sum = (int64_t*)take(8);
+    s.dist = (float*)take(4 * nq * (size_t)s.cap);
+    s.chunks = (Chunk*)take(sizeof(Chunk) * (size_t)s.max_chunks);
+    s.pos = (int32_t*)take(4 * nq * s.page);
+    s.key = (float*)take(4 * nq * s.page);
+    uint8_t* stage = take((8 + 8) * nq * s.page + 4 * nq);
+    s.out_ids = (int64_t*)stage;
+    s.out_d = stage ? (double*)(stage + 8 * nq * s.page) : nullptr;
+    s.counts = stage ? (int32_t*)(stage + 16 * nq * s.page) : nullptr;
+    return off;
+}
+
+// query image and probe order of every query: the GetScanLists of vb_ivf_scan_lists, in sub-batches
+static int ivf_scan_setup(vb_ivf_scan& s, const void* queries) {
+    Ivf& ix = *s.ix;
+    Context& c = ctx();
+    const size_t state_bytes = (size_t)((uint8_t*)s.dist - (uint8_t*)s.seg_begin);
+    VB_CUDA(cudaMemsetAsync(s.seg_begin, 0, state_bytes, c.stream));
+    const size_t rawq = raw_row_bytes(ix.elem, ix.dim);
+    const int64_t bq = std::min<int64_t>(s.nq, 65535);
+    for (int64_t q0 = 0; q0 < s.nq; q0 += bq) {
+        const int64_t m = std::min(bq, s.nq - q0);
+        void* qimg;
+        size_t qstride;
+        VB_TRY(upload_queries(ix.elem, ix.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, true, WS_QIMG, &qimg, &qstride));
+        VB_REQUIRE(qstride == s.qstride, "query image stride %zu, expected %zu", qstride, s.qstride);
+        uint8_t* mine = s.qimg + (size_t)q0 * s.qstride;
+        VB_CUDA(cudaMemcpyAsync(mine, qimg, (size_t)m * s.qstride, cudaMemcpyDeviceToDevice, c.stream));
+        int32_t* d_lists;
+        float* d_ldist;
+        if (c.one_query && m <= ONE_MAX_Q && one_probe_fits(ix.lists, s.qstride, s.max_probes))
+            VB_TRY(ivf_one_probes(ix, mine, s.qstride, m, s.max_probes, &d_lists, &d_ldist));
+        else
+            VB_TRY(ivf_select_probes(ix, mine, s.qstride, m, s.max_probes, &d_lists, &d_ldist));
+        VB_CUDA(cudaMemcpyAsync(s.probe + (size_t)q0 * s.max_probes, d_lists, sizeof(int32_t) * (size_t)m * s.max_probes,
+                                cudaMemcpyDeviceToDevice, c.stream));
+    }
+    VB_CUDA(cudaStreamSynchronize(c.stream));
+    return VB_OK;
+}
+
+}  // namespace vb
+
 extern "C" {
 
 // ----------------------------------------------------------------------------- operator
@@ -870,6 +976,7 @@ int vb_ivf_load(vb_ivf* h, const void* centers, const int64_t* list_offsets, con
     VB_TRY(require_init());
     VB_REQUIRE(h && centers && list_offsets, "null argument");
     Ivf& ix = h->ix;
+    ++ix.generation;
     table_free(ix.centers);
     table_free(ix.rows);
     VB_TRY(ivf_set_offsets(ix, list_offsets));
@@ -891,6 +998,7 @@ int vb_ivf_load_dev(vb_ivf* h, const void* centers_dev, const int64_t* list_offs
     VB_TRY(require_init());
     VB_REQUIRE(h && centers_dev && list_offsets_host, "null argument");
     Ivf& ix = h->ix;
+    ++ix.generation;
     table_free(ix.centers);
     table_free(ix.rows);
     VB_TRY(ivf_set_offsets(ix, list_offsets_host));
@@ -917,6 +1025,7 @@ int vb_ivf_begin_load(vb_ivf* h, const void* centers) {
     VB_TRY(require_init());
     VB_REQUIRE(h && centers, "null argument");
     Ivf& ix = h->ix;
+    ++ix.generation;
     table_free(ix.centers);
     table_free(ix.rows);
     VB_TRY(table_append_host(ix.centers, centers, ix.lists));
@@ -950,6 +1059,7 @@ int vb_ivf_end_load(vb_ivf* h) {
     Ivf& ix = h->ix;
     for (int l = ix.next_list; l <= ix.lists; ++l) ix.pending_off[(size_t)l] = ix.rows.n;
     ix.loading = false;
+    ++ix.generation;
     VB_TRY(ivf_set_offsets(ix, ix.pending_off.data()));
     if (ix.d_ids) cudaFree(ix.d_ids);
     ix.d_ids = nullptr;
@@ -972,6 +1082,7 @@ int vb_ivf_replace_list(vb_ivf* h, int list, const void* rows, const int64_t* id
     Ivf& ix = h->ix;
     VB_REQUIRE(list >= 0 && list < ix.lists && n >= 0 && (n == 0 || (rows && ids)), "bad list / rows");
     Context& c = ctx();
+    ++ix.generation;
     const int64_t lo = ix.h_list_off[(size_t)list], hi = ix.h_list_off[(size_t)list + 1];
     const int64_t total = ix.rows.n, tail = total - hi, new_total = lo + n + tail;
     Table T;
@@ -1445,6 +1556,111 @@ int vb_ivf_search_sharded(vb_ivf* h, const void* queries, int64_t nq, int probes
     VB_CUDA(cudaMemcpyAsync(hd.data(), d_dist, sizeof(float) * (size_t)nq * k, cudaMemcpyDeviceToHost, c.stream));
     VB_CUDA(cudaStreamSynchronize(c.stream));
     for (size_t i = 0; i < hd.size(); ++i) out_dist[i] = (double)hd[i];
+    return VB_OK;
+}
+
+// ---- ivfflat.iterative_scan for a batch of queries (vb_ivf_iter.cu)
+
+int vb_ivf_scan_begin(vb_ivf* h, const void* queries, int64_t nq, int probes, int max_probes, int page, vb_ivf_scan** out) {
+    VB_TRY(require_init());
+    VB_REQUIRE(out, "vb_ivf_scan_begin: null handle pointer");
+    *out = nullptr;
+    if (!h || !h->ix.loaded) {
+        set_error("vb_ivf_scan_begin: index not loaded");
+        return VB_ESTATE;
+    }
+    VB_REQUIRE(queries, "vb_ivf_scan_begin: queries must not be NULL (a NULL-query scan takes vb_ivf_scan_items)");
+    VB_REQUIRE(nq >= 1, "vb_ivf_scan_begin: nq must be >= 1 (got %lld)", (long long)nq);
+    VB_REQUIRE(probes >= 1 && max_probes >= 1, "vb_ivf_scan_begin: probes and max_probes must be >= 1 (got %d, %d)", probes, max_probes);
+    VB_REQUIRE(page >= 1 && page <= 2048, "vb_ivf_scan_begin: page must be in 1..2048 (got %d)", page);
+    Ivf& ix = h->ix;
+    vb_ivf_scan s;
+    s.ix = &ix;
+    s.generation = ix.generation;
+    s.nq = nq;
+    s.probes = std::min(probes, ix.lists);                                   // src/ivfscan.c:268-277
+    s.max_probes = std::min(std::max(max_probes, probes), ix.lists);
+    s.page = page;
+    s.cap = ivf_cap(ix, s.probes);
+    VB_REQUIRE(s.cap < (int64_t)INT32_MAX, "vb_ivf_scan_begin: %lld candidates per group", (long long)s.cap);
+    s.rpc = scan_chunk_rows(ix.rows);
+    s.max_chunks = nq * (s.cap / s.rpc + s.probes + 1);
+    VB_REQUIRE(s.max_chunks < (int64_t)INT32_MAX, "vb_ivf_scan_begin: too many scan chunks (%lld): open fewer queries per handle",
+               (long long)s.max_chunks);
+    s.qstride = ivf_qstride(ix);
+    const size_t bytes = ivf_scan_carve(s, nullptr);
+    size_t free_b = 0, total_b = 0;
+    VB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    if (bytes > free_b) {
+        set_error("vb_ivf_scan_begin: %lld queries need %zu bytes of device memory (%zu per query), %zu are free", (long long)nq, bytes,
+                  ivf_scan_bytes_per_query(s), free_b);
+        return VB_ENOMEM;
+    }
+    if (cudaMalloc(&s.mem, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("vb_ivf_scan_begin: allocation of %zu bytes failed (%zu per query)", bytes, ivf_scan_bytes_per_query(s));
+        return VB_ENOMEM;
+    }
+    ivf_scan_carve(s, (uint8_t*)s.mem);
+    const int rc = ivf_scan_setup(s, queries);
+    if (rc != VB_OK) {
+        cudaFree(s.mem);
+        return rc;
+    }
+    *out = new vb_ivf_scan(s);
+    return VB_OK;
+}
+
+int vb_ivf_scan_next(vb_ivf_scan* s, int64_t* out_ids, double* out_dist, int32_t* out_counts) {
+    VB_TRY(require_init());
+    VB_REQUIRE(s && out_ids && out_dist && out_counts, "vb_ivf_scan_next: null argument");
+    Ivf& ix = *s->ix;
+    if (!ix.loaded || ix.generation != s->generation) {
+        set_error("vb_ivf_scan_next: index changed since the scan began");
+        return VB_ESTATE;
+    }
+    Context& c = ctx();
+    const int64_t nq = s->nq;
+    VB_TRY(launch_ivf_iter_advance(nq, s->probes, s->max_probes, s->probe, ix.d_list_off, s->glists, s->list_index, s->returned,
+                                   s->seg_len, s->active));
+    VB_CUDA(cudaMemsetAsync(s->n_chunks, 0, sizeof(int), c.stream));
+    ivf_build_chunks_kernel<<<(unsigned)nq, 128, 0, c.stream>>>(s->glists, s->probes, ix.d_list_off, s->rpc, s->cap, s->cand_off, s->seg_begin,
+                                                                s->seg_len, s->chunks, s->n_chunks, s->cand_sum, s->active);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    VB_TRY(launch_scan_chunks(ix.rows, key_metric(ix.metric), s->qimg, s->qstride, s->chunks, s->n_chunks, (int)s->max_chunks, s->dist, true));
+    VB_TRY(launch_segment_topk_floor(s->dist, s->seg_begin, s->seg_len, nq, s->page, s->floor_key, s->returned, s->counts, s->pos, s->key));
+    const int64_t n = nq * s->page;
+    ivf_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(ix.metric, nq, s->page, s->probes, s->pos, s->key, s->glists,
+                                                                        s->cand_off, ix.d_list_off, ix.d_ids, s->out_ids, nullptr, s->out_d);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    void* pin;
+    const size_t bytes = 16 * (size_t)n + 4 * (size_t)nq;
+    VB_TRY(pinned_buffer2(bytes, &pin));
+    VB_CUDA(cudaMemcpyAsync(pin, s->out_ids, bytes, cudaMemcpyDeviceToHost, c.stream));
+    VB_CUDA(cudaStreamSynchronize(c.stream));
+    memcpy(out_ids, pin, 8 * (size_t)n);
+    memcpy(out_dist, (const uint8_t*)pin + 8 * (size_t)n, 8 * (size_t)n);
+    memcpy(out_counts, (const uint8_t*)pin + 16 * (size_t)n, 4 * (size_t)nq);
+    return VB_OK;
+}
+
+int vb_ivf_scan_lists_done(vb_ivf_scan* s, int32_t* out) {
+    VB_TRY(require_init());
+    VB_REQUIRE(s && out, "vb_ivf_scan_lists_done: null argument");
+    VB_CUDA(cudaMemcpyAsync(out, s->list_index, sizeof(int32_t) * (size_t)s->nq, cudaMemcpyDeviceToHost, ctx().stream));
+    VB_CUDA(cudaStreamSynchronize(ctx().stream));
+    return VB_OK;
+}
+
+int vb_ivf_scan_end(vb_ivf_scan* s) {
+    if (!s) return VB_OK;
+    if (s->mem) {
+        cudaStreamSynchronize(ctx().stream);
+        cudaFree(s->mem);
+    }
+    delete s;
     return VB_OK;
 }
 

@@ -246,7 +246,7 @@ int launch_scan_regular_f64(const Table& t, int metric, const void* q_dev, size_
 }
 
 int launch_scan_chunks(const Table& t, int metric, const void* q_dev, size_t qstride, const Chunk* chunks_dev,
-                       const int* n_chunks_dev, int max_chunks, float* out) {
+                       const int* n_chunks_dev, int max_chunks, float* out, bool ldg_only) {
     if (max_chunks <= 0) return VB_OK;
     ScanArgs a{};
     a.rows = t.d;
@@ -258,7 +258,7 @@ int launch_scan_chunks(const Table& t, int metric, const void* q_dev, size_t qst
     a.chunks = chunks_dev;
     a.n_chunks_dev = n_chunks_dev;
     a.out = out;
-    if (use_bulk_scan(t, t.n, qstride))
+    if (!ldg_only && use_bulk_scan(t, t.n, qstride))
         return launch_scan_bulk(t.elem, metric, a, false, max_chunks);
     int grid = std::min(max_chunks, scan_grid());
     return launch_scan_any<float>(t.elem, metric, a, grid, ctx().stream);
@@ -292,12 +292,15 @@ __device__ __forceinline__ uint64_t composite_key(float f, uint32_t pos) {
 
 // One CTA per segment.  Radix-select the k smallest composite keys (distance, position)
 // -- all keys are distinct, so there is no tie handling -- then bitonic-sort them in smem.
-__global__ void __launch_bounds__(TOPK_THREADS) segment_topk_kernel(const float* __restrict__ keys,
-                                                                    const int64_t* __restrict__ seg_begin,
-                                                                    const int32_t* __restrict__ seg_len, int k,
-                                                                    int kpow2, int32_t* __restrict__ out_pos,
-                                                                    float* __restrict__ out_key,
-                                                                    const int32_t* __restrict__ only_flagged) {
+// FLOOR (the paged selection of vb_ivf_iter.cu): only keys strictly above floor_key[seg] compete when returned[seg] > 0;
+// keys are unique, so those are exactly the ones not returned yet, and successive pages concatenate to the full sort.
+// Thread 0 then moves the floor to the last key selected, adds the page to returned[seg] and writes its size to count[seg].
+template <bool FLOOR>
+__device__ __forceinline__ void segment_topk_body(const float* __restrict__ keys, const int64_t* __restrict__ seg_begin,
+                                                  const int32_t* __restrict__ seg_len, int k, int kpow2, int32_t* __restrict__ out_pos,
+                                                  float* __restrict__ out_key, const int32_t* __restrict__ only_flagged,
+                                                  uint64_t* __restrict__ floor_key, int32_t* __restrict__ returned,
+                                                  int32_t* __restrict__ count) {
     extern __shared__ uint64_t sel[];  // kpow2 entries
     if (only_flagged != nullptr && only_flagged[blockIdx.x] == 0) return;   // (the slab selection's overflow path)
     __shared__ uint32_t hist[256];
@@ -308,9 +311,17 @@ __global__ void __launch_bounds__(TOPK_THREADS) segment_topk_kernel(const float*
     const float* kp = keys + seg_begin[seg];
     const uint32_t n = (uint32_t)seg_len[seg];
     const int tid = threadIdx.x;
+    uint32_t done = 0;   // keys returned by earlier pages (FLOOR)
+    uint64_t fl = 0;
+    if constexpr (FLOOR) {
+        done = (uint32_t)returned[seg];
+        fl = floor_key[seg];
+    }
+    const uint32_t rem = n - done;
+    auto above = [&](uint64_t key) { return !FLOOR || done == 0 || key > fl; };
 
     uint64_t thresh = ~0ull;  // select keys <= thresh
-    if (n > (uint32_t)k) {
+    if (rem > (uint32_t)k) {
         if (tid == 0) {
             s_prefix = 0;
             s_mask = 0;
@@ -332,7 +343,7 @@ __global__ void __launch_bounds__(TOPK_THREADS) segment_topk_kernel(const float*
                 bool in = false;
                 if (i < n) {
                     key = composite_key(kp[i], i);
-                    in = (key & mask) == prefix;
+                    in = (key & mask) == prefix && above(key);
                 }
                 const unsigned act = __ballot_sync(0xffffffffu, in);
                 if (in) {
@@ -368,7 +379,7 @@ __global__ void __launch_bounds__(TOPK_THREADS) segment_topk_kernel(const float*
     __syncthreads();
     for (uint32_t i = tid; i < n; i += TOPK_THREADS) {
         uint64_t key = composite_key(kp[i], i);
-        if (key <= thresh) {
+        if (key <= thresh && above(key)) {
             uint32_t slot = atomicAdd(&s_count, 1u);
             if (slot < (uint32_t)kpow2) sel[slot] = key;
         }
@@ -391,7 +402,7 @@ __global__ void __launch_bounds__(TOPK_THREADS) segment_topk_kernel(const float*
             __syncthreads();
         }
     }
-    const uint32_t m = min(n, (uint32_t)k);
+    const uint32_t m = min(rem, (uint32_t)k);
     for (int i = tid; i < k; i += TOPK_THREADS) {
         if ((uint32_t)i < m) {
             uint64_t key = sel[i];
@@ -402,6 +413,46 @@ __global__ void __launch_bounds__(TOPK_THREADS) segment_topk_kernel(const float*
             out_key[(int64_t)seg * k + i] = __int_as_float(0x7F800000);
         }
     }
+    if constexpr (FLOOR) {
+        if (tid == 0) {
+            if (m > 0) {
+                floor_key[seg] = sel[m - 1];
+                returned[seg] = (int32_t)(done + m);
+            }
+            count[seg] = (int32_t)m;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(TOPK_THREADS) segment_topk_kernel(const float* __restrict__ keys,
+                                                                    const int64_t* __restrict__ seg_begin,
+                                                                    const int32_t* __restrict__ seg_len, int k,
+                                                                    int kpow2, int32_t* __restrict__ out_pos,
+                                                                    float* __restrict__ out_key,
+                                                                    const int32_t* __restrict__ only_flagged) {
+    segment_topk_body<false>(keys, seg_begin, seg_len, k, kpow2, out_pos, out_key, only_flagged, nullptr, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(TOPK_THREADS) segment_topk_floor_kernel(const float* __restrict__ keys,
+                                                                          const int64_t* __restrict__ seg_begin,
+                                                                          const int32_t* __restrict__ seg_len, int k, int kpow2,
+                                                                          int32_t* __restrict__ out_pos, float* __restrict__ out_key,
+                                                                          uint64_t* __restrict__ floor_key,
+                                                                          int32_t* __restrict__ returned, int32_t* __restrict__ count) {
+    segment_topk_body<true>(keys, seg_begin, seg_len, k, kpow2, out_pos, out_key, nullptr, floor_key, returned, count);
+}
+
+int launch_segment_topk_floor(const float* keys, const int64_t* seg_begin_dev, const int32_t* seg_len_dev, int64_t nseg, int k,
+                              uint64_t* floor_key, int32_t* returned, int32_t* count, int32_t* out_pos, float* out_key) {
+    if (nseg == 0) return VB_OK;
+    VB_REQUIRE(k >= 1 && k <= TOPK_MAX_K, "paged selection: page %d outside 1..%d", k, TOPK_MAX_K);
+    int kpow2 = 2;
+    while (kpow2 < k) kpow2 <<= 1;
+    segment_topk_floor_kernel<<<(unsigned)nseg, TOPK_THREADS, (size_t)kpow2 * 8, ctx().stream>>>(keys, seg_begin_dev, seg_len_dev, k, kpow2,
+                                                                                                 out_pos, out_key, floor_key, returned, count);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
 }
 
 // ---- the k' nearest of a candidate run from the slab minima of the tensor-core filter -------------------------------------

@@ -7,6 +7,8 @@ does not cover: k-means assign on the tensor cores (config D shape, one GPU's sh
     python tools/bench_extra.py hnsw     [--elem halfvec|bit --rows N --dim D --ef EF]
     python tools/bench_extra.py exact    [--rows N --dim D]
     python tools/bench_extra.py rerank   [--rows N --dim D]     (bit HNSW candidates re-ranked on the fp32 rows)
+    python tools/bench_extra.py ivf-iter [--rows N --dim D --lists L --probes P --max-probes M --page K --queries Q]
+                                          (ivfflat.iterative_scan for filtered LIMIT 10 queries vs the per-scan loop)
 
 All timing with CUDA events on the library stream; inputs resident in HBM.
 """
@@ -256,21 +258,25 @@ def bench_rerank(args):
                                    "note": "bytes = valid candidates x row stride + candidate ids + queries"}}))
 
 
-def bench_ivf(args):
-    """IVFFlat scan throughput for halfvec / bit rows (bench.py covers vector)."""
+def build_ivf_index(args, seed=3):
+    """the index of bench_ivf: rows of a low intrinsic dimension generated on the device, k-means on 50 * lists samples,
+    rows grouped by list, loaded from device buffers (ids = row numbers)"""
     import torch
     import pgvector_b200 as pv
     pv.init(0)
     dev = torch.device("cuda", 0)
-    stream = torch.cuda.ExternalStream(pv.stream_handle(), device=dev)
-    g = torch.Generator(device=dev).manual_seed(3)
+    g = torch.Generator(device=dev).manual_seed(seed)
     frame = torch.linalg.qr(torch.randn((args.dim, 16), generator=g, device=dev))[0]
     x = torch.randn((args.rows, 16), generator=g, device=dev) @ frame.T + 0.02 * torch.randn((args.rows, args.dim), generator=g, device=dev)
     q = torch.randn((args.queries, 16), generator=g, device=dev) @ frame.T + 0.02 * torch.randn((args.queries, args.dim), generator=g, device=dev)
-    if args.elem == "halfvec":
+    if args.elem == "vector":
+        elem, opclass, kmetric, pmetric, rb = pv.VECTOR, "vector_l2_ops", pv.L2, pv.L2_SQUARED, args.dim * 4
+        rows_t, q_t = x.contiguous(), q.contiguous()
+        host = lambda t: t.cpu().numpy()
+    elif args.elem == "halfvec":
         elem, opclass, kmetric, pmetric, rb = pv.HALFVEC, "halfvec_l2_ops", pv.L2, pv.L2_SQUARED, args.dim * 2
         rows_t, q_t = x.half().contiguous(), q.half().contiguous()
-        rows_np = rows_t.cpu().numpy().view(np.uint16)
+        host = lambda t: t.cpu().numpy().view(np.uint16)
     else:
         elem, opclass, kmetric, pmetric, rb = pv.BIT, "bit_hamming_ops", pv.HAMMING, pv.HAMMING, args.dim // 8
         def pack(t):
@@ -278,13 +284,14 @@ def bench_ivf(args):
             w = torch.tensor([128, 64, 32, 16, 8, 4, 2, 1], dtype=torch.uint8, device=dev)
             return (b * w).sum(-1).to(torch.uint8).contiguous()
         rows_t, q_t = pack(x), pack(q)
-        rows_np = rows_t.cpu().numpy()
+        host = lambda t: t.cpu().numpy()
     del x
     torch.cuda.synchronize()
     ns = min(args.rows, 50 * args.lists)
-    ts = pv.Table(elem, args.dim).append(rows_np[:ns])
+    ts = pv.Table(elem, args.dim).append(host(rows_t[:ns]))
     init = pv.kmeans_pp_init(ts, kmetric, args.lists, seed=42)
     centers, iters = pv.kmeans(ts, kmetric, init, max_iter=100)
+    ts.free()
     ta = pv.Table(elem, args.dim).append(rows_t)
     assign = pv.assign(ta, pmetric, centers)
     ta.free()
@@ -294,9 +301,19 @@ def bench_ivf(args):
     offsets = np.zeros(args.lists + 1, dtype=np.int64)
     offsets[1:] = np.cumsum(counts.numpy())
     grouped = rows_t[order].contiguous()
+    del rows_t
     centers_t = torch.from_numpy(centers).to(dev)
     torch.cuda.synchronize()
     ix = pv.IvfflatIndex(opclass, args.dim, args.lists).load(centers_t, offsets, grouped, order.contiguous())
+    return dict(pv=pv, torch=torch, dev=dev, ix=ix, q_t=q_t, host=host, opclass=opclass, rb=rb, counts=counts, offsets=offsets,
+                iters=iters, keep=(centers_t, grouped, order))
+
+
+def bench_ivf(args):
+    """IVFFlat scan throughput for halfvec / bit rows (bench.py covers vector)."""
+    b = build_ivf_index(args)
+    pv, torch, dev, ix, q_t, opclass, rb, counts, iters = b["pv"], b["torch"], b["dev"], b["ix"], b["q_t"], b["opclass"], b["rb"], b["counts"], b["iters"]
+    stream = torch.cuda.ExternalStream(pv.stream_handle(), device=dev)
     k, B = 10, args.queries
     ids = torch.empty((B, k), dtype=torch.int64, device=dev)
     dist = torch.empty((B, k), dtype=torch.float32, device=dev)
@@ -313,6 +330,90 @@ def bench_ivf(args):
                       "queries_per_s": B / (ms / 1000.0), "ms_per_batch": ms, "candidates_per_query": cand / B,
                       "roofline": {"bound": "hbm", "kernel": "list scan", "achieved": gbs, "peak": hbm, "unit": "GB/s", "frac": gbs / hbm,
                                    "bytes_per_launch": cand * rb, "avg_launch_ms": scan_ms / scan_n, "share_of_step": scan_ms / scan_n / ms, "peak_source": src}}))
+
+
+def bench_ivf_iter(args):
+    """ivfflat.iterative_scan for a batch of filtered LIMIT 10 queries (WHERE id % 100 = 0): vb_ivf_scan_next pages until every
+    query has 10 matches or is exhausted, against the per-scan loop (vb_ivf_scan_lists + successive vb_ivf_scan_items) on a
+    sample of the queries, whose results must be equal."""
+    b = build_ivf_index(args)
+    pv, ix, q_t, opclass, rb, counts, offsets = b["pv"], b["ix"], b["q_t"], b["opclass"], b["rb"], b["counts"], b["offsets"]
+    q = b["host"](q_t)
+    nq, p, page, limit = args.queries, min(args.probes, args.lists), args.page, 10
+    P = min(max(args.max_probes, args.probes), args.lists)
+    keep = lambda ids: ids % 100 == 0
+    lens = np.diff(offsets)
+    order, _ = ix.scan_lists(q, P)                                   # the probe order the handle uses
+    cum = np.concatenate([np.zeros((nq, 1), np.int64), np.cumsum(lens[order], axis=1)], axis=1)
+
+    def run():
+        t0 = time.perf_counter()
+        scan = ix.iterative_scan(q, probes=p, max_probes=P, page=page)
+        begin_s = time.perf_counter() - t0
+        found = [[] for _ in range(nq)]
+        live = np.ones(nq, dtype=bool)
+        call_s, rows_read = [], []
+        done = np.zeros(nq, dtype=np.int64)
+        while live.any():
+            t0 = time.perf_counter()
+            ids, dist, cnt = scan.next_batch()
+            call_s.append(time.perf_counter() - t0)
+            now = scan.lists_done().astype(np.int64)
+            rows_read.append(int((cum[np.arange(nq), now] - cum[np.arange(nq), done]).sum()))
+            done = now
+            for i in np.nonzero(live)[0]:
+                c = int(cnt[i])
+                m = keep(ids[i, :c])
+                found[i].extend(zip(ids[i, :c][m].tolist(), dist[i, :c][m].tolist()))
+                if len(found[i]) >= limit or c == 0:
+                    found[i] = found[i][:limit]
+                    live[i] = False
+        scan.close()
+        return begin_s, call_s, rows_read, found, done
+
+    run()                                                            # warm-up: modules, workspaces, pinned staging
+    begin_s, call_s, rows_read, found, done = run()
+
+    def per_scan(i):                                                 # today's path for one query
+        out = []
+        for g0 in range(0, P, p):
+            ids, dist, n = ix.scan_items(q[i], order[i, g0:g0 + p])
+            m = keep(ids)
+            out.extend(zip(ids[m].tolist(), dist[m].tolist()))
+            if len(out) >= limit:
+                break
+        return out[:limit]
+
+    sample = list(range(0, nq, max(1, nq // args.sample)))[:args.sample]
+    per_scan(0)
+    t0 = time.perf_counter()
+    base = [per_scan(i) for i in sample]
+    base_s = time.perf_counter() - t0
+    pv.set_option("scan_impl", 0)                                    # the LDG scan everywhere: the arithmetic the handle uses
+    base0 = [per_scan(i) for i in sample]
+    pv.set_option("scan_impl", 2)
+    assert all(found[i] == w for i, w in zip(sample, base0)), "iterative scan != per-scan loop (scan_impl = 0)"
+    hbm, _, _, src = peaks()
+    total_s = begin_s + sum(call_s)
+    scan_bytes = [r * rb for r in rows_read]
+    rate = [by / s / 1e9 for by, s in zip(scan_bytes, call_s)]
+    print(json.dumps({"bench": "ivf-iter",
+                      "workload": f"IVFFlat {opclass} {args.rows}x{args.dim}, lists={args.lists}, probes={p}, max_probes={P}, page={page}, {nq} queries, "
+                                  f"WHERE id % 100 = 0 LIMIT {limit} (list sizes {int(counts.min())}/{int(counts.float().mean())}/{int(counts.max())})",
+                      "card": card(),
+                      "begin_ms": begin_s * 1e3, "next_calls": len(call_s),
+                      "ms_per_next": {"first": call_s[0] * 1e3, "resumed_mean": float(np.mean(call_s[1:]) * 1e3) if len(call_s) > 1 else None,
+                                      "resumed_max": float(np.max(call_s[1:]) * 1e3) if len(call_s) > 1 else None},
+                      "groups_per_query": float(np.mean(np.ceil(done / p))),
+                      "queries_done": {"with_10_matches": int(sum(len(f) >= limit for f in found)), "exhausted_first": int(sum(len(f) < limit for f in found))},
+                      "filtered_queries_per_s": nq / total_s,
+                      "roofline": {"bound": "hbm", "kernel": "whole vb_ivf_scan_next call (advance + chunks + LDG group scan + page select + finish + copy)",
+                                   "bytes_per_call": scan_bytes, "achieved_per_call": rate, "peak": hbm, "unit": "GB/s",
+                                   "frac_first_call": rate[0] / hbm, "peak_source": src,
+                                   "note": "bytes = rows of the groups scanned in the call x row bytes; later calls scan only queries that moved to a new group"},
+                      "per_scan_baseline": {"queries": len(sample), "filtered_queries_per_s": len(sample) / base_s,
+                                            "identical_to_handle_scan_impl0": True,
+                                            "identical_to_handle_default_options": all(found[i] == w for i, w in zip(sample, base))}}))
 
 
 def bench_kmeans(args):
@@ -428,7 +529,7 @@ def bench_sparse(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "kmeans", "sparse", "rerank"])
+    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "ivf-iter", "kmeans", "sparse", "rerank"])
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--lists", type=int, default=1000)
     ap.add_argument("--probes", type=int, default=10)
@@ -439,9 +540,14 @@ if __name__ == "__main__":
     ap.add_argument("--ef", type=int, default=None)
     ap.add_argument("--queries", type=int, default=None)
     ap.add_argument("--nnz", type=int, default=100)
+    ap.add_argument("--max-probes", type=int, default=100)
+    ap.add_argument("--page", type=int, default=100)
+    ap.add_argument("--sample", type=int, default=16)
     a = ap.parse_args()
     if a.what == "rerank":      # config E's query batch and ef_search
         a.queries, a.ef = a.queries or 2048, a.ef or 200
+    if a.what == "ivf-iter":
+        a.queries = a.queries or 2048
     a.queries, a.ef = a.queries or 4096, a.ef or 100
     if a.what == "sparse":
         a.rows = a.rows or 1_000_000
@@ -463,6 +569,11 @@ if __name__ == "__main__":
     elif a.what == "kmeans":
         a.dim = a.dim or 1536
         bench_kmeans(a)
+    elif a.what == "ivf-iter":
+        a.rows = a.rows or 1_000_000
+        a.dim = a.dim or 1536
+        a.elem = "vector" if a.elem == "halfvec" and "--elem" not in sys.argv else a.elem
+        bench_ivf_iter(a)
     elif a.what == "ivf":
         a.rows = a.rows or 1_000_000
         a.dim = a.dim or (1536 if a.elem == "halfvec" else 1024)
