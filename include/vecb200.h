@@ -177,6 +177,50 @@ int			vb_table_rerank(vb_table *t, int metric, const void *queries, int64_t nq, 
 int			vb_table_rerank_dev(vb_table *t, int metric, const void *queries_dev, int64_t nq, const int64_t *cand_dev, int c,
 								int k, int64_t *out_ids_dev, float *out_dist_dev);
 
+/* ------------------------------------------------------------- row filters */
+
+/*
+ * A row filter: the allowed rows of one table or one IVFFlat image, resident on the device -- what a B-tree or bitmap
+ * scan on a filter column yields for "WHERE <predicate> ORDER BY v <op> q LIMIT k" (README "Filtering").  Queries that
+ * take a filter never read, score, select or copy a row it does not allow.
+ *
+ * Table filters: rows = row numbers of t (append order).  Host variant: a value outside [0, n) fails with VB_EINVAL
+ * naming its position and value; _dev variant: such values are ignored.  Rows appended to t later are not in the
+ * filter; the filter stays valid (row numbers do not move).
+ * IVFFlat filters: ids = heap ids as given at load (row positions when the image was loaded with ids == NULL).  Ids the
+ * image does not hold are ignored (a TID set from a bitmap scan of the heap may name rows this index does not hold);
+ * every image row whose id is in the set is allowed, so an id the image holds on several rows allows them all.
+ * The filter records the image it was made for: after vb_ivf_load*, vb_ivf_end_load or vb_ivf_replace_list, any use of
+ * it fails with VB_ESTATE ("index changed since the filter was created").
+ * Duplicates collapse.  n == 0 is an empty filter.  Using a filter with a table or index other than its own fails with
+ * VB_EINVAL, also after its own was freed (every table and image carries a process-wide unique stamp).  The exact top-k
+ * takes filters of fewer than 2^31 rows.  Creation synchronises (it reads back the number of allowed rows); the caller's arrays may be reused at once.
+ */
+typedef struct vb_filter vb_filter;
+struct vb_ivf;	/* the IVFFlat image, below */
+int			vb_table_filter_create(vb_table *t, const int64_t *rows, int64_t n, vb_filter **out);
+int			vb_table_filter_create_dev(vb_table *t, const int64_t *rows_dev, int64_t n, vb_filter **out);
+int			vb_ivf_filter_create(struct vb_ivf *ix, const int64_t *ids, int64_t n, vb_filter **out);
+int			vb_ivf_filter_create_dev(struct vb_ivf *ix, const int64_t *ids_dev, int64_t n, vb_filter **out);
+int64_t		vb_filter_rows(const vb_filter *f);	/* rows allowed (0 for NULL) */
+int			vb_filter_free(vb_filter *f);
+
+/*
+ * Filtered exact top-k: for each query q, the k nearest of the rows filters[filter_of_query[q]] allows.
+ * filter_of_query is host memory in both variants ([nq], entries in [0, nfilters); NULL when nfilters == 1); an entry
+ * out of range fails with VB_EINVAL naming the query.  One call can batch queries with different predicates.
+ * Each query's result is bit-identical, ids and distances, to vb_table_rerank(t, metric, q, cand = its filter's allowed
+ * rows in ascending order, k): the same metrics, 1 <= k <= 2048, ties to the smaller row number, the same -1 padding
+ * when fewer than k rows are allowed.  A filter of every row therefore gives vb_exact_topk under scan_impl = 0.
+ * _dev variant: queries and outputs on the device, asynchronous on vb_stream().
+ */
+int			vb_exact_topk_filtered(vb_table *t, int metric, const void *queries, int64_t nq, int k,
+								   const vb_filter *const *filters, int nfilters, const int32_t *filter_of_query,
+								   int64_t *out_ids, double *out_dist);
+int			vb_exact_topk_filtered_dev(vb_table *t, int metric, const void *queries_dev, int64_t nq, int k,
+									   const vb_filter *const *filters, int nfilters, const int32_t *filter_of_query,
+									   int64_t *out_ids_dev, float *out_dist_dev);
+
 /* ---------------------------------------------------------------- sparsevec */
 
 /*
@@ -330,6 +374,20 @@ int			vb_ivf_search_prefetched(vb_ivf *ix, int slot, int probes, int k, int64_t 
 typedef struct vb_ivf_scan vb_ivf_scan;
 int			vb_ivf_scan_begin(vb_ivf *ix, const void *queries, int64_t nq, int probes, int max_probes, int page,
 							  vb_ivf_scan **out);
+/*
+ * The same scan with a row filter per query (see vb_filter above): query q uses filters[filter_of_query[q]] (host
+ * array; NULL when nfilters == 1; an entry out of range fails with VB_EINVAL naming the query).  Its sequence is the
+ * subsequence of S_q whose ids the filter allows: same order, same float8 distances bit for bit.  A page never spans
+ * two groups; a group with no allowed row is skipped like an empty one, so out_counts[q] == 0 still means exhausted.
+ * vb_ivf_scan_lists_done after a page is what the unfiltered handle reports when it returns those rows, and P at
+ * exhaustion.  Rows the filter rejects are never read, scored, selected or copied.  Begin copies what it needs from the
+ * filters into the handle's own allocation (the filters may be freed at once) and sizes the group buffers by the p
+ * largest allowed counts per list; VB_ENOMEM names the bytes the filters take too.  next, lists_done and end are the
+ * unfiltered handle's.
+ */
+int			vb_ivf_scan_begin_filtered(vb_ivf *ix, const void *queries, int64_t nq, int probes, int max_probes, int page,
+									   const vb_filter *const *filters, int nfilters, const int32_t *filter_of_query,
+									   vb_ivf_scan **out);
 int			vb_ivf_scan_next(vb_ivf_scan *scan, int64_t *out_ids, double *out_dist, int32_t *out_counts);
 int			vb_ivf_scan_lists_done(vb_ivf_scan *scan, int32_t *out);	/* [nq]: the reference's so->listIndex */
 int			vb_ivf_scan_end(vb_ivf_scan *scan);

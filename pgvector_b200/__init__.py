@@ -209,8 +209,17 @@ class Table:
         p = load().vb_table_device_rows(self.h, C.byref(stride))
         return int(p or 0), int(stride.value)
 
-    def exact_topk(self, metric, queries, k):
-        """ORDER BY v <op> q LIMIT k without an index (SURVEY 3.4)."""
+    def filter(self, rows):
+        """a row Filter of this table: the allowed row numbers (numpy array, or a torch CUDA int64 tensor whose values
+        outside [0, n) are ignored).  Rows appended later are not in it."""
+        return Filter._create(self, "vb_table_filter_create", rows)
+
+    def exact_topk(self, metric, queries, k, filter=None, filter_of_query=None):
+        """ORDER BY v <op> q LIMIT k without an index (SURVEY 3.4).  filter: a Filter of this table (WHERE row IN ...),
+        or a list of them with filter_of_query[q] = the index of query q's filter; each query then gets exactly what
+        rerank() returns for its filter's rows in ascending order (k <= 2048)."""
+        if filter is not None:
+            return self._exact_topk_filtered(metric, queries, int(k), filter, filter_of_query)
         if _is_torch(queries):
             import torch
             nq = queries.shape[0]
@@ -227,6 +236,31 @@ class Table:
         ids = np.empty((nq, k), dtype=np.int64)
         dist = np.empty((nq, k), dtype=np.float64)
         _lib.check(load().vb_exact_topk(self.h, metric, _ptr(queries), nq, k, _ptr(ids), _ptr(dist)))
+        return ids, dist
+
+    def _exact_topk_filtered(self, metric, queries, k, filter, filter_of_query):
+        farr, nf, fq = _filter_args(filter, filter_of_query)
+        if _is_torch(queries):
+            import torch
+            nq = queries.shape[0]
+            if fq is not None and len(fq) != nq:
+                raise ValueError(f"filter_of_query must have {nq} entries, got {len(fq)}")
+            queries = queries.contiguous()
+            ids = torch.empty((nq, k), dtype=torch.int64, device=queries.device)
+            dist = torch.empty((nq, k), dtype=torch.float32, device=queries.device)
+            _after_torch(queries)
+            _lib.check(load().vb_exact_topk_filtered_dev(self.h, metric, _ptr(queries), nq, k, farr, nf, _ptr(fq), _ptr(ids), _ptr(dist)))
+            synchronize()   # the library runs on its own stream; results are handed back complete
+            return ids, dist
+        queries = _host(self.elem, queries)
+        if queries.ndim == 1:
+            queries = queries.reshape(1, -1)
+        nq = queries.shape[0]
+        if fq is not None and len(fq) != nq:
+            raise ValueError(f"filter_of_query must have {nq} entries, got {len(fq)}")
+        ids = np.empty((nq, k), dtype=np.int64)
+        dist = np.empty((nq, k), dtype=np.float64)
+        _lib.check(load().vb_exact_topk_filtered(self.h, metric, _ptr(queries), nq, k, farr, nf, _ptr(fq), _ptr(ids), _ptr(dist)))
         return ids, dist
 
     def rerank(self, metric, queries, candidates, k):
@@ -404,13 +438,19 @@ class IvfflatIndex:
         _lib.check(load().vb_ivf_search(self.h, _ptr(q), nq, p, k, _ptr(ids), _ptr(dist)))
         return ids, dist
 
-    def iterative_scan(self, queries, probes=None, max_probes=None, page=100):
+    def filter(self, ids):
+        """a row Filter of this index: the allowed heap ids as given at load (numpy array, or a torch CUDA int64
+        tensor); ids the index does not hold are ignored.  It is refused once the index changes."""
+        return Filter._create(self, "vb_ivf_filter_create", ids)
+
+    def iterative_scan(self, queries, probes=None, max_probes=None, page=100, filter=None, filter_of_query=None):
         """ivfflat.iterative_scan = relaxed_order for a batch of queries: an IvfflatScan whose next_batch() returns the next
         page of every query's sequence (src/ivfscan.c:400-406).  probes / max_probes mirror ivfflat.probes /
         ivfflat.max_probes; max_probes defaults to probes (iterative_scan = off).  Cosine opclasses: pass
-        prepare_query(queries)."""
+        prepare_query(queries).  filter: a Filter of this index, or a list of them with filter_of_query[q] = the index
+        of query q's filter: each sequence is then the unfiltered one restricted to the ids its filter allows."""
         p = int(probes or self.probes)
-        return IvfflatScan(self, queries, p, int(max_probes or p), int(page))
+        return IvfflatScan(self, queries, p, int(max_probes or p), int(page), filter=filter, filter_of_query=filter_of_query)
 
     def search_into(self, queries_dev, k, probes, ids_dev, dist_dev):
         """asynchronous device-resident search into preallocated torch tensors (bench inner loop): enqueued on the
@@ -471,7 +511,7 @@ class IvfflatScan:
     the next <= page elements of every query, nearest first within a group of `probes` lists; counts == 0 marks an
     exhausted scan.  Close it (or use it as a context manager) before the index changes or is freed."""
 
-    def __init__(self, index, queries, probes, max_probes, page):
+    def __init__(self, index, queries, probes, max_probes, page, filter=None, filter_of_query=None):
         q = None if queries is None else _host(index.elem, queries)   # (NULL queries: the library refuses them)
         if q is not None and q.ndim == 1:
             q = q.reshape(1, -1)
@@ -479,7 +519,14 @@ class IvfflatScan:
         self.nq = 0 if q is None else q.shape[0]
         self.h = None
         h = C.c_void_p()
-        _lib.check(load().vb_ivf_scan_begin(index.h, _ptr(q), self.nq, probes, max_probes, page, C.byref(h)))
+        if filter is None:
+            _lib.check(load().vb_ivf_scan_begin(index.h, _ptr(q), self.nq, probes, max_probes, page, C.byref(h)))
+        else:
+            farr, nf, fq = _filter_args(filter, filter_of_query)
+            if fq is not None and len(fq) != self.nq:
+                raise ValueError(f"filter_of_query must have {self.nq} entries, got {len(fq)}")
+            _lib.check(load().vb_ivf_scan_begin_filtered(index.h, _ptr(q), self.nq, probes, max_probes, page, farr, nf, _ptr(fq),
+                                                         C.byref(h)))
         self.h = h
 
     def next_batch(self):
@@ -521,6 +568,64 @@ class IvfflatScan:
             self.close()
         except Exception:
             pass
+
+
+# --------------------------------------------------------------------- row filters
+
+class Filter:
+    """A row filter: the allowed rows of one Table (row numbers) or one IvfflatIndex (heap ids), resident on the device
+    -- what a B-tree or bitmap scan on a filter column yields for WHERE <predicate> ORDER BY v <op> q LIMIT k.  Made by
+    Table.filter / IvfflatIndex.filter; len() = rows allowed.  Free it (or use it as a context manager) when done."""
+
+    def __init__(self, owner, h):
+        self.owner, self.h = owner, h
+
+    @classmethod
+    def _create(cls, owner, fn, rows):
+        h = C.c_void_p()
+        if _is_torch(rows):
+            import torch
+            if not rows.is_cuda or rows.dtype != torch.int64 or rows.dim() != 1:
+                raise TypeError("filter: a tensor of rows must be a 1-d int64 CUDA tensor")
+            rows = rows.contiguous()
+            _after_torch(rows)
+            _lib.check(getattr(load(), fn + "_dev")(owner.h, _ptr(rows), rows.shape[0], C.byref(h)))
+        else:
+            rows = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
+            _lib.check(getattr(load(), fn)(owner.h, _ptr(rows), rows.shape[0], C.byref(h)))
+        return cls(owner, h)
+
+    def __len__(self):
+        return int(load().vb_filter_rows(self.h)) if self.h else 0
+
+    def free(self):
+        if self.h:
+            load().vb_filter_free(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.free()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def _filter_args(filter, filter_of_query):
+    """(C array of filter handles, count, int32 filter_of_query or None) for the filtered entry points"""
+    filters = [filter] if isinstance(filter, Filter) else list(filter)
+    if not filters or any(not isinstance(f, Filter) or not f.h for f in filters):
+        raise ValueError("filter: a Filter, or a non-empty list of live Filters")
+    if filter_of_query is None and len(filters) > 1:
+        raise ValueError("filter_of_query is required with more than one filter")
+    fq = None if filter_of_query is None else np.ascontiguousarray(filter_of_query, dtype=np.int32).reshape(-1)
+    arr = (C.c_void_p * len(filters))(*[f.h.value for f in filters])
+    return arr, len(filters), fq
 
 
 # --------------------------------------------------------------------- IVFFlat build

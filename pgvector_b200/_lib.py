@@ -54,6 +54,14 @@ SIGNATURES = {
     "vb_exact_topk_dev": (_i, [_vp, _i, _vp, _i64, _i, _vp, _vp]),
     "vb_table_rerank": (_i, [_vp, _i, _vp, _i64, _vp, _i, _i, _vp, _vp]),
     "vb_table_rerank_dev": (_i, [_vp, _i, _vp, _i64, _vp, _i, _i, _vp, _vp]),
+    "vb_table_filter_create": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
+    "vb_table_filter_create_dev": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
+    "vb_ivf_filter_create": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
+    "vb_ivf_filter_create_dev": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
+    "vb_filter_rows": (_i64, [_vp]),
+    "vb_filter_free": (_i, [_vp]),
+    "vb_exact_topk_filtered": (_i, [_vp, _i, _vp, _i64, _i, _vp, _i, _vp, _vp, _vp]),
+    "vb_exact_topk_filtered_dev": (_i, [_vp, _i, _vp, _i64, _i, _vp, _i, _vp, _vp, _vp]),
     "vb_ivf_create": (_i, [_i, _i, _i, _i, C.POINTER(_vp)]),
     "vb_ivf_load": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "vb_ivf_load_dev": (_i, [_vp, _vp, _vp, _vp, _vp]),
@@ -68,6 +76,7 @@ SIGNATURES = {
     "vb_ivf_search": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
     "vb_ivf_search_dev": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
     "vb_ivf_scan_begin": (_i, [_vp, _vp, _i64, _i, _i, _i, C.POINTER(_vp)]),
+    "vb_ivf_scan_begin_filtered": (_i, [_vp, _vp, _i64, _i, _i, _i, _vp, _i, _vp, C.POINTER(_vp)]),
     "vb_ivf_scan_next": (_i, [_vp, _vp, _vp, _vp]),
     "vb_ivf_scan_lists_done": (_i, [_vp, _vp]),
     "vb_ivf_scan_end": (_i, [_vp]),

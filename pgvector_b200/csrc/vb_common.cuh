@@ -6,6 +6,7 @@
 #include <stdint.h>
 #include <stddef.h>
 #include <string>
+#include <vector>
 
 #include "../../include/vecb200.h"
 
@@ -257,6 +258,36 @@ constexpr int ONE_MAX_Q = 16;   // queries per call the fused path takes
 // vb_ivf_iter.cu: a query of an iterative scan whose group of lists is used up moves to its next non-empty group
 int launch_ivf_iter_advance(int64_t nq, int probes, int max_probes, const int32_t* probe_lists, const int64_t* list_off,
                             int32_t* glists, int32_t* list_index, int32_t* returned, int32_t* seg_len, int32_t* active);
+// a filtered iterative scan: probe_lists[q][j] = l becomes the virtual list fq[q] * lists + l (-1 stays -1), so that the
+// advance, chunk and finish kernels read list l of the query's row filter from the handle's concatenated offset table
+int launch_ivf_filter_lists(int64_t nq, int max_probes, int lists, const int32_t* fq_dev, int32_t* probe_lists);
+
+// ---------------------------------------------------------------- row filters (vb_filter.cu)
+// The allowed rows of one table or one IVFFlat image, ascending.  An IVFFlat image stores rows grouped by list, so the
+// allowed rows of list l are one run pos[off[l] .. off[l + 1]).
+// process-wide unique stamp of a table or IVFFlat image: a filter matches its owner by address and stamp, so a filter
+// that outlived its owner is refused even when a new owner is allocated at the same address
+uint64_t next_owner_uid();
+struct Filter {
+    const void* owner = nullptr;   // the vb_table or vb_ivf it was made for
+    uint64_t owner_uid = 0;        // and that owner's stamp
+    bool ivf = false;
+    uint64_t generation = 0;       // IVFFlat: Ivf::generation at creation
+    int64_t n = 0;                 // rows allowed
+    int lists = 0;
+    void* mem = nullptr;           // one allocation: pos | ids | off
+    int64_t* pos = nullptr;        // [n] table: row numbers; IVFFlat: rows of the list-ordered image
+    int64_t* ids = nullptr;        // [n] IVFFlat: the heap ids of pos
+    int64_t* off = nullptr;        // [lists + 1] IVFFlat: per-list runs of pos
+    std::vector<int64_t> h_off;    // host copy of off (allowed counts per list: sizes a scan handle's group buffers)
+};
+// table: rows = row numbers (values outside [0, n_rows) ignored; the host variant validates before this call)
+int filter_build_table(int64_t n_rows, const int64_t* rows, int64_t n, bool host, Filter* f);
+// IVFFlat image of n_rows rows: image_ids = heap ids of the rows (nullptr: row positions), list_off [lists + 1] device
+int filter_build_ivf(int64_t n_rows, const int64_t* image_ids, const int64_t* list_off, int lists, const int64_t* ids, int64_t n,
+                     bool host, Filter* f);
+void filter_release(Filter* f);
+
 int list_tile_rows();
 bool list_major_supported(int elem, int key_metric);
 int launch_list_major(const Table& rows, int key_metric, const void* qimg, size_t qstride, int64_t nq, const int32_t* d_lists,
@@ -268,4 +299,8 @@ int launch_list_major(const Table& rows, int key_metric, const void* qimg, size_
 // opaque handle types of the C ABI
 struct vb_table {
     vb::Table t;
+    uint64_t uid = vb::next_owner_uid();
+};
+struct vb_filter {
+    vb::Filter f;
 };

@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <functional>
 #include <numeric>
 #include <vector>
 
@@ -630,6 +631,7 @@ using namespace vb;
 
 struct vb_ivf {
     Ivf ix;
+    uint64_t uid = next_owner_uid();   // matched by the row filters made for this image
 };
 
 // ivfflat.iterative_scan for a batch of queries (vb_ivf_iter.cu).  Everything kept between calls lives in `mem`, one
@@ -661,6 +663,13 @@ struct vb_ivf_scan {
     int64_t* out_ids = nullptr;    // staging, copied back at once: ids [nq][page] | float8 [nq][page] | counts [nq]
     double* out_d = nullptr;
     int32_t* counts = nullptr;
+    // row filters (vb_ivf_scan_begin_filtered), copied at begin: probe[] holds virtual lists f * lists + l, whose runs
+    // foff gives in fpos / fids; an unfiltered handle has nfilters = 0 and none of these
+    int nfilters = 0;
+    int64_t fallowed = 0;          // positions of all filters
+    int64_t* fpos = nullptr;       // [fallowed] rows of the list-ordered image, filter after filter
+    int64_t* fids = nullptr;       // [fallowed] their heap ids
+    int64_t* foff = nullptr;       // [nfilters * lists + 1]
 };
 
 namespace vb {
@@ -701,7 +710,17 @@ static size_t ivf_scan_carve(vb_ivf_scan& s, uint8_t* base) {
     s.out_ids = (int64_t*)stage;
     s.out_d = stage ? (double*)(stage + 8 * nq * s.page) : nullptr;
     s.counts = stage ? (int32_t*)(stage + 16 * nq * s.page) : nullptr;
+    if (s.nfilters) {
+        s.fpos = (int64_t*)take(8 * (size_t)std::max<int64_t>(s.fallowed, 1));
+        s.fids = (int64_t*)take(8 * (size_t)std::max<int64_t>(s.fallowed, 1));
+        s.foff = (int64_t*)take(8 * ((size_t)s.nfilters * s.ix->lists + 1));
+    }
     return off;
+}
+
+// device bytes the row filters' copies take in a handle
+static size_t ivf_scan_filter_bytes(const vb_ivf_scan& s) {
+    return s.nfilters ? 16 * (size_t)std::max<int64_t>(s.fallowed, 1) + 8 * ((size_t)s.nfilters * s.ix->lists + 1) : 0;
 }
 
 // query image and probe order of every query: the GetScanLists of vb_ivf_scan_lists, in sub-batches
@@ -1561,18 +1580,52 @@ int vb_ivf_search_sharded(vb_ivf* h, const void* queries, int64_t nq, int probes
 
 // ---- ivfflat.iterative_scan for a batch of queries (vb_ivf_iter.cu)
 
-int vb_ivf_scan_begin(vb_ivf* h, const void* queries, int64_t nq, int probes, int max_probes, int page, vb_ivf_scan** out) {
+}  // extern "C"
+
+namespace vb {
+
+// filtered handle: the filters' positions, heap ids and offset tables into the handle's allocation, and the probe
+// order renamed to the filters' virtual lists (launch_ivf_filter_lists)
+static int ivf_scan_copy_filters(vb_ivf_scan& s, const vb_filter* const* filters, const int32_t* filter_of_query) {
+    Ivf& ix = *s.ix;
+    Context& c = ctx();
+    const int lists = ix.lists;
+    std::vector<int64_t> foff((size_t)s.nfilters * lists + 1);
+    int64_t base = 0;
+    for (int i = 0; i < s.nfilters; ++i) {
+        const Filter& f = filters[i]->f;
+        for (int l = 0; l < lists; ++l) foff[(size_t)i * lists + l] = base + f.h_off[(size_t)l];
+        if (f.n) {
+            VB_CUDA(cudaMemcpyAsync(s.fpos + base, f.pos, 8 * (size_t)f.n, cudaMemcpyDeviceToDevice, c.stream));
+            VB_CUDA(cudaMemcpyAsync(s.fids + base, f.ids, 8 * (size_t)f.n, cudaMemcpyDeviceToDevice, c.stream));
+        }
+        base += f.n;
+    }
+    foff.back() = base;
+    VB_CUDA(cudaMemcpyAsync(s.foff, foff.data(), 8 * foff.size(), cudaMemcpyHostToDevice, c.stream));
+    if (filter_of_query && s.nfilters > 1) {
+        void* d_fq;
+        VB_TRY(workspace(WS_MISC, sizeof(int32_t) * (size_t)s.nq, &d_fq));
+        VB_CUDA(cudaMemcpyAsync(d_fq, filter_of_query, sizeof(int32_t) * (size_t)s.nq, cudaMemcpyHostToDevice, c.stream));
+        VB_TRY(launch_ivf_filter_lists(s.nq, s.max_probes, lists, (const int32_t*)d_fq, s.probe));
+    }
+    VB_CUDA(cudaStreamSynchronize(c.stream));   // foff is a stack-owned vector
+    return VB_OK;
+}
+
+static int ivf_scan_begin_impl(const char* fn, vb_ivf* h, const void* queries, int64_t nq, int probes, int max_probes, int page,
+                               const vb_filter* const* filters, int nfilters, const int32_t* filter_of_query, vb_ivf_scan** out) {
     VB_TRY(require_init());
-    VB_REQUIRE(out, "vb_ivf_scan_begin: null handle pointer");
+    VB_REQUIRE(out, "%s: null handle pointer", fn);
     *out = nullptr;
     if (!h || !h->ix.loaded) {
-        set_error("vb_ivf_scan_begin: index not loaded");
+        set_error("%s: index not loaded", fn);
         return VB_ESTATE;
     }
-    VB_REQUIRE(queries, "vb_ivf_scan_begin: queries must not be NULL (a NULL-query scan takes vb_ivf_scan_items)");
-    VB_REQUIRE(nq >= 1, "vb_ivf_scan_begin: nq must be >= 1 (got %lld)", (long long)nq);
-    VB_REQUIRE(probes >= 1 && max_probes >= 1, "vb_ivf_scan_begin: probes and max_probes must be >= 1 (got %d, %d)", probes, max_probes);
-    VB_REQUIRE(page >= 1 && page <= 2048, "vb_ivf_scan_begin: page must be in 1..2048 (got %d)", page);
+    VB_REQUIRE(queries, "%s: queries must not be NULL (a NULL-query scan takes vb_ivf_scan_items)", fn);
+    VB_REQUIRE(nq >= 1, "%s: nq must be >= 1 (got %lld)", fn, (long long)nq);
+    VB_REQUIRE(probes >= 1 && max_probes >= 1, "%s: probes and max_probes must be >= 1 (got %d, %d)", fn, probes, max_probes);
+    VB_REQUIRE(page >= 1 && page <= 2048, "%s: page must be in 1..2048 (got %d)", fn, page);
     Ivf& ix = h->ix;
     vb_ivf_scan s;
     s.ix = &ix;
@@ -1581,34 +1634,116 @@ int vb_ivf_scan_begin(vb_ivf* h, const void* queries, int64_t nq, int probes, in
     s.probes = std::min(probes, ix.lists);                                   // src/ivfscan.c:268-277
     s.max_probes = std::min(std::max(max_probes, probes), ix.lists);
     s.page = page;
-    s.cap = ivf_cap(ix, s.probes);
-    VB_REQUIRE(s.cap < (int64_t)INT32_MAX, "vb_ivf_scan_begin: %lld candidates per group", (long long)s.cap);
+    if (filters) {
+        VB_REQUIRE(nfilters >= 1 && (int64_t)nfilters * ix.lists < (int64_t)INT32_MAX, "%s: %d row filters", fn, nfilters);
+        VB_REQUIRE(filter_of_query || nfilters == 1, "%s: filter_of_query may only be NULL with one filter (got %d)", fn, nfilters);
+        for (int i = 0; i < nfilters; ++i) {
+            VB_REQUIRE(filters[i], "%s: filter %d is NULL", fn, i);
+            const Filter& f = filters[i]->f;
+            VB_REQUIRE(f.ivf && f.owner == h && f.owner_uid == h->uid, "%s: filter %d was made for another table or index", fn, i);
+            if (f.generation != ix.generation) {
+                set_error("%s: filter %d: index changed since the filter was created", fn, i);
+                return VB_ESTATE;
+            }
+        }
+        for (int64_t q = 0; q < nq && filter_of_query; ++q)
+            VB_REQUIRE(filter_of_query[q] >= 0 && filter_of_query[q] < nfilters, "%s: filter_of_query[%lld] = %d, not in 0..%d", fn,
+                       (long long)q, filter_of_query[q], nfilters - 1);
+        // a group holds at most the p largest allowed counts of one filter's lists
+        s.nfilters = nfilters;
+        s.cap = 1;
+        std::vector<int64_t> cnt((size_t)ix.lists);
+        for (int i = 0; i < nfilters; ++i) {
+            const Filter& f = filters[i]->f;
+            for (int l = 0; l < ix.lists; ++l) cnt[(size_t)l] = f.h_off[(size_t)l + 1] - f.h_off[(size_t)l];
+            std::partial_sort(cnt.begin(), cnt.begin() + s.probes, cnt.end(), std::greater<int64_t>());
+            s.cap = std::max(s.cap, std::accumulate(cnt.begin(), cnt.begin() + s.probes, (int64_t)0));
+            s.fallowed += f.n;
+        }
+    } else {
+        s.cap = ivf_cap(ix, s.probes);
+    }
+    VB_REQUIRE(s.cap < (int64_t)INT32_MAX, "%s: %lld candidates per group", fn, (long long)s.cap);
     s.rpc = scan_chunk_rows(ix.rows);
     s.max_chunks = nq * (s.cap / s.rpc + s.probes + 1);
-    VB_REQUIRE(s.max_chunks < (int64_t)INT32_MAX, "vb_ivf_scan_begin: too many scan chunks (%lld): open fewer queries per handle",
+    VB_REQUIRE(s.max_chunks < (int64_t)INT32_MAX, "%s: too many scan chunks (%lld): open fewer queries per handle", fn,
                (long long)s.max_chunks);
     s.qstride = ivf_qstride(ix);
     const size_t bytes = ivf_scan_carve(s, nullptr);
     size_t free_b = 0, total_b = 0;
     VB_CUDA(cudaMemGetInfo(&free_b, &total_b));
     if (bytes > free_b) {
-        set_error("vb_ivf_scan_begin: %lld queries need %zu bytes of device memory (%zu per query), %zu are free", (long long)nq, bytes,
-                  ivf_scan_bytes_per_query(s), free_b);
+        if (s.nfilters)
+            set_error("%s: %lld queries need %zu bytes of device memory (%zu per query, %zu for the row filters), %zu are free", fn,
+                      (long long)nq, bytes, ivf_scan_bytes_per_query(s), ivf_scan_filter_bytes(s), free_b);
+        else
+            set_error("%s: %lld queries need %zu bytes of device memory (%zu per query), %zu are free", fn, (long long)nq, bytes,
+                      ivf_scan_bytes_per_query(s), free_b);
         return VB_ENOMEM;
     }
     if (cudaMalloc(&s.mem, bytes) != cudaSuccess) {
         cudaGetLastError();
-        set_error("vb_ivf_scan_begin: allocation of %zu bytes failed (%zu per query)", bytes, ivf_scan_bytes_per_query(s));
+        set_error("%s: allocation of %zu bytes failed (%zu per query)", fn, bytes, ivf_scan_bytes_per_query(s));
         return VB_ENOMEM;
     }
     ivf_scan_carve(s, (uint8_t*)s.mem);
-    const int rc = ivf_scan_setup(s, queries);
+    int rc = ivf_scan_setup(s, queries);
+    if (rc == VB_OK && s.nfilters) rc = ivf_scan_copy_filters(s, filters, filter_of_query);
     if (rc != VB_OK) {
         cudaFree(s.mem);
         return rc;
     }
     *out = new vb_ivf_scan(s);
     return VB_OK;
+}
+
+}  // namespace vb
+
+extern "C" {
+
+int vb_ivf_scan_begin(vb_ivf* h, const void* queries, int64_t nq, int probes, int max_probes, int page, vb_ivf_scan** out) {
+    return ivf_scan_begin_impl("vb_ivf_scan_begin", h, queries, nq, probes, max_probes, page, nullptr, 0, nullptr, out);
+}
+
+int vb_ivf_scan_begin_filtered(vb_ivf* h, const void* queries, int64_t nq, int probes, int max_probes, int page,
+                               const vb_filter* const* filters, int nfilters, const int32_t* filter_of_query, vb_ivf_scan** out) {
+    if (!filters) {
+        set_error("vb_ivf_scan_begin_filtered: no row filter given");
+        if (out) *out = nullptr;
+        return VB_EINVAL;
+    }
+    return ivf_scan_begin_impl("vb_ivf_scan_begin_filtered", h, queries, nq, probes, max_probes, page, filters, nfilters, filter_of_query,
+                               out);
+}
+
+static int ivf_filter_create(vb_ivf* h, const int64_t* ids, int64_t n, bool host, vb_filter** out) {
+    VB_TRY(require_init());
+    VB_REQUIRE(out, "vb_ivf_filter_create: null filter pointer");
+    *out = nullptr;
+    if (!h || !h->ix.loaded) {
+        set_error("vb_ivf_filter_create: index not loaded");
+        return VB_ESTATE;
+    }
+    VB_REQUIRE(n >= 0 && (ids || n == 0), "vb_ivf_filter_create: null ids or negative count %lld", (long long)n);
+    Ivf& ix = h->ix;
+    vb_filter* f = new vb_filter;
+    f->f.owner = h;
+    f->f.owner_uid = h->uid;
+    f->f.generation = ix.generation;
+    const int rc = filter_build_ivf(ix.rows.n, ix.d_ids, ix.d_list_off, ix.lists, ids, n, host, &f->f);
+    if (rc != VB_OK) {
+        filter_release(&f->f);
+        delete f;
+        return rc;
+    }
+    *out = f;
+    return VB_OK;
+}
+
+int vb_ivf_filter_create(vb_ivf* h, const int64_t* ids, int64_t n, vb_filter** out) { return ivf_filter_create(h, ids, n, true, out); }
+
+int vb_ivf_filter_create_dev(vb_ivf* h, const int64_t* ids_dev, int64_t n, vb_filter** out) {
+    return ivf_filter_create(h, ids_dev, n, false, out);
 }
 
 int vb_ivf_scan_next(vb_ivf_scan* s, int64_t* out_ids, double* out_dist, int32_t* out_counts) {
@@ -1621,18 +1756,26 @@ int vb_ivf_scan_next(vb_ivf_scan* s, int64_t* out_ids, double* out_dist, int32_t
     }
     Context& c = ctx();
     const int64_t nq = s->nq;
-    VB_TRY(launch_ivf_iter_advance(nq, s->probes, s->max_probes, s->probe, ix.d_list_off, s->glists, s->list_index, s->returned,
+    // a filtered handle: the same kernels over the filters' runs (virtual lists), the allowed rows gathered by position
+    const int64_t* list_off = s->nfilters ? s->foff : ix.d_list_off;
+    const int64_t* ids = s->nfilters ? s->fids : ix.d_ids;
+    VB_TRY(launch_ivf_iter_advance(nq, s->probes, s->max_probes, s->probe, list_off, s->glists, s->list_index, s->returned,
                                    s->seg_len, s->active));
     VB_CUDA(cudaMemsetAsync(s->n_chunks, 0, sizeof(int), c.stream));
-    ivf_build_chunks_kernel<<<(unsigned)nq, 128, 0, c.stream>>>(s->glists, s->probes, ix.d_list_off, s->rpc, s->cap, s->cand_off, s->seg_begin,
+    ivf_build_chunks_kernel<<<(unsigned)nq, 128, 0, c.stream>>>(s->glists, s->probes, list_off, s->rpc, s->cap, s->cand_off, s->seg_begin,
                                                                 s->seg_len, s->chunks, s->n_chunks, s->cand_sum, s->active);
     VB_CUDA(cudaGetLastError());
     count_launch();
-    VB_TRY(launch_scan_chunks(ix.rows, key_metric(ix.metric), s->qimg, s->qstride, s->chunks, s->n_chunks, (int)s->max_chunks, s->dist, true));
+    if (s->nfilters)
+        VB_TRY(launch_scan_gather(ix.rows, key_metric(ix.metric), s->qimg, s->qstride, s->fpos, s->chunks, s->n_chunks, (int)s->max_chunks,
+                                  s->dist));
+    else
+        VB_TRY(launch_scan_chunks(ix.rows, key_metric(ix.metric), s->qimg, s->qstride, s->chunks, s->n_chunks, (int)s->max_chunks, s->dist,
+                                  true));
     VB_TRY(launch_segment_topk_floor(s->dist, s->seg_begin, s->seg_len, nq, s->page, s->floor_key, s->returned, s->counts, s->pos, s->key));
     const int64_t n = nq * s->page;
     ivf_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(ix.metric, nq, s->page, s->probes, s->pos, s->key, s->glists,
-                                                                        s->cand_off, ix.d_list_off, ix.d_ids, s->out_ids, nullptr, s->out_d);
+                                                                        s->cand_off, list_off, ids, s->out_ids, nullptr, s->out_d);
     VB_CUDA(cudaGetLastError());
     count_launch();
     void* pin;

@@ -73,4 +73,24 @@ int launch_ivf_iter_advance(int64_t nq, int probes, int max_probes, const int32_
     return VB_OK;
 }
 
+// A filtered handle (vb_ivf_scan_begin_filtered) keeps the offset tables of its row filters side by side: list l of
+// filter f is the run foff[f lists + l] .. foff[f lists + l + 1] of the concatenated allowed positions.  Renaming every
+// probed list to that virtual list is all the advance, chunk and finish kernels need: they read the filter's runs
+// through the list_off they already take, so they are the same kernels for both kinds of handle.
+__global__ void ivf_filter_lists_kernel(int64_t n, int max_probes, int lists, const int32_t* __restrict__ fq, int32_t* __restrict__ probe_lists) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int32_t l = probe_lists[i];
+    if (l >= 0) probe_lists[i] = fq[i / max_probes] * lists + l;
+}
+
+int launch_ivf_filter_lists(int64_t nq, int max_probes, int lists, const int32_t* fq_dev, int32_t* probe_lists) {
+    const int64_t n = nq * max_probes;
+    if (n <= 0) return VB_OK;
+    ivf_filter_lists_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx().stream>>>(n, max_probes, lists, fq_dev, probe_lists);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
+}
+
 }  // namespace vb

@@ -9,6 +9,8 @@ does not cover: k-means assign on the tensor cores (config D shape, one GPU's sh
     python tools/bench_extra.py rerank   [--rows N --dim D]     (bit HNSW candidates re-ranked on the fp32 rows)
     python tools/bench_extra.py ivf-iter [--rows N --dim D --lists L --probes P --max-probes M --page K --queries Q]
                                           (ivfflat.iterative_scan for filtered LIMIT 10 queries vs the per-scan loop)
+    python tools/bench_extra.py filter   [--rows N --dim D --lists L --probes P --max-probes M --page K --queries Q]
+                                          (row filters on the device: filtered iterative scan and exact top-k vs host filtering)
 
 All timing with CUDA events on the library stream; inputs resident in HBM.
 """
@@ -416,6 +418,144 @@ def bench_ivf_iter(args):
                                             "identical_to_handle_default_options": all(found[i] == w for i, w in zip(sample, base))}}))
 
 
+def bench_filter(args):
+    """Row filters on the device against filtering on the host, on bench_ivf's index (ids = row numbers):
+    - the filtered iterative scan (vb_ivf_scan_begin_filtered) of WHERE id % c = 0 LIMIT 10 against the unfiltered
+      handle whose pages the host filters (the ivf-iter workload), first 10 matches of every query asserted equal;
+    - the filtered exact top-k (vb_exact_topk_filtered_dev) over the same rows as a table against vb_table_rerank_dev
+      with the allowed rows expanded into a candidate matrix, results asserted equal;
+    - 64 per-query filters (id % 64) in one call against 64 single-filter calls, results asserted equal."""
+    b = build_ivf_index(args)
+    pv, torch, dev, ix, q_t, opclass, rb, counts, offsets = (b["pv"], b["torch"], b["dev"], b["ix"], b["q_t"], b["opclass"], b["rb"],
+                                                             b["counts"], b["offsets"])
+    grouped, order = b["keep"][1], b["keep"][2]
+    stream = torch.cuda.ExternalStream(pv.stream_handle(), device=dev)
+    q = b["host"](q_t)
+    nq, p, limit = args.queries, min(args.probes, args.lists), 10
+    P = min(max(args.max_probes, args.probes), args.lists)
+    img_ids = order.cpu().numpy()                                     # heap id (= row number) of every image row
+    list_of_row = np.repeat(np.arange(args.lists), np.diff(offsets))
+    probe_order, _ = ix.scan_lists(q, P)
+    hbm, _, _, src = peaks()
+
+    def drain(scan, keep):
+        """pages until every query has `limit` matches or is exhausted: (seconds per call, lists_done per call, matches)"""
+        found = [[] for _ in range(nq)]
+        live = np.ones(nq, dtype=bool)
+        call_s, done = [], [np.zeros(nq, dtype=np.int64)]
+        while live.any():
+            t0 = time.perf_counter()
+            ids, dist, cnt = scan.next_batch()
+            call_s.append(time.perf_counter() - t0)
+            done.append(scan.lists_done().astype(np.int64))
+            for i in np.nonzero(live)[0]:
+                c = int(cnt[i])
+                m = keep(ids[i, :c]) if keep else slice(None)
+                found[i].extend(zip(ids[i, :c][m].tolist(), dist[i, :c][m].tolist()))
+                if len(found[i]) >= limit or c == 0:
+                    found[i] = found[i][:limit]
+                    live[i] = False
+        return call_s, done, found
+
+    def rows_per_call(done, per_list):
+        cum = np.concatenate([np.zeros((nq, 1), np.int64), np.cumsum(per_list[probe_order], axis=1)], axis=1)
+        return [int((cum[np.arange(nq), b1] - cum[np.arange(nq), b0]).sum()) for b0, b1 in zip(done, done[1:])]
+
+    out = {"bench": "filter", "card": card(), "peak": {"hbm_gbs": hbm, "source": src},
+           "workload": f"IVFFlat {opclass} {args.rows}x{args.dim}, lists={args.lists}, probes={p}, max_probes={P}, {nq} queries, "
+                       f"WHERE id % c = 0 LIMIT {limit} (list sizes {int(counts.min())}/{int(counts.float().mean())}/{int(counts.max())})"}
+    for c in (100, 1000):
+        allowed_ids = np.arange(0, args.rows, c, dtype=np.int64)
+        allowed_per_list = np.bincount(list_of_row[img_ids % c == 0], minlength=args.lists)
+        keep = lambda ids, c=c: ids % c == 0
+        res = {}
+        for name, make in (("host_filtered", lambda: ix.iterative_scan(q, probes=p, max_probes=P, page=args.page)),
+                           ("device_filtered", lambda: ix.iterative_scan(q, probes=p, max_probes=P, page=limit, filter=f))):
+            for rep in range(2):                                      # the first run warms modules, workspaces and staging
+                t0 = time.perf_counter()
+                f = ix.filter(allowed_ids) if name == "device_filtered" else None   # (building the filter is counted)
+                scan = make()
+                begin_s = time.perf_counter() - t0
+                call_s, done, found = drain(scan, keep if name == "host_filtered" else None)
+                scan.close()
+                if f is not None:
+                    f.free()
+            per_list = np.diff(offsets) if name == "host_filtered" else allowed_per_list
+            rows = rows_per_call(done, per_list)
+            rate = [r * rb / s / 1e9 for r, s in zip(rows, call_s)]
+            res[name] = {"page": args.page if name == "host_filtered" else limit, "begin_ms": begin_s * 1e3, "next_calls": len(call_s),
+                         "ms_per_next": {"first": call_s[0] * 1e3, "mean": float(np.mean(call_s)) * 1e3},
+                         "groups_per_query": float(np.mean(np.ceil(done[-1] / p))),
+                         "filtered_queries_per_s": nq / (begin_s + sum(call_s)),
+                         "gathered_bytes_per_call": [r * rb for r in rows],
+                         "frac_of_peak_per_call": [x / hbm for x in rate], "found": found}
+        assert res["host_filtered"]["found"] == res["device_filtered"]["found"], f"id % {c}: device filter != host filter"
+        for r in res.values():
+            r.pop("found")
+        res["note"] = ("bytes = rows of the groups a call scanned (host_filtered: every row; device_filtered: the allowed rows) x row "
+                       "bytes, over the whole call's time (selection, finish and the copy back included)")
+        out[f"ivf_iterative_id_mod_{c}"] = res
+
+    # the same rows as a table, in image order: row r holds heap id img_ids[r]
+    table = pv.Table(pv.VECTOR if args.elem == "vector" else pv.HALFVEC if args.elem == "halfvec" else pv.BIT, args.dim).append(grouped)
+    metric = pv.L2 if args.elem != "bit" else pv.HAMMING
+    k = limit
+    ids_a = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    dist_a = torch.empty((nq, k), dtype=torch.float32, device=dev)
+    ids_b, dist_b = torch.empty_like(ids_a), torch.empty_like(dist_a)
+    stride = table.device_rows()[1]
+    lib = pv.load()
+
+    def filtered(fs, fq, qq=q_t, oi=ids_a, od=dist_a):
+        farr, nf, fqa = pv._filter_args(fs, fq)
+        pv._lib.check(lib.vb_exact_topk_filtered_dev(table.h, metric, pv._ptr(qq), qq.shape[0], k, farr, nf, pv._ptr(fqa), pv._ptr(oi),
+                                                     pv._ptr(od)))
+
+    for c in (100, 1000):
+        rows = np.nonzero(img_ids % c == 0)[0].astype(np.int64)
+        with table.filter(rows) as f:
+            cand = torch.from_numpy(rows).to(dev).expand(nq, -1).contiguous()
+
+            def rerank():
+                pv._lib.check(lib.vb_table_rerank_dev(table.h, metric, pv._ptr(q_t), nq, pv._ptr(cand), cand.shape[1], k, pv._ptr(ids_b),
+                                                      pv._ptr(dist_b)))
+
+            ms_f = timed(pv, torch, stream, lambda: filtered(f, None), warmup=2, steps=10)
+            ms_r = timed(pv, torch, stream, rerank, warmup=2, steps=10)
+            assert torch.equal(ids_a, ids_b) and torch.equal(dist_a, dist_b), f"id % {c}: filtered top-k != rerank"
+            by = nq * len(rows) * stride
+            out[f"exact_id_mod_{c}"] = {"allowed_rows": len(rows), "ms_per_batch": {"filtered": ms_f, "rerank_expanded": ms_r},
+                                        "candidate_bytes_uploaded_by_rerank": int(cand.numel() * 8), "gathered_bytes": by,
+                                        "frac_of_peak": {"filtered": by / (ms_f / 1e3) / 1e9 / hbm, "rerank_expanded": by / (ms_r / 1e3) / 1e9 / hbm},
+                                        "identical_results": True}
+            del cand
+
+    # 64 per-query filters in one call against one call per filter
+    nf = 64
+    fs = [table.filter(np.nonzero(img_ids % nf == i)[0]) for i in range(nf)]
+    fq = (np.arange(nq) % nf).astype(np.int32)
+    ms_one = timed(pv, torch, stream, lambda: filtered(fs, fq), warmup=2, steps=5)
+    sel = [torch.from_numpy(np.nonzero(fq == i)[0]).to(dev) for i in range(nf)]
+    qs = [q_t[s].contiguous() for s in sel]
+    outs = [(torch.empty((len(s), k), dtype=torch.int64, device=dev), torch.empty((len(s), k), dtype=torch.float32, device=dev)) for s in sel]
+
+    def per_filter():
+        for i in range(nf):
+            filtered(fs[i], None, qs[i], *outs[i])
+
+    ms_many = timed(pv, torch, stream, per_filter, warmup=2, steps=5)
+    for i in range(nf):
+        assert torch.equal(ids_a[sel[i]], outs[i][0]) and torch.equal(dist_a[sel[i]], outs[i][1]), f"filter {i}: one call != per-filter call"
+    by = sum(len(s) * len(fs[i]) for i, s in enumerate(sel)) * stride
+    out["exact_64_filters_id_mod_64"] = {"ms_per_batch": {"one_call": ms_one, "64_calls": ms_many}, "gathered_bytes": by,
+                                         "frac_of_peak": {"one_call": by / (ms_one / 1e3) / 1e9 / hbm, "64_calls": by / (ms_many / 1e3) / 1e9 / hbm},
+                                         "identical_results": True}
+    for f in fs:
+        f.free()
+    table.free()
+    print(json.dumps(out))
+
+
 def bench_kmeans(args):
     """k-means of config D on one GPU: 50 * lists samples x dim, lists centres (k-means++ seeding + Lloyd iterations)."""
     import torch
@@ -529,7 +669,7 @@ def bench_sparse(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "ivf-iter", "kmeans", "sparse", "rerank"])
+    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "ivf-iter", "filter", "kmeans", "sparse", "rerank"])
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--lists", type=int, default=1000)
     ap.add_argument("--probes", type=int, default=10)
@@ -546,7 +686,7 @@ if __name__ == "__main__":
     a = ap.parse_args()
     if a.what == "rerank":      # config E's query batch and ef_search
         a.queries, a.ef = a.queries or 2048, a.ef or 200
-    if a.what == "ivf-iter":
+    if a.what in ("ivf-iter", "filter"):
         a.queries = a.queries or 2048
     a.queries, a.ef = a.queries or 4096, a.ef or 100
     if a.what == "sparse":
@@ -569,11 +709,11 @@ if __name__ == "__main__":
     elif a.what == "kmeans":
         a.dim = a.dim or 1536
         bench_kmeans(a)
-    elif a.what == "ivf-iter":
+    elif a.what in ("ivf-iter", "filter"):
         a.rows = a.rows or 1_000_000
         a.dim = a.dim or 1536
         a.elem = "vector" if a.elem == "halfvec" and "--elem" not in sys.argv else a.elem
-        bench_ivf_iter(a)
+        (bench_ivf_iter if a.what == "ivf-iter" else bench_filter)(a)
     elif a.what == "ivf":
         a.rows = a.rows or 1_000_000
         a.dim = a.dim or (1536 if a.elem == "halfvec" else 1024)
