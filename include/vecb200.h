@@ -21,8 +21,9 @@
  *     library stream (vb_stream()); host-buffer variants synchronise before
  *     returning.  _dev variants return with their work enqueued, with two stated
  *     exceptions: the batched vb_ivf_search*_dev read ONE 8-byte pair of certificate
- *     counters per sub-batch of queries (the tensor-core filter re-runs an
- *     uncertified batch exactly before the results may be used), and
+ *     counters per sub-batch of queries, with up to 64 numbers of the queries filter
+ *     level 0 could not certify (the tensor-core filter re-runs uncertified queries
+ *     before the results may be used; a re-run synchronises again), and
  *     vb_hnsw_search_dev reads one overflow flag per call (visited-table growth).
  *   - rows are row-major and contiguous in the caller's buffers (vector: dim
  *     fp32; halfvec: dim IEEE binary16; bit: (dim+7)/8 bytes, MSB first, tail
@@ -400,6 +401,10 @@ int64_t		vb_ivf_tc_fallbacks(const vb_ivf *ix);
 /* Queries (cumulative) the first filter level (hi plane of the rows only, option "tc_level1") could not certify; their
  * batches were repeated with both planes.  After such a batch the level rests for 64 batches. */
 int64_t		vb_ivf_tc_level1_fallbacks(const vb_ivf *ix);
+/* Queries (cumulative) filter level 0 (int8 rows, option "tc_level0") could not certify.  Only those queries were
+ * searched again, from level 1 on; level 0 rests for 64 batches after one whose failed queries probe, in expectation,
+ * more than a quarter of the lists (1 - (1 - probes / lists)^failed > 1/4), where the re-run costs more than level 0 saved. */
+int64_t		vb_ivf_tc_level0_fallbacks(const vb_ivf *ix);
 
 /*
  * Traffic accounting of the tensor-core filter kernel (profiling, off by default): with on != 0 every launch also
@@ -511,7 +516,9 @@ int64_t		vb_last_assign_rechecked(void);
  * tensor-core distances, exact fp32 re-score of k' candidates, certificate, exact fallback) wherever it applies.
  * Every setting returns the same neighbours.  "tc_level1" (default 1): the tensor-core filter first reads only the
  * hi plane of the rows (half the HBM traffic, 2^-7 relative error bound) and repeats a batch with both planes when a
- * certificate fails.  "tensor_cores" as vb_set_tensor_cores.  "one_query" (default 1): calls with at most 16 queries --
+ * certificate fails.  "tc_level0" (default 1, effective where "tc_level1" is on): batched searches (vb_ivf_search*,
+ * not the sharded one) start one level lower, at int8 rows (a quarter of the bf16 planes' bytes, bound ~ max |x - x^| |q|,
+ * k' = 128); only the queries it cannot certify are searched again, from level 1 on.  "tensor_cores" as vb_set_tensor_cores.  "one_query" (default 1): calls with at most 16 queries --
  * one backend's scan: vb_ivf_scan_lists, vb_ivf_scan_items, vb_ivf_search -- run as two fused distance + select
  * kernels (the last CTA to finish selects; csrc/vb_ivf_one.cu) instead of the general launch sequence; 0 = general path.
  */

@@ -50,6 +50,7 @@ struct Context {
     int slab_select = 1;               // selection from the filter's slab minima (0: full radix selection of every run)
     uint64_t query_epoch = 0;          // bumped by every upload_queries(): caches keyed on a query image are valid for one batch only
     int tc_level1 = 1;                 // batched list scan: try the hi-plane-only filter first (vb_set_option "tc_level1")
+    int tc_level0 = 1;                 // ... and in front of it the int8 filter, where tc_level1 is on (vb_set_option "tc_level0")
     int pp_filter = 1;                 // k-means++ on large fp32 sample tables: triangle-inequality + bf16 filters in front of the exact distances
     unsigned long long pp_stats[3] = {0, 0, 0};   // last seeding: samples skipped by the triangle rule / stopped by the bf16 bound / re-scored exactly
     int fused_refine = 3;              // tensor-core filter, after the k' select: 3 = select + exact re-score + certificate with one CTA per query,
@@ -216,10 +217,18 @@ struct ListTcImage {
     int64_t n_tiles = 0;
     float xmax = 0.f;            // max |row|
     bool finite = true;          // false when a row norm is Inf / NaN (no error bound -> exact path only)
+    // level 0 (int8 rows), built on first use where it fits: [tile][128-dim block][128 rows x 128 B], same swizzle
+    uint8_t* planes8 = nullptr;
+    float* xs = nullptr;         // per-row scale s_x = max |x_i| / 127 (x ~ s_x * x8)
+    int n_kblocks8 = 0;
+    float rmax = 0.f;            // max over rows of |x - s_x x8|, rounded up
+    bool l0_tried = false;       // the int8 plane was built or found not to fit
 };
 bool list_tc_supported(int elem, int key_metric, int k);
 int list_tc_kp(int k, int level = 2);
 int list_tc_prepare(const Table& rows, ListTcImage* im);
+// the int8 plane, row scales and rmax of level 0 (rows must already be prepared)
+int list_tc_prepare_l0(const Table& rows, ListTcImage* im);
 void list_tc_release(ListTcImage* im);
 int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                    const int32_t* d_lists, int probes, const int32_t* cand_off, int64_t cap, const int64_t* d_list_off, int n_lists,
@@ -244,7 +253,7 @@ int launch_list_tc_select_refine(const Table& rows, const ListTcImage& im, int k
 int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                               int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
                               const float* dist, const float* smin, int64_t cap, int64_t cap_s, const int32_t* seg_len, const float* qn,
-                              int32_t* out_pos, float* out_key, int* fail_dev, int level = 2);
+                              int32_t* out_pos, float* out_key, int* fail_dev, int level = 2, int32_t* fail_list = nullptr);
 // vb_ivf_one.cu: the scan of one query (or a handful) as two fused distance + select kernels
 bool one_probe_fits(int lists, size_t qstride, int probes);
 bool one_scan_fits(int64_t cap, size_t qstride, int probes, int64_t k);

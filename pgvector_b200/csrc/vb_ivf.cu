@@ -64,7 +64,15 @@ struct Ivf {
     bool force_level2 = false;        // re-run of a batch whose level-1 (hi plane only) certificate failed
     int last_list_level = 0;          // filter level the last batched list scan ran at (0 = exact kernels)
     int l1_cooldown = 0;              // batches left before level 1 is tried again after it failed
-    int64_t last_tc_failed = 0, total_tc_failed = 0, total_l1_failed = 0;
+    int l0_cooldown = 0;              // the same for level 0 (after a batch where it failed often)
+    bool allow_level0 = false;        // set by the batched search, which runs level 0's uncertified queries again on their own
+    bool repairing = false;           // that re-run: it takes the batched filter chain whatever its size
+    bool last_level0 = false;         // the last batched list scan ran at level 0 (last_list_level 0 means the exact kernels)
+    int32_t* d_l0_fail = nullptr;     // the queries level 0 could not certify ([d_tc_fail[1]] of them)
+    int64_t l0_fail_cap = 0;
+    void* d_repair = nullptr;         // gathered queries and results of such a re-run (device queries / results)
+    size_t repair_bytes = 0;
+    int64_t last_tc_failed = 0, total_tc_failed = 0, total_l1_failed = 0, total_l0_failed = 0;
     bool loaded = false;
     uint64_t generation = 0;          // bumped whenever rows or lists change: an iterative scan handle refuses a changed image
     // streaming load (vb_ivf_begin_load / vb_ivf_load_list / vb_ivf_end_load)
@@ -333,6 +341,20 @@ static int ivf_ensure_tc_image(Ivf& ix) {
     return VB_OK;
 }
 
+// the int8 plane of level 0 (a quarter of the bf16 planes), built on first use where it fits with 4 GiB to spare
+static int ivf_ensure_l0_image(Ivf& ix) {
+    if (ix.tc.l0_tried) return VB_OK;
+    const size_t rows = (size_t)ix.tc.n_tiles * 128;
+    const size_t need = rows * ((size_t)(ix.rows.dim + 127) / 128) * 128 + rows * 4;
+    size_t free_b = 0, total_b = 0;
+    VB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    if (free_b < need + ((size_t)4 << 30)) {
+        ix.tc.l0_tried = true;
+        return VB_OK;
+    }
+    return list_tc_prepare_l0(ix.rows, &ix.tc);
+}
+
 // scan the given probe lists for a batch of queries and keep the k nearest per query
 static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, const int32_t* d_lists, int probes, int k,
                          int64_t* out_ids_dev, float* out_f_dev, double* out_d_dev, int32_t** cand_total_dev) {
@@ -371,27 +393,46 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
     // so each probed list is read once per batch instead of once per query; small k goes through the tensor-core
     // filter (HBM-bound), larger k through the fp32 list-major kernel (FMA-pipe bound).
     const int km = key_metric(ix.metric);
-    const bool batched = nq * probes >= 256;
+    const bool batched = nq * probes >= 256 || ix.repairing;
     bool tc = (c.scan_impl == 4 || c.scan_impl == 2) && !ix.force_exact && batched && list_tc_supported(ix.elem, km, k) && ix.rows.n > 0;
     if (tc) {
         VB_TRY(ivf_ensure_tc_image(ix));
         tc = ix.tc.finite;   // rows with Inf / NaN norms have no error bound: exact path
     }
     ix.last_list_level = 0;
+    ix.last_level0 = false;
     if (tc) {
         // level 1 reads only the hi plane of the rows (half the HBM traffic, error bound 2^-7 |x||q|): it certifies
         // whenever the neighbours are separated by more than that, otherwise the batch is repeated at level 2 (both
         // planes, 2^-12) and level 1 rests for a while
-        const int level = (c.tc_level1 && !ix.force_level2 && ix.l1_cooldown == 0 && list_tc_kp(k, 1) <= 128) ? 1 : 2;
+        int level = (c.tc_level1 && !ix.force_level2 && ix.l1_cooldown == 0 && list_tc_kp(k, 1) <= 128) ? 1 : 2;
         if (ix.l1_cooldown > 0 && !ix.force_level2) --ix.l1_cooldown;
-        ix.last_list_level = level;
-        const int kp = list_tc_kp(k, level);
-        const float* qn = nullptr;
         // slab minima for the selection (vb_common.cuh slab_base): with them the k' nearest are found from 32 k' candidates
         // per query instead of the whole run
         const int64_t cap_s = slab_cap(cap, probes);
-        const bool slabs = c.slab_select && c.fused_refine != 2 && kp <= 128 && nq * cap_s < (int64_t)INT32_MAX &&
-                           (size_t)cap_s * 4 + 20 * 1024 <= 160 * 1024;
+        const bool slabs_fit = c.slab_select && c.fused_refine != 2 && nq * cap_s < (int64_t)INT32_MAX &&
+                               (size_t)cap_s * 4 + 20 * 1024 <= 160 * 1024;
+        // level 0 in front of level 1: int8 rows (1 byte per element, bound ~R_max |q|, k' = 128).  Its uncertified queries
+        // are listed by the one-CTA-per-query refine and searched again on their own by the batched search
+        // (ivf_search_impl), the only caller that allows it.
+        if (level == 1 && c.tc_level0 && ix.allow_level0 && c.fused_refine == 3 && slabs_fit && list_tc_kp(k, 0) <= 128) {
+            if (ix.l0_cooldown > 0) {
+                --ix.l0_cooldown;
+            } else {
+                VB_TRY(ivf_ensure_l0_image(ix));
+                if (ix.tc.planes8) level = 0;
+            }
+        }
+        if (level == 0 && ix.l0_fail_cap < nq) {
+            if (ix.d_l0_fail) VB_CUDA(cudaFree(ix.d_l0_fail));
+            VB_CUDA(cudaMalloc(&ix.d_l0_fail, sizeof(int32_t) * (size_t)nq));
+            ix.l0_fail_cap = nq;
+        }
+        ix.last_list_level = level;
+        ix.last_level0 = level == 0;
+        const int kp = list_tc_kp(k, level);
+        const float* qn = nullptr;
+        const bool slabs = slabs_fit && kp <= 128;
         void* d_smin = nullptr;
         if (slabs) VB_TRY(workspace(WS_SMIN, sizeof(float) * (size_t)nq * cap_s, &d_smin));
         VB_TRY(launch_list_tc(ix.rows, ix.tc, km, qimg, qstride, nq, d_lists, probes, cand_off, cap, ix.d_list_off, ix.lists,
@@ -414,7 +455,7 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
             // counts as uncertified: the repeat of the batch takes the kernels below)
             VB_TRY(launch_list_tc_cta_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
                                              (const float*)d_dist, (const float*)d_smin, cap, cap_s, seg_len, qn, pos, key, ix.d_tc_fail + 1,
-                                             level));
+                                             level, level == 0 ? ix.d_l0_fail : nullptr));
             if (!ix.defer_tc_check) {
                 VB_CUDA(cudaMemcpyAsync(&n_failed, ix.d_tc_fail + 1, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
                 VB_CUDA(cudaStreamSynchronize(c.stream));
@@ -1156,6 +1197,8 @@ int vb_ivf_free(vb_ivf* h) {
     list_tc_release(&h->ix.ctc);
     if (h->ix.d_centre_off) cudaFree(h->ix.d_centre_off);
     if (h->ix.d_tc_fail) cudaFree(h->ix.d_tc_fail);
+    if (h->ix.d_l0_fail) cudaFree(h->ix.d_l0_fail);
+    if (h->ix.d_repair) cudaFree(h->ix.d_repair);
     if (h->ix.d_ticket) cudaFree(h->ix.d_ticket);
     for (int i = 0; i < 2; ++i) {
         if (h->ix.q_buf[i]) cudaFree(h->ix.q_buf[i]);
@@ -1288,9 +1331,91 @@ int vb_ivf_scan_items(vb_ivf* h, const void* q, const int32_t* lists, int nlists
     return VB_OK;
 }
 
-// host: results go to host memory (int64 ids + float8 distances); q_host: the queries are host memory
+__global__ void gather_queries_kernel(const uint8_t* __restrict__ src, size_t row_bytes, const int32_t* __restrict__ idx,
+                                      uint8_t* __restrict__ dst) {
+    const uint8_t* s = src + (size_t)idx[blockIdx.x] * row_bytes;
+    uint8_t* d = dst + (size_t)blockIdx.x * row_bytes;
+    for (size_t i = threadIdx.x; i < row_bytes; i += blockDim.x) d[i] = s[i];
+}
+__global__ void scatter_results_kernel(const int64_t* __restrict__ ids, const float* __restrict__ dist, const int32_t* __restrict__ idx,
+                                       int64_t n, int k, int64_t* __restrict__ out_ids, float* __restrict__ out_f) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= n * k) return;
+    const int64_t o = (int64_t)idx[i / k] * k + i % k;
+    out_ids[o] = ids[i];
+    out_f[o] = dist[i];
+}
+
 static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, bool host, bool q_host, int64_t* out_ids,
-                           float* out_f, double* out_d) {
+                           float* out_f, double* out_d, bool level0 = true);
+
+struct ResetFlag {   // clears a flag on every exit of a scope
+    bool& f;
+    ~ResetFlag() { f = false; }
+};
+
+// The queries `fail` (numbers within `queries`, nf of them) that level 0 could not certify are searched again on their own,
+// from level 1 on, and their rows of the outputs overwritten.  The re-run takes the batched filter chain whatever its size
+// (not the fused one-query kernels): a query certified at level 1 or 2 carries the filter's exact re-score, as it would in
+// a batch-wide repeat.  When the re-run needs the exact kernels, the caller computes the whole sub-batch there instead,
+// as it does without level 0 (the list-major kernel's sums may differ from the re-score's in the last bit).
+static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t>& fail, int probes, int k, bool host, bool q_host,
+                             int64_t* out_ids, float* out_f, double* out_d) {
+    Ivf& ix = h->ix;
+    Context& c = ctx();
+    std::sort(fail.begin(), fail.end());
+    const int64_t nf = (int64_t)fail.size();
+    const size_t rawq = raw_row_bytes(ix.elem, ix.dim);
+    const size_t q_bytes = (rawq * (size_t)nf + 15) & ~(size_t)15;
+    const size_t need = q_bytes + (sizeof(int64_t) + sizeof(float)) * (size_t)nf * k + sizeof(int64_t) + sizeof(int32_t) * (size_t)nf;
+    if (ix.repair_bytes < need) {
+        if (ix.d_repair) VB_CUDA(cudaFree(ix.d_repair));
+        VB_CUDA(cudaMalloc(&ix.d_repair, need));
+        ix.repair_bytes = need;
+    }
+    uint8_t* d_q = (uint8_t*)ix.d_repair;
+    int64_t* d_ids = (int64_t*)(d_q + q_bytes);
+    int64_t* d_cand_saved = d_ids + (size_t)nf * k;   // the caller's candidate count: the re-run's scans do not add to it
+    float* d_f = (float*)(d_cand_saved + 1);
+    int32_t* d_idx = (int32_t*)(d_f + (size_t)nf * k);
+    VB_CUDA(cudaMemcpyAsync(d_idx, fail.data(), sizeof(int32_t) * (size_t)nf, cudaMemcpyHostToDevice, c.stream));
+    std::vector<uint8_t> hq;
+    const void* sub = d_q;
+    if (q_host) {
+        hq.resize(rawq * (size_t)nf);
+        for (int64_t i = 0; i < nf; ++i) memcpy(hq.data() + (size_t)i * rawq, (const uint8_t*)queries + (size_t)fail[(size_t)i] * rawq, rawq);
+        sub = hq.data();
+    } else {
+        gather_queries_kernel<<<(unsigned)nf, 128, 0, c.stream>>>((const uint8_t*)queries, rawq, d_idx, d_q);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    VB_CUDA(cudaMemcpyAsync(d_cand_saved, ix.d_cand_sum, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
+    ResetFlag flag{ix.repairing};
+    ix.repairing = true;
+    if (host) {
+        std::vector<int64_t> ti((size_t)nf * k);
+        std::vector<double> td((size_t)nf * k);
+        VB_TRY(ivf_search_impl(h, sub, nf, probes, k, true, q_host, ti.data(), nullptr, td.data(), false));
+        VB_CUDA(cudaMemcpyAsync(ix.d_cand_sum, d_cand_saved, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
+        for (int64_t i = 0; i < nf; ++i) {
+            memcpy(out_ids + (size_t)fail[(size_t)i] * k, ti.data() + (size_t)i * k, sizeof(int64_t) * k);
+            memcpy(out_d + (size_t)fail[(size_t)i] * k, td.data() + (size_t)i * k, sizeof(double) * k);
+        }
+        return VB_OK;
+    }
+    VB_TRY(ivf_search_impl(h, sub, nf, probes, k, false, false, d_ids, d_f, nullptr, false));
+    VB_CUDA(cudaMemcpyAsync(ix.d_cand_sum, d_cand_saved, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
+    scatter_results_kernel<<<(unsigned)((nf * k + 255) / 256), 256, 0, c.stream>>>(d_ids, d_f, d_idx, nf, k, out_ids, out_f);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
+}
+
+// host: results go to host memory (int64 ids + float8 distances); q_host: the queries are host memory.  level0: the list
+// scan may start at filter level 0 (false for the re-run of the queries it could not certify)
+static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, bool host, bool q_host, int64_t* out_ids,
+                           float* out_f, double* out_d, bool level0) {
     VB_TRY(require_init());
     VB_REQUIRE(h && h->ix.loaded, "index not loaded");
     VB_REQUIRE(queries && probes >= 1 && k >= 1, "bad search arguments");
@@ -1299,7 +1424,7 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
     probes = std::min(probes, ix.lists);
     if (nq <= 0) return VB_OK;
     const size_t rawq = raw_row_bytes(ix.elem, ix.dim);
-    if (ivf_one_applies(ix, nq, probes, k, ivf_cap(ix, probes))) {
+    if (!ix.repairing && ivf_one_applies(ix, nq, probes, k, ivf_cap(ix, probes))) {
         // a handful of queries (one backend's scan): two fused launches, no memsets, one copy back
         const int64_t cap = ivf_cap(ix, probes);
         void* qimg;
@@ -1324,15 +1449,20 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
     }
     const int64_t bq = ivf_batch_limit(ix, probes);
     if (!ix.d_cand_sum) VB_CUDA(cudaMalloc(&ix.d_cand_sum, sizeof(int64_t)));
-    VB_CUDA(cudaMemsetAsync(ix.d_cand_sum, 0, sizeof(int64_t), c.stream));
+    if (level0) VB_CUDA(cudaMemsetAsync(ix.d_cand_sum, 0, sizeof(int64_t), c.stream));   // (a re-run adds to its caller's count)
     // One pass of a sub-batch.  The tensor-core filter runs optimistically: its certificate counters are read back
-    // together with the results (one synchronisation per sub-batch); a sub-batch with an uncertified query is run
-    // again on the exact kernels.
+    // together with the results (one synchronisation per sub-batch).  Queries level 0 could not certify are listed and
+    // searched again on their own; otherwise a sub-batch with an uncertified query is run again at level 2, then on the
+    // exact kernels.
+    constexpr int L0_LIST_READ = 64;   // failed queries read back with the counters (more take a second copy)
+    int32_t l0_list[L0_LIST_READ];
     auto run = [&](int64_t q0, int64_t m, int mode, int* fails) -> int {   // mode 0: automatic, 1: filter level 2, 2: exact
         const bool exact = mode == 2;
         ix.force_exact = exact;
         ix.force_level2 = mode == 1;
         ix.defer_tc_check = !exact;
+        ResetFlag reset{ix.allow_level0};
+        ix.allow_level0 = level0 && mode == 0;
         if (ix.d_tc_fail) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), c.stream));
         void* qimg;
         size_t qstride;
@@ -1354,6 +1484,9 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
         fails[0] = fails[1] = 0;
         const bool check = !exact && ix.d_tc_fail != nullptr;
         if (check) VB_CUDA(cudaMemcpyAsync(fails, ix.d_tc_fail, 2 * sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+        if (check && ix.last_level0)
+            VB_CUDA(cudaMemcpyAsync(l0_list, ix.d_l0_fail, sizeof(int32_t) * (size_t)std::min<int64_t>(m, L0_LIST_READ),
+                                    cudaMemcpyDeviceToHost, c.stream));
         if (host || check) VB_CUDA(cudaStreamSynchronize(c.stream));
         return VB_OK;
     };
@@ -1362,6 +1495,25 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
         const int64_t m = std::min(bq, nq - q0);
         int fails[2];
         rc = run(q0, m, 0, fails);
+        if (rc == VB_OK && fails[0] == 0 && fails[1] > 0 && ix.last_level0) {
+            // level 0 could not separate the neighbours of some queries: only those go on, from level 1.  Their re-run
+            // streams the lists they probe at level 1: with n failed queries, about 1 - (1 - probes / lists)^n of what a
+            // level-1 pass over the batch streams, while level 0 saved half of that pass.  Past a quarter (the re-run also
+            // selects probes and synchronises again) level 0 no longer pays, and it rests for the next 64 batches (the data
+            // decides this, not the batch).  At 1000 lists and probes 10 that is 29 failed queries.
+            ix.total_l0_failed += fails[1];
+            if (1.0 - std::pow(1.0 - (double)probes / ix.lists, (double)fails[1]) > 0.25) ix.l0_cooldown = 64;
+            std::vector<int32_t> fail(l0_list, l0_list + std::min(fails[1], L0_LIST_READ));
+            if (fails[1] > L0_LIST_READ) {
+                fail.resize((size_t)fails[1]);
+                VB_CUDA(cudaMemcpy(fail.data(), ix.d_l0_fail, sizeof(int32_t) * (size_t)fails[1], cudaMemcpyDeviceToHost));
+            }
+            const int64_t exact0 = ix.total_tc_failed;
+            rc = ivf_repair_level0(h, (const uint8_t*)queries + (size_t)q0 * rawq, fail, probes, k, host, q_host, out_ids + q0 * k,
+                                   out_f ? out_f + q0 * k : nullptr, out_d ? out_d + q0 * k : nullptr);
+            if (rc == VB_OK && ix.total_tc_failed > exact0) rc = run(q0, m, 2, fails);   // neither level 1 nor 2 certified them
+            continue;
+        }
         if (rc == VB_OK && fails[0] == 0 && fails[1] > 0 && ix.last_list_level == 1) {
             // the hi-plane filter could not separate the neighbours of some query: both planes, and leave level 1 alone
             // for the next batches (the data decides this, not the batch)
@@ -1814,6 +1966,7 @@ int vb_ivf_tc_traffic(int on, int64_t* out8) {
 
 int64_t vb_ivf_tc_fallbacks(const vb_ivf* h) { return h ? h->ix.total_tc_failed : 0; }
 int64_t vb_ivf_tc_level1_fallbacks(const vb_ivf* h) { return h ? h->ix.total_l1_failed : 0; }
+int64_t vb_ivf_tc_level0_fallbacks(const vb_ivf* h) { return h ? h->ix.total_l0_failed : 0; }
 
 int64_t vb_ivf_last_candidates(const vb_ivf* h) {
     if (!h || !h->ix.d_cand_sum) return 0;

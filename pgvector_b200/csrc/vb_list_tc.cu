@@ -36,6 +36,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <vector>
 
 namespace vb {
@@ -99,13 +100,16 @@ __device__ __forceinline__ bool lc_job(const LcArgs& a, int j, LcJob& jb) {
 // One (unit, query tile) for one consumer warpgroup: the MMAs of all K blocks, then the epilogue.  NQ = queries per
 // column group; the accumulator holds the 64 x 2 NQ product x . [q_hi ; q_lo] (NQ registers), whose column groups
 // [0, NQ) and [NQ, 2 NQ) are added -- register i + NQ / 2 holds column c + NQ of register i's column c.
-template <int NQ>
+// I8 (level 0): the operands are int8 planes, 128 dimensions per K block, and the int32 accumulator is exact; the
+// epilogue scales it by s_x (xs, per row) and t_q (tq, per query).
+template <int NQ, bool I8>
 __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_stages, uint32_t stage_bytes, uint32_t a_bytes,
                                         uint64_t* full_bar, uint64_t* empty_bar, float* slab_buf, uint32_t& it, const LcJob& jb,
-                                        int qt) {
+                                        int qt, const float* xs, const float* tq) {
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
     const int wg = warp / 4, t = threadIdx.x % 128;
     float acc[NQ];
+    int iacc[I8 ? NQ : 1];
     for (int kb = 0; kb < a.n_kblocks; ++kb, ++it) {
         const int s = it % n_stages;
         const uint32_t ph = (it / n_stages) & 1;
@@ -115,6 +119,15 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
         const uint64_t da_hi = make_sw128_desc(sa), da_lo = make_sw128_desc(sa + LC_A_PLANE);
         const uint64_t db = make_sw128_desc(sb);
         wgmma_fence();
+        if constexpr (I8) {
+            // x8 . [q_hi ; q_lo]: four k32 steps over the 128 int8 of the block
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint64_t adv = (uint64_t)((k * 32) >> 4);
+                if constexpr (NQ == 64) wgmma_s8_n128(iacc, da_hi + adv, db + adv, (kb | k) != 0);
+                else wgmma_s8_n64(iacc, da_hi + adv, db + adv, (kb | k) != 0);
+            }
+        } else {
 #pragma unroll
         for (int k = 0; k < TC_K / 16; ++k) {
             const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);
@@ -134,6 +147,7 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
             }
             if (!a.hi_only && k + 1 < TC_K / 16) wgmma_fence();   // the next K step returns to the wider shape
         }
+        }
         wgmma_commit();
         wgmma_wait<0>();
         __syncwarp();
@@ -148,12 +162,13 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
     const int frag_col = 2 * (t % 4);
     int64_t r_table[2];
     bool valid_row[2];
-    float xnr[2];
+    float xnr[2], xsr[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         r_table[h] = (int64_t)un.tile * LC_M + frag_row + 8 * h;
         valid_row[h] = r_table[h] >= lo && r_table[h] < hi;
         xnr[h] = valid_row[h] && a.is_l2 ? a.xn[r_table[h]] : 0.f;
+        xsr[h] = I8 && valid_row[h] ? xs[r_table[h]] : 0.f;
     }
     const int gb = a.grp_begin[un.list];
     // warps 2p and 2p + 1 hold the 32 rows of table-aligned slab p of the tile (if any of them belongs to the list)
@@ -168,17 +183,20 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
         for (int e = 0; e < 2; ++e) {
             const int col = qt * LC_N + 8 * cb + frag_col + e;
             int64_t po = 0;
-            float qn = 0.f;
+            float qn = 0.f, tqc = 0.f;
             if (col < cnt) {
                 po = a.pair_out[gb + col];
                 if (a.is_l2) qn = a.qn[a.pair_q[gb + col]];
+                if (I8) tqc = tq[a.pair_q[gb + col]];
             }
             float m = __int_as_float(0x7F800000);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int i = 4 * cb + 2 * h + e;
                 if (col < cnt && valid_row[h]) {
-                    const float dot = acc[i] + acc[i + NQ / 2];
+                    // level 0: x^.q^ = s_x t_q (x8.q_hi + x8.q_lo / 254), the roundings bounded in lc_make_bound
+                    const float dot = I8 ? xsr[h] * (tqc * fmaf((float)iacc[i + NQ / 2], 1.0f / 254.0f, (float)iacc[i]))
+                                         : acc[i] + acc[i + NQ / 2];
                     const float val = a.is_l2 ? fmaf(-2.f, dot, xnr[h] + qn) : -dot;
                     a.out[po + (r_table[h] - lo)] = val;
                     m = fminf(m, val);
@@ -211,14 +229,17 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
     }
 }
 
-__global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) {
+template <bool I8>
+__device__ __forceinline__ void list_tc_body(const LcArgs& a, const float* xs, const float* tq) {
     extern __shared__ uint8_t lc_smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(lc_smem_raw) + 1023) & ~(uintptr_t)1023);
     // stage ring: level 2 = 4 stages of (A hi+lo 32 KB | B 16 KB), level 1 = 7 stages of (A hi 16 KB | B 16 KB) --
     // the bytes in flight per SM are what keeps HBM busy
-    const int n_stages = a.hi_only ? LC_STAGES_L1 : LC_STAGES;
-    const uint32_t stage_bytes = a.hi_only ? LC_STAGE_L1 : LC_STAGE;
-    const uint32_t a_bytes = a.hi_only ? LC_A_PLANE : LC_A_STAGE;   // the hi plane leads each 32 KB block of the image
+    // level 0 = level 1's ring: 16 KB of int8 rows (128 dimensions) + the 16 KB [q_hi ; q_lo] int8 tile per stage
+    const int n_stages = I8 || a.hi_only ? LC_STAGES_L1 : LC_STAGES;
+    const uint32_t stage_bytes = I8 || a.hi_only ? LC_STAGE_L1 : LC_STAGE;
+    const uint32_t a_bytes = I8 || a.hi_only ? LC_A_PLANE : LC_A_STAGE;   // the hi plane leads each 32 KB block of the image
+    const uint32_t a_tile_block = I8 ? LC_A_PLANE : LC_A_STAGE;            // bytes per (tile, K block) of the image
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)n_stages * stage_bytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + LC_MAX_STAGES;
@@ -256,7 +277,7 @@ __global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) {
                     const uint8_t* gb = a.B + ((size_t)(gt0 + qt) * a.n_kblocks + kb) * LC_B_STAGE;
                     if (leader) {
                         mbar_arrive_expect_tx(&full_bar[s], a_bytes + (n32 ? LC_B_STAGE / 2 : LC_B_STAGE));
-                        bulk_g2s(sa, a.A + ((size_t)un.tile * a.n_kblocks + kb) * LC_A_STAGE, a_bytes, &full_bar[s]);
+                        bulk_g2s(sa, a.A + ((size_t)un.tile * a.n_kblocks + kb) * a_tile_block, a_bytes, &full_bar[s]);
                         if (n32) {   // [q_hi rows 0..31 | q_lo rows 0..31] back to back = one 64-row operand
                             bulk_g2s(sb, gb, LC_B_PLANE / 2, &full_bar[s]);
                             bulk_g2s(sb + LC_B_PLANE / 2, gb + LC_B_PLANE, LC_B_PLANE / 2, &full_bar[s]);
@@ -278,11 +299,17 @@ __global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) {
             LcJob jb;
             if (!lc_job(a, j, jb)) continue;
             for (int qt = jb.q_lo; qt < jb.q_hi; ++qt) {
-                if (jb.cnt - qt * LC_N <= 32) lc_tile<32>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt);
-                else lc_tile<64>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt);
+                if (jb.cnt - qt * LC_N <= 32) lc_tile<32, I8>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt, xs, tq);
+                else lc_tile<64, I8>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt, xs, tq);
             }
         }
     }
+}
+
+__global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) { list_tc_body<false>(a, nullptr, nullptr); }
+// level 0: a.A = the int8 plane, a.n_kblocks = its 128-dimension blocks, a.B = query tiles from pack_groups_i8_kernel
+__global__ void __launch_bounds__(LC_THREADS, 1) list_tc_l0_kernel(LcArgs a, const float* __restrict__ xs, const float* __restrict__ tq) {
+    list_tc_body<true>(a, xs, tq);
 }
 
 // gather + split the queries of every (query, list) pair into the B tiles of its list's group:
@@ -319,6 +346,140 @@ __global__ void pack_groups_kernel(const float* __restrict__ qimg, size_t qstrid
     const size_t off = (size_t)r * 128 + (size_t)((c ^ (r & 7)) * 16);
     *reinterpret_cast<uint4*>(base + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
     *reinterpret_cast<uint4*>(base + LC_B_PLANE + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+}
+
+
+// ---- level 0: int8 rows and queries ----------------------------------------------------------------------------------
+//
+// Rows: x ~ s_x x8 with s_x = max |x_i| / 127 and x8 = rint(x / s_x) (per-row absmax).  Queries: q ~ t_q (q_hi + q_lo / 254)
+// with t_q = max |q_i| / 127, q_hi = rint(q / t_q) and q_lo = rint((q - t_q q_hi) 254 / t_q), both in [-127, 127].  x8 . q_hi
+// and x8 . q_lo are ONE wgmma m64 n(2n) k32 s8 per K step, exact in int32 (|x8 . q| <= 127^2 dim < 2^31 for dim < 133000).
+
+// one query coordinate; the packing and the bound kernel call the same function, so the bound is computed from exactly
+// the values the tensor cores multiply
+__device__ __forceinline__ void l0_quant_q(float v, float tq, int& hi, int& lo) {
+    if (!(tq > 0.f && tq < 3.0e38f)) {
+        hi = lo = 0;
+        return;
+    }
+    const float h = fminf(fmaxf(rintf(__fdiv_rn(v, tq)), -127.f), 127.f);
+    const float r = fmaf(-tq, h, v);
+    const float l = fminf(fmaxf(rintf(__fdiv_rn(r * 254.f, tq)), -127.f), 127.f);
+    hi = (int)h;
+    lo = (int)l;
+}
+
+// rows -> int8 plane [tile][128-dim block][128 rows x 128 B] (128-byte swizzle: byte (r, kk) at r * 128 +
+// ((kk / 16) ^ (r & 7)) * 16 + kk % 16), s_x per row, and max |x - s_x x8| over the rows (rounded up, as float bits):
+// one warp per row of the tile-padded table
+template <int ELEM>
+__global__ void pack_rows_i8_kernel(const uint8_t* __restrict__ rows, size_t stride, int64_t n, int dim, int n_kblocks8, int64_t n_padded,
+                                    uint8_t* __restrict__ out, float* __restrict__ xs, unsigned* __restrict__ rmax_bits) {
+    const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32;
+    const int lane = threadIdx.x % 32;
+    if (r >= n_padded) return;
+    const uint8_t* src = rows + (size_t)std::min<int64_t>(r, n - 1) * stride;
+    auto ld = [&](int e) -> float {
+        if (r >= n || e >= dim) return 0.f;
+        return ELEM == VB_VECTOR ? reinterpret_cast<const float*>(src)[e] : __half2float(reinterpret_cast<const __half*>(src)[e]);
+    };
+    float amax = 0.f;
+    for (int e = lane; e < dim; e += 32) amax = fmaxf(amax, fabsf(ld(e)));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const float sx = amax / 127.f;
+    const int64_t tile = r / LC_M;
+    const int rr = (int)(r % LC_M);
+    double res = 0.0;
+    for (int ch = lane; ch < n_kblocks8 * 8; ch += 32) {
+        const int kb = ch / 8, c = ch % 8, e0 = kb * 128 + c * 16;
+        uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const float v = ld(e0 + j);
+            const float x8 = sx > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(v, sx)), -127.f), 127.f) : 0.f;
+            const double d = (double)v - (double)sx * (double)x8;
+            res += d * d;
+            w[j / 4] |= (uint32_t)(uint8_t)(int8_t)(int)x8 << (8 * (j % 4));
+        }
+        uint8_t* base = out + ((size_t)tile * n_kblocks8 + kb) * LC_A_PLANE;
+        *reinterpret_cast<uint4*>(base + (size_t)rr * 128 + (size_t)((c ^ (rr & 7)) * 16)) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) res += __shfl_xor_sync(0xffffffffu, res, o);
+    if (lane == 0) {
+        xs[r] = sx;
+        if (r < n) atomicMax(rmax_bits, __float_as_uint(__double2float_ru(sqrt(res) * (1.0 + 1.0 / 1048576.0))));
+    }
+}
+
+// per query of the batch (one warp each): t_q, the packed query q8 = [q_hi | q_lo] (qpad int8 each, zero past qdim: quantised
+// once here, copied into the tiles of every probed list by pack_groups_i8_kernel), and the level-0 bound eps(q) >= |d~ - d_fp32|
+// over every row (lc_make_bound derives it), handed to the refine kernels squared, in the place of |q|^2 (qe2)
+__global__ void l0_query_kernel(const float* __restrict__ qimg, size_t qstride, int qdim, int qpad, int64_t nq, float xmax, float rmax,
+                                int is_l2, float c_sum, float* __restrict__ tq_out, float* __restrict__ qe2_out, int8_t* __restrict__ q8) {
+    const int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32;
+    const int lane = threadIdx.x % 32;
+    if (q >= nq) return;
+    const float* src = reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(qimg) + (size_t)q * qstride);
+    float amax = 0.f;
+    for (int e = lane; e < qdim; e += 32) amax = fmaxf(amax, fabsf(src[e]));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const float tq = amax / 127.f;
+    double n2 = 0.0, r2 = 0.0, h2 = 0.0, l2 = 0.0;
+    int8_t* qh = q8 + (size_t)q * 2 * qpad;
+    for (int e = qdim + lane; e < qpad; e += 32) qh[e] = qh[qpad + e] = 0;
+    for (int e = lane; e < qdim; e += 32) {
+        const float v = src[e];
+        int hi, lo;
+        l0_quant_q(v, tq, hi, lo);
+        qh[e] = (int8_t)hi;
+        qh[qpad + e] = (int8_t)lo;
+        const double d = (double)v - (double)tq * ((double)hi + (double)lo / 254.0);
+        n2 += (double)v * v;
+        r2 += d * d;
+        h2 += (double)hi * hi;
+        l2 += (double)lo * lo;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        n2 += __shfl_xor_sync(0xffffffffu, n2, o);
+        r2 += __shfl_xor_sync(0xffffffffu, r2, o);
+        h2 += __shfl_xor_sync(0xffffffffu, h2, o);
+        l2 += __shfl_xor_sync(0xffffffffu, l2, o);
+    }
+    if (lane == 0) {
+        const double X = (double)xmax * (1.0 + 1.0 / 1024.0) + (double)rmax;   // >= |x^| = |s_x x8| of every row
+        const double qnorm = sqrt(n2), rq = sqrt(r2), qabs = (double)tq * (sqrt(h2) + sqrt(l2) / 254.0);
+        const double dot = (double)rmax * qnorm + X * rq + X * qabs / 1048576.0 + 1e-30;
+        double eps = is_l2 ? 2.0 * dot + (double)c_sum * (X * X + n2) : dot + X * qnorm / 131072.0;
+        eps *= 1.0 + 1.0 / 1024.0;
+        tq_out[q] = tq;
+        qe2_out[q] = __double2float_ru(eps * eps);   // NaN / Inf (a query without finite norm): the certificate fails
+    }
+}
+
+// pack_groups_kernel for level 0: thread = one 16-byte chunk (16 dimensions) of one pair, copied from l0_query_kernel's q8
+__global__ void pack_groups_i8_kernel(const int8_t* __restrict__ q8, int qpad, int n_kblocks8, int64_t n_pairs,
+                                      const int32_t* __restrict__ pair_q, const int32_t* __restrict__ pair_list,
+                                      const int32_t* __restrict__ grp_begin, const int32_t* __restrict__ gt_begin,
+                                      uint8_t* __restrict__ out) {
+    const int64_t chunk = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int chunks_per_row = n_kblocks8 * 8;
+    const int64_t slot = chunk / chunks_per_row;
+    if (slot >= n_pairs) return;
+    const int cr = (int)(chunk % chunks_per_row);
+    const int kb = cr / 8, c = cr % 8;
+    const int l = pair_list[slot];
+    const int j = (int)(slot - grp_begin[l]);
+    const int64_t gtile = gt_begin[l] + j / LC_N;
+    const int r = j % LC_N;
+    const int8_t* src = q8 + (size_t)pair_q[slot] * 2 * qpad + kb * 128 + c * 16;
+    uint8_t* base = out + ((size_t)(gtile * n_kblocks8 + kb) * 2) * LC_B_PLANE;
+    const size_t off = (size_t)r * 128 + (size_t)((c ^ (r & 7)) * 16);
+    *reinterpret_cast<uint4*>(base + off) = *reinterpret_cast<const uint4*>(src);
+    *reinterpret_cast<uint4*>(base + LC_B_PLANE + off) = *reinterpret_cast<const uint4*>(src + qpad);
 }
 
 // |d~ - d_fp32| <= eps(q) for every candidate of query q
@@ -667,15 +828,15 @@ __global__ void __launch_bounds__(SR_WARPS * 32) select_refine_kernel(const uint
 // time on a single warp), ranked and certified.  Same arithmetic, same tie rule, same outputs as select_refine_kernel;
 // a query whose selection overflows its buffer (ties by the thousand) counts as uncertified and the batch is repeated
 // on the kernels above.
-template <int ELEM, int METRIC>
-__global__ void __launch_bounds__(SS_THREADS) cta_refine_kernel(const uint8_t* __restrict__ rows, size_t stride, int V,
+template <int ELEM, int METRIC, bool LIST>
+__device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows, size_t stride, int V,
                                                                 const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
                                                                 LcBound bound, const float* __restrict__ qn, const float* __restrict__ dist,
                                                                 const float* __restrict__ smin, int64_t cap, int64_t cap_s,
                                                                 const int32_t* __restrict__ seg_len, const int32_t* __restrict__ probe_lists,
                                                                 const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
                                                                 int32_t* __restrict__ out_pos, float* __restrict__ out_key,
-                                                                int* __restrict__ n_failed) {
+                                                                int* __restrict__ n_failed, int32_t* __restrict__ fail_list) {
     extern __shared__ uint64_t cr_smem[];
     uint64_t* cand = cr_smem;                                                   // [SS_CAND]
     uint64_t* fin = cand + SS_CAND;                                             // [kp] final keys
@@ -694,7 +855,10 @@ __global__ void __launch_bounds__(SS_THREADS) cta_refine_kernel(const uint8_t* _
     else n = direct_select_cta(dist + (int64_t)q * cap, n_run, kp, cand, work);
     if (n < 0) {
         // not selected here: the query reports as uncertified (outputs are rewritten by the repeat of the batch)
-        if (tid == 0) atomicAdd(n_failed, 1);
+        if (tid == 0) {
+            const int i = atomicAdd(n_failed, 1);
+            if (LIST) fail_list[i] = q;
+        }
         for (int i = tid; i < k; i += SS_THREADS) {
             out_pos[(int64_t)q * k + i] = -1;
             out_key[(int64_t)q * k + i] = __int_as_float(0x7F800000);
@@ -769,8 +933,35 @@ __global__ void __launch_bounds__(SS_THREADS) cta_refine_kernel(const uint8_t* _
     // ---- certificate: candidates beyond the k' exist -> the last of the k' must already be above the threshold
     if (tid == 0 && n_run > kp) {
         const bool ok = key_to_float((uint32_t)(thr >> 32)) > T;     // false for NaN
-        if (!ok) atomicAdd(n_failed, 1);
+        if (!ok) {
+            const int i = atomicAdd(n_failed, 1);
+            if (LIST) fail_list[i] = q;
+        }
     }
+}
+
+template <int ELEM, int METRIC>
+__global__ void __launch_bounds__(SS_THREADS) cta_refine_kernel(const uint8_t* __restrict__ rows, size_t stride, int V,
+                                                                const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
+                                                                LcBound bound, const float* __restrict__ qn, const float* __restrict__ dist,
+                                                                const float* __restrict__ smin, int64_t cap, int64_t cap_s,
+                                                                const int32_t* __restrict__ seg_len, const int32_t* __restrict__ probe_lists,
+                                                                const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
+                                                                int32_t* __restrict__ out_pos, float* __restrict__ out_key,
+                                                                int* __restrict__ n_failed) {
+    cta_refine_body<ELEM, METRIC, false>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, nullptr);
+}
+// level 0: also lists the uncertified queries (fail_list[0 .. *n_failed)), which are then run again on their own
+template <int ELEM, int METRIC>
+__global__ void __launch_bounds__(SS_THREADS) cta_refine_list_kernel(const uint8_t* __restrict__ rows, size_t stride, int V,
+                                                                const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
+                                                                LcBound bound, const float* __restrict__ qn, const float* __restrict__ dist,
+                                                                const float* __restrict__ smin, int64_t cap, int64_t cap_s,
+                                                                const int32_t* __restrict__ seg_len, const int32_t* __restrict__ probe_lists,
+                                                                const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
+                                                                int32_t* __restrict__ out_pos, float* __restrict__ out_key,
+                                                                int* __restrict__ n_failed, int32_t* __restrict__ fail_list) {
+    cta_refine_body<ELEM, METRIC, true>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, fail_list);
 }
 
 // Bytes one launch of list_tc_kernel moves, from the same job list the kernel walks (profiling only):
@@ -802,6 +993,9 @@ __global__ void lc_traffic_kernel(LcArgs a, uint32_t a_bytes, unsigned long long
 
 enum { WSC_B = 21, WSC_N = 22, WSC_K = 23 };
 
+// c_sum of lc_make_bound: the fp32 norms, the final sum and the exact distance, relative to |x|^2 + |q|^2
+static float lc_c_sum(int dim) { return std::max(1.0f / 65536.0f, 3.0f * ((float)dim / 32.0f + 8.0f) / 16777216.0f); }
+
 static unsigned long long* g_traffic = nullptr;   // device accumulators of lc_traffic_kernel, per filter use (0 = lists, 1 = centres)
 static bool g_traffic_on = false;
 
@@ -813,6 +1007,7 @@ bool list_tc_supported(int elem, int key_metric, int k) {
 int list_tc_kp(int k, int level) {
     // candidates kept per query.  Only those under the threshold are re-scored, so a generous k' costs a slightly
     // larger selection, not more exact distances; the certificate fails only when ALL k' are under the threshold.
+    if (level == 0) return k <= 10 ? 128 : 1 << 20;   // level 0's bound is ~4x level 1's: twice the candidates
     if (level == 1) return k <= 10 ? 64 : k <= 40 ? 128 : 1 << 20;
     return k <= 10 ? 32 : k <= 24 ? 48 : k <= 40 ? 64 : 1 << 20;
 }
@@ -859,7 +1054,37 @@ int list_tc_prepare(const Table& rows, ListTcImage* im) {
     return VB_OK;
 }
 
+int list_tc_prepare_l0(const Table& rows, ListTcImage* im) {
+    cudaStream_t s = ctx().stream;
+    im->l0_tried = true;
+    const int n_kblocks8 = (rows.dim + 127) / 128;
+    const int64_t n_padded = im->n_tiles * LC_M;
+    VB_CUDA(cudaMalloc(&im->planes8, std::max<size_t>((size_t)im->n_tiles * n_kblocks8 * LC_A_PLANE, 16)));
+    VB_CUDA(cudaMalloc(&im->xs, sizeof(float) * (size_t)std::max<int64_t>(n_padded, 1)));
+    im->n_kblocks8 = n_kblocks8;
+    im->rmax = 0.f;
+    if (rows.n == 0) return VB_OK;
+    unsigned* d_rmax;
+    VB_CUDA(cudaMalloc(&d_rmax, sizeof(unsigned)));
+    VB_CUDA(cudaMemsetAsync(d_rmax, 0, sizeof(unsigned), s));
+    const unsigned grid = (unsigned)((n_padded * 32 + 255) / 256);
+    if (rows.elem == VB_VECTOR)
+        pack_rows_i8_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(rows.d, rows.stride, rows.n, rows.dim, n_kblocks8, n_padded, im->planes8, im->xs, d_rmax);
+    else
+        pack_rows_i8_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(rows.d, rows.stride, rows.n, rows.dim, n_kblocks8, n_padded, im->planes8, im->xs, d_rmax);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    unsigned bits = 0;
+    VB_CUDA(cudaMemcpyAsync(&bits, d_rmax, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    VB_CUDA(cudaFree(d_rmax));
+    memcpy(&im->rmax, &bits, sizeof(float));
+    return VB_OK;
+}
+
 void list_tc_release(ListTcImage* im) {
+    if (im->planes8) cudaFree(im->planes8);
+    if (im->xs) cudaFree(im->xs);
     if (im->planes) cudaFree(im->planes);
     if (im->xn) cudaFree(im->xn);
     if (im->units) cudaFree(im->units);
@@ -876,8 +1101,13 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
     VB_TRY(build_query_groups(d_lists, nq, probes, cand_off, cap, n_lists, LC_N, &g, smin ? cap_s : 0));
     const int64_t max_gtiles = g.n_pairs / LC_N + n_lists + 1;
     void *d_B, *d_qn;
-    VB_TRY(workspace(WSC_B, (size_t)max_gtiles * im.n_kblocks * LC_B_STAGE, &d_B));
-    VB_TRY(workspace(WSC_N, sizeof(float) * (size_t)nq + 64, &d_qn));
+    // (level 0: the B tiles take half of this, the packed queries q8 follow them)
+    const size_t q8_bytes = level == 0 ? (size_t)nq * 2 * im.n_kblocks8 * 128 : 0;
+    VB_TRY(workspace(WSC_B, (size_t)max_gtiles * im.n_kblocks * LC_B_STAGE + q8_bytes, &d_B));
+    // [|q|^2 | level 0: t_q | level 0: eps(q)^2], one size for every level so that the |q|^2 cache below stays put
+    VB_TRY(workspace(WSC_N, sizeof(float) * (size_t)nq * 3 + 64, &d_qn));
+    float* d_tq = (float*)d_qn + nq;
+    float* d_qe2 = d_tq + nq;
     // the query image is fp32 with the rows' padded dimension count for both element types
     const int qdim = (int)(qstride / 4);
     {
@@ -896,18 +1126,33 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
             qn_buf = d_qn;
         }
     }
-    const int64_t chunks = g.n_pairs * im.n_kblocks * 8;
-    pack_groups_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>((const float*)qimg, qstride, qdim, im.n_kblocks, g.n_pairs,
-                                                                        g.pair_q, g.pair_list, g.begin, g.gt_begin, (uint8_t*)d_B);
+    const bool l0 = level == 0;
+    const int n_kblocks = l0 ? im.n_kblocks8 : im.n_kblocks;
+    const int64_t chunks = g.n_pairs * n_kblocks * 8;
+    if (l0) {
+        VB_REQUIRE(im.planes8 != nullptr && !one_list_all_queries, "list scan level 0 without its int8 image");
+        const int qpad = n_kblocks * 128;
+        int8_t* q8 = (int8_t*)d_B + (size_t)max_gtiles * n_kblocks * LC_B_STAGE;
+        l0_query_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, s>>>((const float*)qimg, qstride, std::min(qdim, qpad), qpad, nq, im.xmax,
+                                                                          im.rmax, key_metric == VB_L2_SQUARED, lc_c_sum(rows.dim), d_tq,
+                                                                          d_qe2, q8);
+        pack_groups_i8_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>(q8, qpad, n_kblocks, g.n_pairs, g.pair_q, g.pair_list,
+                                                                               g.begin, g.gt_begin, (uint8_t*)d_B);
+        count_launch();
+    } else {
+        pack_groups_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>((const float*)qimg, qstride, qdim, n_kblocks, g.n_pairs,
+                                                                            g.pair_q, g.pair_list, g.begin, g.gt_begin, (uint8_t*)d_B);
+    }
     VB_CUDA(cudaGetLastError());
     count_launch();
     static bool attr_set = false;
     if (!attr_set) {
         VB_CUDA(cudaFuncSetAttribute(list_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LC_SMEM));
+        VB_CUDA(cudaFuncSetAttribute(list_tc_l0_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LC_SMEM));
         attr_set = true;
     }
     LcArgs a{};
-    a.A = im.planes;
+    a.A = l0 ? im.planes8 : im.planes;
     a.B = (const uint8_t*)d_B;
     a.units = im.units;
     a.n_units = im.n_units;
@@ -922,23 +1167,25 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
     a.out = out;
     a.smin = smin;
     a.pair_sbase = g.pair_sbase;
-    a.n_kblocks = im.n_kblocks;
+    a.n_kblocks = n_kblocks;
     a.is_l2 = key_metric == VB_L2_SQUARED;
     a.hi_only = level == 1;
     a.uniform_nqt = one_list_all_queries ? (int)((nq * probes + LC_N - 1) / LC_N) : 0;
     a.n_jobs = a.uniform_nqt ? im.n_units * a.uniform_nqt : im.n_units;
     const int grid = std::max(1, std::min(a.n_jobs, c.sm_count));
     prof_begin(one_list_all_queries ? VB_PROF_CENTRE_TC : VB_PROF_LIST_TC);
-    list_tc_kernel<<<grid, LC_THREADS, LC_SMEM, s>>>(a);
+    if (l0) list_tc_l0_kernel<<<grid, LC_THREADS, LC_SMEM, s>>>(a, im.xs, d_tq);
+    else list_tc_kernel<<<grid, LC_THREADS, LC_SMEM, s>>>(a);
     prof_end(one_list_all_queries ? VB_PROF_CENTRE_TC : VB_PROF_LIST_TC);
     VB_CUDA(cudaGetLastError());
     count_launch();
     if (g_traffic_on && g_traffic) {
-        lc_traffic_kernel<<<32, 256, 0, s>>>(a, level == 1 ? LC_A_PLANE : LC_A_STAGE, g_traffic + (one_list_all_queries ? 4 : 0));
+        // (level 0: a.n_kblocks counts 128-dimension blocks of 16 KB per tile)
+        lc_traffic_kernel<<<32, 256, 0, s>>>(a, level <= 1 ? LC_A_PLANE : LC_A_STAGE, g_traffic + (one_list_all_queries ? 4 : 0));
         VB_CUDA(cudaGetLastError());
     }
-    (void)rows;
-    *qn_out = (const float*)d_qn;
+    // the refine kernels take the bound's per-query input: |q|^2, or at level 0 eps(q)^2 (lc_make_bound)
+    *qn_out = l0 ? d_qe2 : (const float*)d_qn;
     return VB_OK;
 }
 
@@ -967,9 +1214,26 @@ int list_tc_traffic(int on, int64_t* out8) {
 // over for longer rows, where the accumulation term grows past them.
 // The fp32 norms, the final sum and the rounding of the exact fp32 distance it is compared with: 2^-16 (|x|^2 +
 // |q|^2) for L2, 2^-17 |x||q| for the inner product.
+//
+// Level 0 (int8, l0_query_kernel computes it per query).  x^ = s_x x8, q^ = t_q (q_hi + q_lo / 254), r_x = |x - x^| <= R
+// (rmax, every row), r_q = |q - q^| (computed from the packed integers), so |x^| <= xmax + R =: X and
+//   |x.q - x^.q^| = |(x - x^).q + x^.(q - q^)| <= R |q| + X r_q.
+// The tensor cores compute I_hi = x8.q_hi and I_lo = x8.q_lo exactly (int32); the epilogue's
+// s_x (t_q fma(float(I_lo), 1/254, float(I_hi))) rounds six times (two conversions, the constant, the fma, two products):
+// <= 8 u s_x t_q (|I_hi| + |I_lo| / 254) <= 2^-21 X t_q (|q_hi| + |q_lo| / 254) by Cauchy-Schwarz (u = 2^-24); 2^-20 is used.
+// L2: twice the dot term plus c_sum (X^2 + |q|^2) (the norms, the final sum, the exact distance, as at levels 1 / 2); the
+// inner product: the dot term plus 2^-17 X |q|.  The sums are taken in double, the result widened by 2^-10 and rounded up.
+// It reaches the refine kernels as eps(q)^2 in the place of |q|^2, with the unit bound below: lc_eps() = sqrt(eps(q)^2).
+
 static LcBound lc_make_bound(const Table& rows, const ListTcImage& im, int key_metric, int level) {
     LcBound bound;
     bound.is_l2 = key_metric == VB_L2_SQUARED;
+    if (level == 0) {
+        bound.c_dot = 1.0f;
+        bound.c_sum = 0.0f;
+        bound.xmax = 1.0f;
+        return bound;
+    }
     const float steps = (float)(im.n_kblocks * (TC_K / 16));
     const float rep = level == 1 ? 1.0f / 256.0f + 1.0f / 65536.0f : 3.0f / 65536.0f;
     const float acc = 2.0f * (level == 1 ? 2.0f : 3.0f) * steps / 8388608.0f;
@@ -979,7 +1243,7 @@ static LcBound lc_make_bound(const Table& rows, const ListTcImage& im, int key_m
     bound.c_dot = bound.is_l2 ? 2.0f * c_ip : c_ip + 1.0f / 131072.0f;
     // norms and the exact fp32 distance each sum dim / 32 terms per lane plus a shuffle tree: 3 * (dim / 32 + 8) * 2^-24 of
     // (|x|^2 + |q|^2) covers the two norms and the distance (<= 2 (|x|^2 + |q|^2)); 2^-16 up to ~2700 dimensions
-    bound.c_sum = std::max(1.0f / 65536.0f, 3.0f * ((float)rows.dim / 32.0f + 8.0f) / 16777216.0f);
+    bound.c_sum = lc_c_sum(rows.dim);
     bound.xmax = im.xmax;
     return bound;
 }
@@ -1071,7 +1335,7 @@ int launch_list_tc_select_refine(const Table& rows, const ListTcImage& im, int k
 int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                               int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
                               const float* dist, const float* smin, int64_t cap, int64_t cap_s, const int32_t* seg_len, const float* qn,
-                              int32_t* out_pos, float* out_key, int* fail_dev, int level) {
+                              int32_t* out_pos, float* out_key, int* fail_dev, int level, int32_t* fail_list) {
     if (nq == 0) return VB_OK;
     Context& c = ctx();
     cudaStream_t s = c.stream;
@@ -1082,6 +1346,14 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
     VB_REQUIRE(kp <= 256 && smem <= 200 * 1024 && (smin || cap <= SS_CAND), "cta_refine: k' = %d / %zu bytes of shared memory not supported", kp, smem);
 #define VB_CR(E, M)                                                                                                              \
     do {                                                                                                                         \
+        if (fail_list) {                                                                                                         \
+            auto kern = cta_refine_list_kernel<E, M>;                                                                            \
+            if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
+            kern<<<(unsigned)nq, SS_THREADS, smem, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, k, kp, probes, bound, qn, dist, \
+                                                       smin, cap, cap_s, seg_len, d_lists, cand_off, d_list_off, out_pos, out_key, fail_dev, \
+                                                       fail_list);                                                              \
+            break;                                                                                                               \
+        }                                                                                                                        \
         auto kern = cta_refine_kernel<E, M>;                                                                                     \
         if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));       \
         kern<<<(unsigned)nq, SS_THREADS, smem, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, k, kp, probes, bound, qn, dist, smin, \

@@ -11,6 +11,8 @@ does not cover: k-means assign on the tensor cores (config D shape, one GPU's sh
                                           (ivfflat.iterative_scan for filtered LIMIT 10 queries vs the per-scan loop)
     python tools/bench_extra.py filter   [--rows N --dim D --lists L --probes P --max-probes M --page K --queries Q]
                                           (row filters on the device: filtered iterative scan and exact top-k vs host filtering)
+    python tools/bench_extra.py level0   [--rows N --dim D --lists L --probes P --rounds R --law rank16|mixture --load S]
+                                          (the batched list scan with filter level 0 (int8 rows) on and off, alternating)
 
 All timing with CUDA events on the library stream; inputs resident in HBM.
 """
@@ -332,6 +334,84 @@ def bench_ivf(args):
                       "queries_per_s": B / (ms / 1000.0), "ms_per_batch": ms, "candidates_per_query": cand / B,
                       "roofline": {"bound": "hbm", "kernel": "list scan", "achieved": gbs, "peak": hbm, "unit": "GB/s", "frac": gbs / hbm,
                                    "bytes_per_launch": cand * rb, "avg_launch_ms": scan_ms / scan_n, "share_of_step": scan_ms / scan_n / ms, "peak_source": src}}))
+
+
+def bench_level0(args):
+    """config B (IVFFlat L2, 2048-query batches, k 10) on bench.py's own data and index -- its law, its queries (the first
+    four batches of 2048) and its index recipe, through its functions -- with "tc_level0" 1 and 0 in alternating rounds in
+    one process: step time, list_tc_kernel time and bytes, refine time, level-0 fallbacks per batch, and whether the two
+    arms return identical ids and distances for every batch."""
+    import argparse as ap_
+    import torch
+    import bench
+    import pgvector_b200 as pv
+    pv.init(0)
+    dev = torch.device("cuda", 0)
+    bargs = ap_.Namespace(rows=args.rows, dim=args.dim, lists=args.lists, latent_dim=16, components=1000, queries=10_000)
+    rows, queries = bench.make_dataset(bargs, args.law, dev)
+    torch.cuda.synchronize()
+    centers, offsets, grouped, order, how = bench.build_index_arrays(bargs, args.law, rows, pv)
+    del rows
+    torch.cuda.empty_cache()
+    ix = pv.IvfflatIndex("vector_l2_ops", args.dim, args.lists).load(centers, offsets, grouped, order)
+    q_t = queries[:4 * 2048]
+    stream = torch.cuda.ExternalStream(pv.stream_handle(), device=dev)
+    k, B = 10, 2048
+    batches = [q_t[i:i + B].contiguous() for i in range(0, q_t.shape[0] - B + 1, B)]
+    ids = torch.empty((B, k), dtype=torch.int64, device=dev)
+    dist = torch.empty((B, k), dtype=torch.float32, device=dev)
+    step = [0]
+
+    def one():
+        ix.search_into(batches[step[0] % len(batches)], k, args.probes, ids, dist)
+        step[0] += 1
+
+    def outputs():
+        got = []
+        for qb in batches:
+            ix.search_into(qb, k, args.probes, ids, dist)
+            got.append((ids.cpu().numpy().copy(), dist.cpu().numpy().copy()))
+        return got
+
+    rounds, ref = [], {}
+    for r in range(args.rounds):
+        for arm in (1, 0):
+            pv.set_option("tc_level0", arm)
+            n = 16 * len(batches)
+            f0 = ix.tc_level0_fallbacks()
+            # bench.py's conditions: the timed steps follow `--load` untimed ones (its clock-sampler load, 600 steps), so
+            # a power-limited card is at its sustained clock; the SM clock is sampled over both (bench.ClockSampler)
+            sampler = bench.ClockSampler(0)
+            sampler.start()
+            ms = timed(pv, torch, stream, one, warmup=args.load, steps=n)
+            clocks = sampler.stop()
+            fails = (ix.tc_level0_fallbacks() - f0) / (n + args.load)
+            pv.prof_enable(True)
+            for p in (pv.PROF_LIST_TC, pv.PROF_TOPK):
+                pv.prof_read(p)
+            ms_prof = timed(pv, torch, stream, one, warmup=0, steps=2 * len(batches))   # as bench.py times: kernel brackets on
+            tc_ms, tc_n = pv.prof_read(pv.PROF_LIST_TC)
+            rf_ms, rf_n = pv.prof_read(pv.PROF_TOPK)
+            pv.prof_enable(False)
+            pv.tc_traffic(True, read=True)
+            one()
+            pv.synchronize()
+            t = pv.tc_traffic(False, read=True)
+            got = outputs()
+            if arm not in ref:
+                ref[arm] = got
+            rounds.append({"round": r, "tc_level0": arm, "ms_per_step": ms, "queries_per_s": B / (ms / 1000.0),
+                           "ms_per_step_with_kernel_brackets": ms_prof, "sm_mhz": clocks.get("sm_mhz"),
+                           "clock_reasons": clocks.get("reasons"),
+                           "list_tc_ms": tc_ms / max(tc_n, 1), "list_tc_launches_per_step": tc_n / (2 * len(batches)),
+                           "list_tc_bytes_per_launch": int((t[1] + t[2]) / max(t[3], 1)), "refine_ms": rf_ms / max(rf_n, 1),
+                           "level0_fallback_queries_per_batch": fails})
+    same = all(np.array_equal(a[0], b_[0]) and np.array_equal(a[1], b_[1]) for a, b_ in zip(ref[1], ref[0]))
+    ratio = [rounds[i + 1]["ms_per_step"] / rounds[i]["ms_per_step"] for i in range(0, len(rounds), 2)]   # off / on
+    print(json.dumps({"bench": "level0", "card": card(),
+                      "workload": f"IVFFlat vector_l2_ops {args.rows}x{args.dim}, lists={args.lists}, probes={args.probes}, k={k}, "
+                                  f"{len(batches)} batches of {B} queries, bench.py's {args.law} law and index ({how})",
+                      "rounds": rounds, "speedup_level0_per_round": ratio, "outputs_identical": bool(same)}))
 
 
 def bench_ivf_iter(args):
@@ -669,7 +749,7 @@ def bench_sparse(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "ivf-iter", "filter", "kmeans", "sparse", "rerank"])
+    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "ivf-iter", "filter", "kmeans", "sparse", "rerank", "level0"])
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--lists", type=int, default=1000)
     ap.add_argument("--probes", type=int, default=10)
@@ -683,11 +763,16 @@ if __name__ == "__main__":
     ap.add_argument("--max-probes", type=int, default=100)
     ap.add_argument("--page", type=int, default=100)
     ap.add_argument("--sample", type=int, default=16)
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--law", default="rank16", choices=["rank16", "mixture"])
+    ap.add_argument("--load", type=int, default=600)
     a = ap.parse_args()
     if a.what == "rerank":      # config E's query batch and ef_search
         a.queries, a.ef = a.queries or 2048, a.ef or 200
     if a.what in ("ivf-iter", "filter"):
         a.queries = a.queries or 2048
+    if a.what == "level0":
+        a.queries = a.queries or 4 * 2048
     a.queries, a.ef = a.queries or 4096, a.ef or 100
     if a.what == "sparse":
         a.rows = a.rows or 1_000_000
@@ -714,6 +799,11 @@ if __name__ == "__main__":
         a.dim = a.dim or 1536
         a.elem = "vector" if a.elem == "halfvec" and "--elem" not in sys.argv else a.elem
         (bench_ivf_iter if a.what == "ivf-iter" else bench_filter)(a)
+    elif a.what == "level0":
+        a.rows = a.rows or 1_000_000
+        a.dim = a.dim or 1536
+        a.elem = "vector" if "--elem" not in sys.argv else a.elem
+        bench_level0(a)
     elif a.what == "ivf":
         a.rows = a.rows or 1_000_000
         a.dim = a.dim or (1536 if a.elem == "halfvec" else 1024)
