@@ -100,16 +100,13 @@ __device__ __forceinline__ bool lc_job(const LcArgs& a, int j, LcJob& jb) {
 // One (unit, query tile) for one consumer warpgroup: the MMAs of all K blocks, then the epilogue.  NQ = queries per
 // column group; the accumulator holds the 64 x 2 NQ product x . [q_hi ; q_lo] (NQ registers), whose column groups
 // [0, NQ) and [NQ, 2 NQ) are added -- register i + NQ / 2 holds column c + NQ of register i's column c.
-// I8 (level 0): the operands are int8 planes, 128 dimensions per K block, and the int32 accumulator is exact; the
-// epilogue scales it by s_x (xs, per row) and t_q (tq, per query).
-template <int NQ, bool I8>
+template <int NQ>
 __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_stages, uint32_t stage_bytes, uint32_t a_bytes,
                                         uint64_t* full_bar, uint64_t* empty_bar, float* slab_buf, uint32_t& it, const LcJob& jb,
-                                        int qt, const float* xs, const float* tq) {
+                                        int qt) {
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
     const int wg = warp / 4, t = threadIdx.x % 128;
     float acc[NQ];
-    int iacc[I8 ? NQ : 1];
     for (int kb = 0; kb < a.n_kblocks; ++kb, ++it) {
         const int s = it % n_stages;
         const uint32_t ph = (it / n_stages) & 1;
@@ -119,15 +116,6 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
         const uint64_t da_hi = make_sw128_desc(sa), da_lo = make_sw128_desc(sa + LC_A_PLANE);
         const uint64_t db = make_sw128_desc(sb);
         wgmma_fence();
-        if constexpr (I8) {
-            // x8 . [q_hi ; q_lo]: four k32 steps over the 128 int8 of the block
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                if constexpr (NQ == 64) wgmma_s8_n128(iacc, da_hi + adv, db + adv, (kb | k) != 0);
-                else wgmma_s8_n64(iacc, da_hi + adv, db + adv, (kb | k) != 0);
-            }
-        } else {
 #pragma unroll
         for (int k = 0; k < TC_K / 16; ++k) {
             const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);
@@ -147,7 +135,6 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
             }
             if (!a.hi_only && k + 1 < TC_K / 16) wgmma_fence();   // the next K step returns to the wider shape
         }
-        }
         wgmma_commit();
         wgmma_wait<0>();
         __syncwarp();
@@ -162,13 +149,12 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
     const int frag_col = 2 * (t % 4);
     int64_t r_table[2];
     bool valid_row[2];
-    float xnr[2], xsr[2];
+    float xnr[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         r_table[h] = (int64_t)un.tile * LC_M + frag_row + 8 * h;
         valid_row[h] = r_table[h] >= lo && r_table[h] < hi;
         xnr[h] = valid_row[h] && a.is_l2 ? a.xn[r_table[h]] : 0.f;
-        xsr[h] = I8 && valid_row[h] ? xs[r_table[h]] : 0.f;
     }
     const int gb = a.grp_begin[un.list];
     // warps 2p and 2p + 1 hold the 32 rows of table-aligned slab p of the tile (if any of them belongs to the list)
@@ -183,20 +169,17 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
         for (int e = 0; e < 2; ++e) {
             const int col = qt * LC_N + 8 * cb + frag_col + e;
             int64_t po = 0;
-            float qn = 0.f, tqc = 0.f;
+            float qn = 0.f;
             if (col < cnt) {
                 po = a.pair_out[gb + col];
                 if (a.is_l2) qn = a.qn[a.pair_q[gb + col]];
-                if (I8) tqc = tq[a.pair_q[gb + col]];
             }
             float m = __int_as_float(0x7F800000);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int i = 4 * cb + 2 * h + e;
                 if (col < cnt && valid_row[h]) {
-                    // level 0: x^.q^ = s_x t_q (x8.q_hi + x8.q_lo / 254), the roundings bounded in lc_make_bound
-                    const float dot = I8 ? xsr[h] * (tqc * fmaf((float)iacc[i + NQ / 2], 1.0f / 254.0f, (float)iacc[i]))
-                                         : acc[i] + acc[i + NQ / 2];
+                    const float dot = acc[i] + acc[i + NQ / 2];
                     const float val = a.is_l2 ? fmaf(-2.f, dot, xnr[h] + qn) : -dot;
                     a.out[po + (r_table[h] - lo)] = val;
                     m = fminf(m, val);
@@ -229,17 +212,14 @@ __device__ __forceinline__ void lc_tile(const LcArgs& a, uint8_t* smem, int n_st
     }
 }
 
-template <bool I8>
-__device__ __forceinline__ void list_tc_body(const LcArgs& a, const float* xs, const float* tq) {
+__device__ __forceinline__ void list_tc_body(const LcArgs& a) {
     extern __shared__ uint8_t lc_smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(lc_smem_raw) + 1023) & ~(uintptr_t)1023);
     // stage ring: level 2 = 4 stages of (A hi+lo 32 KB | B 16 KB), level 1 = 7 stages of (A hi 16 KB | B 16 KB) --
     // the bytes in flight per SM are what keeps HBM busy
-    // level 0 = level 1's ring: 16 KB of int8 rows (128 dimensions) + the 16 KB [q_hi ; q_lo] int8 tile per stage
-    const int n_stages = I8 || a.hi_only ? LC_STAGES_L1 : LC_STAGES;
-    const uint32_t stage_bytes = I8 || a.hi_only ? LC_STAGE_L1 : LC_STAGE;
-    const uint32_t a_bytes = I8 || a.hi_only ? LC_A_PLANE : LC_A_STAGE;   // the hi plane leads each 32 KB block of the image
-    const uint32_t a_tile_block = I8 ? LC_A_PLANE : LC_A_STAGE;            // bytes per (tile, K block) of the image
+    const int n_stages = a.hi_only ? LC_STAGES_L1 : LC_STAGES;
+    const uint32_t stage_bytes = a.hi_only ? LC_STAGE_L1 : LC_STAGE;
+    const uint32_t a_bytes = a.hi_only ? LC_A_PLANE : LC_A_STAGE;   // the hi plane leads each 32 KB block of the image
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)n_stages * stage_bytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + LC_MAX_STAGES;
@@ -277,7 +257,7 @@ __device__ __forceinline__ void list_tc_body(const LcArgs& a, const float* xs, c
                     const uint8_t* gb = a.B + ((size_t)(gt0 + qt) * a.n_kblocks + kb) * LC_B_STAGE;
                     if (leader) {
                         mbar_arrive_expect_tx(&full_bar[s], a_bytes + (n32 ? LC_B_STAGE / 2 : LC_B_STAGE));
-                        bulk_g2s(sa, a.A + ((size_t)un.tile * a.n_kblocks + kb) * a_tile_block, a_bytes, &full_bar[s]);
+                        bulk_g2s(sa, a.A + ((size_t)un.tile * a.n_kblocks + kb) * LC_A_STAGE, a_bytes, &full_bar[s]);
                         if (n32) {   // [q_hi rows 0..31 | q_lo rows 0..31] back to back = one 64-row operand
                             bulk_g2s(sb, gb, LC_B_PLANE / 2, &full_bar[s]);
                             bulk_g2s(sb + LC_B_PLANE / 2, gb + LC_B_PLANE, LC_B_PLANE / 2, &full_bar[s]);
@@ -299,17 +279,231 @@ __device__ __forceinline__ void list_tc_body(const LcArgs& a, const float* xs, c
             LcJob jb;
             if (!lc_job(a, j, jb)) continue;
             for (int qt = jb.q_lo; qt < jb.q_hi; ++qt) {
-                if (jb.cnt - qt * LC_N <= 32) lc_tile<32, I8>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt, xs, tq);
-                else lc_tile<64, I8>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt, xs, tq);
+                if (jb.cnt - qt * LC_N <= 32) lc_tile<32>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt);
+                else lc_tile<64>(a, smem, n_stages, stage_bytes, a_bytes, full_bar, empty_bar, slab_buf, it, jb, qt);
             }
         }
     }
 }
 
-__global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) { list_tc_body<false>(a, nullptr, nullptr); }
-// level 0: a.A = the int8 plane, a.n_kblocks = its 128-dimension blocks, a.B = query tiles from pack_groups_i8_kernel
+__global__ void __launch_bounds__(LC_THREADS, 1) list_tc_kernel(LcArgs a) { list_tc_body(a); }
+
+// ----------------------------------------------------------------------------- level 0 (int8)
+// a.A = the int8 plane ([tile][128-dimension block][128 rows x 128 B]), a.n_kblocks = its 128-dimension blocks, a.B =
+// the [q_hi ; q_lo] int8 query tiles of pack_groups_i8_kernel.  Level 1's ring: 7 stages of 16 KB of rows + the 16 KB
+// query tile.  What differs from list_tc_kernel:
+//   - the producer tells the consumers which (unit, query tile) a stage starts through a tag beside the stage, so the
+//     consumers read no job list;
+//   - the consumers release a stage one K block late, behind wgmma_wait<1>: the next block's MMAs are issued before
+//     the previous block's finish (the int32 sums are exact, so the order cannot change them);
+//   - the epilogue's operands (list bounds, row scales and norms, each column's output offset, slab base, t_q and
+//     |q|^2) are loaded while the MMAs of the tile run, one dependent level per K block, each column by one lane of
+//     its quad group and shuffled to the others: the epilogue itself waits on no global load.  (It ran after the last
+//     K block behind a chain of three dependent loads, with the ring's stages held and no MMA issued.)
+struct L0Tag {
+    int32_t list, tile, cnt, qt;   // list < 0: no more work
+};
+
+template <int NQ>
+__device__ __forceinline__ void l0_tile(const LcArgs& a, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, float* slab_buf,
+                                        uint32_t& it, const L0Tag tg, const float* __restrict__ xs, const float* __restrict__ tq) {
+    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+    const int wg = warp / 4, t = threadIdx.x % 128;
+    const int qt = tg.qt, cnt = tg.cnt;
+    const int frag_row = wg * 64 + 16 * (t / 32) + (t % 32) / 4;   // and frag_row + 8
+    const int frag_col = 2 * (t % 4);
+    // dependent level 1: the list and its rows
+    const int64_t lo = a.list_off[tg.list], hi = a.list_off[tg.list + 1];
+    const int gb = a.grp_begin[tg.list];
+    int64_t r_table[2];
+    float xn_r[2], xs_r[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        r_table[h] = (int64_t)tg.tile * LC_M + frag_row + 8 * h;   // < n_tiles * 128: xn and xs cover the padding
+        xn_r[h] = a.is_l2 ? a.xn[r_table[h]] : 0.f;
+        xs_r[h] = xs[r_table[h]];
+    }
+    // lane 4 c + (t % 4) loads columns 8 c + frag_col + {0, 1} of the tile (c < NQ / 8): levels 2 and 3 during the MMAs
+    const int my_col = qt * LC_N + 8 * (lane / 4) + frag_col;
+    const bool col_ok[2] = {lane / 4 < NQ / 8 && my_col < cnt, lane / 4 < NQ / 8 && my_col + 1 < cnt};
+    int64_t po_l[2] = {0, 0};
+    int32_t pq_l[2] = {0, 0}, sb_l[2] = {0, 0};
+    float qn_l[2] = {0.f, 0.f}, tq_l[2] = {0.f, 0.f};
+    int iacc[NQ];
+    for (int kb = 0; kb < a.n_kblocks; ++kb, ++it) {
+        const int s = it % LC_STAGES_L1;
+        if (kb > 0) mbar_wait(&full_bar[s], (it / LC_STAGES_L1) & 1);   // (the first block's was waited for with the tag)
+        const uint32_t st = smem_u32(smem + (size_t)s * LC_STAGE_L1);
+        const uint64_t da = make_sw128_desc(st + (uint32_t)wg * (64 * 128)), db = make_sw128_desc(st + LC_A_PLANE);
+        wgmma_fence();
+        // x8 . [q_hi ; q_lo]: four k32 steps over the 128 int8 of the block
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t adv = (uint64_t)((k * 32) >> 4);
+            if constexpr (NQ == 64) wgmma_s8_n128(iacc, da + adv, db + adv, (kb | k) != 0);
+            else wgmma_s8_n64(iacc, da + adv, db + adv, (kb | k) != 0);
+        }
+        wgmma_commit();
+        // at most this block's group is pending: the previous block's stage is free
+        wgmma_wait<1>();
+        __syncwarp();
+        if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[(it + LC_STAGES_L1 - 1) % LC_STAGES_L1]);
+        if (kb == 0) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+                if (col_ok[e]) {
+                    po_l[e] = a.pair_out[gb + my_col + e];
+                    pq_l[e] = a.pair_q[gb + my_col + e];
+                    if (a.smin) sb_l[e] = a.pair_sbase[gb + my_col + e];
+                }
+        }
+        if (kb == a.n_kblocks / 2) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+                if (col_ok[e]) {
+                    if (a.is_l2) qn_l[e] = a.qn[pq_l[e]];
+                    tq_l[e] = tq[pq_l[e]];
+                }
+        }
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[(it + LC_STAGES_L1 - 1) % LC_STAGES_L1]);
+
+    // ===== epilogue: rows of the table tile x queries of the group =====
+    bool valid_row[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) valid_row[h] = r_table[h] >= lo && r_table[h] < hi;
+    // warps 2p and 2p + 1 hold the 32 rows of table-aligned slab p of the tile (if any of them belongs to the list)
+    const int pair = warp / 2;
+    const int64_t slab_row0 = (int64_t)tg.tile * LC_M + pair * 32;
+    const bool slabs = a.smin != nullptr && slab_row0 < hi && slab_row0 + 32 > lo;
+    const int slab_local = (int)((slab_row0 >> 5) - (lo >> 5));
+    float col_min[NQ / 4];
+#pragma unroll
+    for (int cb = 0; cb < NQ / 8; ++cb)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int col = qt * LC_N + 8 * cb + frag_col + e;
+            const int src = 4 * cb + (lane & 3);
+            const int64_t po = __shfl_sync(0xffffffffu, po_l[e], src);
+            const float qn = __shfl_sync(0xffffffffu, qn_l[e], src);
+            const float tqc = __shfl_sync(0xffffffffu, tq_l[e], src);
+            float m = __int_as_float(0x7F800000);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int i = 4 * cb + 2 * h + e;
+                if (col < cnt && valid_row[h]) {
+                    // x^.q^ = s_x t_q (x8.q_hi + x8.q_lo / 254), the roundings bounded in lc_make_bound
+                    const float dot = xs_r[h] * (tqc * fmaf((float)iacc[i + NQ / 2], 1.0f / 254.0f, (float)iacc[i]));
+                    const float val = a.is_l2 ? fmaf(-2.f, dot, xn_r[h] + qn) : -dot;
+                    a.out[po + (r_table[h] - lo)] = val;
+                    m = fminf(m, val);
+                }
+            }
+            col_min[2 * cb + e] = m;
+        }
+    if (slabs) {
+        // minimum of each column over the slab's 32 rows: over the 16 rows of this warp (lanes of equal t % 4), then
+        // the odd warp of the pair hands its minima to the even one
+#pragma unroll
+        for (int j = 0; j < NQ / 4; ++j)
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) col_min[j] = fminf(col_min[j], __shfl_xor_sync(0xffffffffu, col_min[j], o));
+        float* buf = slab_buf + pair * LC_N;
+        if ((warp & 1) && lane < 4) {
+#pragma unroll
+            for (int j = 0; j < NQ / 4; ++j) buf[8 * (j / 2) + frag_col + (j % 2)] = col_min[j];
+        }
+        int32_t sb[NQ / 4];
+#pragma unroll
+        for (int j = 0; j < NQ / 4; ++j) sb[j] = __shfl_sync(0xffffffffu, sb_l[j % 2], 4 * (j / 2) + (lane & 3));
+        named_bar_sync(1 + pair, 64);
+        if (!(warp & 1) && lane < 4) {
+#pragma unroll
+            for (int j = 0; j < NQ / 4; ++j) {
+                const int c = 8 * (j / 2) + frag_col + (j % 2);
+                const int col = qt * LC_N + c;
+                if (col < cnt) a.smin[sb[j] + slab_local] = fminf(col_min[j], buf[c]);
+            }
+        }
+        named_bar_sync(1 + pair, 64);   // buf is rewritten by the next tile
+    }
+}
+
 __global__ void __launch_bounds__(LC_THREADS, 1) list_tc_l0_kernel(LcArgs a, const float* __restrict__ xs, const float* __restrict__ tq) {
-    list_tc_body<true>(a, xs, tq);
+    extern __shared__ uint8_t lc_smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(lc_smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)LC_STAGES_L1 * LC_STAGE_L1);
+    uint64_t* full_bar = bars;
+    uint64_t* empty_bar = bars + LC_MAX_STAGES;
+    L0Tag* tags = reinterpret_cast<L0Tag*>(bars + 2 * LC_MAX_STAGES);   // [LC_MAX_STAGES], the tile of a stage's first K block
+    float* slab_buf = reinterpret_cast<float*>(bars + 32);              // [4 warp pairs][LC_N]
+
+    const int warp = threadIdx.x / 32;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < LC_STAGES_L1; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], LC_CONSUMERS / 32);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp == LC_CONSUMERS / 32) {
+        // ===== producer (whole warp converged, one elected lane issues the copies), jobs in static round-robin =====
+        const bool leader = elect_one();
+        uint32_t it = 0;
+        for (int j = blockIdx.x; j < a.n_jobs; j += gridDim.x) {
+            const ListUnit un = a.units[j];
+            const int cnt = a.grp_cnt[un.list];
+            const int gt0 = a.gt_begin[un.list];
+            const int nqt = (cnt + LC_N - 1) / LC_N;
+            for (int qt = 0; qt < nqt; ++qt) {
+                // a query tile with at most 32 queries is multiplied as N = 64: only the first half of each B plane moves
+                const bool n32 = cnt - qt * LC_N <= 32;
+                for (int kb = 0; kb < a.n_kblocks; ++kb, ++it) {
+                    const int s = it % LC_STAGES_L1;
+                    mbar_wait(&empty_bar[s], ((it / LC_STAGES_L1) & 1) ^ 1);
+                    uint8_t* sa = smem + (size_t)s * LC_STAGE_L1;
+                    uint8_t* sb = sa + LC_A_PLANE;
+                    const uint8_t* gb = a.B + ((size_t)(gt0 + qt) * a.n_kblocks + kb) * LC_B_STAGE;
+                    const uint8_t* ga = a.A + ((size_t)un.tile * a.n_kblocks + kb) * LC_A_PLANE;
+                    if (leader) {
+                        if (kb == 0) tags[s] = L0Tag{un.list, un.tile, cnt, qt};   // published by the arrive below
+                        mbar_arrive_expect_tx(&full_bar[s], LC_A_PLANE + (n32 ? LC_B_STAGE / 2 : LC_B_STAGE));
+                        bulk_g2s(sa, ga, LC_A_PLANE, &full_bar[s]);
+                        if (n32) {   // [q_hi rows 0..31 | q_lo rows 0..31] back to back = one 64-row operand
+                            bulk_g2s(sb, gb, LC_B_PLANE / 2, &full_bar[s]);
+                            bulk_g2s(sb + LC_B_PLANE / 2, gb + LC_B_PLANE, LC_B_PLANE / 2, &full_bar[s]);
+                        } else {
+                            bulk_g2s(sb, gb, LC_B_STAGE, &full_bar[s]);
+                        }
+                    }
+                    __syncwarp();
+                }
+            }
+        }
+        // the end of the work: a tag with no copies behind it
+        const int s = it % LC_STAGES_L1;
+        mbar_wait(&empty_bar[s], ((it / LC_STAGES_L1) & 1) ^ 1);
+        if (leader) {
+            tags[s] = L0Tag{-1, 0, 0, 0};
+            mbar_arrive(&full_bar[s]);
+        }
+        __syncwarp();
+    } else {
+        // ===== consumers: warpgroup wg multiplies rows 64 wg .. 64 wg + 63 of the table tile =====
+        uint32_t it = 0;
+        for (;;) {
+            const int s = it % LC_STAGES_L1;
+            mbar_wait(&full_bar[s], (it / LC_STAGES_L1) & 1);
+            const L0Tag tg = tags[s];
+            if (tg.list < 0) break;
+            if (tg.cnt - tg.qt * LC_N <= 32) l0_tile<32>(a, smem, full_bar, empty_bar, slab_buf, it, tg, xs, tq);
+            else l0_tile<64>(a, smem, full_bar, empty_bar, slab_buf, it, tg, xs, tq);
+        }
+    }
 }
 
 // gather + split the queries of every (query, list) pair into the B tiles of its list's group:
