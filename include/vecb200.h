@@ -413,6 +413,11 @@ int64_t		vb_ivf_tc_level0_fallbacks(const vb_ivf *ix);
  * [2] distinct query-tile bytes, [3] launches; [4..7] the same for the centre scan (probe selection).
  */
 int			vb_ivf_tc_traffic(int on, int64_t *out8);
+/*
+ * Counters of the level-0 refine, kept while traffic accounting is on: read and reset into out3 -- [0] rows re-scored
+ * exactly (per-row bounds), [1] rows the global bound (d~ <= k-th d~ + 2 eps(q)) would have re-scored, [2] queries refined.
+ */
+int			vb_ivf_tc_level0_rescored(int64_t *out3);
 
 /*
  * List-sharded search over the library's communicator (vb_comm_init): this rank's image holds its own lists under

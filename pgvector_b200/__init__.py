@@ -875,6 +875,14 @@ def tc_traffic(on=True, read=False):
     return out
 
 
+def tc_level0_rescored():
+    """read and reset the level-0 refine's counters, kept while tc_traffic is on: [rows re-scored exactly, rows the
+    global bound would have re-scored, queries refined]"""
+    out = np.zeros(3, dtype=np.int64)
+    _lib.check(load().vb_ivf_tc_level0_rescored(_ptr(out)))
+    return out
+
+
 def set_tensor_cores(on: bool):
     """False forces the exact fp32 CUDA-core assign kernel (parity tests); True (default) uses the tensor cores (wgmma)."""
     _lib.check(load().vb_set_tensor_cores(1 if on else 0))

@@ -86,6 +86,7 @@ SIGNATURES = {
     "vb_ivf_last_candidates": (_i64, [_vp]),
     "vb_ivf_tc_fallbacks": (_i64, [_vp]),
     "vb_ivf_tc_traffic": (_i, [_i, _vp]),
+    "vb_ivf_tc_level0_rescored": (_i, [_vp]),
     "vb_ivf_search_sharded_dev": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
     "vb_ivf_search_sharded": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
     "vb_exact_topk_sharded_dev": (_i, [_vp, _i, _vp, _i64, _i, _i64, _vp, _vp]),

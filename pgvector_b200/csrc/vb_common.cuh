@@ -220,6 +220,7 @@ struct ListTcImage {
     // level 0 (int8 rows), built on first use where it fits: [tile][128-dim block][128 rows x 128 B], same swizzle
     uint8_t* planes8 = nullptr;
     float* xs = nullptr;         // per-row scale s_x = max |x_i| / 127 (x ~ s_x * x8)
+    float* r8 = nullptr;         // per-row residual |x - s_x x8|, rounded up (0 on padding rows): the refine's per-row bound
     int n_kblocks8 = 0;
     float rmax = 0.f;            // max over rows of |x - s_x x8|, rounded up
     bool l0_tried = false;       // the int8 plane was built or found not to fit
@@ -244,6 +245,9 @@ int launch_list_tc_refine(const Table& rows, const ListTcImage& im, int key_metr
                           float* out_key, int* fail_dev, int* n_failed_host, int level = 2);
 // traffic accounting of list_tc_kernel launches (profiling): enable / read-and-reset 8 counters (lists: 0-3, centres: 4-7)
 int list_tc_traffic(int on, int64_t* out8);
+// read-and-reset the level-0 refine's counters, kept while traffic accounting is on: rows re-scored, rows under the
+// global-bound threshold (d~ <= d~_k + 2 eps(q)), queries refined
+int list_tc_level0_rescored(int64_t* out3);
 int launch_list_tc_select_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                                  int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
                                  const float* dist, const int64_t* seg_begin, const int32_t* seg_len, const float* qn, int32_t* out_pos,

@@ -345,7 +345,7 @@ static int ivf_ensure_tc_image(Ivf& ix) {
 static int ivf_ensure_l0_image(Ivf& ix) {
     if (ix.tc.l0_tried) return VB_OK;
     const size_t rows = (size_t)ix.tc.n_tiles * 128;
-    const size_t need = rows * ((size_t)(ix.rows.dim + 127) / 128) * 128 + rows * 4;
+    const size_t need = rows * ((size_t)(ix.rows.dim + 127) / 128) * 128 + rows * 8;   // (plane, s_x, R_x)
     size_t free_b = 0, total_b = 0;
     VB_CUDA(cudaMemGetInfo(&free_b, &total_b));
     if (free_b < need + ((size_t)4 << 30)) {
@@ -1962,6 +1962,12 @@ int vb_ivf_scan_end(vb_ivf_scan* s) {
 int vb_ivf_tc_traffic(int on, int64_t* out8) {
     VB_TRY(require_init());
     return list_tc_traffic(on, out8);
+}
+
+int vb_ivf_tc_level0_rescored(int64_t* out3) {
+    VB_TRY(require_init());
+    VB_REQUIRE(out3 != nullptr, "vb_ivf_tc_level0_rescored: out3 is NULL");
+    return list_tc_level0_rescored(out3);
 }
 
 int64_t vb_ivf_tc_fallbacks(const vb_ivf* h) { return h ? h->ix.total_tc_failed : 0; }

@@ -564,11 +564,12 @@ __device__ __forceinline__ void l0_quant_q(float v, float tq, int& hi, int& lo) 
 }
 
 // rows -> int8 plane [tile][128-dim block][128 rows x 128 B] (128-byte swizzle: byte (r, kk) at r * 128 +
-// ((kk / 16) ^ (r & 7)) * 16 + kk % 16), s_x per row, and max |x - s_x x8| over the rows (rounded up, as float bits):
-// one warp per row of the tile-padded table
+// ((kk / 16) ^ (r & 7)) * 16 + kk % 16), s_x per row, |x - s_x x8| per row (rounded up; 0 on padding rows) and its max
+// over the rows (as float bits): one warp per row of the tile-padded table
 template <int ELEM>
 __global__ void pack_rows_i8_kernel(const uint8_t* __restrict__ rows, size_t stride, int64_t n, int dim, int n_kblocks8, int64_t n_padded,
-                                    uint8_t* __restrict__ out, float* __restrict__ xs, unsigned* __restrict__ rmax_bits) {
+                                    uint8_t* __restrict__ out, float* __restrict__ xs, float* __restrict__ r8,
+                                    unsigned* __restrict__ rmax_bits) {
     const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32;
     const int lane = threadIdx.x % 32;
     if (r >= n_padded) return;
@@ -603,15 +604,19 @@ __global__ void pack_rows_i8_kernel(const uint8_t* __restrict__ rows, size_t str
     for (int o = 16; o > 0; o >>= 1) res += __shfl_xor_sync(0xffffffffu, res, o);
     if (lane == 0) {
         xs[r] = sx;
-        if (r < n) atomicMax(rmax_bits, __float_as_uint(__double2float_ru(sqrt(res) * (1.0 + 1.0 / 1048576.0))));
+        const float rx = r < n ? __double2float_ru(sqrt(res) * (1.0 + 1.0 / 1048576.0)) : 0.f;
+        r8[r] = rx;
+        if (r < n) atomicMax(rmax_bits, __float_as_uint(rx));
     }
 }
 
 // per query of the batch (one warp each): t_q, the packed query q8 = [q_hi | q_lo] (qpad int8 each, zero past qdim: quantised
 // once here, copied into the tiles of every probed list by pack_groups_i8_kernel), and the level-0 bound eps(q) >= |d~ - d_fp32|
-// over every row (lc_make_bound derives it), handed to the refine kernels squared, in the place of |q|^2 (qe2)
+// over every row (lc_make_bound derives it), handed to the refine kernels squared, in the place of |q|^2 (qe2), and the
+// coefficients (a, b, c, d) of the per-row bound E(x, q) = a R_x + b X_x + c X_x^2 + d (lc_make_bound), rounded up
 __global__ void l0_query_kernel(const float* __restrict__ qimg, size_t qstride, int qdim, int qpad, int64_t nq, float xmax, float rmax,
-                                int is_l2, float c_sum, float* __restrict__ tq_out, float* __restrict__ qe2_out, int8_t* __restrict__ q8) {
+                                int is_l2, float c_sum, float* __restrict__ tq_out, float* __restrict__ qe2_out, float4* __restrict__ coef,
+                                int8_t* __restrict__ q8) {
     const int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32;
     const int lane = threadIdx.x % 32;
     if (q >= nq) return;
@@ -651,6 +656,13 @@ __global__ void l0_query_kernel(const float* __restrict__ qimg, size_t qstride, 
         eps *= 1.0 + 1.0 / 1024.0;
         tq_out[q] = tq;
         qe2_out[q] = __double2float_ru(eps * eps);   // NaN / Inf (a query without finite norm): the certificate fails
+        // the same sum with R_x and X_x of one row in the place of rmax and X, split by its dependence on the row
+        const double w = 1.0 + 1.0 / 1024.0, dq = rq + qabs / 1048576.0;
+        const double ca = is_l2 ? 2.0 * qnorm : qnorm;
+        const double cb = is_l2 ? 2.0 * dq : dq + qnorm / 131072.0;
+        const double cc = is_l2 ? (double)c_sum : 0.0;
+        const double cd = is_l2 ? 2e-30 + (double)c_sum * n2 : 1e-30;
+        coef[q] = make_float4(__double2float_ru(ca * w), __double2float_ru(cb * w), __double2float_ru(cc * w), __double2float_ru(cd * w));
     }
 }
 
@@ -1022,6 +1034,12 @@ __global__ void __launch_bounds__(SR_WARPS * 32) select_refine_kernel(const uint
 // time on a single warp), ranked and certified.  Same arithmetic, same tie rule, same outputs as select_refine_kernel;
 // a query whose selection overflows its buffer (ties by the thousand) counts as uncertified and the batch is repeated
 // on the kernels above.
+//
+// LIST (level 0 only): the uncertified queries are also listed, and the re-score uses per-row bounds E_i (lc_make_bound)
+// instead of (k-th d~) + 2 eps.  Phase 1 re-scores the k candidates of smallest d~ and sets T to their k-th exact
+// distance; phase 2 re-scores every other listed candidate with d~_i - E_i <= T (NaN included).  A candidate left out has
+// d >= d~_i - E_i > T, so it is behind k re-scored ones.  The certificate then needs d~_{k'} > T + E_max(q), T the k-th
+// exact distance of the re-scored set: every unselected row has d >= d~ - E_max >= d~_{k'} - E_max > T.
 template <int ELEM, int METRIC, bool LIST>
 __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows, size_t stride, int V,
                                                                 const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
@@ -1030,7 +1048,9 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
                                                                 const int32_t* __restrict__ seg_len, const int32_t* __restrict__ probe_lists,
                                                                 const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
                                                                 int32_t* __restrict__ out_pos, float* __restrict__ out_key,
-                                                                int* __restrict__ n_failed, int32_t* __restrict__ fail_list) {
+                                                                int* __restrict__ n_failed, int32_t* __restrict__ fail_list,
+                                                                const float* __restrict__ xn, const float* __restrict__ r8,
+                                                                const float4* __restrict__ coef, unsigned long long* __restrict__ counters) {
     extern __shared__ uint64_t cr_smem[];
     uint64_t* cand = cr_smem;                                                   // [SS_CAND]
     uint64_t* fin = cand + SS_CAND;                                             // [kp] final keys
@@ -1070,11 +1090,14 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
     // per-probe candidate offsets and list bounds are in shared memory already.
     const int32_t* co = cand_off + (int64_t)q * (probes + 1);
     const SsWork W = ss_work_layout(work, cap_s, probes);
+    // LIST: d~_i - E_i of every listed candidate, in fin's storage until the ranking below
+    float* lb = reinterpret_cast<float*>(fin);
     for (int i = tid; i < kp; i += SS_THREADS) {
         exact[i] = __int_as_float(0x7F800000);
         rowp[i] = rows;
         if (i < have) {
             const int32_t ps = (int32_t)(uint32_t)cand[i];
+            int64_t g;                                        // row of the (list-ordered) table
             if (smin) {
                 int lo = 0, hi = probes;
                 while (hi - lo > 1) {
@@ -1083,7 +1106,7 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
                     else hi = mid;
                 }
                 // (empty lists share an offset with their successor: the search ends on the last of them, the non-empty one)
-                rowp[i] = rows + (size_t)(W.lo[lo] + (ps - W.co[lo])) * stride;
+                g = W.lo[lo] + (ps - W.co[lo]);
             } else {
                 int lo = 0, hi = probes;
                 while (hi - lo > 1) {
@@ -1093,21 +1116,60 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
                 }
                 while (lo + 1 < probes && co[lo + 1] <= ps) ++lo;   // empty lists share an offset
                 const int l = probe_lists[(int64_t)q * probes + lo];
-                rowp[i] = rows + (size_t)(list_off[l] + (ps - co[lo])) * stride;
+                g = list_off[l] + (ps - co[lo]);
+            }
+            rowp[i] = rows + (size_t)g * stride;
+            if (LIST) {
+                // E_i = a R_x + b X_x + c X_x^2 + d with X_x = |x| (1 + 2^-10) + R_x, every step rounded up (lc_make_bound)
+                const float4 cf = coef[q];
+                const float R = r8[g];
+                const float X = __fadd_ru(__fmul_ru(__fsqrt_ru(xn[g]), 1.0f + 1.0f / 1024.0f), R);
+                const float E = __fmaf_ru(cf.z, __fmul_ru(X, X), __fmaf_ru(cf.y, X, __fmaf_ru(cf.x, R, cf.w)));
+                lb[i] = key_to_float((uint32_t)(cand[i] >> 32)) - E;
             }
         }
     }
     __syncthreads();
-    // ---- exact re-score of the candidates with approx <= T (NaN compares false: re-scored too), one row per warp
-    for (int i = warp; i < have; i += SS_THREADS / 32) {
-        const float a = key_to_float((uint32_t)(cand[i] >> 32));
-        if (a > T) continue;                                 // warp-uniform
+    auto rescore = [&](int i) {
         const uint4* rp = reinterpret_cast<const uint4*>(rowp[i]);
         Acc<ELEM, METRIC> acc;
 #pragma unroll 4
         for (int v = lane; v < V; v += 32) acc.add(__ldg(rp + v), sq, v);
         acc.template reduce<32>();
         if (lane == 0) exact[i] = (float)acc.value();
+    };
+    __shared__ float s_tk;                                   // LIST: the k-th exact distance of the re-scored set
+    if (!LIST) {
+        // ---- exact re-score of the candidates with approx <= T (NaN compares false: re-scored too), one row per warp
+        for (int i = warp; i < have; i += SS_THREADS / 32) {
+            const float a = key_to_float((uint32_t)(cand[i] >> 32));
+            if (a > T) continue;                             // warp-uniform
+            rescore(i);
+        }
+    } else {
+        // ---- phase 1: the k smallest d~; T1 = the k-th exact distance (+inf when fewer than k, or one is NaN)
+        const float inf = __int_as_float(0x7F800000);
+        const int kk = min(k, have);
+        int n_rs = 0;                                        // rows this warp re-scored
+        for (int i = warp; i < kk; i += SS_THREADS / 32, ++n_rs) rescore(i);
+        __syncthreads();
+        float T1 = kk < k ? inf : -inf;
+        for (int i = 0; i < kk && T1 < inf; ++i) T1 = exact[i] == exact[i] ? fmaxf(T1, exact[i]) : inf;
+        // ---- phase 2: the others with d~_i - E_i <= T1 (fl(d~_i - E_i) > T1 implies d~_i - E_i > T1: rounding is monotone)
+        for (int i = kk + warp; i < have; i += SS_THREADS / 32) {
+            if (lb[i] > T1) continue;                        // warp-uniform; NaN is re-scored
+            rescore(i);
+            ++n_rs;
+        }
+        if (counters) {
+            // profiling: rows re-scored, and the rows the global bound would re-score (d~ <= d~_k + 2 eps(q))
+            if (lane == 0) atomicAdd(&counters[0], (unsigned long long)n_rs);
+            int n_glob = 0;
+            for (int i = tid; i < have; i += SS_THREADS) n_glob += !(key_to_float((uint32_t)(cand[i] >> 32)) > T);
+            n_glob = __reduce_add_sync(0xffffffffu, n_glob);
+            if (lane == 0) atomicAdd(&counters[1], (unsigned long long)n_glob);
+            if (tid == 0) atomicAdd(&counters[2], 1ull);
+        }
     }
     __syncthreads();
     // ---- order by (exact distance, position), emit the first k
@@ -1123,10 +1185,14 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
             out_pos[(int64_t)q * k + rank] = present ? (int32_t)(uint32_t)mine : -1;
             out_key[(int64_t)q * k + rank] = present ? key_to_float((uint32_t)(mine >> 32)) : __int_as_float(0x7F800000);
         }
+        if (LIST && rank == k - 1) s_tk = key_to_float((uint32_t)(mine >> 32));
     }
+    if (LIST) __syncthreads();
     // ---- certificate: candidates beyond the k' exist -> the last of the k' must already be above the threshold
     if (tid == 0 && n_run > kp) {
-        const bool ok = key_to_float((uint32_t)(thr >> 32)) > T;     // false for NaN
+        // (LIST: the threshold T + E_max(q) is rounded up, E_max = eps(q) >= E_i of every row, from its square rounded up)
+        const float Tc = LIST ? __fadd_ru(s_tk, __fsqrt_ru(qn[q])) : T;
+        const bool ok = key_to_float((uint32_t)(thr >> 32)) > Tc;     // false for NaN
         if (!ok) {
             const int i = atomicAdd(n_failed, 1);
             if (LIST) fail_list[i] = q;
@@ -1143,9 +1209,11 @@ __global__ void __launch_bounds__(SS_THREADS) cta_refine_kernel(const uint8_t* _
                                                                 const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
                                                                 int32_t* __restrict__ out_pos, float* __restrict__ out_key,
                                                                 int* __restrict__ n_failed) {
-    cta_refine_body<ELEM, METRIC, false>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, nullptr);
+    cta_refine_body<ELEM, METRIC, false>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, nullptr,
+                                         nullptr, nullptr, nullptr, nullptr);
 }
-// level 0: also lists the uncertified queries (fail_list[0 .. *n_failed)), which are then run again on their own
+// level 0: the per-row re-score rule (xn, r8: the image's |x|^2 and residuals; coef: l0_query_kernel's coefficients;
+// counters: profiling, or null), and the uncertified queries listed (fail_list[0 .. *n_failed)), then run again on their own
 template <int ELEM, int METRIC>
 __global__ void __launch_bounds__(SS_THREADS) cta_refine_list_kernel(const uint8_t* __restrict__ rows, size_t stride, int V,
                                                                 const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
@@ -1154,8 +1222,11 @@ __global__ void __launch_bounds__(SS_THREADS) cta_refine_list_kernel(const uint8
                                                                 const int32_t* __restrict__ seg_len, const int32_t* __restrict__ probe_lists,
                                                                 const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
                                                                 int32_t* __restrict__ out_pos, float* __restrict__ out_key,
-                                                                int* __restrict__ n_failed, int32_t* __restrict__ fail_list) {
-    cta_refine_body<ELEM, METRIC, true>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, fail_list);
+                                                                int* __restrict__ n_failed, int32_t* __restrict__ fail_list,
+                                                                const float* __restrict__ xn, const float* __restrict__ r8,
+                                                                const float4* __restrict__ coef, unsigned long long* __restrict__ counters) {
+    cta_refine_body<ELEM, METRIC, true>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, fail_list,
+                                        xn, r8, coef, counters);
 }
 
 // Bytes one launch of list_tc_kernel moves, from the same job list the kernel walks (profiling only):
@@ -1190,7 +1261,15 @@ enum { WSC_B = 21, WSC_N = 22, WSC_K = 23 };
 // c_sum of lc_make_bound: the fp32 norms, the final sum and the exact distance, relative to |x|^2 + |q|^2
 static float lc_c_sum(int dim) { return std::max(1.0f / 65536.0f, 3.0f * ((float)dim / 32.0f + 8.0f) / 16777216.0f); }
 
-static unsigned long long* g_traffic = nullptr;   // device accumulators of lc_traffic_kernel, per filter use (0 = lists, 1 = centres)
+// level 0's per-row bound coefficients: the float4 array after eps(q)^2 in launch_list_tc's WSC_N workspace, which hands
+// the refine kernels eps(q)^2 (qe2) for the batch's nq queries
+static float4* l0_row_coef(const float* qe2, int64_t nq) {
+    return reinterpret_cast<float4*>(((uintptr_t)(qe2 + nq) + 15) & ~(uintptr_t)15);
+}
+
+// device accumulators: [0..3] / [4..7] lc_traffic_kernel per filter use (lists / centres), [8..10] the level-0 refine's
+// counters (list_tc_level0_rescored)
+static unsigned long long* g_traffic = nullptr;
 static bool g_traffic_on = false;
 
 bool list_tc_supported(int elem, int key_metric, int k) {
@@ -1255,6 +1334,7 @@ int list_tc_prepare_l0(const Table& rows, ListTcImage* im) {
     const int64_t n_padded = im->n_tiles * LC_M;
     VB_CUDA(cudaMalloc(&im->planes8, std::max<size_t>((size_t)im->n_tiles * n_kblocks8 * LC_A_PLANE, 16)));
     VB_CUDA(cudaMalloc(&im->xs, sizeof(float) * (size_t)std::max<int64_t>(n_padded, 1)));
+    VB_CUDA(cudaMalloc(&im->r8, sizeof(float) * (size_t)std::max<int64_t>(n_padded, 1)));
     im->n_kblocks8 = n_kblocks8;
     im->rmax = 0.f;
     if (rows.n == 0) return VB_OK;
@@ -1263,9 +1343,11 @@ int list_tc_prepare_l0(const Table& rows, ListTcImage* im) {
     VB_CUDA(cudaMemsetAsync(d_rmax, 0, sizeof(unsigned), s));
     const unsigned grid = (unsigned)((n_padded * 32 + 255) / 256);
     if (rows.elem == VB_VECTOR)
-        pack_rows_i8_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(rows.d, rows.stride, rows.n, rows.dim, n_kblocks8, n_padded, im->planes8, im->xs, d_rmax);
+        pack_rows_i8_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(rows.d, rows.stride, rows.n, rows.dim, n_kblocks8, n_padded, im->planes8, im->xs,
+                                                            im->r8, d_rmax);
     else
-        pack_rows_i8_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(rows.d, rows.stride, rows.n, rows.dim, n_kblocks8, n_padded, im->planes8, im->xs, d_rmax);
+        pack_rows_i8_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(rows.d, rows.stride, rows.n, rows.dim, n_kblocks8, n_padded, im->planes8, im->xs,
+                                                             im->r8, d_rmax);
     VB_CUDA(cudaGetLastError());
     count_launch();
     unsigned bits = 0;
@@ -1279,6 +1361,7 @@ int list_tc_prepare_l0(const Table& rows, ListTcImage* im) {
 void list_tc_release(ListTcImage* im) {
     if (im->planes8) cudaFree(im->planes8);
     if (im->xs) cudaFree(im->xs);
+    if (im->r8) cudaFree(im->r8);
     if (im->planes) cudaFree(im->planes);
     if (im->xn) cudaFree(im->xn);
     if (im->units) cudaFree(im->units);
@@ -1298,8 +1381,9 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
     // (level 0: the B tiles take half of this, the packed queries q8 follow them)
     const size_t q8_bytes = level == 0 ? (size_t)nq * 2 * im.n_kblocks8 * 128 : 0;
     VB_TRY(workspace(WSC_B, (size_t)max_gtiles * im.n_kblocks * LC_B_STAGE + q8_bytes, &d_B));
-    // [|q|^2 | level 0: t_q | level 0: eps(q)^2], one size for every level so that the |q|^2 cache below stays put
-    VB_TRY(workspace(WSC_N, sizeof(float) * (size_t)nq * 3 + 64, &d_qn));
+    // [|q|^2 | level 0: t_q | level 0: eps(q)^2 | level 0: per-row bound coefficients (l0_row_coef)], one size for every
+    // level so that the |q|^2 cache below stays put
+    VB_TRY(workspace(WSC_N, sizeof(float) * (size_t)nq * 3 + 16 + sizeof(float4) * (size_t)nq + 64, &d_qn));
     float* d_tq = (float*)d_qn + nq;
     float* d_qe2 = d_tq + nq;
     // the query image is fp32 with the rows' padded dimension count for both element types
@@ -1329,7 +1413,7 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
         int8_t* q8 = (int8_t*)d_B + (size_t)max_gtiles * n_kblocks * LC_B_STAGE;
         l0_query_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, s>>>((const float*)qimg, qstride, std::min(qdim, qpad), qpad, nq, im.xmax,
                                                                           im.rmax, key_metric == VB_L2_SQUARED, lc_c_sum(rows.dim), d_tq,
-                                                                          d_qe2, q8);
+                                                                          d_qe2, l0_row_coef(d_qe2, nq), q8);
         pack_groups_i8_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>(q8, qpad, n_kblocks, g.n_pairs, g.pair_q, g.pair_list,
                                                                                g.begin, g.gt_begin, (uint8_t*)d_B);
         count_launch();
@@ -1386,8 +1470,8 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
 int list_tc_traffic(int on, int64_t* out8) {
     cudaStream_t s = ctx().stream;
     if (!g_traffic) {
-        VB_CUDA(cudaMalloc(&g_traffic, 8 * sizeof(unsigned long long)));
-        VB_CUDA(cudaMemsetAsync(g_traffic, 0, 8 * sizeof(unsigned long long), s));
+        VB_CUDA(cudaMalloc(&g_traffic, 11 * sizeof(unsigned long long)));
+        VB_CUDA(cudaMemsetAsync(g_traffic, 0, 11 * sizeof(unsigned long long), s));
     }
     if (out8) {
         VB_CUDA(cudaMemcpyAsync(out8, g_traffic, 8 * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
@@ -1395,6 +1479,16 @@ int list_tc_traffic(int on, int64_t* out8) {
         VB_CUDA(cudaMemsetAsync(g_traffic, 0, 8 * sizeof(unsigned long long), s));
     }
     g_traffic_on = on != 0;
+    return VB_OK;
+}
+
+int list_tc_level0_rescored(int64_t* out3) {
+    cudaStream_t s = ctx().stream;
+    for (int i = 0; i < 3; ++i) out3[i] = 0;
+    if (!g_traffic) return VB_OK;
+    VB_CUDA(cudaMemcpyAsync(out3, g_traffic + 8, 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    VB_CUDA(cudaMemsetAsync(g_traffic + 8, 0, 3 * sizeof(unsigned long long), s));
     return VB_OK;
 }
 
@@ -1418,6 +1512,22 @@ int list_tc_traffic(int on, int64_t* out8) {
 // L2: twice the dot term plus c_sum (X^2 + |q|^2) (the norms, the final sum, the exact distance, as at levels 1 / 2); the
 // inner product: the dot term plus 2^-17 X |q|.  The sums are taken in double, the result widened by 2^-10 and rounded up.
 // It reaches the refine kernels as eps(q)^2 in the place of |q|^2, with the unit bound below: lc_eps() = sqrt(eps(q)^2).
+//
+// Per row (the level-0 refine's re-score rule).  Every step above holds for one row with its own r_x in the place of R
+// and |x| in the place of xmax: |x^| <= |x| + r_x, the epilogue's roundings are <= 2^-21 |x^| t_q (|q_hi| + |q_lo| / 254),
+// and the norm term is c_sum (|x|^2 + |q|^2).  So with R_x = r8[x] >= r_x (pack_rows_i8_kernel: sqrt of the double sum,
+// widened by 2^-20, rounded up) and X_x = |x| (1 + 2^-10) + R_x:
+//   E(x, q) = [2 (R_x |q| + X_x r_q + X_x qabs 2^-20) + c_sum (X_x^2 + |q|^2)] (1 + 2^-10)          (L2; +2e-30)
+//   E(x, q) = [R_x |q| + X_x r_q + X_x qabs 2^-20 + X_x |q| 2^-17] (1 + 2^-10)                       (inner product)
+// E_max = eps(q) is E at R_max and xmax.  |x| comes from the fp32 |x|^2 of the image (xn), whose relative error
+// (dim / 32 + 5) 2^-24 is far below the 2^-10 on |x|.  l0_query_kernel splits E = a R_x + b X_x + c X_x^2 + d, computing
+// a, b, c, d in double with the factor 2^-10 folded in and rounding each up to fp32; the refine evaluates X_x and E
+// with every fp32 operation rounded up (__fsqrt_ru, __fmul_ru, __fadd_ru, __fmaf_ru on non-negative terms), so its E_i
+// >= E(x, q).  It then forms fl(d~_i - E_i) in round-to-nearest and skips the row when that is > T: rounding is monotone
+// and T is an fp32 value, so fl(d~_i - E_i) > T implies d~_i - E_i > T exactly, and d_fp32 >= d~_i - E_i > T.  The
+// certificate compares d~_{k'} with fl_ru(T + sqrt_ru(eps(q)^2)) >= T + eps(q).  NaN anywhere re-scores the row or
+// fails the certificate.  (tests/test_level0_rowbound.py checks |d~ - d| <= E against float64 on rows with mixed
+// residuals.)
 
 static LcBound lc_make_bound(const Table& rows, const ListTcImage& im, int key_metric, int level) {
     LcBound bound;
@@ -1538,6 +1648,7 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
     const size_t smem = (size_t)SS_CAND * 8 + (size_t)kp * 16 + qstride + (smin ? ss_select_smem_bytes(cap_s, probes) : (size_t)cap * 4) +
                         (size_t)kp * 4 + 16;
     VB_REQUIRE(kp <= 256 && smem <= 200 * 1024 && (smin || cap <= SS_CAND), "cta_refine: k' = %d / %zu bytes of shared memory not supported", kp, smem);
+    VB_REQUIRE(!fail_list || (level == 0 && im.r8), "cta_refine: the listing kernel is level 0's and needs its int8 image");
 #define VB_CR(E, M)                                                                                                              \
     do {                                                                                                                         \
         if (fail_list) {                                                                                                         \
@@ -1545,7 +1656,8 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
             if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
             kern<<<(unsigned)nq, SS_THREADS, smem, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, k, kp, probes, bound, qn, dist, \
                                                        smin, cap, cap_s, seg_len, d_lists, cand_off, d_list_off, out_pos, out_key, fail_dev, \
-                                                       fail_list);                                                              \
+                                                       fail_list, im.xn, im.r8, l0_row_coef(qn, nq),                             \
+                                                       g_traffic_on ? g_traffic + 8 : nullptr);                                 \
             break;                                                                                                               \
         }                                                                                                                        \
         auto kern = cta_refine_kernel<E, M>;                                                                                     \

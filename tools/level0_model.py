@@ -16,6 +16,13 @@ It reports R_max (absolute and relative to |x|), eps(q) against level 1's, the f
 re-scored rows per query, for k' = 64 and 128.  (d~ is evaluated in float64 here; the kernel's fp32 epilogue differs from
 it by far less than the bound's rounding terms.)
 
+It also evaluates the rule the level-0 refine uses, with each row's own bound E(x, q) (R_x and |x| in the place of R_max
+and x_max) and an exact threshold:
+    re-score the k smallest d~, T1 = their k-th exact distance; re-score the other listed ones with d~ - E(x, q) <= T1;
+    T = the k-th exact distance of the re-scored set; a query fails when it has more than k' candidates and the k'-th
+    smallest d~ is <= T + eps(q),
+and reports its re-scored rows per query and its failures for k' = 32, 64 and 128.
+
     python tools/level0_model.py [--rows N --dim D --lists L --probes P --queries Q --law rank16|mixture]
 """
 from __future__ import annotations
@@ -95,7 +102,12 @@ def main():
 
     fails = {64: 0, 128: 0}
     rescored = {64: [], 128: []}
+    row_fails = {32: 0, 64: 0, 128: 0}
+    row_rescored = []
     eps0, eps1 = [], []
+    w = 1 + 1 / 1024
+    res_up = res * (1 + 1 / 1048576)
+    Xrow = xnorm * w + res_up
     for qi in range(a.queries):
         q = queries[qi]
         lists, _ = oix.scan_lists(q, a.probes)
@@ -112,6 +124,23 @@ def main():
         eps1.append(e1)
         xi = x8[cand].astype(np.float64)
         approx = xn[cand] + n2 - 2 * sx[cand].astype(np.float64) * float(tq) * (xi @ h.astype(np.float64) + (xi @ lo.astype(np.float64)) / 254)
+        # the per-row rule (l0_query_kernel's coefficients, cta_refine_body's two phases)
+        order = np.argsort(approx, kind="stable")
+        sa = approx[order]
+        top = cand[order[:128]]
+        exact = ((grouped[top].astype(np.float64) - q) ** 2).sum(1)
+        dq = rq + qabs / 1048576
+        Xc = Xrow[top]
+        lb = sa[:128] - w * (2 * np.sqrt(n2) * res_up[top] + 2 * dq * Xc + c_sum * Xc * Xc + c_sum * n2 + 2e-30)
+        kk = min(a.k, len(sa))
+        T1 = exact[:kk].max() if kk == a.k else np.inf
+        for kp in (32, 64, 128):
+            sel = np.concatenate([np.arange(kk), kk + np.flatnonzero(~(lb[kk:kp] > T1))])
+            T = np.sort(exact[sel])[a.k - 1] if len(sel) >= a.k else np.inf
+            if kp == 128:
+                row_rescored.append(len(sel))
+            if len(sa) > kp and not sa[kp - 1] > T + e0:
+                row_fails[kp] += 1
         approx.sort()
         for kp in (64, 128):
             top = approx[:kp]
@@ -130,6 +159,11 @@ def main():
         "failures_per_2048_batch": {str(kp): per_batch(fails[kp]) for kp in fails},
         "failure_fraction": {str(kp): fails[kp] / a.queries for kp in fails},
         "rescored_rows_per_query_mean": {str(kp): float(np.mean(rescored[kp])) for kp in rescored},
+        "per_row_rule": {
+            "rescored_rows_per_query_mean": float(np.mean(row_rescored)),
+            "rescored_rows_per_query_p90": float(np.percentile(row_rescored, 90)),
+            "failures_per_2048_batch": {str(kp): per_batch(row_fails[kp]) for kp in row_fails},
+        },
     }))
 
 
