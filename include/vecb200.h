@@ -196,6 +196,7 @@ int			vb_table_rerank_dev(vb_table *t, int metric, const void *queries_dev, int6
  * Duplicates collapse.  n == 0 is an empty filter.  Using a filter with a table or index other than its own fails with
  * VB_EINVAL, also after its own was freed (every table and image carries a process-wide unique stamp).  The exact top-k
  * takes filters of fewer than 2^31 rows.  Creation synchronises (it reads back the number of allowed rows); the caller's arrays may be reused at once.
+ * HNSW images take element filters (vb_hnsw_filter_create, with the HNSW scan below).
  */
 typedef struct vb_filter vb_filter;
 struct vb_ivf;	/* the IVFFlat image, below */
@@ -597,6 +598,38 @@ int			vb_hnsw_scan_begin(vb_hnsw *h, const void *queries, int64_t nq, int ef_sea
 int			vb_hnsw_scan_next(vb_hnsw_scan *scan, int64_t *out_ids, double *out_distances, int32_t *out_counts);
 int			vb_hnsw_scan_tuples(vb_hnsw_scan *scan, int64_t *out_tuples);	/* [nq] the tuples counters */
 int			vb_hnsw_scan_end(vb_hnsw_scan *scan);
+
+/*
+ * Element filters of an HNSW image (see vb_filter above): elements = element numbers in [0, n).  Host variant: a value
+ * out of range fails with VB_EINVAL naming its position and value; _dev variant: such values are ignored.  Duplicates
+ * collapse, n == 0 is an empty filter; vb_filter_rows and vb_filter_free apply.  The image holds no heap TIDs: the caller
+ * allows an element when any of its heap TIDs passes (a row a GPU build folded into another element, dup_of, is reached
+ * through that element) and withholds the rejected TIDs of an element the scan returns (INTEGRATION.md section 7c).
+ * A filter is refused (VB_EINVAL) by any other index, table or IVFFlat image, also after its own was freed, and an HNSW
+ * filter by their entry points; after vb_hnsw_load / vb_hnsw_build* of its image, begin fails with VB_ESTATE ("index
+ * changed since the filter was created").
+ */
+int			vb_hnsw_filter_create(vb_hnsw *h, const int64_t *elements, int64_t n, vb_filter **out);
+int			vb_hnsw_filter_create_dev(vb_hnsw *h, const int64_t *elements_dev, int64_t n, vb_filter **out);
+
+/*
+ * The iterative scan with an element filter per query: query q uses filters[filter_of_query[q]] (host array; NULL when
+ * nfilters == 1; an entry out of range fails with VB_EINVAL naming the query).  Let S_q be the unfiltered handle's
+ * sequence (its batches concatenated until out_counts == 0).  The filtered sequence is S_q restricted to the allowed
+ * elements: same order, same element numbers, same float8 distances bit for bit.  The traversal is the unfiltered one:
+ * rejected elements are visited, expanded, counted in `tuples` and kept as discarded candidates, as in the reference,
+ * where the predicate is applied above the index.
+ * vb_hnsw_scan_next on this handle writes out_ids / out_distances [nq x page] (1 <= page <= 2048, -1 / +inf padded):
+ * the next min(page, remaining) allowed elements of each query, across underlying batches; out_counts[q] < page only
+ * when the sequence is exhausted, and 0 (for good) once it is.  Underlying batches run inside the call, only while the
+ * page is not full: after a call that fills its page, tuples equals the unfiltered handle's after the batch holding the
+ * call's last element; after one that does not, the scan has run to its end.  Begin copies the filters' bitsets (the
+ * filters may be freed at once) and counts them in the VB_ENOMEM check.  next fails with VB_ESTATE, writing nothing,
+ * once the image has been loaded or built again.  vb_hnsw_scan_tuples and vb_hnsw_scan_end are shared.
+ */
+int			vb_hnsw_scan_begin_filtered(vb_hnsw *h, const void *queries, int64_t nq, int ef_search,
+										int64_t max_scan_tuples, int page, const vb_filter *const *filters, int nfilters,
+										const int32_t *filter_of_query, vb_hnsw_scan **out);
 
 #ifdef __cplusplus
 }

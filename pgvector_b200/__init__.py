@@ -577,9 +577,10 @@ class IvfflatScan:
 # --------------------------------------------------------------------- row filters
 
 class Filter:
-    """A row filter: the allowed rows of one Table (row numbers) or one IvfflatIndex (heap ids), resident on the device
-    -- what a B-tree or bitmap scan on a filter column yields for WHERE <predicate> ORDER BY v <op> q LIMIT k.  Made by
-    Table.filter / IvfflatIndex.filter; len() = rows allowed.  Free it (or use it as a context manager) when done."""
+    """A row filter: the allowed rows of one Table (row numbers), one IvfflatIndex (heap ids) or one HnswIndex (element
+    numbers), resident on the device -- what a B-tree or bitmap scan on a filter column yields for WHERE <predicate>
+    ORDER BY v <op> q LIMIT k.  Made by Table.filter / IvfflatIndex.filter / HnswIndex.filter; len() = rows allowed.
+    Free it (or use it as a context manager) when done."""
 
     def __init__(self, owner, h):
         self.owner, self.h = owner, h
@@ -768,10 +769,21 @@ class HnswIndex:
         _lib.check(load().vb_hnsw_search_dev(self.h, _ptr(queries_dev), queries_dev.shape[0], int(ef), int(k),
                                              _ptr(ids_dev), _ptr(dist_dev), _ptr(nd_dev)))
 
-    def iterative_scan(self, queries, ef_search=None, max_scan_tuples=20000):
+    def filter(self, elements):
+        """an element Filter of this index: the allowed element numbers (numpy array, or a torch CUDA int64 tensor whose
+        values outside [0, n) are ignored).  It is refused once the index is loaded or built again."""
+        return Filter._create(self, "vb_hnsw_filter_create", elements)
+
+    def iterative_scan(self, queries, ef_search=None, max_scan_tuples=20000, filter=None, filter_of_query=None, page=None):
         """hnsw.iterative_scan for a batch of queries: an HnswScan whose next_batch() mirrors ResumeScanItems
-        (src/hnswscan.c:62-87); max_scan_tuples mirrors hnsw.max_scan_tuples (src/hnsw.c:101-105)."""
-        return HnswScan(self, queries, int(ef_search or self.ef_search), int(max_scan_tuples))
+        (src/hnswscan.c:62-87); max_scan_tuples mirrors hnsw.max_scan_tuples (src/hnsw.c:101-105).  filter: a Filter of
+        this index, or a list of them with filter_of_query[q] = the index of query q's filter: next_batch() then returns
+        the next `page` (default ef_search) elements of each query's sequence that its filter allows."""
+        ef = int(ef_search or self.ef_search)
+        if filter is None and page is not None:
+            raise ValueError("page applies to a filtered scan only (an unfiltered scan returns ef_search per batch)")
+        return HnswScan(self, queries, ef, int(max_scan_tuples), filter=filter, filter_of_query=filter_of_query,
+                        page=ef if page is None else int(page))
 
     def free(self):
         if self.h:
@@ -787,20 +799,31 @@ class HnswIndex:
 
 class HnswScan:
     """One iterative index scan per query (src/hnswscan.c:228-340): next_batch() returns (ids, distances, counts) of
-    the next <= ef_search elements of every query, nearest first; counts == 0 marks an exhausted scan."""
+    the next <= ef_search elements of every query, nearest first; counts == 0 marks an exhausted scan.  With a filter,
+    the next <= page allowed elements, counts < page only once the sequence is exhausted."""
 
-    def __init__(self, index, queries, ef, max_scan_tuples):
+    def __init__(self, index, queries, ef, max_scan_tuples, filter=None, filter_of_query=None, page=None):
         q = _host(index.elem, queries)
         if q.ndim == 1:
             q = q.reshape(1, -1)
         self.index, self.nq, self.ef = index, q.shape[0], ef
+        self.h = None
         h = C.c_void_p()
-        _lib.check(load().vb_hnsw_scan_begin(index.h, _ptr(q), self.nq, ef, max_scan_tuples, C.byref(h)))
+        if filter is None:
+            self.width = ef
+            _lib.check(load().vb_hnsw_scan_begin(index.h, _ptr(q), self.nq, ef, max_scan_tuples, C.byref(h)))
+        else:
+            self.width = int(page)
+            farr, nf, fq = _filter_args(filter, filter_of_query)
+            if fq is not None and len(fq) != self.nq:
+                raise ValueError(f"filter_of_query must have {self.nq} entries, got {len(fq)}")
+            _lib.check(load().vb_hnsw_scan_begin_filtered(index.h, _ptr(q), self.nq, ef, max_scan_tuples, self.width, farr, nf,
+                                                          _ptr(fq), C.byref(h)))
         self.h = h
 
     def next_batch(self):
-        ids = np.empty((self.nq, self.ef), dtype=np.int64)
-        dist = np.empty((self.nq, self.ef), dtype=np.float64)
+        ids = np.empty((self.nq, self.width), dtype=np.int64)
+        dist = np.empty((self.nq, self.width), dtype=np.float64)
         cnt = np.empty(self.nq, dtype=np.int32)
         _lib.check(load().vb_hnsw_scan_next(self.h, _ptr(ids), _ptr(dist), _ptr(cnt)))
         return ids, dist, cnt

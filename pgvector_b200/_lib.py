@@ -122,6 +122,9 @@ SIGNATURES = {
     "vb_hnsw_scan_next": (_i, [_vp, _vp, _vp, _vp]),
     "vb_hnsw_scan_tuples": (_i, [_vp, _vp]),
     "vb_hnsw_scan_end": (_i, [_vp]),
+    "vb_hnsw_filter_create": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
+    "vb_hnsw_filter_create_dev": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
+    "vb_hnsw_scan_begin_filtered": (_i, [_vp, _vp, _i64, _i, _i64, _i, _vp, _i, _vp, C.POINTER(_vp)]),
 }
 
 

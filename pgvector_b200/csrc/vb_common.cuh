@@ -277,28 +277,35 @@ int launch_ivf_filter_lists(int64_t nq, int max_probes, int lists, const int32_t
 
 // ---------------------------------------------------------------- row filters (vb_filter.cu)
 // The allowed rows of one table or one IVFFlat image, ascending.  An IVFFlat image stores rows grouped by list, so the
-// allowed rows of list l are one run pos[off[l] .. off[l + 1]).
-// process-wide unique stamp of a table or IVFFlat image: a filter matches its owner by address and stamp, so a filter
-// that outlived its owner is refused even when a new owner is allocated at the same address
+// allowed rows of list l are one run pos[off[l] .. off[l + 1]).  The allowed elements of an HNSW image are a bitset:
+// its iterative scan tests the elements a traversal returns, it never enumerates the allowed ones.
+// process-wide unique stamp of a table, IVFFlat or HNSW image: a filter matches its owner by address and stamp, so a
+// filter that outlived its owner is refused even when a new owner is allocated at the same address
 uint64_t next_owner_uid();
+enum FilterKind { FILTER_TABLE, FILTER_IVF, FILTER_HNSW };
 struct Filter {
-    const void* owner = nullptr;   // the vb_table or vb_ivf it was made for
+    const void* owner = nullptr;   // the vb_table, vb_ivf or vb_hnsw it was made for
     uint64_t owner_uid = 0;        // and that owner's stamp
-    bool ivf = false;
-    uint64_t generation = 0;       // IVFFlat: Ivf::generation at creation
+    FilterKind kind = FILTER_TABLE;
+    uint64_t generation = 0;       // IVFFlat / HNSW: the image's generation at creation
     int64_t n = 0;                 // rows allowed
     int lists = 0;
-    void* mem = nullptr;           // one allocation: pos | ids | off
+    void* mem = nullptr;           // one allocation: pos | ids | off (HNSW: bits)
     int64_t* pos = nullptr;        // [n] table: row numbers; IVFFlat: rows of the list-ordered image
     int64_t* ids = nullptr;        // [n] IVFFlat: the heap ids of pos
     int64_t* off = nullptr;        // [lists + 1] IVFFlat: per-list runs of pos
     std::vector<int64_t> h_off;    // host copy of off (allowed counts per list: sizes a scan handle's group buffers)
+    uint32_t* bits = nullptr;      // HNSW: [words] bit e = element e is allowed
+    int64_t words = 0;
 };
 // table: rows = row numbers (values outside [0, n_rows) ignored; the host variant validates before this call)
 int filter_build_table(int64_t n_rows, const int64_t* rows, int64_t n, bool host, Filter* f);
 // IVFFlat image of n_rows rows: image_ids = heap ids of the rows (nullptr: row positions), list_off [lists + 1] device
 int filter_build_ivf(int64_t n_rows, const int64_t* image_ids, const int64_t* list_off, int lists, const int64_t* ids, int64_t n,
                      bool host, Filter* f);
+// HNSW image of n_elems elements: elems = element numbers (values outside [0, n_elems) ignored; the host variant
+// validates before this call)
+int filter_build_hnsw(int64_t n_elems, const int64_t* elems, int64_t n, bool host, Filter* f);
 void filter_release(Filter* f);
 
 int list_tile_rows();

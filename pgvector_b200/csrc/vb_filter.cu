@@ -151,6 +151,7 @@ void filter_release(Filter* f) {
     if (f->mem) cudaFree(f->mem);
     f->mem = nullptr;
     f->pos = f->ids = f->off = nullptr;
+    f->bits = nullptr;
 }
 
 // Temporaries of a build: one allocation, freed before returning (construction is off the scan's hot path).
@@ -177,7 +178,8 @@ static int filter_compact(int64_t n_rows, uint32_t* bits, int64_t* block_sum, co
     VB_CUDA(cudaMemcpyAsync(&f->n, block_sum + nb, sizeof(int64_t), cudaMemcpyDeviceToHost, c.stream));
     VB_CUDA(cudaStreamSynchronize(c.stream));
     const size_t n_pos = (size_t)std::max<int64_t>(f->n, 1);
-    const size_t bytes = 8 * n_pos * (f->ivf ? 2 : 1) + (f->ivf ? 8 * ((size_t)f->lists + 1) : 0);
+    const bool ivf = f->kind == FILTER_IVF;
+    const size_t bytes = 8 * n_pos * (ivf ? 2 : 1) + (ivf ? 8 * ((size_t)f->lists + 1) : 0);
     if (cudaMalloc(&f->mem, bytes) != cudaSuccess) {
         cudaGetLastError();
         f->mem = nullptr;
@@ -185,12 +187,12 @@ static int filter_compact(int64_t n_rows, uint32_t* bits, int64_t* block_sum, co
         return VB_ENOMEM;
     }
     f->pos = (int64_t*)f->mem;
-    f->ids = f->ivf ? f->pos + n_pos : nullptr;
-    f->off = f->ivf ? f->ids + n_pos : nullptr;
+    f->ids = ivf ? f->pos + n_pos : nullptr;
+    f->off = ivf ? f->ids + n_pos : nullptr;
     filter_write_kernel<<<(unsigned)nb, FB_THREADS, 0, c.stream>>>(bits, nwords, block_sum, image_ids, f->pos, f->ids);
     VB_CUDA(cudaGetLastError());
     count_launch();
-    if (f->ivf) {
+    if (ivf) {
         filter_list_off_kernel<<<(unsigned)((f->lists + 1 + 255) / 256), 256, 0, c.stream>>>(list_off, f->lists, f->pos, block_sum + nb,
                                                                                             f->off);
         VB_CUDA(cudaGetLastError());
@@ -224,7 +226,7 @@ int filter_build_table(int64_t n_rows, const int64_t* rows, int64_t n, bool host
         VB_CUDA(cudaGetLastError());
         count_launch();
     }
-    f->ivf = false;
+    f->kind = FILTER_TABLE;
     return filter_compact(n_rows, bits, block_sum, nullptr, nullptr, f);
 }
 
@@ -258,9 +260,49 @@ int filter_build_ivf(int64_t n_rows, const int64_t* image_ids, const int64_t* li
         VB_CUDA(cudaGetLastError());
         count_launch();
     }
-    f->ivf = true;
+    f->kind = FILTER_IVF;
     f->lists = lists;
     return filter_compact(n_rows, bits, block_sum, image_ids, list_off, f);
+}
+
+// The bitset is the filter itself (the HNSW iterative scan tests one bit per returned element); only its count is
+// computed, by the first two steps of the compaction.
+int filter_build_hnsw(int64_t n_elems, const int64_t* elems, int64_t n, bool host, Filter* f) {
+    Context& c = ctx();
+    const int64_t nwords = std::max<int64_t>(1, (n_elems + 31) / 32);
+    const int64_t nb = (nwords + FB_THREADS - 1) / FB_THREADS;
+    f->kind = FILTER_HNSW;
+    f->words = nwords;
+    if (cudaMalloc(&f->mem, 4 * (size_t)nwords) != cudaSuccess) {
+        cudaGetLastError();
+        f->mem = nullptr;
+        set_error("row filter: allocation of %zu bytes failed", 4 * (size_t)nwords);
+        return VB_ENOMEM;
+    }
+    f->bits = (uint32_t*)f->mem;
+    FilterTmp tmp;
+    VB_CUDA(cudaMalloc(&tmp.mem, 8 * ((size_t)nb + 1) + (host ? 8 * (size_t)n : 0)));
+    int64_t* block_sum = (int64_t*)tmp.mem;
+    const int64_t* d_elems = elems;
+    if (host && n) {
+        int64_t* up = block_sum + nb + 1;
+        VB_CUDA(cudaMemcpyAsync(up, elems, 8 * (size_t)n, cudaMemcpyHostToDevice, c.stream));
+        d_elems = up;
+    }
+    VB_CUDA(cudaMemsetAsync(f->bits, 0, 4 * (size_t)nwords, c.stream));
+    if (n) {
+        filter_table_bits_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(d_elems, n, n_elems, f->bits);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    filter_count_kernel<<<(unsigned)nb, FB_THREADS, 0, c.stream>>>(f->bits, nwords, block_sum);
+    VB_CUDA(cudaGetLastError());
+    filter_scan_kernel<<<1, FB_THREADS, 0, c.stream>>>(block_sum, nb);
+    VB_CUDA(cudaGetLastError());
+    count_launch(2);
+    VB_CUDA(cudaMemcpyAsync(&f->n, block_sum + nb, sizeof(int64_t), cudaMemcpyDeviceToHost, c.stream));
+    VB_CUDA(cudaStreamSynchronize(c.stream));
+    return VB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- filtered exact top-k
@@ -320,7 +362,7 @@ static int exact_topk_filtered_impl(vb_table* t, int metric, const void* queries
     for (int i = 0; i < nfilters; ++i) {
         VB_REQUIRE(filters[i], "filtered top-k: filter %d is NULL", i);
         const Filter& f = filters[i]->f;
-        VB_REQUIRE(!f.ivf && f.owner == t && f.owner_uid == t->uid, "filtered top-k: filter %d was made for another table or index", i);
+        VB_REQUIRE(f.kind == FILTER_TABLE && f.owner == t && f.owner_uid == t->uid, "filtered top-k: filter %d was made for another table or index", i);
         VB_REQUIRE(f.n < (int64_t)INT32_MAX, "filtered top-k: filter %d allows %lld rows, at most %d", i, (long long)f.n, INT32_MAX - 1);
     }
     if (nq <= 0) return VB_OK;

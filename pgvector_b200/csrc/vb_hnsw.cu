@@ -378,6 +378,7 @@ int vb_hnsw_load(vb_hnsw* p, const void* rows, int64_t n, const int32_t* levels,
     VB_REQUIRE(p && n >= 0 && n < (int64_t)0x7fffffff, "bad hnsw load arguments");
     Hnsw& h = p->h;
     hnsw_release(h);
+    ++h.generation;
     h.n = n;
     h.entry = n > 0 ? entry : -1;
     if (n == 0) {

@@ -50,6 +50,7 @@ struct Hnsw {
     float *nd0 = nullptr, *upper_d = nullptr;
     int32_t *dup_of = nullptr, *n_heaptids = nullptr;
     int64_t upper_slots = 0;
+    uint64_t generation = 0;  // bumped by every load and build: filters and filtered scan handles refuse a changed image
 };
 
 void hnsw_release(Hnsw& h);
@@ -840,4 +841,5 @@ __device__ __forceinline__ bool hnsw_search_layer(const HnswDev& g, const uint4*
 
 struct vb_hnsw {
     vb::Hnsw h;
+    uint64_t uid = vb::next_owner_uid();   // matched by the element filters made for this image
 };

@@ -473,6 +473,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
     Context& c = ctx();
     cudaStream_t s = c.stream;
     hnsw_release(h);
+    ++h.generation;
     h.n = n;
     h.entry = -1;
     h.entry_level = -1;

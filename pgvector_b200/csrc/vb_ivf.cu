@@ -1792,7 +1792,7 @@ static int ivf_scan_begin_impl(const char* fn, vb_ivf* h, const void* queries, i
         for (int i = 0; i < nfilters; ++i) {
             VB_REQUIRE(filters[i], "%s: filter %d is NULL", fn, i);
             const Filter& f = filters[i]->f;
-            VB_REQUIRE(f.ivf && f.owner == h && f.owner_uid == h->uid, "%s: filter %d was made for another table or index", fn, i);
+            VB_REQUIRE(f.kind == FILTER_IVF && f.owner == h && f.owner_uid == h->uid, "%s: filter %d was made for another table or index", fn, i);
             if (f.generation != ix.generation) {
                 set_error("%s: filter %d: index changed since the filter was created", fn, i);
                 return VB_ESTATE;

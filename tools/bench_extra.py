@@ -13,6 +13,8 @@ does not cover: k-means assign on the tensor cores (config D shape, one GPU's sh
                                           (row filters on the device: filtered iterative scan and exact top-k vs host filtering)
     python tools/bench_extra.py level0   [--rows N --dim D --lists L --probes P --rounds R --law rank16|mixture --load S]
                                           (the batched list scan with filter level 0 (int8 rows) on and off, alternating)
+    python tools/bench_extra.py hnsw-filter [--rows N --dim D --ef EF --queries Q]
+                                          (element filters on the device for hnsw.iterative_scan vs host filtering)
 
 All timing with CUDA events on the library stream; inputs resident in HBM.
 """
@@ -636,6 +638,107 @@ def bench_filter(args):
     print(json.dumps(out))
 
 
+def bench_hnsw_filter(args):
+    """Element filters on the device against filtering on the host for hnsw.iterative_scan, at config C's shape: halfvec
+    cosine rows of bench_hnsw's low-intrinsic-dimension law, the graph built on the device (m 16), ef_search 100,
+    max_scan_tuples 20000, WHERE element % c = 0 LIMIT 10.
+    - host_filtered: the unfiltered handle, drained until every query has 10 matches (every call advances every query);
+    - device_filtered: the filtered handle with page = 10 (building the filter is counted).
+    The first 10 matches of every query are asserted identical."""
+    import torch
+    import pgvector_b200 as pv
+    pv.init(0)
+    dev = torch.device("cuda", 0)
+    n, dim, nq, ef, mst, limit = args.rows, args.dim, args.queries, args.ef, 20000, 10
+    g = torch.Generator(device=dev).manual_seed(6)
+    frame = torch.linalg.qr(torch.randn((dim, 16), generator=g, device=dev))[0]
+
+    def law(m):
+        x = torch.randn((m, 16), generator=g, device=dev) @ frame.T + 0.02 * torch.randn((m, dim), generator=g, device=dev)
+        return torch.nn.functional.normalize(x, dim=1).half()
+
+    rows = torch.cat([law(min(65536, n - i)) for i in range(0, n, 65536)])
+    q = law(nq).view(torch.int16).cpu().numpy().view(np.uint16)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    gi = pv.HnswIndex("halfvec_cosine_ops", dim, m=16).build(rows, ef_construction=64)
+    pv.synchronize()
+    build_s = time.perf_counter() - t0
+    del rows
+    dup = int((gi.export()["dup_of"] >= 0).sum())
+    out = {"bench": "hnsw-filter", "card": card(),
+           "workload": f"HNSW halfvec_cosine_ops {n}x{dim}, m=16 (built on the device in {build_s:.0f}s, {dup} folded duplicates), "
+                       f"ef_search={ef}, max_scan_tuples={mst}, {nq} queries, WHERE element % c = 0 LIMIT {limit}"}
+
+    def host_arm(c, tuples_each_call=False):
+        t0 = time.perf_counter()
+        sc = gi.iterative_scan(q, ef_search=ef, max_scan_tuples=mst)
+        found = [[] for _ in range(nq)]
+        live = np.ones(nq, dtype=bool)
+        at_call = np.zeros(nq, np.int64)
+        tup = [np.zeros(nq, np.int64)]
+        calls = 0
+        while live.any():
+            ids, dist, cnt = sc.next_batch()
+            calls += 1
+            if tuples_each_call:
+                tup.append(sc.tuples())
+            for i in np.nonzero(live)[0]:
+                k = int(cnt[i])
+                m = ids[i, :k] % c == 0
+                found[i].extend(zip(ids[i, :k][m].tolist(), dist[i, :k][m].tolist()))
+                if len(found[i]) >= limit or k == 0:
+                    found[i] = found[i][:limit]
+                    live[i] = False
+                    at_call[i] = calls
+        tuples = sc.tuples()
+        sec = time.perf_counter() - t0
+        sc.close()
+        return sec, calls, found, tuples, at_call, tup
+
+    def device_arm(c):
+        t0 = time.perf_counter()
+        f = gi.filter(np.arange(0, n, c, dtype=np.int64))
+        sc = gi.iterative_scan(q, ef_search=ef, max_scan_tuples=mst, filter=f, page=limit)
+        f.free()
+        found = [[] for _ in range(nq)]
+        live = np.ones(nq, dtype=bool)
+        calls = 0
+        while live.any():
+            ids, dist, cnt = sc.next_batch()
+            calls += 1
+            for i in np.nonzero(live)[0]:
+                k = int(cnt[i])
+                found[i].extend(zip(ids[i, :k].tolist(), dist[i, :k].tolist()))
+                if len(found[i]) >= limit or k < limit:
+                    live[i] = False
+        tuples = sc.tuples()
+        sec = time.perf_counter() - t0
+        sc.close()
+        return sec, calls, found, tuples
+
+    for c in (10, 100, 1000):
+        for _ in range(2):                                            # the first run warms modules, workspaces and staging
+            h_s, h_calls, h_found, h_tup, _, _ = host_arm(c)
+            d_s, d_calls, d_found, d_tup = device_arm(c)
+        assert h_found == d_found, f"element % {c}: device filter != host filter"
+        # untimed: the unfiltered batch holding each query's 10th match, and whether it came from the drain
+        _, _, _, _, at_call, tup = host_arm(c, tuples_each_call=True)
+        tup = np.stack(tup)
+        drained = tup[at_call - 1, np.arange(nq)] >= mst
+        out[f"element_mod_{c}"] = {
+            "host_filtered": {"next_calls": h_calls, "ms": h_s * 1e3, "filtered_queries_per_s": nq / h_s,
+                              "mean_tuples_per_query": float(h_tup.mean())},
+            "device_filtered": {"next_calls": d_calls, "ms": d_s * 1e3, "filtered_queries_per_s": nq / d_s,
+                                "mean_tuples_per_query": float(d_tup.mean()),
+                                # from the untimed replay of the unfiltered handle, not read from the filtered kernel: the
+                                # batch holding each query's 10th match, which is where the filtered handle stops that query
+                                "unfiltered_batches_to_10th_match_replayed": {"mean": float(at_call.mean()), "max": int(at_call.max())},
+                                "queries_reaching_the_drain_replayed": int(drained.sum())},
+            "identical_first_10": True}
+    print(json.dumps(out))
+
+
 def bench_kmeans(args):
     """k-means of config D on one GPU: 50 * lists samples x dim, lists centres (k-means++ seeding + Lloyd iterations)."""
     import torch
@@ -749,7 +852,8 @@ def bench_sparse(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "ivf-iter", "filter", "kmeans", "sparse", "rerank", "level0"])
+    ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "ivf-iter", "filter", "kmeans", "sparse", "rerank", "level0",
+                                        "hnsw-filter"])
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--lists", type=int, default=1000)
     ap.add_argument("--probes", type=int, default=10)
@@ -769,7 +873,7 @@ if __name__ == "__main__":
     a = ap.parse_args()
     if a.what == "rerank":      # config E's query batch and ef_search
         a.queries, a.ef = a.queries or 2048, a.ef or 200
-    if a.what in ("ivf-iter", "filter"):
+    if a.what in ("ivf-iter", "filter", "hnsw-filter"):
         a.queries = a.queries or 2048
     if a.what == "level0":
         a.queries = a.queries or 4 * 2048
@@ -787,6 +891,10 @@ if __name__ == "__main__":
         a.rows = a.rows or 100_000
         a.dim = a.dim or (768 if a.elem == "halfvec" else 1024)
         bench_hnsw(a)
+    elif a.what == "hnsw-filter":         # config C's shape
+        a.rows = a.rows or 1_000_000
+        a.dim = a.dim or 768
+        bench_hnsw_filter(a)
     elif a.what == "rerank":
         a.rows = a.rows or 1_000_000
         a.dim = a.dim or 1024
