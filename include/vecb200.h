@@ -563,6 +563,65 @@ int			vb_hnsw_build(vb_hnsw *h, const void *rows, int64_t n, int ef_construction
 						  const int32_t *levels);
 int			vb_hnsw_build_dev(vb_hnsw *h, const void *rows_dev, int64_t n, int ef_construction, uint64_t seed,
 							  const int32_t *levels);
+/*
+ * INSERT into a resident image (aminsert = HnswInsertTupleOnDisk, src/hnswinsert.c:696-743), so the image stays valid
+ * across inserts and only the changed neighbour slots go to the pages.
+ *
+ * Element numbers: row i of the call becomes element n_old + i, a duplicate too (as in vb_hnsw_build): out_dup_of[i]
+ * (may be NULL) and vb_hnsw_export's dup_of give the element the row was folded into, or -1.  A folded element gets
+ * no neighbours and no incoming links.  levels: the caller's draws (the extension takes them from pg_prng), capped at
+ * HnswGetMaxLevel(m) as in the build; NULL = drawn from `seed` with the build's expression.
+ *
+ * Semantics: HnswInsertTupleOnDisk for each row, in batches.  Rows go in in order; rows of one batch do not see each
+ * other (the reference's concurrent inserters).  A batch holds at most max(1, graph size / hnsw_build_fraction) rows,
+ * at most hnsw_build_batch (vb_set_option), and ends at a row that rises above the entry level; with batches of one
+ * row the result is the serial reference insert.  The on-disk rules:
+ *   - candidates whose element is being deleted (heap TID count 0) help the search but are removed before
+ *     SelectNeighbors (RemoveElements, src/hnswutils.c:1237-1259);
+ *   - a row is folded into the first equal layer-0 neighbour, in neighbour order, with 1..9 heap TIDs; 0 (being
+ *     deleted) or 10 (full) is skipped (FindDuplicateOnDisk / AddDuplicateOnDisk, src/hnswinsert.c:586-663);
+ *   - a neighbour's list that is not full takes the new element in its first free slot; a full list has its distances
+ *     recomputed from the neighbour's own row, its first neighbour that is being deleted is replaced, and otherwise
+ *     HnswUpdateConnection (src/hnswutils.c:1184-1231) replaces the pruned connection in its slot, or changes nothing
+ *     when the new element is the one pruned (GetUpdateIndex, src/hnswinsert.c:409-448).  Stored distances are never
+ *     read, so a loaded image and a built one behave alike;
+ *   - the entry point moves only to a strictly higher level, never to a folded row; into an empty image the first
+ *     row becomes the entry point, with no neighbours.
+ * ef_construction is checked as by vb_hnsw_build.
+ *
+ * Heap TID counts drive RemoveElements, the preference for deleted neighbours and duplicate folding: after
+ * vb_hnsw_load every element counts 1, after vb_hnsw_build the build's counts; folds add to them.
+ * vb_hnsw_set_heaptid_counts (host [n], 0..10) passes what the glue saw on the pages (0 = being deleted).  The
+ * search never reads them.
+ *
+ * Change records: *out_nchanges (may be NULL) of them; vb_hnsw_insert_changes copies them, sorted by (element, layer,
+ * slot): one per neighbour-array slot whose value after the call differs from its value before -- every filled slot
+ * of the new elements and every slot UpdateNeighborOnDisk rewrote in an existing element; slot indexes the layer's lm
+ * entries (2m at layer 0, m above).  A slot rewritten twice in one call appears once, with its final value: applied
+ * to a vb_hnsw_export taken before the call they give exactly the export taken after it.  cap below the count fails
+ * with VB_EINVAL, writing nothing.  The records stay valid until the next insert, load or build.
+ *
+ * Growth and failure: the device arrays grow geometrically (the graph is not double-buffered).  Before any kernel
+ * runs, the call validates its arguments and reserves capacity, upper slots, record space and visited tables; after
+ * VB_EINVAL or VB_ENOMEM (which names the bytes) the image is as it was.
+ *
+ * An insert bumps the image's generation, like a load: element filters made before it and filtered scan handles
+ * begun before it fail with VB_ESTATE (their bitsets cover the old elements only).  Unfiltered vb_hnsw_scan handles
+ * and vb_hnsw_search* work on the grown graph.
+ */
+typedef struct vb_hnsw_slot
+{
+	int32_t		element,
+				layer,
+				slot,
+				neighbor;
+} vb_hnsw_slot;
+int			vb_hnsw_insert(vb_hnsw *h, const void *rows, int64_t n, int ef_construction, uint64_t seed,
+						   const int32_t *levels, int32_t *out_dup_of, int64_t *out_nchanges);
+int			vb_hnsw_insert_dev(vb_hnsw *h, const void *rows_dev, int64_t n, int ef_construction, uint64_t seed,
+							   const int32_t *levels, int32_t *out_dup_of, int64_t *out_nchanges);
+int			vb_hnsw_insert_changes(vb_hnsw *h, vb_hnsw_slot *out, int64_t cap);	/* the last insert's records */
+int			vb_hnsw_set_heaptid_counts(vb_hnsw *h, const int32_t *counts);
 int64_t		vb_hnsw_rows(const vb_hnsw *h);
 int64_t		vb_hnsw_upper_slots(const vb_hnsw *h);
 int			vb_hnsw_export(vb_hnsw *h, int32_t *levels, int32_t *nbr0, int64_t *upper_off, int32_t *upper,

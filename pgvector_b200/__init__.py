@@ -697,6 +697,10 @@ def assign(rows: Table, metric, centers):
 
 # --------------------------------------------------------------------- HNSW
 
+# one change record of HnswIndex.insert (vb_hnsw_slot)
+HNSW_SLOT_DTYPE = np.dtype([("element", np.int32), ("layer", np.int32), ("slot", np.int32), ("neighbor", np.int32)])
+
+
 class HnswIndex:
     """Device image of an hnsw index and its scan (src/hnswscan.c, src/hnswutils.c:824-987).
 
@@ -735,6 +739,45 @@ class HnswIndex:
             self.n = rows.shape[0]
             _lib.check(load().vb_hnsw_build(self.h, _ptr(rows), self.n, int(ef_construction), int(seed), _ptr(lv)))
         return self
+
+    def insert(self, rows, ef_construction=64, seed=42, levels=None):
+        """INSERT into the resident image (batched HnswInsertTupleOnDisk, src/hnswinsert.c:696-743): row i becomes
+        element n_old + i.  Returns (dup_of [n], the element each row was folded into or -1; the change records, a
+        structured array of (element, layer, slot, neighbor) sorted by (element, layer, slot): every neighbour-array
+        slot whose value changed, with its new value)."""
+        lv = None if levels is None else np.ascontiguousarray(levels, dtype=np.int32)
+        nchg = C.c_int64(0)
+        if _is_torch(rows):
+            _after_torch(rows)
+            n = rows.shape[0]
+            dup = np.empty(n, dtype=np.int32)
+            _lib.check(load().vb_hnsw_insert_dev(self.h, _ptr(rows), n, int(ef_construction), int(seed), _ptr(lv), _ptr(dup),
+                                                 C.byref(nchg)))
+        else:
+            rows = _host(self.elem, rows)
+            if rows.ndim == 1:
+                rows = rows.reshape(1, -1)
+            n = rows.shape[0]
+            dup = np.empty(n, dtype=np.int32)
+            _lib.check(load().vb_hnsw_insert(self.h, _ptr(rows), n, int(ef_construction), int(seed), _ptr(lv), _ptr(dup),
+                                             C.byref(nchg)))
+        self.n = int(load().vb_hnsw_rows(self.h))
+        return dup, self.changes(int(nchg.value))
+
+    def changes(self, count):
+        """the last insert's change records (count = the number it reported)"""
+        out = np.empty(count, dtype=HNSW_SLOT_DTYPE)
+        _lib.check(load().vb_hnsw_insert_changes(self.h, _ptr(out), count))
+        return out
+
+    def set_heaptid_counts(self, counts):
+        """heap TIDs per element as the pages hold them (0..10; 0 = being deleted): they drive the insert's
+        RemoveElements, its preference for deleted neighbours and duplicate folding"""
+        counts = np.ascontiguousarray(counts, dtype=np.int32)
+        n = int(load().vb_hnsw_rows(self.h))
+        if counts.shape != (n,):
+            raise ValueError(f"counts must have {n} entries, got {counts.shape}")
+        _lib.check(load().vb_hnsw_set_heaptid_counts(self.h, _ptr(counts)))
 
     def export(self):
         """the graph as arrays (the layout load() takes, plus dup_of): what the page writer consumes"""

@@ -338,12 +338,17 @@ void hnsw_release(Hnsw& h) {
     cudaFree(h.upper_d);
     cudaFree(h.dup_of);
     cudaFree(h.n_heaptids);
+    cudaFree(h.rec_key);
+    cudaFree(h.rec_val);
     h.levels = h.nbr0 = h.upper_off = h.upper = nullptr;
     h.nd0 = h.upper_d = nullptr;
     h.dup_of = h.n_heaptids = nullptr;
+    h.rec_key = nullptr;
+    h.rec_val = nullptr;
     h.vis = nullptr;
     h.vis_bytes = 0;
     h.upper_slots = 0;
+    h.elem_cap = h.slot_cap = h.rec_cap = h.n_changes = 0;
     h.loaded = false;
 }
 
@@ -403,6 +408,9 @@ int vb_hnsw_load(vb_hnsw* p, const void* rows, int64_t n, const int32_t* levels,
     VB_CUDA(cudaMemcpy(h.nbr0, nbr0, sizeof(int32_t) * (size_t)n * lm0, cudaMemcpyHostToDevice));
     VB_CUDA(cudaMemcpy(h.upper_off, uo.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice));
     if (upper_slots > 0) VB_CUDA(cudaMemcpy(h.upper, upper, sizeof(int32_t) * (size_t)upper_slots * h.m, cudaMemcpyHostToDevice));
+    h.upper_slots = upper_slots;
+    h.elem_cap = n;
+    h.slot_cap = std::max<int64_t>(upper_slots, 1);
     h.loaded = true;
     return VB_OK;
 }

@@ -50,7 +50,14 @@ struct Hnsw {
     float *nd0 = nullptr, *upper_d = nullptr;
     int32_t *dup_of = nullptr, *n_heaptids = nullptr;
     int64_t upper_slots = 0;
-    uint64_t generation = 0;  // bumped by every load and build: filters and filtered scan handles refuse a changed image
+    uint64_t generation = 0;  // bumped by every load, build and insert: filters and filtered scan handles refuse a changed image
+    // capacities of the per-element arrays (levels, upper_off, nbr0, nd0, dup_of, n_heaptids) and of the upper slots
+    // (upper, upper_d): vb_hnsw_insert grows them geometrically
+    int64_t elem_cap = 0, slot_cap = 0;
+    // the last insert's change records, sorted by (element, layer, slot): key = element << 14 | layer << 8 | slot
+    uint64_t* rec_key = nullptr;
+    int32_t* rec_val = nullptr;
+    int64_t rec_cap = 0, n_changes = 0;
 };
 
 void hnsw_release(Hnsw& h);

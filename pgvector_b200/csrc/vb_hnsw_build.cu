@@ -55,6 +55,14 @@ struct BuildDev {
     int* overflow;
 };
 
+// vb_hnsw_insert's change records: one (key, neighbour) per neighbour-array slot written, key = element << 14 | layer << 8
+// | slot.  (A parameter of its own, so the build kernels' parameter layout stays as it was.)
+struct InsertRec {
+    uint64_t* key;
+    int32_t* val;
+    int* n;
+};
+
 constexpr int HB_CAND = 256;     // candidates of one HnswUpdateConnection: lm + 1 <= 201, padded to a power of two
 
 __device__ __forceinline__ float key64_to_float(uint64_t k) { return (float)key64_to_double(k); }
@@ -104,8 +112,9 @@ __device__ __forceinline__ void prune_against(const HnswDev& g, const uint4* img
     }
 }
 
-// K1: one warp = one new element
-template <int ELEM, int METRIC, int LPR>
+// K1: one warp = one new element.  INS (vb_hnsw_insert): candidates whose element is being deleted (heap TID count 0)
+// help the search but are removed before SelectNeighbors (RemoveElements, src/hnswutils.c:1237-1259, 1343-1344).
+template <int ELEM, int METRIC, int LPR, bool INS = false>
 __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_insert_kernel(BuildDev b, uint32_t* __restrict__ vis_all, uint32_t vis_cap,
                                                                     uint32_t vis_upper) {
     extern __shared__ uint4 smem[];
@@ -168,9 +177,28 @@ __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_insert_kernel(BuildDev b, 
             const int lm = lc == 0 ? lm0 : g.m;
             int32_t* out_ids = lc == 0 ? b.nbr0_w + (size_t)e * lm : b.upper_w + ((size_t)g.upper_off[e] + (lc - 1)) * (size_t)lm;
             float* out_d = lc == 0 ? b.nd0 + (size_t)e * lm : b.upper_d + ((size_t)g.upper_off[e] + (lc - 1)) * (size_t)lm;
-            const int len = S.len;
+            int len = S.len;
             const uint64_t* wk = S.rk;     // W, nearest first; stays intact: it is the next layer's entry list (ep = w)
             const uint32_t* wi = S.ri;
+            if constexpr (INS) {
+                // the kept candidates go to the second key / id buffers, which the in-place merge leaves unused
+                int kept = 0;
+                for (int i0 = 0; i0 < len; i0 += 32) {
+                    const int i = i0 + lane;
+                    const bool keep = i < len && b.n_heaptids[S.ri[i] & 0x7fffffffu] != 0;
+                    const unsigned km = __ballot_sync(0xffffffffu, keep);
+                    if (keep) {
+                        const int p = kept + __popc(km & ((1u << lane) - 1u));
+                        S.nk[p] = S.rk[i];
+                        S.ni[p] = S.ri[i];
+                    }
+                    kept += __popc(km);
+                }
+                __syncwarp();
+                wk = S.nk;
+                wi = S.ni;
+                len = kept;
+            }
             if (len <= lm) {
                 // SelectNeighbors returns the list as it is (:1077-1078): W drained from the max-heap = farthest first
                 for (int i = lane; i < lm; i += 32) {
@@ -215,7 +243,10 @@ __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_insert_kernel(BuildDev b, 
     }
 }
 
-// K1b: duplicates (FindDuplicateInMemory, src/hnswbuild.c:343-364) and the update records of every chosen neighbour
+// K1b: duplicates (FindDuplicateInMemory, src/hnswbuild.c:343-364) and the update records of every chosen neighbour.
+// DISK (vb_hnsw_insert): FindDuplicateOnDisk / AddDuplicateOnDisk (src/hnswinsert.c:586-663): the row joins the first
+// equal neighbour with 1..9 heap TIDs; one being deleted (0) or full (10) is skipped.
+template <bool DISK = false>
 __global__ void __launch_bounds__(128) hnsw_finalize_kernel(BuildDev b) {
     if (*b.overflow) return;   // K1 is repeated with larger visited tables: no side effect may have happened yet
     const HnswDev& g = b.g;
@@ -240,6 +271,24 @@ __global__ void __launch_bounds__(128) hnsw_finalize_kernel(BuildDev b) {
                 eq = eq && x.x == y.x && x.y == y.y && x.z == y.z && x.w == y.w;
             }
             if (!__all_sync(0xffffffffu, eq)) break;   // "exit early since ordered by distance"
+            if constexpr (DISK) {
+                int c = 0;
+                if (lane == 0) {
+                    c = b.n_heaptids[t];
+                    while (c >= 1 && c < 10) {
+                        const int o = atomicCAS(&b.n_heaptids[t], c, c + 1);
+                        if (o == c) break;
+                        c = o;
+                    }
+                }
+                c = __shfl_sync(0xffffffffu, c, 0);
+                if (c >= 1 && c < 10) {
+                    dup = true;
+                    if (lane == 0) b.dup_of[e] = t;
+                    break;
+                }
+                continue;
+            }
             int old = 0;
             if (lane == 0) old = atomicAdd(&b.n_heaptids[t], 1);
             old = __shfl_sync(0xffffffffu, old, 0);
@@ -390,6 +439,189 @@ __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_update_kernel(BuildDev b, 
     }
 }
 
+// shared memory of one warp of hnsw_update_disk_kernel (bytes, 16-aligned)
+__host__ __device__ inline size_t hb_update_disk_smem(int qvec) {
+    size_t b = hb_update_smem(qvec);
+    b += (size_t)HB_CAND * 4 * 2;              // ids of the list as scored, their distances to the target
+    return (b + 15) & ~(size_t)15;
+}
+
+__device__ __forceinline__ void hb_record(const InsertRec& r, int t, int lc, int slot, int32_t v) {
+    const int p = atomicAdd(r.n, 1);
+    r.key[p] = ((uint64_t)(uint32_t)t << 14) | ((uint64_t)lc << 8) | (uint64_t)slot;
+    r.val[p] = v;
+}
+
+// K2 of vb_hnsw_insert: one warp per (target, layer) run = UpdateNeighborOnDisk (src/hnswinsert.c:409-448, 506-518)
+// for each incoming element in insertion order.  The stored distances are not used: a full list has its distances
+// recomputed from the target's own row (LoadElementsForInsert, :383-403), with the scan arithmetic, once per run and
+// kept in shared memory for the run's later updates.  Then:
+//   room left                     -> the first free slot;
+//   a neighbour being deleted     -> the first such neighbour is replaced;
+//   otherwise                     -> HnswUpdateConnection (src/hnswutils.c:1184-1231): SelectNeighbors over the lm
+//                                    connections and the new element, nearest first; the pruned connection is replaced
+//                                    in its slot, nothing changes when the new element is the one pruned.
+// Every slot written is recorded (rec_key / rec_val); later records of a slot supersede earlier ones.
+template <int ELEM, int METRIC, int LPR>
+__global__ void __launch_bounds__(HN_WARPS * 32) hnsw_update_disk_kernel(BuildDev b, const uint64_t* __restrict__ keys,
+                                                                         const float* __restrict__ vals, int n_edges, InsertRec r) {
+    extern __shared__ uint4 smem[];
+    const HnswDev& g = b.g;
+    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+    uint8_t* base = reinterpret_cast<uint8_t*>(smem) + (size_t)warp * hb_update_disk_smem(b.qvec);
+    uint4* img = reinterpret_cast<uint4*>(base);
+    uint64_t* ck = reinterpret_cast<uint64_t*>(img + b.qvec);
+    uint64_t* bkey = ck + HB_CAND;
+    uint32_t* bid = reinterpret_cast<uint32_t*>(bkey + 32);
+    int32_t* bj = reinterpret_cast<int32_t*>(bid + 32);
+    uint32_t* cid = reinterpret_cast<uint32_t*>(bj + 32);
+    float* cd = reinterpret_cast<float*>(cid + HB_CAND);
+    uint8_t* dead = reinterpret_cast<uint8_t*>(cd + HB_CAND);
+
+    const int64_t gwarp = blockIdx.x * (int64_t)HN_WARPS + warp;
+    const int64_t nwarps = gridDim.x * (int64_t)HN_WARPS;
+    for (int64_t i = gwarp; i < n_edges; i += nwarps) {
+        const uint64_t head = keys[i] >> 20;
+        if (i > 0 && (keys[i - 1] >> 20) == head) continue;   // not the first record of its (target, layer) run
+        const int t = (int)(head >> 6), lc = (int)(head & 63);
+        const int lm = lc == 0 ? 2 * g.m : g.m;
+        int32_t* ids = lc == 0 ? b.nbr0_w + (size_t)t * lm : b.upper_w + ((size_t)g.upper_off[t] + (lc - 1)) * (size_t)lm;
+        bool have_d = false;
+        for (int64_t p = i; p < n_edges && (keys[p] >> 20) == head; ++p) {
+            const int src = b.b0 + (int)(keys[p] & 0xFFFFFu);
+            const float d = vals[p];
+            // current length = first invalid entry
+            int count = lm;
+            for (int off = 0; off < lm; off += 32) {
+                const int nid = off + lane < lm ? ids[off + lane] : -1;
+                const unsigned inval = ~__ballot_sync(0xffffffffu, nid >= 0);
+                if (inval) {
+                    count = min(lm, off + __ffs(inval) - 1);
+                    break;
+                }
+            }
+            int slot = -1;
+            if (count < lm) {
+                slot = count;
+            } else {
+                if (!have_d) {
+                    load_row_image<ELEM, METRIC>(g.rows + (size_t)t * g.stride, g.V, img, lane);
+                    for (int j = lane; j < lm; j += 32) cid[j] = (uint32_t)ids[j];
+                    __syncwarp();
+                    hnsw_score_batch<ELEM, METRIC, LPR>(g, img, cid, lm, ck, lane);
+                    __syncwarp();
+                    for (int j = lane; j < lm; j += 32) cd[j] = key64_to_float(ck[j]);
+                    __syncwarp();
+                    have_d = true;
+                }
+                for (int off = 0; off < lm && slot < 0; off += 32) {
+                    const int j = off + lane;
+                    const unsigned zm = __ballot_sync(0xffffffffu, j < lm && b.n_heaptids[ids[j]] == 0);
+                    if (zm) slot = off + __ffs(zm) - 1;
+                }
+                if (slot < 0) {
+                    // candidates = the lm connections + the new element, nearest first
+                    const int n = lm + 1;
+                    int P = 2;
+                    while (P < n) P <<= 1;
+                    for (int j = lane; j < P; j += 32) {
+                        uint64_t key = ~0ull;
+                        if (j < lm) key = ((uint64_t)orderable_key(cd[j]) << 32) | (uint32_t)ids[j];
+                        else if (j == lm) key = ((uint64_t)orderable_key(d) << 32) | (uint32_t)src;
+                        ck[j] = key;
+                        dead[j] = 0;
+                    }
+                    __syncwarp();
+                    for (int size = 2; size <= P; size <<= 1)
+                        for (int st = size >> 1; st > 0; st >>= 1) {
+                            for (int a = lane; a < P; a += 32) {
+                                const int c = a ^ st;
+                                if (c > a) {
+                                    const uint64_t x = ck[a], y = ck[c];
+                                    const bool up = (a & size) == 0;
+                                    if ((x > y) == up) {
+                                        ck[a] = y;
+                                        ck[c] = x;
+                                    }
+                                }
+                            }
+                            __syncwarp();
+                        }
+                    int nAcc = 0;
+                    for (int c = 0; c < n; ++c) {
+                        if (dead[c]) continue;
+                        ++nAcc;
+                        if (nAcc == lm || c == n - 1) break;
+                        load_row_image<ELEM, METRIC>(g.rows + (size_t)(uint32_t)ck[c] * g.stride, g.V, img, lane);
+                        __syncwarp();
+                        prune_against<ELEM, METRIC, LPR>(
+                            g, img, c + 1, n, dead, bid, bj, bkey, lane, [&](int j) { return (uint32_t)ck[j]; },
+                            [&](int j) { return key_to_float((uint32_t)(ck[j] >> 32)); });
+                        if (dead[n - 1]) break;   // the farthest candidate is pruned: it is the one that goes
+                    }
+                    __syncwarp();
+                    int drop = -1;
+                    for (int j0 = ((n - 1) / 32) * 32; j0 >= 0 && drop < 0; j0 -= 32) {
+                        const int j = j0 + lane;
+                        const unsigned dm = __ballot_sync(0xffffffffu, j < n && dead[j]);
+                        if (dm) drop = j0 + 31 - __clz(dm);
+                    }
+                    if (drop < 0) drop = n - 1;
+                    const uint32_t drop_id = (uint32_t)ck[drop];
+                    if (drop_id != (uint32_t)src) {
+                        for (int off = 0; off < lm && slot < 0; off += 32) {
+                            const int j = off + lane;
+                            const unsigned hm = __ballot_sync(0xffffffffu, j < lm && (uint32_t)ids[j] == drop_id);
+                            if (hm) slot = off + __ffs(hm) - 1;
+                        }
+                    }
+                    __syncwarp();
+                }
+            }
+            if (slot >= 0 && lane == 0) {
+                ids[slot] = src;
+                if (have_d) cd[slot] = d;
+                hb_record(r, t, lc, slot, src);
+            }
+            __syncwarp();
+        }
+    }
+}
+
+// the change records of the new elements: every filled slot of their own lists, as they stand after the last batch
+__global__ void __launch_bounds__(128) hnsw_new_records_kernel(BuildDev b, InsertRec r, int64_t e0, int64_t ne) {
+    const HnswDev& g = b.g;
+    const int lane = threadIdx.x % 32;
+    const int64_t gwarp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32;
+    const int64_t nwarps = (gridDim.x * (int64_t)blockDim.x) / 32;
+    for (int64_t w = gwarp; w < ne; w += nwarps) {
+        const int e = (int)(e0 + w);
+        if (b.dup_of[e] >= 0) continue;
+        for (int lc = 0; lc <= g.levels[e]; ++lc) {
+            const int lm = lc == 0 ? 2 * g.m : g.m;
+            const int32_t* ids = lc == 0 ? b.nbr0_w + (size_t)e * lm : b.upper_w + ((size_t)g.upper_off[e] + (lc - 1)) * (size_t)lm;
+            for (int off = 0; off < lm; off += 32) {
+                const int v = off + lane < lm ? ids[off + lane] : -1;
+                const unsigned vm = __ballot_sync(0xffffffffu, v >= 0);
+                if (vm == 0) break;
+                int p = 0;
+                if (lane == 0) p = atomicAdd(r.n, __popc(vm));
+                p = __shfl_sync(0xffffffffu, p, 0) + __popc(vm & ((1u << lane) - 1u));
+                if (v >= 0) {
+                    r.key[p] = ((uint64_t)(uint32_t)e << 14) | ((uint64_t)lc << 8) | (uint64_t)(off + lane);
+                    r.val[p] = v;
+                }
+            }
+        }
+    }
+}
+
+// after the stable sort by key: a record is kept when it is the last of its slot (the slot's final value)
+__global__ void hnsw_last_of_key_kernel(const uint64_t* __restrict__ keys, int64_t n, uint8_t* __restrict__ keep) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i < n) keep[i] = (i + 1 == n || keys[i + 1] != keys[i]) ? 1 : 0;
+}
+
 __global__ void fill_i32_kernel(int32_t* p, int64_t n, int32_t v) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i < n) p[i] = v;
@@ -397,16 +629,17 @@ __global__ void fill_i32_kernel(int32_t* p, int64_t n, int32_t v) {
 
 // ----------------------------------------------------------------------------- host side
 
-enum { WSB_KEYS = 14, WSB_KEYS2 = 15, WSB_VALS = 16, WSB_VALS2 = 17, WSB_TMP = 18, WSB_FLAGS = 19 };
+enum { WSB_KEYS = 14, WSB_KEYS2 = 15, WSB_VALS = 16, WSB_VALS2 = 17, WSB_TMP = 18, WSB_FLAGS = 19, WSB_KEEP = 20 };
 
 struct BuildLaunch {
     int (*insert)(const BuildDev&, uint32_t*, uint32_t, uint32_t, int, size_t, int*);
-    int (*update)(const BuildDev&, const uint64_t*, const float*, int, int, size_t, int*);
+    int (*update)(const BuildDev&, const uint64_t*, const float*, int, const InsertRec&, int, size_t, int*);
 };
 
-template <int ELEM, int METRIC, int LPR>
+// INS: the kernels of vb_hnsw_insert (RemoveElements in K1, UpdateNeighborOnDisk in K2)
+template <int ELEM, int METRIC, int LPR, bool INS>
 static int launch_insert(const BuildDev& b, uint32_t* vis, uint32_t vis_cap, uint32_t vis_upper, int grid, size_t smem, int* occ) {
-    auto kern = hnsw_insert_kernel<ELEM, METRIC, LPR>;
+    auto kern = hnsw_insert_kernel<ELEM, METRIC, LPR, INS>;
     if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (occ) {
         VB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, HN_WARPS * 32, smem));
@@ -417,42 +650,47 @@ static int launch_insert(const BuildDev& b, uint32_t* vis, uint32_t vis_cap, uin
     count_launch();
     return VB_OK;
 }
-template <int ELEM, int METRIC, int LPR>
-static int launch_update(const BuildDev& b, const uint64_t* keys, const float* vals, int n_edges, int grid, size_t smem, int* occ) {
+template <int ELEM, int METRIC, int LPR, bool INS>
+static int launch_update(const BuildDev& b, const uint64_t* keys, const float* vals, int n_edges, const InsertRec& r, int grid, size_t smem,
+                         int* occ) {
     auto kern = hnsw_update_kernel<ELEM, METRIC, LPR>;
-    if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    auto kern_disk = hnsw_update_disk_kernel<ELEM, METRIC, LPR>;
+    const void* k = INS ? (const void*)kern_disk : (const void*)kern;
+    if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (occ) {
-        VB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, HN_WARPS * 32, smem));
+        VB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, k, HN_WARPS * 32, smem));
         return VB_OK;
     }
-    kern<<<grid, HN_WARPS * 32, smem, ctx().stream>>>(b, keys, vals, n_edges);
+    if (INS) kern_disk<<<grid, HN_WARPS * 32, smem, ctx().stream>>>(b, keys, vals, n_edges, r);
+    else kern<<<grid, HN_WARPS * 32, smem, ctx().stream>>>(b, keys, vals, n_edges);
     VB_CUDA(cudaGetLastError());
     count_launch();
     return VB_OK;
 }
 
-template <int ELEM, int METRIC>
+template <int ELEM, int METRIC, bool INS>
 static BuildLaunch pick_lpr(int V) {
     // lanes per row: a whole warp for rows of >= 512 bytes, 8 lanes for >= 128 bytes, one lane for tiny rows
-    if (V >= 32) return BuildLaunch{launch_insert<ELEM, METRIC, 32>, launch_update<ELEM, METRIC, 32>};
-    if (V >= 8) return BuildLaunch{launch_insert<ELEM, METRIC, 8>, launch_update<ELEM, METRIC, 8>};
-    return BuildLaunch{launch_insert<ELEM, METRIC, 1>, launch_update<ELEM, METRIC, 1>};
+    if (V >= 32) return BuildLaunch{launch_insert<ELEM, METRIC, 32, INS>, launch_update<ELEM, METRIC, 32, INS>};
+    if (V >= 8) return BuildLaunch{launch_insert<ELEM, METRIC, 8, INS>, launch_update<ELEM, METRIC, 8, INS>};
+    return BuildLaunch{launch_insert<ELEM, METRIC, 1, INS>, launch_update<ELEM, METRIC, 1, INS>};
 }
 
+template <bool INS>
 static bool pick_kernels(const Hnsw& h, int V, BuildLaunch* out) {
     if (h.elem == VB_VECTOR) {
-        if (h.metric == VB_L2_SQUARED) *out = pick_lpr<VB_VECTOR, VB_L2_SQUARED>(V);
-        else if (h.metric == VB_NEG_IP) *out = pick_lpr<VB_VECTOR, VB_NEG_IP>(V);
-        else if (h.metric == VB_L1) *out = pick_lpr<VB_VECTOR, VB_L1>(V);
+        if (h.metric == VB_L2_SQUARED) *out = pick_lpr<VB_VECTOR, VB_L2_SQUARED, INS>(V);
+        else if (h.metric == VB_NEG_IP) *out = pick_lpr<VB_VECTOR, VB_NEG_IP, INS>(V);
+        else if (h.metric == VB_L1) *out = pick_lpr<VB_VECTOR, VB_L1, INS>(V);
         else return false;
     } else if (h.elem == VB_HALFVEC) {
-        if (h.metric == VB_L2_SQUARED) *out = pick_lpr<VB_HALFVEC, VB_L2_SQUARED>(V);
-        else if (h.metric == VB_NEG_IP) *out = pick_lpr<VB_HALFVEC, VB_NEG_IP>(V);
-        else if (h.metric == VB_L1) *out = pick_lpr<VB_HALFVEC, VB_L1>(V);
+        if (h.metric == VB_L2_SQUARED) *out = pick_lpr<VB_HALFVEC, VB_L2_SQUARED, INS>(V);
+        else if (h.metric == VB_NEG_IP) *out = pick_lpr<VB_HALFVEC, VB_NEG_IP, INS>(V);
+        else if (h.metric == VB_L1) *out = pick_lpr<VB_HALFVEC, VB_L1, INS>(V);
         else return false;
     } else {
-        if (h.metric == VB_HAMMING) *out = pick_lpr<VB_BIT, VB_HAMMING>(V);
-        else if (h.metric == VB_JACCARD) *out = pick_lpr<VB_BIT, VB_JACCARD>(V);
+        if (h.metric == VB_HAMMING) *out = pick_lpr<VB_BIT, VB_HAMMING, INS>(V);
+        else if (h.metric == VB_JACCARD) *out = pick_lpr<VB_BIT, VB_JACCARD, INS>(V);
         else return false;
     }
     return true;
@@ -502,6 +740,8 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
         VB_REQUIRE(slots < (int64_t)0x7fffffff, "upper slot overflow");
     }
     h.upper_slots = slots;
+    h.elem_cap = n;
+    h.slot_cap = std::max<int64_t>(slots, 1);
     const size_t up_elems = (size_t)std::max<int64_t>(slots, 1) * m;
     VB_CUDA(cudaMalloc(&h.levels, sizeof(int32_t) * (size_t)n));
     VB_CUDA(cudaMalloc(&h.upper_off, sizeof(int32_t) * (size_t)n));
@@ -522,7 +762,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
 
     BuildLaunch K;
     const int V = (int)(h.rows.stride / 16);
-    if (!pick_kernels(h, V, &K)) {
+    if (!pick_kernels<false>(h, V, &K)) {
         set_error("hnsw build: unsupported metric %d for element type %d", h.metric, h.elem);
         return VB_EINVAL;
     }
@@ -553,7 +793,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
 
     int occ_ins = 1, occ_upd = 1;
     VB_TRY(K.insert(b, nullptr, 0, 0, 0, smem_ins, &occ_ins));
-    VB_TRY(K.update(b, nullptr, nullptr, 0, 0, smem_upd, &occ_upd));
+    VB_TRY(K.update(b, nullptr, nullptr, 0, InsertRec{}, 0, smem_upd, &occ_upd));
     const int max_grid_ins = c.sm_count * std::max(1, occ_ins);
     const int max_grid_upd = c.sm_count * std::max(1, occ_upd) * 4;
 
@@ -620,7 +860,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
             }
             VB_CUDA(cudaMemsetAsync(d_flags, 0, 2 * sizeof(int), s));
             VB_TRY(K.insert(b, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
-            hnsw_finalize_kernel<<<(unsigned)std::min<int64_t>((B * 32 + 127) / 128, (int64_t)c.sm_count * 16), 128, 0, s>>>(b);
+            hnsw_finalize_kernel<false><<<(unsigned)std::min<int64_t>((B * 32 + 127) / 128, (int64_t)c.sm_count * 16), 128, 0, s>>>(b);
             VB_CUDA(cudaGetLastError());
             count_launch();
             VB_CUDA(cudaMemcpyAsync(flags, d_flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -641,7 +881,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
                                                     (float*)d_v2, n_edges, 0, 57, s));
             count_launch();
             const int grid_upd = (int)std::min<int64_t>(((int64_t)n_edges + HN_WARPS - 1) / HN_WARPS, max_grid_upd);
-            VB_TRY(K.update(b, (const uint64_t*)d_k2, (const float*)d_v2, n_edges, grid_upd, smem_upd, nullptr));
+            VB_TRY(K.update(b, (const uint64_t*)d_k2, (const float*)d_v2, n_edges, InsertRec{}, grid_upd, smem_upd, nullptr));
         }
         if (promote >= 0) {
             // UpdateGraphInMemory (src/hnswbuild.c:428-430): a duplicate never becomes the entry point
@@ -657,6 +897,313 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
     }
     VB_CUDA(cudaStreamSynchronize(s));
     h.loaded = true;
+    return VB_OK;
+}
+
+// ----------------------------------------------------------------------------- insert into a resident image
+
+// *p grows to new_bytes keeping its first used_bytes; fill >= -1: the array is new and its first fill_n entries are set
+static int hnsw_grow(void** p, size_t used_bytes, size_t new_bytes, const char* what, int64_t fill_n = 0, int32_t fill = 0) {
+    cudaStream_t s = ctx().stream;
+    void* q = nullptr;
+    if (cudaMalloc(&q, std::max<size_t>(new_bytes, 16)) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("hnsw insert: %s (%zu bytes) does not fit in device memory", what, new_bytes);
+        return VB_ENOMEM;
+    }
+    if (*p && used_bytes) VB_CUDA(cudaMemcpyAsync(q, *p, used_bytes, cudaMemcpyDeviceToDevice, s));
+    if (fill_n > 0) {
+        fill_i32_kernel<<<(unsigned)((fill_n + 255) / 256), 256, 0, s>>>((int32_t*)q, fill_n, fill);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    VB_CUDA(cudaStreamSynchronize(s));
+    cudaFree(*p);
+    *p = q;
+    return VB_OK;
+}
+
+// heap TID counts and the duplicate map of a loaded image: every element counts 1 and none is folded
+static int hnsw_ensure_counts(Hnsw& h) {
+    const size_t bytes = sizeof(int32_t) * (size_t)std::max<int64_t>(h.elem_cap, 1);
+    if (!h.dup_of) VB_TRY(hnsw_grow((void**)&h.dup_of, 0, bytes, "duplicate map", h.n, -1));
+    if (!h.n_heaptids) VB_TRY(hnsw_grow((void**)&h.n_heaptids, 0, bytes, "heap TID counts", h.n, 1));
+    return VB_OK;
+}
+
+// Batched HnswInsertTupleOnDisk (src/hnswinsert.c:696-743) into the resident graph: the build's batch loop with the
+// on-disk rules (RemoveElements in K1, FindDuplicateOnDisk in K1b, UpdateNeighborOnDisk in K2), then the change
+// records: every slot K2 wrote plus the new elements' own lists, stably sorted by (element, layer, slot) and reduced to
+// the last record of each slot.  Everything the call needs is reserved before the first kernel.
+static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t n, int efc, uint64_t seed, const int32_t* levels_in,
+                            int32_t* out_dup_of, int64_t* out_nchanges) {
+    VB_REQUIRE(h.loaded, "hnsw index not loaded");
+    VB_REQUIRE(efc >= 4 && efc <= 1000, "ef_construction must be 4..1000 (src/hnsw.h:57-59)");
+    VB_REQUIRE(efc >= 2 * h.m, "ef_construction must be greater than or equal to 2 * m (src/hnswbuild.c:713-716)");
+    const int64_t n0 = h.n;
+    VB_REQUIRE(n >= 0 && n0 + n < (int64_t)0x7fffffff, "bad row count");
+    VB_REQUIRE(rows || n == 0, "null rows");
+    BuildLaunch K;
+    const int V = (int)(h.rows.stride / 16);
+    if (!pick_kernels<true>(h, V, &K)) {
+        set_error("hnsw insert: unsupported metric %d for element type %d", h.metric, h.elem);
+        return VB_EINVAL;
+    }
+    const int m = h.m, lm0 = 2 * m;
+    const int qvec = h.elem == VB_HALFVEC ? 2 * V : V;
+    const size_t smem_ins = hb_insert_smem(qvec, efc, lm0) * HN_WARPS;
+    const size_t smem_upd = hb_update_disk_smem(qvec) * HN_WARPS;
+    VB_REQUIRE(smem_ins <= 200 * 1024 && smem_upd <= 200 * 1024,
+               "ef_construction %d / m %d with this dimension need %zu bytes of shared memory per CTA", efc, m, smem_ins);
+
+    // levels (HnswInitElement, src/hnswutils.c:248-254), capped at HnswGetMaxLevel(m), and the new upper slots
+    const double ml = 1.0 / std::log((double)m);
+    const int max_level = std::min((int)((8192 - 24 - 8 - 4 - 4) / 6 / m) - 2, 63);   // src/hnsw.h:133 with BLCKSZ = 8192
+    std::vector<int32_t> levels((size_t)n), uoff((size_t)n);
+    uint64_t rs = seed ^ 0x2545f4914f6cdd1dULL;
+    const int64_t slots0 = h.upper_slots;
+    int64_t slots = slots0, total_edges = 0;
+    for (int64_t i = 0; i < n; ++i) {
+        int lv = levels_in ? levels_in[i] : (int)(-std::log(build_uniform(&rs)) * ml);
+        VB_REQUIRE(lv >= 0, "negative level");
+        lv = std::min(lv, max_level);
+        levels[(size_t)i] = lv;
+        uoff[(size_t)i] = lv > 0 ? (int32_t)slots : -1;
+        slots += lv;
+        VB_REQUIRE(slots < (int64_t)0x7fffffff, "upper slot overflow");
+        total_edges += lm0 + (int64_t)lv * m;
+    }
+    VB_REQUIRE(total_edges < (int64_t)0x7fffffff / 2, "too many connection updates in one call");
+    if (out_nchanges) *out_nchanges = 0;
+    if (n == 0) {
+        h.n_changes = 0;
+        return VB_OK;
+    }
+    // one record per slot K2 writes (at most one per connection update) plus the new elements' lists
+    const int64_t recs = 2 * total_edges;
+    const int64_t n1 = n0 + n;
+    Context& c = ctx();
+    cudaStream_t s = c.stream;
+
+    // ---- reservations: nothing below changes the image until they have all succeeded
+    VB_TRY(table_reserve(h.rows, n1));
+    VB_TRY(hnsw_ensure_counts(h));
+    {
+        const int64_t ecap = n1 > h.elem_cap ? std::max<int64_t>(n1, h.elem_cap + h.elem_cap / 2) : h.elem_cap;
+        const int64_t scap = slots > h.slot_cap ? std::max<int64_t>(slots, h.slot_cap + h.slot_cap / 2) : h.slot_cap;
+        struct Arr {
+            void** p;
+            size_t bytes;   // per element or per upper slot
+            bool upper, keep;
+            const char* what;
+        } arrs[] = {{(void**)&h.levels, 4, false, true, "levels"},
+                    {(void**)&h.upper_off, 4, false, true, "upper slot offsets"},
+                    {(void**)&h.nbr0, 4 * (size_t)lm0, false, true, "layer-0 neighbours"},
+                    {(void**)&h.nd0, 4 * (size_t)lm0, false, false, "layer-0 distances"},
+                    {(void**)&h.dup_of, 4, false, true, "duplicate map"},
+                    {(void**)&h.n_heaptids, 4, false, true, "heap TID counts"},
+                    {(void**)&h.upper, 4 * (size_t)m, true, true, "upper neighbours"},
+                    {(void**)&h.upper_d, 4 * (size_t)m, true, false, "upper distances"}};
+        // (the distances are scratch for the new elements' own lists: the on-disk update never reads a stored one)
+        for (const Arr& a : arrs) {
+            const int64_t cap = a.upper ? scap : ecap, have = a.upper ? h.slot_cap : h.elem_cap, used = a.upper ? slots0 : n0;
+            if (*a.p && cap == have) continue;
+            VB_TRY(hnsw_grow(a.p, a.keep ? (size_t)used * a.bytes : 0, (size_t)cap * a.bytes, a.what));
+        }
+        h.elem_cap = ecap;
+        h.slot_cap = scap;
+    }
+    if (recs > h.rec_cap) {
+        h.n_changes = 0;
+        h.rec_cap = 0;
+        VB_TRY(hnsw_grow((void**)&h.rec_key, 0, sizeof(uint64_t) * (size_t)recs, "change records"));
+        VB_TRY(hnsw_grow((void**)&h.rec_val, 0, sizeof(int32_t) * (size_t)recs, "change records"));
+        h.rec_cap = recs;
+    }
+    void *d_k1, *d_k2, *d_v1, *d_v2, *d_keep, *d_flags, *d_tmp;
+    VB_TRY(workspace(WSB_KEYS, sizeof(uint64_t) * (size_t)total_edges, &d_k1));
+    VB_TRY(workspace(WSB_KEYS2, sizeof(uint64_t) * (size_t)recs, &d_k2));
+    VB_TRY(workspace(WSB_VALS, sizeof(float) * (size_t)total_edges, &d_v1));
+    VB_TRY(workspace(WSB_VALS2, sizeof(float) * (size_t)recs, &d_v2));
+    VB_TRY(workspace(WSB_KEEP, (size_t)recs, &d_keep));
+    VB_TRY(workspace(WSB_FLAGS, 64, &d_flags));
+    size_t tmp_bytes = 0;
+    {
+        size_t t1 = 0, t2 = 0, t3 = 0, t4 = 0;
+        VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
+                                                (int)total_edges, 0, 57, s));
+        VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t2, (const uint64_t*)h.rec_key, (uint64_t*)d_k2, (const int32_t*)h.rec_val,
+                                                (int32_t*)d_v2, (int)recs, 0, 45, s));
+        VB_CUDA(cub::DeviceSelect::Flagged(nullptr, t3, (const uint64_t*)d_k2, (const uint8_t*)d_keep, h.rec_key, (int*)d_flags, (int)recs, s));
+        VB_CUDA(cub::DeviceSelect::Flagged(nullptr, t4, (const int32_t*)d_v2, (const uint8_t*)d_keep, h.rec_val, (int*)d_flags, (int)recs, s));
+        tmp_bytes = std::max(std::max(t1, t2), std::max(t3, t4));
+        VB_TRY(workspace(WSB_TMP, tmp_bytes, &d_tmp));
+    }
+    int occ_ins = 1, occ_upd = 1;
+    VB_TRY(K.insert(BuildDev{}, nullptr, 0, 0, 0, smem_ins, &occ_ins));
+    VB_TRY(K.update(BuildDev{}, nullptr, nullptr, 0, InsertRec{}, 0, smem_upd, &occ_upd));
+    const int max_grid_ins = c.sm_count * std::max(1, occ_ins);
+    const int max_grid_upd = c.sm_count * std::max(1, occ_upd) * 4;
+    uint32_t cap = 1u << 14;
+    while (cap < (uint32_t)(efc * m * 16) && cap < (1u << 22)) cap <<= 1;
+    auto reserve_vis = [&](uint32_t vis_cap) -> int {
+        const size_t need = (size_t)max_grid_ins * HN_WARPS * vis_cap * sizeof(uint32_t);
+        if (h.vis_bytes >= need) return VB_OK;
+        if (h.vis) {
+            VB_CUDA(cudaStreamSynchronize(s));
+            cudaFree(h.vis);
+            h.vis = nullptr;
+            h.vis_bytes = 0;
+        }
+        if (cudaMalloc(&h.vis, need) != cudaSuccess) {
+            cudaGetLastError();
+            set_error("hnsw insert: visited tables (%zu bytes) do not fit", need);
+            return VB_ENOMEM;
+        }
+        h.vis_bytes = need;
+        return VB_OK;
+    };
+    VB_TRY(reserve_vis(cap + std::max<uint32_t>(2048u, cap / 8)));
+
+    // ---- the image changes from here on
+    ++h.generation;
+    h.n_changes = 0;
+    if (rows_on_host) VB_TRY(table_append_host(h.rows, rows, n));
+    else VB_TRY(table_append_dev(h.rows, rows, n));
+    VB_CUDA(cudaMemcpyAsync(h.levels + n0, levels.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, s));
+    VB_CUDA(cudaMemcpyAsync(h.upper_off + n0, uoff.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, s));
+    VB_CUDA(cudaMemsetAsync(h.nbr0 + (size_t)n0 * lm0, 0xFF, sizeof(int32_t) * (size_t)n * lm0, s));
+    if (slots > slots0) VB_CUDA(cudaMemsetAsync(h.upper + (size_t)slots0 * m, 0xFF, sizeof(int32_t) * (size_t)(slots - slots0) * m, s));
+    VB_CUDA(cudaMemsetAsync(h.dup_of + n0, 0xFF, sizeof(int32_t) * (size_t)n, s));
+    fill_i32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(h.n_heaptids + n0, n, 1);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    h.n = n1;
+    h.upper_slots = slots;
+
+    BuildDev b{};
+    b.g.rows = h.rows.d;
+    b.g.stride = h.rows.stride;
+    b.g.V = V;
+    b.g.levels = h.levels;
+    b.g.nbr0 = h.nbr0;
+    b.g.upper_off = h.upper_off;
+    b.g.upper = h.upper;
+    b.g.m = m;
+    b.g.n = n1;
+    b.nbr0_w = h.nbr0;
+    b.upper_w = h.upper;
+    b.nd0 = h.nd0;
+    b.upper_d = h.upper_d;
+    b.dup_of = h.dup_of;
+    b.n_heaptids = h.n_heaptids;
+    b.efc = efc;
+    b.qvec = qvec;
+    b.n_edges = (int*)d_flags;
+    b.overflow = b.n_edges + 1;
+    b.edge_key = (uint64_t*)d_k1;
+    b.edge_val = (float*)d_v1;
+    const InsertRec rec{h.rec_key, h.rec_val, b.n_edges + 2};
+    VB_CUDA(cudaMemsetAsync(rec.n, 0, sizeof(int), s));
+
+    // batches as in the build (hnsw_build_fraction / hnsw_build_batch of the graph inserted into so far)
+    const int64_t frac = std::max<int64_t>(1, c.hnsw_build_fraction);
+    const int64_t b_max = std::min<int64_t>(1 << 20, std::max<int64_t>(1, c.hnsw_build_batch));
+    int64_t done = n0;
+    if (h.entry < 0) {   // empty image: the first row is the entry point, with no neighbours (src/hnswutils.c:1300-1302)
+        h.entry = n0;
+        h.entry_level = levels[0];
+        done = n0 + 1;
+    }
+    while (done < n1) {
+        int64_t B = std::min<int64_t>(std::min<int64_t>(b_max, std::max<int64_t>(1, done / frac)), n1 - done);
+        int64_t promote = -1;
+        for (int64_t i = 0; i < B; ++i)
+            if (levels[(size_t)(done - n0 + i)] > h.entry_level) {   // the entry point moves to a strictly higher level only
+                promote = done + i;
+                B = i + 1;
+                break;
+            }
+        b.g.entry = (int)h.entry;
+        b.g.entry_level = h.entry_level;
+        b.b0 = (int)done;
+        b.B = (int)B;
+        const int grid_ins = (int)std::min<int64_t>((B + HN_WARPS - 1) / HN_WARPS, max_grid_ins);
+        int flags[2] = {0, 0};
+        for (int attempt = 0;; ++attempt) {
+            const uint32_t vis_upper = std::max<uint32_t>(2048u, cap / 8);
+            const uint32_t vis_cap = cap + vis_upper;
+            VB_TRY(reserve_vis(vis_cap));
+            VB_CUDA(cudaMemsetAsync(d_flags, 0, 2 * sizeof(int), s));
+            VB_TRY(K.insert(b, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
+            hnsw_finalize_kernel<true><<<(unsigned)std::min<int64_t>((B * 32 + 127) / 128, (int64_t)c.sm_count * 16), 128, 0, s>>>(b);
+            VB_CUDA(cudaGetLastError());
+            count_launch();
+            VB_CUDA(cudaMemcpyAsync(flags, d_flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+            VB_CUDA(cudaStreamSynchronize(s));
+            if (!flags[1]) break;
+            cap <<= 2;   // a visited table overflowed: repeat the batch's searches with larger ones (nothing was published)
+            VB_REQUIRE(attempt < 5 && cap <= (1u << 26), "hnsw insert: visited set overflow");
+        }
+        const int n_edges = flags[0];
+        VB_REQUIRE(n_edges <= total_edges, "hnsw insert: record overflow (%d > %lld)", n_edges, (long long)total_edges);
+        if (n_edges > 0) {
+            size_t tb = 0;
+            VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
+                                                    n_edges, 0, 57, s));
+            VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+            VB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
+                                                    n_edges, 0, 57, s));
+            count_launch();
+            const int grid_upd = (int)std::min<int64_t>(((int64_t)n_edges + HN_WARPS - 1) / HN_WARPS, max_grid_upd);
+            VB_TRY(K.update(b, (const uint64_t*)d_k2, (const float*)d_v2, n_edges, rec, grid_upd, smem_upd, nullptr));
+        }
+        if (promote >= 0) {
+            // a folded row never becomes the entry point
+            int32_t dup = -1;
+            VB_CUDA(cudaMemcpyAsync(&dup, h.dup_of + promote, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+            VB_CUDA(cudaStreamSynchronize(s));
+            if (dup < 0) {
+                h.entry = promote;
+                h.entry_level = levels[(size_t)(promote - n0)];
+            }
+        }
+        done += B;
+    }
+
+    // ---- change records
+    hnsw_new_records_kernel<<<(unsigned)std::min<int64_t>((n * 32 + 127) / 128, (int64_t)c.sm_count * 16), 128, 0, s>>>(b, rec, n0, n);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    int n_rec = 0, n_sel = 0;
+    VB_CUDA(cudaMemcpyAsync(&n_rec, rec.n, sizeof(int), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    VB_REQUIRE(n_rec <= recs, "hnsw insert: change record overflow (%d > %lld)", n_rec, (long long)recs);
+    if (n_rec > 0) {
+        int* d_nsel = b.n_edges + 3;
+        size_t tb = 0;
+        VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)h.rec_key, (uint64_t*)d_k2, (const int32_t*)h.rec_val,
+                                                (int32_t*)d_v2, n_rec, 0, 45, s));
+        VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+        VB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)h.rec_key, (uint64_t*)d_k2, (const int32_t*)h.rec_val,
+                                                (int32_t*)d_v2, n_rec, 0, 45, s));
+        hnsw_last_of_key_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, s>>>((const uint64_t*)d_k2, n_rec, (uint8_t*)d_keep);
+        VB_CUDA(cudaGetLastError());
+        tb = 0;
+        VB_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, (const uint64_t*)d_k2, (const uint8_t*)d_keep, h.rec_key, d_nsel, n_rec, s));
+        VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+        VB_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, (const uint64_t*)d_k2, (const uint8_t*)d_keep, h.rec_key, d_nsel, n_rec, s));
+        tb = 0;
+        VB_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, (const int32_t*)d_v2, (const uint8_t*)d_keep, h.rec_val, d_nsel, n_rec, s));
+        VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+        VB_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, (const int32_t*)d_v2, (const uint8_t*)d_keep, h.rec_val, d_nsel, n_rec, s));
+        count_launch(4);
+        VB_CUDA(cudaMemcpyAsync(&n_sel, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, s));
+    }
+    if (out_dup_of) VB_CUDA(cudaMemcpyAsync(out_dup_of, h.dup_of + n0, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    h.n_changes = n_sel;
+    if (out_nchanges) *out_nchanges = n_sel;
     return VB_OK;
 }
 
@@ -676,6 +1223,57 @@ int vb_hnsw_build_dev(vb_hnsw* p, const void* rows_dev, int64_t n, int ef_constr
     VB_TRY(require_init());
     VB_REQUIRE(p, "null index");
     return hnsw_build_impl(p->h, rows_dev, false, n, ef_construction, seed, levels);
+}
+
+int vb_hnsw_insert(vb_hnsw* p, const void* rows, int64_t n, int ef_construction, uint64_t seed, const int32_t* levels, int32_t* out_dup_of,
+                   int64_t* out_nchanges) {
+    VB_TRY(require_init());
+    VB_REQUIRE(p, "null index");
+    return hnsw_insert_impl(p->h, rows, true, n, ef_construction, seed, levels, out_dup_of, out_nchanges);
+}
+
+int vb_hnsw_insert_dev(vb_hnsw* p, const void* rows_dev, int64_t n, int ef_construction, uint64_t seed, const int32_t* levels,
+                       int32_t* out_dup_of, int64_t* out_nchanges) {
+    VB_TRY(require_init());
+    VB_REQUIRE(p, "null index");
+    return hnsw_insert_impl(p->h, rows_dev, false, n, ef_construction, seed, levels, out_dup_of, out_nchanges);
+}
+
+int vb_hnsw_insert_changes(vb_hnsw* p, vb_hnsw_slot* out, int64_t cap) {
+    VB_TRY(require_init());
+    VB_REQUIRE(p && p->h.loaded, "hnsw index not loaded");
+    const Hnsw& h = p->h;
+    const int64_t nc = h.n_changes;
+    VB_REQUIRE(cap >= nc, "vb_hnsw_insert_changes: cap %lld is smaller than the %lld change records", (long long)cap, (long long)nc);
+    VB_REQUIRE(out || nc == 0, "vb_hnsw_insert_changes: null output");
+    if (nc == 0) return VB_OK;
+    std::vector<uint64_t> k((size_t)nc);
+    std::vector<int32_t> v((size_t)nc);
+    cudaStream_t s = ctx().stream;
+    VB_CUDA(cudaMemcpyAsync(k.data(), h.rec_key, sizeof(uint64_t) * (size_t)nc, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaMemcpyAsync(v.data(), h.rec_val, sizeof(int32_t) * (size_t)nc, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    for (int64_t i = 0; i < nc; ++i) {
+        out[i].element = (int32_t)(k[(size_t)i] >> 14);
+        out[i].layer = (int32_t)((k[(size_t)i] >> 8) & 63);
+        out[i].slot = (int32_t)(k[(size_t)i] & 255);
+        out[i].neighbor = v[(size_t)i];
+    }
+    return VB_OK;
+}
+
+int vb_hnsw_set_heaptid_counts(vb_hnsw* p, const int32_t* counts) {
+    VB_TRY(require_init());
+    VB_REQUIRE(p && p->h.loaded, "hnsw index not loaded");
+    Hnsw& h = p->h;
+    VB_REQUIRE(counts || h.n == 0, "null counts");
+    for (int64_t i = 0; i < h.n; ++i)
+        VB_REQUIRE(counts[i] >= 0 && counts[i] <= 10, "vb_hnsw_set_heaptid_counts: counts[%lld] = %d is not in 0..10 (HNSW_HEAPTIDS, src/hnsw.h:69)",
+                   (long long)i, counts[i]);
+    if (h.n == 0) return VB_OK;
+    VB_TRY(hnsw_ensure_counts(h));
+    VB_CUDA(cudaMemcpy(h.n_heaptids, counts, sizeof(int32_t) * (size_t)h.n, cudaMemcpyHostToDevice));
+    return VB_OK;
 }
 
 int64_t vb_hnsw_rows(const vb_hnsw* p) { return p ? p->h.n : 0; }
