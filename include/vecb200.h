@@ -290,6 +290,43 @@ int			vb_ivf_begin_load(vb_ivf *ix, const void *centers);
 int			vb_ivf_load_list(vb_ivf *ix, int list, const void *rows, const int64_t *ids, int64_t n);
 int			vb_ivf_end_load(vb_ivf *ix);
 int			vb_ivf_replace_list(vb_ivf *ix, int list, const void *rows, const int64_t *ids, int64_t n);
+/*
+ * In-place inserts and deletes (ivfflatinsert, ivfflatbulkdelete) on a loaded image, without reloading or repacking it.
+ *
+ * vb_ivf_insert is InsertTuple (src/ivfinsert.c:72-181) for each of the n rows, in call order.  Row i goes to the list
+ * FindInsertPage picks (support-1 distance to every centre, a running minimum that starts at list 0 and moves only on a
+ * strict <): for every row that is vb_ivf_scan_lists(row, 1) on the same image, except that a row whose distance to
+ * centre 0 is NaN (vector_ip_ops with elements near 1e38) stays in list 0.  out_lists[i] receives it.  Each row is
+ * appended at the end of its list, rows of one call in call order: the reference's placement whenever the list's insert
+ * page is its last page (after a build, a load, and any number of inserts).  After a VACUUM freed space on an earlier
+ * page the AM fills that space first; a caller that needs that position replaces the list (vb_ivf_replace_list).
+ * Position only decides exact ties, which list scans break by (distance, scan position).  Rows come as stored (cosine
+ * opclasses pass l2-normalised rows, as vb_ivf_load takes them); ids are the rows' heap TIDs and must not be NULL.
+ * vb_ivf_insert_dev takes device rows and ids; its out_lists (host) may be NULL.
+ *
+ * vb_ivf_delete is ivfflatbulkdelete (src/ivfvacuum.c:18-143): every row whose heap id is in ids[0 .. n) is removed, ids
+ * the image does not hold are ignored, survivors keep their order within each list, and *out_removed (may be NULL) is
+ * the reference's tuples_removed.  Lists may become empty.
+ *
+ * vb_ivf_list_offsets copies the image's list offsets, [lists + 1].
+ *
+ * Only the rows from the first changed one onward move, in place, and the derived state (list offsets, the packed
+ * planes of the tensor-core filter where they were built, and the norm bounds its certificates use) is brought up to
+ * date on the device; the centre planes are untouched.  A loaded table has no headroom: the first insert grows it by
+ * half again (the growth allocates the new table beside the old one, releasing the packed planes first when both do
+ * not fit beside them; the next batched scan rebuilds them).  A call that changes rows bumps the image's generation, as
+ * vb_ivf_replace_list does: row filters and iterative scan handles made before it fail with VB_ESTATE.  n == 0 does
+ * nothing.  An image that is not loaded, or was loaded without ids, fails with VB_ESTATE; a NULL pointer with
+ * VB_EINVAL.  After VB_EINVAL or VB_ENOMEM (whose message names the bytes) the image is as it was: the call validates,
+ * reserves and allocates before any row moves.  A CUDA error after rows started moving leaves the image unloaded (later
+ * calls get VB_ESTATE until the next load).  Images of the list-sharded search (vb_ivf_search_sharded) are not
+ * supported.
+ */
+int			vb_ivf_insert(vb_ivf *ix, const void *rows, const int64_t *ids, int64_t n, int32_t *out_lists);
+int			vb_ivf_insert_dev(vb_ivf *ix, const void *rows_dev, const int64_t *ids_dev, int64_t n,
+							  int32_t *out_lists /* host, may be NULL */ );
+int			vb_ivf_delete(vb_ivf *ix, const int64_t *ids, int64_t n, int64_t *out_removed);
+int			vb_ivf_list_offsets(const vb_ivf *ix, int64_t *out /* [lists + 1] */ );
 int			vb_ivf_free(vb_ivf *ix);
 
 /*

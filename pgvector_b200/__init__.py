@@ -390,6 +390,61 @@ class IvfflatIndex:
         self._off[l + 1:] += delta
         return self
 
+    def insert(self, rows, ids):
+        """INSERT into the resident image without reloading it (InsertTuple, src/ivfinsert.c:72-181, row after row):
+        each row is appended to the list FindInsertPage picks.  Returns the lists (int32 [n]).  ids are the rows' heap
+        ids.  Cosine opclasses: the rows are l2-normalised here, and a row of norm 0 is skipped with list -1, as
+        IvfflatCheckNorm does.  torch CUDA rows take the device path (cosine rows are normalised on the host); their
+        ids are taken as int64 on the rows' device."""
+        n = rows.shape[0] if rows.ndim > 1 else 1
+        out = np.full(n, -1, dtype=np.int32)
+        if _is_torch(rows) and rows.is_cuda and not self.normalize:
+            import torch
+            width = {VECTOR: 4, HALFVEC: 2, BIT: 1}[self.elem]
+            cols = self.dim if self.elem != BIT else (self.dim + 7) // 8
+            if rows.element_size() != width or rows.dtype.is_complex or tuple(rows.reshape(n, -1).shape) != (n, cols):
+                raise TypeError(f"device rows for {self.opclass} must be [n, {cols}] of {width}-byte elements, "
+                                f"not {tuple(rows.shape)} {rows.dtype}")
+            rows = rows.reshape(n, -1).contiguous()
+            ids = torch.as_tensor(ids, device=rows.device).to(torch.int64).reshape(n).contiguous()
+            _after_torch(rows, ids)
+            _lib.check(load().vb_ivf_insert_dev(self.h, _ptr(rows), _ptr(ids), n, _ptr(out)))
+        else:
+            if _is_torch(rows):
+                rows = rows.cpu().numpy()
+            if _is_torch(ids):
+                ids = ids.cpu().numpy()
+            rows = _host(self.elem, rows).reshape(n, -1)
+            ids = np.ascontiguousarray(ids, dtype=np.int64).reshape(n)
+            keep = slice(None)
+            if self.normalize:
+                keep = np.flatnonzero(vector_norm(rows, self.elem) > 0)
+                rows = l2_normalize(rows[keep], self.elem) if keep.size else rows[keep]
+                ids = np.ascontiguousarray(ids[keep])
+            got = np.empty(rows.shape[0], dtype=np.int32)
+            _lib.check(load().vb_ivf_insert(self.h, _ptr(np.ascontiguousarray(rows)), _ptr(ids), rows.shape[0], _ptr(got)))
+            out[keep] = got
+        self._refresh_offsets()
+        return out
+
+    def delete(self, ids):
+        """VACUUM's ivfflatbulkdelete on the resident image: removes every row whose heap id is in `ids` (ids it does not
+        hold are ignored); survivors keep their order.  Returns the number of rows removed (tuples_removed)."""
+        ids = np.ascontiguousarray(ids, dtype=np.int64).reshape(-1)
+        removed = C.c_int64(0)
+        _lib.check(load().vb_ivf_delete(self.h, _ptr(ids), ids.shape[0], C.byref(removed)))
+        self._refresh_offsets()
+        return int(removed.value)
+
+    def list_offsets(self):
+        """the image's list offsets [lists + 1]"""
+        off = np.empty(self.lists + 1, dtype=np.int64)
+        _lib.check(load().vb_ivf_list_offsets(self.h, _ptr(off)))
+        return off
+
+    def _refresh_offsets(self):
+        self._off = self.list_offsets()
+
     def scan_lists(self, queries, max_probes=None):
         """GetScanLists: nearest lists per query, ascending."""
         mp = int(max_probes or self.probes)

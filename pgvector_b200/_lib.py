@@ -70,6 +70,10 @@ SIGNATURES = {
     "vb_ivf_load_list": (_i, [_vp, _i, _vp, _vp, _i64]),
     "vb_ivf_end_load": (_i, [_vp]),
     "vb_ivf_replace_list": (_i, [_vp, _i, _vp, _vp, _i64]),
+    "vb_ivf_insert": (_i, [_vp, _vp, _vp, _i64, _vp]),
+    "vb_ivf_insert_dev": (_i, [_vp, _vp, _vp, _i64, _vp]),
+    "vb_ivf_delete": (_i, [_vp, _vp, _i64, C.POINTER(_i64)]),
+    "vb_ivf_list_offsets": (_i, [_vp, _vp]),
     "vb_ivf_free": (_i, [_vp]),
     "vb_ivf_scan_lists": (_i, [_vp, _vp, _i64, _i, _vp, _vp]),
     "vb_ivf_scan_items": (_i, [_vp, _vp, _vp, _i, _i64, _vp, _vp, _vp]),

@@ -231,6 +231,15 @@ int list_tc_prepare(const Table& rows, ListTcImage* im);
 // the int8 plane, row scales and rmax of level 0 (rows must already be prepared)
 int list_tc_prepare_l0(const Table& rows, ListTcImage* im);
 void list_tc_release(ListTcImage* im);
+// In-place changes of the table (vb_ivf_insert / vb_ivf_delete).  list_tc_reserve, before the rows move: plane buffers
+// (built ones only) that hold fewer than nt tiles are freed and allocated again with half again as many; *whole / *whole8
+// say the bf16 / int8 plane must then be packed from tile 0.  When an allocation fails the image is released (the next
+// batched scan rebuilds it, if it fits) and false is returned.  cap_tiles / cap_tiles8: the tiles the buffers hold.
+bool list_tc_reserve(ListTcImage* im, int64_t nt, int64_t* cap_tiles, int64_t* cap_tiles8, bool* whole, bool* whole8);
+// list_tc_repack, after: the planes, |x|^2 and (if built) the int8 plane, s_x and R_x re-packed from the given tiles on,
+// n_tiles set, and xmax / finite / rmax recomputed over the whole table as list_tc_prepare(_l0) compute them (d_stats:
+// 4 device words of scratch)
+int list_tc_repack(const Table& rows, ListTcImage* im, int64_t first_tile, int64_t first_tile8, unsigned* d_stats);
 int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                    const int32_t* d_lists, int probes, const int32_t* cand_off, int64_t cap, const int64_t* d_list_off, int n_lists,
                    float* out, const float** qn_out, bool one_list_all_queries = false, int level = 2, float* smin = nullptr,

@@ -75,6 +75,10 @@ struct Ivf {
     int64_t last_tc_failed = 0, total_tc_failed = 0, total_l1_failed = 0, total_l0_failed = 0;
     bool loaded = false;
     uint64_t generation = 0;          // bumped whenever rows or lists change: an iterative scan handle refuses a changed image
+    bool has_ids = false;             // loaded with heap ids (vb_ivf_insert / vb_ivf_delete need them)
+    int64_t ids_cap = -1;             // rows d_ids holds (-1: exactly rows.n, as a load allocates it)
+    int64_t tc_cap_tiles = 0;         // tiles the plane buffers of tc hold (bf16 planes + xn; int8 plane + xs + r8)
+    int64_t tc_cap_tiles8 = 0;
     // streaming load (vb_ivf_begin_load / vb_ivf_load_list / vb_ivf_end_load)
     bool loading = false;
     int next_list = 0;
@@ -312,6 +316,24 @@ static int ivf_select_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t 
     return VB_OK;
 }
 
+// the (list, table tile) work units of the tensor-core scan, from the list offsets
+static int ivf_build_units(Ivf& ix) {
+    std::vector<ListUnit> units;
+    for (int l = 0; l < ix.lists; ++l) {
+        const int64_t lo = ix.h_list_off[(size_t)l], hi = ix.h_list_off[(size_t)l + 1];
+        if (hi <= lo) continue;
+        for (int64_t t = lo / 128; t <= (hi - 1) / 128; ++t) units.push_back(ListUnit{l, (int32_t)t});
+    }
+    if (ix.tc.units) VB_CUDA(cudaFree(ix.tc.units));
+    ix.tc.units = nullptr;
+    ix.tc.n_units = (int)units.size();
+    if (!units.empty()) {
+        VB_CUDA(cudaMalloc(&ix.tc.units, sizeof(ListUnit) * units.size()));
+        VB_CUDA(cudaMemcpy(ix.tc.units, units.data(), sizeof(ListUnit) * units.size(), cudaMemcpyHostToDevice));
+    }
+    return VB_OK;
+}
+
 // packed planes, row norms and the (list, table tile) work units of the tensor-core scan; built lazily because the
 // planes double the index footprint and only batched searches use them
 static int ivf_ensure_tc_image(Ivf& ix) {
@@ -327,18 +349,8 @@ static int ivf_ensure_tc_image(Ivf& ix) {
         }
     }
     VB_TRY(list_tc_prepare(ix.rows, &ix.tc));
-    std::vector<ListUnit> units;
-    for (int l = 0; l < ix.lists; ++l) {
-        const int64_t lo = ix.h_list_off[(size_t)l], hi = ix.h_list_off[(size_t)l + 1];
-        if (hi <= lo) continue;
-        for (int64_t t = lo / 128; t <= (hi - 1) / 128; ++t) units.push_back(ListUnit{l, (int32_t)t});
-    }
-    ix.tc.n_units = (int)units.size();
-    if (!units.empty()) {
-        VB_CUDA(cudaMalloc(&ix.tc.units, sizeof(ListUnit) * units.size()));
-        VB_CUDA(cudaMemcpy(ix.tc.units, units.data(), sizeof(ListUnit) * units.size(), cudaMemcpyHostToDevice));
-    }
-    return VB_OK;
+    ix.tc_cap_tiles = ix.tc.n_tiles;
+    return ivf_build_units(ix);
 }
 
 // the int8 plane of level 0 (a quarter of the bf16 planes), built on first use where it fits with 4 GiB to spare
@@ -352,6 +364,7 @@ static int ivf_ensure_l0_image(Ivf& ix) {
         ix.tc.l0_tried = true;
         return VB_OK;
     }
+    ix.tc_cap_tiles8 = ix.tc.n_tiles;
     return list_tc_prepare_l0(ix.rows, &ix.tc);
 }
 
@@ -1001,7 +1014,10 @@ int vb_ivf_create(int elem, int metric, int dim, int lists, vb_ivf** out) {
     return VB_OK;
 }
 
-static int ivf_set_offsets(Ivf& ix, const int64_t* list_offsets) {
+// list offsets, lengths, device offsets and list-major row tiles; release: a load or list replacement, whose rows are
+// about to change (the packed planes are rebuilt on the next tensor-core scan), rather than an in-place insert or delete
+// (which re-packs them itself)
+static int ivf_set_layout(Ivf& ix, const int64_t* list_offsets, bool release) {
     ix.h_list_off.assign(list_offsets, list_offsets + ix.lists + 1);
     VB_REQUIRE(ix.h_list_off[0] == 0, "list_offsets[0] must be 0");
     ix.sorted_len.resize((size_t)ix.lists);
@@ -1022,8 +1038,11 @@ static int ivf_set_offsets(Ivf& ix, const int64_t* list_offsets) {
     }
     if (ix.d_tiles) cudaFree(ix.d_tiles);
     ix.d_tiles = nullptr;
-    list_tc_release(&ix.tc);   // rows are about to change: planes are rebuilt on the next tensor-core scan
-    list_tc_release(&ix.ctc);
+    if (release) {
+        list_tc_release(&ix.tc);   // rows are about to change: planes are rebuilt on the next tensor-core scan
+        list_tc_release(&ix.ctc);
+        ix.ids_cap = -1;
+    }
     ix.n_tiles = (int)tiles.size();
     if (ix.n_tiles) {
         VB_CUDA(cudaMalloc(&ix.d_tiles, sizeof(ListTile) * tiles.size()));
@@ -1031,6 +1050,8 @@ static int ivf_set_offsets(Ivf& ix, const int64_t* list_offsets) {
     }
     return VB_OK;
 }
+
+static int ivf_set_offsets(Ivf& ix, const int64_t* list_offsets) { return ivf_set_layout(ix, list_offsets, true); }
 
 int vb_ivf_load(vb_ivf* h, const void* centers, const int64_t* list_offsets, const void* rows, const int64_t* ids) {
     VB_TRY(require_init());
@@ -1045,6 +1066,7 @@ int vb_ivf_load(vb_ivf* h, const void* centers, const int64_t* list_offsets, con
     VB_TRY(table_append_host(ix.rows, rows, n));
     if (ix.d_ids) cudaFree(ix.d_ids);
     ix.d_ids = nullptr;
+    ix.has_ids = ids != nullptr;
     if (ids && n > 0) {
         VB_CUDA(cudaMalloc(&ix.d_ids, sizeof(int64_t) * (size_t)n));
         VB_CUDA(cudaMemcpy(ix.d_ids, ids, sizeof(int64_t) * (size_t)n, cudaMemcpyHostToDevice));
@@ -1067,6 +1089,7 @@ int vb_ivf_load_dev(vb_ivf* h, const void* centers_dev, const int64_t* list_offs
     VB_TRY(table_append_dev(ix.rows, rows_dev, n));
     if (ix.d_ids) cudaFree(ix.d_ids);
     ix.d_ids = nullptr;
+    ix.has_ids = ids_dev != nullptr;
     if (ids_dev && n > 0) {
         VB_CUDA(cudaMalloc(&ix.d_ids, sizeof(int64_t) * (size_t)n));
         VB_CUDA(cudaMemcpyAsync(ix.d_ids, ids_dev, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToDevice, ctx().stream));
@@ -1123,6 +1146,7 @@ int vb_ivf_end_load(vb_ivf* h) {
     VB_TRY(ivf_set_offsets(ix, ix.pending_off.data()));
     if (ix.d_ids) cudaFree(ix.d_ids);
     ix.d_ids = nullptr;
+    ix.has_ids = true;
     const int64_t n = ix.rows.n;
     if (n > 0) {
         VB_CUDA(cudaMalloc(&ix.d_ids, sizeof(int64_t) * (size_t)n));
@@ -1183,6 +1207,352 @@ int vb_ivf_replace_list(vb_ivf* h, int list, const void* rows, const int64_t* id
     const int64_t delta = n - (hi - lo);
     for (int l = list + 1; l <= ix.lists; ++l) off[(size_t)l] += delta;
     return ivf_set_offsets(ix, off.data());
+}
+
+// ---- in-place inserts and deletes (ivfflatinsert, ivfflatbulkdelete)
+//
+// Both move the rows of the list-ordered table to new places in a monotone pattern: an insert moves every row up by the
+// rows inserted into lists before its own, a delete moves every kept row down by the rows removed before it.  Only the
+// suffix from the first changed row moves, window by window through a bounded staging buffer -- back to front when rows
+// move up, front to back when they move down -- so that no window's destinations reach the sources of a window not yet
+// staged, and the table is never copied whole.  The derived state follows in place: list offsets and tiles, and the
+// packed planes of the tensor-core filter (where built) from the 128-row tile that holds the first changed row on, with
+// the norm statistics its certificates use recomputed over the whole table (list_tc_repack).
+
+constexpr size_t IVF_MOVE_WINDOW_BYTES = (size_t)256 << 20;
+
+// one warp per row: row i of src and its id to table row dst[i] (dst[i] < 0: dropped)
+__global__ void ivf_move_rows_kernel(const uint8_t* __restrict__ src, const int64_t* __restrict__ src_ids, int64_t m,
+                                     const int64_t* __restrict__ dst, size_t stride, uint8_t* __restrict__ rows, int64_t* __restrict__ ids) {
+    const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (i >= m) return;
+    const int64_t d = dst[i];
+    if (d < 0) return;
+    const uint4* s = reinterpret_cast<const uint4*>(src + (size_t)i * stride);
+    uint4* o = reinterpret_cast<uint4*>(rows + (size_t)d * stride);
+    for (size_t w = lane; w < stride / 16; w += 32) o[w] = s[w];
+    if (lane == 0) ids[d] = src_ids[i];
+}
+
+// insert: row first + i of list l goes to first + i + shift[l] (list_off: the offsets before the insert)
+__global__ void ivf_insert_dst_kernel(const int64_t* __restrict__ list_off, int lists, const int64_t* __restrict__ shift, int64_t first,
+                                      int64_t n, int64_t* __restrict__ dst) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int64_t r = first + i;
+    if (r >= n) return;
+    int lo = 0, hi = lists;   // the list of row r: the largest l with list_off[l] <= r (list_off[lists] = n > r)
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (list_off[mid] <= r) lo = mid;
+        else hi = mid;
+    }
+    dst[i] = r + shift[lo];
+}
+
+// delete: row first + i goes down by the removed rows before it, or is dropped (gone[0 .. m): the removed rows, ascending)
+__global__ void ivf_delete_dst_kernel(const int64_t* __restrict__ gone, int64_t m, int64_t first, int64_t n, int64_t* __restrict__ dst) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int64_t r = first + i;
+    if (r >= n) return;
+    int64_t lo = 0, hi = m;   // first gone[j] >= r
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (gone[mid] < r) lo = mid + 1;
+        else hi = mid;
+    }
+    dst[i] = lo < m && gone[lo] == r ? -1 : r - lo;
+}
+
+// table rows [first, n) to dst[0 .. n - first), in windows of `window` rows staged in stage / stage_ids
+static int ivf_move_suffix(Ivf& ix, int64_t first, int64_t n, const int64_t* dst, bool up, uint8_t* stage, int64_t* stage_ids,
+                           int64_t window) {
+    Context& c = ctx();
+    const size_t stride = ix.rows.stride;
+    const int64_t nwin = (n - first + window - 1) / window;
+    for (int64_t w = 0; w < nwin; ++w) {
+        const int64_t a = up ? std::max(first, n - (w + 1) * window) : first + w * window;
+        const int64_t m = up ? n - w * window - a : std::min(window, n - a);
+        VB_CUDA(cudaMemcpyAsync(stage, ix.rows.d + (size_t)a * stride, (size_t)m * stride, cudaMemcpyDeviceToDevice, c.stream));
+        VB_CUDA(cudaMemcpyAsync(stage_ids, ix.d_ids + a, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToDevice, c.stream));
+        ivf_move_rows_kernel<<<(unsigned)((m * 32 + 255) / 256), 256, 0, c.stream>>>(stage, stage_ids, m, dst + (a - first), stride, ix.rows.d,
+                                                                                   ix.d_ids);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    return VB_OK;
+}
+
+// FindInsertPage (src/ivfinsert.c:19-67) for n rows: the list vb_ivf_scan_lists(rows, 1) selects (the fused one-query
+// kernel for a few rows, the certified tensor-core pass for batches), except that a row whose distance to centre 0 is NaN
+// stays in list 0: the reference's running minimum starts there, and no distance compares smaller than a NaN
+static int ivf_insert_lists(Ivf& ix, const void* rows, int64_t n, bool host, int32_t* out) {
+    Context& c = ctx();
+    const size_t raw = raw_row_bytes(ix.elem, ix.dim);
+    const int64_t bq = 65535;
+    std::vector<float> d0;
+    for (int64_t q0 = 0; q0 < n; q0 += bq) {
+        const int64_t m = std::min(bq, n - q0);
+        void* qimg;
+        size_t qstride;
+        VB_TRY(upload_queries(ix.elem, ix.dim, (const uint8_t*)rows + (size_t)q0 * raw, m, host, WS_QIMG, &qimg, &qstride));
+        int32_t* d_lists;
+        float* d_ldist;
+        if (c.one_query && m <= ONE_MAX_Q && one_probe_fits(ix.lists, qstride, 1))
+            VB_TRY(ivf_one_probes(ix, qimg, qstride, m, 1, &d_lists, &d_ldist));
+        else
+            VB_TRY(ivf_select_probes(ix, qimg, qstride, m, 1, &d_lists, &d_ldist));
+        VB_CUDA(cudaMemcpyAsync(out + q0, d_lists, sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c.stream));
+        if (ix.elem != VB_BIT) {   // (Hamming distances are never NaN)
+            void* d_d0;
+            VB_TRY(workspace(WS_DIST, sizeof(float) * (size_t)m, &d_d0));
+            VB_TRY(launch_scan_regular(ix.centers, key_metric(ix.metric), qimg, qstride, m, 1, (float*)d_d0, 1));
+            d0.resize((size_t)m);
+            VB_CUDA(cudaMemcpyAsync(d0.data(), d_d0, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c.stream));
+        }
+        VB_CUDA(cudaStreamSynchronize(c.stream));
+        if (ix.elem != VB_BIT)
+            for (int64_t i = 0; i < m; ++i)
+                if (std::isnan(d0[(size_t)i])) out[q0 + i] = 0;
+    }
+    return VB_OK;
+}
+
+// Temporaries of one insert or delete: one device allocation, freed on every exit
+struct IvfTmp {
+    void* mem = nullptr;
+    ~IvfTmp() {
+        if (mem) {
+            cudaStreamSynchronize(ctx().stream);
+            cudaFree(mem);
+        }
+    }
+};
+
+static int ivf_alloc_tmp(const char* fn, IvfTmp& tmp, size_t bytes) {
+    if (cudaMalloc(&tmp.mem, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        tmp.mem = nullptr;
+        set_error("%s: allocation of %zu bytes of device memory failed", fn, bytes);
+        return VB_ENOMEM;
+    }
+    return VB_OK;
+}
+
+// list offsets and tiles of the changed image, and its planes re-packed from the tile of row `first` on
+static int ivf_finish_update(Ivf& ix, const std::vector<int64_t>& new_off, int64_t first, bool whole, bool whole8, unsigned* d_stats) {
+    // the move kernels still read the old offsets from d_list_off, which ivf_set_layout overwrites with a copy that is
+    // not ordered after the library stream's work
+    VB_CUDA(cudaStreamSynchronize(ctx().stream));
+    VB_TRY(ivf_set_layout(ix, new_off.data(), false));
+    if (ix.tc.planes) {
+        VB_TRY(list_tc_repack(ix.rows, &ix.tc, whole ? 0 : first / 128, whole8 ? 0 : first / 128, d_stats));
+        VB_TRY(ivf_build_units(ix));
+    }
+    VB_CUDA(cudaStreamSynchronize(ctx().stream));
+    return VB_OK;
+}
+
+static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+static int ivf_insert_impl(const char* fn, vb_ivf* h, const void* rows, const int64_t* ids, int64_t n, int32_t* out_lists, bool host) {
+    VB_TRY(require_init());
+    VB_REQUIRE(h, "%s: null index", fn);
+    if (!h->ix.loaded) {
+        set_error("%s: index not loaded", fn);
+        return VB_ESTATE;
+    }
+    if (!h->ix.has_ids) {
+        set_error("%s: the index was loaded without heap ids", fn);
+        return VB_ESTATE;
+    }
+    VB_REQUIRE(n >= 0, "%s: negative row count %lld", fn, (long long)n);
+    if (n == 0) return VB_OK;
+    VB_REQUIRE(rows && ids, "%s: rows and ids must not be NULL", fn);
+    Ivf& ix = h->ix;
+    Context& c = ctx();
+    const int64_t n_old = ix.rows.n, n_new = n_old + n;
+    const size_t stride = ix.rows.stride, raw = raw_row_bytes(ix.elem, ix.dim);
+    std::vector<int32_t> lists((size_t)n);
+    VB_TRY(ivf_insert_lists(ix, rows, n, host, lists.data()));
+    if (out_lists) memcpy(out_lists, lists.data(), sizeof(int32_t) * (size_t)n);
+    // placement: appended to its list, rows of the call in call order
+    const int L = ix.lists;
+    std::vector<int64_t> cnt((size_t)L, 0), shift((size_t)L), new_off((size_t)L + 1), fill((size_t)L);
+    for (int32_t l : lists) ++cnt[(size_t)l];
+    int64_t before = 0;
+    int lmin = L;
+    for (int l = 0; l < L; ++l) {
+        shift[(size_t)l] = before;
+        new_off[(size_t)l] = ix.h_list_off[(size_t)l] + before;
+        fill[(size_t)l] = ix.h_list_off[(size_t)l + 1] + before;   // the new rows of list l start at its old end, moved
+        before += cnt[(size_t)l];
+        if (cnt[(size_t)l] && lmin == L) lmin = l;
+    }
+    new_off[(size_t)L] = n_new;
+    const int64_t first = ix.h_list_off[(size_t)lmin + 1];         // rows before the end of the first list that grows stay
+    std::vector<int64_t> dst_new((size_t)n);
+    for (int64_t i = 0; i < n; ++i) dst_new[(size_t)i] = fill[(size_t)lists[(size_t)i]]++;
+    // reserve and allocate everything before a row moves
+    const int64_t suffix = n_old - first;
+    const int64_t window = std::max<int64_t>(1, std::min<int64_t>(suffix, (int64_t)(IVF_MOVE_WINDOW_BYTES / stride)));
+    const size_t tmp_bytes = align256(8 * (size_t)(suffix + n)) + align256(8 * (size_t)L) + align256(16) +
+                             (suffix > 0 ? align256((size_t)window * stride) + align256(8 * (size_t)window) : 0) + align256((size_t)n * stride) +
+                             (host ? align256(8 * (size_t)n) : 0);
+    const int64_t ids_cap = ix.ids_cap < 0 ? n_old : ix.ids_cap;
+    if (n_new > ix.rows.cap || n_new > ids_cap) {
+        // growth by half again: release the packed planes first when the larger table does not fit beside them (the
+        // next batched scan rebuilds them, if they fit then)
+        const int64_t ncap = std::max(n_new, ix.rows.cap + ix.rows.cap / 2);
+        const size_t grow = (size_t)ncap * (stride + 8) + tmp_bytes;
+        size_t free_b = 0, total_b = 0;
+        VB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        if (free_b < grow + ((size_t)1 << 30) && ix.tc.planes) {
+            list_tc_release(&ix.tc);
+            ix.tc_cap_tiles = ix.tc_cap_tiles8 = 0;
+        }
+        const int rc = table_reserve(ix.rows, n_new);
+        if (rc != VB_OK) {
+            set_error("%s: growing the row table to %lld rows (%zu bytes) failed", fn, (long long)n_new, (size_t)n_new * stride);
+            return rc;
+        }
+        int64_t* nid = nullptr;
+        if (cudaMalloc(&nid, sizeof(int64_t) * (size_t)ix.rows.cap) != cudaSuccess) {
+            cudaGetLastError();
+            set_error("%s: allocation of %zu bytes for the heap ids failed", fn, sizeof(int64_t) * (size_t)ix.rows.cap);
+            return VB_ENOMEM;
+        }
+        if (n_old) VB_CUDA(cudaMemcpyAsync(nid, ix.d_ids, sizeof(int64_t) * (size_t)n_old, cudaMemcpyDeviceToDevice, c.stream));
+        VB_CUDA(cudaStreamSynchronize(c.stream));
+        if (ix.d_ids) cudaFree(ix.d_ids);
+        ix.d_ids = nid;
+        ix.ids_cap = ix.rows.cap;
+    }
+    IvfTmp tmp;
+    VB_TRY(ivf_alloc_tmp(fn, tmp, tmp_bytes));
+    uint8_t* p = (uint8_t*)tmp.mem;
+    auto take = [&](size_t b) {
+        uint8_t* q = p;
+        p += align256(b);
+        return q;
+    };
+    int64_t* d_dst = (int64_t*)take(8 * (size_t)(suffix + n));   // the suffix's destinations, then the new rows'
+    int64_t* d_shift = (int64_t*)take(8 * (size_t)L);
+    unsigned* d_stats = (unsigned*)take(16);
+    uint8_t* stage = suffix > 0 ? take((size_t)window * stride) : nullptr;
+    int64_t* stage_ids = suffix > 0 ? (int64_t*)take(8 * (size_t)window) : nullptr;
+    uint8_t* d_rows = take((size_t)n * stride);
+    const int64_t* d_new_ids = host ? (const int64_t*)take(8 * (size_t)n) : ids;
+    bool whole = false, whole8 = false;
+    if (ix.tc.planes && !list_tc_reserve(&ix.tc, (n_new + 127) / 128, &ix.tc_cap_tiles, &ix.tc_cap_tiles8, &whole, &whole8))
+        ix.tc_cap_tiles = ix.tc_cap_tiles8 = 0;
+    // the new rows at the table's stride, their ids and destinations
+    if (raw != stride) VB_CUDA(cudaMemsetAsync(d_rows, 0, (size_t)n * stride, c.stream));
+    VB_CUDA(cudaMemcpy2DAsync(d_rows, stride, rows, raw, raw, (size_t)n, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c.stream));
+    if (host) VB_CUDA(cudaMemcpyAsync((void*)d_new_ids, ids, 8 * (size_t)n, cudaMemcpyHostToDevice, c.stream));
+    VB_CUDA(cudaMemcpyAsync(d_dst + suffix, dst_new.data(), 8 * (size_t)n, cudaMemcpyHostToDevice, c.stream));
+    VB_CUDA(cudaMemcpyAsync(d_shift, shift.data(), 8 * (size_t)L, cudaMemcpyHostToDevice, c.stream));
+    VB_CUDA(cudaStreamSynchronize(c.stream));   // (host vectors)
+    ++ix.generation;
+    auto move = [&]() -> int {
+        if (suffix > 0) {
+            ivf_insert_dst_kernel<<<(unsigned)((suffix + 255) / 256), 256, 0, c.stream>>>(ix.d_list_off, L, d_shift, first, n_old, d_dst);
+            VB_CUDA(cudaGetLastError());
+            count_launch();
+            VB_TRY(ivf_move_suffix(ix, first, n_old, d_dst, true, stage, stage_ids, window));
+        }
+        ivf_move_rows_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, c.stream>>>(d_rows, d_new_ids, n, d_dst + suffix, stride, ix.rows.d,
+                                                                                    ix.d_ids);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+        ix.rows.n = n_new;
+        return ivf_finish_update(ix, new_off, first, whole, whole8, d_stats);
+    };
+    const int rc = move();
+    if (rc != VB_OK) ix.loaded = false;   // rows may have moved: the image must be loaded again
+    return rc;
+}
+
+int vb_ivf_insert(vb_ivf* h, const void* rows, const int64_t* ids, int64_t n, int32_t* out_lists) {
+    VB_REQUIRE(out_lists || n <= 0, "vb_ivf_insert: out_lists must not be NULL");
+    return ivf_insert_impl("vb_ivf_insert", h, rows, ids, n, out_lists, true);
+}
+
+int vb_ivf_insert_dev(vb_ivf* h, const void* rows_dev, const int64_t* ids_dev, int64_t n, int32_t* out_lists) {
+    return ivf_insert_impl("vb_ivf_insert_dev", h, rows_dev, ids_dev, n, out_lists, false);
+}
+
+int vb_ivf_delete(vb_ivf* h, const int64_t* ids, int64_t n, int64_t* out_removed) {
+    VB_TRY(require_init());
+    const char* fn = "vb_ivf_delete";
+    VB_REQUIRE(h, "%s: null index", fn);
+    if (!h->ix.loaded) {
+        set_error("%s: index not loaded", fn);
+        return VB_ESTATE;
+    }
+    if (!h->ix.has_ids) {
+        set_error("%s: the index was loaded without heap ids", fn);
+        return VB_ESTATE;
+    }
+    VB_REQUIRE(n >= 0 && (ids || n == 0), "%s: null ids or negative count %lld", fn, (long long)n);
+    if (out_removed) *out_removed = 0;
+    Ivf& ix = h->ix;
+    Context& c = ctx();
+    const int64_t n_old = ix.rows.n;
+    if (n == 0 || n_old == 0) return VB_OK;
+    // the rows to remove: a row filter of the ids (sorted on the device, one binary search per row, a ballot per bitset
+    // word, compacted by a prefix scan), and its per-list counts
+    struct FilterHold {
+        Filter f;
+        ~FilterHold() {
+            if (f.mem) cudaStreamSynchronize(ctx().stream);
+            filter_release(&f);
+        }
+    } gone;
+    VB_TRY(filter_build_ivf(n_old, ix.d_ids, ix.d_list_off, ix.lists, ids, n, true, &gone.f));
+    const int64_t m = gone.f.n;
+    if (m == 0) return VB_OK;
+    int64_t first = 0;
+    VB_CUDA(cudaMemcpy(&first, gone.f.pos, sizeof(int64_t), cudaMemcpyDeviceToHost));
+    const int L = ix.lists;
+    std::vector<int64_t> new_off((size_t)L + 1);
+    for (int l = 0; l <= L; ++l) new_off[(size_t)l] = ix.h_list_off[(size_t)l] - gone.f.h_off[(size_t)l];
+    const int64_t suffix = n_old - first;
+    const size_t stride = ix.rows.stride;
+    const int64_t window = std::max<int64_t>(1, std::min<int64_t>(suffix, (int64_t)(IVF_MOVE_WINDOW_BYTES / stride)));
+    IvfTmp tmp;
+    VB_TRY(ivf_alloc_tmp(fn, tmp, align256(8 * (size_t)suffix) + align256(16) + align256((size_t)window * stride) + align256(8 * (size_t)window)));
+    int64_t* d_dst = (int64_t*)tmp.mem;
+    unsigned* d_stats = (unsigned*)((uint8_t*)tmp.mem + align256(8 * (size_t)suffix));
+    uint8_t* stage = (uint8_t*)d_stats + align256(16);
+    int64_t* stage_ids = (int64_t*)(stage + align256((size_t)window * stride));
+    ++ix.generation;
+    auto move = [&]() -> int {
+        ivf_delete_dst_kernel<<<(unsigned)((suffix + 255) / 256), 256, 0, c.stream>>>(gone.f.pos, m, first, n_old, d_dst);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+        VB_TRY(ivf_move_suffix(ix, first, n_old, d_dst, false, stage, stage_ids, window));
+        ix.rows.n = n_old - m;
+        return ivf_finish_update(ix, new_off, first, false, false, d_stats);
+    };
+    const int rc = move();
+    if (rc != VB_OK) {
+        ix.loaded = false;
+        return rc;
+    }
+    if (out_removed) *out_removed = m;
+    return VB_OK;
+}
+
+int vb_ivf_list_offsets(const vb_ivf* h, int64_t* out) {
+    VB_TRY(require_init());
+    VB_REQUIRE(h && out, "vb_ivf_list_offsets: null argument");
+    if (!h->ix.loaded) {
+        set_error("vb_ivf_list_offsets: index not loaded");
+        return VB_ESTATE;
+    }
+    memcpy(out, h->ix.h_list_off.data(), sizeof(int64_t) * ((size_t)h->ix.lists + 1));
+    return VB_OK;
 }
 
 int vb_ivf_free(vb_ivf* h) {

@@ -1368,6 +1368,114 @@ void list_tc_release(ListTcImage* im) {
     *im = ListTcImage{};
 }
 
+// the whole table's norm statistics after an in-place change, as list_tc_prepare (host loop over |x|^2) and
+// list_tc_prepare_l0 (atomicMax of R_x) compute them: out[0] = max finite |x|^2 (float bits), out[1] = 1 when some
+// |x|^2 is NaN or above 3e38, out[2] = max R_x (float bits; r8 may be NULL)
+__global__ void norm_stats_kernel(const float* __restrict__ xn, const float* __restrict__ r8, int64_t n, unsigned* __restrict__ out) {
+    unsigned m2 = 0u, bad = 0u, rm = 0u;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const float v = xn[i];
+        if (!(v == v) || v > 3.0e38f) bad = 1u;
+        else m2 = max(m2, __float_as_uint(v));
+        if (r8) rm = max(rm, __float_as_uint(r8[i]));
+    }
+    if (m2) atomicMax(&out[0], m2);
+    if (bad) atomicMax(&out[1], bad);
+    if (rm) atomicMax(&out[2], rm);
+}
+
+bool list_tc_reserve(ListTcImage* im, int64_t nt, int64_t* cap_tiles, int64_t* cap_tiles8, bool* whole, bool* whole8) {
+    *whole = *whole8 = false;
+    bool ok = true;
+    if (im->planes && nt > *cap_tiles) {
+        // planes and norms are derived from the rows: the old buffers go before the larger ones are allocated
+        cudaFree(im->planes);
+        cudaFree(im->xn);
+        im->planes = nullptr;
+        im->xn = nullptr;
+        const int64_t cap = std::max(nt, *cap_tiles + *cap_tiles / 2);
+        ok = cudaMalloc(&im->planes, std::max<size_t>((size_t)cap * im->n_kblocks * LC_A_STAGE, 16)) == cudaSuccess &&
+             cudaMalloc(&im->xn, sizeof(float) * (size_t)cap * LC_M) == cudaSuccess;
+        *cap_tiles = cap;
+        *whole = true;
+    }
+    if (ok && im->planes8 && nt > *cap_tiles8) {
+        cudaFree(im->planes8);
+        cudaFree(im->xs);
+        cudaFree(im->r8);
+        im->planes8 = nullptr;
+        im->xs = im->r8 = nullptr;
+        const int64_t cap = std::max(nt, *cap_tiles8 + *cap_tiles8 / 2);
+        ok = cudaMalloc(&im->planes8, std::max<size_t>((size_t)cap * im->n_kblocks8 * LC_A_PLANE, 16)) == cudaSuccess &&
+             cudaMalloc(&im->xs, sizeof(float) * (size_t)cap * LC_M) == cudaSuccess &&
+             cudaMalloc(&im->r8, sizeof(float) * (size_t)cap * LC_M) == cudaSuccess;
+        *cap_tiles8 = cap;
+        *whole8 = true;
+    }
+    if (!ok) {
+        cudaGetLastError();
+        list_tc_release(im);
+        *cap_tiles = *cap_tiles8 = 0;
+    }
+    return ok;
+}
+
+int list_tc_repack(const Table& rows, ListTcImage* im, int64_t first_tile, int64_t first_tile8, unsigned* d_stats) {
+    Context& c = ctx();
+    cudaStream_t s = c.stream;
+    const int64_t n = rows.n;
+    const int64_t nt = (n + LC_M - 1) / LC_M;
+    const bool l0 = im->planes8 != nullptr;
+    const int64_t t0 = std::min(first_tile, nt), t08 = std::min(first_tile8, nt);
+    im->n_tiles = nt;
+    VB_CUDA(cudaMemsetAsync(d_stats, 0, 4 * sizeof(unsigned), s));
+    if (nt > t0) {
+        const int64_t r0 = t0 * LC_M, pr = (nt - t0) * LC_M;
+        const unsigned grid = (unsigned)((pr * im->n_kblocks * 8 + 255) / 256);
+        const unsigned g2 = (unsigned)((pr * 32 + 255) / 256);
+        uint8_t* planes = im->planes + (size_t)t0 * im->n_kblocks * LC_A_STAGE;
+        if (rows.elem == VB_VECTOR) {
+            pack_planes_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(rows.d, rows.stride, r0, n - r0, rows.dim, LC_M, im->n_kblocks, planes, nullptr);
+            row_sqnorm_kernel<VB_VECTOR><<<g2, 256, 0, s>>>(rows.d + (size_t)r0 * rows.stride, rows.stride, n - r0, rows.dim, im->xn + r0, pr, 0.f);
+        } else {
+            pack_planes_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(rows.d, rows.stride, r0, n - r0, rows.dim, LC_M, im->n_kblocks, planes, nullptr);
+            row_sqnorm_kernel<VB_HALFVEC><<<g2, 256, 0, s>>>(rows.d + (size_t)r0 * rows.stride, rows.stride, n - r0, rows.dim, im->xn + r0, pr, 0.f);
+        }
+        VB_CUDA(cudaGetLastError());
+        count_launch(2);
+    }
+    if (l0 && nt > t08) {
+        const int64_t r0 = t08 * LC_M, pr = (nt - t08) * LC_M;
+        const unsigned grid = (unsigned)((pr * 32 + 255) / 256);
+        uint8_t* planes8 = im->planes8 + (size_t)t08 * im->n_kblocks8 * LC_A_PLANE;
+        const uint8_t* src = rows.d + (size_t)r0 * rows.stride;
+        if (rows.elem == VB_VECTOR)
+            pack_rows_i8_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(src, rows.stride, n - r0, rows.dim, im->n_kblocks8, pr, planes8, im->xs + r0,
+                                                                im->r8 + r0, d_stats + 3);
+        else
+            pack_rows_i8_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(src, rows.stride, n - r0, rows.dim, im->n_kblocks8, pr, planes8, im->xs + r0,
+                                                                 im->r8 + r0, d_stats + 3);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    if (n > 0) {
+        norm_stats_kernel<<<(unsigned)std::min<int64_t>((n + 255) / 256, 4 * (int64_t)c.sm_count), 256, 0, s>>>(im->xn, l0 ? im->r8 : nullptr,
+                                                                                                             n, d_stats);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    unsigned st[4] = {0u, 0u, 0u, 0u};
+    VB_CUDA(cudaMemcpyAsync(st, d_stats, sizeof(st), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    float m2, rmax;
+    memcpy(&m2, &st[0], sizeof(float));
+    memcpy(&rmax, &st[2], sizeof(float));
+    im->xmax = std::sqrt(m2);
+    im->finite = st[1] == 0u;
+    if (l0) im->rmax = rmax;
+    return VB_OK;
+}
+
 // approximate pass: fills `out` (the per-query candidate runs) with d~
 int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                    const int32_t* d_lists, int probes, const int32_t* cand_off, int64_t cap, const int64_t* d_list_off, int n_lists,
