@@ -274,7 +274,7 @@ int launch_assign_tc(const Table& X, int metric, const Table& Cn, int k, int32_t
         a.k = k;
         a.is_l2 = is_l2;
         a.cmax = std::sqrt(cmax2);
-        // |err(x.c)| <= tol |x||c| for the split product (same derivation as launch_list_tc_refine, vb_list_tc.cu):
+        // |err(x.c)| <= tol |x||c| for the split product (same derivation as lc_make_bound, vb_list_tc.cu):
         //   representation: hi.hi + hi.lo + lo.hi drops lo.lo and the two bf16 residuals: 3 * 2^-16;
         //   accumulation: one fp32 rounding of the accumulator per MMA, 3 MMAs per 16-element K step, 2^-23 each
         //     (truncation), doubled for the alignment of the 16 products inside an MMA -> 6 * (dim / 16) * 2^-23.
@@ -338,10 +338,6 @@ int vb_set_option(const char* name, int64_t value) {
     }
     if (!strcmp(name, "pp_filter")) {
         vb::ctx().pp_filter = (int)value;
-        return VB_OK;
-    }
-    if (!strcmp(name, "fused_refine")) {
-        vb::ctx().fused_refine = (int)value;
         return VB_OK;
     }
     if (!strcmp(name, "hnsw_l2_persist")) {

@@ -53,9 +53,6 @@ struct Context {
     int tc_level0 = 1;                 // ... and in front of it the int8 filter, where tc_level1 is on (vb_set_option "tc_level0")
     int pp_filter = 1;                 // k-means++ on large fp32 sample tables: triangle-inequality + bf16 filters in front of the exact distances
     unsigned long long pp_stats[3] = {0, 0, 0};   // last seeding: samples skipped by the triangle rule / stopped by the bf16 bound / re-scored exactly
-    int fused_refine = 3;              // tensor-core filter, after the k' select: 3 = select + exact re-score + certificate with one CTA per query,
-                                       // 1 = re-score + certificate in one warp-per-query kernel fed by the selection kernel,
-                                       // 0 = rescore_kernel + certify_kernel, 2 = the select runs inside the warp-per-query kernel too
     int one_query = 1;                 // scans of at most 16 queries: two fused distance + select kernels (vb_ivf_one.cu); 0 = the general path
     int scan_impl = 2;                 // 0 = LDG variant (vb_scan.cu), 1 = bulk-copy / TMA variant (vb_scan_bulk.cu), 2 = by table size
     int hnsw_build_fraction = 64;      // HNSW build: a batch is at most 1/fraction of the elements already inserted
@@ -248,25 +245,22 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
 int launch_slab_select(const float* dist, const float* smin, int64_t nq, int probes, const int32_t* probe_lists, const int32_t* cand_off,
                        const int64_t* list_off, int64_t cap, int64_t cap_s, const int64_t* seg_begin, const int32_t* seg_len, int kp,
                        int32_t* out_pos, float* out_key);
-int launch_list_tc_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
-                          int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
-                          const int32_t* seg_len, const float* qn, const int32_t* pos_kp, const float* approx_kp, int32_t* out_pos,
-                          float* out_key, int* fail_dev, int* n_failed_host, int level = 2);
 // traffic accounting of list_tc_kernel launches (profiling): enable / read-and-reset 8 counters (lists: 0-3, centres: 4-7)
 int list_tc_traffic(int on, int64_t* out8);
 // read-and-reset the level-0 refine's counters, kept while traffic accounting is on: rows re-scored, rows under the
 // global-bound threshold (d~ <= d~_k + 2 eps(q)), queries refined
 int list_tc_level0_rescored(int64_t* out3);
-int launch_list_tc_select_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
-                                 int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
-                                 const float* dist, const int64_t* seg_begin, const int32_t* seg_len, const float* qn, int32_t* out_pos,
-                                 float* out_key, int* fail_dev, int* n_failed_host, int level = 2, const int32_t* pre_pos = nullptr,
-                                 const float* pre_key = nullptr);
-// the same three steps with one CTA per query (selection CTA-wide, re-score on eight warps); smin == nullptr: short runs
+// the exact re-score of the k' nearest of every query's candidate run, their final order and the certificate, with one CTA
+// per query.  The k' are selected in the kernel from the slab minima (smin), taken as selected (pre_pos / pre_key
+// [nq][kp], sorted, -1 padded: launch_slab_select / launch_segment_topk_v), or else selected in the kernel from the whole
+// run dist[q * cap ..) of seg_len[q] <= CR_RUN_MAX entries.  The number of uncertified queries is ADDED to *fail_dev
+// (level 0: and they are listed in fail_list).
+constexpr int CR_RUN_MAX = 4096;
 int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                               int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
-                              const float* dist, const float* smin, int64_t cap, int64_t cap_s, const int32_t* seg_len, const float* qn,
-                              int32_t* out_pos, float* out_key, int* fail_dev, int level = 2, int32_t* fail_list = nullptr);
+                              const float* dist, const float* smin, const int32_t* pre_pos, const float* pre_key, int64_t cap,
+                              int64_t cap_s, const int32_t* seg_len, const float* qn, int32_t* out_pos, float* out_key, int* fail_dev,
+                              int level = 2, int32_t* fail_list = nullptr);
 // vb_ivf_one.cu: the scan of one query (or a handful) as two fused distance + select kernels
 bool one_probe_fits(int lists, size_t qstride, int probes);
 bool one_scan_fits(int64_t cap, size_t qstride, int probes, int64_t k);

@@ -243,29 +243,15 @@ static int ivf_select_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t 
                               (float*)d_cdist, &qn, true));
         int n_failed = 0;
         if (!ix.defer_tc_check) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, sizeof(int), c.stream));
-        // a run of a few thousand centre distances is selected inside the refine kernel (one warp streams it in a few
-        // steps: cheaper than a launch of the CTA-per-query radix selection, 43 us for 2048 x 1000); long runs are not
-        if (c.fused_refine == 3 && ix.lists <= 2048) {
-            // one CTA per query: the run of centre distances is short enough to be selected directly
-            VB_TRY(launch_list_tc_cta_refine(ix.centers, ix.ctc, km, qimg, qstride, nq, probes, kp, 1, zero_lists, pair_off, ix.d_centre_off,
-                                             (const float*)d_cdist, nullptr, ix.lists, 0, sl, qn, lists, ldist, ix.d_tc_fail, 2));
-            if (!ix.defer_tc_check) {
-                VB_CUDA(cudaMemcpyAsync(&n_failed, ix.d_tc_fail, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-                VB_CUDA(cudaStreamSynchronize(c.stream));
-            }
-        } else if (c.fused_refine == 2 || (c.fused_refine != 0 && ix.lists <= 4096)) {
-            VB_TRY(launch_list_tc_select_refine(ix.centers, ix.ctc, km, qimg, qstride, nq, probes, kp, 1, zero_lists, pair_off, ix.d_centre_off,
-                                                (const float*)d_cdist, sb, sl, qn, lists, ldist, ix.d_tc_fail,
-                                                ix.defer_tc_check ? nullptr : &n_failed));
-        } else if (c.fused_refine != 0) {
-            VB_TRY(launch_segment_topk_v((const float*)d_cdist, sb, sl, nullptr, nullptr, nq, kp, pos_kp, key_kp));
-            VB_TRY(launch_list_tc_select_refine(ix.centers, ix.ctc, km, qimg, qstride, nq, probes, kp, 1, zero_lists, pair_off, ix.d_centre_off,
-                                                (const float*)d_cdist, sb, sl, qn, lists, ldist, ix.d_tc_fail,
-                                                ix.defer_tc_check ? nullptr : &n_failed, 2, pos_kp, key_kp));
-        } else {
-            VB_TRY(launch_segment_topk_v((const float*)d_cdist, sb, sl, nullptr, nullptr, nq, kp, pos_kp, key_kp));
-            VB_TRY(launch_list_tc_refine(ix.centers, ix.ctc, km, qimg, qstride, nq, probes, kp, 1, zero_lists, pair_off, ix.d_centre_off, sl,
-                                         qn, pos_kp, key_kp, lists, ldist, ix.d_tc_fail, ix.defer_tc_check ? nullptr : &n_failed));
+        // a run of at most CR_RUN_MAX centre distances is selected inside the refine kernel, a longer one by a launch of its own
+        const bool pre = ix.lists > CR_RUN_MAX;
+        if (pre) VB_TRY(launch_segment_topk_v((const float*)d_cdist, sb, sl, nullptr, nullptr, nq, kp, pos_kp, key_kp));
+        VB_TRY(launch_list_tc_cta_refine(ix.centers, ix.ctc, km, qimg, qstride, nq, probes, kp, 1, zero_lists, pair_off, ix.d_centre_off,
+                                         (const float*)d_cdist, nullptr, pre ? pos_kp : nullptr, pre ? key_kp : nullptr, ix.lists, 0, sl,
+                                         qn, lists, ldist, ix.d_tc_fail, 2));
+        if (!ix.defer_tc_check) {
+            VB_CUDA(cudaMemcpyAsync(&n_failed, ix.d_tc_fail, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+            VB_CUDA(cudaStreamSynchronize(c.stream));
         }
         prof_end(VB_PROF_SCAN_LISTS);
         ix.total_tc_failed += n_failed;
@@ -423,12 +409,12 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
         // slab minima for the selection (vb_common.cuh slab_base): with them the k' nearest are found from 32 k' candidates
         // per query instead of the whole run
         const int64_t cap_s = slab_cap(cap, probes);
-        const bool slabs_fit = c.slab_select && c.fused_refine != 2 && nq * cap_s < (int64_t)INT32_MAX &&
+        const bool slabs_fit = c.slab_select && nq * cap_s < (int64_t)INT32_MAX &&
                                (size_t)cap_s * 4 + 20 * 1024 <= 160 * 1024;
         // level 0 in front of level 1: int8 rows (1 byte per element, bound ~R_max |q|, k' = 128).  Its uncertified queries
         // are listed by the one-CTA-per-query refine and searched again on their own by the batched search
         // (ivf_search_impl), the only caller that allows it.
-        if (level == 1 && c.tc_level0 && ix.allow_level0 && c.fused_refine == 3 && slabs_fit && list_tc_kp(k, 0) <= 128) {
+        if (level == 1 && c.tc_level0 && ix.allow_level0 && slabs_fit && list_tc_kp(k, 0) <= 128) {
             if (ix.l0_cooldown > 0) {
                 --ix.l0_cooldown;
             } else {
@@ -463,37 +449,26 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
             VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), c.stream));
         }
         if (!ix.defer_tc_check) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail + 1, 0, sizeof(int), c.stream));
-        if (c.fused_refine == 3 && slabs && !ix.force_level2) {
+        if (slabs && !ix.force_level2) {
             // one CTA per query: slab selection, re-score on eight warps, ranking, certificate (a selection that overflows
-            // counts as uncertified: the repeat of the batch takes the kernels below)
+            // counts as uncertified: the repeat of the batch selects below)
             VB_TRY(launch_list_tc_cta_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
-                                             (const float*)d_dist, (const float*)d_smin, cap, cap_s, seg_len, qn, pos, key, ix.d_tc_fail + 1,
-                                             level, level == 0 ? ix.d_l0_fail : nullptr));
-            if (!ix.defer_tc_check) {
-                VB_CUDA(cudaMemcpyAsync(&n_failed, ix.d_tc_fail + 1, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-                VB_CUDA(cudaStreamSynchronize(c.stream));
-            }
-        } else if (c.fused_refine == 2) {
-            VB_TRY(launch_list_tc_select_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
-                                                (const float*)d_dist, seg_begin, seg_len, qn, pos, key, ix.d_tc_fail + 1,
-                                                ix.defer_tc_check ? nullptr : &n_failed, level));
-        } else if (c.fused_refine == 1 || c.fused_refine == 3) {
-            if (slabs)
-                VB_TRY(launch_slab_select((const float*)d_dist, (const float*)d_smin, nq, probes, d_lists, cand_off, ix.d_list_off, cap,
-                                          cap_s, seg_begin, seg_len, kp, pos_kp, key_kp));
-            else
-                VB_TRY(launch_segment_topk_v((const float*)d_dist, seg_begin, seg_len, nullptr, nullptr, nq, kp, pos_kp, key_kp));
-            VB_TRY(launch_list_tc_select_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
-                                                (const float*)d_dist, seg_begin, seg_len, qn, pos, key, ix.d_tc_fail + 1,
-                                                ix.defer_tc_check ? nullptr : &n_failed, level, pos_kp, key_kp));
+                                             (const float*)d_dist, (const float*)d_smin, nullptr, nullptr, cap, cap_s, seg_len, qn, pos, key,
+                                             ix.d_tc_fail + 1, level, level == 0 ? ix.d_l0_fail : nullptr));
         } else {
+            // the k' selected by a launch of their own (slab_select_kernel hands what overflows it to the full selection)
             if (slabs)
                 VB_TRY(launch_slab_select((const float*)d_dist, (const float*)d_smin, nq, probes, d_lists, cand_off, ix.d_list_off, cap,
                                           cap_s, seg_begin, seg_len, kp, pos_kp, key_kp));
             else
                 VB_TRY(launch_segment_topk_v((const float*)d_dist, seg_begin, seg_len, nullptr, nullptr, nq, kp, pos_kp, key_kp));
-            VB_TRY(launch_list_tc_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off, seg_len, qn,
-                                         pos_kp, key_kp, pos, key, ix.d_tc_fail + 1, ix.defer_tc_check ? nullptr : &n_failed, level));
+            VB_TRY(launch_list_tc_cta_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
+                                             (const float*)d_dist, nullptr, pos_kp, key_kp, cap, cap_s, seg_len, qn, pos, key,
+                                             ix.d_tc_fail + 1, level));
+        }
+        if (!ix.defer_tc_check) {
+            VB_CUDA(cudaMemcpyAsync(&n_failed, ix.d_tc_fail + 1, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+            VB_CUDA(cudaStreamSynchronize(c.stream));
         }
         prof_end(VB_PROF_TOPK);
         ix.last_tc_failed = n_failed;

@@ -696,344 +696,18 @@ struct LcBound {
 __device__ __forceinline__ float lc_eps(const LcBound& b, float qn) {
     return b.c_dot * sqrtf(qn) * b.xmax + (b.is_l2 ? b.c_sum * (b.xmax * b.xmax + qn) : 0.f);
 }
-// Only candidates with d~ <= (k-th smallest d~) + 2 eps can belong to the k nearest: the k candidates with the
-// smallest d~ all have d <= (k-th d~) + eps, and anything above the threshold has d > (k-th d~) + eps.
-__device__ __forceinline__ float lc_threshold(const LcBound& b, float qn, const float* approx_q, int k, int kp) {
-    return approx_q[min(k, kp) - 1] + 2.f * lc_eps(b, qn);
+// shared memory of cta_refine_body's selection beside its fixed buffers: the slab tables, or a short run's keys
+__host__ __device__ inline size_t cr_work_bytes(bool slabs, bool pre, int64_t cap, int64_t cap_s, int probes) {
+    return slabs ? ss_select_smem_bytes(cap_s, probes) : pre ? 0 : (size_t)cap * 4;
 }
 
-// exact distance of the candidates under the threshold: one warp per (query, candidate), the arithmetic of the
-// scan kernels; the others get +inf (they sort behind every re-scored one)
-template <int ELEM, int METRIC>
-__global__ void rescore_kernel(const uint8_t* __restrict__ rows, size_t stride, int V, const uint8_t* __restrict__ qimg,
-                               size_t qstride, int64_t nq, int k, int kp, int probes, LcBound bound, const float* __restrict__ qn,
-                               const int32_t* __restrict__ pos, const float* __restrict__ approx,
-                               const int32_t* __restrict__ probe_lists, const int32_t* __restrict__ cand_off,
-                               const int64_t* __restrict__ list_off, float* __restrict__ exact) {
-    const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32;
-    const int lane = threadIdx.x % 32;
-    if (w >= nq * kp) return;
-    const int64_t q = w / kp;
-    const int32_t ps = pos[w];
-    if (ps < 0 || approx[w] > lc_threshold(bound, qn[q], approx + q * kp, k, kp)) {   // NaN compares false: re-scored
-        if (lane == 0) exact[w] = __int_as_float(0x7F800000);
-        return;
-    }
-    const int32_t* co = cand_off + q * (probes + 1);
-    int lo = 0, hi = probes;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (co[mid] <= ps) lo = mid;
-        else hi = mid;
-    }
-    while (lo + 1 < probes && co[lo + 1] <= ps) ++lo;   // empty lists share an offset
-    const int l = probe_lists[q * probes + lo];
-    const int64_t row = list_off[l] + (ps - co[lo]);
-    const uint4* rp = reinterpret_cast<const uint4*>(rows + (size_t)row * stride);
-    const uint4* sq = reinterpret_cast<const uint4*>(qimg + (size_t)q * qstride);
-    Acc<ELEM, METRIC> acc;
-#pragma unroll 4
-    for (int v = lane; v < V; v += 32) acc.add(__ldg(rp + v), sq, v);
-    acc.template reduce<32>();
-    if (lane == 0) exact[w] = (float)acc.value();
-}
-
-// one warp per query: order the re-scored candidates by (exact distance, position), emit the first k, and check
-// the certificate: the k'-th approximate distance lies above the threshold, so no candidate outside the k' can
-// be under it either (or every candidate of the query was among the k')
-__global__ void certify_kernel(int64_t nq, int k, int kp, LcBound bound,
-                               const float* __restrict__ qn, const int32_t* __restrict__ seg_len,
-                               const int32_t* __restrict__ pos_kp, const float* __restrict__ approx_kp,
-                               const float* __restrict__ exact_kp, int32_t* __restrict__ out_pos, float* __restrict__ out_key,
-                               int* __restrict__ n_failed, uint8_t* __restrict__ failed) {
-    const int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32;
-    const int lane = threadIdx.x % 32;
-    if (q >= nq) return;
-    __shared__ uint64_t s_key[8][LC_MAX_KP];
-    uint64_t* keys = s_key[(threadIdx.x / 32) % 8];
-    for (int i = lane; i < LC_MAX_KP; i += 32) {
-        uint64_t key = 0xFFFFFFFF00000000ull | (uint32_t)i;   // absent entries sort last, distinct
-        if (i < kp) {
-            const int32_t p = pos_kp[q * kp + i];
-            if (p >= 0) key = ((uint64_t)orderable_key(exact_kp[q * kp + i]) << 32) | (uint32_t)p;
-        }
-        keys[i] = key;
-    }
-    __syncwarp();
-    for (int i = lane; i < kp; i += 32) {
-        const uint64_t mine = keys[i];
-        int rank = 0;
-        for (int j = 0; j < kp; ++j) rank += keys[j] < mine;
-        if (rank < k) {
-            const bool present = pos_kp[q * kp + i] >= 0;
-            out_pos[q * k + rank] = present ? (int32_t)(uint32_t)mine : -1;
-            out_key[q * k + rank] = present ? key_to_float((uint32_t)(mine >> 32)) : __int_as_float(0x7F800000);
-        }
-    }
-    if (lane == 0) {
-        bool ok = true;
-        if (seg_len[q] > kp)   // candidates beyond the k' exist: the last of the k' must already be above the threshold
-            ok = approx_kp[q * kp + kp - 1] > lc_threshold(bound, qn[q], approx_kp + q * kp, k, kp);   // false for NaN
-        failed[q] = ok ? 0 : 1;
-        if (!ok) atomicAdd(n_failed, 1);
-    }
-}
-
-// ---- the three steps after the approximate pass in ONE kernel (one warp per query) -----------------------------------
-//
-// select : the k' smallest approximate distances of the query's candidate run by (distance, position) -- the same
-//          composite key as segment_topk_kernel.  The warp keeps the k' best as a sorted list spread over its lanes
-//          (R = k' / 32 registers per lane, rank i at register i / 32, lane i % 32) and streams the run 32 candidates at
-//          a time; only candidates under the current k'-th key are inserted (~k' ln(n / k') insertions).
-// re-score: the candidates under the certificate threshold are a PREFIX of that sorted list; each is re-scored with
-//          the scan arithmetic (Acc<>, one row per warp pass, the loop of rescore_kernel), two rows in flight.
-// certify: rank by (exact distance, position), emit the first k, and check the certificate -- certify_kernel's rules.
-// Results are bit-identical to segment_topk_kernel + rescore_kernel + certify_kernel (tests compare the two paths).
-template <int R>
-struct WarpTopList {
-    uint64_t key[R];
-    __device__ __forceinline__ void fill(uint64_t v) {
-#pragma unroll
-        for (int r = 0; r < R; ++r) key[r] = v;
-    }
-    // insert x (known to be smaller than the current last key); the displaced last key is dropped
-    __device__ __forceinline__ void insert(uint64_t x, int lane) {
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            const unsigned gt = __ballot_sync(0xffffffffu, key[r] > x);
-            if (gt == 0) continue;                       // warp-uniform
-            const int first = __ffs(gt) - 1;
-            const uint64_t carry = __shfl_sync(0xffffffffu, key[r], 31);
-            const uint64_t up = __shfl_up_sync(0xffffffffu, key[r], 1);
-            if (lane > first) key[r] = up;
-            else if (lane == first) key[r] = x;
-            x = carry;
-        }
-    }
-    __device__ __forceinline__ uint64_t at(int i) const {   // rank i, warp-uniform i
-        uint64_t v = 0;
-#pragma unroll
-        for (int r = 0; r < R; ++r)
-            if (i / 32 == r) v = __shfl_sync(0xffffffffu, key[r], i % 32);
-        return v;
-    }
-};
-
-constexpr int SR_WARPS = 4;
-#ifndef VB_SR_PARALLEL_ADDR
-#define VB_SR_PARALLEL_ADDR 1
-#endif
-
-template <int ELEM, int METRIC, int R>
-__global__ void __launch_bounds__(SR_WARPS * 32) select_refine_kernel(const uint8_t* __restrict__ rows, size_t stride, int V,
-                                                                      const uint8_t* __restrict__ qimg, size_t qstride, int64_t nq, int k,
-                                                                      int kp, int probes, LcBound bound, const float* __restrict__ qn,
-                                                                      const float* __restrict__ dist, const int64_t* __restrict__ seg_begin,
-                                                                      const int32_t* __restrict__ seg_len,
-                                                                      const int32_t* __restrict__ probe_lists,
-                                                                      const int32_t* __restrict__ cand_off,
-                                                                      const int64_t* __restrict__ list_off, int32_t* __restrict__ out_pos,
-                                                                      float* __restrict__ out_key, int* __restrict__ n_failed,
-                                                                      const int32_t* __restrict__ pre_pos,
-                                                                      const float* __restrict__ pre_key) {
-    extern __shared__ uint4 sr_smem[];
-    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-    const int qvec = (int)(qstride / 16);
-    uint4* sq = sr_smem + (size_t)warp * qvec;
-    const int64_t q = blockIdx.x * (int64_t)SR_WARPS + warp;
-    if (q >= nq) return;
-    const uint4* gq = reinterpret_cast<const uint4*>(qimg + (size_t)q * qstride);
-    for (int i = lane; i < qvec; i += 32) sq[i] = gq[i];
-
-    // ---- select
-    const float* dp = dist + seg_begin[q];
-    const int n = seg_len[q];
-    WarpTopList<R> top;
-    top.fill(~0ull);
-    // the sentinel ~0ull sorts after every real key (position < 2^32 - 1), so the first k' candidates simply displace it
-    uint64_t thr = ~0ull;                                   // current k'-th key
-    const int kl = (kp - 1) % 32, kr = (kp - 1) / 32;
-    constexpr int UNR = 4;
-    if (pre_pos != nullptr) {
-        // the k' nearest were selected by segment_topk_kernel (sorted by (distance, position), -1 padded): load them
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            const int i = r * 32 + lane;
-            if (i < kp) {
-                const int32_t p = pre_pos[q * kp + i];
-                if (p >= 0) top.key[r] = ((uint64_t)orderable_key(pre_key[q * kp + i]) << 32) | (uint32_t)p;
-            }
-        }
-        uint64_t t = 0;
-#pragma unroll
-        for (int r = 0; r < R; ++r)
-            if (r == kr) t = __shfl_sync(0xffffffffu, top.key[r], kl);
-        thr = t;
-    }
-    for (int base = 0; pre_pos == nullptr && base < n; base += 32 * UNR) {
-        float v[UNR];
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) {
-            const int i = base + u * 32 + lane;
-            v[u] = i < n ? dp[i] : 0.f;
-        }
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) {
-            const int i = base + u * 32 + lane;
-            const uint64_t key = i < n ? (((uint64_t)orderable_key(v[u]) << 32) | (uint32_t)i) : ~0ull;
-            unsigned m = __ballot_sync(0xffffffffu, key < thr);
-            while (m) {
-                const int j = __ffs(m) - 1;
-                m &= m - 1;
-                const uint64_t x = __shfl_sync(0xffffffffu, key, j);
-                if (x < thr) {                              // warp-uniform
-                    top.insert(x, lane);
-                    uint64_t t = 0;
-#pragma unroll
-                    for (int r = 0; r < R; ++r)
-                        if (r == kr) t = __shfl_sync(0xffffffffu, top.key[r], kl);
-                    thr = t;
-                }
-            }
-        }
-    }
-    __syncwarp();
-
-    // ---- threshold: (k-th smallest approximate distance) + 2 eps; the candidates under it are a prefix of the list
-    const float qnq = qn[q];
-    const int have = min(n, kp);                            // real entries in the list
-    const int kth = min(k, kp) - 1;
-    const uint64_t kth_key = top.at(kth);
-    const float kth_approx = kth_key == ~0ull ? __int_as_float(0x7F800000) : key_to_float((uint32_t)(kth_key >> 32));
-    const float T = kth_approx + 2.f * lc_eps(bound, qnq);
-    // entries of rank i: approx_i <= T  <=>  not (approx_i > T)   (NaN compares false: re-scored, like rescore_kernel)
-    float exact[R];
-#pragma unroll
-    for (int r = 0; r < R; ++r) exact[r] = __int_as_float(0x7F800000);
-    const int32_t* co = cand_off + q * (probes + 1);
-#if VB_SR_PARALLEL_ADDR
-    // Row address of every listed candidate, one candidate per lane (R per lane): position -> probe (binary search of the
-    // query's candidate offsets) -> list -> row.  That is five dependent loads; done inside the re-score loop they were
-    // paid once per PAIR of candidates, ahead of the row reads, by the whole warp.
-    const uint8_t* rowp[R];
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-        const int i = r * 32 + lane;
-        const uint64_t ki = top.key[r];
-        rowp[r] = rows;
-        if (i < have && ki != ~0ull) {
-            const int32_t ps = (int32_t)(uint32_t)ki;
-            int lo = 0, hi = probes;
-            while (hi - lo > 1) {
-                const int mid = (lo + hi) >> 1;
-                if (co[mid] <= ps) lo = mid;
-                else hi = mid;
-            }
-            while (lo + 1 < probes && co[lo + 1] <= ps) ++lo;   // empty lists share an offset
-            const int l = probe_lists[q * probes + lo];
-            rowp[r] = rows + (size_t)(list_off[l] + (ps - co[lo])) * stride;
-        }
-    }
-#endif
-    for (int i0 = 0; i0 < have; i0 += 2) {
-        const uint64_t k0 = top.at(i0);
-        const uint64_t k1 = i0 + 1 < have ? top.at(i0 + 1) : ~0ull;
-        const float a0 = key_to_float((uint32_t)(k0 >> 32));
-        const float a1 = k1 == ~0ull ? 0.f : key_to_float((uint32_t)(k1 >> 32));
-        const bool do0 = !(a0 > T), do1 = k1 != ~0ull && !(a1 > T);
-        if (!do0 && !do1) continue;                         // (no early exit: NaN distances sort last and are re-scored too)
-        const uint4* rp[2];
-#if VB_SR_PARALLEL_ADDR
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-            const int it = min(i0 + t, R * 32 - 1);         // (warp-uniform; the clamp only guards the shuffle of an absent k1)
-            unsigned long long a = 0;
-#pragma unroll
-            for (int r = 0; r < R; ++r)
-                if (it / 32 == r) a = __shfl_sync(0xffffffffu, (unsigned long long)rowp[r], it % 32);
-            rp[t] = reinterpret_cast<const uint4*>((t == 0 ? do0 : do1) ? (const uint8_t*)a : rows);
-        }
-#else
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-            const int32_t ps = (int32_t)(uint32_t)(t == 0 ? k0 : k1);
-            int lo = 0, hi = probes;
-            if ((t == 0 ? do0 : do1)) {
-                while (hi - lo > 1) {
-                    const int mid = (lo + hi) >> 1;
-                    if (co[mid] <= ps) lo = mid;
-                    else hi = mid;
-                }
-                while (lo + 1 < probes && co[lo + 1] <= ps) ++lo;   // empty lists share an offset
-                const int l = probe_lists[q * probes + lo];
-                rp[t] = reinterpret_cast<const uint4*>(rows + (size_t)(list_off[l] + (ps - co[lo])) * stride);
-            } else {
-                rp[t] = reinterpret_cast<const uint4*>(rows);
-            }
-        }
-#endif
-        Acc<ELEM, METRIC> acc0, acc1;
-        if (do0 && do1) {
-#pragma unroll 4
-            for (int v = lane; v < V; v += 32) {
-                const uint4 x0 = __ldg(rp[0] + v), x1 = __ldg(rp[1] + v);
-                acc0.add(x0, sq, v);
-                acc1.add(x1, sq, v);
-            }
-        } else if (do0) {
-#pragma unroll 4
-            for (int v = lane; v < V; v += 32) acc0.add(__ldg(rp[0] + v), sq, v);
-        } else {
-#pragma unroll 4
-            for (int v = lane; v < V; v += 32) acc1.add(__ldg(rp[1] + v), sq, v);
-        }
-        acc0.template reduce<32>();
-        acc1.template reduce<32>();
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            if (do0 && i0 / 32 == r && lane == i0 % 32) exact[r] = (float)acc0.value();
-            if (do1 && (i0 + 1) / 32 == r && lane == (i0 + 1) % 32) exact[r] = (float)acc1.value();
-        }
-    }
-
-    // ---- order by (exact distance, position), emit the first k
-    uint64_t fin[R];
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-        const int i = r * 32 + lane;
-        const bool present = i < kp && top.key[r] != ~0ull;    // (ranks >= k' hold displaced leftovers, not candidates)
-        fin[r] = present ? (((uint64_t)orderable_key(exact[r]) << 32) | (uint32_t)top.key[r]) : (0xFFFFFFFF00000000ull | (uint32_t)i);
-    }
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-        int rank = 0;
-#pragma unroll
-        for (int r2 = 0; r2 < R; ++r2)
-            for (int j = 0; j < 32; ++j) {
-                const uint64_t o = __shfl_sync(0xffffffffu, fin[r2], j);
-                rank += (r2 * 32 + j < kp) && o < fin[r];
-            }
-        const int i = r * 32 + lane;
-        if (i < kp && rank < k) {
-            const bool present = top.key[r] != ~0ull;
-            out_pos[q * k + rank] = present ? (int32_t)(uint32_t)fin[r] : -1;
-            out_key[q * k + rank] = present ? key_to_float((uint32_t)(fin[r] >> 32)) : __int_as_float(0x7F800000);
-        }
-    }
-    // ---- certificate: candidates beyond the k' exist -> the last of the k' must already be above the threshold
-    if (lane == 0) {
-        bool ok = true;
-        if (n > kp) ok = key_to_float((uint32_t)(thr >> 32)) > T;     // thr = the k'-th key; false for NaN
-        if (!ok) atomicAdd(n_failed, 1);
-    }
-}
-
-// Steps 2 + 3 + 4 with ONE CTA per query (cta_refine_kernel): the selection is CTA-wide (slab minima, or the whole run
-// when it is short: the distances of a query to every centre), the candidates under the certificate threshold are then
-// re-scored by the CTA's eight warps in parallel (one row per warp at a time; select_refine_kernel walks them two at a
-// time on a single warp), ranked and certified.  Same arithmetic, same tie rule, same outputs as select_refine_kernel;
-// a query whose selection overflows its buffer (ties by the thousand) counts as uncertified and the batch is repeated
-// on the kernels above.
+// Steps 2 + 3 + 4 with ONE CTA per query (cta_refine_kernel): the k' nearest by (d~, position) come from one of three
+// sources -- a CTA-wide selection from the slab minima (smin), the k' preselected by launch_slab_select /
+// launch_segment_topk_v (pre_pos / pre_key [nq][kp], sorted, -1 padded), or an exact selection of the whole run when it
+// is short (at most CR_RUN_MAX entries: the distances of a query to every centre).  The candidates under the certificate
+// threshold are then re-scored by the CTA's eight warps in parallel (one row per warp at a time), ranked and certified.
+// A query whose slab selection overflows its buffer (ties by the thousand) counts as uncertified and the batch is
+// repeated with the k' preselected.
 //
 // LIST (level 0 only): the uncertified queries are also listed, and the re-score uses per-row bounds E_i (lc_make_bound)
 // instead of (k-th d~) + 2 eps.  Phase 1 re-scores the k candidates of smallest d~ and sets T to their k-th exact
@@ -1044,13 +718,16 @@ template <int ELEM, int METRIC, bool LIST>
 __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows, size_t stride, int V,
                                                                 const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
                                                                 LcBound bound, const float* __restrict__ qn, const float* __restrict__ dist,
-                                                                const float* __restrict__ smin, int64_t cap, int64_t cap_s,
+                                                                const float* __restrict__ smin, const int32_t* __restrict__ pre_pos,
+                                                                const float* __restrict__ pre_key, int64_t cap, int64_t cap_s,
                                                                 const int32_t* __restrict__ seg_len, const int32_t* __restrict__ probe_lists,
                                                                 const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
                                                                 int32_t* __restrict__ out_pos, float* __restrict__ out_key,
                                                                 int* __restrict__ n_failed, int32_t* __restrict__ fail_list,
                                                                 const float* __restrict__ xn, const float* __restrict__ r8,
                                                                 const float4* __restrict__ coef, unsigned long long* __restrict__ counters) {
+    const bool slabs = LIST || smin != nullptr;                                 // (level 0 always has slab minima)
+    const bool pre = !LIST && pre_pos != nullptr;
     extern __shared__ uint64_t cr_smem[];
     uint64_t* cand = cr_smem;                                                   // [SS_CAND]
     uint64_t* fin = cand + SS_CAND;                                             // [kp] final keys
@@ -1058,15 +735,27 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
     uint4* sq = reinterpret_cast<uint4*>(rowp + kp);                            // [qvec] query image (cand, fin and rowp are 16 kp + 16384 bytes: aligned)
     const int qvec = (int)(qstride / 16);
     void* work = sq + qvec;                                                     // the selection's work area (16-byte aligned)
-    float* exact = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(work) + (smin ? ss_select_smem_bytes(cap_s, probes) : (size_t)cap * 4));   // [kp]
+    float* exact = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(work) + cr_work_bytes(slabs, pre, cap, cap_s, probes));   // [kp]
     const int q = blockIdx.x;
     const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32;
     const uint4* gq = reinterpret_cast<const uint4*>(qimg + (size_t)q * qstride);
     for (int i = tid; i < qvec; i += SS_THREADS) sq[i] = gq[i];
     const int n_run = seg_len[q];
     int n;
-    if (smin) n = slab_select_cta(dist, smin, probes, probe_lists, cand_off, list_off, cap, cap_s, q, kp, cand, work);
-    else n = direct_select_cta(dist + (int64_t)q * cap, n_run, kp, cand, work);
+    if (pre) {
+        // kp <= SS_THREADS: one entry per thread; the -1 padding follows the valid entries
+        const int32_t p = tid < kp ? pre_pos[(int64_t)q * kp + tid] : -1;
+        if (p >= 0) cand[tid] = ((uint64_t)orderable_key(pre_key[(int64_t)q * kp + tid]) << 32) | (uint32_t)p;
+        n = __syncthreads_count(p >= 0);
+    } else if (slabs) {
+        n = slab_select_cta(dist, smin, probes, probe_lists, cand_off, list_off, cap, cap_s, q, kp, cand, work);
+    } else {
+        uint32_t* keys = reinterpret_cast<uint32_t*>(work);
+        const float* dq = dist + (int64_t)q * cap;
+        for (int i = tid; i < n_run; i += SS_THREADS) keys[i] = orderable_key(dq[i]);
+        __syncthreads();
+        n = select_exact_cta(keys, n_run, kp, cand);
+    }
     if (n < 0) {
         // not selected here: the query reports as uncertified (outputs are rewritten by the repeat of the batch)
         if (tid == 0) {
@@ -1080,7 +769,8 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
         return;
     }
     const int have = min(n, kp);
-    // ---- threshold: (k-th smallest approximate distance) + 2 eps
+    // ---- threshold: (k-th smallest approximate distance) + 2 eps.  Only candidates with d~ under it can belong to the k
+    // nearest: the k candidates with the smallest d~ all have d <= (k-th d~) + eps, anything above it has d > (k-th d~) + eps.
     const int kth = min(k, kp) - 1;
     const uint64_t kth_key = kth < have ? cand[kth] : ~0ull;
     const float kth_approx = kth_key == ~0ull ? __int_as_float(0x7F800000) : key_to_float((uint32_t)(kth_key >> 32));
@@ -1098,7 +788,7 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
         if (i < have) {
             const int32_t ps = (int32_t)(uint32_t)cand[i];
             int64_t g;                                        // row of the (list-ordered) table
-            if (smin) {
+            if (slabs) {
                 int lo = 0, hi = probes;
                 while (hi - lo > 1) {
                     const int mid = (lo + hi) >> 1;
@@ -1204,12 +894,13 @@ template <int ELEM, int METRIC>
 __global__ void __launch_bounds__(SS_THREADS) cta_refine_kernel(const uint8_t* __restrict__ rows, size_t stride, int V,
                                                                 const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
                                                                 LcBound bound, const float* __restrict__ qn, const float* __restrict__ dist,
-                                                                const float* __restrict__ smin, int64_t cap, int64_t cap_s,
+                                                                const float* __restrict__ smin, const int32_t* __restrict__ pre_pos,
+                                                                const float* __restrict__ pre_key, int64_t cap, int64_t cap_s,
                                                                 const int32_t* __restrict__ seg_len, const int32_t* __restrict__ probe_lists,
                                                                 const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
                                                                 int32_t* __restrict__ out_pos, float* __restrict__ out_key,
                                                                 int* __restrict__ n_failed) {
-    cta_refine_body<ELEM, METRIC, false>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, nullptr,
+    cta_refine_body<ELEM, METRIC, false>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, pre_pos, pre_key, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, nullptr,
                                          nullptr, nullptr, nullptr, nullptr);
 }
 // level 0: the per-row re-score rule (xn, r8: the image's |x|^2 and residuals; coef: l0_query_kernel's coefficients;
@@ -1225,7 +916,7 @@ __global__ void __launch_bounds__(SS_THREADS) cta_refine_list_kernel(const uint8
                                                                 int* __restrict__ n_failed, int32_t* __restrict__ fail_list,
                                                                 const float* __restrict__ xn, const float* __restrict__ r8,
                                                                 const float4* __restrict__ coef, unsigned long long* __restrict__ counters) {
-    cta_refine_body<ELEM, METRIC, true>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, fail_list,
+    cta_refine_body<ELEM, METRIC, true>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, nullptr, nullptr, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, fail_list,
                                         xn, r8, coef, counters);
 }
 
@@ -1256,7 +947,7 @@ __global__ void lc_traffic_kernel(LcArgs a, uint32_t a_bytes, unsigned long long
 
 // ----------------------------------------------------------------------------- host side
 
-enum { WSC_B = 21, WSC_N = 22, WSC_K = 23 };
+enum { WSC_B = 21, WSC_N = 22 };
 
 // c_sum of lc_make_bound: the fp32 norms, the final sum and the exact distance, relative to |x|^2 + |q|^2
 static float lc_c_sum(int dim) { return std::max(1.0f / 65536.0f, 3.0f * ((float)dim / 32.0f + 8.0f) / 16777216.0f); }
@@ -1660,103 +1351,21 @@ static LcBound lc_make_bound(const Table& rows, const ListTcImage& im, int key_m
     return bound;
 }
 
-// steps 3 + 4: exact re-score of the selected candidates, final order, certificate.  The number of queries whose
-// certificate failed is ADDED to *fail_dev (a device counter the caller zeroes); with n_failed_host the counter is
-// also read back (one stream synchronisation), otherwise the caller checks it when it synchronises anyway.
-int launch_list_tc_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
-                          int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
-                          const int32_t* seg_len, const float* qn, const int32_t* pos_kp, const float* approx_kp, int32_t* out_pos,
-                          float* out_key, int* fail_dev, int* n_failed_host, int level) {
-    Context& c = ctx();
-    cudaStream_t s = c.stream;
-    void* d_ws;
-    VB_TRY(workspace(WSC_K, sizeof(float) * (size_t)nq * kp + (size_t)nq + 64, &d_ws));
-    int* n_failed = fail_dev;
-    float* exact = (float*)d_ws + 16;
-    uint8_t* failed = (uint8_t*)(exact + (size_t)nq * kp);
-    const int V = (int)(rows.stride / 16);
-    const unsigned grid = (unsigned)((nq * kp * 32 + 255) / 256);
-    const LcBound bound = lc_make_bound(rows, im, key_metric, level);
-#define VB_RS(E, M) rescore_kernel<E, M><<<grid, 256, 0, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, nq, k, kp, probes, bound, qn, pos_kp, approx_kp, d_lists, cand_off, d_list_off, exact)
-    if (rows.elem == VB_VECTOR) {
-        if (key_metric == VB_L2_SQUARED) VB_RS(VB_VECTOR, VB_L2_SQUARED);
-        else VB_RS(VB_VECTOR, VB_NEG_IP);
-    } else {
-        if (key_metric == VB_L2_SQUARED) VB_RS(VB_HALFVEC, VB_L2_SQUARED);
-        else VB_RS(VB_HALFVEC, VB_NEG_IP);
-    }
-#undef VB_RS
-    certify_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, s>>>(nq, k, kp, bound, qn, seg_len, pos_kp, approx_kp, exact, out_pos, out_key,
-                                                                    n_failed, failed);
-    VB_CUDA(cudaGetLastError());
-    count_launch(2);
-    if (n_failed_host) {
-        VB_CUDA(cudaMemcpyAsync(n_failed_host, n_failed, sizeof(int), cudaMemcpyDeviceToHost, s));
-        VB_CUDA(cudaStreamSynchronize(s));
-    }
-    return VB_OK;
-}
-
-// steps 2 + 3 + 4 in one kernel (select_refine_kernel): k' select, exact re-score, final order, certificate
-int launch_list_tc_select_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
-                                 int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
-                                 const float* dist, const int64_t* seg_begin, const int32_t* seg_len, const float* qn, int32_t* out_pos,
-                                 float* out_key, int* fail_dev, int* n_failed_host, int level, const int32_t* pre_pos,
-                                 const float* pre_key) {
-    Context& c = ctx();
-    cudaStream_t s = c.stream;
-    const LcBound bound = lc_make_bound(rows, im, key_metric, level);
-    const int V = (int)(rows.stride / 16);
-    const size_t smem = qstride * SR_WARPS;
-    const unsigned grid = (unsigned)((nq + SR_WARPS - 1) / SR_WARPS);
-    const int R = (kp + 31) / 32;
-#define VB_SR2(E, M, RR)                                                                                                              \
-    do {                                                                                                                              \
-        auto kern = select_refine_kernel<E, M, RR>;                                                                                   \
-        if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));            \
-        kern<<<grid, SR_WARPS * 32, smem, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, nq, k, kp, probes, bound, qn, dist, \
-                                              seg_begin, seg_len, d_lists, cand_off, d_list_off, out_pos, out_key, fail_dev, pre_pos, \
-                                              pre_key);                                                                              \
-    } while (0)
-#define VB_SR(E, M)                   \
-    do {                              \
-        if (R <= 1) VB_SR2(E, M, 1);  \
-        else if (R == 2) VB_SR2(E, M, 2); \
-        else VB_SR2(E, M, 4);         \
-    } while (0)
-    VB_REQUIRE(kp <= 128 && smem <= 200 * 1024, "select_refine: k' = %d / query image of %zu bytes not supported", kp, qstride);
-    if (rows.elem == VB_VECTOR) {
-        if (key_metric == VB_L2_SQUARED) VB_SR(VB_VECTOR, VB_L2_SQUARED);
-        else VB_SR(VB_VECTOR, VB_NEG_IP);
-    } else {
-        if (key_metric == VB_L2_SQUARED) VB_SR(VB_HALFVEC, VB_L2_SQUARED);
-        else VB_SR(VB_HALFVEC, VB_NEG_IP);
-    }
-#undef VB_SR
-#undef VB_SR2
-    VB_CUDA(cudaGetLastError());
-    count_launch();
-    if (n_failed_host) {
-        VB_CUDA(cudaMemcpyAsync(n_failed_host, fail_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
-        VB_CUDA(cudaStreamSynchronize(s));
-    }
-    return VB_OK;
-}
-
-// steps 2 + 3 + 4 with one CTA per query; smin == nullptr: the run is short (<= SS_CAND) and selected directly
+// steps 2 + 3 + 4 with one CTA per query
 int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                               int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
-                              const float* dist, const float* smin, int64_t cap, int64_t cap_s, const int32_t* seg_len, const float* qn,
-                              int32_t* out_pos, float* out_key, int* fail_dev, int level, int32_t* fail_list) {
+                              const float* dist, const float* smin, const int32_t* pre_pos, const float* pre_key, int64_t cap,
+                              int64_t cap_s, const int32_t* seg_len, const float* qn, int32_t* out_pos, float* out_key, int* fail_dev,
+                              int level, int32_t* fail_list) {
     if (nq == 0) return VB_OK;
     Context& c = ctx();
     cudaStream_t s = c.stream;
     const LcBound bound = lc_make_bound(rows, im, key_metric, level);
     const int V = (int)(rows.stride / 16);
-    const size_t smem = (size_t)SS_CAND * 8 + (size_t)kp * 16 + qstride + (smin ? ss_select_smem_bytes(cap_s, probes) : (size_t)cap * 4) +
-                        (size_t)kp * 4 + 16;
-    VB_REQUIRE(kp <= 256 && smem <= 200 * 1024 && (smin || cap <= SS_CAND), "cta_refine: k' = %d / %zu bytes of shared memory not supported", kp, smem);
-    VB_REQUIRE(!fail_list || (level == 0 && im.r8), "cta_refine: the listing kernel is level 0's and needs its int8 image");
+    const size_t smem = (size_t)SS_CAND * 8 + (size_t)kp * 16 + qstride + cr_work_bytes(smin, pre_pos, cap, cap_s, probes) + (size_t)kp * 4 + 16;
+    VB_REQUIRE(kp <= SS_THREADS && smem <= 200 * 1024 && (smin || pre_pos || cap <= CR_RUN_MAX),
+               "cta_refine: k' = %d / %zu bytes of shared memory not supported", kp, smem);
+    VB_REQUIRE(!fail_list || (level == 0 && im.r8 && smin), "cta_refine: the listing kernel is level 0's and needs its int8 image and slab minima");
 #define VB_CR(E, M)                                                                                                              \
     do {                                                                                                                         \
         if (fail_list) {                                                                                                         \
@@ -1771,7 +1380,8 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
         auto kern = cta_refine_kernel<E, M>;                                                                                     \
         if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));       \
         kern<<<(unsigned)nq, SS_THREADS, smem, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, k, kp, probes, bound, qn, dist, smin, \
-                                                   cap, cap_s, seg_len, d_lists, cand_off, d_list_off, out_pos, out_key, fail_dev);   \
+                                                   pre_pos, pre_key, cap, cap_s, seg_len, d_lists, cand_off, d_list_off, out_pos, out_key,   \
+                                                   fail_dev);                                                                               \
     } while (0)
     if (rows.elem == VB_VECTOR) {
         if (key_metric == VB_L2_SQUARED) VB_CR(VB_VECTOR, VB_L2_SQUARED);

@@ -1,5 +1,5 @@
 // vb_slab_select.cuh -- CTA-wide selection of the k' nearest of one query's candidate run, shared by
-// slab_select_kernel (vb_scan.cu) and cta_refine_kernel (vb_list_tc.cu).
+// slab_select_kernel (vb_scan.cu), cta_refine_kernel (vb_list_tc.cu) and the one-query kernels (vb_ivf_one.cu).
 //
 // The tensor-core filter's epilogue stores, beside the dense d~ array, min d~ of every slab (32 table-aligned rows of one
 // probed list, slab_base() in vb_common.cuh).  tau = the k'-th smallest slab minimum is an upper bound of the k'-th
@@ -210,32 +210,6 @@ __device__ __forceinline__ int slab_select_cta(const float* __restrict__ dist, c
     if (n > (uint32_t)SS_CAND) return -1;
     ss_sort_cand(cand, n);
     return (int)n;
-}
-
-// a short run (n <= SS_CAND candidates, e.g. the distances of one query to every centre): the k-th smallest key is
-// radix-selected, the keys up to it gathered and sorted (a full sort of the run costs 50 k warp instructions per query).
-// `work`: n words of shared memory.  Returns the number gathered (>= min(k, n)), or -1 past SS_CAND (cannot happen: n <= SS_CAND).
-__device__ __forceinline__ int direct_select_cta(const float* __restrict__ dq, int n, int k, uint64_t* cand, void* work) {
-    __shared__ uint32_t s_cnt;
-    uint32_t* keys = reinterpret_cast<uint32_t*>(work);
-    const int tid = threadIdx.x;
-    for (int i = tid; i < n; i += SS_THREADS) keys[i] = orderable_key(dq[i]);
-    if (tid == 0) s_cnt = 0;
-    __syncthreads();
-    uint32_t tau = 0xFFFFFFFFu;
-    if (n > k) tau = ss_radix_kth(keys, n, k);
-    for (int i = tid; i < n; i += SS_THREADS) {
-        const uint32_t key = keys[i];
-        if (key <= tau) {
-            const uint32_t slot = atomicAdd(&s_cnt, 1u);
-            if (slot < (uint32_t)SS_CAND) cand[slot] = ((uint64_t)key << 32) | (uint32_t)i;
-        }
-    }
-    __syncthreads();
-    const uint32_t m = s_cnt;
-    if (m > (uint32_t)SS_CAND) return -1;
-    ss_sort_cand(cand, m);
-    return (int)m;
 }
 
 // EXACTLY the min(k, n) smallest of keys[0 .. n) (shared memory, orderable keys) by (key, index), sorted, as composites

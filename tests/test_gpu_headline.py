@@ -3,7 +3,7 @@ lists = 100, probes = 10, k = 10 through the tensor-core filter (scan_impl 4) at
 synthetic laws bench.py reports (intrinsic dimension 16, and SURVEY 8(d)'s isotropic Gaussian mixture), against the
 oracle port of src/ivfscan.c:47-187 -- plus near-tie sets at dim 1536 and at IVFFLAT_MAX_DIM = 2000
 (src/ivfflat.h:37) whose neighbour gaps sit around the certificate's error bound, where a wrong dimension term in
-the bound (vb_list_tc.cu launch_list_tc_refine) would certify wrong neighbours."""
+the bound (vb_list_tc.cu lc_make_bound) would certify wrong neighbours."""
 import os
 
 import numpy as np
@@ -168,42 +168,47 @@ def test_near_ties_at_long_rows(pv, dim, gap):
 
 
 @pytest.mark.parametrize("k,probes", [(10, 10), (1, 3), (40, 10), (24, 7)])
-def test_fused_select_refine_equals_the_three_kernel_path(pv, headline, k, probes):
-    """cta_refine_kernel (option fused_refine = 3, the default: selection, exact re-score, ranking and certificate with one
-    CTA per query) and select_refine_kernel (= 1: one warp per query after the selection kernel; = 2: it also selects)
-    return bit for bit what segment_topk_kernel + rescore_kernel + certify_kernel (= 0) return, at both filter levels,
-    incl. the counters"""
+def test_refine_of_preselected_candidates_equals_the_slab_selecting_refine(pv, headline, k, probes):
+    """The one-CTA-per-query refine selects the k' nearest from the slab minima itself (slab_select 1) or takes them from
+    the full selection kernel (slab_select 0): both routes return bit for bit the same neighbours, distances, probe lists
+    and counters at both filter levels, and where no batch fell back to the exact kernels, what the per-query LDG scan
+    (scan_impl 0) returns.  Each route runs on a fresh copy of the index, so both start from the same filter-level state
+    (a level-1 failure rests level 1 for the next batches of that index), and level 0 -- which needs slab minima -- is off."""
     law, gix, oix, queries, _ = headline
     out = {}
     try:
+        pv.set_option("scan_impl", 0)
+        want = gix.search(queries, k=k, probes=probes)
         pv.set_option("scan_impl", 4)
+        pv.set_option("tc_level0", 0)
         for level1 in (1, 0):
             pv.set_option("tc_level1", level1)
-            for fused in (0, 1, 2, 3):
-                pv.set_option("fused_refine", fused)
-                f0, l0 = gix.tc_fallbacks(), gix.tc_level1_fallbacks()
-                ids, dist = gix.search(queries, k=k, probes=probes)
-                lists, ldist = gix.scan_lists(queries[:300], probes)
-                out[level1, fused] = (ids, dist, lists, ldist, gix.tc_fallbacks() - f0, gix.tc_level1_fallbacks() - l0)
+            for slab in (1, 0):
+                pv.set_option("slab_select", slab)
+                ix = pv.IvfflatIndex("vector_l2_ops", DIM, LISTS).load(oix.centers, oix.offsets, oix.rows, oix.ids)
+                ids, dist = ix.search(queries, k=k, probes=probes)
+                lists, ldist = ix.scan_lists(queries[:300], probes)
+                out[level1, slab] = (ids, dist, lists, ldist, ix.tc_fallbacks(), ix.tc_level1_fallbacks())
+                ix.free()
     finally:
-        pv.set_option("fused_refine", 3)
+        pv.set_option("slab_select", 1)
+        pv.set_option("tc_level0", 1)
         pv.set_option("tc_level1", 1)
         pv.set_option("scan_impl", int(os.environ.get("VB_TEST_SCAN_IMPL", "2")))
     for level1 in (1, 0):
-        a = out[level1, 0]
-        for fused in (1, 2, 3):
-            b = out[level1, fused]
-            for x, y in zip(a[:4], b[:4]):
-                assert np.array_equal(x, y), (level1, fused, k, probes)
-            assert a[4:] == b[4:]
+        a, b = out[level1, 1], out[level1, 0]
+        for x, y in zip(a[:4], b[:4]):
+            assert np.array_equal(x, y), (level1, k, probes)
+        assert a[4:] == b[4:]
+        if a[4] == 0:
+            assert np.array_equal(a[0], want[0]) and np.array_equal(a[1], want[1]), (level1, k, probes)
 
 
 @pytest.mark.parametrize("k,probes", [(10, 10), (1, 3), (40, 20)])
-def test_selection_from_slab_minima_equals_the_full_selection(pv, headline, k, probes):
+def test_slab_selection_equals_the_full_selection(pv, headline, k, probes):
     """The filter's epilogue stores the minimum d~ of every 32-row slab; the k' nearest are then selected from the slabs
     whose minimum is under the k'-th smallest slab minimum (vb_scan.cu slab_select_kernel) instead of a radix selection
-    over the whole candidate run.  Same candidates, same order: outputs are bit-identical, at both filter levels and
-    with either refine path."""
+    over the whole candidate run.  Same candidates, same order: outputs are bit-identical, at both filter levels."""
     law, ix, oix, queries, _ = headline
     qs = queries[:300]
     out = {}
@@ -211,22 +216,18 @@ def test_selection_from_slab_minima_equals_the_full_selection(pv, headline, k, p
         pv.set_option("scan_impl", 4)
         for level1 in (1, 0):
             pv.set_option("tc_level1", level1)
-            for fused in (3, 1, 0):
-                pv.set_option("fused_refine", fused)
-                for slab in (0, 1):
-                    pv.set_option("slab_select", slab)
-                    f0 = ix.tc_fallbacks()
-                    out[(level1, fused, slab)] = ix.search(qs, k=k, probes=probes) + (ix.tc_fallbacks() - f0,)
+            for slab in (0, 1):
+                pv.set_option("slab_select", slab)
+                f0 = ix.tc_fallbacks()
+                out[(level1, slab)] = ix.search(qs, k=k, probes=probes) + (ix.tc_fallbacks() - f0,)
     finally:
         pv.set_option("slab_select", 1)
-        pv.set_option("fused_refine", 3)
         pv.set_option("tc_level1", 1)
         pv.set_option("scan_impl", int(os.environ.get("VB_TEST_SCAN_IMPL", "2")))
     for level1 in (1, 0):
-        for fused in (3, 1, 0):
-            i0, d0, f0 = out[(level1, fused, 0)]
-            i1, d1, f1 = out[(level1, fused, 1)]
-            assert np.array_equal(i0, i1) and np.array_equal(d0, d1) and f0 == f1
+        i0, d0, f0 = out[(level1, 0)]
+        i1, d1, f1 = out[(level1, 1)]
+        assert np.array_equal(i0, i1) and np.array_equal(d0, d1) and f0 == f1
 
 
 def test_selection_from_slab_minima_with_ties_by_the_thousand(pv):
