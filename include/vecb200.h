@@ -636,7 +636,7 @@ int			vb_hnsw_build_dev(vb_hnsw *h, const void *rows_dev, int64_t n, int ef_cons
  * of the new elements and every slot UpdateNeighborOnDisk rewrote in an existing element; slot indexes the layer's lm
  * entries (2m at layer 0, m above).  A slot rewritten twice in one call appears once, with its final value: applied
  * to a vb_hnsw_export taken before the call they give exactly the export taken after it.  cap below the count fails
- * with VB_EINVAL, writing nothing.  The records stay valid until the next insert, load or build.
+ * with VB_EINVAL, writing nothing.  The records stay valid until the next insert, vacuum, load or build.
  *
  * Growth and failure: the device arrays grow geometrically (the graph is not double-buffered).  Before any kernel
  * runs, the call validates its arguments and reserves capacity, upper slots, record space and visited tables; after
@@ -657,8 +657,36 @@ int			vb_hnsw_insert(vb_hnsw *h, const void *rows, int64_t n, int ef_constructio
 						   const int32_t *levels, int32_t *out_dup_of, int64_t *out_nchanges);
 int			vb_hnsw_insert_dev(vb_hnsw *h, const void *rows_dev, int64_t n, int ef_construction, uint64_t seed,
 							   const int32_t *levels, int32_t *out_dup_of, int64_t *out_nchanges);
-int			vb_hnsw_insert_changes(vb_hnsw *h, vb_hnsw_slot *out, int64_t cap);	/* the last insert's records */
+int			vb_hnsw_insert_changes(vb_hnsw *h, vb_hnsw_slot *out, int64_t cap);	/* the last insert's or vacuum's records */
 int			vb_hnsw_set_heaptid_counts(vb_hnsw *h, const int32_t *counts);
+
+/*
+ * VACUUM of a resident image: the graph part of hnswbulkdelete (src/hnswvacuum.c:776-797).  counts (host [vb_hnsw_rows])
+ * are the heap TIDs each element keeps after RemoveHeapTids (:35-173), which the glue runs on the pages: 0..10, 0 = the
+ * element is deleted now or was deleted by an earlier vacuum; rows vb_hnsw_insert folded into another element must be
+ * 0.  They replace the image's counts, as vb_hnsw_set_heaptid_counts does.  Then:
+ *   1. RepairGraphEntryPoint (:279-373): the highest live point (the first live element of a strictly higher level, in
+ *      element order, which is page order) -- or the fallback point when that is the entry point -- is repaired when
+ *      NeedsUpdated; an entry point being deleted is replaced by the highest point (-1 when nothing is live); a live one
+ *      is repaired when NeedsUpdated, searching from the highest point.
+ *   2. RepairGraph (:378-502): every live element other than the entry point for which NeedsUpdated (:178-220) holds
+ *      -- a slot on any layer names an element of count 0, or the last layer-0 slot is empty -- is repaired, in element
+ *      order, in batches of at most max(1, live / hnsw_build_fraction) elements (capped by hnsw_build_batch), with
+ *      NeedsUpdated evaluated at each batch's start.  A repair is RepairGraphElement: HnswFindElementNeighbors with
+ *      existing = true (elements of count 0 do not count towards ef, ef_construction + 1, the element itself and
+ *      elements of count 0 removed before SelectNeighbors) against the graph as of the batch start; its whole neighbour
+ *      tuple is replaced, then HnswUpdateNeighborsOnDisk with ConnectionExists (src/hnswinsert.c:453-468) updates its
+ *      neighbours.  With batches of one element the result is the serial reference's.
+ *   3. MarkDeleted (:594-729): every neighbour slot of every element of count 0 is cleared.  Such elements stay in the
+ *      image as unreachable tombstones; their numbers are not reused, so the image grows until it is reloaded.
+ * *out_nrepaired (may be NULL) = the repairs made; change records as for vb_hnsw_insert: every slot whose value
+ * differs from before the call (a cleared slot has neighbor -1), through vb_hnsw_insert_changes.
+ * Arguments are validated and memory reserved before any kernel runs (VB_EINVAL / VB_ENOMEM leave the image as it
+ * was).  A vacuum bumps the generation like an insert; unfiltered vb_hnsw_scan handles keep working (a tombstone they
+ * return from their discarded set has count 0, so the glue hands out no heap TIDs for it).
+ */
+int			vb_hnsw_vacuum(vb_hnsw *h, const int32_t *counts, int ef_construction, int64_t *out_nrepaired,
+						   int64_t *out_nchanges);
 int64_t		vb_hnsw_rows(const vb_hnsw *h);
 int64_t		vb_hnsw_upper_slots(const vb_hnsw *h);
 int			vb_hnsw_export(vb_hnsw *h, int32_t *levels, int32_t *nbr0, int64_t *upper_off, int32_t *upper,

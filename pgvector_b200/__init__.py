@@ -819,8 +819,22 @@ class HnswIndex:
         self.n = int(load().vb_hnsw_rows(self.h))
         return dup, self.changes(int(nchg.value))
 
+    def vacuum(self, counts, ef_construction=64):
+        """VACUUM's graph work on the resident image (hnswbulkdelete after RemoveHeapTids, src/hnswvacuum.c): counts
+        [n] are the heap TIDs each element keeps (0..10; 0 = deleted now or by an earlier vacuum).  Elements that link to
+        a deleted one are repaired, the entry point is replaced when it is deleted, and deleted elements lose every
+        neighbour; their numbers are not reused.  Returns (the change records, as insert() returns them; the number of
+        elements repaired)."""
+        counts = np.ascontiguousarray(counts, dtype=np.int32)
+        n = int(load().vb_hnsw_rows(self.h))
+        if counts.shape != (n,):
+            raise ValueError(f"counts must have {n} entries, got {counts.shape}")
+        nrep, nchg = C.c_int64(0), C.c_int64(0)
+        _lib.check(load().vb_hnsw_vacuum(self.h, _ptr(counts), int(ef_construction), C.byref(nrep), C.byref(nchg)))
+        return self.changes(int(nchg.value)), int(nrep.value)
+
     def changes(self, count):
-        """the last insert's change records (count = the number it reported)"""
+        """the last insert's or vacuum's change records (count = the number it reported)"""
         out = np.empty(count, dtype=HNSW_SLOT_DTYPE)
         _lib.check(load().vb_hnsw_insert_changes(self.h, _ptr(out), count))
         return out

@@ -121,6 +121,7 @@ SIGNATURES = {
     "vb_hnsw_insert_dev": (_i, [_vp, _vp, _i64, _i, _u64, _vp, _vp, C.POINTER(_i64)]),
     "vb_hnsw_insert_changes": (_i, [_vp, _vp, _i64]),
     "vb_hnsw_set_heaptid_counts": (_i, [_vp, _vp]),
+    "vb_hnsw_vacuum": (_i, [_vp, _vp, _i, C.POINTER(_i64), C.POINTER(_i64)]),
     "vb_hnsw_rows": (_i64, [_vp]),
     "vb_hnsw_upper_slots": (_i64, [_vp]),
     "vb_hnsw_export": (_i, [_vp, _vp, _vp, _vp, _vp, C.POINTER(_i64), _vp]),

@@ -50,11 +50,11 @@ struct Hnsw {
     float *nd0 = nullptr, *upper_d = nullptr;
     int32_t *dup_of = nullptr, *n_heaptids = nullptr;
     int64_t upper_slots = 0;
-    uint64_t generation = 0;  // bumped by every load, build and insert: filters and filtered scan handles refuse a changed image
+    uint64_t generation = 0;  // bumped by every load, build, insert and vacuum: filters and filtered scan handles refuse a changed image
     // capacities of the per-element arrays (levels, upper_off, nbr0, nd0, dup_of, n_heaptids) and of the upper slots
     // (upper, upper_d): vb_hnsw_insert grows them geometrically
     int64_t elem_cap = 0, slot_cap = 0;
-    // the last insert's change records, sorted by (element, layer, slot): key = element << 14 | layer << 8 | slot
+    // the last insert's or vacuum's change records, sorted by (element, layer, slot): key = element << 14 | layer << 8 | slot
     uint64_t* rec_key = nullptr;
     int32_t* rec_val = nullptr;
     int64_t rec_cap = 0, n_changes = 0;
@@ -616,16 +616,69 @@ __device__ __forceinline__ void hnsw_merge_batch(HnswWarpState& S, int cnt, int 
 }
 #endif
 
+// The vacuum's admission of one expansion's fresh neighbours (bkey / bid [0..cnt), list order) into R, one at a time as
+// the reference does, because under CountElement (src/hnswutils.c:713-728, 957-974) the result depends on the order:
+// elements with no heap TIDs do not count towards ef.  wlen counts the counted additions and is never decremented;
+// while wlen < ef everything is added, afterwards an element is added when it is nearer than R's last one, and each
+// counted addition past ef removes R's last one, counted or not.  R can therefore hold more than ef entries.  Returns
+// false when an addition needs more than wcap entries (R is then incomplete: the caller reruns with a larger one).
+__device__ __forceinline__ bool hnsw_admit_counted(HnswWarpState& S, int cnt, int ef, int& wlen, const int32_t* __restrict__ counts,
+                                                   int wcap, int lane) {
+    const uint64_t mk = lane < cnt ? S.bkey[lane] : 0ull;
+    const uint32_t mi = lane < cnt ? S.bid[lane] : 0u;
+    const unsigned cm = __ballot_sync(0xffffffffu, lane < cnt && counts[mi & 0x7fffffffu] != 0);
+    for (int i = 0; i < cnt; ++i) {
+        const uint64_t k = __shfl_sync(0xffffffffu, mk, i);
+        const uint32_t id = __shfl_sync(0xffffffffu, mi, i) & 0x7fffffffu;
+        const int len = S.len;
+        if (!(wlen < ef || ent_less(k, id, S.rk[len - 1], S.ri[len - 1]))) continue;
+        const bool counted = (cm >> i) & 1u;
+        const bool pop = counted && wlen >= ef;   // (then k is nearer than R's last one: it lands before it)
+        const int nlen = pop ? len : len + 1;
+        if (nlen > wcap) return false;
+        int p = 0;   // entries of R before (k, id)
+        for (int j = lane; j < len; j += 32) p += ent_less(S.rk[j], S.ri[j], k, id) ? 1 : 0;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) p += __shfl_xor_sync(0xffffffffu, p, o);
+        for (int j0 = nlen - 1; j0 > p; j0 -= 32) {
+            const int j = j0 - lane;
+            uint64_t kj = 0;
+            uint32_t ij = 0;
+            if (j > p) {
+                kj = S.rk[j - 1];
+                ij = S.ri[j - 1];
+            }
+            __syncwarp();
+            if (j > p) {
+                S.rk[j] = kj;
+                S.ri[j] = ij;
+            }
+            __syncwarp();
+        }
+        if (lane == 0) {
+            S.rk[p] = k;
+            S.ri[p] = id;   // unexpanded
+        }
+        __syncwarp();
+        S.len = nlen;
+        if (counted) ++wlen;
+    }
+    return true;
+}
+
 // HnswSearchLayer (src/hnswutils.c:824-987) at layer lc with ef = efl from the entry points already in R
 // (S.len of them, sorted).  tab / cap: this layer's visited table (cleared here, InitVisited :671-680).
 // ndist (may be null) accumulates the reference's `tuples` counter (:866-873, 905-906).  Returns false when the
 // visited table filled beyond three quarters (the caller retries with a larger one).
 // ITER: the iterative scan's variant -- everything seen and not kept goes to `sink`; init_visited = false resumes on
 // the visited table of the previous call (entry points are neither re-added nor counted, :864-873).
-template <int ELEM, int METRIC, int LPR, bool ITER = false>
+// VAC: the vacuum's variant -- elements with counts[] == 0 do not count towards ef (hnsw_admit_counted); R holds up to
+// wcap entries, and *wfull is set (and false returned) when that is not enough.
+template <int ELEM, int METRIC, int LPR, bool ITER = false, bool VAC = false>
 __device__ __forceinline__ bool hnsw_search_layer(const HnswDev& g, const uint4* sq, int lc, int efl, int lane, HnswWarpState& S,
                                                   uint32_t* tab, uint32_t cap, int64_t* ndist, HnswSink* sink = nullptr,
-                                                  bool init_visited = true) {
+                                                  bool init_visited = true, const int32_t* counts = nullptr, int wcap = 0,
+                                                  bool* wfull = nullptr) {
     const int lm = lc == 0 ? 2 * g.m : g.m;
     const uint32_t mask = cap - 1;
     uint32_t inserted = 0;
@@ -640,7 +693,7 @@ __device__ __forceinline__ bool hnsw_search_layer(const HnswDev& g, const uint4*
         }
         __syncwarp();
         // entry points: visited, unexpanded; they count towards `tuples` (src/hnswutils.c:866-873)
-        if (S.len > efl) S.len = efl;   // ef shrinks only between an ef_construction layer and ... never; kept for safety
+        if (!VAC && S.len > efl) S.len = efl;   // ef shrinks only between an ef_construction layer and ... never; kept for safety
 #if VB_AB_VISB
         for (int i0 = 0; i0 < S.len; i0 += 32) {
             const int i = i0 + lane;
@@ -665,6 +718,12 @@ __device__ __forceinline__ bool hnsw_search_layer(const HnswDev& g, const uint4*
     }
 
     bool ok = true;
+    int wlen = 0;   // VAC: counted entries added (the entry points are the previous layer's W)
+    if constexpr (VAC) {
+        for (int i = lane; i < S.len; i += 32) wlen += counts[S.ri[i] & 0x7fffffffu] != 0 ? 1 : 0;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) wlen += __shfl_xor_sync(0xffffffffu, wlen, o);
+    }
     uint32_t pre_c = VIS_EMPTY;   // VB_AB_NEXTPF: the element whose list sits in pre_nid
     int pre_nid = -1;
     for (;;) {
@@ -828,8 +887,19 @@ __device__ __forceinline__ bool hnsw_search_layer(const HnswDev& g, const uint4*
             }
 #endif
 
-            hnsw_merge_batch<ITER>(S, cnt, efl, lane, sink);
+            if constexpr (VAC) {
+                if (!hnsw_admit_counted(S, cnt, efl, wlen, counts, wcap, lane)) {
+                    *wfull = true;
+                    ok = false;
+                    break;
+                }
+            } else {
+                hnsw_merge_batch<ITER>(S, cnt, efl, lane, sink);
+            }
             if (first_inval < 32) break;
+        }
+        if constexpr (VAC) {
+            if (!ok) break;
         }
         // keep the table at most three quarters full; otherwise report and let the host retry with a larger one
 #ifndef VB_AB_VIS

@@ -63,6 +63,22 @@ struct InsertRec {
     int* n;
 };
 
+// vb_hnsw_vacuum's side of K1 / K2 (a parameter of its own, so the build and insert kernels keep their parameter layout):
+// the batch repairs the elements list[0..B); K1 writes their new lists to the staging area, which is published only after
+// every search of the batch has finished.
+struct VacDev {
+    const int32_t* list;     // [B] elements repaired by this batch, ascending
+    int32_t* stage0;         // [B][2m] new layer-0 lists, by list position
+    int32_t* stage_up;       // [slots][m] new upper lists, at the element's own upper slots
+    const int32_t* counts;   // [n] heap TID counts (0 = being deleted or deleted)
+    uint64_t* wk;            // per-warp W in global memory ([warps][2][wcap] keys, ids, pruned indices and flags), or null:
+    uint32_t* wi;            // W in shared memory, wcap entries
+    uint16_t* wd;
+    uint8_t* dead;
+    int wcap;
+    int* wfull;              // set when a repair's W needs more than wcap entries
+};
+
 constexpr int HB_CAND = 256;     // candidates of one HnswUpdateConnection: lm + 1 <= 201, padded to a power of two
 
 __device__ __forceinline__ float key64_to_float(uint64_t k) { return (float)key64_to_double(k); }
@@ -114,36 +130,59 @@ __device__ __forceinline__ void prune_against(const HnswDev& g, const uint4* img
 
 // K1: one warp = one new element.  INS (vb_hnsw_insert): candidates whose element is being deleted (heap TID count 0)
 // help the search but are removed before SelectNeighbors (RemoveElements, src/hnswutils.c:1237-1259, 1343-1344).
-template <int ELEM, int METRIC, int LPR, bool INS = false>
+// VAC (vb_hnsw_vacuum): one warp = one repaired element, list[w] = RepairGraphElement (src/hnswvacuum.c:225-274) =
+// HnswFindElementNeighbors with existing = true: elements being deleted do not count towards ef (R holds v.wcap
+// entries), ef_construction + 1 (b.efc already is), the element itself is removed too, and the whole new tuple goes to
+// the staging area (the layers above the entry point's level are left empty, as the reference's are).
+template <int ELEM, int METRIC, int LPR, bool INS = false, bool VAC = false>
 __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_insert_kernel(BuildDev b, uint32_t* __restrict__ vis_all, uint32_t vis_cap,
-                                                                    uint32_t vis_upper) {
+                                                                    uint32_t vis_upper, VacDev v) {
     extern __shared__ uint4 smem[];
     const HnswDev& g = b.g;
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
     const int efc = b.efc, lm0 = 2 * g.m;
-    uint8_t* base = reinterpret_cast<uint8_t*>(smem) + (size_t)warp * hb_insert_smem(b.qvec, efc, lm0);
+    const int wc = VAC ? v.wcap : efc;   // capacity of R and of the candidate arrays
+    uint8_t* base = reinterpret_cast<uint8_t*>(smem) + (size_t)warp * hb_insert_smem(b.qvec, VAC && v.wk ? 0 : wc, lm0);
     uint4* sq = reinterpret_cast<uint4*>(base);
     uint4* img = sq + b.qvec;
     uint64_t* keyA = reinterpret_cast<uint64_t*>(img + b.qvec);
-    uint64_t* keyB = keyA + efc;
-    uint64_t* bkey = keyB + efc;
+    uint64_t* keyB = keyA + (VAC && v.wk ? 0 : wc);
+    uint64_t* bkey = keyB + (VAC && v.wk ? 0 : wc);
     uint32_t* idA = reinterpret_cast<uint32_t*>(bkey + 32);
-    uint32_t* idB = idA + efc;
-    uint32_t* bid = idB + efc;
+    uint32_t* idB = idA + (VAC && v.wk ? 0 : wc);
+    uint32_t* bid = idB + (VAC && v.wk ? 0 : wc);
     int32_t* bj = reinterpret_cast<int32_t*>(bid + 32);
     int32_t* sel = bj + 32;
     uint16_t* wd = reinterpret_cast<uint16_t*>(sel + lm0);
-    uint8_t* dead = reinterpret_cast<uint8_t*>(wd + efc);
+    uint8_t* dead = reinterpret_cast<uint8_t*>(wd + (VAC && v.wk ? 0 : wc));
 
     const int gwarp = blockIdx.x * HN_WARPS + warp;
     const int nwarps = gridDim.x * HN_WARPS;
     uint32_t* vis = vis_all + (size_t)gwarp * vis_cap;
+    if constexpr (VAC) {
+        if (v.wk) {
+            keyA = v.wk + (size_t)gwarp * 2 * wc;
+            keyB = keyA + wc;
+            idA = v.wi + (size_t)gwarp * 2 * wc;
+            idB = idA + wc;
+            wd = v.wd + (size_t)gwarp * wc;
+            dead = v.dead + (size_t)gwarp * wc;
+        }
+    }
 
     for (int w = gwarp; w < b.B; w += nwarps) {
-        const int e = b.b0 + w;
+        const int e = VAC ? v.list[w] : b.b0 + w;
         load_row_image<ELEM, METRIC>(g.rows + (size_t)e * g.stride, g.V, sq, lane);
         __syncwarp();
         const int level = g.levels[e];
+        if constexpr (VAC) {
+            // the whole tuple is rewritten: every layer starts empty
+            for (int i = lane; i < lm0; i += 32) v.stage0[(size_t)w * lm0 + i] = -1;
+            for (int lc = 1; lc <= level; ++lc)
+                for (int i = lane; i < g.m; i += 32) v.stage_up[((size_t)g.upper_off[e] + (lc - 1)) * g.m + i] = -1;
+            __syncwarp();
+            if (g.entry < 0) continue;   // no entry point: no neighbours (src/hnswutils.c:1297-1299)
+        }
 
         HnswWarpState S;
         S.rk = keyA;
@@ -166,16 +205,20 @@ __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_insert_kernel(BuildDev b, 
             S.len = 1;
             __syncwarp();
         }
-        bool failed = false;
+        bool failed = false, wfull = false;
         // 1st phase: greedy search to the insert level (src/hnswutils.c:1308-1313)
         int lc = g.entry_level;
-        for (; lc > level && !failed; --lc) failed = !hnsw_search_layer<ELEM, METRIC, LPR>(g, sq, lc, 1, lane, S, vis, vis_upper, nullptr);
+        for (; lc > level && !failed; --lc)
+            failed = !hnsw_search_layer<ELEM, METRIC, LPR, false, VAC>(g, sq, lc, 1, lane, S, vis, vis_upper, nullptr, nullptr, true,
+                                                                       v.counts, wc, &wfull);
         // 2nd phase (:1322-1354): level = min(level, entryLevel)
         for (; lc >= 0 && !failed; --lc) {
-            failed = !hnsw_search_layer<ELEM, METRIC, LPR>(g, sq, lc, efc, lane, S, vis + vis_upper, vis_cap - vis_upper, nullptr);
+            failed = !hnsw_search_layer<ELEM, METRIC, LPR, false, VAC>(g, sq, lc, efc, lane, S, vis + vis_upper, vis_cap - vis_upper, nullptr,
+                                                                       nullptr, true, v.counts, wc, &wfull);
             if (failed) break;
             const int lm = lc == 0 ? lm0 : g.m;
-            int32_t* out_ids = lc == 0 ? b.nbr0_w + (size_t)e * lm : b.upper_w + ((size_t)g.upper_off[e] + (lc - 1)) * (size_t)lm;
+            int32_t* out_ids = VAC ? (lc == 0 ? v.stage0 + (size_t)w * lm : v.stage_up + ((size_t)g.upper_off[e] + (lc - 1)) * (size_t)lm)
+                                   : lc == 0 ? b.nbr0_w + (size_t)e * lm : b.upper_w + ((size_t)g.upper_off[e] + (lc - 1)) * (size_t)lm;
             float* out_d = lc == 0 ? b.nd0 + (size_t)e * lm : b.upper_d + ((size_t)g.upper_off[e] + (lc - 1)) * (size_t)lm;
             int len = S.len;
             const uint64_t* wk = S.rk;     // W, nearest first; stays intact: it is the next layer's entry list (ep = w)
@@ -185,7 +228,8 @@ __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_insert_kernel(BuildDev b, 
                 int kept = 0;
                 for (int i0 = 0; i0 < len; i0 += 32) {
                     const int i = i0 + lane;
-                    const bool keep = i < len && b.n_heaptids[S.ri[i] & 0x7fffffffu] != 0;
+                    const uint32_t id = i < len ? S.ri[i] & 0x7fffffffu : 0u;
+                    const bool keep = i < len && b.n_heaptids[id] != 0 && (!VAC || id != (uint32_t)e);
                     const unsigned km = __ballot_sync(0xffffffffu, keep);
                     if (keep) {
                         const int p = kept + __popc(km & ((1u << lane) - 1u));
@@ -238,7 +282,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_insert_kernel(BuildDev b, 
             }
             __syncwarp();
         }
-        if (failed && lane == 0) atomicExch(b.overflow, 1);
+        if (failed && lane == 0) atomicExch(VAC && wfull ? v.wfull : b.overflow, 1);
         __syncwarp();
     }
 }
@@ -462,9 +506,12 @@ __device__ __forceinline__ void hb_record(const InsertRec& r, int t, int lc, int
 //                                    connections and the new element, nearest first; the pruned connection is replaced
 //                                    in its slot, nothing changes when the new element is the one pruned.
 // Every slot written is recorded (rec_key / rec_val); later records of a slot supersede earlier ones.
-template <int ELEM, int METRIC, int LPR>
+// VAC (vb_hnsw_vacuum): the source is the repaired element v.list[...], and a target that already links to it is left as
+// it is (ConnectionExists, src/hnswinsert.c:453-468, 503-505); the records come from the diff of the whole call instead.
+template <int ELEM, int METRIC, int LPR, bool VAC = false>
 __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_update_disk_kernel(BuildDev b, const uint64_t* __restrict__ keys,
-                                                                         const float* __restrict__ vals, int n_edges, InsertRec r) {
+                                                                         const float* __restrict__ vals, int n_edges, InsertRec r,
+                                                                         VacDev v) {
     extern __shared__ uint4 smem[];
     const HnswDev& g = b.g;
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
@@ -488,20 +535,27 @@ __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_update_disk_kernel(BuildDe
         int32_t* ids = lc == 0 ? b.nbr0_w + (size_t)t * lm : b.upper_w + ((size_t)g.upper_off[t] + (lc - 1)) * (size_t)lm;
         bool have_d = false;
         for (int64_t p = i; p < n_edges && (keys[p] >> 20) == head; ++p) {
-            const int src = b.b0 + (int)(keys[p] & 0xFFFFFu);
+            const int src = VAC ? v.list[keys[p] & 0xFFFFFu] : b.b0 + (int)(keys[p] & 0xFFFFFu);
             const float d = vals[p];
             // current length = first invalid entry
             int count = lm;
+            bool exists = false;
             for (int off = 0; off < lm; off += 32) {
                 const int nid = off + lane < lm ? ids[off + lane] : -1;
                 const unsigned inval = ~__ballot_sync(0xffffffffu, nid >= 0);
+                if constexpr (VAC) {
+                    const int valid = inval ? __ffs(inval) - 1 : 32;
+                    exists = exists || __any_sync(0xffffffffu, lane < valid && nid == src);
+                }
                 if (inval) {
                     count = min(lm, off + __ffs(inval) - 1);
                     break;
                 }
             }
             int slot = -1;
-            if (count < lm) {
+            if (VAC && exists) {
+                // ConnectionExists: the target keeps its list
+            } else if (count < lm) {
                 slot = count;
             } else {
                 if (!have_d) {
@@ -581,7 +635,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_update_disk_kernel(BuildDe
             if (slot >= 0 && lane == 0) {
                 ids[slot] = src;
                 if (have_d) cd[slot] = d;
-                hb_record(r, t, lc, slot, src);
+                if (!VAC) hb_record(r, t, lc, slot, src);
             }
             __syncwarp();
         }
@@ -630,67 +684,72 @@ __global__ void fill_i32_kernel(int32_t* p, int64_t n, int32_t v) {
 // ----------------------------------------------------------------------------- host side
 
 enum { WSB_KEYS = 14, WSB_KEYS2 = 15, WSB_VALS = 16, WSB_VALS2 = 17, WSB_TMP = 18, WSB_FLAGS = 19, WSB_KEEP = 20 };
+enum { WSB_VSEL = 21, WSB_VOLD0 = 22, WSB_VOLDUP = 23, WSB_VSTAGE0 = 24, WSB_VSTAGEUP = 25 };
 
 struct BuildLaunch {
-    int (*insert)(const BuildDev&, uint32_t*, uint32_t, uint32_t, int, size_t, int*);
-    int (*update)(const BuildDev&, const uint64_t*, const float*, int, const InsertRec&, int, size_t, int*);
+    int (*insert)(const BuildDev&, const VacDev&, uint32_t*, uint32_t, uint32_t, int, size_t, int*);
+    int (*update)(const BuildDev&, const VacDev&, const uint64_t*, const float*, int, const InsertRec&, int, size_t, int*);
 };
 
-// INS: the kernels of vb_hnsw_insert (RemoveElements in K1, UpdateNeighborOnDisk in K2)
-template <int ELEM, int METRIC, int LPR, bool INS>
-static int launch_insert(const BuildDev& b, uint32_t* vis, uint32_t vis_cap, uint32_t vis_upper, int grid, size_t smem, int* occ) {
-    auto kern = hnsw_insert_kernel<ELEM, METRIC, LPR, INS>;
+// the three modes of the batch loop: the build, vb_hnsw_insert (RemoveElements in K1, UpdateNeighborOnDisk in K2) and
+// vb_hnsw_vacuum (RepairGraphElement in K1, UpdateNeighborOnDisk with ConnectionExists in K2)
+enum { HB_BUILD = 0, HB_INSERT = 1, HB_VACUUM = 2 };
+
+template <int ELEM, int METRIC, int LPR, int MODE>
+static int launch_insert(const BuildDev& b, const VacDev& v, uint32_t* vis, uint32_t vis_cap, uint32_t vis_upper, int grid, size_t smem,
+                         int* occ) {
+    auto kern = hnsw_insert_kernel<ELEM, METRIC, LPR, MODE != HB_BUILD, MODE == HB_VACUUM>;
     if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (occ) {
         VB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, HN_WARPS * 32, smem));
         return VB_OK;
     }
-    kern<<<grid, HN_WARPS * 32, smem, ctx().stream>>>(b, vis, vis_cap, vis_upper);
+    kern<<<grid, HN_WARPS * 32, smem, ctx().stream>>>(b, vis, vis_cap, vis_upper, v);
     VB_CUDA(cudaGetLastError());
     count_launch();
     return VB_OK;
 }
-template <int ELEM, int METRIC, int LPR, bool INS>
-static int launch_update(const BuildDev& b, const uint64_t* keys, const float* vals, int n_edges, const InsertRec& r, int grid, size_t smem,
-                         int* occ) {
+template <int ELEM, int METRIC, int LPR, int MODE>
+static int launch_update(const BuildDev& b, const VacDev& v, const uint64_t* keys, const float* vals, int n_edges, const InsertRec& r,
+                         int grid, size_t smem, int* occ) {
     auto kern = hnsw_update_kernel<ELEM, METRIC, LPR>;
-    auto kern_disk = hnsw_update_disk_kernel<ELEM, METRIC, LPR>;
-    const void* k = INS ? (const void*)kern_disk : (const void*)kern;
+    auto kern_disk = hnsw_update_disk_kernel<ELEM, METRIC, LPR, MODE == HB_VACUUM>;
+    const void* k = MODE != HB_BUILD ? (const void*)kern_disk : (const void*)kern;
     if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (occ) {
         VB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, k, HN_WARPS * 32, smem));
         return VB_OK;
     }
-    if (INS) kern_disk<<<grid, HN_WARPS * 32, smem, ctx().stream>>>(b, keys, vals, n_edges, r);
+    if (MODE != HB_BUILD) kern_disk<<<grid, HN_WARPS * 32, smem, ctx().stream>>>(b, keys, vals, n_edges, r, v);
     else kern<<<grid, HN_WARPS * 32, smem, ctx().stream>>>(b, keys, vals, n_edges);
     VB_CUDA(cudaGetLastError());
     count_launch();
     return VB_OK;
 }
 
-template <int ELEM, int METRIC, bool INS>
+template <int ELEM, int METRIC, int MODE>
 static BuildLaunch pick_lpr(int V) {
     // lanes per row: a whole warp for rows of >= 512 bytes, 8 lanes for >= 128 bytes, one lane for tiny rows
-    if (V >= 32) return BuildLaunch{launch_insert<ELEM, METRIC, 32, INS>, launch_update<ELEM, METRIC, 32, INS>};
-    if (V >= 8) return BuildLaunch{launch_insert<ELEM, METRIC, 8, INS>, launch_update<ELEM, METRIC, 8, INS>};
-    return BuildLaunch{launch_insert<ELEM, METRIC, 1, INS>, launch_update<ELEM, METRIC, 1, INS>};
+    if (V >= 32) return BuildLaunch{launch_insert<ELEM, METRIC, 32, MODE>, launch_update<ELEM, METRIC, 32, MODE>};
+    if (V >= 8) return BuildLaunch{launch_insert<ELEM, METRIC, 8, MODE>, launch_update<ELEM, METRIC, 8, MODE>};
+    return BuildLaunch{launch_insert<ELEM, METRIC, 1, MODE>, launch_update<ELEM, METRIC, 1, MODE>};
 }
 
-template <bool INS>
+template <int MODE>
 static bool pick_kernels(const Hnsw& h, int V, BuildLaunch* out) {
     if (h.elem == VB_VECTOR) {
-        if (h.metric == VB_L2_SQUARED) *out = pick_lpr<VB_VECTOR, VB_L2_SQUARED, INS>(V);
-        else if (h.metric == VB_NEG_IP) *out = pick_lpr<VB_VECTOR, VB_NEG_IP, INS>(V);
-        else if (h.metric == VB_L1) *out = pick_lpr<VB_VECTOR, VB_L1, INS>(V);
+        if (h.metric == VB_L2_SQUARED) *out = pick_lpr<VB_VECTOR, VB_L2_SQUARED, MODE>(V);
+        else if (h.metric == VB_NEG_IP) *out = pick_lpr<VB_VECTOR, VB_NEG_IP, MODE>(V);
+        else if (h.metric == VB_L1) *out = pick_lpr<VB_VECTOR, VB_L1, MODE>(V);
         else return false;
     } else if (h.elem == VB_HALFVEC) {
-        if (h.metric == VB_L2_SQUARED) *out = pick_lpr<VB_HALFVEC, VB_L2_SQUARED, INS>(V);
-        else if (h.metric == VB_NEG_IP) *out = pick_lpr<VB_HALFVEC, VB_NEG_IP, INS>(V);
-        else if (h.metric == VB_L1) *out = pick_lpr<VB_HALFVEC, VB_L1, INS>(V);
+        if (h.metric == VB_L2_SQUARED) *out = pick_lpr<VB_HALFVEC, VB_L2_SQUARED, MODE>(V);
+        else if (h.metric == VB_NEG_IP) *out = pick_lpr<VB_HALFVEC, VB_NEG_IP, MODE>(V);
+        else if (h.metric == VB_L1) *out = pick_lpr<VB_HALFVEC, VB_L1, MODE>(V);
         else return false;
     } else {
-        if (h.metric == VB_HAMMING) *out = pick_lpr<VB_BIT, VB_HAMMING, INS>(V);
-        else if (h.metric == VB_JACCARD) *out = pick_lpr<VB_BIT, VB_JACCARD, INS>(V);
+        if (h.metric == VB_HAMMING) *out = pick_lpr<VB_BIT, VB_HAMMING, MODE>(V);
+        else if (h.metric == VB_JACCARD) *out = pick_lpr<VB_BIT, VB_JACCARD, MODE>(V);
         else return false;
     }
     return true;
@@ -762,7 +821,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
 
     BuildLaunch K;
     const int V = (int)(h.rows.stride / 16);
-    if (!pick_kernels<false>(h, V, &K)) {
+    if (!pick_kernels<HB_BUILD>(h, V, &K)) {
         set_error("hnsw build: unsupported metric %d for element type %d", h.metric, h.elem);
         return VB_EINVAL;
     }
@@ -792,8 +851,8 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
     b.qvec = qvec;
 
     int occ_ins = 1, occ_upd = 1;
-    VB_TRY(K.insert(b, nullptr, 0, 0, 0, smem_ins, &occ_ins));
-    VB_TRY(K.update(b, nullptr, nullptr, 0, InsertRec{}, 0, smem_upd, &occ_upd));
+    VB_TRY(K.insert(b, VacDev{}, nullptr, 0, 0, 0, smem_ins, &occ_ins));
+    VB_TRY(K.update(b, VacDev{}, nullptr, nullptr, 0, InsertRec{}, 0, smem_upd, &occ_upd));
     const int max_grid_ins = c.sm_count * std::max(1, occ_ins);
     const int max_grid_upd = c.sm_count * std::max(1, occ_upd) * 4;
 
@@ -859,7 +918,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
                 h.vis_bytes = need;
             }
             VB_CUDA(cudaMemsetAsync(d_flags, 0, 2 * sizeof(int), s));
-            VB_TRY(K.insert(b, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
+            VB_TRY(K.insert(b, VacDev{}, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
             hnsw_finalize_kernel<false><<<(unsigned)std::min<int64_t>((B * 32 + 127) / 128, (int64_t)c.sm_count * 16), 128, 0, s>>>(b);
             VB_CUDA(cudaGetLastError());
             count_launch();
@@ -881,7 +940,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
                                                     (float*)d_v2, n_edges, 0, 57, s));
             count_launch();
             const int grid_upd = (int)std::min<int64_t>(((int64_t)n_edges + HN_WARPS - 1) / HN_WARPS, max_grid_upd);
-            VB_TRY(K.update(b, (const uint64_t*)d_k2, (const float*)d_v2, n_edges, InsertRec{}, grid_upd, smem_upd, nullptr));
+            VB_TRY(K.update(b, VacDev{}, (const uint64_t*)d_k2, (const float*)d_v2, n_edges, InsertRec{}, grid_upd, smem_upd, nullptr));
         }
         if (promote >= 0) {
             // UpdateGraphInMemory (src/hnswbuild.c:428-430): a duplicate never becomes the entry point
@@ -945,7 +1004,7 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
     VB_REQUIRE(rows || n == 0, "null rows");
     BuildLaunch K;
     const int V = (int)(h.rows.stride / 16);
-    if (!pick_kernels<true>(h, V, &K)) {
+    if (!pick_kernels<HB_INSERT>(h, V, &K)) {
         set_error("hnsw insert: unsupported metric %d for element type %d", h.metric, h.elem);
         return VB_EINVAL;
     }
@@ -1040,8 +1099,8 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
         VB_TRY(workspace(WSB_TMP, tmp_bytes, &d_tmp));
     }
     int occ_ins = 1, occ_upd = 1;
-    VB_TRY(K.insert(BuildDev{}, nullptr, 0, 0, 0, smem_ins, &occ_ins));
-    VB_TRY(K.update(BuildDev{}, nullptr, nullptr, 0, InsertRec{}, 0, smem_upd, &occ_upd));
+    VB_TRY(K.insert(BuildDev{}, VacDev{}, nullptr, 0, 0, 0, smem_ins, &occ_ins));
+    VB_TRY(K.update(BuildDev{}, VacDev{}, nullptr, nullptr, 0, InsertRec{}, 0, smem_upd, &occ_upd));
     const int max_grid_ins = c.sm_count * std::max(1, occ_ins);
     const int max_grid_upd = c.sm_count * std::max(1, occ_upd) * 4;
     uint32_t cap = 1u << 14;
@@ -1135,7 +1194,7 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
             const uint32_t vis_cap = cap + vis_upper;
             VB_TRY(reserve_vis(vis_cap));
             VB_CUDA(cudaMemsetAsync(d_flags, 0, 2 * sizeof(int), s));
-            VB_TRY(K.insert(b, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
+            VB_TRY(K.insert(b, VacDev{}, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
             hnsw_finalize_kernel<true><<<(unsigned)std::min<int64_t>((B * 32 + 127) / 128, (int64_t)c.sm_count * 16), 128, 0, s>>>(b);
             VB_CUDA(cudaGetLastError());
             count_launch();
@@ -1156,7 +1215,7 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
                                                     n_edges, 0, 57, s));
             count_launch();
             const int grid_upd = (int)std::min<int64_t>(((int64_t)n_edges + HN_WARPS - 1) / HN_WARPS, max_grid_upd);
-            VB_TRY(K.update(b, (const uint64_t*)d_k2, (const float*)d_v2, n_edges, rec, grid_upd, smem_upd, nullptr));
+            VB_TRY(K.update(b, VacDev{}, (const uint64_t*)d_k2, (const float*)d_v2, n_edges, rec, grid_upd, smem_upd, nullptr));
         }
         if (promote >= 0) {
             // a folded row never becomes the entry point
@@ -1205,6 +1264,447 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
     h.n_changes = n_sel;
     if (out_nchanges) *out_nchanges = n_sel;
     return VB_OK;
+}
+
+// ----------------------------------------------------------------------------- vacuum a resident image
+
+// NeedsUpdated (src/hnswvacuum.c:178-220) of the elements [from, n): live, not `skip`, and a slot on any layer names an
+// element with no heap TIDs, or the last layer-0 slot is empty
+__global__ void hnsw_needs_update_kernel(HnswDev g, const int32_t* __restrict__ counts, int64_t from, int skip, uint8_t* __restrict__ flag) {
+    const int64_t e = from + blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (e >= g.n) return;
+    const int lm0 = 2 * g.m;
+    bool need = false;
+    if (counts[e] != 0 && e != skip) {
+        const int32_t* l0 = g.nbr0 + (size_t)e * lm0;
+        need = l0[lm0 - 1] < 0;
+        for (int i = 0; i < lm0 && !need; ++i) need = l0[i] >= 0 && counts[l0[i]] == 0;
+        for (int lc = 1; lc <= g.levels[e] && !need; ++lc) {
+            const int32_t* u = g.upper + ((size_t)g.upper_off[e] + (lc - 1)) * g.m;
+            for (int i = 0; i < g.m && !need; ++i) need = u[i] >= 0 && counts[u[i]] == 0;
+        }
+    }
+    flag[e - from] = need ? 1 : 0;
+}
+
+// the update records of a repair batch (UpdateNeighborsOnDisk's loop, src/hnswinsert.c:545-580): one per staged neighbour,
+// source = the position in the batch's list
+__global__ void __launch_bounds__(128) hnsw_vacuum_edges_kernel(BuildDev b, VacDev v) {
+    const HnswDev& g = b.g;
+    const int lane = threadIdx.x % 32;
+    const int gwarp = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32);
+    const int nwarps = (int)((gridDim.x * (int64_t)blockDim.x) / 32);
+    const int lm0 = 2 * g.m;
+    if (g.entry < 0) return;
+    for (int w = gwarp; w < b.B; w += nwarps) {
+        const int e = v.list[w];
+        const int top = min(g.levels[e], g.entry_level);
+        for (int lc = top; lc >= 0; --lc) {
+            const int lm = lc == 0 ? lm0 : g.m;
+            const int32_t* ids = lc == 0 ? v.stage0 + (size_t)w * lm : v.stage_up + ((size_t)g.upper_off[e] + (lc - 1)) * (size_t)lm;
+            const float* ds = lc == 0 ? b.nd0 + (size_t)e * lm : b.upper_d + ((size_t)g.upper_off[e] + (lc - 1)) * (size_t)lm;
+            for (int off = 0; off < lm; off += 32) {
+                const int t = off + lane < lm ? ids[off + lane] : -1;
+                const unsigned vm = __ballot_sync(0xffffffffu, t >= 0);
+                const int cnt = __popc(vm);
+                if (cnt == 0) break;
+                int slot = 0;
+                if (lane == 0) slot = atomicAdd(b.n_edges, cnt);
+                slot = __shfl_sync(0xffffffffu, slot, 0);
+                if (t >= 0) {
+                    const int p = slot + __popc(vm & ((1u << lane) - 1u));
+                    b.edge_key[p] = ((uint64_t)(uint32_t)t << 26) | ((uint64_t)lc << 20) | (uint64_t)w;
+                    b.edge_val[p] = ds[off + lane];
+                }
+            }
+        }
+    }
+}
+
+// the staged tuples of the batch replace the repaired elements' own (PageIndexTupleOverwrite, src/hnswvacuum.c:264-266)
+__global__ void hnsw_vacuum_publish_kernel(BuildDev b, VacDev v) {
+    const HnswDev& g = b.g;
+    const int w = blockIdx.x;
+    const int e = v.list[w];
+    const int lm0 = 2 * g.m;
+    for (int i = threadIdx.x; i < lm0; i += blockDim.x) b.nbr0_w[(size_t)e * lm0 + i] = v.stage0[(size_t)w * lm0 + i];
+    for (int lc = 1; lc <= g.levels[e]; ++lc) {
+        const size_t o = ((size_t)g.upper_off[e] + (lc - 1)) * g.m;
+        for (int i = threadIdx.x; i < g.m; i += blockDim.x) b.upper_w[o + i] = v.stage_up[o + i];
+    }
+}
+
+// MarkDeleted (src/hnswvacuum.c:594-729): every neighbour slot of an element with no heap TIDs is cleared
+__global__ void hnsw_mark_deleted_kernel(BuildDev b, const int32_t* __restrict__ counts) {
+    const HnswDev& g = b.g;
+    const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (e >= g.n || counts[e] != 0) return;
+    const int lm0 = 2 * g.m;
+    for (int i = 0; i < lm0; ++i) b.nbr0_w[(size_t)e * lm0 + i] = -1;
+    for (int lc = 1; lc <= g.levels[e]; ++lc)
+        for (int i = 0; i < g.m; ++i) b.upper_w[((size_t)g.upper_off[e] + (lc - 1)) * g.m + i] = -1;
+}
+
+// the change records of a vacuum: every slot whose value differs from the snapshot taken before the call
+__global__ void hnsw_slot_diff_kernel(HnswDev g, const int32_t* __restrict__ old0, const int32_t* __restrict__ old_up, InsertRec r) {
+    const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (e >= g.n) return;
+    const int lm0 = 2 * g.m;
+    for (int lc = 0; lc <= g.levels[e]; ++lc) {
+        const int lm = lc == 0 ? lm0 : g.m;
+        const size_t o = lc == 0 ? (size_t)e * lm0 : ((size_t)g.upper_off[e] + (lc - 1)) * g.m;
+        const int32_t* now = lc == 0 ? g.nbr0 : g.upper;
+        const int32_t* was = lc == 0 ? old0 : old_up;
+        for (int i = 0; i < lm; ++i)
+            if (now[o + i] != was[o + i]) hb_record(r, (int)e, lc, i, now[o + i]);
+    }
+}
+
+// hnswbulkdelete's graph work (src/hnswvacuum.c:776-797 without RemoveHeapTids, which the caller runs on the pages) on the
+// resident image: RepairGraphEntryPoint, RepairGraph in batches (NeedsUpdated evaluated at each batch's start, the batch
+// taken from the candidates in element order), MarkDeleted, then the change records as the diff against a snapshot of the
+// neighbour arrays.  Everything the call needs is reserved before the first kernel.
+static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* out_nrepaired, int64_t* out_nchanges) {
+    VB_REQUIRE(h.loaded, "hnsw index not loaded");
+    VB_REQUIRE(efc >= 4 && efc <= 1000, "ef_construction must be 4..1000 (src/hnsw.h:57-59)");
+    VB_REQUIRE(efc >= 2 * h.m, "ef_construction must be greater than or equal to 2 * m (src/hnswbuild.c:713-716)");
+    const int64_t n = h.n;
+    VB_REQUIRE(counts || n == 0, "null counts");
+    for (int64_t i = 0; i < n; ++i)
+        VB_REQUIRE(counts[i] >= 0 && counts[i] <= 10, "vb_hnsw_vacuum: counts[%lld] = %d is not in 0..10 (HNSW_HEAPTIDS, src/hnsw.h:69)",
+                   (long long)i, counts[i]);
+    BuildLaunch K;
+    const int V = (int)(h.rows.stride / 16);
+    if (!pick_kernels<HB_VACUUM>(h, V, &K)) {
+        set_error("hnsw vacuum: unsupported metric %d for element type %d", h.metric, h.elem);
+        return VB_EINVAL;
+    }
+    if (out_nrepaired) *out_nrepaired = 0;
+    if (out_nchanges) *out_nchanges = 0;
+    const int m = h.m, lm0 = 2 * m;
+    const int qvec = h.elem == VB_HALFVEC ? 2 * V : V;
+    const int efv = efc + 1;   // "Add one for existing element" (src/hnswutils.c:1315-1317)
+    // R in shared memory holds a few times ef: elements being deleted do not count towards ef
+    int wcap_s = 4 * efv;
+    while (wcap_s > efv && hb_insert_smem(qvec, wcap_s, lm0) * HN_WARPS > 160 * 1024) wcap_s -= efv / 2 + 1;
+    const size_t smem_ins = hb_insert_smem(qvec, wcap_s, lm0) * HN_WARPS;
+    const size_t smem_glob = hb_insert_smem(qvec, 0, lm0) * HN_WARPS;
+    const size_t smem_upd = hb_update_disk_smem(qvec) * HN_WARPS;
+    VB_REQUIRE(wcap_s >= efv && smem_ins <= 200 * 1024 && smem_upd <= 200 * 1024,
+               "ef_construction %d / m %d with this dimension need %zu bytes of shared memory per CTA", efc, m, smem_ins);
+    if (n == 0) {
+        ++h.generation;
+        h.n_changes = 0;
+        return VB_OK;
+    }
+    Context& c = ctx();
+    cudaStream_t s = c.stream;
+
+    std::vector<int32_t> levels((size_t)n), dup((size_t)n, -1);
+    VB_CUDA(cudaMemcpyAsync(levels.data(), h.levels, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, s));
+    if (h.dup_of) VB_CUDA(cudaMemcpyAsync(dup.data(), h.dup_of, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    int64_t live = 0;
+    for (int64_t i = 0; i < n; ++i) {
+        VB_REQUIRE(dup[(size_t)i] < 0 || counts[i] == 0, "vb_hnsw_vacuum: row %lld was folded into element %d and is no element: its count must be 0",
+                   (long long)i, dup[(size_t)i]);
+        live += counts[i] != 0;
+    }
+    const int64_t frac = std::max<int64_t>(1, c.hnsw_build_fraction);
+    const int64_t b_max = std::min<int64_t>(std::min<int64_t>(1 << 20, std::max<int64_t>(1, c.hnsw_build_batch)), std::max<int64_t>(1, live / frac));
+    const int top_level = std::max(h.entry_level, 0);
+    const int64_t max_edges = b_max * (lm0 + (int64_t)top_level * m);
+    VB_REQUIRE(max_edges < (int64_t)0x7fffffff, "too many connection updates in one batch");
+    const int64_t slots = h.upper_slots;
+    const int64_t recs = n * lm0 + slots * m;   // every slot can change at most once
+    VB_REQUIRE(recs < (int64_t)0x7fffffff, "hnsw vacuum: too many neighbour slots");
+
+    // ---- reservations: nothing below changes the image until they have all succeeded
+    VB_TRY(hnsw_ensure_counts(h));
+    // distance scratch of the repaired elements' lists (an image made by vb_hnsw_load has none)
+    if (!h.nd0) VB_TRY(hnsw_grow((void**)&h.nd0, 0, sizeof(float) * (size_t)h.elem_cap * lm0, "layer-0 distances"));
+    if (!h.upper_d) VB_TRY(hnsw_grow((void**)&h.upper_d, 0, sizeof(float) * (size_t)h.slot_cap * m, "upper distances"));
+    if (recs > h.rec_cap) {
+        h.n_changes = 0;
+        h.rec_cap = 0;
+        VB_TRY(hnsw_grow((void**)&h.rec_key, 0, sizeof(uint64_t) * (size_t)recs, "change records"));
+        VB_TRY(hnsw_grow((void**)&h.rec_val, 0, sizeof(int32_t) * (size_t)recs, "change records"));
+        h.rec_cap = recs;
+    }
+    void *d_k1, *d_k2, *d_v1, *d_v2, *d_flags, *d_tmp, *d_need, *d_sel, *d_old0, *d_oldup, *d_stage0, *d_stageup;
+    VB_TRY(workspace(WSB_KEYS, sizeof(uint64_t) * (size_t)std::max<int64_t>(max_edges, 1), &d_k1));
+    VB_TRY(workspace(WSB_KEYS2, sizeof(uint64_t) * (size_t)std::max(max_edges, recs), &d_k2));
+    VB_TRY(workspace(WSB_VALS, sizeof(float) * (size_t)std::max<int64_t>(max_edges, 1), &d_v1));
+    VB_TRY(workspace(WSB_VALS2, sizeof(float) * (size_t)std::max(max_edges, recs), &d_v2));
+    VB_TRY(workspace(WSB_KEEP, (size_t)n, &d_need));
+    VB_TRY(workspace(WSB_FLAGS, 64, &d_flags));
+    VB_TRY(workspace(WSB_VSEL, sizeof(int32_t) * (size_t)(n + 1), &d_sel));
+    VB_TRY(workspace(WSB_VOLD0, sizeof(int32_t) * (size_t)n * lm0, &d_old0));
+    VB_TRY(workspace(WSB_VOLDUP, sizeof(int32_t) * (size_t)std::max<int64_t>(slots, 1) * m, &d_oldup));
+    VB_TRY(workspace(WSB_VSTAGE0, sizeof(int32_t) * (size_t)b_max * lm0, &d_stage0));
+    VB_TRY(workspace(WSB_VSTAGEUP, sizeof(int32_t) * (size_t)std::max<int64_t>(slots, 1) * m, &d_stageup));
+    {
+        size_t t1 = 0, t2 = 0, t3 = 0;
+        VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
+                                                (int)std::max<int64_t>(max_edges, 1), 0, 57, s));
+        VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t2, (const uint64_t*)d_k2, h.rec_key, (const int32_t*)d_v2, h.rec_val, (int)recs, 0,
+                                                45, s));
+        VB_CUDA(cub::DeviceSelect::Flagged(nullptr, t3, cub::CountingInputIterator<int32_t>(0), (const uint8_t*)d_need, (int32_t*)d_sel,
+                                           (int*)d_flags, (int)n, s));
+        VB_TRY(workspace(WSB_TMP, std::max(t1, std::max(t2, t3)), &d_tmp));
+    }
+    int occ_ins = 1, occ_glob = 1, occ_upd = 1;
+    VB_TRY(K.insert(BuildDev{}, VacDev{}, nullptr, 0, 0, 0, smem_ins, &occ_ins));
+    VB_TRY(K.insert(BuildDev{}, VacDev{}, nullptr, 0, 0, 0, smem_glob, &occ_glob));
+    VB_TRY(K.update(BuildDev{}, VacDev{}, nullptr, nullptr, 0, InsertRec{}, 0, smem_upd, &occ_upd));
+    const int max_grid_ins = c.sm_count * std::max(1, std::max(occ_ins, occ_glob));
+    const int max_grid_upd = c.sm_count * std::max(1, occ_upd) * 4;
+    uint32_t cap = 1u << 14;
+    while (cap < (uint32_t)(efv * m * 16) && cap < (1u << 22)) cap <<= 1;
+    auto reserve_vis = [&](uint32_t vis_cap) -> int {
+        const size_t need = (size_t)max_grid_ins * HN_WARPS * vis_cap * sizeof(uint32_t);
+        if (h.vis_bytes >= need) return VB_OK;
+        if (h.vis) {
+            VB_CUDA(cudaStreamSynchronize(s));
+            cudaFree(h.vis);
+            h.vis = nullptr;
+            h.vis_bytes = 0;
+        }
+        if (cudaMalloc(&h.vis, need) != cudaSuccess) {
+            cudaGetLastError();
+            set_error("hnsw vacuum: visited tables (%zu bytes) do not fit", need);
+            return VB_ENOMEM;
+        }
+        h.vis_bytes = need;
+        return VB_OK;
+    };
+    VB_TRY(reserve_vis(cap + std::max<uint32_t>(2048u, cap / 8)));
+
+    // ---- the image changes from here on
+    ++h.generation;
+    h.n_changes = 0;
+    VB_CUDA(cudaMemcpyAsync(h.n_heaptids, counts, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, s));
+    VB_CUDA(cudaMemcpyAsync(d_old0, h.nbr0, sizeof(int32_t) * (size_t)n * lm0, cudaMemcpyDeviceToDevice, s));
+    if (slots > 0) VB_CUDA(cudaMemcpyAsync(d_oldup, h.upper, sizeof(int32_t) * (size_t)slots * m, cudaMemcpyDeviceToDevice, s));
+
+    BuildDev b{};
+    b.g.rows = h.rows.d;
+    b.g.stride = h.rows.stride;
+    b.g.V = V;
+    b.g.levels = h.levels;
+    b.g.nbr0 = h.nbr0;
+    b.g.upper_off = h.upper_off;
+    b.g.upper = h.upper;
+    b.g.m = m;
+    b.g.n = n;
+    b.nbr0_w = h.nbr0;
+    b.upper_w = h.upper;
+    b.nd0 = h.nd0;
+    b.upper_d = h.upper_d;
+    b.dup_of = h.dup_of;
+    b.n_heaptids = h.n_heaptids;
+    b.efc = efv;
+    b.qvec = qvec;
+    b.n_edges = (int*)d_flags;
+    b.overflow = b.n_edges + 1;
+    b.edge_key = (uint64_t*)d_k1;
+    b.edge_val = (float*)d_v1;
+    VacDev v{};
+    v.stage0 = (int32_t*)d_stage0;
+    v.stage_up = (int32_t*)d_stageup;
+    v.counts = h.n_heaptids;
+    v.wcap = wcap_s;
+    v.wfull = b.n_edges + 2;
+    int* d_nsel = b.n_edges + 3;
+    void* wbuf = nullptr;   // R in global memory, after a repair overflowed the shared one
+    size_t wbuf_bytes = 0;
+    int64_t nrep = 0;
+
+    // NeedsUpdated of the elements [from, n) (skip: the entry point) into d_need
+    auto needs = [&](int64_t from, int skip) -> int {
+        hnsw_needs_update_kernel<<<(unsigned)((n - from + 255) / 256), 256, 0, s>>>(b.g, h.n_heaptids, from, skip, (uint8_t*)d_need);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+        return VB_OK;
+    };
+    // RepairGraphElement of the B elements d_list[0..B) against the graph as it stands, from entry point `ep`
+    auto repair = [&](const int32_t* d_list, int B, int64_t ep) -> int {
+        b.g.entry = (int)ep;
+        b.g.entry_level = ep >= 0 ? levels[(size_t)ep] : -1;
+        b.B = B;
+        v.list = d_list;
+        const int grid_ins = (int)std::min<int64_t>((B + HN_WARPS - 1) / HN_WARPS, max_grid_ins);
+        int flags[3] = {0, 0, 0};
+        for (int attempt = 0;; ++attempt) {
+            const uint32_t vis_upper = std::max<uint32_t>(2048u, cap / 8);
+            const uint32_t vis_cap = cap + vis_upper;
+            VB_TRY(reserve_vis(vis_cap));
+            VB_CUDA(cudaMemsetAsync(d_flags, 0, 3 * sizeof(int), s));
+            VB_TRY(K.insert(b, v, h.vis, vis_cap, vis_upper, grid_ins, v.wk ? smem_glob : smem_ins, nullptr));
+            VB_CUDA(cudaMemcpyAsync(flags, d_flags, 3 * sizeof(int), cudaMemcpyDeviceToHost, s));
+            VB_CUDA(cudaStreamSynchronize(s));
+            if (flags[2]) {
+                // a repair's R overflowed: repeat the batch's searches with R in global memory, four times as large (nothing
+                // was published)
+                VB_REQUIRE(v.wcap < 65535, "hnsw vacuum: a repair keeps more than 65535 candidates");
+                v.wcap = (int)std::min<int64_t>(65535, (int64_t)v.wcap * 4);
+                const size_t per = (size_t)v.wcap * (2 * 8 + 2 * 4 + 2 + 1);
+                const size_t need = per * (size_t)max_grid_ins * HN_WARPS;
+                if (wbuf_bytes < need) {
+                    if (wbuf) {
+                        VB_CUDA(cudaStreamSynchronize(s));
+                        cudaFree(wbuf);
+                        wbuf = nullptr;
+                        wbuf_bytes = 0;
+                    }
+                    if (cudaMalloc(&wbuf, need) != cudaSuccess) {
+                        cudaGetLastError();
+                        set_error("hnsw vacuum: candidate buffers (%zu bytes) do not fit", need);
+                        return VB_ENOMEM;
+                    }
+                    wbuf_bytes = need;
+                }
+                const size_t nw = (size_t)max_grid_ins * HN_WARPS * v.wcap;
+                v.wk = (uint64_t*)wbuf;
+                v.wi = (uint32_t*)(v.wk + 2 * nw);
+                v.wd = (uint16_t*)(v.wi + 2 * nw);
+                v.dead = (uint8_t*)(v.wd + nw);
+                continue;
+            }
+            if (!flags[1]) break;
+            cap <<= 2;   // a visited table overflowed: repeat the batch's searches with larger ones (nothing was published)
+            VB_REQUIRE(attempt < 8 && cap <= (1u << 26), "hnsw vacuum: visited set overflow");
+        }
+        hnsw_vacuum_edges_kernel<<<(unsigned)std::min<int64_t>(((int64_t)B * 32 + 127) / 128, (int64_t)c.sm_count * 16), 128, 0, s>>>(b, v);
+        VB_CUDA(cudaGetLastError());
+        hnsw_vacuum_publish_kernel<<<(unsigned)B, 64, 0, s>>>(b, v);
+        VB_CUDA(cudaGetLastError());
+        count_launch(2);
+        int n_edges = 0;
+        VB_CUDA(cudaMemcpyAsync(&n_edges, b.n_edges, sizeof(int), cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaStreamSynchronize(s));
+        VB_REQUIRE(n_edges <= max_edges, "hnsw vacuum: record overflow (%d > %lld)", n_edges, (long long)max_edges);
+        if (n_edges > 0) {
+            size_t tb = 0;
+            VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
+                                                    n_edges, 0, 57, s));
+            VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+            VB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
+                                                    n_edges, 0, 57, s));
+            count_launch();
+            const int grid_upd = (int)std::min<int64_t>(((int64_t)n_edges + HN_WARPS - 1) / HN_WARPS, max_grid_upd);
+            VB_TRY(K.update(b, v, (const uint64_t*)d_k2, (const float*)d_v2, n_edges, InsertRec{}, grid_upd, smem_upd, nullptr));
+        }
+        nrep += B;
+        return VB_OK;
+    };
+    auto repair_one = [&](int64_t e, int64_t ep) -> int {
+        const int32_t e32 = (int32_t)e;
+        VB_CUDA(cudaMemcpyAsync(d_sel, &e32, sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        return repair((const int32_t*)d_sel, 1, ep);
+    };
+    auto needs_one = [&](int64_t e, bool* out) -> int {
+        VB_TRY(needs(e, -1));
+        uint8_t f = 0;
+        VB_CUDA(cudaMemcpyAsync(&f, d_need, 1, cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaStreamSynchronize(s));
+        *out = f != 0;
+        return VB_OK;
+    };
+    int rc = VB_OK;
+    auto run = [&]() -> int {
+        // RemoveHeapTids' highest and fallback points (src/hnswvacuum.c:133-157): live, the first of a strictly higher level
+        int64_t highest = -1, fallback = -1;
+        int hl = -1, fl = -1;
+        for (int64_t i = 0; i < n; ++i) {
+            if (counts[i] == 0) continue;
+            const int lv = levels[(size_t)i];
+            if (lv > hl) {
+                fallback = highest;
+                fl = hl;
+                highest = i;
+                hl = lv;
+            } else if (lv > fl) {
+                fallback = i;
+                fl = lv;
+            }
+        }
+        // RepairGraphEntryPoint (:279-373)
+        if (highest >= 0) {
+            if (highest == h.entry) highest = fallback;
+            bool need = false;
+            if (highest >= 0) VB_TRY(needs_one(highest, &need));
+            if (need) VB_TRY(repair_one(highest, h.entry));
+        }
+        if (h.entry >= 0) {
+            if (counts[h.entry] == 0) {
+                h.entry = highest;
+                h.entry_level = highest >= 0 ? levels[(size_t)highest] : -1;
+            } else {
+                bool need = false;
+                VB_TRY(needs_one(h.entry, &need));
+                if (need) VB_TRY(repair_one(h.entry, highest));
+            }
+        }
+        // the entry point is the highest live element, so RepairGraph never moves it (:461-482)
+        VB_REQUIRE(h.entry < 0 ? live == 0 : (counts[h.entry] != 0 && h.entry_level == hl),
+                   "hnsw vacuum: the entry point (%lld, level %d) is not the highest live element (level %d)", (long long)h.entry,
+                   h.entry_level, hl);
+        // RepairGraph (:378-502): batches of the candidates in element order, NeedsUpdated at each batch's start
+        int64_t from = 0;
+        while (h.entry >= 0 && from < n) {
+            VB_TRY(needs(from, (int)h.entry));
+            size_t tb = 0;
+            VB_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, cub::CountingInputIterator<int32_t>((int32_t)from), (const uint8_t*)d_need,
+                                               (int32_t*)d_sel, d_nsel, (int)(n - from), s));
+            VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+            VB_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, cub::CountingInputIterator<int32_t>((int32_t)from), (const uint8_t*)d_need,
+                                               (int32_t*)d_sel, d_nsel, (int)(n - from), s));
+            count_launch();
+            int nsel = 0;
+            VB_CUDA(cudaMemcpyAsync(&nsel, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, s));
+            VB_CUDA(cudaStreamSynchronize(s));
+            if (nsel == 0) break;
+            const int B = (int)std::min<int64_t>(nsel, b_max);
+            int32_t last = 0;
+            VB_CUDA(cudaMemcpyAsync(&last, (const int32_t*)d_sel + (B - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+            VB_TRY(repair((const int32_t*)d_sel, B, h.entry));
+            from = B < nsel ? (int64_t)last + 1 : n;
+        }
+        // MarkDeleted (:594-729)
+        hnsw_mark_deleted_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(b, h.n_heaptids);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+        // change records: the slots that differ from the snapshot, sorted by (element, layer, slot)
+        const InsertRec rec{(uint64_t*)d_k2, (int32_t*)d_v2, d_nsel};
+        VB_CUDA(cudaMemsetAsync(d_nsel, 0, sizeof(int), s));
+        hnsw_slot_diff_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(b.g, (const int32_t*)d_old0, (const int32_t*)d_oldup, rec);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+        int n_rec = 0;
+        VB_CUDA(cudaMemcpyAsync(&n_rec, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaStreamSynchronize(s));
+        if (n_rec > 0) {
+            size_t tb = 0;
+            VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)d_k2, h.rec_key, (const int32_t*)d_v2, h.rec_val, n_rec, 0, 45,
+                                                    s));
+            VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+            VB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)d_k2, h.rec_key, (const int32_t*)d_v2, h.rec_val, n_rec, 0, 45,
+                                                    s));
+            count_launch();
+        }
+        VB_CUDA(cudaStreamSynchronize(s));
+        h.n_changes = n_rec;
+        if (out_nchanges) *out_nchanges = n_rec;
+        if (out_nrepaired) *out_nrepaired = nrep;
+        return VB_OK;
+    };
+    rc = run();
+    if (wbuf) {
+        cudaStreamSynchronize(s);
+        cudaFree(wbuf);
+    }
+    return rc;
 }
 
 }  // namespace vb
@@ -1260,6 +1760,12 @@ int vb_hnsw_insert_changes(vb_hnsw* p, vb_hnsw_slot* out, int64_t cap) {
         out[i].neighbor = v[(size_t)i];
     }
     return VB_OK;
+}
+
+int vb_hnsw_vacuum(vb_hnsw* p, const int32_t* counts, int ef_construction, int64_t* out_nrepaired, int64_t* out_nchanges) {
+    VB_TRY(require_init());
+    VB_REQUIRE(p, "null index");
+    return hnsw_vacuum_impl(p->h, counts, ef_construction, out_nrepaired, out_nchanges);
 }
 
 int vb_hnsw_set_heaptid_counts(vb_hnsw* p, const int32_t* counts) {
