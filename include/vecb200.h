@@ -19,12 +19,13 @@
  *   - "host" pointers are ordinary process memory; "_dev" variants take device
  *     pointers valid on the library's current device.  Work is enqueued on the
  *     library stream (vb_stream()); host-buffer variants synchronise before
- *     returning.  _dev variants return with their work enqueued, with two stated
+ *     returning.  _dev variants return with their work enqueued, with three stated
  *     exceptions: the batched vb_ivf_search*_dev read ONE 8-byte pair of certificate
  *     counters per sub-batch of queries, with up to 64 numbers of the queries filter
  *     level 0 could not certify (the tensor-core filter re-runs uncertified queries
- *     before the results may be used; a re-run synchronises again), and
- *     vb_hnsw_search_dev reads one overflow flag per call (visited-table growth).
+ *     before the results may be used; a re-run synchronises again),
+ *     vb_hnsw_search_dev reads one overflow flag per call (visited-table growth), and
+ *     vb_table_aggregate_dev reads sum's 4-byte overflow flag (float_overflow_error).
  *   - rows are row-major and contiguous in the caller's buffers (vector: dim
  *     fp32; halfvec: dim IEEE binary16; bit: (dim+7)/8 bytes, MSB first, tail
  *     bits zero -- exactly the payload of Vector.x (src/vector.h:18-24),
@@ -222,6 +223,55 @@ int			vb_exact_topk_filtered(vb_table *t, int metric, const void *queries, int64
 int			vb_exact_topk_filtered_dev(vb_table *t, int metric, const void *queries_dev, int64_t nq, int k,
 									   const vb_filter *const *filters, int nfilters, const int32_t *filter_of_query,
 									   int64_t *out_ids_dev, float *out_dist_dev);
+
+/* -------------------------------------------------------------- aggregates */
+
+/*
+ * avg(vector), sum(vector), avg(halfvec), sum(halfvec) (sql/vector.sql:163-198, 607-642) over the rows of a table, with
+ * GROUP BY: "SELECT avg(v) FROM t" and "SELECT g, avg(v) FROM t GROUP BY g".  t holds VB_VECTOR or VB_HALFVEC rows
+ * (VB_BIT: VB_EINVAL, the reference has no bit aggregates).
+ *
+ * group_of_row [n] puts row i in group group_of_row[i] in [0, ngroups), or leaves it out with -1 (a WHERE that rejects
+ * it, or a NULL value); NULL puts every row in group 0 and requires ngroups == 1.
+ *
+ * The plan.  For each group g, S_g = its rows in ascending row number, cut into runs of R = run_rows consecutive rows
+ * (the last may be short; R = 0 or R >= |S_g| is one run, the serial plan):
+ *   run state    the transition function over the run's rows in order from the initial condition.  avg, INITCOND '{0}':
+ *                the first row sets n = 1, s_i = (double) x_i (vector_accum's new-array branch, so a -0 survives), each
+ *                later row adds (double) x_i in float8 (src/vector.c:1148-1204; halfvec widens by HalfToFloat4,
+ *                src/halfvec.c:1104-1160).  sum, strict with no initcond: the first row is the state, each later row is
+ *                added by vector_add (fp32 add, src/vector.c:824-852) or halfvec_add (add, round to fp16,
+ *                src/halfvec.c:764-798);
+ *   group state  the run states combined left to right, combine(combine(r0, r1), r2) ...: avg by vector_combine (sums and
+ *                counts added, src/vector.c:1209-1284), sum by the transition's add;
+ *   final        avg: (float) (s_i / n) (src/vector.c:1289-1318), Float4ToHalf of that for halfvec (src/halfvec.c:1165-1194);
+ *                sum: the state.  A group with no rows has count 0 (the SQL NULL) and a zero-filled result.
+ * R = 0 without groups is PostgreSQL's serial "SELECT avg(v) FROM t" in table order; R = ceil(n / W) is a Partial
+ * Aggregate of W participants taking contiguous ranges.  Results depend on R only through rounding, as the reference's
+ * depend on its plan; for a given R they are deterministic and independent of the launch configuration.
+ *
+ * Outputs: out [ngroups x dim] (fp32 for vector, IEEE binary16 for halfvec), out_counts [ngroups], and for avg optionally
+ * out_state [ngroups x (dim + 1)] = n, s_1 .. s_dim: the float8 transition state vector_accum / vector_combine hold, which
+ * a Partial Aggregate hands to the Finalize Aggregate (so a caller can combine it with partial states computed
+ * elsewhere).  sum's state is out itself: sum requires out_state == NULL.
+ *
+ * Errors.  sum: a transition or combine step that produces an infinite element fails with VB_EINVAL and
+ * float_overflow_error()'s text, "value out of range: overflow"; which steps exist depends on R, so whether a call fails
+ * does too (the host variant then writes nothing).  avg: the float8 state cannot overflow for finite rows; what a
+ * non-finite row gives is unspecified.  Validation before any kernel runs: an unknown agg, ngroups < 1, run_rows < 0, a
+ * NULL group_of_row with ngroups != 1, or (host variant) a group id outside [-1, ngroups), which names the row and the
+ * value, fail with VB_EINVAL; the _dev variant counts such ids as -1.  Grouped calls take tables of at most 2^31 - 1
+ * rows.  VB_ENOMEM names the bytes needed (row list and sort space, run states, staged results) and allocates nothing.
+ * An empty table gives every count 0.
+ * _dev variant: group_of_row and the outputs on the device; asynchronous on vb_stream() except for one 4-byte read of
+ * sum's overflow flag.
+ */
+#define VB_AGG_AVG 0
+#define VB_AGG_SUM 1
+int			vb_table_aggregate(vb_table *t, int agg, const int32_t *group_of_row, int ngroups, int64_t run_rows,
+							   void *out, int64_t *out_counts, double *out_state);
+int			vb_table_aggregate_dev(vb_table *t, int agg, const int32_t *group_of_row_dev, int ngroups, int64_t run_rows,
+								   void *out_dev, int64_t *out_counts_dev, double *out_state_dev);
 
 /* ---------------------------------------------------------------- sparsevec */
 

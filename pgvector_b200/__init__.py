@@ -182,6 +182,16 @@ def jaccard_distance(a, rows, dim=None, **kw):
 
 # --------------------------------------------------------------------- resident table / exact scan
 
+AGG_AVG, AGG_SUM = 0, 1
+# Rows per run of Table.avg / Table.sum.  The run kernel has one thread per (run, 128-byte column span of a row), so the
+# runs of a table are its parallelism: at 1024 rows, 1M x 1536 fp32 rows are 977 runs x 1536 threads and 2M x 768
+# halfvec rows 1954 runs x 384 threads, several waves of a full H100 each, every thread with the next 8 rows' loads in
+# flight during its adds (2.3 TB/s for the fp32 shape on an H100 80GB HBM3 at 700 W, DESIGN.md section 5).  Shorter
+# runs add run states to write and combine (one float8 per column per run, under 1 % of the rows' bytes here); the
+# combine walks a group's runs serially, which stays short next to the row stream at this length.
+DEFAULT_RUN_ROWS = 1024
+
+
 class Table:
     """[n x dim] rows resident in HBM."""
 
@@ -301,6 +311,53 @@ class Table:
         _lib.check(load().vb_table_rerank(self.h, metric, _ptr(queries), nq, _ptr(candidates), candidates.shape[1], k,
                                           _ptr(ids), _ptr(dist)))
         return ids, dist
+
+    def avg(self, groups=None, ngroups=None, run_rows=DEFAULT_RUN_ROWS, state=False):
+        """avg(v) of the rows, "GROUP BY" groups[i] (-1 = row left out; None = every row in one group): returns
+        (values [G, dim] float32 / float16, counts [G]), plus the float8 transition state [G, dim + 1] = n, s_1 .. s_dim
+        when state=True.  Each group's rows are aggregated in runs of run_rows consecutive rows whose states are combined
+        left to right (0 = one run: the serial plan); the rounding depends on it as the reference's depends on its plan.
+        numpy groups (or None) run the host variant and return numpy arrays; a torch CUDA int32 tensor runs the _dev
+        variant and returns CUDA tensors.  A group with count 0 is the SQL NULL (its values are zero-filled)."""
+        return self._aggregate(AGG_AVG, groups, ngroups, run_rows, state)
+
+    def sum(self, groups=None, ngroups=None, run_rows=DEFAULT_RUN_ROWS):
+        """sum(v) of the rows, as avg() groups and splits them: returns (values [G, dim], counts [G]).  An infinite
+        element raises VecB200Error ("value out of range: overflow"), as float_overflow_error() does."""
+        return self._aggregate(AGG_SUM, groups, ngroups, run_rows, False)
+
+    def _aggregate(self, agg, groups, ngroups, run_rows, state):
+        if self.elem not in (VECTOR, HALFVEC):
+            raise ValueError(f"{_TYPE_NAME[self.elem]} has no aggregates")
+        run_rows = int(run_rows)
+        if groups is None:
+            ngroups = 1 if ngroups is None else int(ngroups)
+        elif ngroups is None:
+            ngroups = max(1, int(groups.max()) + 1) if len(groups) else 1
+        ngroups = int(ngroups)
+        dim = self.dim
+        if _is_torch(groups):
+            import torch
+            if not groups.is_cuda or groups.dtype != torch.int32 or groups.dim() != 1:
+                raise TypeError("groups must be a 1-d int32 CUDA tensor or a host array")
+            groups = groups.contiguous()
+            dev = groups.device
+            vals = torch.empty((ngroups, dim), dtype=torch.float32 if self.elem == VECTOR else torch.float16, device=dev)
+            counts = torch.empty(ngroups, dtype=torch.int64, device=dev)
+            st = torch.empty((ngroups, dim + 1), dtype=torch.float64, device=dev) if state else None
+            _after_torch(groups)
+            _lib.check(load().vb_table_aggregate_dev(self.h, agg, _ptr(groups), ngroups, run_rows, _ptr(vals), _ptr(counts), _ptr(st)))
+            synchronize()   # the library runs on its own stream; results are handed back complete
+        else:
+            if groups is not None:
+                groups = np.ascontiguousarray(groups, dtype=np.int32)
+                if groups.shape != (len(self),):
+                    raise ValueError(f"groups must have one entry per row ({len(self)}), got shape {groups.shape}")
+            vals = np.empty((ngroups, dim), dtype=np.float32 if self.elem == VECTOR else np.float16)
+            counts = np.empty(ngroups, dtype=np.int64)
+            st = np.empty((ngroups, dim + 1), dtype=np.float64) if state else None
+            _lib.check(load().vb_table_aggregate(self.h, agg, _ptr(groups), ngroups, run_rows, _ptr(vals), _ptr(counts), _ptr(st)))
+        return (vals, counts, st) if state else (vals, counts)
 
     def exact_topk_sharded(self, metric, queries_dev, k, id_offset):
         """exact top-k over a row-sharded table (collective over the library's communicator); torch CUDA tensors"""

@@ -62,6 +62,8 @@ SIGNATURES = {
     "vb_filter_free": (_i, [_vp]),
     "vb_exact_topk_filtered": (_i, [_vp, _i, _vp, _i64, _i, _vp, _i, _vp, _vp, _vp]),
     "vb_exact_topk_filtered_dev": (_i, [_vp, _i, _vp, _i64, _i, _vp, _i, _vp, _vp, _vp]),
+    "vb_table_aggregate": (_i, [_vp, _i, _vp, _i, _i64, _vp, _vp, _vp]),
+    "vb_table_aggregate_dev": (_i, [_vp, _i, _vp, _i, _i64, _vp, _vp, _vp]),
     "vb_ivf_create": (_i, [_i, _i, _i, _i, C.POINTER(_vp)]),
     "vb_ivf_load": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "vb_ivf_load_dev": (_i, [_vp, _vp, _vp, _vp, _vp]),
