@@ -102,6 +102,7 @@ int			vb_stream_wait_event(void *cuda_event);
 #define VB_PROF_HNSW 4
 #define VB_PROF_LIST_TC 5		/* list_tc_kernel alone (the tensor-core filter pass over the probed lists) */
 #define VB_PROF_CENTRE_TC 6		/* the same kernel over the centre table (probe selection of query batches) */
+#define VB_PROF_FILTER_MASK 7	/* the row-filter mask of vb_ivf_search_filtered over the candidate distances */
 int			vb_prof_enable(int on);
 /* Synchronises, then returns accumulated milliseconds and bracketed launches since the last read of `kernel`. */
 int			vb_prof_read(int kernel, double *total_ms, int64_t *launches);
@@ -405,6 +406,39 @@ int			vb_ivf_search(vb_ivf *ix, const void *queries, int64_t nq, int probes, int
 /* Same with device-resident queries and outputs (float distances), asynchronous on vb_stream(). */
 int			vb_ivf_search_dev(vb_ivf *ix, const void *queries_dev, int64_t nq, int probes, int k,
 							  int64_t *out_ids_dev, float *out_dist_dev);
+/*
+ * vb_ivf_search with a row filter per query (see vb_filter above): the plan of WHERE <predicate> ORDER BY v <op> q
+ * LIMIT k with ivfflat.iterative_scan = off, for a batch of queries.
+ *
+ * Result.  Query q uses filters[filter_of_query[q]]; filter_of_query is a host array in both variants, NULL when
+ * nfilters == 1.  For each query the result is the first k rows of vb_ivf_search's order over its probed lists (by
+ * (distance, scan position); the lists are those of vb_ivf_scan_lists(q, probes)) restricted to the ids its filter
+ * allows, padded with -1 / +inf when fewer than k allowed rows lie in the probed lists (where the reference returns
+ * fewer rows).  An allowed row whose distance is +inf or NaN is a result, in that order's place; a rejected row never is.
+ *
+ * Bit identity.  An allowed row gets bit for bit the distance vb_ivf_search computes for it on the same path, so with a
+ * filter that allows every row the output equals vb_ivf_search's, ids and distances, under every scan_impl, tc_level1
+ * and tc_level0.  The filtered call never takes the fused one-query kernels: for calls of at most 16 queries, the
+ * comparison is with vb_ivf_search under option one_query = 0.
+ *
+ * Reads.  Unlike the other filtered calls this one reads rejected rows: the probed lists are read whole, once per batch,
+ * because the queries of a batch share them, and each query's candidate distances are masked (VB_PROF_FILTER_MASK)
+ * before anything selects from them.  Rejected rows are never selected, re-scored or returned.  For very selective
+ * filters, vb_exact_topk_filtered (the exact scan of the allowed rows) or the filtered iterative scan
+ * (vb_ivf_scan_begin_filtered), which read the allowed rows only, move fewer bytes.
+ *
+ * Errors.  An index that is not loaded: VB_ESTATE.  A filter of another table, index or image, also after its owner was
+ * freed: VB_EINVAL.  A filter made before a load, vb_ivf_replace_list, vb_ivf_insert or vb_ivf_delete: VB_ESTATE ("index
+ * changed since the filter was created").  A filter_of_query entry out of range: VB_EINVAL naming the query.  k and
+ * probes have the limits of vb_ivf_search; VB_ENOMEM names the bytes.  The host variant writes nothing on any error.
+ * Images of the list-sharded search are not supported.  The filters may be freed once the call returns.
+ */
+int			vb_ivf_search_filtered(vb_ivf *ix, const void *queries, int64_t nq, int probes, int k,
+								   const vb_filter *const *filters, int nfilters, const int32_t *filter_of_query,
+								   int64_t *out_ids, double *out_dist);
+int			vb_ivf_search_filtered_dev(vb_ivf *ix, const void *queries_dev, int64_t nq, int probes, int k,
+									   const vb_filter *const *filters, int nfilters, const int32_t *filter_of_query,
+									   int64_t *out_ids_dev, float *out_dist_dev);
 /*
  * Pipelined host path.  vb_ivf_prefetch_queries starts the host->device copy of the NEXT batch of queries on a second
  * stream (slot 0 or 1; `queries` should be page-locked and must stay valid until the matching search returns) and

@@ -529,9 +529,14 @@ class IvfflatIndex:
         _lib.check(load().vb_ivf_scan_items(self.h, _ptr(qh), _ptr(lists), len(lists), cap, _ptr(ids), _ptr(dist), C.byref(n)))
         return ids[:cap], dist[:cap], int(n.value)
 
-    def search(self, queries, k, probes=None):
-        """first batch of ivfflatgettuple for many queries: k nearest of the probed lists."""
+    def search(self, queries, k, probes=None, filter=None, filter_of_query=None):
+        """first batch of ivfflatgettuple for many queries: k nearest of the probed lists.  filter: a Filter of this index,
+        or a list of them with filter_of_query[q] = the index of query q's filter: each query then gets the first k of
+        its unfiltered order over the probed lists that its filter allows (-1 / +inf padded), WHERE ... ORDER BY ... LIMIT k
+        with ivfflat.iterative_scan = off."""
         p = int(probes or self.probes)
+        if filter is not None:
+            return self._search_filtered(queries, int(k), p, filter, filter_of_query)
         if _is_torch(queries):
             import torch
             nq = queries.shape[0]
@@ -548,6 +553,31 @@ class IvfflatIndex:
         ids = np.empty((nq, k), dtype=np.int64)
         dist = np.empty((nq, k), dtype=np.float64)
         _lib.check(load().vb_ivf_search(self.h, _ptr(q), nq, p, k, _ptr(ids), _ptr(dist)))
+        return ids, dist
+
+    def _search_filtered(self, queries, k, p, filter, filter_of_query):
+        farr, nf, fq = _filter_args(filter, filter_of_query)
+        if _is_torch(queries):
+            import torch
+            nq = queries.shape[0]
+            if fq is not None and len(fq) != nq:
+                raise ValueError(f"filter_of_query must have {nq} entries, got {len(fq)}")
+            queries = queries.contiguous()
+            ids = torch.empty((nq, k), dtype=torch.int64, device=queries.device)
+            dist = torch.empty((nq, k), dtype=torch.float32, device=queries.device)
+            _after_torch(queries)
+            _lib.check(load().vb_ivf_search_filtered_dev(self.h, _ptr(queries), nq, p, k, farr, nf, _ptr(fq), _ptr(ids), _ptr(dist)))
+            synchronize()   # the library runs on its own stream; results are handed back complete
+            return ids, dist
+        q = _host(self.elem, queries)
+        if q.ndim == 1:
+            q = q.reshape(1, -1)
+        nq = q.shape[0]
+        if fq is not None and len(fq) != nq:
+            raise ValueError(f"filter_of_query must have {nq} entries, got {len(fq)}")
+        ids = np.empty((nq, k), dtype=np.int64)
+        dist = np.empty((nq, k), dtype=np.float64)
+        _lib.check(load().vb_ivf_search_filtered(self.h, _ptr(q), nq, p, k, farr, nf, _ptr(fq), _ptr(ids), _ptr(dist)))
         return ids, dist
 
     def filter(self, ids):

@@ -81,6 +81,8 @@ SIGNATURES = {
     "vb_ivf_scan_items": (_i, [_vp, _vp, _vp, _i, _i64, _vp, _vp, _vp]),
     "vb_ivf_search": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
     "vb_ivf_search_dev": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
+    "vb_ivf_search_filtered": (_i, [_vp, _vp, _i64, _i, _i, _vp, _i, _vp, _vp, _vp]),
+    "vb_ivf_search_filtered_dev": (_i, [_vp, _vp, _i64, _i, _i, _vp, _i, _vp, _vp, _vp]),
     "vb_ivf_scan_begin": (_i, [_vp, _vp, _i64, _i, _i, _i, C.POINTER(_vp)]),
     "vb_ivf_scan_begin_filtered": (_i, [_vp, _vp, _i64, _i, _i, _i, _vp, _i, _vp, C.POINTER(_vp)]),
     "vb_ivf_scan_next": (_i, [_vp, _vp, _vp, _vp]),

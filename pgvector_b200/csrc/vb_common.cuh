@@ -256,11 +256,13 @@ int list_tc_level0_rescored(int64_t* out3);
 // run dist[q * cap ..) of seg_len[q] <= CR_RUN_MAX entries.  The number of uncertified queries is ADDED to *fail_dev
 // (level 0: and they are listed in fail_list).
 constexpr int CR_RUN_MAX = 4096;
+// has_nan (vb_ivf_search_filtered): the runs were masked (FILTER_REJECTED marks rejected entries): marked candidates are
+// not candidates, and a query with an allowed NaN d~ (has_nan[q]) counts as uncertified.
 int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                               int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
                               const float* dist, const float* smin, const int32_t* pre_pos, const float* pre_key, int64_t cap,
                               int64_t cap_s, const int32_t* seg_len, const float* qn, int32_t* out_pos, float* out_key, int* fail_dev,
-                              int level = 2, int32_t* fail_list = nullptr);
+                              int level = 2, int32_t* fail_list = nullptr, const int32_t* has_nan = nullptr);
 // vb_ivf_one.cu: the scan of one query (or a handful) as two fused distance + select kernels
 bool one_probe_fits(int lists, size_t qstride, int probes);
 bool one_scan_fits(int64_t cap, size_t qstride, int probes, int64_t k);
@@ -310,6 +312,11 @@ int filter_build_ivf(int64_t n_rows, const int64_t* image_ids, const int64_t* li
 // validates before this call)
 int filter_build_hnsw(int64_t n_elems, const int64_t* elems, int64_t n, bool host, Filter* f);
 void filter_release(Filter* f);
+// The batched filtered IVFFlat search (vb_ivf_search_filtered) masks each query's run of candidate distances: a rejected
+// entry holds these bits, a negative NaN.  orderable_key() sorts every NaN after +inf, so a rejected entry is never
+// selected ahead of an allowed one; the bits tell it apart from an allowed row's NaN distance (the GPU computes NaN as
+// 0x7FFFFFFF, and the mask rewrites an allowed NaN that carries these bits to that).
+constexpr uint32_t FILTER_REJECTED = 0xFFFFFFFFu;
 
 int list_tile_rows();
 bool list_major_supported(int elem, int key_metric);

@@ -170,6 +170,153 @@ __global__ void ivf_finish_kernel(int metric, int64_t nq, int k, int probes, con
     if (out_d) out_d[i] = v;
 }
 
+// ----------------------------------------------------------------------------- row filters of the batched search
+//
+// vb_ivf_search_filtered scans the probed lists whole, as vb_ivf_search does, and masks each query's run of candidate
+// distances before anything selects from it: ivf_mask_kernel rewrites every entry whose row the query's filter rejects
+// to FILTER_REJECTED and recomputes the slab minima over the allowed entries.  Every selection then sees the allowed
+// entries first, in their unfiltered order; ivf_unmask_kernel turns a rejected entry that reached the top k into -1 / +inf.
+
+struct MaskFilter {        // one row filter as the mask reads it (vb_filter.cu): sorted image rows, per-list runs
+    const int64_t* pos;
+    const int64_t* off;
+};
+struct IvfMask {           // the device arguments of one sub-batch
+    const MaskFilter* filters;   // [nfilters]
+    const int32_t* fq;           // [nq] filter of each query (nullptr: filters[0] for all)
+    int32_t* has_nan;            // [nq] set when an allowed entry of the query's run is NaN
+};
+
+// One CTA per (query, probe) pair, one warp per 32-row slab of the list at a time: the slab's allowed rows are the
+// filter's positions from a binary search for the slab's first row on (at most 32 of them, one per lane).
+__global__ void __launch_bounds__(256) ivf_mask_kernel(IvfMask mk, int probes, const int32_t* __restrict__ probe_lists,
+                                                       const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
+                                                       int64_t cap, float* __restrict__ dist, float* __restrict__ smin, int64_t cap_s) {
+    const int64_t q = blockIdx.x / probes;
+    const int p = (int)(blockIdx.x % probes);
+    const int l = probe_lists[q * probes + p];
+    if (l < 0) return;
+    const int64_t lo = list_off[l], hi = list_off[l + 1];
+    if (hi <= lo) return;
+    const MaskFilter f = mk.filters[mk.fq ? mk.fq[q] : 0];
+    const int64_t a0 = f.off[l], a1 = f.off[l + 1];
+    const int32_t co = cand_off[q * (probes + 1) + p];
+    float* dq = dist + q * cap + co - lo;   // dq[r]: row r of the list-ordered table
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t s0 = lo >> 5, ns = ((hi - 1) >> 5) - s0 + 1;
+    bool nan_seen = false;
+    for (int64_t s = warp; s < ns; s += 8) {
+        const int64_t r0 = (s0 + s) << 5;
+        int64_t j = a0;
+        if (lane == 0) {
+            int64_t b = a1;   // first allowed position >= r0
+            while (j < b) {
+                const int64_t mid = (j + b) >> 1;
+                if (f.pos[mid] < r0) j = mid + 1;
+                else b = mid;
+            }
+        }
+        j = __shfl_sync(0xffffffffu, j, 0);
+        const int64_t pr = j + lane < a1 ? f.pos[j + lane] : INT64_MAX;
+        const unsigned allowed = __reduce_or_sync(0xffffffffu, pr < r0 + 32 ? 1u << (unsigned)(pr - r0) : 0u);
+        const int64_t r = r0 + lane;
+        uint32_t key = 0xFFFFFFFFu;
+        if (r >= lo && r < hi) {
+            float d = __uint_as_float(FILTER_REJECTED);
+            if ((allowed >> lane) & 1u) {
+                d = dq[r];
+                if (d != d) {
+                    nan_seen = true;
+                    d = __uint_as_float(0x7FFFFFFFu);
+                }
+            }
+            dq[r] = d;
+            key = orderable_key(d);
+        }
+        key = __reduce_min_sync(0xffffffffu, key);
+        if (smin != nullptr && lane == 0) smin[slab_base(q, cap_s, co, p) + s] = key == 0xFFFFFFFFu ? __uint_as_float(FILTER_REJECTED) : key_to_float(key);
+    }
+    if (nan_seen) mk.has_nan[q] = 1;
+}
+
+// After ivf_finish_kernel on a masked run.  One warp per query.  Without an allowed NaN, rejected entries sort after every
+// allowed one: a selected rejected entry becomes -1 / +inf.  With one, rejected and allowed NaN entries share the key of
+// NaN and are ordered by position, so the NaN tail of the result (slot f on) is rebuilt: the allowed NaN entries of the
+// run in scan order, then -1 / +inf.
+__global__ void ivf_unmask_kernel(int metric, int64_t nq, int k, int probes, const int32_t* __restrict__ pos, const float* __restrict__ key,
+                                  const float* __restrict__ dist, int64_t cap, const int32_t* __restrict__ has_nan,
+                                  const int32_t* __restrict__ probe_lists, const int32_t* __restrict__ cand_off,
+                                  const int64_t* __restrict__ list_off, const int64_t* __restrict__ ids, int64_t* __restrict__ out_ids,
+                                  float* __restrict__ out_f, double* __restrict__ out_d) {
+    const int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (q >= nq) return;   // whole warps
+    const float* dq = dist + q * cap;
+    const double pad = finish_value(metric, __int_as_float(0x7F800000));
+    auto clear = [&](int64_t i) {
+        out_ids[i] = -1;
+        if (out_f) out_f[i] = (float)pad;
+        if (out_d) out_d[i] = pad;
+    };
+    if (has_nan[q] == 0) {
+        for (int i = lane; i < k; i += 32) {
+            const int32_t ps = pos[q * k + i];
+            if (ps >= 0 && __float_as_uint(dq[ps]) == FILTER_REJECTED) clear(q * k + i);
+        }
+        return;
+    }
+    int f = k;   // the first slot holding padding or a NaN key
+    for (int i0 = 0; i0 < k && f == k; i0 += 32) {
+        const int i = i0 + lane;
+        const unsigned b = __ballot_sync(0xffffffffu, i < k && (pos[q * k + i] < 0 || key[q * k + i] != key[q * k + i]));
+        if (b) f = i0 + __ffs(b) - 1;
+    }
+    const int32_t* co = cand_off + q * (probes + 1);
+    const double vnan = finish_value(metric, __int_as_float(0x7FC00000));
+    for (int p = 0; p < probes && f < k; ++p) {
+        const int l = probe_lists[q * probes + p];
+        if (l < 0) continue;
+        const int64_t lo = list_off[l];
+        for (int32_t c = co[p]; c < co[p + 1] && f < k; c += 32) {
+            const int32_t ps = c + lane;
+            const float d = ps < co[p + 1] ? dq[ps] : 0.f;
+            const bool take = d != d && __float_as_uint(d) != FILTER_REJECTED;
+            const unsigned b = __ballot_sync(0xffffffffu, take);
+            const int slot = f + __popc(b & ((1u << lane) - 1u));
+            if (take && slot < k) {
+                const int64_t row = lo + (ps - co[p]);
+                out_ids[q * k + slot] = ids ? ids[row] : row;
+                if (out_f) out_f[q * k + slot] = (float)vnan;
+                if (out_d) out_d[q * k + slot] = vnan;
+            }
+            f += __popc(b);
+        }
+    }
+    for (int i = f + lane; i < k; i += 32) clear(q * k + i);
+}
+
+static int ivf_mask_runs(const IvfMask& mk, int64_t nq, const int32_t* d_lists, int probes, const int32_t* cand_off, const int64_t* list_off,
+                         int64_t cap, float* dist, float* smin, int64_t cap_s) {
+    Context& c = ctx();
+    prof_begin(VB_PROF_FILTER_MASK);
+    VB_CUDA(cudaMemsetAsync(mk.has_nan, 0, sizeof(int32_t) * (size_t)nq, c.stream));
+    ivf_mask_kernel<<<(unsigned)(nq * probes), 256, 0, c.stream>>>(mk, probes, d_lists, cand_off, list_off, cap, dist, smin, cap_s);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    prof_end(VB_PROF_FILTER_MASK);
+    return VB_OK;
+}
+
+static int ivf_unmask(const Ivf& ix, const IvfMask& mk, int64_t nq, int k, int probes, const int32_t* pos, const float* key, const float* dist,
+                      int64_t cap, const int32_t* d_lists, const int32_t* cand_off, int64_t* out_ids, float* out_f, double* out_d) {
+    Context& c = ctx();
+    ivf_unmask_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, c.stream>>>(ix.metric, nq, k, probes, pos, key, dist, cap, mk.has_nan, d_lists,
+                                                                             cand_off, ix.d_list_off, ix.d_ids, out_ids, out_f, out_d);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
+}
+
 static int64_t ivf_cap(const Ivf& ix, int probes) {
     int64_t cap = 0;
     for (int i = 0; i < probes && i < (int)ix.sorted_len.size(); ++i) cap += ix.sorted_len[(size_t)i];
@@ -354,9 +501,10 @@ static int ivf_ensure_l0_image(Ivf& ix) {
     return list_tc_prepare_l0(ix.rows, &ix.tc);
 }
 
-// scan the given probe lists for a batch of queries and keep the k nearest per query
+// scan the given probe lists for a batch of queries and keep the k nearest per query (mask: of the rows each query's
+// row filter allows)
 static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, const int32_t* d_lists, int probes, int k,
-                         int64_t* out_ids_dev, float* out_f_dev, double* out_d_dev, int32_t** cand_total_dev) {
+                         int64_t* out_ids_dev, float* out_f_dev, double* out_d_dev, int32_t** cand_total_dev, const IvfMask* mask = nullptr) {
     Context& c = ctx();
     const int rpc = scan_chunk_rows(ix.rows);
     const int64_t cap = ivf_cap(ix, probes);
@@ -437,6 +585,9 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
         VB_TRY(launch_list_tc(ix.rows, ix.tc, km, qimg, qstride, nq, d_lists, probes, cand_off, cap, ix.d_list_off, ix.lists,
                               (float*)d_dist, &qn, false, level, (float*)d_smin, cap_s));
         prof_end(VB_PROF_SCAN_ITEMS);
+        if (mask)
+            VB_TRY(ivf_mask_runs(*mask, nq, d_lists, probes, cand_off, ix.d_list_off, cap, (float*)d_dist, (float*)d_smin, cap_s));
+        const int32_t* has_nan = mask ? mask->has_nan : nullptr;
         VB_TRY(workspace(WS_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)nq * (k + kp), &d_pos));
         int32_t* pos = (int32_t*)d_pos;
         float* key = (float*)(pos + (size_t)nq * k);
@@ -454,7 +605,7 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
             // counts as uncertified: the repeat of the batch selects below)
             VB_TRY(launch_list_tc_cta_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
                                              (const float*)d_dist, (const float*)d_smin, nullptr, nullptr, cap, cap_s, seg_len, qn, pos, key,
-                                             ix.d_tc_fail + 1, level, level == 0 ? ix.d_l0_fail : nullptr));
+                                             ix.d_tc_fail + 1, level, level == 0 ? ix.d_l0_fail : nullptr, has_nan));
         } else {
             // the k' selected by a launch of their own (slab_select_kernel hands what overflows it to the full selection)
             if (slabs)
@@ -464,7 +615,7 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
                 VB_TRY(launch_segment_topk_v((const float*)d_dist, seg_begin, seg_len, nullptr, nullptr, nq, kp, pos_kp, key_kp));
             VB_TRY(launch_list_tc_cta_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
                                              (const float*)d_dist, nullptr, pos_kp, key_kp, cap, cap_s, seg_len, qn, pos, key,
-                                             ix.d_tc_fail + 1, level));
+                                             ix.d_tc_fail + 1, level, nullptr, has_nan));
         }
         if (!ix.defer_tc_check) {
             VB_CUDA(cudaMemcpyAsync(&n_failed, ix.d_tc_fail + 1, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
@@ -479,6 +630,9 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
                                                                                       out_d_dev);
             VB_CUDA(cudaGetLastError());
             count_launch();
+            if (mask)
+                VB_TRY(ivf_unmask(ix, *mask, nq, k, probes, pos, key, (const float*)d_dist, cap, d_lists, cand_off, out_ids_dev, out_f_dev,
+                                  out_d_dev));
             if (cand_total_dev) *cand_total_dev = seg_len;
             return VB_OK;
         }
@@ -493,6 +647,7 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
         VB_TRY(launch_scan_chunks(ix.rows, km, qimg, qstride, chunks, n_chunks, (int)max_chunks, (float*)d_dist));
     }
     prof_end(VB_PROF_SCAN_ITEMS);
+    if (mask) VB_TRY(ivf_mask_runs(*mask, nq, d_lists, probes, cand_off, ix.d_list_off, cap, (float*)d_dist, nullptr, 0));
     VB_TRY(workspace(WS_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)nq * k, &d_pos));
     int32_t* pos = (int32_t*)d_pos;
     float* key = (float*)(pos + (size_t)nq * k);
@@ -515,6 +670,8 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
                                                                               out_d_dev);
     VB_CUDA(cudaGetLastError());
     count_launch();
+    if (mask)
+        VB_TRY(ivf_unmask(ix, *mask, nq, k, probes, pos, key, (const float*)d_dist, cap, d_lists, cand_off, out_ids_dev, out_f_dev, out_d_dev));
     if (cand_total_dev) *cand_total_dev = seg_len;
     return VB_OK;
 }
@@ -1691,8 +1848,34 @@ __global__ void scatter_results_kernel(const int64_t* __restrict__ ids, const fl
     out_f[o] = dist[i];
 }
 
+// the row filters of a vb_ivf_search_filtered call (validated): query q of the call uses filters[fq ? fq[q] : 0]
+struct IvfFilterSpec {
+    const vb_filter* const* filters;
+    int nfilters;
+    const int32_t* fq;   // host
+};
+
 static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, bool host, bool q_host, int64_t* out_ids,
-                           float* out_f, double* out_d, bool level0 = true);
+                           float* out_f, double* out_d, bool level0 = true, const IvfFilterSpec* filt = nullptr);
+
+enum { WS_FILT = 23 };   // the mask arguments of a sub-batch (the sparsevec calls' slot: they never run inside a search)
+
+// the mask arguments of queries [q0, q0 + m) of a filtered call: the filters' positions and runs, in place
+static int ivf_upload_mask(const IvfFilterSpec& filt, int64_t q0, int64_t m, IvfMask* mk) {
+    Context& c = ctx();
+    const size_t tab = ((sizeof(MaskFilter) * (size_t)filt.nfilters) + 15) & ~(size_t)15;
+    void* d;
+    VB_TRY(workspace(WS_FILT, tab + 2 * sizeof(int32_t) * (size_t)m, &d));
+    std::vector<MaskFilter> h((size_t)filt.nfilters);
+    for (int i = 0; i < filt.nfilters; ++i) h[(size_t)i] = MaskFilter{filt.filters[i]->f.pos, filt.filters[i]->f.off};
+    VB_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(MaskFilter) * h.size(), cudaMemcpyHostToDevice, c.stream));
+    int32_t* fq = (int32_t*)((uint8_t*)d + tab);
+    if (filt.fq) VB_CUDA(cudaMemcpyAsync(fq, filt.fq + q0, sizeof(int32_t) * (size_t)m, cudaMemcpyHostToDevice, c.stream));
+    mk->filters = (const MaskFilter*)d;
+    mk->fq = filt.fq ? fq : nullptr;
+    mk->has_nan = fq + m;
+    return VB_OK;
+}
 
 struct ResetFlag {   // clears a flag on every exit of a scope
     bool& f;
@@ -1704,12 +1887,24 @@ struct ResetFlag {   // clears a flag on every exit of a scope
 // (not the fused one-query kernels): a query certified at level 1 or 2 carries the filter's exact re-score, as it would in
 // a batch-wide repeat.  When the re-run needs the exact kernels, the caller computes the whole sub-batch there instead,
 // as it does without level 0 (the list-major kernel's sums may differ from the re-score's in the last bit).
+// (filt: the row filters of `queries`, whose failed queries' entries of filter_of_query go along)
 static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t>& fail, int probes, int k, bool host, bool q_host,
-                             int64_t* out_ids, float* out_f, double* out_d) {
+                             int64_t* out_ids, float* out_f, double* out_d, const IvfFilterSpec* filt) {
     Ivf& ix = h->ix;
     Context& c = ctx();
     std::sort(fail.begin(), fail.end());
     const int64_t nf = (int64_t)fail.size();
+    std::vector<int32_t> sub_fq;
+    IvfFilterSpec sub_filt;
+    if (filt) {
+        sub_filt = *filt;
+        if (filt->fq) {
+            sub_fq.resize((size_t)nf);
+            for (int64_t i = 0; i < nf; ++i) sub_fq[(size_t)i] = filt->fq[fail[(size_t)i]];
+            sub_filt.fq = sub_fq.data();
+        }
+        filt = &sub_filt;
+    }
     const size_t rawq = raw_row_bytes(ix.elem, ix.dim);
     const size_t q_bytes = (rawq * (size_t)nf + 15) & ~(size_t)15;
     const size_t need = q_bytes + (sizeof(int64_t) + sizeof(float)) * (size_t)nf * k + sizeof(int64_t) + sizeof(int32_t) * (size_t)nf;
@@ -1741,7 +1936,7 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
     if (host) {
         std::vector<int64_t> ti((size_t)nf * k);
         std::vector<double> td((size_t)nf * k);
-        VB_TRY(ivf_search_impl(h, sub, nf, probes, k, true, q_host, ti.data(), nullptr, td.data(), false));
+        VB_TRY(ivf_search_impl(h, sub, nf, probes, k, true, q_host, ti.data(), nullptr, td.data(), false, filt));
         VB_CUDA(cudaMemcpyAsync(ix.d_cand_sum, d_cand_saved, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
         for (int64_t i = 0; i < nf; ++i) {
             memcpy(out_ids + (size_t)fail[(size_t)i] * k, ti.data() + (size_t)i * k, sizeof(int64_t) * k);
@@ -1749,7 +1944,7 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
         }
         return VB_OK;
     }
-    VB_TRY(ivf_search_impl(h, sub, nf, probes, k, false, false, d_ids, d_f, nullptr, false));
+    VB_TRY(ivf_search_impl(h, sub, nf, probes, k, false, false, d_ids, d_f, nullptr, false, filt));
     VB_CUDA(cudaMemcpyAsync(ix.d_cand_sum, d_cand_saved, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
     scatter_results_kernel<<<(unsigned)((nf * k + 255) / 256), 256, 0, c.stream>>>(d_ids, d_f, d_idx, nf, k, out_ids, out_f);
     VB_CUDA(cudaGetLastError());
@@ -1760,7 +1955,7 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
 // host: results go to host memory (int64 ids + float8 distances); q_host: the queries are host memory.  level0: the list
 // scan may start at filter level 0 (false for the re-run of the queries it could not certify)
 static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, bool host, bool q_host, int64_t* out_ids,
-                           float* out_f, double* out_d, bool level0) {
+                           float* out_f, double* out_d, bool level0, const IvfFilterSpec* filt) {
     VB_TRY(require_init());
     VB_REQUIRE(h && h->ix.loaded, "index not loaded");
     VB_REQUIRE(queries && probes >= 1 && k >= 1, "bad search arguments");
@@ -1769,7 +1964,8 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
     probes = std::min(probes, ix.lists);
     if (nq <= 0) return VB_OK;
     const size_t rawq = raw_row_bytes(ix.elem, ix.dim);
-    if (!ix.repairing && ivf_one_applies(ix, nq, probes, k, ivf_cap(ix, probes))) {
+    // (the fused one-query kernels select inside the scan: a filtered call takes the general path and its mask)
+    if (!ix.repairing && !filt && ivf_one_applies(ix, nq, probes, k, ivf_cap(ix, probes))) {
         // a handful of queries (one backend's scan): two fused launches, no memsets, one copy back
         const int64_t cap = ivf_cap(ix, probes);
         void* qimg;
@@ -1812,6 +2008,9 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
         void* qimg;
         size_t qstride;
         VB_TRY(upload_queries(ix.elem, ix.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, q_host, WS_QIMG, &qimg, &qstride));
+        IvfMask mk{};
+        if (filt) VB_TRY(ivf_upload_mask(*filt, q0, m, &mk));
+        const IvfMask* mask = filt ? &mk : nullptr;
         int32_t* d_lists;
         float* d_ldist;
         VB_TRY(ivf_select_probes(ix, qimg, qstride, m, probes, &d_lists, &d_ldist));
@@ -1820,11 +2019,11 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
             VB_TRY(workspace(WS_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
             int64_t* o_ids = (int64_t*)d_out;
             double* o_d = (double*)(o_ids + (size_t)m * k);
-            VB_TRY(ivf_scan_topk(ix, qimg, qstride, m, d_lists, probes, k, o_ids, nullptr, o_d, nullptr));
+            VB_TRY(ivf_scan_topk(ix, qimg, qstride, m, d_lists, probes, k, o_ids, nullptr, o_d, nullptr, mask));
             VB_CUDA(cudaMemcpyAsync(out_ids + q0 * k, o_ids, sizeof(int64_t) * (size_t)m * k, cudaMemcpyDeviceToHost, c.stream));
             VB_CUDA(cudaMemcpyAsync(out_d + q0 * k, o_d, sizeof(double) * (size_t)m * k, cudaMemcpyDeviceToHost, c.stream));
         } else {
-            VB_TRY(ivf_scan_topk(ix, qimg, qstride, m, d_lists, probes, k, out_ids + q0 * k, out_f + q0 * k, nullptr, nullptr));
+            VB_TRY(ivf_scan_topk(ix, qimg, qstride, m, d_lists, probes, k, out_ids + q0 * k, out_f + q0 * k, nullptr, nullptr, mask));
         }
         fails[0] = fails[1] = 0;
         const bool check = !exact && ix.d_tc_fail != nullptr;
@@ -1854,8 +2053,13 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
                 VB_CUDA(cudaMemcpy(fail.data(), ix.d_l0_fail, sizeof(int32_t) * (size_t)fails[1], cudaMemcpyDeviceToHost));
             }
             const int64_t exact0 = ix.total_tc_failed;
+            IvfFilterSpec sub_filt;
+            if (filt) {
+                sub_filt = *filt;
+                if (filt->fq) sub_filt.fq = filt->fq + q0;
+            }
             rc = ivf_repair_level0(h, (const uint8_t*)queries + (size_t)q0 * rawq, fail, probes, k, host, q_host, out_ids + q0 * k,
-                                   out_f ? out_f + q0 * k : nullptr, out_d ? out_d + q0 * k : nullptr);
+                                   out_f ? out_f + q0 * k : nullptr, out_d ? out_d + q0 * k : nullptr, filt ? &sub_filt : nullptr);
             if (rc == VB_OK && ix.total_tc_failed > exact0) rc = run(q0, m, 2, fails);   // neither level 1 nor 2 certified them
             continue;
         }
@@ -1885,6 +2089,61 @@ int vb_ivf_search(vb_ivf* h, const void* queries, int64_t nq, int probes, int k,
 }
 int vb_ivf_search_dev(vb_ivf* h, const void* queries_dev, int64_t nq, int probes, int k, int64_t* out_ids_dev, float* out_dist_dev) {
     return ivf_search_impl(h, queries_dev, nq, probes, k, false, false, out_ids_dev, out_dist_dev, nullptr);
+}
+
+}  // extern "C"
+
+// vb_ivf_search with a row filter per query: the arguments are checked as the filtered handle checks them, then the
+// batched search runs with its runs masked.  The host variant searches into staging buffers and copies them out only
+// when the whole call succeeded.
+static int ivf_search_filtered_impl(const char* fn, vb_ivf* h, const void* queries, int64_t nq, int probes, int k,
+                                    const vb_filter* const* filters, int nfilters, const int32_t* filter_of_query, bool host,
+                                    int64_t* out_ids, float* out_f, double* out_d) {
+    VB_TRY(require_init());
+    if (!h || !h->ix.loaded) {
+        set_error("%s: index not loaded", fn);
+        return VB_ESTATE;
+    }
+    Ivf& ix = h->ix;
+    VB_REQUIRE(queries, "%s: queries must not be NULL", fn);
+    VB_REQUIRE(probes >= 1 && k >= 1, "%s: probes and k must be >= 1 (got %d, %d)", fn, probes, k);
+    VB_REQUIRE(filters && nfilters >= 1, "%s: no row filter given", fn);
+    VB_REQUIRE(filter_of_query || nfilters == 1, "%s: filter_of_query may only be NULL with one filter (got %d)", fn, nfilters);
+    for (int i = 0; i < nfilters; ++i) {
+        VB_REQUIRE(filters[i], "%s: filter %d is NULL", fn, i);
+        const Filter& f = filters[i]->f;
+        VB_REQUIRE(f.kind == FILTER_IVF && f.owner == h && f.owner_uid == h->uid, "%s: filter %d was made for another table or index", fn, i);
+        if (f.generation != ix.generation) {
+            set_error("%s: filter %d: index changed since the filter was created", fn, i);
+            return VB_ESTATE;
+        }
+    }
+    for (int64_t q = 0; q < nq && filter_of_query; ++q)
+        VB_REQUIRE(filter_of_query[q] >= 0 && filter_of_query[q] < nfilters, "%s: filter_of_query[%lld] = %d, not in 0..%d", fn,
+                   (long long)q, filter_of_query[q], nfilters - 1);
+    if (nq <= 0) return VB_OK;
+    VB_REQUIRE(out_ids && (out_f || out_d), "%s: null output", fn);
+    const IvfFilterSpec filt{filters, nfilters, nfilters > 1 ? filter_of_query : nullptr};
+    if (!host) return ivf_search_impl(h, queries, nq, probes, k, false, false, out_ids, out_f, nullptr, true, &filt);
+    std::vector<int64_t> ids((size_t)nq * k);
+    std::vector<double> dist((size_t)nq * k);
+    VB_TRY(ivf_search_impl(h, queries, nq, probes, k, true, true, ids.data(), nullptr, dist.data(), true, &filt));
+    memcpy(out_ids, ids.data(), sizeof(int64_t) * ids.size());
+    memcpy(out_d, dist.data(), sizeof(double) * dist.size());
+    return VB_OK;
+}
+
+extern "C" {
+
+int vb_ivf_search_filtered(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, const vb_filter* const* filters, int nfilters,
+                           const int32_t* filter_of_query, int64_t* out_ids, double* out_dist) {
+    return ivf_search_filtered_impl("vb_ivf_search_filtered", h, queries, nq, probes, k, filters, nfilters, filter_of_query, true, out_ids,
+                                    nullptr, out_dist);
+}
+int vb_ivf_search_filtered_dev(vb_ivf* h, const void* queries_dev, int64_t nq, int probes, int k, const vb_filter* const* filters,
+                               int nfilters, const int32_t* filter_of_query, int64_t* out_ids_dev, float* out_dist_dev) {
+    return ivf_search_filtered_impl("vb_ivf_search_filtered_dev", h, queries_dev, nq, probes, k, filters, nfilters, filter_of_query, false,
+                                    out_ids_dev, out_dist_dev, nullptr);
 }
 
 // Pipelined host path: the queries of the NEXT call are copied to the device on a second stream while the current

@@ -714,7 +714,15 @@ __host__ __device__ inline size_t cr_work_bytes(bool slabs, bool pre, int64_t ca
 // distance; phase 2 re-scores every other listed candidate with d~_i - E_i <= T (NaN included).  A candidate left out has
 // d >= d~_i - E_i > T, so it is behind k re-scored ones.  The certificate then needs d~_{k'} > T + E_max(q), T the k-th
 // exact distance of the re-scored set: every unselected row has d >= d~ - E_max >= d~_{k'} - E_max > T.
-template <int ELEM, int METRIC, bool LIST>
+//
+// MASK (vb_ivf_search_filtered): the run is masked, rejected entries hold FILTER_REJECTED, the slab minima are those of the
+// allowed entries, and has_nan[q] says an allowed entry of query q has a NaN d~.  Candidates with a NaN key are then
+// rejected ones (such a query counts as uncertified otherwise) and are dropped: `have` counts the allowed candidates.
+// Fewer than k' of them means every allowed row of the run is a candidate (a selection of at least k' entries holds a
+// rejected one only after every allowed one: the slab selection then took every entry of the run, tau being the key of
+// NaN), so the result is complete and needs no certificate.  A run with fewer than k' slabs that hold an allowed row and
+// more than SS_CAND entries overflows the slab selection; the query then counts as uncertified, as a tie overflow does.
+template <int ELEM, int METRIC, bool LIST, bool MASK = false>
 __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows, size_t stride, int V,
                                                                 const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
                                                                 LcBound bound, const float* __restrict__ qn, const float* __restrict__ dist,
@@ -725,7 +733,8 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
                                                                 int32_t* __restrict__ out_pos, float* __restrict__ out_key,
                                                                 int* __restrict__ n_failed, int32_t* __restrict__ fail_list,
                                                                 const float* __restrict__ xn, const float* __restrict__ r8,
-                                                                const float4* __restrict__ coef, unsigned long long* __restrict__ counters) {
+                                                                const float4* __restrict__ coef, unsigned long long* __restrict__ counters,
+                                                                const int32_t* __restrict__ has_nan = nullptr) {
     const bool slabs = LIST || smin != nullptr;                                 // (level 0 always has slab minima)
     const bool pre = !LIST && pre_pos != nullptr;
     extern __shared__ uint64_t cr_smem[];
@@ -768,7 +777,8 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
         }
         return;
     }
-    const int have = min(n, kp);
+    int have = min(n, kp);
+    if constexpr (MASK) have = __syncthreads_count(tid < have && (cand[tid] >> 32) != 0xFFFFFFFFull);   // (kp <= SS_THREADS; sorted)
     // ---- threshold: (k-th smallest approximate distance) + 2 eps.  Only candidates with d~ under it can belong to the k
     // nearest: the k candidates with the smallest d~ all have d <= (k-th d~) + eps, anything above it has d > (k-th d~) + eps.
     const int kth = min(k, kp) - 1;
@@ -878,6 +888,21 @@ __device__ __forceinline__ void cta_refine_body(const uint8_t* __restrict__ rows
         if (LIST && rank == k - 1) s_tk = key_to_float((uint32_t)(mine >> 32));
     }
     if (LIST) __syncthreads();
+    if constexpr (MASK) {
+        // ---- certificate of a masked run: only when k' allowed candidates were kept and the run holds more entries
+        if (tid == 0) {
+            bool ok = has_nan[q] == 0;
+            if (ok && have >= kp && n_run > kp) {
+                const float Tc = LIST ? __fadd_ru(s_tk, __fsqrt_ru(qn[q])) : T;
+                ok = key_to_float((uint32_t)(thr >> 32)) > Tc;
+            }
+            if (!ok) {
+                const int i = atomicAdd(n_failed, 1);
+                if (LIST) fail_list[i] = q;
+            }
+        }
+        return;
+    }
     // ---- certificate: candidates beyond the k' exist -> the last of the k' must already be above the threshold
     if (tid == 0 && n_run > kp) {
         // (LIST: the threshold T + E_max(q) is rounded up, E_max = eps(q) >= E_i of every row, from its square rounded up)
@@ -918,6 +943,37 @@ __global__ void __launch_bounds__(SS_THREADS) cta_refine_list_kernel(const uint8
                                                                 const float4* __restrict__ coef, unsigned long long* __restrict__ counters) {
     cta_refine_body<ELEM, METRIC, true>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, nullptr, nullptr, cap, cap_s, seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, fail_list,
                                         xn, r8, coef, counters);
+}
+// the two above over masked runs (vb_ivf_search_filtered)
+template <int ELEM, int METRIC>
+__global__ void __launch_bounds__(SS_THREADS) cta_refine_masked_kernel(const uint8_t* __restrict__ rows, size_t stride, int V,
+                                                                const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
+                                                                LcBound bound, const float* __restrict__ qn, const float* __restrict__ dist,
+                                                                const float* __restrict__ smin, const int32_t* __restrict__ pre_pos,
+                                                                const float* __restrict__ pre_key, int64_t cap, int64_t cap_s,
+                                                                const int32_t* __restrict__ seg_len, const int32_t* __restrict__ probe_lists,
+                                                                const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
+                                                                int32_t* __restrict__ out_pos, float* __restrict__ out_key,
+                                                                int* __restrict__ n_failed, const int32_t* __restrict__ has_nan) {
+    cta_refine_body<ELEM, METRIC, false, true>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, pre_pos, pre_key, cap, cap_s,
+                                               seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, nullptr, nullptr, nullptr,
+                                               nullptr, nullptr, has_nan);
+}
+template <int ELEM, int METRIC>
+__global__ void __launch_bounds__(SS_THREADS) cta_refine_list_masked_kernel(const uint8_t* __restrict__ rows, size_t stride, int V,
+                                                                const uint8_t* __restrict__ qimg, size_t qstride, int k, int kp, int probes,
+                                                                LcBound bound, const float* __restrict__ qn, const float* __restrict__ dist,
+                                                                const float* __restrict__ smin, int64_t cap, int64_t cap_s,
+                                                                const int32_t* __restrict__ seg_len, const int32_t* __restrict__ probe_lists,
+                                                                const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off,
+                                                                int32_t* __restrict__ out_pos, float* __restrict__ out_key,
+                                                                int* __restrict__ n_failed, int32_t* __restrict__ fail_list,
+                                                                const float* __restrict__ xn, const float* __restrict__ r8,
+                                                                const float4* __restrict__ coef, unsigned long long* __restrict__ counters,
+                                                                const int32_t* __restrict__ has_nan) {
+    cta_refine_body<ELEM, METRIC, true, true>(rows, stride, V, qimg, qstride, k, kp, probes, bound, qn, dist, smin, nullptr, nullptr, cap, cap_s,
+                                              seg_len, probe_lists, cand_off, list_off, out_pos, out_key, n_failed, fail_list, xn, r8, coef,
+                                              counters, has_nan);
 }
 
 // Bytes one launch of list_tc_kernel moves, from the same job list the kernel walks (profiling only):
@@ -1356,7 +1412,7 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
                               int k, int kp, int probes, const int32_t* d_lists, const int32_t* cand_off, const int64_t* d_list_off,
                               const float* dist, const float* smin, const int32_t* pre_pos, const float* pre_key, int64_t cap,
                               int64_t cap_s, const int32_t* seg_len, const float* qn, int32_t* out_pos, float* out_key, int* fail_dev,
-                              int level, int32_t* fail_list) {
+                              int level, int32_t* fail_list, const int32_t* has_nan) {
     if (nq == 0) return VB_OK;
     Context& c = ctx();
     cudaStream_t s = c.stream;
@@ -1368,6 +1424,23 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
     VB_REQUIRE(!fail_list || (level == 0 && im.r8 && smin), "cta_refine: the listing kernel is level 0's and needs its int8 image and slab minima");
 #define VB_CR(E, M)                                                                                                              \
     do {                                                                                                                         \
+        if (fail_list && has_nan) {                                                                                              \
+            auto kern = cta_refine_list_masked_kernel<E, M>;                                                                     \
+            if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
+            kern<<<(unsigned)nq, SS_THREADS, smem, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, k, kp, probes, bound, qn, dist, \
+                                                       smin, cap, cap_s, seg_len, d_lists, cand_off, d_list_off, out_pos, out_key, fail_dev, \
+                                                       fail_list, im.xn, im.r8, l0_row_coef(qn, nq),                             \
+                                                       g_traffic_on ? g_traffic + 8 : nullptr, has_nan);                        \
+            break;                                                                                                               \
+        }                                                                                                                        \
+        if (has_nan) {                                                                                                           \
+            auto kern = cta_refine_masked_kernel<E, M>;                                                                          \
+            if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
+            kern<<<(unsigned)nq, SS_THREADS, smem, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, k, kp, probes, bound, qn, dist, \
+                                                       smin, pre_pos, pre_key, cap, cap_s, seg_len, d_lists, cand_off, d_list_off, out_pos, \
+                                                       out_key, fail_dev, has_nan);                                              \
+            break;                                                                                                               \
+        }                                                                                                                        \
         if (fail_list) {                                                                                                         \
             auto kern = cta_refine_list_kernel<E, M>;                                                                            \
             if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
