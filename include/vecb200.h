@@ -103,6 +103,13 @@ int			vb_stream_wait_event(void *cuda_event);
 #define VB_PROF_LIST_TC 5		/* list_tc_kernel alone (the tensor-core filter pass over the probed lists) */
 #define VB_PROF_CENTRE_TC 6		/* the same kernel over the centre table (probe selection of query batches) */
 #define VB_PROF_FILTER_MASK 7	/* the row-filter mask of vb_ivf_search_filtered over the candidate distances */
+/* the phases of vb_ivf_build* (VB_PROF_ASSIGN stays with vb_assign and the Lloyd iterations' assign step) */
+#define VB_PROF_BUILD_SAMPLE 8	/* draw, gather and (spherical) normalise + compact the samples */
+#define VB_PROF_BUILD_SEED 9	/* k-means++ seeding */
+#define VB_PROF_BUILD_LLOYD 10	/* Lloyd iterations */
+#define VB_PROF_BUILD_DEST 11	/* list numbers -> list offsets, image order and per-row destinations */
+#define VB_PROF_BUILD_PLACE 12	/* the placement kernel alone (one bracket per launch) */
+#define VB_PROF_BUILD_ASSIGN 13	/* pass one: the list of every row (per chunk: padding / normalisation, assign) */
 int			vb_prof_enable(int on);
 /* Synchronises, then returns accumulated milliseconds and bracketed launches since the last read of `kernel`. */
 int			vb_prof_read(int kernel, double *total_ms, int64_t *launches);
@@ -650,6 +657,68 @@ int64_t		vb_last_assign_rechecked(void);
  * kernels (the last CTA to finish selects; csrc/vb_ivf_one.cu) instead of the general launch sequence; 0 = general path.
  */
 int			vb_set_option(const char *name, int64_t value);
+
+/*
+ * CREATE INDEX ... USING ivfflat in one call (ivfflatbuild, src/ivfbuild.c): the n rows of the call become a resident,
+ * searchable image of `ix` (made by vb_ivf_create; any element type and metric it accepts).  The call composes the
+ * entry points above -- it equals them bit for bit on the same samples and draws -- and adds what lay between them:
+ *
+ *   samples   SampleRows (src/ivfbuild.c:132-156).  opts->sample_rows, in the caller's order, or n_samples distinct rows
+ *             drawn on the device: row numbers perm(0 .. n_samples - 1) of a 4-round Feistel permutation of [0, 2^b)
+ *             keyed by the seed (b even, 2^b >= n), cycle-walked into [0, n) -- a bijection, so the draws are distinct
+ *             without a table of size n -- and sorted ascending.  The reference's block sampler and reservoir are
+ *             PRNG-driven and not reproduced; parity is defined from shared sample_rows / first_row / u.  The k-means
+ *             metric follows the opclass: VB_L2 (L2 squared), VB_SPHERICAL (negative inner product, i.e. the ip and the
+ *             cosine opclasses), VB_HAMMING (bit).  Spherical: samples of norm 0 are dropped and the others
+ *             l2-normalised (vb_l2_normalize_batch's arithmetic), keeping their order, whatever `normalize` says
+ *             (AddSample, src/ivfbuild.c:66-73).  Fewer usable samples than lists is VB_EINVAL.
+ *   centres   vb_kmeans_pp_init[_draws], then vb_kmeans, on those samples; they become the image's centre table
+ *             (vb_ivf_centers reads it back, for CreateListPages).
+ *   assign    AddTupleToSort (src/ivfbuild.c:161-219).  normalize != 0 (the cosine opclasses): a row of norm 0 is not
+ *             indexed (out_lists[i] = -1) and the others are l2-normalised before the argmin and stored normalised.
+ *             out_lists[i] = vb_assign's list of (normalised) row i: the first minimum wins.
+ *   place     row i is stored in list out_lists[i], rows of one list in call order (the order a serial heap scan feeds
+ *             the tuplesort in; list scans break exact ties by position).  out_order[p], p < vb_ivf_rows(ix), is the
+ *             call's row number stored at image row p -- with vb_ivf_list_offsets, what InsertTuples walks -- and -1
+ *             from there on.  The image ends as vb_ivf_load leaves it for the same centres, offsets, grouped rows and
+ *             ids: generation bumped, packed tensor-core planes released (the next batched scan builds them).
+ *
+ * vb_ivf_build streams the host rows twice through two pinned staging buffers of chunk_rows rows (0 = 128 MB worth,
+ * at least 1024 and at most 2^20 rows; a buffer is chunk_rows * (row bytes + 8) bytes, and exists twice pinned -- kept
+ * by the library for later calls -- and twice on the device; caller memory that is already page-locked is read in
+ * place), the copy of chunk c + 1 overlapping the
+ * work on chunk c: pass one assigns and keeps 4 bytes per row, pass two scatters each chunk's rows to their final image
+ * rows.  The device holds one copy of the indexed rows, their ids, 36 bytes per row of list numbers, sort buffers and
+ * destinations, the samples, and the chunk buffers.  vb_ivf_build_dev reads the caller's device rows in place (assign,
+ * then one gather in image order), so it holds the caller's copy and the image.  Both synchronise before returning.
+ *
+ * Everything that can be refused without touching the image happens first: arguments (n < 1, n >= 2^31, NULL rows or
+ * ids -- an image without ids cannot take inserts --, sample_rows out of range or repeated: VB_EINVAL; an active
+ * communicator, whose images are shards: VB_ESTATE), the samples, the k-means and the assign.  After such a failure a
+ * loaded image is as it was.  Then the old rows are released, the new table is allocated and the rows are placed: a
+ * VB_ENOMEM (its message names the bytes) or CUDA error from there on leaves the image unloaded (VB_ESTATE until the
+ * next load or build).  Row filters and scan handles made before a build fail with VB_ESTATE afterwards.
+ */
+typedef struct vb_ivf_build_opts
+{
+	uint64_t	seed;			/* sample draw (sample_rows == NULL), k-means++ draws (u == NULL), empty-cluster reseed */
+	int			max_iter;		/* Lloyd iterations, 0 = 500 (src/ivfkmeans.c:347) */
+	const int64_t *sample_rows;	/* host, [n_samples] row numbers of this call's rows; NULL = drawn by the library */
+	int64_t		n_samples;		/* with sample_rows; otherwise 0 = min(n, max(50 * lists, 10000)) (src/ivfbuild.c:448-455) */
+	int64_t		first_row;		/* with u: index INTO THE USABLE SAMPLES of the first centre, as vb_kmeans_pp_init_draws */
+	const double *u;			/* host, [lists - 1] RandomDouble() draws; NULL = from seed */
+	int64_t		chunk_rows;		/* vb_ivf_build: rows per streamed chunk, 0 = automatic */
+} vb_ivf_build_opts;
+
+int			vb_ivf_build(vb_ivf *ix, const void *rows, const int64_t *ids, int64_t n, int normalize,
+						 const vb_ivf_build_opts *opts /* NULL = defaults, seed 42 */ ,
+						 int32_t *out_lists /* host [n], may be NULL */ , int64_t *out_order /* host [n], may be NULL */ ,
+						 int *iters_out /* may be NULL */ );
+int			vb_ivf_build_dev(vb_ivf *ix, const void *rows_dev, const int64_t *ids_dev, int64_t n, int normalize,
+							 const vb_ivf_build_opts *opts, int32_t *out_lists /* host */ , int64_t *out_order /* host */ ,
+							 int *iters_out);
+/* The centre table of a loaded image: [lists] packed rows of the index's element type, to host memory. */
+int			vb_ivf_centers(const vb_ivf *ix, void *out);
 
 /* -------------------------------------------------------------------- HNSW */
 

@@ -60,6 +60,8 @@ def launch_count() -> int:
 
 
 PROF_SCAN_ITEMS, PROF_SCAN_LISTS, PROF_TOPK, PROF_ASSIGN, PROF_HNSW, PROF_LIST_TC, PROF_CENTRE_TC = range(7)
+# the phases of IvfflatIndex.build
+PROF_BUILD_SAMPLE, PROF_BUILD_SEED, PROF_BUILD_LLOYD, PROF_BUILD_DEST, PROF_BUILD_PLACE, PROF_BUILD_ASSIGN = range(8, 14)
 
 
 def prof_enable(on=True):
@@ -447,6 +449,71 @@ class IvfflatIndex:
         self._off[l + 1:] += delta
         return self
 
+    def _device_rows(self, rows, n):
+        """torch CUDA rows as the _dev entry points read them: [n, cols] of the element's width, contiguous"""
+        width = {VECTOR: 4, HALFVEC: 2, BIT: 1}[self.elem]
+        cols = self.dim if self.elem != BIT else (self.dim + 7) // 8
+        if rows.element_size() != width or rows.dtype.is_complex or tuple(rows.reshape(n, -1).shape) != (n, cols):
+            raise TypeError(f"device rows for {self.opclass} must be [n, {cols}] of {width}-byte elements, "
+                            f"not {tuple(rows.shape)} {rows.dtype}")
+        return rows.reshape(n, -1).contiguous()
+
+    def build(self, rows, ids, seed=42, sample_rows=None, n_samples=None, first_row=None, u=None, max_iter=500, chunk_rows=None):
+        """CREATE INDEX on the device (ivfflatbuild, src/ivfbuild.c): samples, k-means++, Lloyd, assign and placement of
+        `rows` into a resident image, in one call.  Returns (lists, order, iters): the list of every row (int32 [n]; -1
+        for a row of norm 0 under a cosine opclass, which is not indexed), the row number stored at every image row (int64
+        [n], -1 past len(index)) and the Lloyd iterations run.  `sample_rows` (row numbers) or `n_samples` rows drawn from
+        `seed` train the centres; `first_row` and `u` are the k-means++ draws, as kmeans_pp_init_draws takes them.  numpy
+        rows are streamed from the host in chunks of `chunk_rows`; torch CUDA rows are read in place."""
+        n = rows.shape[0] if rows.ndim > 1 else 1
+        if (first_row is None) != (u is None):
+            raise ValueError("first_row and u come together")
+        opts = _lib.IvfBuildOpts(seed=int(seed), max_iter=int(max_iter), chunk_rows=int(chunk_rows or 0))
+        if sample_rows is not None:
+            sample_rows = np.ascontiguousarray(sample_rows, dtype=np.int64).reshape(-1)
+            opts.sample_rows, opts.n_samples = sample_rows.ctypes.data, sample_rows.shape[0]
+        elif n_samples is not None:
+            opts.n_samples = int(n_samples)
+        if u is not None:
+            u = np.ascontiguousarray(u, dtype=np.float64).reshape(-1)
+            if u.shape[0] < self.lists - 1:
+                raise ValueError(f"u holds {u.shape[0]} draws, {self.lists - 1} are needed")
+            opts.first_row, opts.u = int(first_row), u.ctypes.data
+        lists = np.empty(n, dtype=np.int32)
+        order = np.empty(n, dtype=np.int64)
+        iters = C.c_int()
+        if _is_torch(rows) and rows.is_cuda:
+            import torch
+            rows = self._device_rows(rows, n)
+            if ids is not None:
+                ids = torch.as_tensor(ids, device=rows.device).to(torch.int64).reshape(n).contiguous()
+            _after_torch(rows, ids)
+            fn = load().vb_ivf_build_dev
+        else:
+            if _is_torch(rows):
+                rows = rows.numpy()
+            if _is_torch(ids):
+                ids = ids.cpu().numpy()
+            rows = _host(self.elem, rows).reshape(n, -1)
+            if rows.shape[1] != (self.dim if self.elem != BIT else (self.dim + 7) // 8):
+                raise TypeError(f"rows for {self.opclass} of {self.dim} dimensions must not be {tuple(rows.shape)}")
+            ids = None if ids is None else np.ascontiguousarray(ids, dtype=np.int64).reshape(n)
+            fn = load().vb_ivf_build
+        _lib.check(fn(self.h, _ptr(rows), _ptr(ids), n, 1 if self.normalize else 0, C.byref(opts), _ptr(lists), _ptr(order),
+                      C.byref(iters)))
+        self._refresh_offsets()
+        return lists, order, iters.value
+
+    def centers(self):
+        """the centre table of the image, [lists] rows of the element type (what CreateListPages writes)"""
+        cols = self.dim if self.elem != BIT else (self.dim + 7) // 8
+        out = np.empty((self.lists, cols), dtype=_NP[self.elem])
+        _lib.check(load().vb_ivf_centers(self.h, _ptr(out)))
+        return out
+
+    def __len__(self):
+        return int(load().vb_ivf_rows(self.h))
+
     def insert(self, rows, ids):
         """INSERT into the resident image without reloading it (InsertTuple, src/ivfinsert.c:72-181, row after row):
         each row is appended to the list FindInsertPage picks.  Returns the lists (int32 [n]).  ids are the rows' heap
@@ -457,12 +524,7 @@ class IvfflatIndex:
         out = np.full(n, -1, dtype=np.int32)
         if _is_torch(rows) and rows.is_cuda and not self.normalize:
             import torch
-            width = {VECTOR: 4, HALFVEC: 2, BIT: 1}[self.elem]
-            cols = self.dim if self.elem != BIT else (self.dim + 7) // 8
-            if rows.element_size() != width or rows.dtype.is_complex or tuple(rows.reshape(n, -1).shape) != (n, cols):
-                raise TypeError(f"device rows for {self.opclass} must be [n, {cols}] of {width}-byte elements, "
-                                f"not {tuple(rows.shape)} {rows.dtype}")
-            rows = rows.reshape(n, -1).contiguous()
+            rows = self._device_rows(rows, n)
             ids = torch.as_tensor(ids, device=rows.device).to(torch.int64).reshape(n).contiguous()
             _after_torch(rows, ids)
             _lib.check(load().vb_ivf_insert_dev(self.h, _ptr(rows), _ptr(ids), n, _ptr(out)))

@@ -76,6 +76,9 @@ SIGNATURES = {
     "vb_ivf_insert_dev": (_i, [_vp, _vp, _vp, _i64, _vp]),
     "vb_ivf_delete": (_i, [_vp, _vp, _i64, C.POINTER(_i64)]),
     "vb_ivf_list_offsets": (_i, [_vp, _vp]),
+    "vb_ivf_build": (_i, [_vp, _vp, _vp, _i64, _i, _vp, _vp, _vp, C.POINTER(_i)]),
+    "vb_ivf_build_dev": (_i, [_vp, _vp, _vp, _i64, _i, _vp, _vp, _vp, C.POINTER(_i)]),
+    "vb_ivf_centers": (_i, [_vp, _vp]),
     "vb_ivf_free": (_i, [_vp]),
     "vb_ivf_scan_lists": (_i, [_vp, _vp, _i64, _i, _vp, _vp]),
     "vb_ivf_scan_items": (_i, [_vp, _vp, _vp, _i, _i64, _vp, _vp, _vp]),
@@ -139,6 +142,12 @@ SIGNATURES = {
     "vb_hnsw_filter_create_dev": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
     "vb_hnsw_scan_begin_filtered": (_i, [_vp, _vp, _i64, _i, _i64, _i, _vp, _i, _vp, C.POINTER(_vp)]),
 }
+
+
+class IvfBuildOpts(C.Structure):
+    """vb_ivf_build_opts"""
+    _fields_ = [("seed", _u64), ("max_iter", _i), ("sample_rows", _vp), ("n_samples", _i64), ("first_row", _i64), ("u", _vp),
+                ("chunk_rows", _i64)]
 
 
 class VecB200Error(RuntimeError):

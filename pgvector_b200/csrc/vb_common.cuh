@@ -80,6 +80,11 @@ inline void count_launch(int n = 1) { ctx().launches += n; }
 // optional event brackets around a kernel class (vb_prof_enable)
 void prof_begin(int which);
 void prof_end(int which);
+struct ProfScope {   // a bracket that is closed on every exit of its scope
+    int which;
+    explicit ProfScope(int w) : which(w) { prof_begin(w); }
+    ~ProfScope() { prof_end(which); }
+};
 
 // ---------------------------------------------------------------- communicator (vb_comm.cu)
 // world size / rank of the library's NCCL communicator (1 / 0 when none was created)
@@ -170,6 +175,29 @@ int launch_assign(const Table& X, int metric, const Table& Cn, int k, int32_t* o
 // all-pairs fp32 distances X x Cn -> out[x * ld + c] (register-tiled CUDA-core kernel, vb_kmeans.cu)
 int launch_distance_matrix(const Table& X, int metric, const Table& Cn, int k, float* out, int64_t ld);
 void set_tc_enabled(bool on);
+// the seeding and Lloyd code behind vb_kmeans_pp_init[_draws] and vb_kmeans (vb_kmeans.cu), for vb_ivf_build
+int kmeans_pp(const Table& X, int kmeans_metric, void* centers_host, int k, uint64_t seed, int64_t first_row = -1,
+              const double* u_in = nullptr, int64_t* picked_out = nullptr);
+int kmeans_run(const Table& X, int kmeans_metric, void* centers_host, int k, int max_iter, uint64_t seed, vb_allreduce_fn allreduce,
+               void* actx, int* iters_out);
+
+// ---------------------------------------------------------------- IVFFlat build (vb_ivf_build.cu)
+// ns distinct rows of [0, n) drawn from the seed, ascending (device, [ns])
+int build_draw_samples(int64_t n, int64_t ns, uint64_t seed, int64_t* rows_out);
+// The placement pass: work item j reads source row s = src_idx ? src_idx[j] : j (packed rows, `pitch` bytes apart) and
+// writes table row d = dst_idx ? dst_idx[j] : j (d < 0: skipped) at the padded stride, pad bytes zero, with its id
+// (src_ids ? src_ids[s] : s) to out_ids[d] when out_ids is given.  normalize (vector / halfvec): the row is stored
+// l2-normalised, and zero (optional, [m]) receives 1 where the norm is not > 0, else 0; out == nullptr computes only zero.
+int launch_place_rows(int elem, int dim, bool normalize, const void* src, size_t pitch, const int64_t* src_ids, const int64_t* src_idx,
+                      const int64_t* dst_idx, int64_t m, uint8_t* out, size_t out_stride, int64_t* out_ids, int32_t* zero);
+// lists[i] = -1 where zero[i]
+int build_mark_skipped(const int32_t* zero, int64_t m, int32_t* lists);
+// keep-order compaction map of the rows with zero[i] == 0: dst[i] = position among them, or -1; *kept = their number
+int build_compact_map(const int32_t* zero, int64_t m, int64_t* dst, int64_t* kept);
+// From the list numbers (-1 = not indexed) of n rows: order[p] = the row stored at image row p (lists ascending, call
+// order inside a list; the rows that are not indexed follow), dst[i] = image row of row i or -1, list_off [lists + 1]
+// (host).  order and dst are device arrays of n.
+int build_destinations(const int32_t* lists_of_row, int64_t n, int lists, int64_t* order, int64_t* dst, int64_t* list_off_host);
 
 // list-major batched list scan (vb_list_tile.cu): the (query, probe) pairs of a batch grouped by list, one CTA
 // per static row tile of the index against every query probing that list

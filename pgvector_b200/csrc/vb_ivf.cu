@@ -1687,6 +1687,323 @@ int vb_ivf_list_offsets(const vb_ivf* h, int64_t* out) {
     return VB_OK;
 }
 
+}  // extern "C"
+
+// ---- CREATE INDEX in one call (ivfflatbuild): samples, k-means, assign, destinations, placement (vb_ivf_build.cu)
+
+constexpr size_t IVF_BUILD_CHUNK_BYTES = (size_t)128 << 20;
+
+// The caller's rows as device memory at the packed row pitch, `chunk` rows at a time.  Device rows are handed out in
+// place.  Host rows go through two pinned and two device buffers: the copy of chunk c + 1 is issued on the copy stream
+// before the work on chunk c is enqueued on the library stream, and events hand the buffers back and forth.  `pick`
+// (host row numbers) streams those rows instead of all of them, gathered row by row into the pinned buffer.
+// The pinned buffers are the library's shared, grow-only ones: another host upload (the centres of the k-means, say)
+// may free and re-allocate them between two passes, so every pass asks for them again and no pass keeps the pointers.
+struct IvfBuildSource {
+    const uint8_t* rows;
+    const int64_t* ids;
+    int64_t n;
+    size_t raw;
+    bool host;
+    int64_t chunk;
+    void* pin[2] = {nullptr, nullptr};
+    IvfTmp dev[2];
+    cudaEvent_t copied[2] = {nullptr, nullptr}, done[2] = {nullptr, nullptr};
+    bool rows_pinned = false;
+    ~IvfBuildSource() {
+        for (int b = 0; b < 2; ++b) {
+            if (copied[b]) cudaEventDestroy(copied[b]);
+            if (done[b]) cudaEventDestroy(done[b]);
+        }
+        cudaStreamSynchronize(ctx().copy_stream);
+    }
+    size_t ids_at() const { return align256((size_t)chunk * raw + 16); }   // offset of a chunk's ids in its buffers
+    size_t buffer_bytes() const { return ids_at() + 8 * (size_t)chunk; }
+    int prepare(const char* fn) {
+        if (!host) return VB_OK;
+        for (int b = 0; b < 2; ++b) {
+            VB_TRY(ivf_alloc_tmp(fn, dev[b], buffer_bytes()));
+            VB_CUDA(cudaEventCreateWithFlags(&copied[b], cudaEventDisableTiming));
+            VB_CUDA(cudaEventCreateWithFlags(&done[b], cudaEventDisableTiming));
+        }
+        cudaPointerAttributes attr;
+        rows_pinned = cudaPointerGetAttributes(&attr, rows) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+        cudaGetLastError();   // (older drivers report an unregistered pointer as an error)
+        return VB_OK;
+    }
+    int issue(int64_t c, const int64_t* pick, int64_t total, bool with_ids) {
+        Context& cx = ctx();
+        const int b = (int)(c & 1);
+        const int64_t r0 = c * chunk, m = std::min(chunk, total - r0);
+        VB_CUDA(cudaEventSynchronize(copied[b]));   // the pinned buffer's last copy has left it
+        const uint8_t* src = rows + (size_t)r0 * raw;
+        if (pick) {
+            for (int64_t i = 0; i < m; ++i) memcpy((uint8_t*)pin[b] + (size_t)i * raw, rows + (size_t)pick[r0 + i] * raw, raw);
+            src = (const uint8_t*)pin[b];
+        } else if (!rows_pinned) {
+            memcpy(pin[b], src, (size_t)m * raw);
+            src = (const uint8_t*)pin[b];
+        }
+        VB_CUDA(cudaStreamWaitEvent(cx.copy_stream, done[b], 0));   // the device buffer's last chunk has been worked on
+        VB_CUDA(cudaMemcpyAsync(dev[b].mem, src, (size_t)m * raw, cudaMemcpyHostToDevice, cx.copy_stream));
+        if (with_ids) {
+            memcpy((uint8_t*)pin[b] + ids_at(), ids + r0, 8 * (size_t)m);
+            VB_CUDA(cudaMemcpyAsync((uint8_t*)dev[b].mem + ids_at(), (uint8_t*)pin[b] + ids_at(), 8 * (size_t)m, cudaMemcpyHostToDevice,
+                                    cx.copy_stream));
+        }
+        VB_CUDA(cudaEventRecord(copied[b], cx.copy_stream));
+        return VB_OK;
+    }
+    // work(first row, rows, device rows, device ids) for every chunk, in order
+    template <typename F>
+    int stream(const int64_t* pick, int64_t total, bool with_ids, F&& work) {
+        Context& cx = ctx();
+        const int64_t nc = (total + chunk - 1) / chunk;
+        if (!host) {
+            for (int64_t c = 0; c < nc; ++c)
+                VB_TRY(work(c * chunk, std::min(chunk, total - c * chunk), rows + (size_t)(c * chunk) * raw, ids + c * chunk));
+            return VB_OK;
+        }
+        VB_CUDA(cudaStreamSynchronize(cx.copy_stream));   // (the last pass's copies: the buffers may move below)
+        VB_TRY(pinned_buffer(buffer_bytes(), &pin[0]));
+        VB_TRY(pinned_buffer2(buffer_bytes(), &pin[1]));
+        VB_TRY(issue(0, pick, total, with_ids));
+        for (int64_t c = 0; c < nc; ++c) {
+            const int b = (int)(c & 1);
+            if (c + 1 < nc) VB_TRY(issue(c + 1, pick, total, with_ids));
+            VB_CUDA(cudaStreamWaitEvent(cx.stream, copied[b], 0));
+            VB_TRY(work(c * chunk, std::min(chunk, total - c * chunk), (const uint8_t*)dev[b].mem,
+                        (const int64_t*)((const uint8_t*)dev[b].mem + ids_at())));
+            VB_CUDA(cudaEventRecord(done[b], cx.stream));
+        }
+        return VB_OK;
+    }
+};
+
+struct TableHold {   // a table freed on every exit unless it was handed on
+    Table t;
+    ~TableHold() { table_free(t); }
+};
+
+static int ivf_build_impl(const char* fn, vb_ivf* h, const void* rows, const int64_t* ids, int64_t n, int normalize,
+                          const vb_ivf_build_opts* opts, int32_t* out_lists, int64_t* out_order, int* iters_out, bool host) {
+    VB_TRY(require_init());
+    VB_REQUIRE(h, "%s: null index", fn);
+    VB_REQUIRE(rows && ids, "%s: rows and ids must not be NULL (an image without heap ids cannot take inserts)", fn);
+    VB_REQUIRE(n >= 1 && n < (int64_t)INT32_MAX, "%s: row count %lld out of range (1 .. 2^31 - 2)", fn, (long long)n);
+    Ivf& ix = h->ix;
+    if (comm_world() > 1 || ix.loading) {
+        set_error(ix.loading ? "%s: inside vb_ivf_begin_load / vb_ivf_end_load"
+                             : "%s: a communicator is active and this image is a shard; the sharded build is not supported", fn);
+        return VB_ESTATE;
+    }
+    VB_REQUIRE(!normalize || (ix.elem != VB_BIT && ix.metric == VB_NEG_IP),
+               "%s: normalize is the rule of the cosine opclasses (vector / halfvec, negative inner product)", fn);
+    static const vb_ivf_build_opts defaults = {42, 0, nullptr, 0, 0, nullptr, 0};
+    const vb_ivf_build_opts& o = opts ? *opts : defaults;
+    Context& c = ctx();
+    const int L = ix.lists;
+    const size_t stride = ix.rows.stride, raw = raw_row_bytes(ix.elem, ix.dim);
+    const int km = ix.elem == VB_BIT ? VB_HAMMING : ix.metric == VB_L2_SQUARED ? VB_L2 : VB_SPHERICAL;
+    const bool norm_rows = normalize != 0;
+
+    // the sample rows
+    std::vector<int64_t> pick;
+    int64_t ns;
+    if (o.sample_rows) {
+        ns = o.n_samples;
+        VB_REQUIRE(ns >= 1 && ns <= n, "%s: %lld sample rows for %lld rows", fn, (long long)ns, (long long)n);
+        pick.assign(o.sample_rows, o.sample_rows + ns);
+        std::vector<int64_t> sorted(pick);
+        std::sort(sorted.begin(), sorted.end());
+        VB_REQUIRE(sorted.front() >= 0 && sorted.back() < n, "%s: sample row %lld out of range (%lld rows)", fn,
+                   (long long)(sorted.front() < 0 ? sorted.front() : sorted.back()), (long long)n);
+        const auto dup = std::adjacent_find(sorted.begin(), sorted.end());
+        VB_REQUIRE(dup == sorted.end(), "%s: sample row %lld is repeated", fn, dup == sorted.end() ? 0LL : (long long)*dup);
+    } else {
+        VB_REQUIRE(o.n_samples >= 0, "%s: negative sample count", fn);
+        ns = std::min<int64_t>(n, o.n_samples > 0 ? o.n_samples : std::max<int64_t>(50 * (int64_t)L, 10000));   // src/ivfbuild.c:448-455
+    }
+    VB_REQUIRE(ns >= L, "%s: %lld samples are fewer than %d lists", fn, (long long)ns, L);
+    VB_REQUIRE(!o.u || o.first_row >= 0, "%s: first_row must not be negative", fn);
+
+    IvfBuildSource src{(const uint8_t*)rows, ids, n, raw, host, 0};
+    const int64_t auto_chunk = std::min<int64_t>((int64_t)1 << 20, std::max<int64_t>(1024, (int64_t)(IVF_BUILD_CHUNK_BYTES / raw)));
+    src.chunk = std::min<int64_t>(n, o.chunk_rows > 0 ? o.chunk_rows : auto_chunk);
+    VB_TRY(src.prepare(fn));
+
+    // centres: samples (spherical: the usable ones, normalised), seeding, Lloyd -- through the host, as vb_kmeans hands
+    // them over (lists x dim elements)
+    std::vector<uint8_t> cent(raw * (size_t)L);
+    int iters = 0;
+    {
+        IvfTmp t_pick, t_raw, t_unit;
+        VB_TRY(ivf_alloc_tmp(fn, t_pick, 8 * (size_t)ns));
+        int64_t* d_pick = (int64_t*)t_pick.mem;
+        Table S = ix.rows;   // (element type, dimensions, stride)
+        {
+            ProfScope span(VB_PROF_BUILD_SAMPLE);
+            if (o.sample_rows) {
+                VB_CUDA(cudaMemcpyAsync(d_pick, pick.data(), 8 * (size_t)ns, cudaMemcpyHostToDevice, c.stream));
+            } else {
+                VB_TRY(build_draw_samples(n, ns, o.seed, d_pick));
+                if (host) {
+                    pick.resize((size_t)ns);
+                    VB_CUDA(cudaMemcpyAsync(pick.data(), d_pick, 8 * (size_t)ns, cudaMemcpyDeviceToHost, c.stream));
+                    VB_CUDA(cudaStreamSynchronize(c.stream));
+                }
+            }
+            VB_TRY(ivf_alloc_tmp(fn, t_raw, (size_t)ns * stride + 16));
+            S.d = (uint8_t*)t_raw.mem;
+            S.n = S.cap = ns;
+            if (host)
+                VB_TRY(src.stream(pick.data(), ns, false, [&](int64_t r0, int64_t m, const uint8_t* d_rows, const int64_t*) {
+                    return launch_place_rows(ix.elem, ix.dim, false, d_rows, raw, nullptr, nullptr, nullptr, m, S.d + (size_t)r0 * stride, stride,
+                                             nullptr, nullptr);
+                }));
+            else
+                VB_TRY(launch_place_rows(ix.elem, ix.dim, false, rows, raw, nullptr, d_pick, nullptr, ns, S.d, stride, nullptr, nullptr));
+            if (km == VB_SPHERICAL) {
+                // AddSample: a sample that cannot be normalised is dropped, the others are stored as unit vectors
+                const size_t b_rows = align256((size_t)ns * stride + 16), b_zero = align256(4 * (size_t)ns);
+                VB_TRY(ivf_alloc_tmp(fn, t_unit, b_rows + b_zero + 8 * (size_t)ns));
+                int32_t* d_zero = (int32_t*)((uint8_t*)t_unit.mem + b_rows);
+                int64_t* d_to = (int64_t*)((uint8_t*)t_unit.mem + b_rows + b_zero);
+                int64_t kept = 0;
+                VB_TRY(launch_place_rows(ix.elem, ix.dim, true, S.d, stride, nullptr, nullptr, nullptr, ns, nullptr, stride, nullptr, d_zero));
+                VB_TRY(build_compact_map(d_zero, ns, d_to, &kept));
+                VB_TRY(launch_place_rows(ix.elem, ix.dim, true, S.d, stride, nullptr, nullptr, d_to, ns, (uint8_t*)t_unit.mem, stride, nullptr,
+                                         nullptr));
+                S.d = (uint8_t*)t_unit.mem;
+                S.n = kept;
+            }
+        }
+        VB_REQUIRE(S.n >= L, "%s: %lld usable samples (norm > 0) are fewer than %d lists", fn, (long long)S.n, L);
+        VB_REQUIRE(!o.u || o.first_row < S.n, "%s: first_row %lld is not one of the %lld usable samples", fn, (long long)o.first_row,
+                   (long long)S.n);
+        {
+            ProfScope span(VB_PROF_BUILD_SEED);
+            VB_TRY(o.u ? kmeans_pp(S, km, cent.data(), L, 0, o.first_row, o.u) : kmeans_pp(S, km, cent.data(), L, o.seed));
+        }
+        {
+            ProfScope span(VB_PROF_BUILD_LLOYD);
+            VB_TRY(kmeans_run(S, km, cent.data(), L, o.max_iter, o.seed, nullptr, nullptr, &iters));
+        }
+    }
+    TableHold Cn;
+    Cn.t = ix.rows;
+    Cn.t.d = nullptr;
+    Cn.t.n = Cn.t.cap = 0;
+    VB_TRY(table_append_host(Cn.t, cent.data(), L));
+
+    // pass one: the list of every row (4 bytes per row stay); cosine: of the normalised row, -1 for a row of norm 0
+    IvfTmp t_lists, t_prep, t_dst;
+    VB_TRY(ivf_alloc_tmp(fn, t_lists, 4 * (size_t)n));
+    int32_t* d_lists = (int32_t*)t_lists.mem;
+    // A chunk is a table as it lies when its rows need no padding or normalisation and start 16-byte aligned.  Tables the
+    // library allocates carry 16 spare bytes behind the last row; the caller's device rows carry none, so of those the
+    // last row goes through the padded buffer like a chunk that needs preparing, and the row behind every row read in
+    // place is the caller's own.
+    const bool prep = norm_rows || raw != stride || (!host && ((uintptr_t)rows & 15) != 0);
+    if (!host) src.chunk = prep ? std::min(n, auto_chunk) : std::max<int64_t>(n - 1, 1);
+    const int64_t prep_rows = prep ? src.chunk : 1;
+    const size_t b_prep = align256((size_t)prep_rows * stride + 16);
+    VB_TRY(ivf_alloc_tmp(fn, t_prep, b_prep + 4 * (size_t)prep_rows));
+    uint8_t* d_prep = (uint8_t*)t_prep.mem;
+    int32_t* d_zero = norm_rows ? (int32_t*)(d_prep + b_prep) : nullptr;
+    VB_TRY(src.stream(nullptr, n, false, [&](int64_t r0, int64_t m, const uint8_t* d_rows, const int64_t*) {
+        ProfScope span(VB_PROF_BUILD_ASSIGN);
+        Table X = ix.rows;
+        X.d = const_cast<uint8_t*>(d_rows);
+        X.n = X.cap = m;
+        if (prep || (!host && r0 + m == n)) {
+            VB_TRY(launch_place_rows(ix.elem, ix.dim, norm_rows, d_rows, raw, nullptr, nullptr, nullptr, m, d_prep, stride, nullptr, d_zero));
+            X.d = d_prep;
+        }
+        VB_TRY(launch_assign(X, ix.metric, Cn.t, L, d_lists + r0));
+        return norm_rows ? build_mark_skipped(d_zero, m, d_lists + r0) : VB_OK;
+    }));
+
+    // destinations: list offsets, the image order, and the image row of every row
+    VB_TRY(ivf_alloc_tmp(fn, t_dst, 2 * align256(8 * (size_t)n)));
+    int64_t* d_order = (int64_t*)t_dst.mem;
+    int64_t* d_dst = (int64_t*)((uint8_t*)t_dst.mem + align256(8 * (size_t)n));
+    std::vector<int64_t> off((size_t)L + 1);
+    VB_TRY(build_destinations(d_lists, n, L, d_order, d_dst, off.data()));
+    const int64_t n_idx = off[(size_t)L];
+    for (int l = 0; l < L; ++l)
+        VB_REQUIRE(off[(size_t)l + 1] - off[(size_t)l] < (int64_t)INT32_MAX, "%s: list %d would hold too many rows", fn, l);
+
+    // from here on the image changes: the old rows go before the new table is allocated
+    ++ix.generation;
+    ix.loaded = false;
+    table_free(ix.rows);
+    if (ix.d_ids) cudaFree(ix.d_ids);
+    ix.d_ids = nullptr;
+    ix.has_ids = false;
+    list_tc_release(&ix.tc);
+    list_tc_release(&ix.ctc);
+    table_free(ix.centers);
+    ix.centers = Cn.t;
+    Cn.t.d = nullptr;
+    if (table_reserve(ix.rows, std::max<int64_t>(n_idx, 1)) != VB_OK) {
+        set_error("%s: allocation of %zu bytes of device memory for the row table failed", fn, (size_t)std::max<int64_t>(n_idx, 1) * stride + 16);
+        return VB_ENOMEM;
+    }
+    if (n_idx > 0 && cudaMalloc(&ix.d_ids, 8 * (size_t)n_idx) != cudaSuccess) {
+        cudaGetLastError();
+        ix.d_ids = nullptr;
+        set_error("%s: allocation of %zu bytes of device memory for the heap ids failed", fn, 8 * (size_t)n_idx);
+        return VB_ENOMEM;
+    }
+    // pass two: every row moves once -- host rows scattered chunk by chunk to their image rows, device rows gathered in
+    // image order
+    if (!host) src.chunk = n;
+    VB_TRY(src.stream(nullptr, n, true, [&](int64_t r0, int64_t m, const uint8_t* d_rows, const int64_t* d_ids) {
+        ProfScope span(VB_PROF_BUILD_PLACE);
+        return host ? launch_place_rows(ix.elem, ix.dim, norm_rows, d_rows, raw, d_ids, nullptr, d_dst + r0, m, ix.rows.d, stride,
+                                                ix.d_ids, nullptr)
+                            : launch_place_rows(ix.elem, ix.dim, norm_rows, d_rows, raw, d_ids, d_order, nullptr, n_idx, ix.rows.d, stride,
+                                                ix.d_ids, nullptr);
+    }));
+    if (out_lists) VB_CUDA(cudaMemcpyAsync(out_lists, d_lists, 4 * (size_t)n, cudaMemcpyDeviceToHost, c.stream));
+    if (out_order) VB_CUDA(cudaMemcpyAsync(out_order, d_order, 8 * (size_t)n, cudaMemcpyDeviceToHost, c.stream));
+    VB_CUDA(cudaStreamSynchronize(c.stream));
+    if (out_order) std::fill(out_order + n_idx, out_order + n, (int64_t)-1);
+    ix.rows.n = n_idx;
+    VB_TRY(ivf_set_offsets(ix, off.data()));
+    ix.has_ids = true;
+    ix.loaded = true;
+    if (iters_out) *iters_out = iters;
+    return VB_OK;
+}
+
+extern "C" {
+
+int vb_ivf_build(vb_ivf* h, const void* rows, const int64_t* ids, int64_t n, int normalize, const vb_ivf_build_opts* opts,
+                 int32_t* out_lists, int64_t* out_order, int* iters_out) {
+    return ivf_build_impl("vb_ivf_build", h, rows, ids, n, normalize, opts, out_lists, out_order, iters_out, true);
+}
+
+int vb_ivf_build_dev(vb_ivf* h, const void* rows_dev, const int64_t* ids_dev, int64_t n, int normalize, const vb_ivf_build_opts* opts,
+                     int32_t* out_lists, int64_t* out_order, int* iters_out) {
+    return ivf_build_impl("vb_ivf_build_dev", h, rows_dev, ids_dev, n, normalize, opts, out_lists, out_order, iters_out, false);
+}
+
+int vb_ivf_centers(const vb_ivf* h, void* out) {
+    VB_TRY(require_init());
+    VB_REQUIRE(h && out, "vb_ivf_centers: null argument");
+    if (!h->ix.loaded) {
+        set_error("vb_ivf_centers: index not loaded");
+        return VB_ESTATE;
+    }
+    const Ivf& ix = h->ix;
+    const size_t raw = raw_row_bytes(ix.elem, ix.dim);
+    VB_CUDA(cudaMemcpy2DAsync(out, raw, ix.centers.d, ix.centers.stride, raw, (size_t)ix.lists, cudaMemcpyDeviceToHost, ctx().stream));
+    VB_CUDA(cudaStreamSynchronize(ctx().stream));
+    return VB_OK;
+}
+
 int vb_ivf_free(vb_ivf* h) {
     if (!h) return VB_OK;
     table_free(h->ix.centers);

@@ -569,8 +569,8 @@ static int kmeans_update_centers(const Table& X, KmeansState& st, int k, bool sp
 }
 
 
-static int kmeans_run(const Table& X, int kmeans_metric, void* centers_host, int k, int max_iter, uint64_t seed,
-                      vb_allreduce_fn allreduce, void* actx, int* iters_out) {
+int kmeans_run(const Table& X, int kmeans_metric, void* centers_host, int k, int max_iter, uint64_t seed,
+               vb_allreduce_fn allreduce, void* actx, int* iters_out) {
     Context& c = ctx();
     cudaStream_t s = c.stream;
     const bool spherical = kmeans_metric == VB_SPHERICAL;
@@ -999,8 +999,8 @@ static double host_uniform(uint64_t* st) {
 
 // first_row / u: the draws of InitCenters (src/ivfkmeans.c:36, 78) when the caller supplies them (parity tests feed the
 // oracle the same ones); otherwise they come from the seed.  picked_out (optional, host): the chosen sample rows.
-static int kmeans_pp(const Table& X, int kmeans_metric, void* centers_host, int k, uint64_t seed, int64_t first_row = -1,
-                     const double* u_in = nullptr, int64_t* picked_out = nullptr) {
+int kmeans_pp(const Table& X, int kmeans_metric, void* centers_host, int k, uint64_t seed, int64_t first_row, const double* u_in,
+              int64_t* picked_out) {
     Context& c = ctx();
     cudaStream_t s = c.stream;
     const int64_t n = X.n;
