@@ -192,7 +192,8 @@ int			vb_table_rerank_dev(vb_table *t, int metric, const void *queries_dev, int6
 /*
  * A row filter: the allowed rows of one table or one IVFFlat image, resident on the device -- what a B-tree or bitmap
  * scan on a filter column yields for "WHERE <predicate> ORDER BY v <op> q LIMIT k" (README "Filtering").  Queries that
- * take a filter never read, score, select or copy a row it does not allow.
+ * take a filter never read, score, select or copy a row it does not allow.  Sparse tables take filters of their own
+ * (vb_sparse_table_filter_create, with the sparsevec calls below).
  *
  * Table filters: rows = row numbers of t (append order).  Host variant: a value outside [0, n) fails with VB_EINVAL
  * naming its position and value; _dev variant: such values are ignored.  Rows appended to t later are not in the
@@ -317,6 +318,41 @@ int			vb_sparse_table_free(vb_sparse_table *t);
  */
 int			vb_sparse_exact_topk(vb_sparse_table *t, int metric, int q_dim, int64_t nq, const int64_t *q_off, const int32_t *q_idx,
 								 const float *q_val, int k, int64_t *out_ids, double *out_dist);
+
+/*
+ * Row filters of a sparse table (see vb_filter above): rows = row numbers of t (append order).  A value outside [0, n)
+ * fails with VB_EINVAL naming its position and value.  Duplicates collapse, n == 0 is an empty filter; rows appended
+ * later are not in the filter, and it stays valid.  vb_filter_rows and vb_filter_free apply.  A sparse filter is refused
+ * (VB_EINVAL, "made for another table or index") by any other sparse table, by its own after that was freed, and by
+ * every dense, IVFFlat and HNSW call; the sparse calls refuse their filters.
+ */
+int			vb_sparse_table_filter_create(vb_sparse_table *t, const int64_t *rows, int64_t n, vb_filter **out);
+/*
+ * Filtered exact top-k: for each query q, the k nearest of the rows filters[filter_of_query[q]] allows -- the plan of
+ * "WHERE <predicate> ORDER BY v <op> q LIMIT k" with a B-tree or bitmap scan on the filter column.  filter_of_query is a
+ * host array [nq], NULL when nfilters == 1; an entry out of range fails with VB_EINVAL naming the query.  Metrics, k and
+ * q_dim as vb_sparse_exact_topk (its texts).  Each query's result is bit-identical, ids and distances, to
+ * vb_sparse_table_rerank with cand = its filter's allowed rows in ascending order: ties to the smaller row number, -1 /
+ * +inf padding when fewer than k rows are allowed.  A filter of every row therefore gives vb_sparse_exact_topk's output.
+ * Rows the filter rejects are never read, scored, selected or copied.
+ *
+ * Re-rank: for each query, the k nearest of ITS candidate rows -- the outer "ORDER BY v <op> q LIMIT k" over another
+ * index's result (hybrid search: a dense or quantized index fetches the candidates, the sparse column orders them).
+ * cand[q*c + j] = a row number of t; -1 = no candidate.  A value outside [-1, n) fails with VB_EINVAL naming the query,
+ * the position and the value.  A row listed twice is scored twice; ties go to the earlier candidate position, and a NaN
+ * distance (cosine against a zero-norm row) ranks before the padding.  Every distance is bit-identical to the one
+ * vb_sparse_exact_topk reports for that row.  c >= 0.
+ *
+ * Both: everything is validated before any kernel runs, and on any error nothing is written to out_ids / out_dist.
+ * Queries run in sub-batches of at most 65535 whose distance runs stay under 1 GiB; VB_ENOMEM names the bytes that could
+ * not be allocated.  The filters may be freed once the call returns.
+ */
+int			vb_sparse_exact_topk_filtered(vb_sparse_table *t, int metric, int q_dim, int64_t nq, const int64_t *q_off,
+										  const int32_t *q_idx, const float *q_val, int k, const vb_filter *const *filters,
+										  int nfilters, const int32_t *filter_of_query, int64_t *out_ids, double *out_dist);
+int			vb_sparse_table_rerank(vb_sparse_table *t, int metric, int q_dim, int64_t nq, const int64_t *q_off,
+								   const int32_t *q_idx, const float *q_val, const int64_t *cand, int c, int k, int64_t *out_ids,
+								   double *out_dist);
 
 /* ---------------------------------------------------------------- IVFFlat */
 

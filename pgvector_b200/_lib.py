@@ -44,6 +44,9 @@ SIGNATURES = {
     "vb_sparse_table_nnz": (_i64, [_vp]),
     "vb_sparse_table_free": (_i, [_vp]),
     "vb_sparse_exact_topk": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _i, _vp, _vp]),
+    "vb_sparse_table_filter_create": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
+    "vb_sparse_exact_topk_filtered": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
+    "vb_sparse_table_rerank": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),
     "vb_table_create": (_i, [_i, _i, C.POINTER(_vp)]),
     "vb_table_append": (_i, [_vp, _vp, _i64]),
     "vb_table_append_dev": (_i, [_vp, _vp, _i64]),

@@ -312,12 +312,12 @@ int launch_ivf_filter_lists(int64_t nq, int max_probes, int lists, const int32_t
 // The allowed rows of one table or one IVFFlat image, ascending.  An IVFFlat image stores rows grouped by list, so the
 // allowed rows of list l are one run pos[off[l] .. off[l + 1]).  The allowed elements of an HNSW image are a bitset:
 // its iterative scan tests the elements a traversal returns, it never enumerates the allowed ones.
-// process-wide unique stamp of a table, IVFFlat or HNSW image: a filter matches its owner by address and stamp, so a
-// filter that outlived its owner is refused even when a new owner is allocated at the same address
+// process-wide unique stamp of a table, sparse table, IVFFlat or HNSW image: a filter matches its owner by address and
+// stamp, so a filter that outlived its owner is refused even when a new owner is allocated at the same address
 uint64_t next_owner_uid();
-enum FilterKind { FILTER_TABLE, FILTER_IVF, FILTER_HNSW };
+enum FilterKind { FILTER_TABLE, FILTER_IVF, FILTER_HNSW, FILTER_SPARSE };
 struct Filter {
-    const void* owner = nullptr;   // the vb_table, vb_ivf or vb_hnsw it was made for
+    const void* owner = nullptr;   // the vb_table, vb_sparse_table, vb_ivf or vb_hnsw it was made for
     uint64_t owner_uid = 0;        // and that owner's stamp
     FilterKind kind = FILTER_TABLE;
     uint64_t generation = 0;       // IVFFlat / HNSW: the image's generation at creation
@@ -333,6 +333,11 @@ struct Filter {
 };
 // table: rows = row numbers (values outside [0, n_rows) ignored; the host variant validates before this call)
 int filter_build_table(int64_t n_rows, const int64_t* rows, int64_t n, bool host, Filter* f);
+// A filter of row numbers of a table of n_rows rows (owner, its stamp, kind FILTER_TABLE or FILTER_SPARSE): the body of
+// vb_table_filter_create[_dev] and vb_sparse_table_filter_create.  fn names the entry point in the messages; owner ==
+// nullptr fails ("null table").  The host variant validates every row first.
+int table_filter_create(const char* fn, const void* owner, uint64_t owner_uid, int64_t n_rows, FilterKind kind, const int64_t* rows,
+                        int64_t n, bool host, vb_filter** out);
 // IVFFlat image of n_rows rows: image_ids = heap ids of the rows (nullptr: row positions), list_off [lists + 1] device
 int filter_build_ivf(int64_t n_rows, const int64_t* image_ids, const int64_t* list_off, int lists, const int64_t* ids, int64_t n,
                      bool host, Filter* f);
@@ -345,6 +350,39 @@ void filter_release(Filter* f);
 // selected ahead of an allowed one; the bits tell it apart from an allowed row's NaN distance (the GPU computes NaN as
 // 0x7FFFFFFF, and the mask rewrites an allowed NaN that carries these bits to that).
 constexpr uint32_t FILTER_REJECTED = 0xFFFFFFFFu;
+
+// The work lists of a filtered exact top-k (vb_exact_topk_filtered, vb_sparse_exact_topk_filtered).  Per sub-batch of
+// queries: per-query arguments, the chunks of each query's allowed rows (Chunk::row_begin indexes the call's concatenated
+// position arrays, one copy per filter; Chunk::out_off its distance run), and the scan launches over them.
+struct FilterQuery {
+    int64_t run;     // first distance of the query's run (segment begin)
+    int64_t base;    // first position of its filter in the concatenated position array
+    int64_t cbase;   // its first chunk: the chunks of the queries that share a filter are one block, filters in order
+    int32_t len;     // rows its filter allows
+    int32_t pad;
+};
+struct FilterBatch {
+    std::vector<FilterQuery> qa;          // queries q0 .. q0 + qa.size() of the call
+    std::vector<int64_t> launch_begin;    // scan launch l covers chunks [launch_begin[l], launch_begin[l] + launch_count[l])
+    std::vector<int32_t> launch_count;
+    int64_t run = 0;                      // distances of the sub-batch
+    int64_t max_chunks = 0;
+};
+// The positions of the filters side by side: fbase [nfilters + 1] (host), *rows = the device array (a single filter is
+// read in place, several are copied into workspace slot ws_slot)
+int filter_concat_positions(const vb_filter* const* filters, int nfilters, int ws_slot, std::vector<int64_t>* fbase, const int64_t** rows);
+// The next sub-batch from query q0 on: as many queries as keep its distances under ~1 GiB (at least one), at most max_q.
+// A filter's queries get one block of chunks; each block gets a scan launch of its own once it fills grid_chunks chunks
+// (the whole grid then reads one filter's rows, which stay in L2 for its other queries), smaller blocks share one.
+int filter_batch_plan(const vb_filter* const* filters, int nfilters, const int32_t* filter_of_query, const int64_t* fbase, int64_t q0,
+                      int64_t nq, int64_t max_q, int rows_per_chunk, int64_t grid_chunks, FilterBatch* b);
+// filter_chunks_kernel: seg_begin / seg_len / chunks of the sub-batch's nq queries (qa_dev = FilterBatch::qa on the device)
+int launch_filter_chunks(const FilterQuery* qa_dev, int64_t nq, int rows_per_chunk, int64_t* seg_begin, int32_t* seg_len, Chunk* chunks);
+// rerank_prepare_kernel (vb_rerank.cu): ids[q c + j], j < seg_len[q] = the candidates of query q in [0, n), in candidate
+// order; seg_begin[q] = q c; the chunks of each query's run (row_begin = out_off into ids / distances) appended at
+// *n_chunks (device, zeroed by the caller)
+int launch_rerank_prepare(const int64_t* cand, int64_t nq, int c, int64_t n, int rows_per_chunk, int64_t* ids, int64_t* seg_begin,
+                          int32_t* seg_len, Chunk* chunks, int* n_chunks);
 
 int list_tile_rows();
 bool list_major_supported(int elem, int key_metric);

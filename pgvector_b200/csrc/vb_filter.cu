@@ -6,7 +6,8 @@
 // Construction, all on the device (the host never sees image positions):
 //   IVFFlat: CUB radix sort of the given heap ids; filter_ivf_bits_kernel, one thread per image row, binary-searches
 //            its id and a warp ballot writes each 32-row word of a bitset (no atomics);
-//   table:   filter_table_bits_kernel sets the bits of the given row numbers;
+//   table:   filter_table_bits_kernel sets the bits of the given row numbers (a sparse table's filters too, of their
+//            own kind: vb_sparse_table_filter_create);
 //   then filter_count_kernel / filter_scan_kernel / filter_write_kernel compact the bitset into ascending positions
 //   (per-block popcounts, one scan of the block sums, per-thread offsets), and filter_list_off_kernel, one thread per
 //   list, binary-searches the image's list offsets in the positions to give each list's run.
@@ -20,6 +21,8 @@
 //   3. segment_topk_kernel over each query's run: ties by position = by row number (positions are ascending);
 //   4. filter_finish_kernel: position -> row number, the operator's epilogue.
 // Roofline: HBM gathers of the allowed rows, bytes = sum over queries of allowed rows x row stride.
+// The sparse filtered top-k (vb_sparse.cu) takes the same sub-batch plan, chunks and selection, with
+// sparse_gather_kernel as step 2.
 #include "vb_common.cuh"
 #include "vb_distance.cuh"
 
@@ -307,15 +310,6 @@ int filter_build_hnsw(int64_t n_elems, const int64_t* elems, int64_t n, bool hos
 
 // ---------------------------------------------------------------------------------------------- filtered exact top-k
 
-// per-query arguments of a sub-batch, uploaded once: the query's distance run and its filter's run of positions
-struct FilterQuery {
-    int64_t run;     // first distance of the query's run (segment begin)
-    int64_t base;    // first position of its filter in the concatenated position array
-    int64_t cbase;   // its first chunk: the chunks of the queries that share a filter are one block, filters in order
-    int32_t len;     // rows its filter allows
-    int32_t pad;
-};
-
 // One warp per query: the chunks of its allowed rows and its segment.
 __global__ void __launch_bounds__(256) filter_chunks_kernel(const FilterQuery* __restrict__ qa, int64_t nq, int rows_per_chunk,
                                                             int64_t* __restrict__ seg_begin, int32_t* __restrict__ seg_len,
@@ -337,6 +331,67 @@ __global__ void __launch_bounds__(256) filter_chunks_kernel(const FilterQuery* _
         ch.q = (int32_t)q;
         chunks[a.cbase + i] = ch;
     }
+}
+
+int launch_filter_chunks(const FilterQuery* qa_dev, int64_t nq, int rows_per_chunk, int64_t* seg_begin, int32_t* seg_len, Chunk* chunks) {
+    Context& cx = ctx();
+    filter_chunks_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, cx.stream>>>(qa_dev, nq, rows_per_chunk, seg_begin, seg_len, chunks);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
+}
+
+int filter_concat_positions(const vb_filter* const* filters, int nfilters, int ws_slot, std::vector<int64_t>* fbase, const int64_t** rows) {
+    Context& cx = ctx();
+    fbase->assign((size_t)nfilters + 1, 0);
+    for (int i = 0; i < nfilters; ++i) (*fbase)[(size_t)i + 1] = (*fbase)[(size_t)i] + filters[i]->f.n;
+    *rows = filters[0]->f.pos;
+    if (nfilters > 1) {
+        void* d_cat;
+        VB_TRY(workspace(ws_slot, 8 * (size_t)std::max<int64_t>(fbase->back(), 1), &d_cat));
+        for (int i = 0; i < nfilters; ++i)
+            if (filters[i]->f.n)
+                VB_CUDA(cudaMemcpyAsync((int64_t*)d_cat + (*fbase)[(size_t)i], filters[i]->f.pos, 8 * (size_t)filters[i]->f.n,
+                                        cudaMemcpyDeviceToDevice, cx.stream));
+        *rows = (const int64_t*)d_cat;
+    }
+    return VB_OK;
+}
+
+int filter_batch_plan(const vb_filter* const* filters, int nfilters, const int32_t* filter_of_query, const int64_t* fbase, int64_t q0,
+                      int64_t nq, int64_t max_q, int rpc, int64_t grid_chunks, FilterBatch* b) {
+    const int64_t dist_cap = (int64_t)(1ull << 28);   // distances per sub-batch: ~1 GiB
+    std::vector<int32_t> group((size_t)nfilters, 0);
+    std::vector<int64_t> cbase((size_t)nfilters);
+    b->qa.clear();
+    b->run = 0;
+    b->max_chunks = 0;
+    for (int64_t q = q0; q < nq && q - q0 < max_q; ++q) {
+        const int fi = filter_of_query ? filter_of_query[q] : 0;
+        const int64_t len = filters[fi]->f.n;
+        if (!b->qa.empty() && b->run + len > dist_cap) break;
+        b->qa.push_back(FilterQuery{b->run, fbase[fi], (int64_t)group[(size_t)fi]++, (int32_t)len, 0});
+        b->run += len;
+        b->max_chunks += (len + rpc - 1) / rpc;
+    }
+    // each filter's queries get one block of chunks, in filter order, query after query (cbase held the rank)
+    int64_t cb = 0;
+    b->launch_begin.assign(1, 0);
+    b->launch_count.clear();
+    for (int i = 0; i < nfilters; ++i) {
+        cbase[(size_t)i] = cb;
+        cb += (int64_t)group[(size_t)i] * ((filters[i]->f.n + rpc - 1) / rpc);
+        if (cb - b->launch_begin.back() >= grid_chunks || (i == nfilters - 1 && cb > b->launch_begin.back())) {
+            b->launch_count.push_back((int32_t)(cb - b->launch_begin.back()));
+            b->launch_begin.push_back(cb);
+        }
+    }
+    for (size_t j = 0; j < b->qa.size(); ++j) {
+        const int fi = filter_of_query ? filter_of_query[q0 + (int64_t)j] : 0;
+        b->qa[j].cbase = cbase[(size_t)fi] + b->qa[j].cbase * ((b->qa[j].len + rpc - 1) / rpc);
+    }
+    VB_REQUIRE(b->max_chunks < (int64_t)INT32_MAX, "filtered top-k: too many scan chunks (%lld)", (long long)b->max_chunks);
+    return VB_OK;
 }
 
 __global__ void filter_finish_kernel(int metric, int64_t total, int k, const FilterQuery* __restrict__ qa, const int32_t* __restrict__ pos,
@@ -373,62 +428,23 @@ static int exact_topk_filtered_impl(vb_table* t, int metric, const void* queries
     Context& cx = ctx();
     Table& T = t->t;
     // the filters' positions side by side (one device copy per filter; a single filter is read in place)
-    std::vector<int64_t> fbase((size_t)nfilters + 1, 0);
-    for (int i = 0; i < nfilters; ++i) fbase[(size_t)i + 1] = fbase[(size_t)i] + filters[i]->f.n;
-    const int64_t* rows = filters[0]->f.pos;
-    if (nfilters > 1) {
-        void* d_cat;
-        VB_TRY(workspace(WSF_POSCAT, 8 * (size_t)std::max<int64_t>(fbase.back(), 1), &d_cat));
-        for (int i = 0; i < nfilters; ++i)
-            if (filters[i]->f.n)
-                VB_CUDA(cudaMemcpyAsync((int64_t*)d_cat + fbase[(size_t)i], filters[i]->f.pos, 8 * (size_t)filters[i]->f.n,
-                                        cudaMemcpyDeviceToDevice, cx.stream));
-        rows = (const int64_t*)d_cat;
-    }
+    std::vector<int64_t> fbase;
+    const int64_t* rows;
+    VB_TRY(filter_concat_positions(filters, nfilters, WSF_POSCAT, &fbase, &rows));
     const size_t rawq = raw_row_bytes(T.elem, T.dim);
     const int rpc = scan_chunk_rows(T);
     const int km = key_metric(metric);
-    const int64_t dist_cap = (int64_t)(1ull << 28);   // distances per sub-batch: ~1 GiB
     // A scan launch spreads its chunk list over the whole grid in contiguous slices.  Queries that share a filter read
     // the same rows, so each filter's block of chunks gets a launch of its own once it fills the grid: every CTA then
     // reads that filter's rows, which stay in L2 for the other queries.  Smaller blocks share a launch.
     const int64_t grid_chunks = 8 * (int64_t)cx.sm_count;
-    std::vector<FilterQuery> qa;
-    std::vector<int32_t> group((size_t)nfilters);
-    std::vector<int64_t> cbase((size_t)nfilters);
-    std::vector<int64_t> launch_begin;
-    std::vector<int32_t> launch_count;
+    FilterBatch b;
     for (int64_t q0 = 0; q0 < nq;) {
-        // the next sub-batch: as many queries as keep the distance array under ~1 GiB (at least one)
-        qa.clear();
-        int64_t run = 0, max_chunks = 0;
-        std::fill(group.begin(), group.end(), 0);
-        for (int64_t q = q0; q < nq; ++q) {
-            const int fi = filter_of_query ? filter_of_query[q] : 0;
-            const int64_t len = filters[fi]->f.n;
-            if (!qa.empty() && run + len > dist_cap) break;
-            qa.push_back(FilterQuery{run, fbase[(size_t)fi], (int64_t)group[(size_t)fi]++, (int32_t)len, 0});
-            run += len;
-            max_chunks += (len + rpc - 1) / rpc;
-        }
-        const int64_t m = (int64_t)qa.size();
-        // each filter's queries get one block of chunks, in filter order, query after query (cbase held the rank)
-        int64_t cb = 0;
-        launch_begin.assign(1, 0);
-        launch_count.clear();
-        for (int i = 0; i < nfilters; ++i) {
-            cbase[(size_t)i] = cb;
-            cb += (int64_t)group[(size_t)i] * ((filters[i]->f.n + rpc - 1) / rpc);
-            if (cb - launch_begin.back() >= grid_chunks || (i == nfilters - 1 && cb > launch_begin.back())) {
-                launch_count.push_back((int32_t)(cb - launch_begin.back()));
-                launch_begin.push_back(cb);
-            }
-        }
-        for (int64_t j = 0; j < m; ++j) {
-            const int fi = filter_of_query ? filter_of_query[q0 + j] : 0;
-            qa[(size_t)j].cbase = cbase[(size_t)fi] + qa[(size_t)j].cbase * ((qa[(size_t)j].len + rpc - 1) / rpc);
-        }
-        VB_REQUIRE(max_chunks < (int64_t)INT32_MAX, "filtered top-k: too many scan chunks (%lld)", (long long)max_chunks);
+        VB_TRY(filter_batch_plan(filters, nfilters, filter_of_query, fbase.data(), q0, nq, INT64_MAX, rpc, grid_chunks, &b));
+        const std::vector<FilterQuery>& qa = b.qa;
+        const std::vector<int64_t>& launch_begin = b.launch_begin;
+        const std::vector<int32_t>& launch_count = b.launch_count;
+        const int64_t m = (int64_t)qa.size(), run = b.run, max_chunks = b.max_chunks;
         void *qimg, *d_qa, *d_chunks, *d_dist, *d_pos;
         size_t qstride;
         VB_TRY(upload_queries(T.elem, T.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, host, WSF_QIMG, &qimg, &qstride));
@@ -441,10 +457,7 @@ static int exact_topk_filtered_impl(vb_table* t, int metric, const void* queries
         VB_CUDA(cudaMemcpyAsync(d_qa, qa.data(), sizeof(FilterQuery) * (size_t)m, cudaMemcpyHostToDevice, cx.stream));
         if (nl) VB_CUDA(cudaMemcpyAsync(d_count, launch_count.data(), sizeof(int32_t) * nl, cudaMemcpyHostToDevice, cx.stream));
         VB_TRY(workspace(WSF_CHUNKS, sizeof(Chunk) * (size_t)max_chunks + 64, &d_chunks));
-        filter_chunks_kernel<<<(unsigned)((m * 32 + 255) / 256), 256, 0, cx.stream>>>((const FilterQuery*)d_qa, m, rpc, seg_begin, seg_len,
-                                                                                     (Chunk*)d_chunks);
-        VB_CUDA(cudaGetLastError());
-        count_launch();
+        VB_TRY(launch_filter_chunks((const FilterQuery*)d_qa, m, rpc, seg_begin, seg_len, (Chunk*)d_chunks));
         VB_TRY(workspace(WSF_DIST, sizeof(float) * (size_t)std::max<int64_t>(run, 1), &d_dist));
         for (size_t l = 0; l < nl; ++l)
             VB_TRY(launch_scan_gather(T, km, qimg, qstride, rows, (const Chunk*)d_chunks + launch_begin[l], d_count + l, launch_count[l],
@@ -479,26 +492,27 @@ static int exact_topk_filtered_impl(vb_table* t, int metric, const void* queries
     return VB_OK;
 }
 
-static int table_filter_create(vb_table* t, const int64_t* rows, int64_t n, bool host, vb_filter** out) {
+int table_filter_create(const char* fn, const void* owner, uint64_t owner_uid, int64_t n_rows, FilterKind kind, const int64_t* rows,
+                        int64_t n, bool host, vb_filter** out) {
     VB_TRY(require_init());
-    VB_REQUIRE(out, "vb_table_filter_create: null filter pointer");
+    VB_REQUIRE(out, "%s: null filter pointer", fn);
     *out = nullptr;
-    VB_REQUIRE(t, "vb_table_filter_create: null table");
-    VB_REQUIRE(n >= 0 && (rows || n == 0), "vb_table_filter_create: null rows or negative count %lld", (long long)n);
-    const int64_t n_rows = t->t.n;
+    VB_REQUIRE(owner, "%s: null table", fn);
+    VB_REQUIRE(n >= 0 && (rows || n == 0), "%s: null rows or negative count %lld", fn, (long long)n);
     if (host)
         for (int64_t i = 0; i < n; ++i)
-            VB_REQUIRE(rows[i] >= 0 && rows[i] < n_rows, "vb_table_filter_create: rows[%lld] = %lld is not a row of the table (0..%lld)",
-                       (long long)i, (long long)rows[i], (long long)n_rows - 1);
+            VB_REQUIRE(rows[i] >= 0 && rows[i] < n_rows, "%s: rows[%lld] = %lld is not a row of the table (0..%lld)", fn, (long long)i,
+                       (long long)rows[i], (long long)n_rows - 1);
     vb_filter* h = new vb_filter;
-    h->f.owner = t;
-    h->f.owner_uid = t->uid;
+    h->f.owner = owner;
+    h->f.owner_uid = owner_uid;
     const int rc = filter_build_table(n_rows, rows, n, host, &h->f);
     if (rc != VB_OK) {
         filter_release(&h->f);
         delete h;
         return rc;
     }
+    h->f.kind = kind;
     *out = h;
     return VB_OK;
 }
@@ -510,11 +524,11 @@ using namespace vb;
 extern "C" {
 
 int vb_table_filter_create(vb_table* t, const int64_t* rows, int64_t n, vb_filter** out) {
-    return table_filter_create(t, rows, n, true, out);
+    return table_filter_create("vb_table_filter_create", t, t ? t->uid : 0, t ? t->t.n : 0, FILTER_TABLE, rows, n, true, out);
 }
 
 int vb_table_filter_create_dev(vb_table* t, const int64_t* rows_dev, int64_t n, vb_filter** out) {
-    return table_filter_create(t, rows_dev, n, false, out);
+    return table_filter_create("vb_table_filter_create", t, t ? t->uid : 0, t ? t->t.n : 0, FILTER_TABLE, rows_dev, n, false, out);
 }
 
 int64_t vb_filter_rows(const vb_filter* f) { return f ? f->f.n : 0; }

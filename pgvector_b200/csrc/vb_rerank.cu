@@ -61,6 +61,16 @@ __global__ void __launch_bounds__(256) rerank_prepare_kernel(const int64_t* __re
     }
 }
 
+int launch_rerank_prepare(const int64_t* cand, int64_t nq, int c, int64_t n, int rows_per_chunk, int64_t* ids, int64_t* seg_begin,
+                          int32_t* seg_len, Chunk* chunks, int* n_chunks) {
+    Context& cx = ctx();
+    rerank_prepare_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, cx.stream>>>(cand, nq, c, n, rows_per_chunk, ids, seg_begin, seg_len,
+                                                                                   chunks, n_chunks);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
+}
+
 __global__ void rerank_finish_kernel(int metric, int64_t total, int k, int c, const int32_t* __restrict__ pos,
                                      const float* __restrict__ key, const int64_t* __restrict__ ids, int64_t* __restrict__ out_ids,
                                      float* __restrict__ out_f, double* __restrict__ out_d) {
@@ -116,10 +126,7 @@ static int rerank_impl(vb_table* t, int metric, const void* queries, int64_t nq,
         int64_t* seg_begin = (int64_t*)d_seg;
         int32_t* seg_len = (int32_t*)(seg_begin + m);
         VB_CUDA(cudaMemsetAsync(n_chunks, 0, sizeof(int), cx.stream));
-        rerank_prepare_kernel<<<(unsigned)((m * 32 + 255) / 256), 256, 0, cx.stream>>>((const int64_t*)d_cand, m, c, n, rpc, (int64_t*)d_ids,
-                                                                                      seg_begin, seg_len, (Chunk*)d_chunks, n_chunks);
-        VB_CUDA(cudaGetLastError());
-        count_launch();
+        VB_TRY(launch_rerank_prepare((const int64_t*)d_cand, m, c, n, rpc, (int64_t*)d_ids, seg_begin, seg_len, (Chunk*)d_chunks, n_chunks));
         VB_TRY(workspace(WSR_DIST, sizeof(float) * mc, &d_dist));
         VB_TRY(launch_scan_gather(T, km, qimg, qstride, (const int64_t*)d_ids, (const Chunk*)d_chunks, n_chunks, (int)max_chunks,
                                   (float*)d_dist));

@@ -1,7 +1,7 @@
 // vb_sparse.cu -- sparsevec on the device (SURVEY 8 f4): the distance functions of src/sparsevec.c:826-1057
 // (l2_distance / l2_squared_distance / inner_product / negative_inner_product / cosine_distance / l1_distance),
 // l2_norm / l2_normalize (src/sparsevec.c:1062-1150), a resident CSR row table and the exact (no index) top-k
-// over it.
+// over it, filtered (row filters of vb_filter.cu) or over per-query candidate rows (re-rank).
 //
 // A sparsevec is (dim, nnz, indices[nnz] ascending 0-based, values[nnz]) -- src/sparsevec.h:21-32; a batch of rows is
 // CSR: row r = entries row_off[r] .. row_off[r+1] of idx[] / val[].
@@ -60,23 +60,35 @@ __device__ __forceinline__ int sp_find(const int32_t* s_idx, const int32_t* s_bu
     return -1;
 }
 
-// KEY: VB_L2_SQUARED, VB_NEG_IP, VB_COSINE or VB_L1.  out_d (float8 of SQL function `metric`) or out_f (ordering key).
-// grid: x = row slices, y = queries.  out[(q * n + r)].
-template <int KEY>
-__global__ void __launch_bounds__(SP_WARPS * 32)
-sparse_scan_kernel(SparseQueries Q, int shift, const int64_t* __restrict__ row_off, const int32_t* __restrict__ idx,
-                   const float* __restrict__ val, int64_t n, int metric, double* __restrict__ out_d, float* __restrict__ out_f) {
-    constexpr bool FLAGS = KEY == VB_L2_SQUARED || KEY == VB_L1;
-    extern __shared__ __align__(16) uint8_t smem[];
-    const int q = blockIdx.y;
-    const int64_t qb = Q.off[q];
-    const int qn = (int)(Q.off[q + 1] - qb);
-    const int nwords = (qn + 31) >> 5;
+// A query staged in shared memory (sp_stage): its indices and values, the bucket directory and the matched-position
+// bitmaps of the warps (L2 squared and L1 only).
+struct SpStaged {
+    const int32_t* idx;
+    const float* val;
+    const int32_t* bucket;
+    uint32_t* flags;   // warp w's bitmap: flags + w * nwords
+    int qn, nwords;
+};
+
+// where a query of qn entries is staged in the dynamic shared memory
+__device__ __forceinline__ SpStaged sp_layout(uint8_t* smem, int qn) {
     int32_t* s_idx = reinterpret_cast<int32_t*>(smem);
     float* s_val = reinterpret_cast<float*>(s_idx + qn);
     int32_t* s_bucket = reinterpret_cast<int32_t*>(s_val + qn);
     uint32_t* s_flags = reinterpret_cast<uint32_t*>(s_bucket + SP_BUCKETS + 1);
-    __shared__ float s_qnorm;
+    return SpStaged{s_idx, s_val, s_bucket, s_flags, qn, (qn + 31) >> 5};
+}
+
+// Every thread of the CTA stages query q; the staging ends with a barrier.  *s_qnorm (cosine): the query's fp32 sum of
+// squares.  The caller must make sure no warp still reads a previous query's staging.
+template <int KEY>
+__device__ __forceinline__ SpStaged sp_stage(const SparseQueries& Q, int q, int shift, uint8_t* smem, float* s_qnorm) {
+    const int64_t qb = Q.off[q];
+    const int qn = (int)(Q.off[q + 1] - qb);
+    const SpStaged sq = sp_layout(smem, qn);
+    int32_t* s_idx = const_cast<int32_t*>(sq.idx);
+    float* s_val = const_cast<float*>(sq.val);
+    int32_t* s_bucket = const_cast<int32_t*>(sq.bucket);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     for (int i = threadIdx.x; i < qn; i += blockDim.x) {
@@ -100,72 +112,138 @@ sparse_scan_kernel(SparseQueries Q, int shift, const int64_t* __restrict__ row_o
         for (int i = lane; i < qn; i += 32) s += s_val[i] * s_val[i];
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (lane == 0) s_qnorm = s;
+        if (lane == 0) *s_qnorm = s;
     }
     __syncthreads();
+    return sq;
+}
 
-    uint32_t* flags = s_flags + (size_t)warp * nwords;
+// The per-row arithmetic of every sparse scan: one warp scores the row of entries beg .. end against the staged query.
+// Lanes stride the row's entries; the query entries the row does not match are summed from the warp's bitmap `flags`
+// (L2 squared, L1); then an xor-shuffle reduce.  Returns, on every lane, the float8 of KEY's function -- `metric` tells
+// VB_IP from VB_NEG_IP, sqrt_l2 takes the square root for VB_L2 -- whose float is the ordering key.  Every scan calls
+// this one body, so their distances agree bit for bit.
+template <int KEY>
+__device__ __forceinline__ double sp_score_row(int64_t beg, int64_t end, const int32_t* __restrict__ idx, const float* __restrict__ val,
+                                               const SpStaged& sq, int shift, uint32_t* flags, float qnorm, int metric, bool sqrt_l2,
+                                               int lane) {
+    constexpr bool FLAGS = KEY == VB_L2_SQUARED || KEY == VB_L1;
+    const int32_t* s_idx = sq.idx;
+    const float* s_val = sq.val;
+    const int32_t* s_bucket = sq.bucket;
+    const int qn = sq.qn, nwords = sq.nwords;
+    if (FLAGS) {
+        for (int w = lane; w < nwords; w += 32) flags[w] = 0u;
+        __syncwarp();
+    }
+    float acc = 0.f, rn = 0.f;
+    for (int64_t p = beg + lane; p < end; p += 32) {
+        const int32_t ri = __ldg(idx + p);
+        const float rv = __ldg(val + p);
+        const int pos = sp_find(s_idx, s_bucket, shift, ri);
+        const float qv = pos >= 0 ? s_val[pos] : 0.f;
+        if (KEY == VB_L2_SQUARED) {
+            const float t = rv - qv;
+            acc += t * t;
+        } else if (KEY == VB_L1) {
+            acc += fabsf(rv - qv);
+        } else {
+            acc += rv * qv;
+            if (KEY == VB_COSINE) rn += rv * rv;
+        }
+        if (FLAGS && pos >= 0) atomicOr(&flags[pos >> 5], 1u << (pos & 31));
+    }
+    if (FLAGS) {
+        __syncwarp();
+        for (int w = lane; w < nwords; w += 32) {
+            uint32_t m = ~flags[w];
+            if (w == nwords - 1 && (qn & 31)) m &= (1u << (qn & 31)) - 1u;
+            while (m) {
+                const int b = __ffs(m) - 1;
+                m &= m - 1;
+                const float qv = s_val[w * 32 + b];
+                acc += KEY == VB_L2_SQUARED ? qv * qv : fabsf(qv);
+            }
+        }
+        __syncwarp();
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        if (KEY == VB_COSINE) rn += __shfl_xor_sync(0xffffffffu, rn, o);
+    }
+    double v;
+    if (KEY == VB_COSINE) {
+        // src/sparsevec.c:985-1009: similarity / sqrt((double) norma * (double) normb), clamped, 1 - similarity
+        double sim = (double)acc / sqrt((double)rn * (double)qnorm);
+        if (sim > 1.0) sim = 1.0;
+        else if (sim < -1.0) sim = -1.0;
+        v = 1.0 - sim;
+    } else if (KEY == VB_NEG_IP) {
+        v = metric == VB_IP ? (double)acc : (double)-acc;
+    } else if (KEY == VB_L2_SQUARED) {
+        v = sqrt_l2 ? sqrt((double)acc) : (double)acc;
+    } else {
+        v = (double)acc;
+    }
+    return v;
+}
+
+// KEY: VB_L2_SQUARED, VB_NEG_IP, VB_COSINE or VB_L1.  out_d (float8 of SQL function `metric`) or out_f (ordering key).
+// grid: x = row slices, y = queries.  out[(q * n + r)].
+template <int KEY>
+__global__ void __launch_bounds__(SP_WARPS * 32)
+sparse_scan_kernel(SparseQueries Q, int shift, const int64_t* __restrict__ row_off, const int32_t* __restrict__ idx,
+                   const float* __restrict__ val, int64_t n, int metric, double* __restrict__ out_d, float* __restrict__ out_f) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    __shared__ float s_qnorm;
+    const int q = blockIdx.y;
+    const SpStaged sq = sp_stage<KEY>(Q, q, shift, smem, &s_qnorm);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint32_t* flags = sq.flags + (size_t)warp * sq.nwords;
+    const bool sqrt_l2 = metric == VB_L2 && out_d;
     const int64_t wstride = (int64_t)gridDim.x * SP_WARPS;
     for (int64_t r = (int64_t)blockIdx.x * SP_WARPS + warp; r < n; r += wstride) {
-        const int64_t beg = row_off[r], end = row_off[r + 1];
-        if (FLAGS) {
-            for (int w = lane; w < nwords; w += 32) flags[w] = 0u;
-            __syncwarp();
-        }
-        float acc = 0.f, rn = 0.f;
-        for (int64_t p = beg + lane; p < end; p += 32) {
-            const int32_t ri = __ldg(idx + p);
-            const float rv = __ldg(val + p);
-            const int pos = sp_find(s_idx, s_bucket, shift, ri);
-            const float qv = pos >= 0 ? s_val[pos] : 0.f;
-            if (KEY == VB_L2_SQUARED) {
-                const float t = rv - qv;
-                acc += t * t;
-            } else if (KEY == VB_L1) {
-                acc += fabsf(rv - qv);
-            } else {
-                acc += rv * qv;
-                if (KEY == VB_COSINE) rn += rv * rv;
-            }
-            if (FLAGS && pos >= 0) atomicOr(&flags[pos >> 5], 1u << (pos & 31));
-        }
-        if (FLAGS) {
-            __syncwarp();
-            for (int w = lane; w < nwords; w += 32) {
-                uint32_t m = ~flags[w];
-                if (w == nwords - 1 && (qn & 31)) m &= (1u << (qn & 31)) - 1u;
-                while (m) {
-                    const int b = __ffs(m) - 1;
-                    m &= m - 1;
-                    const float qv = s_val[w * 32 + b];
-                    acc += KEY == VB_L2_SQUARED ? qv * qv : fabsf(qv);
-                }
-            }
-            __syncwarp();
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            acc += __shfl_xor_sync(0xffffffffu, acc, o);
-            if (KEY == VB_COSINE) rn += __shfl_xor_sync(0xffffffffu, rn, o);
-        }
+        const double v = sp_score_row<KEY>(row_off[r], row_off[r + 1], idx, val, sq, shift, flags, s_qnorm, metric, sqrt_l2, lane);
         if (lane == 0) {
-            double v;
-            if (KEY == VB_COSINE) {
-                // src/sparsevec.c:985-1009: similarity / sqrt((double) norma * (double) normb), clamped, 1 - similarity
-                double sim = (double)acc / sqrt((double)rn * (double)s_qnorm);
-                if (sim > 1.0) sim = 1.0;
-                else if (sim < -1.0) sim = -1.0;
-                v = 1.0 - sim;
-            } else if (KEY == VB_NEG_IP) {
-                v = metric == VB_IP ? (double)acc : (double)-acc;
-            } else if (KEY == VB_L2_SQUARED) {
-                v = (metric == VB_L2 && out_d) ? sqrt((double)acc) : (double)acc;
-            } else {
-                v = (double)acc;
-            }
             const size_t at = (size_t)q * (size_t)n + (size_t)r;
             if (out_d) out_d[at] = v;
             else out_f[at] = (float)v;
+        }
+    }
+}
+
+// The listed rows of a chunk list: row j of chunk c is table row rows[c.row_begin + j], its ordering key goes to
+// out[c.out_off + j].  *n_chunks chunks; each CTA takes a contiguous slice of them and stages a query only when the
+// slice moves on to the next one (the chunks of a query are consecutive), so a query is staged once per CTA that
+// scores its rows.  One warp per listed row, through sp_score_row: keys bit-identical to sparse_scan_kernel's out_f.
+// (The bound of 4 CTAs per SM lets ptxas use up to 64 registers; left to itself it stops at 32 and spills.)
+template <int KEY>
+__global__ void __launch_bounds__(SP_WARPS * 32, 4)
+sparse_gather_kernel(SparseQueries Q, int shift, const int64_t* __restrict__ row_off, const int32_t* __restrict__ idx,
+                     const float* __restrict__ val, const int64_t* __restrict__ rows, const Chunk* __restrict__ chunks,
+                     const int* __restrict__ n_chunks, int metric, float* __restrict__ out) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    __shared__ float s_qnorm;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t total = *n_chunks;
+    const int64_t per = (total + gridDim.x - 1) / gridDim.x;
+    const int64_t c_begin = per * blockIdx.x;
+    const int64_t c_end = min(total, c_begin + per);
+    int cur_q = -1, qn = 0;
+    for (int64_t c = c_begin; c < c_end; ++c) {
+        const Chunk ch = chunks[c];
+        if (ch.q != cur_q) {   // uniform over the CTA
+            __syncthreads();   // every warp is done with the previous query
+            qn = sp_stage<KEY>(Q, ch.q, shift, smem, &s_qnorm).qn;
+            cur_q = ch.q;
+        }
+        const SpStaged sq = sp_layout(smem, qn);
+        uint32_t* flags = sq.flags + (size_t)warp * sq.nwords;
+        for (int j = warp; j < ch.n_rows; j += SP_WARPS) {
+            const int64_t r = rows[ch.row_begin + j];
+            const double v = sp_score_row<KEY>(row_off[r], row_off[r + 1], idx, val, sq, shift, flags, s_qnorm, metric, false, lane);
+            if (lane == 0) out[ch.out_off + j] = (float)v;
         }
     }
 }
@@ -204,6 +282,35 @@ static int launch_sparse_scan(int metric, int dim, SparseQueries Q, int64_t nq, 
         case VB_COSINE: SP_LAUNCH(VB_COSINE); break;
         case VB_L1: SP_LAUNCH(VB_L1); break;
         default: set_error("metric %d is not defined for sparsevec", metric); return VB_EINVAL;
+    }
+#undef SP_LAUNCH
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
+}
+
+constexpr int SP_CHUNK_ROWS = 256;   // listed rows per chunk of gather work: 32 per warp
+
+// ordering keys of the chunk list's rows (sparse_gather_kernel); *n_chunks_dev <= max_chunks chunks
+static int launch_sparse_gather(int key_metric, int dim, SparseQueries Q, int max_qnnz, const SparseTable& t, const int64_t* rows,
+                                const Chunk* chunks, const int* n_chunks_dev, int max_chunks, float* out) {
+    if (max_chunks <= 0) return VB_OK;
+    Context& c = ctx();
+    const size_t smem = sparse_smem_bytes(max_qnnz);
+    const int shift = sparse_shift(dim);
+    const unsigned grid = (unsigned)std::min(max_chunks, 8 * c.sm_count);
+#define SP_LAUNCH(KEY)                                                                                                     \
+    do {                                                                                                                   \
+        VB_CUDA(cudaFuncSetAttribute(sparse_gather_kernel<KEY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
+        sparse_gather_kernel<KEY><<<grid, SP_WARPS * 32, smem, c.stream>>>(Q, shift, t.row_off, t.idx, t.val, rows, chunks, n_chunks_dev, \
+                                                                           key_metric, out);                               \
+    } while (0)
+    switch (key_metric) {
+        case VB_L2_SQUARED: SP_LAUNCH(VB_L2_SQUARED); break;
+        case VB_NEG_IP: SP_LAUNCH(VB_NEG_IP); break;
+        case VB_COSINE: SP_LAUNCH(VB_COSINE); break;
+        case VB_L1: SP_LAUNCH(VB_L1); break;
+        default: set_error("metric %d is not defined for sparsevec", key_metric); return VB_EINVAL;
     }
 #undef SP_LAUNCH
     VB_CUDA(cudaGetLastError());
@@ -278,11 +385,15 @@ __global__ void sparse_segments_kernel(int64_t nseg, int64_t n, int64_t* begin, 
     }
 }
 
-__global__ void sparse_finish_kernel(int metric, int64_t total, const int32_t* __restrict__ pos, const float* __restrict__ key,
+// Selected position -> row number, ordering key -> float8.  rows == nullptr: the position is the row number (the scan of
+// every row); else entry p of segment s is row rows[seg_rows[s * seg_rows_stride] + p] (a position list per segment).
+__global__ void sparse_finish_kernel(int metric, int64_t total, int k, const int32_t* __restrict__ pos, const float* __restrict__ key,
+                                     const int64_t* __restrict__ rows, const int64_t* __restrict__ seg_rows, int seg_rows_stride,
                                      int64_t* __restrict__ out_ids, double* __restrict__ out_d) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= total) return;
-    out_ids[i] = pos[i];
+    const int32_t p = pos[i];
+    out_ids[i] = !rows || p < 0 ? (int64_t)p : rows[seg_rows[(i / k) * seg_rows_stride] + p];
     // the ordering key is the float8 of the function except for <-> (sqrt of the fp32 L2 squared, src/sparsevec.c:872-883)
     out_d[i] = metric == VB_L2 ? sqrt((double)key[i]) : (double)key[i];
 }
@@ -386,13 +497,190 @@ __global__ void sparse_shift_offsets_kernel(int64_t* off, int64_t n, int64_t add
     if (i < n) off[i] += add;
 }
 
+// queries q0 .. q0 + m of a call's CSR batch to the device, offsets rebased to 0
+static int upload_query_range(int64_t q0, int64_t m, const int64_t* q_off, const int32_t* q_idx, const float* q_val, SparseQueries* Q) {
+    std::vector<int64_t> off((size_t)m + 1);
+    for (int64_t i = 0; i <= m; ++i) off[(size_t)i] = q_off[q0 + i] - q_off[q0];
+    VB_TRY(upload_sparse_queries(m, off.data(), q_idx + q_off[q0], q_val + q_off[q0], Q));
+    VB_CUDA(cudaStreamSynchronize(ctx().stream));   // `off` is a local vector
+    return VB_OK;
+}
+
+// The arguments every sparse top-k checks, in vb_sparse_exact_topk's order and with its texts (the dimension check
+// after nq <= 0, which returns early; *max_q = the largest query nnz).
+static int sparse_topk_args(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, int k,
+                            int* max_q);
+
+// The selection and the epilogue of a sub-batch of m queries whose ordering keys are in `key_runs`: the k nearest of
+// each segment, position -> row number (rows / seg_rows / seg_rows_stride: see sparse_finish_kernel), and the float8s
+// copied to out_ids / out_dist (host).
+static int sparse_select_finish(int metric, int64_t m, int k, const float* key_runs, const int64_t* seg_begin, const int32_t* seg_len,
+                                const int64_t* rows, const int64_t* seg_rows, int seg_rows_stride, int64_t* out_ids, double* out_dist) {
+    cudaStream_t s = ctx().stream;
+    void *d_pos, *d_out;
+    VB_TRY(workspace(WSP_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
+    int32_t* pos = (int32_t*)d_pos;
+    float* key = (float*)(pos + (size_t)m * k);
+    VB_TRY(launch_segment_topk_v(key_runs, seg_begin, seg_len, nullptr, nullptr, m, k, pos, key));
+    VB_TRY(workspace(WSP_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
+    int64_t* o_ids = (int64_t*)d_out;
+    double* o_d = (double*)(o_ids + (size_t)m * k);
+    sparse_finish_kernel<<<(unsigned)((m * k + 255) / 256), 256, 0, s>>>(metric, m * k, k, pos, key, rows, seg_rows, seg_rows_stride, o_ids,
+                                                                         o_d);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    VB_CUDA(cudaMemcpyAsync(out_ids, o_ids, sizeof(int64_t) * (size_t)m * k, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaMemcpyAsync(out_dist, o_d, sizeof(double) * (size_t)m * k, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    return VB_OK;
+}
+
+constexpr int64_t SP_MAX_BATCH = 65535;   // queries per sub-batch (the grid.y limit of sparse_scan_kernel)
+
 }  // namespace vb
 
 using namespace vb;
 
 struct vb_sparse_table {
     SparseTable t;
+    uint64_t uid = vb::next_owner_uid();
 };
+
+namespace vb {
+
+static int sparse_topk_args(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, int k,
+                            int* max_q) {
+    VB_REQUIRE(h && sparse_metric_ok(metric) && metric != VB_IP, "bad sparse table / ordering metric");
+    VB_REQUIRE(k > 0 && k <= 2048, "k must be in 1..2048");
+    if (nq <= 0) return VB_OK;
+    VB_REQUIRE(h->t.dim == q_dim, "different sparsevec dimensions %d and %d", h->t.dim, q_dim);
+    VB_REQUIRE(q_off, "null query / output buffers");
+    return check_csr("queries", h->t.dim, nq, q_off, q_idx, max_q);
+}
+
+// Filtered top-k, one sub-batch after the other: filter_chunks_kernel lays out the chunks of each query's allowed rows
+// (a filter's queries in one block), sparse_gather_kernel scores them (one launch per block that fills the grid, so the
+// grid reads one filter's rows at a time), then the selection and the epilogue of vb_sparse_exact_topk.
+static int sparse_topk_filtered(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
+                                const float* q_val, int k, const vb_filter* const* filters, int nfilters, const int32_t* filter_of_query,
+                                int64_t* out_ids, double* out_dist) {
+    const char* fn = "vb_sparse_exact_topk_filtered";
+    VB_TRY(require_init());
+    int max_q = 0;
+    VB_TRY(sparse_topk_args(h, metric, q_dim, 0, nullptr, nullptr, k, nullptr));
+    VB_REQUIRE(filters && nfilters >= 1, "%s: no row filter given", fn);
+    VB_REQUIRE(filter_of_query || nfilters == 1, "%s: filter_of_query may only be NULL with one filter (got %d)", fn, nfilters);
+    for (int i = 0; i < nfilters; ++i) {
+        VB_REQUIRE(filters[i], "%s: filter %d is NULL", fn, i);
+        const Filter& f = filters[i]->f;
+        VB_REQUIRE(f.kind == FILTER_SPARSE && f.owner == h && f.owner_uid == h->uid, "%s: filter %d was made for another table or index", fn, i);
+        VB_REQUIRE(f.n < (int64_t)INT32_MAX, "%s: filter %d allows %lld rows, at most %d", fn, i, (long long)f.n, INT32_MAX - 1);
+    }
+    if (nq <= 0) return VB_OK;
+    VB_TRY(sparse_topk_args(h, metric, q_dim, nq, q_off, q_idx, k, &max_q));
+    VB_REQUIRE(out_ids && out_dist, "null query / output buffers");
+    for (int64_t q = 0; q < nq && filter_of_query; ++q)
+        VB_REQUIRE(filter_of_query[q] >= 0 && filter_of_query[q] < nfilters, "%s: filter_of_query[%lld] = %d, not in 0..%d", fn, (long long)q,
+                   filter_of_query[q], nfilters - 1);
+    Context& c = ctx();
+    const SparseTable& t = h->t;
+    std::vector<int64_t> fbase;
+    const int64_t* rows;
+    VB_TRY(filter_concat_positions(filters, nfilters, WSP_ROWS, &fbase, &rows));
+    const int km = key_metric(metric);
+    // results are staged on the host so that a failing sub-batch leaves the caller's buffers untouched
+    std::vector<int64_t> ids((size_t)(nq * k));
+    std::vector<double> dist((size_t)(nq * k));
+    FilterBatch b;
+    for (int64_t q0 = 0; q0 < nq;) {
+        VB_TRY(filter_batch_plan(filters, nfilters, filter_of_query, fbase.data(), q0, nq, SP_MAX_BATCH, SP_CHUNK_ROWS, 8 * (int64_t)c.sm_count,
+                                 &b));
+        const int64_t m = (int64_t)b.qa.size();
+        const size_t nl = b.launch_count.size();
+        SparseQueries Q;
+        VB_TRY(upload_query_range(q0, m, q_off, q_idx, q_val, &Q));
+        // per-query arguments | segments | chunks of each gather launch
+        void *d_qa, *d_chunks, *d_keys;
+        const size_t qa_bytes = (sizeof(FilterQuery) * (size_t)m + 255) & ~(size_t)255;
+        VB_TRY(workspace(WSP_SEG, qa_bytes + (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + sizeof(int32_t) * nl + 64, &d_qa));
+        int64_t* seg_begin = (int64_t*)((uint8_t*)d_qa + qa_bytes);
+        int32_t* seg_len = (int32_t*)(seg_begin + m);
+        int32_t* d_count = seg_len + m;
+        VB_CUDA(cudaMemcpyAsync(d_qa, b.qa.data(), sizeof(FilterQuery) * (size_t)m, cudaMemcpyHostToDevice, c.stream));
+        if (nl) VB_CUDA(cudaMemcpyAsync(d_count, b.launch_count.data(), sizeof(int32_t) * nl, cudaMemcpyHostToDevice, c.stream));
+        VB_TRY(workspace(WSP_SCAN, sizeof(Chunk) * (size_t)b.max_chunks + 64, &d_chunks));
+        VB_TRY(launch_filter_chunks((const FilterQuery*)d_qa, m, SP_CHUNK_ROWS, seg_begin, seg_len, (Chunk*)d_chunks));
+        VB_TRY(workspace(WSP_TMP, sizeof(float) * (size_t)std::max<int64_t>(b.run, 1), &d_keys));
+        for (size_t l = 0; l < nl; ++l)
+            VB_TRY(launch_sparse_gather(km, t.dim, Q, max_q, t, rows, (const Chunk*)d_chunks + b.launch_begin[l], d_count + l, b.launch_count[l],
+                                        (float*)d_keys));
+        // entry p of query j's segment is rows[qa[j].base + p]
+        static_assert(sizeof(FilterQuery) % sizeof(int64_t) == 0 && offsetof(FilterQuery, base) % sizeof(int64_t) == 0, "FilterQuery layout");
+        VB_TRY(sparse_select_finish(metric, m, k, (const float*)d_keys, seg_begin, seg_len, rows,
+                                    (const int64_t*)d_qa + offsetof(FilterQuery, base) / sizeof(int64_t),
+                                    (int)(sizeof(FilterQuery) / sizeof(int64_t)), ids.data() + q0 * k, dist.data() + q0 * k));
+        q0 += m;
+    }
+    std::copy(ids.begin(), ids.end(), out_ids);
+    std::copy(dist.begin(), dist.end(), out_dist);
+    return VB_OK;
+}
+
+// Re-rank, one sub-batch after the other: rerank_prepare_kernel compacts each query's candidates in candidate order and
+// lays out their chunks, sparse_gather_kernel scores them, then the selection and the epilogue of vb_sparse_exact_topk.
+static int sparse_rerank(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
+                         const float* q_val, const int64_t* cand, int c, int k, int64_t* out_ids, double* out_dist) {
+    const char* fn = "vb_sparse_table_rerank";
+    VB_TRY(require_init());
+    int max_q = 0;
+    VB_TRY(sparse_topk_args(h, metric, q_dim, 0, nullptr, nullptr, k, nullptr));
+    VB_REQUIRE(c >= 0, "%s: negative candidate count %d", fn, c);
+    if (nq <= 0) return VB_OK;
+    VB_TRY(sparse_topk_args(h, metric, q_dim, nq, q_off, q_idx, k, &max_q));
+    VB_REQUIRE((cand || c == 0) && out_ids && out_dist, "null query / output buffers");
+    const SparseTable& t = h->t;
+    const int64_t n = t.n;
+    for (int64_t i = 0; i < nq * c; ++i) {
+        const int64_t v = cand[i];
+        VB_REQUIRE(v >= -1 && v < n, "%s: candidate %lld of query %lld is %lld, not a row of the table (-1 or 0..%lld)", fn,
+                   (long long)(i % c), (long long)(i / c), (long long)v, (long long)n - 1);
+    }
+    Context& cx = ctx();
+    const int km = key_metric(metric);
+    std::vector<int64_t> ids((size_t)(nq * k));
+    std::vector<double> dist((size_t)(nq * k));
+    // sub-batches keep the keys under ~1 GiB
+    const int64_t bq = std::max<int64_t>(1, std::min<int64_t>(std::min(nq, SP_MAX_BATCH), (int64_t)(1ull << 28) / std::max(c, 1)));
+    for (int64_t q0 = 0; q0 < nq; q0 += bq) {
+        const int64_t m = std::min(bq, nq - q0);
+        const size_t mc = (size_t)m * c;
+        SparseQueries Q;
+        VB_TRY(upload_query_range(q0, m, q_off, q_idx, q_val, &Q));
+        // candidates | their compaction
+        void *d_cand, *d_chunks, *d_seg, *d_keys;
+        VB_TRY(workspace(WSP_ROWS, 2 * sizeof(int64_t) * mc, &d_cand));
+        int64_t* d_ids = (int64_t*)d_cand + mc;
+        if (mc) VB_CUDA(cudaMemcpyAsync(d_cand, cand + (size_t)q0 * c, sizeof(int64_t) * mc, cudaMemcpyHostToDevice, cx.stream));
+        const int64_t max_chunks = m * ((c + SP_CHUNK_ROWS - 1) / SP_CHUNK_ROWS);
+        VB_TRY(workspace(WSP_SCAN, sizeof(Chunk) * (size_t)max_chunks + 64, &d_chunks));
+        int* n_chunks = (int*)((Chunk*)d_chunks + max_chunks);
+        VB_TRY(workspace(WSP_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
+        int64_t* seg_begin = (int64_t*)d_seg;
+        int32_t* seg_len = (int32_t*)(seg_begin + m);
+        VB_CUDA(cudaMemsetAsync(n_chunks, 0, sizeof(int), cx.stream));
+        VB_TRY(launch_rerank_prepare((const int64_t*)d_cand, m, c, n, SP_CHUNK_ROWS, d_ids, seg_begin, seg_len, (Chunk*)d_chunks, n_chunks));
+        VB_TRY(workspace(WSP_TMP, sizeof(float) * mc, &d_keys));
+        VB_TRY(launch_sparse_gather(km, t.dim, Q, max_q, t, d_ids, (const Chunk*)d_chunks, n_chunks, (int)max_chunks, (float*)d_keys));
+        // entry p of query j's segment is d_ids[seg_begin[j] + p] (seg_begin[j] = j c)
+        VB_TRY(sparse_select_finish(metric, m, k, (const float*)d_keys, seg_begin, seg_len, d_ids, seg_begin, 1, ids.data() + q0 * k,
+                                    dist.data() + q0 * k));
+    }
+    std::copy(ids.begin(), ids.end(), out_ids);
+    std::copy(dist.begin(), dist.end(), out_dist);
+    return VB_OK;
+}
+
+}  // namespace vb
 
 extern "C" {
 
@@ -595,13 +883,9 @@ int vb_sparse_exact_topk(vb_sparse_table* h, int metric, int q_dim, int64_t nq, 
     const int64_t bq = std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(nq, 65535), (int64_t)(1ull << 30) / (4 * n)));
     for (int64_t q0 = 0; q0 < nq; q0 += bq) {
         const int64_t m = std::min(bq, nq - q0);
-        // this sub-batch's queries, offsets rebased to 0
-        std::vector<int64_t> off((size_t)m + 1);
-        for (int64_t i = 0; i <= m; ++i) off[(size_t)i] = q_off[q0 + i] - q_off[q0];
         SparseQueries Q;
-        VB_TRY(upload_sparse_queries(m, off.data(), q_idx + q_off[q0], q_val + q_off[q0], &Q));
-        VB_CUDA(cudaStreamSynchronize(s));   // `off` is a local vector
-        void *d_key, *d_seg, *d_pos, *d_out;
+        VB_TRY(upload_query_range(q0, m, q_off, q_idx, q_val, &Q));
+        void *d_key, *d_seg;
         VB_TRY(workspace(WSP_TMP, sizeof(float) * (size_t)m * (size_t)n, &d_key));
         VB_TRY(launch_sparse_scan(key_metric(metric), t.dim, Q, m, max_q, t.row_off, t.idx, t.val, n, nullptr, (float*)d_key));
         VB_TRY(workspace(WSP_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
@@ -610,21 +894,25 @@ int vb_sparse_exact_topk(vb_sparse_table* h, int metric, int q_dim, int64_t nq, 
         sparse_segments_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(m, n, seg_begin, seg_len);
         VB_CUDA(cudaGetLastError());
         count_launch();
-        VB_TRY(workspace(WSP_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
-        int32_t* pos = (int32_t*)d_pos;
-        float* key = (float*)(pos + (size_t)m * k);
-        VB_TRY(launch_segment_topk_v((const float*)d_key, seg_begin, seg_len, nullptr, nullptr, m, k, pos, key));
-        VB_TRY(workspace(WSP_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
-        int64_t* o_ids = (int64_t*)d_out;
-        double* o_d = (double*)(o_ids + (size_t)m * k);
-        sparse_finish_kernel<<<(unsigned)((m * k + 255) / 256), 256, 0, s>>>(metric, m * k, pos, key, o_ids, o_d);
-        VB_CUDA(cudaGetLastError());
-        count_launch();
-        VB_CUDA(cudaMemcpyAsync(out_ids + q0 * k, o_ids, sizeof(int64_t) * (size_t)m * k, cudaMemcpyDeviceToHost, s));
-        VB_CUDA(cudaMemcpyAsync(out_dist + q0 * k, o_d, sizeof(double) * (size_t)m * k, cudaMemcpyDeviceToHost, s));
-        VB_CUDA(cudaStreamSynchronize(s));
+        VB_TRY(sparse_select_finish(metric, m, k, (const float*)d_key, seg_begin, seg_len, nullptr, nullptr, 0, out_ids + q0 * k,
+                                    out_dist + q0 * k));
     }
     return VB_OK;
+}
+
+int vb_sparse_table_filter_create(vb_sparse_table* h, const int64_t* rows, int64_t n, vb_filter** out) {
+    return table_filter_create("vb_sparse_table_filter_create", h, h ? h->uid : 0, h ? h->t.n : 0, FILTER_SPARSE, rows, n, true, out);
+}
+
+int vb_sparse_exact_topk_filtered(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
+                                  const float* q_val, int k, const vb_filter* const* filters, int nfilters, const int32_t* filter_of_query,
+                                  int64_t* out_ids, double* out_dist) {
+    return sparse_topk_filtered(h, metric, q_dim, nq, q_off, q_idx, q_val, k, filters, nfilters, filter_of_query, out_ids, out_dist);
+}
+
+int vb_sparse_table_rerank(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
+                           const float* q_val, const int64_t* cand, int c, int k, int64_t* out_ids, double* out_dist) {
+    return sparse_rerank(h, metric, q_dim, nq, q_off, q_idx, q_val, cand, c, k, out_ids, out_dist);
 }
 
 }  // extern "C"

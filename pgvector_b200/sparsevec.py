@@ -1,5 +1,5 @@
 """sparsevec on the device -- host-side mirror of the reference's sparsevec functions (src/sparsevec.c:826-1150) over
-the C ABI (vb_sparsevec_* / vb_sparse_table_* / vb_sparse_exact_topk).
+the C ABI (vb_sparsevec_* / vb_sparse_table_* / vb_sparse_exact_topk[_filtered]).
 
 A value is ``SparseVector(dim, indices, values)`` with 0-based ascending indices (the on-disk order,
 src/sparsevec.h:17-32); the text form '{index:value,...}/dim' is 1-based like the reference's I/O functions.  A batch
@@ -234,7 +234,8 @@ def l2_normalize(rows):
 
 
 class SparseTable:
-    """sparsevec rows resident in HBM; ``exact_topk`` is the sequential-scan plan ORDER BY v <op> q LIMIT k"""
+    """sparsevec rows resident in HBM; ``exact_topk`` is the sequential-scan plan ORDER BY v <op> q LIMIT k, with
+    row filters (``filter``) for a WHERE clause; ``rerank`` orders candidate rows another index fetched"""
 
     def __init__(self, dim):
         self.dim = int(dim)
@@ -257,11 +258,49 @@ class SparseTable:
     def nnz(self):
         return int(load().vb_sparse_table_nnz(self.h))
 
-    def exact_topk(self, metric, queries, k):
+    def filter(self, rows):
+        """a row Filter of this table (WHERE <predicate> as the row numbers it allows, numpy int64).  Rows appended
+        later are not in it."""
+        from . import Filter
+        rows = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)   # host rows only, like the rest of the sparse API
+        return Filter._create(self, "vb_sparse_table_filter_create", rows)
+
+    def exact_topk(self, metric, queries, k, filter=None, filter_of_query=None):
+        """ORDER BY v <op> q LIMIT k without an index.  filter: a Filter of this table, or a list of them with
+        filter_of_query[q] = the index of query q's filter; each query then gets exactly what rerank() returns for its
+        filter's rows in ascending order (k <= 2048)."""
         q = _rows(queries)
+        k = int(k)
         ids = np.empty((q.n, k), dtype=np.int64)
         dist = np.empty((q.n, k), dtype=np.float64)
-        rc = load().vb_sparse_exact_topk(self.h, metric, q.dim, q.n, _p(q.row_off), _p(q.idx), _p(q.val), k, _p(ids), _p(dist))
+        if filter is None:
+            rc = load().vb_sparse_exact_topk(self.h, metric, q.dim, q.n, _p(q.row_off), _p(q.idx), _p(q.val), k, _p(ids), _p(dist))
+        else:
+            from . import _filter_args
+            farr, nf, fq = _filter_args(filter, filter_of_query)
+            if fq is not None and len(fq) != q.n:
+                raise ValueError(f"filter_of_query must have {q.n} entries, got {len(fq)}")
+            rc = load().vb_sparse_exact_topk_filtered(self.h, metric, q.dim, q.n, _p(q.row_off), _p(q.idx), _p(q.val), k, farr, nf, _p(fq),
+                                                      _p(ids), _p(dist))
+        return self._result(rc, ids, dist)
+
+    def rerank(self, metric, queries, candidates, k):
+        """ORDER BY v <op> q LIMIT k over each query's own candidate rows: candidates[q] = row numbers of this table
+        (-1 = none), typically what a dense or quantized index returned (hybrid search)."""
+        q = _rows(queries)
+        k = int(k)
+        cand = np.asarray(candidates)
+        if cand.dtype != np.int64 or cand.ndim != 2 or cand.shape[0] != q.n:
+            raise ValueError(f"rerank: candidates must be int64 of shape [{q.n}, c], got {cand.dtype} {cand.shape}")
+        cand = np.ascontiguousarray(cand)
+        ids = np.empty((q.n, k), dtype=np.int64)
+        dist = np.empty((q.n, k), dtype=np.float64)
+        rc = load().vb_sparse_table_rerank(self.h, metric, q.dim, q.n, _p(q.row_off), _p(q.idx), _p(q.val), _p(cand), cand.shape[1], k,
+                                           _p(ids), _p(dist))
+        return self._result(rc, ids, dist)
+
+    @staticmethod
+    def _result(rc, ids, dist):
         if rc == _lib.EINVAL:
             msg = load().vb_last_error().decode()
             if msg.startswith("different sparsevec dimensions"):
