@@ -24,8 +24,11 @@
  *     counters per sub-batch of queries, with up to 64 numbers of the queries filter
  *     level 0 could not certify (the tensor-core filter re-runs uncertified queries
  *     before the results may be used; a re-run synchronises again),
- *     vb_hnsw_search_dev reads one overflow flag per call (visited-table growth), and
- *     vb_table_aggregate_dev reads sum's 4-byte overflow flag (float_overflow_error).
+ *     vb_hnsw_search_dev reads one overflow flag per call (visited-table growth),
+ *     vb_table_aggregate_dev reads sum's 4-byte overflow flag (float_overflow_error), and
+ *     the sparsevec _dev calls read the result of their device CSR check: one copy of at
+ *     most 24 bytes (first defect, largest row nnz, total nnz) before any other work
+ *     (the casts: one copy of at most 32 bytes, see vb_dense_to_sparsevec_batch).
  *   - rows are row-major and contiguous in the caller's buffers (vector: dim
  *     fp32; halfvec: dim IEEE binary16; bit: (dim+7)/8 bytes, MSB first, tail
  *     bits zero -- exactly the payload of Vector.x (src/vector.h:18-24),
@@ -286,7 +289,8 @@ int			vb_table_aggregate_dev(vb_table *t, int agg, const int32_t *group_of_row_d
 
 /*
  * sparsevec (src/sparsevec.h:21-32): dim, nnz, indices[nnz] (0-based, ascending), values[nnz].  A batch of rows is CSR:
- * row r = entries row_off[r] .. row_off[r+1] of idx[] / val[] (row_off[0] = 0).  All host buffers.
+ * row r = entries row_off[r] .. row_off[r+1] of idx[] / val[] (row_off[0] = 0).  The calls of this block take host
+ * buffers; the resident table's calls and the casts below also have _dev variants.
  *
  *   vb_sparsevec_distance_batch      out[r] = metric(row r, q) as the float8 of sparsevec's l2_distance /
  *                                    l2_squared_distance / inner_product / negative_inner_product / cosine_distance /
@@ -308,6 +312,17 @@ typedef struct vb_sparse_table vb_sparse_table;	/* n sparsevec rows resident in 
 
 int			vb_sparse_table_create(int dim, vb_sparse_table **out);
 int			vb_sparse_table_append(vb_sparse_table *t, int64_t n, const int64_t *row_off, const int32_t *idx, const float *val);
+/*
+ * Device CSR (the _dev variants of this section): row_off_dev / q_off_dev [n + 1] int64, idx int32, val float, all device
+ * pointers, checked on the device with the host variants' rules and texts -- offsets from 0 and never decreasing, at most
+ * 16000 entries per row, indices inside [0, dim) and strictly ascending -- with " (row r)" naming the first bad row.
+ * That check is the one read back (at most 24 bytes); everything after it is enqueued on vb_stream().  Entries of a row
+ * whose offsets lie outside [0, row_off[n]] are not read (a row before it has bad offsets and is reported).
+ * vb_sparse_table_append_dev appends nothing on any error; growing the table's buffers synchronises, as in the host
+ * variant.
+ */
+int			vb_sparse_table_append_dev(vb_sparse_table *t, int64_t n, const int64_t *row_off_dev, const int32_t *idx_dev,
+									   const float *val_dev);
 int64_t		vb_sparse_table_rows(const vb_sparse_table *t);
 int64_t		vb_sparse_table_nnz(const vb_sparse_table *t);
 int			vb_sparse_table_free(vb_sparse_table *t);
@@ -318,6 +333,10 @@ int			vb_sparse_table_free(vb_sparse_table *t);
  */
 int			vb_sparse_exact_topk(vb_sparse_table *t, int metric, int q_dim, int64_t nq, const int64_t *q_off, const int32_t *q_idx,
 								 const float *q_val, int k, int64_t *out_ids, double *out_dist);
+/* queries and outputs on the device: ids as the host variant's, distances the float of its float8 */
+int			vb_sparse_exact_topk_dev(vb_sparse_table *t, int metric, int q_dim, int64_t nq, const int64_t *q_off_dev,
+										 const int32_t *q_idx_dev, const float *q_val_dev, int k, int64_t *out_ids_dev,
+										 float *out_dist_dev);
 
 /*
  * Row filters of a sparse table (see vb_filter above): rows = row numbers of t (append order).  A value outside [0, n)
@@ -327,6 +346,8 @@ int			vb_sparse_exact_topk(vb_sparse_table *t, int metric, int q_dim, int64_t nq
  * every dense, IVFFlat and HNSW call; the sparse calls refuse their filters.
  */
 int			vb_sparse_table_filter_create(vb_sparse_table *t, const int64_t *rows, int64_t n, vb_filter **out);
+/* rows on the device; values outside [0, n) are ignored (as vb_table_filter_create_dev) */
+int			vb_sparse_table_filter_create_dev(vb_sparse_table *t, const int64_t *rows_dev, int64_t n, vb_filter **out);
 /*
  * Filtered exact top-k: for each query q, the k nearest of the rows filters[filter_of_query[q]] allows -- the plan of
  * "WHERE <predicate> ORDER BY v <op> q LIMIT k" with a B-tree or bitmap scan on the filter column.  filter_of_query is a
@@ -346,13 +367,51 @@ int			vb_sparse_table_filter_create(vb_sparse_table *t, const int64_t *rows, int
  * Both: everything is validated before any kernel runs, and on any error nothing is written to out_ids / out_dist.
  * Queries run in sub-batches of at most 65535 whose distance runs stay under 1 GiB; VB_ENOMEM names the bytes that could
  * not be allocated.  The filters may be freed once the call returns.
+ *
+ * _dev variants: queries (device CSR, above), cand and the outputs on the device, ids as the host variant's and distances
+ * the float of its float8; filters and filter_of_query stay host arrays.  Candidates outside [0, n) are treated as
+ * absent and never read (as vb_table_rerank_dev).  On a refused call nothing is written.
  */
 int			vb_sparse_exact_topk_filtered(vb_sparse_table *t, int metric, int q_dim, int64_t nq, const int64_t *q_off,
 										  const int32_t *q_idx, const float *q_val, int k, const vb_filter *const *filters,
 										  int nfilters, const int32_t *filter_of_query, int64_t *out_ids, double *out_dist);
+int			vb_sparse_exact_topk_filtered_dev(vb_sparse_table *t, int metric, int q_dim, int64_t nq, const int64_t *q_off_dev,
+												  const int32_t *q_idx_dev, const float *q_val_dev, int k,
+												  const vb_filter *const *filters, int nfilters, const int32_t *filter_of_query,
+												  int64_t *out_ids_dev, float *out_dist_dev);
 int			vb_sparse_table_rerank(vb_sparse_table *t, int metric, int q_dim, int64_t nq, const int64_t *q_off,
 								   const int32_t *q_idx, const float *q_val, const int64_t *cand, int c, int k, int64_t *out_ids,
 								   double *out_dist);
+int			vb_sparse_table_rerank_dev(vb_sparse_table *t, int metric, int q_dim, int64_t nq, const int64_t *q_off_dev,
+										   const int32_t *q_idx_dev, const float *q_val_dev, const int64_t *cand_dev, int c, int k,
+										   int64_t *out_ids_dev, float *out_dist_dev);
+
+/*
+ * Casts between the dense types and sparsevec, batched (elem = VB_VECTOR or VB_HALFVEC; rows packed, dim elements each):
+ *   vb_dense_to_sparsevec_batch  vector_to_sparsevec / halfvec_to_sparsevec (src/sparsevec.c:606-689): an element is kept
+ *                                when x != 0 (halfvec: !HalfIsZero), so -0 is dropped; kept elements in ascending index
+ *                                order, halfvec values widened exactly.  out_row_off [n + 1] is always written; when the
+ *                                rows hold more than cap entries the call fails with VB_EINVAL naming the count and writes
+ *                                no indices or values (cap = 0 sizes the output).  Errors: CheckDim's and CheckNnz's texts
+ *                                ("sparsevec must have at least 1 dimension", "sparsevec cannot have more than 16000
+ *                                non-zero elements (row r)").
+ *   vb_sparsevec_to_dense_batch  sparsevec_to_vector / sparsevec_to_halfvec (src/vector.c:1323-1349, src/halfvec.c:1199-1225):
+ *                                out [n x dim] zero-filled, then the entries scattered; halfvec by Float4ToHalf, so a
+ *                                finite value that overflows fails with "\"65520\" is out of range for type halfvec" and a
+ *                                value that rounds to 0 stores a zero.  dim above 16000 fails with "vector cannot have
+ *                                more than 16000 dimensions" (or halfvec's).  The CSR is checked as the table's; on error
+ *                                out is unspecified.
+ * Host variants synchronise.  _dev variants read back one result of at most 24 bytes (to sparsevec: the nnz check and
+ * the total) or 32 bytes (to dense: the CSR check and the first overflowing entry; on that error 4 more bytes, the value).
+ */
+int			vb_dense_to_sparsevec_batch(int elem, int dim, const void *rows, int64_t n, int64_t cap, int64_t *out_row_off,
+										int32_t *out_idx, float *out_val);
+int			vb_dense_to_sparsevec_batch_dev(int elem, int dim, const void *rows_dev, int64_t n, int64_t cap,
+											int64_t *out_row_off_dev, int32_t *out_idx_dev, float *out_val_dev);
+int			vb_sparsevec_to_dense_batch(int elem, int dim, int64_t n, const int64_t *row_off, const int32_t *idx, const float *val,
+										void *out);
+int			vb_sparsevec_to_dense_batch_dev(int elem, int dim, int64_t n, const int64_t *row_off_dev, const int32_t *idx_dev,
+											const float *val_dev, void *out_dev);
 
 /* ---------------------------------------------------------------- IVFFlat */
 

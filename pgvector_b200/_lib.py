@@ -47,6 +47,15 @@ SIGNATURES = {
     "vb_sparse_table_filter_create": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
     "vb_sparse_exact_topk_filtered": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
     "vb_sparse_table_rerank": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),
+    "vb_sparse_table_append_dev": (_i, [_vp, _i64, _vp, _vp, _vp]),
+    "vb_sparse_exact_topk_dev": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _i, _vp, _vp]),
+    "vb_sparse_table_filter_create_dev": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
+    "vb_sparse_exact_topk_filtered_dev": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
+    "vb_sparse_table_rerank_dev": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),
+    "vb_dense_to_sparsevec_batch": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp, _vp]),
+    "vb_dense_to_sparsevec_batch_dev": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp, _vp]),
+    "vb_sparsevec_to_dense_batch": (_i, [_i, _i, _i64, _vp, _vp, _vp, _vp]),
+    "vb_sparsevec_to_dense_batch_dev": (_i, [_i, _i, _i64, _vp, _vp, _vp, _vp]),
     "vb_table_create": (_i, [_i, _i, C.POINTER(_vp)]),
     "vb_table_append": (_i, [_vp, _vp, _i64]),
     "vb_table_append_dev": (_i, [_vp, _vp, _i64]),

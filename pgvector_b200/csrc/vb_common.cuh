@@ -129,6 +129,17 @@ int table_append_host(Table& t, const void* rows, int64_t n);
 int table_append_dev(Table& t, const void* rows_dev, int64_t n);
 void table_free(Table& t);
 
+// Float4ToHalf (src/halfutils.h:244-261): round to nearest even; *overflow = a finite value became infinite, which the
+// reference refuses (vector_to_halfvec, sparsevec_to_halfvec)
+__device__ __forceinline__ __half float_to_half_checked(float x, bool* overflow) {
+    const __half h = __float2half_rn(x);
+    *overflow = __hisinf(h) != 0 && !isinf(x);
+    return h;
+}
+// Float4ToHalf's error for value v: sets "\"<v>\" is out of range for type halfvec" (v in PostgreSQL's float4 output
+// style) and returns VB_EINVAL (vb_ops.cu)
+int half_range_error(float v);
+
 // Pad + (for halfvec) widen queries into the fp32 query image the kernels read.
 // vector/halfvec: float[nq][qstride/4]; bit: bytes[nq][qstride]. host==true: `queries` is host memory.
 int upload_queries(int elem, int dim, const void* queries, int64_t nq, bool host, int ws_slot, void** out_dev, size_t* qstride);

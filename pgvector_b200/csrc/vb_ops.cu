@@ -81,10 +81,9 @@ __global__ void binary_quantize_kernel(const uint8_t* __restrict__ in, size_t in
 __global__ void to_half_kernel(const float* __restrict__ in, int64_t total, __half* __restrict__ out, unsigned long long* __restrict__ first_bad) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= total) return;
-    const float x = in[i];
-    const __half h = __float2half_rn(x);
-    out[i] = h;
-    if (__hisinf(h) != 0 && !isinf(x)) atomicMin(first_bad, (unsigned long long)i);
+    bool over;
+    out[i] = float_to_half_checked(in[i], &over);
+    if (over) atomicMin(first_bad, (unsigned long long)i);
 }
 __global__ void to_float_kernel(const __half* __restrict__ in, int64_t total, float* __restrict__ out) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -118,6 +117,13 @@ static void shortest_float(float v, char* buf, size_t cap) {
         mant[m] = 0;
         snprintf(buf, cap, "%se%c%02d", mant, exp10 < 0 ? '-' : '+', exp10 < 0 ? -exp10 : exp10);
     }
+}
+
+int half_range_error(float v) {
+    char num[64];
+    shortest_float(v, num, sizeof(num));
+    set_error("\"%s\" is out of range for type halfvec", num);
+    return VB_EINVAL;
 }
 
 static int stage_in(int elem, int dim, const void* rows, int64_t n, void** d_in) {
@@ -217,12 +223,7 @@ int vb_vector_to_halfvec_batch(int dim, const void* rows, int64_t n, void* out) 
     VB_CUDA(cudaMemcpyAsync(out, d_out, sizeof(__half) * (size_t)total, cudaMemcpyDeviceToHost, s));
     VB_CUDA(cudaMemcpyAsync(&bad, d_flag, sizeof(bad), cudaMemcpyDeviceToHost, s));
     VB_CUDA(cudaStreamSynchronize(s));
-    if (bad != ~0ull) {
-        char num[64];
-        shortest_float(reinterpret_cast<const float*>(rows)[bad], num, sizeof(num));
-        set_error("\"%s\" is out of range for type halfvec", num);
-        return VB_EINVAL;
-    }
+    if (bad != ~0ull) return half_range_error(reinterpret_cast<const float*>(rows)[bad]);
     return VB_OK;
 }
 

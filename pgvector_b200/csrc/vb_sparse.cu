@@ -385,21 +385,135 @@ __global__ void sparse_segments_kernel(int64_t nseg, int64_t n, int64_t* begin, 
     }
 }
 
-// Selected position -> row number, ordering key -> float8.  rows == nullptr: the position is the row number (the scan of
-// every row); else entry p of segment s is row rows[seg_rows[s * seg_rows_stride] + p] (a position list per segment).
+// Selected position -> row number, ordering key -> float8 (out_d), or the float of that float8 (out_f, the _dev
+// variants).  rows == nullptr: the position is the row number (the scan of every row); else entry p of segment s is row
+// rows[seg_rows[s * seg_rows_stride] + p] (a position list per segment).
 __global__ void sparse_finish_kernel(int metric, int64_t total, int k, const int32_t* __restrict__ pos, const float* __restrict__ key,
                                      const int64_t* __restrict__ rows, const int64_t* __restrict__ seg_rows, int seg_rows_stride,
-                                     int64_t* __restrict__ out_ids, double* __restrict__ out_d) {
+                                     int64_t* __restrict__ out_ids, double* __restrict__ out_d, float* __restrict__ out_f) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= total) return;
     const int32_t p = pos[i];
     out_ids[i] = !rows || p < 0 ? (int64_t)p : rows[seg_rows[(i / k) * seg_rows_stride] + p];
     // the ordering key is the float8 of the function except for <-> (sqrt of the fp32 L2 squared, src/sparsevec.c:872-883)
-    out_d[i] = metric == VB_L2 ? sqrt((double)key[i]) : (double)key[i];
+    const double v = metric == VB_L2 ? sqrt((double)key[i]) : (double)key[i];
+    if (out_f) out_f[i] = (float)v;
+    else out_d[i] = v;
+}
+
+// -1 / +inf: the result of every query over an empty table (_dev variants)
+__global__ void sparse_pad_kernel(int64_t total, int64_t* __restrict__ out_ids, float* __restrict__ out_f) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    out_ids[i] = -1;
+    out_f[i] = INFINITY;
 }
 
 // workspace slots of this file
-enum { WSP_Q = 20, WSP_ROWS = 21, WSP_OUT = 22, WSP_TMP = 23, WSP_SEG = 24, WSP_POS = 25, WSP_SCAN = 26 };
+enum { WSP_Q = 20, WSP_ROWS = 21, WSP_OUT = 22, WSP_TMP = 23, WSP_SEG = 24, WSP_POS = 25, WSP_SCAN = 26, WSP_CHECK = 27 };
+
+// ----------------------------------------------------------------------------- CSR validation on the device
+
+// What sparse_check_kernel finds in n device CSR rows, read back in one copy by check_csr_dev.  bad: the first defect as
+// (row << 8) | SPC_* (~0 = none), the one check_csr would report first; max_nnz: the largest row nnz (sizes the query
+// staging, sparse_smem_bytes); total: off[n].  over: the casts to halfvec, the first entry whose value overflows
+// binary16 (INT64_MAX = none).
+struct SparseCheck {
+    unsigned long long bad;
+    long long max_nnz;
+    long long total;
+    long long over;
+};
+enum { SPC_START = 1, SPC_DECREASE = 2, SPC_NNZ = 3, SPC_NULL_IDX = 4, SPC_BOUNDS = 5, SPC_ORDER = 6 };
+constexpr size_t SPC_READ = offsetof(SparseCheck, over);   // the bytes a validation reads back (24)
+
+__global__ void sparse_check_init_kernel(SparseCheck* c) {
+    c->bad = ~0ull;
+    c->max_nnz = 0;
+    c->total = 0;
+    c->over = INT64_MAX;
+}
+
+// One warp per row, check_csr's rules in check_csr's order: the offsets (off[0] = 0, non-decreasing, at most
+// SP_MAX_NNZ per row), then the entries (each index inside [0, dim), then strictly above the one before; the first bad
+// entry decides).  A row whose entries lie outside [0, off[n]) is not read: that happens only when some row's offsets
+// are bad, and that row is reported.  The smallest (row << 8) | code wins (atomicMin), so the defect reported is the
+// first one check_csr meets.
+__global__ void __launch_bounds__(256) sparse_check_kernel(int64_t n, const int64_t* __restrict__ off, const int32_t* __restrict__ idx,
+                                                           int dim, SparseCheck* __restrict__ out) {
+    const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (r >= n) return;   // whole warps
+    const int64_t beg = off[r], end = off[r + 1], total = off[n];
+    const int64_t len = end - beg;
+    int code = 0;
+    if (r == 0 && beg != 0) code = SPC_START;
+    else if (len < 0) code = SPC_DECREASE;
+    else if (len > SP_MAX_NNZ) code = SPC_NNZ;
+    else if (len > 0 && !idx) code = SPC_NULL_IDX;
+    else if (beg >= 0 && end <= total) {
+        for (int64_t p0 = beg; p0 < end && !code; p0 += 32) {
+            const int64_t p = p0 + lane;
+            int c = 0;
+            if (p < end) {
+                const int32_t v = idx[p];
+                if (v < 0 || v >= dim) c = SPC_BOUNDS;
+                else if (p > beg && v <= idx[p - 1]) c = SPC_ORDER;
+            }
+            const unsigned m = __ballot_sync(0xffffffffu, c != 0);
+            if (m) code = __shfl_sync(0xffffffffu, c, __ffs(m) - 1);
+        }
+    }
+    if (lane == 0) {
+        if (code) atomicMin(&out->bad, ((unsigned long long)r << 8) | (unsigned)code);
+        else atomicMax(&out->max_nnz, (long long)len);
+        if (r == n - 1) out->total = total;
+    }
+}
+
+// check_csr's text for a defect sparse_check_kernel found, with the row number
+static int sparse_check_error(const char* what, unsigned long long bad) {
+    const long long row = (long long)(bad >> 8);
+    switch ((int)(bad & 0xFF)) {
+        case SPC_START: set_error("%s: offsets must start at 0", what); break;
+        case SPC_DECREASE: set_error("%s: offsets must not decrease (row %lld)", what, row); break;
+        case SPC_NNZ: set_error("sparsevec cannot have more than %d non-zero elements (row %lld)", SP_MAX_NNZ, row); break;
+        case SPC_NULL_IDX: set_error("%s: null indices (row %lld)", what, row); break;
+        case SPC_BOUNDS: set_error("sparsevec index out of bounds (row %lld)", row); break;
+        default: set_error("sparsevec indices must be in ascending order (row %lld)", row); break;
+    }
+    return VB_EINVAL;
+}
+
+// Launch the initialisation and the check of n >= 1 device CSR rows into *chk (workspace slot WSP_CHECK); no read.
+static int launch_sparse_check(int dim, int64_t n, const int64_t* off, const int32_t* idx, SparseCheck** chk) {
+    cudaStream_t s = ctx().stream;
+    void* d;
+    VB_TRY(workspace(WSP_CHECK, sizeof(SparseCheck), &d));
+    *chk = (SparseCheck*)d;
+    sparse_check_init_kernel<<<1, 1, 0, s>>>(*chk);
+    sparse_check_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(n, off, idx, dim, *chk);
+    VB_CUDA(cudaGetLastError());
+    count_launch(2);
+    return VB_OK;
+}
+
+// check_csr for n >= 1 device CSR rows: one sparse_check_kernel pass and one read of its 24-byte result (which
+// synchronises).  *max_nnz / *total (optional): the largest row nnz and off[n].
+static int check_csr_dev(const char* what, int dim, int64_t n, const int64_t* off, const int32_t* idx, int* max_nnz, int64_t* total) {
+    VB_REQUIRE(dim >= 1 && dim <= SP_MAX_DIM, "sparsevec must have between 1 and %d dimensions", SP_MAX_DIM);
+    VB_REQUIRE(off, "%s: offsets must start at 0", what);
+    SparseCheck h{~0ull, 0, 0, 0};
+    SparseCheck* d;
+    VB_TRY(launch_sparse_check(dim, n, off, idx, &d));
+    cudaStream_t s = ctx().stream;
+    VB_CUDA(cudaMemcpyAsync(&h, d, SPC_READ, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    if (h.bad != ~0ull) return sparse_check_error(what, h.bad);
+    if (max_nnz) *max_nnz = (int)h.max_nnz;
+    if (total) *total = h.total;
+    return VB_OK;
+}
 
 static bool sparse_metric_ok(int metric) {
     return metric == VB_L2_SQUARED || metric == VB_L2 || metric == VB_IP || metric == VB_NEG_IP || metric == VB_COSINE || metric == VB_L1;
@@ -506,27 +620,46 @@ static int upload_query_range(int64_t q0, int64_t m, const int64_t* q_off, const
     return VB_OK;
 }
 
+// The queries q0 .. q0 + m of a call: host CSR is uploaded (upload_query_range); device CSR is read in place, its
+// offsets absolute into the call's q_idx / q_val (sp_stage reads Q.off[q] .. Q.off[q + 1]), so nothing is copied.
+static int sub_batch_queries(bool host, int64_t q0, int64_t m, const int64_t* q_off, const int32_t* q_idx, const float* q_val,
+                             SparseQueries* Q) {
+    if (host) return upload_query_range(q0, m, q_off, q_idx, q_val, Q);
+    *Q = SparseQueries{q_off + q0, q_idx, q_val};
+    return VB_OK;
+}
+
 // The arguments every sparse top-k checks, in vb_sparse_exact_topk's order and with its texts (the dimension check
-// after nq <= 0, which returns early; *max_q = the largest query nnz).
-static int sparse_topk_args(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, int k,
-                            int* max_q);
+// after nq <= 0, which returns early; *max_q = the largest query nnz).  host == false: the query CSR is on the device
+// and is validated there (check_csr_dev).
+static int sparse_topk_args(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
+                            const float* q_val, int k, bool host, int* max_q);
 
 // The selection and the epilogue of a sub-batch of m queries whose ordering keys are in `key_runs`: the k nearest of
-// each segment, position -> row number (rows / seg_rows / seg_rows_stride: see sparse_finish_kernel), and the float8s
-// copied to out_ids / out_dist (host).
+// each segment, position -> row number (rows / seg_rows / seg_rows_stride: see sparse_finish_kernel).  out_f == nullptr:
+// the float8s are copied to out_ids / out_dist (host); else the ids and the floats go to out_ids / out_f (device), and
+// nothing is waited for.
 static int sparse_select_finish(int metric, int64_t m, int k, const float* key_runs, const int64_t* seg_begin, const int32_t* seg_len,
-                                const int64_t* rows, const int64_t* seg_rows, int seg_rows_stride, int64_t* out_ids, double* out_dist) {
+                                const int64_t* rows, const int64_t* seg_rows, int seg_rows_stride, int64_t* out_ids, double* out_dist,
+                                float* out_f = nullptr) {
     cudaStream_t s = ctx().stream;
     void *d_pos, *d_out;
     VB_TRY(workspace(WSP_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
     int32_t* pos = (int32_t*)d_pos;
     float* key = (float*)(pos + (size_t)m * k);
     VB_TRY(launch_segment_topk_v(key_runs, seg_begin, seg_len, nullptr, nullptr, m, k, pos, key));
+    if (out_f) {
+        sparse_finish_kernel<<<(unsigned)((m * k + 255) / 256), 256, 0, s>>>(metric, m * k, k, pos, key, rows, seg_rows, seg_rows_stride,
+                                                                             out_ids, nullptr, out_f);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+        return VB_OK;
+    }
     VB_TRY(workspace(WSP_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
     int64_t* o_ids = (int64_t*)d_out;
     double* o_d = (double*)(o_ids + (size_t)m * k);
     sparse_finish_kernel<<<(unsigned)((m * k + 255) / 256), 256, 0, s>>>(metric, m * k, k, pos, key, rows, seg_rows, seg_rows_stride, o_ids,
-                                                                         o_d);
+                                                                         o_d, nullptr);
     VB_CUDA(cudaGetLastError());
     count_launch();
     VB_CUDA(cudaMemcpyAsync(out_ids, o_ids, sizeof(int64_t) * (size_t)m * k, cudaMemcpyDeviceToHost, s));
@@ -548,26 +681,31 @@ struct vb_sparse_table {
 
 namespace vb {
 
-static int sparse_topk_args(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, int k,
-                            int* max_q) {
+static int sparse_topk_args(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
+                            const float* q_val, int k, bool host, int* max_q) {
     VB_REQUIRE(h && sparse_metric_ok(metric) && metric != VB_IP, "bad sparse table / ordering metric");
     VB_REQUIRE(k > 0 && k <= 2048, "k must be in 1..2048");
     if (nq <= 0) return VB_OK;
     VB_REQUIRE(h->t.dim == q_dim, "different sparsevec dimensions %d and %d", h->t.dim, q_dim);
     VB_REQUIRE(q_off, "null query / output buffers");
-    return check_csr("queries", h->t.dim, nq, q_off, q_idx, max_q);
+    if (host) return check_csr("queries", h->t.dim, nq, q_off, q_idx, max_q);
+    int64_t total = 0;
+    VB_TRY(check_csr_dev("queries", h->t.dim, nq, q_off, q_idx, max_q, &total));
+    VB_REQUIRE(total == 0 || q_val, "null query / output buffers");
+    return VB_OK;
 }
 
 // Filtered top-k, one sub-batch after the other: filter_chunks_kernel lays out the chunks of each query's allowed rows
 // (a filter's queries in one block), sparse_gather_kernel scores them (one launch per block that fills the grid, so the
-// grid reads one filter's rows at a time), then the selection and the epilogue of vb_sparse_exact_topk.
+// grid reads one filter's rows at a time), then the selection and the epilogue of vb_sparse_exact_topk.  host == false:
+// queries and outputs on the device (out_f: floats), asynchronous after the query check.
 static int sparse_topk_filtered(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
                                 const float* q_val, int k, const vb_filter* const* filters, int nfilters, const int32_t* filter_of_query,
-                                int64_t* out_ids, double* out_dist) {
+                                bool host, int64_t* out_ids, double* out_dist, float* out_f) {
     const char* fn = "vb_sparse_exact_topk_filtered";
     VB_TRY(require_init());
     int max_q = 0;
-    VB_TRY(sparse_topk_args(h, metric, q_dim, 0, nullptr, nullptr, k, nullptr));
+    VB_TRY(sparse_topk_args(h, metric, q_dim, 0, nullptr, nullptr, nullptr, k, host, nullptr));
     VB_REQUIRE(filters && nfilters >= 1, "%s: no row filter given", fn);
     VB_REQUIRE(filter_of_query || nfilters == 1, "%s: filter_of_query may only be NULL with one filter (got %d)", fn, nfilters);
     for (int i = 0; i < nfilters; ++i) {
@@ -577,8 +715,8 @@ static int sparse_topk_filtered(vb_sparse_table* h, int metric, int q_dim, int64
         VB_REQUIRE(f.n < (int64_t)INT32_MAX, "%s: filter %d allows %lld rows, at most %d", fn, i, (long long)f.n, INT32_MAX - 1);
     }
     if (nq <= 0) return VB_OK;
-    VB_TRY(sparse_topk_args(h, metric, q_dim, nq, q_off, q_idx, k, &max_q));
-    VB_REQUIRE(out_ids && out_dist, "null query / output buffers");
+    VB_TRY(sparse_topk_args(h, metric, q_dim, nq, q_off, q_idx, q_val, k, host, &max_q));
+    VB_REQUIRE(out_ids && (host ? out_dist != nullptr : out_f != nullptr), "null query / output buffers");
     for (int64_t q = 0; q < nq && filter_of_query; ++q)
         VB_REQUIRE(filter_of_query[q] >= 0 && filter_of_query[q] < nfilters, "%s: filter_of_query[%lld] = %d, not in 0..%d", fn, (long long)q,
                    filter_of_query[q], nfilters - 1);
@@ -588,9 +726,9 @@ static int sparse_topk_filtered(vb_sparse_table* h, int metric, int q_dim, int64
     const int64_t* rows;
     VB_TRY(filter_concat_positions(filters, nfilters, WSP_ROWS, &fbase, &rows));
     const int km = key_metric(metric);
-    // results are staged on the host so that a failing sub-batch leaves the caller's buffers untouched
-    std::vector<int64_t> ids((size_t)(nq * k));
-    std::vector<double> dist((size_t)(nq * k));
+    // host results are staged on the host so that a failing sub-batch leaves the caller's buffers untouched
+    std::vector<int64_t> ids(host ? (size_t)(nq * k) : 0);
+    std::vector<double> dist(host ? (size_t)(nq * k) : 0);
     FilterBatch b;
     for (int64_t q0 = 0; q0 < nq;) {
         VB_TRY(filter_batch_plan(filters, nfilters, filter_of_query, fbase.data(), q0, nq, SP_MAX_BATCH, SP_CHUNK_ROWS, 8 * (int64_t)c.sm_count,
@@ -598,7 +736,7 @@ static int sparse_topk_filtered(vb_sparse_table* h, int metric, int q_dim, int64
         const int64_t m = (int64_t)b.qa.size();
         const size_t nl = b.launch_count.size();
         SparseQueries Q;
-        VB_TRY(upload_query_range(q0, m, q_off, q_idx, q_val, &Q));
+        VB_TRY(sub_batch_queries(host, q0, m, q_off, q_idx, q_val, &Q));
         // per-query arguments | segments | chunks of each gather launch
         void *d_qa, *d_chunks, *d_keys;
         const size_t qa_bytes = (sizeof(FilterQuery) * (size_t)m + 255) & ~(size_t)255;
@@ -618,49 +756,55 @@ static int sparse_topk_filtered(vb_sparse_table* h, int metric, int q_dim, int64
         static_assert(sizeof(FilterQuery) % sizeof(int64_t) == 0 && offsetof(FilterQuery, base) % sizeof(int64_t) == 0, "FilterQuery layout");
         VB_TRY(sparse_select_finish(metric, m, k, (const float*)d_keys, seg_begin, seg_len, rows,
                                     (const int64_t*)d_qa + offsetof(FilterQuery, base) / sizeof(int64_t),
-                                    (int)(sizeof(FilterQuery) / sizeof(int64_t)), ids.data() + q0 * k, dist.data() + q0 * k));
-        q0 += m;
+                                    (int)(sizeof(FilterQuery) / sizeof(int64_t)), host ? ids.data() + q0 * k : out_ids + q0 * k,
+                                    host ? dist.data() + q0 * k : nullptr, host ? nullptr : out_f + q0 * k));
+        q0 += m;   // (qa is pageable: its copy has been staged by the time cudaMemcpyAsync returned, so it may be refilled)
     }
-    std::copy(ids.begin(), ids.end(), out_ids);
-    std::copy(dist.begin(), dist.end(), out_dist);
+    if (host) {
+        std::copy(ids.begin(), ids.end(), out_ids);
+        std::copy(dist.begin(), dist.end(), out_dist);
+    }
     return VB_OK;
 }
 
 // Re-rank, one sub-batch after the other: rerank_prepare_kernel compacts each query's candidates in candidate order and
 // lays out their chunks, sparse_gather_kernel scores them, then the selection and the epilogue of vb_sparse_exact_topk.
+// host == false: queries, candidates and outputs on the device (out_f: floats), candidates outside [0, n) absent,
+// asynchronous after the query check.
 static int sparse_rerank(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
-                         const float* q_val, const int64_t* cand, int c, int k, int64_t* out_ids, double* out_dist) {
+                         const float* q_val, const int64_t* cand, int c, int k, bool host, int64_t* out_ids, double* out_dist, float* out_f) {
     const char* fn = "vb_sparse_table_rerank";
     VB_TRY(require_init());
     int max_q = 0;
-    VB_TRY(sparse_topk_args(h, metric, q_dim, 0, nullptr, nullptr, k, nullptr));
+    VB_TRY(sparse_topk_args(h, metric, q_dim, 0, nullptr, nullptr, nullptr, k, host, nullptr));
     VB_REQUIRE(c >= 0, "%s: negative candidate count %d", fn, c);
     if (nq <= 0) return VB_OK;
-    VB_TRY(sparse_topk_args(h, metric, q_dim, nq, q_off, q_idx, k, &max_q));
-    VB_REQUIRE((cand || c == 0) && out_ids && out_dist, "null query / output buffers");
+    VB_TRY(sparse_topk_args(h, metric, q_dim, nq, q_off, q_idx, q_val, k, host, &max_q));
+    VB_REQUIRE((cand || c == 0) && out_ids && (host ? out_dist != nullptr : out_f != nullptr), "null query / output buffers");
     const SparseTable& t = h->t;
     const int64_t n = t.n;
-    for (int64_t i = 0; i < nq * c; ++i) {
+    for (int64_t i = 0; host && i < nq * c; ++i) {
         const int64_t v = cand[i];
         VB_REQUIRE(v >= -1 && v < n, "%s: candidate %lld of query %lld is %lld, not a row of the table (-1 or 0..%lld)", fn,
                    (long long)(i % c), (long long)(i / c), (long long)v, (long long)n - 1);
     }
     Context& cx = ctx();
     const int km = key_metric(metric);
-    std::vector<int64_t> ids((size_t)(nq * k));
-    std::vector<double> dist((size_t)(nq * k));
+    std::vector<int64_t> ids(host ? (size_t)(nq * k) : 0);
+    std::vector<double> dist(host ? (size_t)(nq * k) : 0);
     // sub-batches keep the keys under ~1 GiB
     const int64_t bq = std::max<int64_t>(1, std::min<int64_t>(std::min(nq, SP_MAX_BATCH), (int64_t)(1ull << 28) / std::max(c, 1)));
     for (int64_t q0 = 0; q0 < nq; q0 += bq) {
         const int64_t m = std::min(bq, nq - q0);
         const size_t mc = (size_t)m * c;
         SparseQueries Q;
-        VB_TRY(upload_query_range(q0, m, q_off, q_idx, q_val, &Q));
-        // candidates | their compaction
+        VB_TRY(sub_batch_queries(host, q0, m, q_off, q_idx, q_val, &Q));
+        // candidates (host variant: their copy) | their compaction
         void *d_cand, *d_chunks, *d_seg, *d_keys;
         VB_TRY(workspace(WSP_ROWS, 2 * sizeof(int64_t) * mc, &d_cand));
         int64_t* d_ids = (int64_t*)d_cand + mc;
-        if (mc) VB_CUDA(cudaMemcpyAsync(d_cand, cand + (size_t)q0 * c, sizeof(int64_t) * mc, cudaMemcpyHostToDevice, cx.stream));
+        if (!host) d_cand = const_cast<int64_t*>(cand) + (size_t)q0 * c;
+        else if (mc) VB_CUDA(cudaMemcpyAsync(d_cand, cand + (size_t)q0 * c, sizeof(int64_t) * mc, cudaMemcpyHostToDevice, cx.stream));
         const int64_t max_chunks = m * ((c + SP_CHUNK_ROWS - 1) / SP_CHUNK_ROWS);
         VB_TRY(workspace(WSP_SCAN, sizeof(Chunk) * (size_t)max_chunks + 64, &d_chunks));
         int* n_chunks = (int*)((Chunk*)d_chunks + max_chunks);
@@ -672,11 +816,351 @@ static int sparse_rerank(vb_sparse_table* h, int metric, int q_dim, int64_t nq, 
         VB_TRY(workspace(WSP_TMP, sizeof(float) * mc, &d_keys));
         VB_TRY(launch_sparse_gather(km, t.dim, Q, max_q, t, d_ids, (const Chunk*)d_chunks, n_chunks, (int)max_chunks, (float*)d_keys));
         // entry p of query j's segment is d_ids[seg_begin[j] + p] (seg_begin[j] = j c)
-        VB_TRY(sparse_select_finish(metric, m, k, (const float*)d_keys, seg_begin, seg_len, d_ids, seg_begin, 1, ids.data() + q0 * k,
-                                    dist.data() + q0 * k));
+        VB_TRY(sparse_select_finish(metric, m, k, (const float*)d_keys, seg_begin, seg_len, d_ids, seg_begin, 1,
+                                    host ? ids.data() + q0 * k : out_ids + q0 * k, host ? dist.data() + q0 * k : nullptr,
+                                    host ? nullptr : out_f + q0 * k));
     }
-    std::copy(ids.begin(), ids.end(), out_ids);
-    std::copy(dist.begin(), dist.end(), out_dist);
+    if (host) {
+        std::copy(ids.begin(), ids.end(), out_ids);
+        std::copy(dist.begin(), dist.end(), out_dist);
+    }
+    return VB_OK;
+}
+
+// vb_sparse_exact_topk[_dev]: the scan of every row per sub-batch of queries, then the selection and the epilogue.
+static int sparse_exact_topk(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
+                             const float* q_val, int k, bool host, int64_t* out_ids, double* out_dist, float* out_f) {
+    VB_TRY(require_init());
+    VB_REQUIRE(h && sparse_metric_ok(metric) && metric != VB_IP, "bad sparse table / ordering metric");
+    VB_REQUIRE(k > 0 && k <= 2048, "k must be in 1..2048");
+    if (nq <= 0) return VB_OK;
+    SparseTable& t = h->t;
+    VB_REQUIRE(t.dim == q_dim, "different sparsevec dimensions %d and %d", t.dim, q_dim);
+    VB_REQUIRE(q_off && out_ids && (host ? out_dist != nullptr : out_f != nullptr), "null query / output buffers");
+    int max_q = 0;
+    VB_TRY(sparse_topk_args(h, metric, q_dim, nq, q_off, q_idx, q_val, k, host, &max_q));
+    Context& c = ctx();
+    cudaStream_t s = c.stream;
+    const int64_t n = t.n;
+    if (n == 0) {
+        if (!host) {
+            sparse_pad_kernel<<<(unsigned)((nq * k + 255) / 256), 256, 0, s>>>(nq * k, out_ids, out_f);
+            VB_CUDA(cudaGetLastError());
+            count_launch();
+            return VB_OK;
+        }
+        for (int64_t i = 0; i < nq * k; ++i) {
+            out_ids[i] = -1;
+            out_dist[i] = INFINITY;
+        }
+        return VB_OK;
+    }
+    // sub-batches keep the key matrix under ~1 GiB
+    const int64_t bq = std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(nq, 65535), (int64_t)(1ull << 30) / (4 * n)));
+    for (int64_t q0 = 0; q0 < nq; q0 += bq) {
+        const int64_t m = std::min(bq, nq - q0);
+        SparseQueries Q;
+        VB_TRY(sub_batch_queries(host, q0, m, q_off, q_idx, q_val, &Q));
+        void *d_key, *d_seg;
+        VB_TRY(workspace(WSP_TMP, sizeof(float) * (size_t)m * (size_t)n, &d_key));
+        VB_TRY(launch_sparse_scan(key_metric(metric), t.dim, Q, m, max_q, t.row_off, t.idx, t.val, n, nullptr, (float*)d_key));
+        VB_TRY(workspace(WSP_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
+        int64_t* seg_begin = (int64_t*)d_seg;
+        int32_t* seg_len = (int32_t*)(seg_begin + m);
+        sparse_segments_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(m, n, seg_begin, seg_len);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+        VB_TRY(sparse_select_finish(metric, m, k, (const float*)d_key, seg_begin, seg_len, nullptr, nullptr, 0, out_ids + q0 * k,
+                                    host ? out_dist + q0 * k : nullptr, host ? nullptr : out_f + q0 * k));
+    }
+    return VB_OK;
+}
+
+// vb_sparse_table_append[_dev]: rows validated first (nothing is appended on any error), then the table grows
+// (sparse_reserve) and the new rows are copied behind the old ones, their offsets rebased by the table's nnz.
+static int sparse_append(vb_sparse_table* h, int64_t n, const int64_t* row_off, const int32_t* idx, const float* val, bool host) {
+    VB_TRY(require_init());
+    VB_REQUIRE(h && n >= 0 && (n == 0 || row_off), "bad sparse table arguments");
+    if (n == 0) return VB_OK;
+    SparseTable& t = h->t;
+    int64_t tot;
+    if (host) {
+        VB_TRY(check_csr("rows", t.dim, n, row_off, idx, nullptr));
+        tot = row_off[n];
+    } else {
+        VB_TRY(check_csr_dev("rows", t.dim, n, row_off, idx, nullptr, &tot));
+    }
+    VB_REQUIRE(tot == 0 || val, "null sparsevec values");
+    VB_TRY(sparse_reserve(t, t.n + n, t.nnz + tot));
+    cudaStream_t s = ctx().stream;
+    const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+    // offsets of the new rows: row_off[1..n] + nnz so far
+    VB_CUDA(cudaMemcpyAsync(t.row_off + t.n + 1, row_off + 1, sizeof(int64_t) * (size_t)n, kind, s));
+    if (t.nnz > 0) {
+        sparse_shift_offsets_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(t.row_off + t.n + 1, n, t.nnz);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    if (tot > 0) {
+        VB_CUDA(cudaMemcpyAsync(t.idx + t.nnz, idx, sizeof(int32_t) * (size_t)tot, kind, s));
+        VB_CUDA(cudaMemcpyAsync(t.val + t.nnz, val, sizeof(float) * (size_t)tot, kind, s));
+    }
+    if (host) VB_CUDA(cudaStreamSynchronize(s));
+    t.n += n;
+    t.nnz += tot;
+    return VB_OK;
+}
+
+// ----------------------------------------------------------------------------- casts between the dense types and sparsevec
+
+// element i of packed dense rows as the cast sees it: kept (vector: x != 0; halfvec: !HalfIsZero, so -0 is dropped in
+// both) and its float value (halfvec: HalfToFloat4, exact)
+template <int ELEM>
+__device__ __forceinline__ bool dense_elem(const void* __restrict__ rows, size_t i, float* v) {
+    if (ELEM == VB_VECTOR) {
+        *v = __ldg(reinterpret_cast<const float*>(rows) + i);
+        return *v != 0.f;
+    }
+    const unsigned short b = __ldg(reinterpret_cast<const unsigned short*>(rows) + i);
+    *v = __half2float(__ushort_as_half(b));
+    return (b & 0x7FFFu) != 0;
+}
+
+constexpr int SP_CAST_UNROLL = 4;   // elements per lane in flight: each lane loads 4 before the warp's ballots
+
+// Count pass of vector_to_sparsevec / halfvec_to_sparsevec (src/sparsevec.c:606-689): one warp per row, the kept
+// elements ballot-counted.  cnt[r] = the row's nnz; a row above SP_MAX_NNZ is CheckNnz's error (the first such row wins).
+template <int ELEM>
+__global__ void __launch_bounds__(256) dense_count_kernel(const void* __restrict__ rows, int dim, int64_t n, int64_t* __restrict__ cnt,
+                                                          SparseCheck* __restrict__ chk) {
+    const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (r >= n) return;   // whole warps
+    const size_t base = (size_t)r * (size_t)dim;
+    int64_t c = 0;
+    for (int i0 = 0; i0 < dim; i0 += 32 * SP_CAST_UNROLL) {
+        bool keep[SP_CAST_UNROLL];
+#pragma unroll
+        for (int u = 0; u < SP_CAST_UNROLL; ++u) {
+            const int i = i0 + u * 32 + lane;
+            float v;
+            keep[u] = i < dim && dense_elem<ELEM>(rows, base + i, &v);
+        }
+#pragma unroll
+        for (int u = 0; u < SP_CAST_UNROLL; ++u) c += __popc(__ballot_sync(0xffffffffu, keep[u]));
+    }
+    if (lane == 0) {
+        cnt[r] = c;
+        if (c > SP_MAX_NNZ) atomicMin(&chk->bad, ((unsigned long long)r << 8) | SPC_NNZ);
+    }
+}
+
+// Write pass: the kept elements of row r at off[r] .. in ascending index order (ballot + the warp prefix of each step)
+template <int ELEM>
+__global__ void __launch_bounds__(256) dense_write_kernel(const void* __restrict__ rows, int dim, int64_t n, const int64_t* __restrict__ off,
+                                                          int32_t* __restrict__ out_idx, float* __restrict__ out_val) {
+    const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (r >= n) return;   // whole warps
+    const size_t base = (size_t)r * (size_t)dim;
+    const unsigned below = (1u << lane) - 1u;
+    int64_t w = off[r];
+    for (int i0 = 0; i0 < dim; i0 += 32 * SP_CAST_UNROLL) {
+        bool keep[SP_CAST_UNROLL];
+        float v[SP_CAST_UNROLL];
+#pragma unroll
+        for (int u = 0; u < SP_CAST_UNROLL; ++u) {
+            const int i = i0 + u * 32 + lane;
+            keep[u] = i < dim && dense_elem<ELEM>(rows, base + i, &v[u]);
+        }
+#pragma unroll
+        for (int u = 0; u < SP_CAST_UNROLL; ++u) {
+            const unsigned m = __ballot_sync(0xffffffffu, keep[u]);
+            if (keep[u]) {
+                const int64_t at = w + __popc(m & below);
+                out_idx[at] = i0 + u * 32 + lane;
+                out_val[at] = v[u];
+            }
+            w += __popc(m);
+        }
+    }
+}
+
+// sparsevec_to_vector / sparsevec_to_halfvec (src/vector.c:1323-1349, src/halfvec.c:1199-1225): one warp per row, the
+// row zero-filled, then its entries scattered (halfvec: Float4ToHalf, an overflow recorded as the first entry in
+// chk->over).  Nothing is written when chk->bad records a CSR defect (the check ran before, on the same stream).
+template <int ELEM>
+__global__ void __launch_bounds__(256) sparse_to_dense_kernel(int64_t n, const int64_t* __restrict__ off, const int32_t* __restrict__ idx,
+                                                              const float* __restrict__ val, int dim, void* __restrict__ out,
+                                                              SparseCheck* __restrict__ chk) {
+    const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (r >= n || chk->bad != ~0ull) return;   // whole warps
+    const size_t base = (size_t)r * (size_t)dim;
+    for (int i = lane; i < dim; i += 32) {
+        if (ELEM == VB_VECTOR) reinterpret_cast<float*>(out)[base + i] = 0.f;
+        else reinterpret_cast<__half*>(out)[base + i] = __ushort_as_half((unsigned short)0);
+    }
+    __syncwarp();
+    const int64_t end = val ? off[r + 1] : off[r];   // null values: the call fails unless there are no entries
+    for (int64_t p = off[r] + lane; p < end; p += 32) {
+        const float x = val[p];
+        if (ELEM == VB_VECTOR) {
+            reinterpret_cast<float*>(out)[base + idx[p]] = x;
+        } else {
+            bool over;
+            reinterpret_cast<__half*>(out)[base + idx[p]] = float_to_half_checked(x, &over);
+            if (over) atomicMin(&chk->over, (long long)p);
+        }
+    }
+}
+
+static const char* dense_name(int elem) { return elem == VB_VECTOR ? "vector" : "halfvec"; }
+
+// vb_dense_to_sparsevec_batch[_dev]
+static int dense_to_sparse(int elem, int dim, const void* rows, int64_t n, int64_t cap, bool host, int64_t* out_row_off, int32_t* out_idx,
+                           float* out_val) {
+    const char* fn = host ? "vb_dense_to_sparsevec_batch" : "vb_dense_to_sparsevec_batch_dev";
+    VB_TRY(require_init());
+    VB_REQUIRE(elem == VB_VECTOR || elem == VB_HALFVEC, "%s: elem must be VB_VECTOR or VB_HALFVEC, got %d", fn, elem);
+    // CheckDim (src/sparsevec.c:68-80)
+    VB_REQUIRE(dim >= 1, "sparsevec must have at least 1 dimension");
+    VB_REQUIRE(dim <= SP_MAX_DIM, "sparsevec cannot have more than %d dimensions", SP_MAX_DIM);
+    VB_REQUIRE(n >= 0 && n < (int64_t)INT32_MAX && cap >= 0, "%s: bad row count %lld or cap %lld", fn, (long long)n, (long long)cap);
+    VB_REQUIRE(out_row_off && (rows || n == 0), "%s: null rows or offsets", fn);
+    Context& cx = ctx();
+    cudaStream_t s = cx.stream;
+    if (n == 0) {
+        if (host) out_row_off[0] = 0;
+        else VB_CUDA(cudaMemsetAsync(out_row_off, 0, sizeof(int64_t), s));
+        return VB_OK;
+    }
+    const size_t raw = raw_row_bytes(elem, dim);
+    const size_t b_off = sizeof(int64_t) * (size_t)(n + 1);
+    void *d_in = const_cast<void*>(rows), *d_cnt, *d_off = out_row_off, *d_scan, *d_chk;
+    if (host) {
+        VB_TRY(workspace(WSP_ROWS, raw * (size_t)n, &d_in));
+        VB_CUDA(cudaMemcpyAsync(d_in, rows, raw * (size_t)n, cudaMemcpyHostToDevice, s));
+        VB_TRY(workspace(WSP_SEG, b_off, &d_off));
+    }
+    VB_TRY(workspace(WSP_TMP, b_off, &d_cnt));
+    VB_TRY(workspace(WSP_CHECK, sizeof(SparseCheck), &d_chk));
+    SparseCheck* chk = (SparseCheck*)d_chk;
+    int64_t* cnt = (int64_t*)d_cnt;
+    int64_t* off = (int64_t*)d_off;
+    const unsigned grid = (unsigned)((n * 32 + 255) / 256);
+    sparse_check_init_kernel<<<1, 1, 0, s>>>(chk);
+    if (elem == VB_VECTOR) dense_count_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(d_in, dim, n, cnt, chk);
+    else dense_count_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(d_in, dim, n, cnt, chk);
+    VB_CUDA(cudaGetLastError());
+    VB_CUDA(cudaMemsetAsync(cnt + n, 0, sizeof(int64_t), s));
+    size_t scan_bytes = 0;
+    VB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, cnt, off, (int)(n + 1), s));
+    VB_TRY(workspace(WSP_SCAN, scan_bytes + 64, &d_scan));
+    VB_CUDA(cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, cnt, off, (int)(n + 1), s));
+    count_launch(3);
+    VB_CUDA(cudaMemcpyAsync(&chk->total, off + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
+    SparseCheck hc;
+    if (host) VB_CUDA(cudaMemcpyAsync(out_row_off, off, b_off, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaMemcpyAsync(&hc, chk, SPC_READ, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    if (hc.bad != ~0ull) return sparse_check_error(fn, hc.bad);
+    const int64_t total = hc.total;
+    VB_REQUIRE(total <= cap, "%s: the rows have %lld non-zero elements, more than cap = %lld", fn, (long long)total, (long long)cap);
+    if (total == 0) return VB_OK;
+    VB_REQUIRE(out_idx && out_val, "%s: null output indices or values", fn);
+    int32_t* o_idx = out_idx;
+    float* o_val = out_val;
+    const size_t b_idx = (sizeof(int32_t) * (size_t)total + 15) & ~(size_t)15;
+    if (host) {
+        void* d_out;
+        VB_TRY(workspace(WSP_OUT, b_idx + sizeof(float) * (size_t)total, &d_out));
+        o_idx = (int32_t*)d_out;
+        o_val = (float*)((uint8_t*)d_out + b_idx);
+    }
+    if (elem == VB_VECTOR) dense_write_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(d_in, dim, n, off, o_idx, o_val);
+    else dense_write_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(d_in, dim, n, off, o_idx, o_val);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    if (host) {
+        VB_CUDA(cudaMemcpyAsync(out_idx, o_idx, sizeof(int32_t) * (size_t)total, cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaMemcpyAsync(out_val, o_val, sizeof(float) * (size_t)total, cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaStreamSynchronize(s));
+    }
+    return VB_OK;
+}
+
+// vb_sparsevec_to_dense_batch[_dev]
+static int sparse_to_dense(int elem, int dim, int64_t n, const int64_t* row_off, const int32_t* idx, const float* val, void* out, bool host) {
+    const char* fn = host ? "vb_sparsevec_to_dense_batch" : "vb_sparsevec_to_dense_batch_dev";
+    VB_TRY(require_init());
+    VB_REQUIRE(elem == VB_VECTOR || elem == VB_HALFVEC, "%s: elem must be VB_VECTOR or VB_HALFVEC, got %d", fn, elem);
+    // CheckDim of the target type (src/vector.c, src/halfvec.c: VECTOR_MAX_DIM = HALFVEC_MAX_DIM = 16000)
+    VB_REQUIRE(dim >= 1, "%s must have at least 1 dimension", dense_name(elem));
+    VB_REQUIRE(dim <= 16000, "%s cannot have more than %d dimensions", dense_name(elem), 16000);
+    VB_REQUIRE(n >= 0 && (n == 0 || (row_off && out)), "%s: null rows or output", fn);
+    if (n == 0) return VB_OK;
+    Context& cx = ctx();
+    cudaStream_t s = cx.stream;
+    const int64_t* d_off = row_off;
+    const int32_t* d_idx = idx;
+    const float* d_val = val;
+    int64_t total = 0;
+    if (host) {
+        VB_TRY(check_csr("rows", dim, n, row_off, idx, nullptr));
+        total = row_off[n];
+        VB_REQUIRE(total == 0 || val, "null sparsevec values");
+        const size_t b_off = sizeof(int64_t) * (size_t)(n + 1);
+        const size_t b_idx = (sizeof(int32_t) * (size_t)total + 15) & ~(size_t)15;
+        void* d_rows;
+        VB_TRY(workspace(WSP_ROWS, b_off + b_idx + sizeof(float) * (size_t)total + 64, &d_rows));
+        uint8_t* p = (uint8_t*)d_rows;
+        VB_CUDA(cudaMemcpyAsync(p, row_off, b_off, cudaMemcpyHostToDevice, s));
+        if (total > 0) {
+            VB_CUDA(cudaMemcpyAsync(p + b_off, idx, sizeof(int32_t) * (size_t)total, cudaMemcpyHostToDevice, s));
+            VB_CUDA(cudaMemcpyAsync(p + b_off + b_idx, val, sizeof(float) * (size_t)total, cudaMemcpyHostToDevice, s));
+        }
+        d_off = (const int64_t*)p;
+        d_idx = (const int32_t*)(p + b_off);
+        d_val = (const float*)(p + b_off + b_idx);
+    }
+    const size_t out_bytes = (elem == VB_VECTOR ? sizeof(float) : sizeof(__half)) * (size_t)n * (size_t)dim;
+    void* d_out = out;
+    if (host) VB_TRY(workspace(WSP_OUT, out_bytes, &d_out));
+    SparseCheck* chk;
+    if (host) {   // validated above: only the overflow word is needed
+        void* d;
+        VB_TRY(workspace(WSP_CHECK, sizeof(SparseCheck), &d));
+        chk = (SparseCheck*)d;
+        sparse_check_init_kernel<<<1, 1, 0, s>>>(chk);
+        count_launch();
+    } else {
+        VB_TRY(launch_sparse_check(dim, n, d_off, d_idx, &chk));
+    }
+    const unsigned grid = (unsigned)((n * 32 + 255) / 256);
+    if (elem == VB_VECTOR) sparse_to_dense_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(n, d_off, d_idx, d_val, dim, d_out, chk);
+    else sparse_to_dense_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(n, d_off, d_idx, d_val, dim, d_out, chk);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    SparseCheck hc;
+    VB_CUDA(cudaMemcpyAsync(&hc, chk, sizeof(SparseCheck), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    if (hc.bad != ~0ull) return sparse_check_error("rows", hc.bad);
+    if (!host) VB_REQUIRE(hc.total == 0 || val, "null sparsevec values");
+    if (hc.over != INT64_MAX) {
+        float v;
+        if (host) {
+            v = val[hc.over];
+        } else {   // the error path reads the offending value too
+            VB_CUDA(cudaMemcpyAsync(&v, val + hc.over, sizeof(float), cudaMemcpyDeviceToHost, s));
+            VB_CUDA(cudaStreamSynchronize(s));
+        }
+        return half_range_error(v);
+    }
+    if (host) {
+        VB_CUDA(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaStreamSynchronize(s));
+    }
     return VB_OK;
 }
 
@@ -819,30 +1303,11 @@ int vb_sparse_table_create(int dim, vb_sparse_table** out) {
 }
 
 int vb_sparse_table_append(vb_sparse_table* h, int64_t n, const int64_t* row_off, const int32_t* idx, const float* val) {
-    VB_TRY(require_init());
-    VB_REQUIRE(h && n >= 0 && (n == 0 || row_off), "bad sparse table arguments");
-    if (n == 0) return VB_OK;
-    SparseTable& t = h->t;
-    VB_TRY(check_csr("rows", t.dim, n, row_off, idx, nullptr));
-    const int64_t tot = row_off[n];
-    VB_REQUIRE(tot == 0 || val, "null sparsevec values");
-    VB_TRY(sparse_reserve(t, t.n + n, t.nnz + tot));
-    cudaStream_t s = ctx().stream;
-    // offsets of the new rows: row_off[1..n] + nnz so far
-    VB_CUDA(cudaMemcpyAsync(t.row_off + t.n + 1, row_off + 1, sizeof(int64_t) * (size_t)n, cudaMemcpyHostToDevice, s));
-    if (t.nnz > 0) {
-        sparse_shift_offsets_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(t.row_off + t.n + 1, n, t.nnz);
-        VB_CUDA(cudaGetLastError());
-        count_launch();
-    }
-    if (tot > 0) {
-        VB_CUDA(cudaMemcpyAsync(t.idx + t.nnz, idx, sizeof(int32_t) * (size_t)tot, cudaMemcpyHostToDevice, s));
-        VB_CUDA(cudaMemcpyAsync(t.val + t.nnz, val, sizeof(float) * (size_t)tot, cudaMemcpyHostToDevice, s));
-    }
-    VB_CUDA(cudaStreamSynchronize(s));
-    t.n += n;
-    t.nnz += tot;
-    return VB_OK;
+    return sparse_append(h, n, row_off, idx, val, true);
+}
+
+int vb_sparse_table_append_dev(vb_sparse_table* h, int64_t n, const int64_t* row_off_dev, const int32_t* idx_dev, const float* val_dev) {
+    return sparse_append(h, n, row_off_dev, idx_dev, val_dev, false);
 }
 
 int64_t vb_sparse_table_rows(const vb_sparse_table* h) { return h ? h->t.n : 0; }
@@ -860,59 +1325,65 @@ int vb_sparse_table_free(vb_sparse_table* h) {
 
 int vb_sparse_exact_topk(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, const float* q_val,
                          int k, int64_t* out_ids, double* out_dist) {
-    VB_TRY(require_init());
-    VB_REQUIRE(h && sparse_metric_ok(metric) && metric != VB_IP, "bad sparse table / ordering metric");
-    VB_REQUIRE(k > 0 && k <= 2048, "k must be in 1..2048");
-    if (nq <= 0) return VB_OK;
-    SparseTable& t = h->t;
-    VB_REQUIRE(t.dim == q_dim, "different sparsevec dimensions %d and %d", t.dim, q_dim);
-    VB_REQUIRE(q_off && out_ids && out_dist, "null query / output buffers");
-    int max_q = 0;
-    VB_TRY(check_csr("queries", t.dim, nq, q_off, q_idx, &max_q));
-    Context& c = ctx();
-    cudaStream_t s = c.stream;
-    const int64_t n = t.n;
-    if (n == 0) {
-        for (int64_t i = 0; i < nq * k; ++i) {
-            out_ids[i] = -1;
-            out_dist[i] = INFINITY;
-        }
-        return VB_OK;
-    }
-    // sub-batches keep the key matrix under ~1 GiB
-    const int64_t bq = std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(nq, 65535), (int64_t)(1ull << 30) / (4 * n)));
-    for (int64_t q0 = 0; q0 < nq; q0 += bq) {
-        const int64_t m = std::min(bq, nq - q0);
-        SparseQueries Q;
-        VB_TRY(upload_query_range(q0, m, q_off, q_idx, q_val, &Q));
-        void *d_key, *d_seg;
-        VB_TRY(workspace(WSP_TMP, sizeof(float) * (size_t)m * (size_t)n, &d_key));
-        VB_TRY(launch_sparse_scan(key_metric(metric), t.dim, Q, m, max_q, t.row_off, t.idx, t.val, n, nullptr, (float*)d_key));
-        VB_TRY(workspace(WSP_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
-        int64_t* seg_begin = (int64_t*)d_seg;
-        int32_t* seg_len = (int32_t*)(seg_begin + m);
-        sparse_segments_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(m, n, seg_begin, seg_len);
-        VB_CUDA(cudaGetLastError());
-        count_launch();
-        VB_TRY(sparse_select_finish(metric, m, k, (const float*)d_key, seg_begin, seg_len, nullptr, nullptr, 0, out_ids + q0 * k,
-                                    out_dist + q0 * k));
-    }
-    return VB_OK;
+    return sparse_exact_topk(h, metric, q_dim, nq, q_off, q_idx, q_val, k, true, out_ids, out_dist, nullptr);
+}
+
+int vb_sparse_exact_topk_dev(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off_dev, const int32_t* q_idx_dev,
+                             const float* q_val_dev, int k, int64_t* out_ids_dev, float* out_dist_dev) {
+    return sparse_exact_topk(h, metric, q_dim, nq, q_off_dev, q_idx_dev, q_val_dev, k, false, out_ids_dev, nullptr, out_dist_dev);
 }
 
 int vb_sparse_table_filter_create(vb_sparse_table* h, const int64_t* rows, int64_t n, vb_filter** out) {
     return table_filter_create("vb_sparse_table_filter_create", h, h ? h->uid : 0, h ? h->t.n : 0, FILTER_SPARSE, rows, n, true, out);
 }
 
+int vb_sparse_table_filter_create_dev(vb_sparse_table* h, const int64_t* rows_dev, int64_t n, vb_filter** out) {
+    return table_filter_create("vb_sparse_table_filter_create", h, h ? h->uid : 0, h ? h->t.n : 0, FILTER_SPARSE, rows_dev, n, false, out);
+}
+
 int vb_sparse_exact_topk_filtered(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
                                   const float* q_val, int k, const vb_filter* const* filters, int nfilters, const int32_t* filter_of_query,
                                   int64_t* out_ids, double* out_dist) {
-    return sparse_topk_filtered(h, metric, q_dim, nq, q_off, q_idx, q_val, k, filters, nfilters, filter_of_query, out_ids, out_dist);
+    return sparse_topk_filtered(h, metric, q_dim, nq, q_off, q_idx, q_val, k, filters, nfilters, filter_of_query, true, out_ids, out_dist,
+                                nullptr);
+}
+
+int vb_sparse_exact_topk_filtered_dev(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off_dev,
+                                      const int32_t* q_idx_dev, const float* q_val_dev, int k, const vb_filter* const* filters, int nfilters,
+                                      const int32_t* filter_of_query, int64_t* out_ids_dev, float* out_dist_dev) {
+    return sparse_topk_filtered(h, metric, q_dim, nq, q_off_dev, q_idx_dev, q_val_dev, k, filters, nfilters, filter_of_query, false,
+                                out_ids_dev, nullptr, out_dist_dev);
 }
 
 int vb_sparse_table_rerank(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx,
                            const float* q_val, const int64_t* cand, int c, int k, int64_t* out_ids, double* out_dist) {
-    return sparse_rerank(h, metric, q_dim, nq, q_off, q_idx, q_val, cand, c, k, out_ids, out_dist);
+    return sparse_rerank(h, metric, q_dim, nq, q_off, q_idx, q_val, cand, c, k, true, out_ids, out_dist, nullptr);
+}
+
+int vb_sparse_table_rerank_dev(vb_sparse_table* h, int metric, int q_dim, int64_t nq, const int64_t* q_off_dev, const int32_t* q_idx_dev,
+                               const float* q_val_dev, const int64_t* cand_dev, int c, int k, int64_t* out_ids_dev, float* out_dist_dev) {
+    return sparse_rerank(h, metric, q_dim, nq, q_off_dev, q_idx_dev, q_val_dev, cand_dev, c, k, false, out_ids_dev, nullptr, out_dist_dev);
+}
+
+// ----------------------------------------------------------------------------- casts
+
+int vb_dense_to_sparsevec_batch(int elem, int dim, const void* rows, int64_t n, int64_t cap, int64_t* out_row_off, int32_t* out_idx,
+                                float* out_val) {
+    return dense_to_sparse(elem, dim, rows, n, cap, true, out_row_off, out_idx, out_val);
+}
+
+int vb_dense_to_sparsevec_batch_dev(int elem, int dim, const void* rows_dev, int64_t n, int64_t cap, int64_t* out_row_off_dev,
+                                    int32_t* out_idx_dev, float* out_val_dev) {
+    return dense_to_sparse(elem, dim, rows_dev, n, cap, false, out_row_off_dev, out_idx_dev, out_val_dev);
+}
+
+int vb_sparsevec_to_dense_batch(int elem, int dim, int64_t n, const int64_t* row_off, const int32_t* idx, const float* val, void* out) {
+    return sparse_to_dense(elem, dim, n, row_off, idx, val, out, true);
+}
+
+int vb_sparsevec_to_dense_batch_dev(int elem, int dim, int64_t n, const int64_t* row_off_dev, const int32_t* idx_dev, const float* val_dev,
+                                    void* out_dev) {
+    return sparse_to_dense(elem, dim, n, row_off_dev, idx_dev, val_dev, out_dev, false);
 }
 
 }  // extern "C"

@@ -1,9 +1,14 @@
 """sparsevec on the device -- host-side mirror of the reference's sparsevec functions (src/sparsevec.c:826-1150) over
-the C ABI (vb_sparsevec_* / vb_sparse_table_* / vb_sparse_exact_topk[_filtered]).
+the C ABI (vb_sparsevec_* / vb_sparse_table_* / vb_sparse_exact_topk[_filtered], their _dev variants, and the casts
+vb_dense_to_sparsevec_batch / vb_sparsevec_to_dense_batch).
 
 A value is ``SparseVector(dim, indices, values)`` with 0-based ascending indices (the on-disk order,
 src/sparsevec.h:17-32); the text form '{index:value,...}/dim' is 1-based like the reference's I/O functions.  A batch
 of rows is ``SparseRows`` (CSR).  Everything computes on the GPU; nothing here falls back to numpy math.
+
+Device CSR: the table calls also take rows and queries that live on the GPU, as a ``torch.sparse_csr_tensor`` [n, dim] or
+a ``(row_off, idx, val)`` triple of CUDA tensors, and then return CUDA tensors (int64 ids, float32 distances).  Nothing
+goes through host memory; the library checks the CSR on the device.
 """
 from __future__ import annotations
 
@@ -13,6 +18,9 @@ import numpy as np
 
 from . import _lib
 from ._lib import load
+
+VECTOR, HALFVEC = 0, 1
+INT32_MAX = 2**31 - 1
 
 L2_SQUARED, NEG_IP, COSINE, L1, L2, IP = 0, 1, 2, 3, 6, 7
 SPARSEVEC_MAX_DIM = 1_000_000_000     # src/sparsevec.h:11
@@ -161,6 +169,48 @@ class SparseRows:
         return SparseVector(self.dim, self.idx[b:e], self.val[b:e])
 
 
+def _is_cuda(a):
+    return a is not None and not isinstance(a, np.ndarray) and hasattr(a, "data_ptr") and bool(getattr(a, "is_cuda", False))
+
+
+def _device_csr(x, dim):
+    """(n, dim, row_off, idx, val) of CUDA CSR input in the layout the _dev entry points read (int64 offsets, int32
+    indices, float32 values, contiguous), or None for host input.  x: a torch.sparse_csr_tensor [n, dim] (its dim wins)
+    or a (row_off, idx, val) triple of CUDA tensors.  int64 column indices are narrowed with a range check: a value
+    outside [0, 2^31) becomes -1, which the library's device check refuses ("sparsevec index out of bounds (row r)")."""
+    if isinstance(x, (tuple, list)) and len(x) == 3 and all(_is_cuda(a) for a in x):
+        off, idx, val = x
+    elif _is_cuda(x) and str(getattr(x, "layout", "")) == "torch.sparse_csr":
+        off, idx, val = x.crow_indices(), x.col_indices(), x.values()
+        dim = int(x.shape[1])
+    else:
+        return None
+    import torch
+    if off.dim() != 1 or idx.dim() != 1 or val.dim() != 1 or idx.shape != val.shape or off.numel() < 1:
+        raise ValueError("device CSR: row_off [n + 1], idx [nnz] and val [nnz] must be 1-d, idx and val of one length")
+    if idx.dtype == torch.int64:
+        idx = torch.where((idx >= 0) & (idx <= INT32_MAX), idx, torch.full_like(idx, -1))
+    off = off.to(torch.int64).contiguous()
+    idx = idx.to(torch.int32).contiguous()
+    val = val.to(torch.float32).contiguous()
+    return off.numel() - 1, int(dim), off, idx, val
+
+
+def _run_dev(fn, *args, tensors=()):
+    """a _dev call on tensors torch produced: the library stream waits for torch's, and the results are handed back
+    complete (as the dense calls do)"""
+    from . import _after_torch, synchronize
+    _after_torch(*tensors)
+    rc = getattr(load(), fn)(*args)
+    if rc == _lib.OK:
+        synchronize()
+    return rc
+
+
+def _tp(t):
+    return None if t is None else C.c_void_p(t.data_ptr())
+
+
 def _rows(rows):
     if isinstance(rows, SparseRows):
         return rows
@@ -233,6 +283,100 @@ def l2_normalize(rows):
     return SparseRows(rows.dim, off, idx[:kept], val[:kept])
 
 
+# ------------------------------------------------------------------------- casts between the dense types and sparsevec
+
+_CAP_ERROR = "non-zero elements, more than cap"
+
+
+def _to_sparsevec(elem, rows, cap):
+    if _is_cuda(rows):
+        import torch
+        want = torch.float32 if elem == VECTOR else torch.float16
+        if rows.dtype != want:
+            raise TypeError(f"{'vector' if elem == VECTOR else 'halfvec'} rows must be a {want} CUDA tensor, not {rows.dtype}")
+        x = rows.reshape(1, -1) if rows.dim() == 1 else rows
+        x = x.contiguous()
+        n, dim = int(x.shape[0]), int(x.shape[1])
+        off = torch.empty(n + 1, dtype=torch.int64, device=x.device)
+
+        def run(cap):
+            idx = torch.empty(max(cap, 1), dtype=torch.int32, device=x.device)
+            val = torch.empty(max(cap, 1), dtype=torch.float32, device=x.device)
+            rc = _run_dev("vb_dense_to_sparsevec_batch_dev", elem, dim, _tp(x), n, cap, _tp(off), _tp(idx), _tp(val), tensors=(x,))
+            return rc, idx, val
+        rc, idx, val = run(0 if cap is None else int(cap))
+        if cap is None and rc == _lib.EINVAL and _CAP_ERROR in load().vb_last_error().decode():
+            rc, idx, val = run(int(off[-1].item()))   # the offsets were written: they size the output
+        _lib.check(rc)
+        tot = int(off[-1].item())
+        return off, idx[:tot], val[:tot]
+    if elem == VECTOR:
+        x = np.ascontiguousarray(rows, dtype=np.float32)
+    else:
+        x = np.asarray(rows)
+        x = np.ascontiguousarray(x.view(np.uint16) if x.dtype == np.float16 else x, dtype=np.uint16)
+    x = x.reshape(1, -1) if x.ndim == 1 else x
+    n, dim = x.shape
+    off = np.empty(n + 1, dtype=np.int64)
+
+    def run(cap):
+        idx = np.empty(max(cap, 1), dtype=np.int32)
+        val = np.empty(max(cap, 1), dtype=np.float32)
+        return load().vb_dense_to_sparsevec_batch(elem, dim, _p(x), n, cap, _p(off), _p(idx), _p(val)), idx, val
+    rc, idx, val = run(0 if cap is None else int(cap))
+    if cap is None and rc == _lib.EINVAL and _CAP_ERROR in load().vb_last_error().decode():
+        rc, idx, val = run(int(off[-1]))
+    _lib.check(rc)
+    tot = int(off[-1])
+    return SparseRows(dim, off, idx[:tot], val[:tot])
+
+
+def vector_to_sparsevec(rows, cap=None):
+    """vector -> sparsevec (src/sparsevec.c:606-645) of every row: the nonzero elements in index order (-0 is dropped).
+    numpy float32 [n, dim] -> SparseRows; a float32 CUDA tensor -> (row_off, idx, val) CUDA tensors.  cap: an upper
+    bound of the total nnz, if known (one pass); else the offsets of a first pass size the output."""
+    return _to_sparsevec(VECTOR, rows, cap)
+
+
+def halfvec_to_sparsevec(rows, cap=None):
+    """halfvec -> sparsevec (src/sparsevec.c:650-689): numpy float16 (or uint16 bit patterns) [n, dim] -> SparseRows; a
+    float16 CUDA tensor -> (row_off, idx, val) CUDA tensors; values widened exactly, zeros of either sign dropped"""
+    return _to_sparsevec(HALFVEC, rows, cap)
+
+
+def _to_dense(elem, rows, dim):
+    d = _device_csr(rows, dim)
+    if d is not None:
+        import torch
+        n, dim, off, idx, val = d
+        if dim is None:
+            raise ValueError("dim is required for a (row_off, idx, val) triple")
+        out = torch.empty((n, dim), dtype=torch.float32 if elem == VECTOR else torch.float16, device=off.device)
+        rc = _run_dev("vb_sparsevec_to_dense_batch_dev", elem, dim, n, _tp(off), _tp(idx), _tp(val), _tp(out), tensors=(off, idx, val))
+    else:
+        r = _rows(rows)
+        out = np.empty((r.n, r.dim), dtype=np.float32 if elem == VECTOR else np.float16)
+        rc = load().vb_sparsevec_to_dense_batch(elem, r.dim, r.n, _p(r.row_off), _p(r.idx), _p(r.val), _p(out))
+    if rc == _lib.EINVAL:
+        msg = load().vb_last_error().decode()
+        if "is out of range for type halfvec" in msg or "cannot have more than 16000 dimensions" in msg:
+            raise ValueError(msg)
+    _lib.check(rc)
+    return out
+
+
+def sparsevec_to_vector(rows, dim=None):
+    """sparsevec -> vector (src/vector.c:1323-1349) of every row: SparseRows / SparseVectors -> numpy float32 [n, dim];
+    device CSR (dim needed for a triple) -> a float32 CUDA tensor.  dim above 16000 raises ValueError (CheckDim)."""
+    return _to_dense(VECTOR, rows, dim)
+
+
+def sparsevec_to_halfvec(rows, dim=None):
+    """sparsevec -> halfvec (src/halfvec.c:1199-1225): as sparsevec_to_vector, into float16 by Float4ToHalf; a finite
+    value that overflows raises ValueError('"65520" is out of range for type halfvec')"""
+    return _to_dense(HALFVEC, rows, dim)
+
+
 class SparseTable:
     """sparsevec rows resident in HBM; ``exact_topk`` is the sequential-scan plan ORDER BY v <op> q LIMIT k, with
     row filters (``filter``) for a WHERE clause; ``rerank`` orders candidate rows another index fetched"""
@@ -244,6 +388,15 @@ class SparseTable:
         self.h = h
 
     def append(self, rows):
+        """append rows: SparseVectors, SparseRows, or device CSR (a torch.sparse_csr_tensor or a (row_off, idx, val)
+        triple of CUDA tensors, validated on the device; nothing is appended on any error)"""
+        d = _device_csr(rows, self.dim)
+        if d is not None:
+            n, dim, off, idx, val = d
+            if dim != self.dim:
+                raise ValueError(f"expected {self.dim} dimensions, not {dim}")
+            _lib.check(_run_dev("vb_sparse_table_append_dev", self.h, n, _tp(off), _tp(idx), _tp(val), tensors=(off, idx, val)))
+            return self
         rows = _rows(rows)
         if rows.dim != self.dim:
             raise ValueError(f"expected {self.dim} dimensions, not {rows.dim}")
@@ -259,18 +412,36 @@ class SparseTable:
         return int(load().vb_sparse_table_nnz(self.h))
 
     def filter(self, rows):
-        """a row Filter of this table (WHERE <predicate> as the row numbers it allows, numpy int64).  Rows appended
-        later are not in it."""
+        """a row Filter of this table (WHERE <predicate> as the row numbers it allows: numpy int64, or a 1-d int64 CUDA
+        tensor whose values outside [0, rows) are ignored).  Rows appended later are not in it."""
         from . import Filter
-        rows = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)   # host rows only, like the rest of the sparse API
+        if not _is_cuda(rows):
+            rows = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
         return Filter._create(self, "vb_sparse_table_filter_create", rows)
 
     def exact_topk(self, metric, queries, k, filter=None, filter_of_query=None):
         """ORDER BY v <op> q LIMIT k without an index.  filter: a Filter of this table, or a list of them with
         filter_of_query[q] = the index of query q's filter; each query then gets exactly what rerank() returns for its
-        filter's rows in ascending order (k <= 2048)."""
-        q = _rows(queries)
+        filter's rows in ascending order (k <= 2048).  Device CSR queries return CUDA tensors (float32 distances, the
+        float of the host call's float8); filter_of_query stays a host array."""
         k = int(k)
+        d = _device_csr(queries, self.dim)
+        if d is not None:
+            import torch
+            nq, q_dim, off, idx, val = d
+            ids = torch.empty((nq, k), dtype=torch.int64, device=off.device)
+            dist = torch.empty((nq, k), dtype=torch.float32, device=off.device)
+            qa = (self.h, metric, q_dim, nq, _tp(off), _tp(idx), _tp(val), k)
+            if filter is None:
+                rc = _run_dev("vb_sparse_exact_topk_dev", *qa, _tp(ids), _tp(dist), tensors=(off, idx, val))
+            else:
+                from . import _filter_args
+                farr, nf, fq = _filter_args(filter, filter_of_query)
+                if fq is not None and len(fq) != nq:
+                    raise ValueError(f"filter_of_query must have {nq} entries, got {len(fq)}")
+                rc = _run_dev("vb_sparse_exact_topk_filtered_dev", *qa, farr, nf, _p(fq), _tp(ids), _tp(dist), tensors=(off, idx, val))
+            return self._result(rc, ids, dist)
+        q = _rows(queries)
         ids = np.empty((q.n, k), dtype=np.int64)
         dist = np.empty((q.n, k), dtype=np.float64)
         if filter is None:
@@ -286,9 +457,22 @@ class SparseTable:
 
     def rerank(self, metric, queries, candidates, k):
         """ORDER BY v <op> q LIMIT k over each query's own candidate rows: candidates[q] = row numbers of this table
-        (-1 = none), typically what a dense or quantized index returned (hybrid search)."""
-        q = _rows(queries)
+        (-1 = none), typically what a dense or quantized index returned (hybrid search).  Device CSR queries take a
+        [nq, c] int64 CUDA tensor of candidates (values outside [0, rows) are absent) and return CUDA tensors."""
         k = int(k)
+        d = _device_csr(queries, self.dim)
+        if d is not None:
+            import torch
+            nq, q_dim, off, idx, val = d
+            if not _is_cuda(candidates) or candidates.dtype != torch.int64 or candidates.dim() != 2 or candidates.shape[0] != nq:
+                raise ValueError(f"rerank: candidates of device queries must be an int64 CUDA tensor of shape [{nq}, c]")
+            cand = candidates.contiguous()
+            ids = torch.empty((nq, k), dtype=torch.int64, device=off.device)
+            dist = torch.empty((nq, k), dtype=torch.float32, device=off.device)
+            rc = _run_dev("vb_sparse_table_rerank_dev", self.h, metric, q_dim, nq, _tp(off), _tp(idx), _tp(val), _tp(cand),
+                          int(cand.shape[1]), k, _tp(ids), _tp(dist), tensors=(off, idx, val, cand))
+            return self._result(rc, ids, dist)
+        q = _rows(queries)
         cand = np.asarray(candidates)
         if cand.dtype != np.int64 or cand.ndim != 2 or cand.shape[0] != q.n:
             raise ValueError(f"rerank: candidates must be int64 of shape [{q.n}, c], got {cand.dtype} {cand.shape}")
