@@ -19,7 +19,7 @@
  *   - "host" pointers are ordinary process memory; "_dev" variants take device
  *     pointers valid on the library's current device.  Work is enqueued on the
  *     library stream (vb_stream()); host-buffer variants synchronise before
- *     returning.  _dev variants return with their work enqueued, with three stated
+ *     returning.  _dev variants return with their work enqueued, with these stated
  *     exceptions: the batched vb_ivf_search*_dev read ONE 8-byte pair of certificate
  *     counters per sub-batch of queries, with up to 64 numbers of the queries filter
  *     level 0 could not certify (the tensor-core filter re-runs uncertified queries
@@ -28,7 +28,10 @@
  *     vb_table_aggregate_dev reads sum's 4-byte overflow flag (float_overflow_error), and
  *     the sparsevec _dev calls read the result of their device CSR check: one copy of at
  *     most 24 bytes (first defect, largest row nnz, total nnz) before any other work
- *     (the casts: one copy of at most 32 bytes, see vb_dense_to_sparsevec_batch).
+ *     (the casts: one copy of at most 32 bytes, see vb_dense_to_sparsevec_batch),
+ *     vb_l2_normalize_batch_dev reads its 4-byte overflow flag (float_overflow_error), and
+ *     vb_vector_to_halfvec_batch_dev reads the 8-byte index of the first value that does
+ *     not fit, plus that 4-byte value only when there is one (for the error text).
  *   - rows are row-major and contiguous in the caller's buffers (vector: dim
  *     fp32; halfvec: dim IEEE binary16; bit: (dim+7)/8 bytes, MSB first, tail
  *     bits zero -- exactly the payload of Vector.x (src/vector.h:18-24),
@@ -149,6 +152,39 @@ int			vb_binary_quantize_batch(int elem, int dim, const void *rows, int64_t n, u
  */
 int			vb_vector_to_halfvec_batch(int dim, const void *rows, int64_t n, void *out);
 int			vb_halfvec_to_vector_batch(int dim, const void *rows, int64_t n, void *out);
+/*
+ * subvector(v, start, count) of every row (src/vector.c:983-1025, src/halfvec.c:939-981), the value of the README's
+ * "subvector indexing" recipe.  elem = VB_VECTOR or VB_HALFVEC (there is no bit subvector).  The result's dimension
+ * follows the reference from the scalars alone: count < 1 is an error; end = start > dim - count ? dim + 1 :
+ * start + count; start < 1 becomes 1 and start > dim is an error; out_dim = end - start must pass CheckDim (1 ..
+ * 16000).  The errors are "vector must have at least 1 dimension" ("halfvec ..." for halfvec).  *out_dim is written
+ * once these checks pass, before any work, and is left untouched on any error.  out receives n packed rows of
+ * *out_dim elements; with n = 0, rows and out may be NULL, so such a call sizes the output.
+ */
+int			vb_subvector_batch(int elem, int dim, const void *rows, int64_t n, int32_t start, int32_t count, void *out,
+							   int *out_dim);
+
+/*
+ * The same transforms on rows that already live on the device (a model's output, a resident column), for the
+ * expression-index recipes: embedding::halfvec(n), binary_quantize(embedding)::bit(n) and subvector(embedding, 1, n)
+ * under the cosine opclasses.  Rows and outputs are packed (dim elements per row, no padding; bit rows (dim + 7) / 8
+ * bytes; norms one float8 per row), and each result equals its host variant's bit for bit.  Input and output must not
+ * overlap, except that vb_l2_normalize_batch_dev may run in place (out_dev == rows_dev); another overlap is refused.
+ * Refused before any launch (VB_EINVAL): an elem other than VB_VECTOR / VB_HALFVEC, dim <= 0, n < 0, a NULL pointer with
+ * n > 0.  n = 0 launches nothing.
+ * vb_norm_batch_dev, vb_binary_quantize_batch_dev, vb_halfvec_to_vector_batch_dev and vb_subvector_batch_dev are fully
+ * asynchronous on vb_stream() and use no workspace (they can be captured into a CUDA graph).  The two calls that can
+ * fail on the data read back a little (see the conventions above) and synchronise: vb_l2_normalize_batch_dev returns
+ * VB_EINVAL "value out of range: overflow", vb_vector_to_halfvec_batch_dev the host variant's text for the first
+ * offender in row-major order; on either error out_dev is unspecified.
+ */
+int			vb_norm_batch_dev(int elem, int dim, const void *rows_dev, int64_t n, double *out_dev);
+int			vb_l2_normalize_batch_dev(int elem, int dim, const void *rows_dev, int64_t n, void *out_dev);
+int			vb_binary_quantize_batch_dev(int elem, int dim, const void *rows_dev, int64_t n, uint8_t *out_dev);
+int			vb_vector_to_halfvec_batch_dev(int dim, const void *rows_dev, int64_t n, void *out_dev);
+int			vb_halfvec_to_vector_batch_dev(int dim, const void *rows_dev, int64_t n, void *out_dev);
+int			vb_subvector_batch_dev(int elem, int dim, const void *rows_dev, int64_t n, int32_t start, int32_t count,
+								   void *out_dev, int *out_dim);
 
 /* ------------------------------------------------------ resident row tables */
 

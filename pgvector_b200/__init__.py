@@ -518,16 +518,24 @@ class IvfflatIndex:
         """INSERT into the resident image without reloading it (InsertTuple, src/ivfinsert.c:72-181, row after row):
         each row is appended to the list FindInsertPage picks.  Returns the lists (int32 [n]).  ids are the rows' heap
         ids.  Cosine opclasses: the rows are l2-normalised here, and a row of norm 0 is skipped with list -1, as
-        IvfflatCheckNorm does.  torch CUDA rows take the device path (cosine rows are normalised on the host); their
-        ids are taken as int64 on the rows' device."""
+        IvfflatCheckNorm does.  torch CUDA rows take the device path, normalisation included (vector_norm and
+        l2_normalize on the device); their ids are taken as int64 on the rows' device."""
         n = rows.shape[0] if rows.ndim > 1 else 1
         out = np.full(n, -1, dtype=np.int32)
-        if _is_torch(rows) and rows.is_cuda and not self.normalize:
+        if _is_torch(rows) and rows.is_cuda:
             import torch
             rows = self._device_rows(rows, n)
             ids = torch.as_tensor(ids, device=rows.device).to(torch.int64).reshape(n).contiguous()
+            keep = slice(None)
+            if self.normalize:
+                keep_dev = torch.nonzero(vector_norm(rows, self.elem) > 0).reshape(-1)
+                rows = l2_normalize(rows[keep_dev], self.elem) if keep_dev.numel() else rows[keep_dev]
+                ids = ids[keep_dev].contiguous()
+                keep = keep_dev.cpu().numpy()
+            got = np.empty(rows.shape[0], dtype=np.int32)
             _after_torch(rows, ids)
-            _lib.check(load().vb_ivf_insert_dev(self.h, _ptr(rows), _ptr(ids), n, _ptr(out)))
+            _lib.check(load().vb_ivf_insert_dev(self.h, _ptr(rows), _ptr(ids), rows.shape[0], _ptr(got)))
+            out[keep] = got
         else:
             if _is_torch(rows):
                 rows = rows.cpu().numpy()
@@ -1182,9 +1190,46 @@ def set_option(name: str, value: int):
 
 
 # --------------------------------------------------------------------- row transforms
+#
+# numpy rows run the host variants and return numpy arrays (halfvec: uint16 bit patterns).  torch CUDA rows run the _dev
+# variants, which read the rows where they are, and return CUDA tensors: norms float64, vector rows float32, halfvec rows
+# float16 (any 2-byte dtype is read as binary16 bit patterns), bit rows uint8 [n, (dim + 7) // 8].
+
+def _is_cuda(a):
+    return _is_torch(a) and a.is_cuda
+
+
+def _dev_rows(rows, elem):
+    """torch CUDA rows as the _dev transforms read them: (2-d contiguous rows, whether a single row was given)"""
+    import torch
+    if elem == VECTOR and rows.dtype != torch.float32:
+        raise TypeError(f"vector rows on the device must be float32, not {rows.dtype}")
+    if elem == HALFVEC and (rows.element_size() != 2 or rows.dtype.is_complex):
+        raise TypeError(f"halfvec rows on the device must have a 2-byte dtype, not {rows.dtype}")
+    if elem not in (VECTOR, HALFVEC):
+        raise ValueError(f"elem must be VECTOR or HALFVEC, not {elem}")
+    single = rows.dim() == 1
+    r2 = rows.reshape(1, -1) if single else rows
+    if r2.dim() != 2:
+        raise ValueError(f"rows must be 1-d or 2-d, got shape {tuple(rows.shape)}")
+    return r2.contiguous(), single
+
+
+def _dev_call(fn, *args, inputs=()):
+    """a _dev transform after torch's pending work on its inputs; the results are complete when it returns"""
+    _after_torch(*inputs)
+    _lib.check(fn(*args))
+    synchronize()   # the library runs on its own stream; results are handed back complete
+
 
 def vector_norm(rows, elem=VECTOR):
     """vector_norm / l2_norm of every row (src/vector.c:767-780, src/halfvec.c:703-720)."""
+    if _is_cuda(rows):
+        import torch
+        r2, single = _dev_rows(rows, elem)
+        out = torch.empty(r2.shape[0], dtype=torch.float64, device=r2.device)
+        _dev_call(load().vb_norm_batch_dev, elem, r2.shape[1], _ptr(r2), r2.shape[0], _ptr(out), inputs=(r2,))
+        return out[0] if single else out
     rows = _host(elem, rows)
     single = rows.ndim == 1
     r2 = rows.reshape(1, -1) if single else rows
@@ -1195,36 +1240,54 @@ def vector_norm(rows, elem=VECTOR):
 
 def l2_normalize(rows, elem=VECTOR):
     """l2_normalize of every row (src/vector.c:785-819, src/halfvec.c:725-759); raises OverflowError like the reference."""
-    rows = _host(elem, rows)
-    single = rows.ndim == 1
-    r2 = np.ascontiguousarray(rows.reshape(1, -1) if single else rows)
-    out = np.empty_like(r2)
     try:
+        if _is_cuda(rows):
+            import torch
+            r2, single = _dev_rows(rows, elem)
+            out = torch.empty(r2.shape, dtype=torch.float32 if elem == VECTOR else torch.float16, device=r2.device)
+            _dev_call(load().vb_l2_normalize_batch_dev, elem, r2.shape[1], _ptr(r2), r2.shape[0], _ptr(out), inputs=(r2,))
+            return out[0] if single else out
+        rows = _host(elem, rows)
+        single = rows.ndim == 1
+        r2 = np.ascontiguousarray(rows.reshape(1, -1) if single else rows)
+        out = np.empty_like(r2)
         _lib.check(load().vb_l2_normalize_batch(elem, r2.shape[1], _ptr(r2), r2.shape[0], _ptr(out)))
+        return out[0] if single else out
     except VecB200Error as e:
         if "overflow" in str(e):
             raise OverflowError("value out of range: overflow") from None
         raise
-    return out[0] if single else out
 
 
 def vector_to_halfvec(rows):
     """vector::halfvec (src/halfvec.c:540-555): RNE to half bit patterns; raises like the reference on overflow"""
-    rows = _host(VECTOR, rows)
-    single = rows.ndim == 1
-    r2 = np.ascontiguousarray(rows.reshape(1, -1) if single else rows)
-    out = np.empty(r2.shape, dtype=np.uint16)
     try:
+        if _is_cuda(rows):
+            import torch
+            r2, single = _dev_rows(rows, VECTOR)
+            out = torch.empty(r2.shape, dtype=torch.float16, device=r2.device)
+            _dev_call(load().vb_vector_to_halfvec_batch_dev, r2.shape[1], _ptr(r2), r2.shape[0], _ptr(out), inputs=(r2,))
+            return out[0] if single else out
+        rows = _host(VECTOR, rows)
+        single = rows.ndim == 1
+        r2 = np.ascontiguousarray(rows.reshape(1, -1) if single else rows)
+        out = np.empty(r2.shape, dtype=np.uint16)
         _lib.check(load().vb_vector_to_halfvec_batch(r2.shape[1], _ptr(r2), r2.shape[0], _ptr(out)))
+        return out[0] if single else out
     except VecB200Error as e:
         if "out of range for type halfvec" in str(e):
             raise ValueError(str(e).split(": ", 1)[1]) from None
         raise
-    return out[0] if single else out
 
 
 def halfvec_to_vector(rows):
     """halfvec::vector: exact widening"""
+    if _is_cuda(rows):
+        import torch
+        r2, single = _dev_rows(rows, HALFVEC)
+        out = torch.empty(r2.shape, dtype=torch.float32, device=r2.device)
+        _dev_call(load().vb_halfvec_to_vector_batch_dev, r2.shape[1], _ptr(r2), r2.shape[0], _ptr(out), inputs=(r2,))
+        return out[0] if single else out
     rows = _host(HALFVEC, rows)
     single = rows.ndim == 1
     r2 = np.ascontiguousarray(rows.reshape(1, -1) if single else rows)
@@ -1235,9 +1298,53 @@ def halfvec_to_vector(rows):
 
 def binary_quantize(rows, elem=VECTOR):
     """binary_quantize of every row (src/vector.c:952-978): packed bits, MSB first."""
+    if _is_cuda(rows):
+        import torch
+        r2, single = _dev_rows(rows, elem)
+        out = torch.empty((r2.shape[0], (r2.shape[1] + 7) // 8), dtype=torch.uint8, device=r2.device)
+        _dev_call(load().vb_binary_quantize_batch_dev, elem, r2.shape[1], _ptr(r2), r2.shape[0], _ptr(out), inputs=(r2,))
+        return out[0] if single else out
     rows = _host(elem, rows)
     single = rows.ndim == 1
     r2 = np.ascontiguousarray(rows.reshape(1, -1) if single else rows)
     out = np.empty((r2.shape[0], (r2.shape[1] + 7) // 8), dtype=np.uint8)
     _lib.check(load().vb_binary_quantize_batch(elem, r2.shape[1], _ptr(r2), r2.shape[0], _ptr(out)))
+    return out[0] if single else out
+
+
+def subvector(rows, start, count, elem=VECTOR):
+    """subvector(v, start, count) of every row (src/vector.c:983-1025, src/halfvec.c:939-981): `count` elements from
+    1-based `start`, clipped to the row as the reference clips them.  The reference's errors ("vector must have at least
+    1 dimension", ...) raise ValueError."""
+    lib = load()
+    dev = _is_cuda(rows)
+    if dev:
+        r2, single = _dev_rows(rows, elem)
+        fn = lib.vb_subvector_batch_dev
+    else:
+        r2 = _host(elem, rows)
+        single = r2.ndim == 1
+        r2 = np.ascontiguousarray(r2.reshape(1, -1) if single else r2)
+        fn = lib.vb_subvector_batch
+    n, dim = r2.shape
+    d = C.c_int(0)
+
+    def call(src, m, out):
+        rc = fn(elem, dim, src, m, int(start), int(count), out, C.byref(d))
+        if rc == _lib.EINVAL:
+            msg = lib.vb_last_error().decode()
+            if msg.endswith(" must have at least 1 dimension") or " cannot have more than " in msg:
+                raise ValueError(msg)
+        _lib.check(rc)
+
+    call(None, 0, None)   # n = 0 sizes the output
+    if dev:
+        import torch
+        out = torch.empty((n, d.value), dtype=torch.float32 if elem == VECTOR else torch.float16, device=r2.device)
+        _after_torch(r2)
+        call(_ptr(r2), n, _ptr(out))
+        synchronize()   # the library runs on its own stream; results are handed back complete
+    else:
+        out = np.empty((n, d.value), dtype=_NP[elem])
+        call(_ptr(r2), n, _ptr(out))
     return out[0] if single else out

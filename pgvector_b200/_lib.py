@@ -35,6 +35,13 @@ SIGNATURES = {
     "vb_binary_quantize_batch": (_i, [_i, _i, _vp, _i64, _vp]),
     "vb_vector_to_halfvec_batch": (_i, [_i, _vp, _i64, _vp]),
     "vb_halfvec_to_vector_batch": (_i, [_i, _vp, _i64, _vp]),
+    "vb_subvector_batch": (_i, [_i, _i, _vp, _i64, C.c_int32, C.c_int32, _vp, C.POINTER(_i)]),
+    "vb_norm_batch_dev": (_i, [_i, _i, _vp, _i64, _vp]),
+    "vb_l2_normalize_batch_dev": (_i, [_i, _i, _vp, _i64, _vp]),
+    "vb_binary_quantize_batch_dev": (_i, [_i, _i, _vp, _i64, _vp]),
+    "vb_vector_to_halfvec_batch_dev": (_i, [_i, _vp, _i64, _vp]),
+    "vb_halfvec_to_vector_batch_dev": (_i, [_i, _vp, _i64, _vp]),
+    "vb_subvector_batch_dev": (_i, [_i, _i, _vp, _i64, C.c_int32, C.c_int32, _vp, C.POINTER(_i)]),
     "vb_sparsevec_distance_batch": (_i, [_i, _i, _i, C.c_int32, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "vb_sparsevec_norm_batch": (_i, [_i64, _vp, _vp, _vp]),
     "vb_sparsevec_l2_normalize_batch": (_i, [_i64, _vp, _vp, _vp, _vp, _vp, _vp]),
