@@ -31,7 +31,9 @@
  *     (the casts: one copy of at most 32 bytes, see vb_dense_to_sparsevec_batch),
  *     vb_l2_normalize_batch_dev reads its 4-byte overflow flag (float_overflow_error), and
  *     vb_vector_to_halfvec_batch_dev reads the 8-byte index of the first value that does
- *     not fit, plus that 4-byte value only when there is one (for the error text).
+ *     not fit, plus that 4-byte value only when there is one (for the error text), and
+ *     vb_sparse_order_bounds_dev reads the result of its device CSR check like the other
+ *     sparsevec _dev calls.
  *   - rows are row-major and contiguous in the caller's buffers (vector: dim
  *     fp32; halfvec: dim IEEE binary16; bit: (dim+7)/8 bytes, MSB first, tail
  *     bits zero -- exactly the payload of Vector.x (src/vector.h:18-24),
@@ -448,6 +450,70 @@ int			vb_sparsevec_to_dense_batch(int elem, int dim, int64_t n, const int64_t *r
 										void *out);
 int			vb_sparsevec_to_dense_batch_dev(int elem, int dim, int64_t n, const int64_t *row_off_dev, const int32_t *idx_dev,
 											const float *val_dev, void *out_dev);
+
+/* ------------------------------------------------------------ ordering by value */
+
+/*
+ * The btree operator classes vector_ops, halfvec_ops and sparsevec_ops (sql/vector.sql:397, 810, 1180) over a resident
+ * table: ORDER BY v, SELECT DISTINCT v, GROUP BY v, the tuplesort of CREATE [UNIQUE] INDEX ON t (v), and the lookups
+ * WHERE v = $1, v IN (...), v < / <= / >= / > $1.
+ *
+ * Comparators.  Rows are ordered by the reference's comparator of their type:
+ *   vector, halfvec  element by element with < and > on float (halfvec: on HalfToFloat4), the dimension deciding only
+ *                    after that (vector_cmp_internal, src/vector.c:1030-1052; halfvec_cmp_internal, src/halfvec.c:987).
+ *                    Every row of a table has its dimension, so -0 and +0 are equal and +-inf are ordinary values.
+ *   sparsevec        sparsevec_cmp_internal (src/sparsevec.c:1153-1188).  For rows of one dimension it is the
+ *                    lexicographic order of 64-bit keys, one per stored entry (i, v): v < 0: (i << 32) | f(v), otherwise
+ *                    (2 << 62) | ((2^30 - 1 - i) << 32) | f(v), each row ending with the key 1 << 62, where f is the
+ *                    order-preserving map of fp32 bits with -0 made +0.  Exact with stored zeros and +-inf.
+ * Ties: equal rows are ordered by ascending row number (tuplesort gives no stable order; this one is deterministic).
+ * NaN: the reference's input functions refuse it, device rows can hold it.  A row containing NaN does not fail the
+ * call, which still returns a permutation, but where such a row lands is unspecified.
+ *
+ * Results.  perm [n]: row numbers in order.  A group is a maximal run of equal rows in the order; groups are numbered
+ * 0, 1, ... ascending, so group_of_row [n] is the dense rank of each row's value -- the group_of_row vb_table_aggregate
+ * takes, which makes GROUP BY v two calls.  group_start [groups + 1]: the position in perm of each group's first row,
+ * group_start[groups] = n.  DISTINCT v is perm[group_start[g]] for each g (the smallest row number of each group);
+ * count(*) of group g is group_start[g + 1] - group_start[g].  ORDER BY v LIMIT k is perm[0 .. k).
+ *
+ * Bounds.  For each query q, lo = the number of ordered rows < q and hi = the number <= q; the rows equal to q are
+ * perm[lo .. hi), which serves all five btree strategies.  Queries have the table's dimension (dense: packed rows of
+ * dim elements; sparse: CSR as the sparse calls take it, a q_dim other than the table's fails with CheckDims' text,
+ * "different sparsevec dimensions %d and %d").
+ *
+ * Lifetime.  An order covers the rows its table held at creation (vb_order_rows); rows appended later are not in it
+ * and it stays valid, since row numbers do not move.  Bounds read the rows through the table's current buffers, so a
+ * table that grew still works.  Bounds on an order whose table was freed fail with VB_EINVAL, and so does a dense order
+ * given to a sparse bounds call or the reverse; reads need only the order.
+ *
+ * Refusals and failure.  A bit table fails with VB_EINVAL (pgvector has no btree operator class for bit; bit columns
+ * use PostgreSQL's bit_ops), and so does a table of 2^31 rows or more (group_of_row is int32).  Everything is validated
+ * before any launch; on any error nothing is written to the outputs.  VB_ENOMEM names the bytes needed and leaves
+ * nothing allocated.  n = 0 gives an empty order with 0 groups.
+ *
+ * Synchronisation.  Creation synchronises: the sort is host-driven and reads back one 16-byte count per refinement
+ * pass (vb_order_passes: at most the key length + 1, that is dim + 1 for vector, about dim / 2 + 1 for halfvec and
+ * max nnz + 2 for sparsevec; a table of identical rows takes at most 2).  vb_order_read and the host bounds calls
+ * synchronise; vb_order_read_dev and vb_order_bounds_dev are asynchronous on vb_stream() and use no workspace (they can
+ * be captured into a CUDA graph); vb_sparse_order_bounds_dev reads its CSR check first (see the conventions above).
+ * Each output of vb_order_read may be NULL.
+ */
+typedef struct vb_order vb_order;
+int			vb_table_order_create(vb_table *t, vb_order **out);	/* VB_VECTOR / VB_HALFVEC tables */
+int			vb_sparse_table_order_create(vb_sparse_table *t, vb_order **out);
+int64_t		vb_order_rows(const vb_order *o);		/* rows ordered: the table's row count at creation */
+int64_t		vb_order_groups(const vb_order *o);		/* distinct values */
+int64_t		vb_order_passes(const vb_order *o);		/* refinement passes the sort took */
+int			vb_order_read(const vb_order *o, int64_t *perm, int32_t *group_of_row, int64_t *group_start);
+int			vb_order_read_dev(const vb_order *o, int64_t *perm_dev, int32_t *group_of_row_dev, int64_t *group_start_dev);
+int			vb_order_bounds(vb_order *o, const void *queries, int64_t nq, int64_t *out_lo, int64_t *out_hi);
+int			vb_order_bounds_dev(vb_order *o, const void *queries_dev, int64_t nq, int64_t *out_lo_dev, int64_t *out_hi_dev);
+int			vb_sparse_order_bounds(vb_order *o, int q_dim, int64_t nq, const int64_t *q_off, const int32_t *q_idx,
+								   const float *q_val, int64_t *out_lo, int64_t *out_hi);
+/* device CSR checked as in the other sparse _dev calls */
+int			vb_sparse_order_bounds_dev(vb_order *o, int q_dim, int64_t nq, const int64_t *q_off_dev, const int32_t *q_idx_dev,
+									   const float *q_val_dev, int64_t *out_lo_dev, int64_t *out_hi_dev);
+int			vb_order_free(vb_order *o);
 
 /* ---------------------------------------------------------------- IVFFlat */
 

@@ -361,6 +361,11 @@ class Table:
             _lib.check(load().vb_table_aggregate(self.h, agg, _ptr(groups), ngroups, run_rows, _ptr(vals), _ptr(counts), _ptr(st)))
         return (vals, counts, st) if state else (vals, counts)
 
+    def order(self):
+        """the rows in vector_ops / halfvec_ops btree order (ORDER BY v, DISTINCT v, GROUP BY v, WHERE v = / < ... $1)
+        as an Order; rows appended later are not in it"""
+        return Order._create(self, "vb_table_order_create", False)
+
     def exact_topk_sharded(self, metric, queries_dev, k, id_offset):
         """exact top-k over a row-sharded table (collective over the library's communicator); torch CUDA tensors"""
         import torch
@@ -818,6 +823,123 @@ class Filter:
     def free(self):
         if self.h:
             load().vb_filter_free(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.free()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class Order:
+    """The rows of one Table or SparseTable in the order of its btree operator class (vector_ops, halfvec_ops,
+    sparsevec_ops), ties by ascending row number, with the groups of equal rows: perm [n] (row numbers in order),
+    group_of_row [n] (dense rank of each row's value, what Table.avg / Table.sum take as groups), group_start
+    [groups + 1] (position in perm of each group's first row, then n).  bounds(queries) -> (lo, hi): the rows equal to
+    query q are perm[lo[q]:hi[q]].  Made by Table.order / SparseTable.order; free it (or use it as a context manager)
+    when done."""
+
+    def __init__(self, owner, h, sparse):
+        self.owner, self.h, self.sparse = owner, h, sparse
+
+    @classmethod
+    def _create(cls, owner, fn, sparse):
+        h = C.c_void_p()
+        _lib.check(getattr(load(), fn)(owner.h, C.byref(h)))
+        return cls(owner, h, sparse)
+
+    @property
+    def rows(self):
+        """rows ordered: the table's row count when the order was made"""
+        return int(load().vb_order_rows(self.h))
+
+    @property
+    def groups(self):
+        return int(load().vb_order_groups(self.h))
+
+    @property
+    def passes(self):
+        """refinement passes the sort took"""
+        return int(load().vb_order_passes(self.h))
+
+    def read(self, device=False):
+        """(perm int64 [n], group_of_row int32 [n], group_start int64 [groups + 1]): numpy arrays, or CUDA tensors with
+        device=True"""
+        n, g = self.rows, self.groups
+        if device:
+            import torch
+            perm = torch.empty(n, dtype=torch.int64, device="cuda")
+            gor = torch.empty(n, dtype=torch.int32, device="cuda")
+            gst = torch.empty(g + 1, dtype=torch.int64, device="cuda")
+            _lib.check(load().vb_order_read_dev(self.h, _ptr(perm), _ptr(gor), _ptr(gst)))
+            synchronize()   # the library runs on its own stream; results are handed back complete
+            return perm, gor, gst
+        perm = np.empty(n, dtype=np.int64)
+        gor = np.empty(n, dtype=np.int32)
+        gst = np.empty(g + 1, dtype=np.int64)
+        _lib.check(load().vb_order_read(self.h, _ptr(perm), _ptr(gor), _ptr(gst)))
+        return perm, gor, gst
+
+    @property
+    def perm(self):
+        out = np.empty(self.rows, dtype=np.int64)
+        _lib.check(load().vb_order_read(self.h, _ptr(out), None, None))
+        return out
+
+    @property
+    def group_of_row(self):
+        out = np.empty(self.rows, dtype=np.int32)
+        _lib.check(load().vb_order_read(self.h, None, _ptr(out), None))
+        return out
+
+    @property
+    def group_start(self):
+        out = np.empty(self.groups + 1, dtype=np.int64)
+        _lib.check(load().vb_order_read(self.h, None, None, _ptr(out)))
+        return out
+
+    def bounds(self, queries):
+        """(lo, hi) per query: the number of ordered rows < q and <= q.  Dense orders take rows of the table's type (numpy,
+        or a CUDA tensor of float32 / float16 rows, which returns CUDA tensors); sparse orders take SparseRows /
+        SparseVectors or device CSR, as SparseTable.exact_topk does."""
+        if self.sparse:
+            return sparsevec._order_bounds(self, queries)
+        t = self.owner
+        if _is_torch(queries):
+            import torch
+            want = torch.float32 if t.elem == VECTOR else torch.float16
+            q = queries.reshape(1, -1) if queries.dim() == 1 else queries
+            if not q.is_cuda or q.dtype != want or q.dim() != 2 or q.shape[1] != t.dim:
+                raise ValueError(f"bounds: queries must be a {want} CUDA tensor of shape [nq, {t.dim}]")
+            q = q.contiguous()
+            nq = q.shape[0]
+            lo = torch.empty(nq, dtype=torch.int64, device=q.device)
+            hi = torch.empty(nq, dtype=torch.int64, device=q.device)
+            _after_torch(q)
+            _lib.check(load().vb_order_bounds_dev(self.h, _ptr(q), nq, _ptr(lo), _ptr(hi)))
+            synchronize()   # the library runs on its own stream; results are handed back complete
+            return lo, hi
+        q = _host(t.elem, queries)
+        if q.ndim == 1:
+            q = q.reshape(1, -1)
+        if q.ndim != 2 or q.shape[1] != t.dim:
+            raise ValueError(f"bounds: queries must have shape [nq, {t.dim}], got {q.shape}")
+        nq = q.shape[0]
+        lo = np.empty(nq, dtype=np.int64)
+        hi = np.empty(nq, dtype=np.int64)
+        _lib.check(load().vb_order_bounds(self.h, _ptr(q), nq, _ptr(lo), _ptr(hi)))
+        return lo, hi
+
+    def free(self):
+        if self.h:
+            load().vb_order_free(self.h)
             self.h = None
 
     def __enter__(self):

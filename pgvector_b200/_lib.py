@@ -83,6 +83,18 @@ SIGNATURES = {
     "vb_exact_topk_filtered_dev": (_i, [_vp, _i, _vp, _i64, _i, _vp, _i, _vp, _vp, _vp]),
     "vb_table_aggregate": (_i, [_vp, _i, _vp, _i, _i64, _vp, _vp, _vp]),
     "vb_table_aggregate_dev": (_i, [_vp, _i, _vp, _i, _i64, _vp, _vp, _vp]),
+    "vb_table_order_create": (_i, [_vp, C.POINTER(_vp)]),
+    "vb_sparse_table_order_create": (_i, [_vp, C.POINTER(_vp)]),
+    "vb_order_rows": (_i64, [_vp]),
+    "vb_order_groups": (_i64, [_vp]),
+    "vb_order_passes": (_i64, [_vp]),
+    "vb_order_read": (_i, [_vp, _vp, _vp, _vp]),
+    "vb_order_read_dev": (_i, [_vp, _vp, _vp, _vp]),
+    "vb_order_bounds": (_i, [_vp, _vp, _i64, _vp, _vp]),
+    "vb_order_bounds_dev": (_i, [_vp, _vp, _i64, _vp, _vp]),
+    "vb_sparse_order_bounds": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "vb_sparse_order_bounds_dev": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "vb_order_free": (_i, [_vp]),
     "vb_ivf_create": (_i, [_i, _i, _i, _i, C.POINTER(_vp)]),
     "vb_ivf_load": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "vb_ivf_load_dev": (_i, [_vp, _vp, _vp, _vp, _vp]),

@@ -326,6 +326,10 @@ int launch_ivf_filter_lists(int64_t nq, int max_probes, int lists, const int32_t
 // process-wide unique stamp of a table, sparse table, IVFFlat or HNSW image: a filter matches its owner by address and
 // stamp, so a filter that outlived its owner is refused even when a new owner is allocated at the same address
 uint64_t next_owner_uid();
+// Orders (vb_order.cu) read their table at every bounds call: owner_watch(uid) at an order's creation, owner_released(uid)
+// when a table is freed, so that an order of a freed table is refused.
+void owner_watch(uint64_t uid);
+void owner_released(uint64_t uid);
 enum FilterKind { FILTER_TABLE, FILTER_IVF, FILTER_HNSW, FILTER_SPARSE };
 struct Filter {
     const void* owner = nullptr;   // the vb_table, vb_sparse_table, vb_ivf or vb_hnsw it was made for
@@ -394,6 +398,23 @@ int launch_filter_chunks(const FilterQuery* qa_dev, int64_t nq, int rows_per_chu
 // *n_chunks (device, zeroed by the caller)
 int launch_rerank_prepare(const int64_t* cand, int64_t nq, int c, int64_t n, int rows_per_chunk, int64_t* ids, int64_t* seg_begin,
                           int32_t* seg_len, Chunk* chunks, int* n_chunks);
+
+// ---------------------------------------------------------------- sparse CSR for the orders (vb_sparse.cu)
+struct SparseCsr {
+    int dim;
+    int64_t n;
+    const int64_t* off;   // [n + 1] device
+    const int32_t* idx;
+    const float* val;
+};
+// the resident rows of a sparse table as they are now (its buffers move when it grows), and its stamp
+SparseCsr sparse_table_csr(const vb_sparse_table* h);
+uint64_t sparse_table_uid(const vb_sparse_table* h);
+// nq >= 1 sparse queries of a call on a table of dimension dim, checked with the sparse calls' rules and texts (CheckDims,
+// then the CSR: host variant on the host, device CSR by the one checked read-back) and on the device: host CSR uploaded
+// to the queries' workspace, device CSR used in place
+int sparse_queries_on_device(int dim, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, const float* q_val, bool host,
+                             SparseCsr* out);
 
 int list_tile_rows();
 bool list_major_supported(int elem, int key_metric);

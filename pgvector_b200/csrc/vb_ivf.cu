@@ -1035,6 +1035,7 @@ const void* vb_table_device_rows(const vb_table* t, size_t* stride_bytes) {
 int vb_table_free(vb_table* t) {
     if (t) {
         table_free(t->t);
+        owner_released(t->uid);
         delete t;
     }
     return VB_OK;

@@ -695,6 +695,29 @@ static int sparse_topk_args(vb_sparse_table* h, int metric, int q_dim, int64_t n
     return VB_OK;
 }
 
+SparseCsr sparse_table_csr(const vb_sparse_table* h) { return SparseCsr{h->t.dim, h->t.n, h->t.row_off, h->t.idx, h->t.val}; }
+
+uint64_t sparse_table_uid(const vb_sparse_table* h) { return h->uid; }
+
+int sparse_queries_on_device(int dim, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, const float* q_val, bool host,
+                             SparseCsr* out) {
+    VB_REQUIRE(dim == q_dim, "different sparsevec dimensions %d and %d", dim, q_dim);
+    VB_REQUIRE(q_off, "null query / output buffers");
+    if (host) {
+        VB_TRY(check_csr("queries", dim, nq, q_off, q_idx, nullptr));
+        VB_REQUIRE(q_off[nq] == 0 || q_val, "null query / output buffers");
+        SparseQueries Q;
+        VB_TRY(upload_query_range(0, nq, q_off, q_idx, q_val, &Q));
+        *out = SparseCsr{dim, nq, Q.off, Q.idx, Q.val};
+        return VB_OK;
+    }
+    int64_t total = 0;
+    VB_TRY(check_csr_dev("queries", dim, nq, q_off, q_idx, nullptr, &total));
+    VB_REQUIRE(total == 0 || q_val, "null query / output buffers");
+    *out = SparseCsr{dim, nq, q_off, q_idx, q_val};
+    return VB_OK;
+}
+
 // Filtered top-k, one sub-batch after the other: filter_chunks_kernel lays out the chunks of each query's allowed rows
 // (a filter's queries in one block), sparse_gather_kernel scores them (one launch per block that fills the grid, so the
 // grid reads one filter's rows at a time), then the selection and the epilogue of vb_sparse_exact_topk.  host == false:
@@ -1318,6 +1341,7 @@ int vb_sparse_table_free(vb_sparse_table* h) {
         if (h->t.row_off) cudaFree(h->t.row_off);
         if (h->t.idx) cudaFree(h->t.idx);
         if (h->t.val) cudaFree(h->t.val);
+        owner_released(h->uid);
         delete h;
     }
     return VB_OK;

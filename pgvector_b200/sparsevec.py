@@ -377,6 +377,24 @@ def sparsevec_to_halfvec(rows, dim=None):
     return _to_dense(HALFVEC, rows, dim)
 
 
+def _order_bounds(order, queries):
+    """Order.bounds of a sparse table's order: SparseRows / SparseVectors -> numpy (lo, hi); device CSR -> CUDA tensors"""
+    d = _device_csr(queries, order.owner.dim)
+    if d is not None:
+        import torch
+        nq, q_dim, off, idx, val = d
+        lo = torch.empty(nq, dtype=torch.int64, device=off.device)
+        hi = torch.empty(nq, dtype=torch.int64, device=off.device)
+        rc = _run_dev("vb_sparse_order_bounds_dev", order.h, q_dim, nq, _tp(off), _tp(idx), _tp(val), _tp(lo), _tp(hi),
+                      tensors=(off, idx, val))
+        return SparseTable._result(rc, lo, hi)
+    q = _rows(queries)
+    lo = np.empty(q.n, dtype=np.int64)
+    hi = np.empty(q.n, dtype=np.int64)
+    rc = load().vb_sparse_order_bounds(order.h, q.dim, q.n, _p(q.row_off), _p(q.idx), _p(q.val), _p(lo), _p(hi))
+    return SparseTable._result(rc, lo, hi)
+
+
 class SparseTable:
     """sparsevec rows resident in HBM; ``exact_topk`` is the sequential-scan plan ORDER BY v <op> q LIMIT k, with
     row filters (``filter``) for a WHERE clause; ``rerank`` orders candidate rows another index fetched"""
@@ -482,6 +500,12 @@ class SparseTable:
         rc = load().vb_sparse_table_rerank(self.h, metric, q.dim, q.n, _p(q.row_off), _p(q.idx), _p(q.val), _p(cand), cand.shape[1], k,
                                            _p(ids), _p(dist))
         return self._result(rc, ids, dist)
+
+    def order(self):
+        """the rows in sparsevec_ops btree order (ORDER BY v, DISTINCT v, GROUP BY v, WHERE v = / < ... $1) as an
+        Order; rows appended later are not in it"""
+        from . import Order
+        return Order._create(self, "vb_sparse_table_order_create", True)
 
     @staticmethod
     def _result(rc, ids, dist):
