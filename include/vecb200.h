@@ -33,7 +33,9 @@
  *     vb_vector_to_halfvec_batch_dev reads the 8-byte index of the first value that does
  *     not fit, plus that 4-byte value only when there is one (for the error text), and
  *     vb_sparse_order_bounds_dev reads the result of its device CSR check like the other
- *     sparsevec _dev calls.
+ *     sparsevec _dev calls, and vb_arith_batch_dev and vb_array_to_rows_batch_dev read the
+ *     8-byte key of the first value that fails the reference's checks, plus, for a halfvec
+ *     range error only, that source element (at most 8 bytes, for the error text).
  *   - rows are row-major and contiguous in the caller's buffers (vector: dim
  *     fp32; halfvec: dim IEEE binary16; bit: (dim+7)/8 bytes, MSB first, tail
  *     bits zero -- exactly the payload of Vector.x (src/vector.h:18-24),
@@ -187,6 +189,68 @@ int			vb_vector_to_halfvec_batch_dev(int dim, const void *rows_dev, int64_t n, v
 int			vb_halfvec_to_vector_batch_dev(int dim, const void *rows_dev, int64_t n, void *out_dev);
 int			vb_subvector_batch_dev(int elem, int dim, const void *rows_dev, int64_t n, int32_t start, int32_t count,
 								   void *out_dev, int *out_dim);
+
+/*
+ * The operators + - * || of vector and halfvec over batches of rows (sql/vector.sql:274-298, :734-760), e.g. centring a
+ * column (v - mean), per-dimension weights (v * w) or joining two models' embeddings (a || b):
+ *   vb_arith_batch   vector_add / vector_sub / vector_mul (src/vector.c:824-921) and halfvec_add / halfvec_sub /
+ *                    halfvec_mul (src/halfvec.c:766-879), chosen by op.  vector: a op b in fp32; halfvec:
+ *                    Float4ToHalfUnchecked(HalfToFloat4(a) op HalfToFloat4(b)), the fp32 result rounded to nearest even.
+ *                    Subnormals are kept, and a NaN operand passes through.
+ *   vb_concat_batch  vector_concat (src/vector.c:928-947), halfvec_concat (src/halfvec.c:886-903): rows of dim_a + dim_b
+ * elem = VB_VECTOR or VB_HALFVEC.  Rows are packed.  na and nb are equal, or one of them is 1: an operand of one row is
+ * used with every row of the other (SQL's v - $1, $1 || v).  The result has nb rows (na when nb == 1); other counts are
+ * refused.
+ * Before any work: vb_arith_batch requires dim_a == dim_b ("different vector dimensions %d and %d", CheckDims,
+ * src/vector.c:71-77); vb_concat_batch requires dim_a + dim_b <= 16000 ("vector cannot have more than 16000 dimensions",
+ * CheckDim, src/vector.c:95-106), then writes *out_dim (left untouched on any error); with 0 result rows, rows and out may
+ * be NULL, so such a call sizes the output.  halfvec texts say "halfvec".
+ * Data errors are those the reference's row-by-row execution raises first (lowest row, then the first element its
+ * checking loop reaches): "value out of range: overflow" where a result is infinite (isinf / HalfIsInf), and for *,
+ * "value out of range: underflow" where it is zero (halfvec: HalfIsZero, so -0 too) while neither operand is.  || has
+ * none.  On a data error out is unspecified.
+ */
+#define VB_ADD 0				/* vector_add / halfvec_add (+) */
+#define VB_SUB 1				/* vector_sub / halfvec_sub (-) */
+#define VB_MUL 2				/* vector_mul / halfvec_mul (*) */
+int			vb_arith_batch(int elem, int op, int dim_a, const void *a, int64_t na, int dim_b, const void *b, int64_t nb,
+						   void *out);
+int			vb_concat_batch(int elem, int dim_a, const void *a, int64_t na, int dim_b, const void *b, int64_t nb, void *out,
+							int *out_dim);
+/*
+ * The array casts array_to_vector (src/vector.c:443-512) and array_to_halfvec (src/halfvec.c:442-509): n rows of dim
+ * elements of integer[], real[] or double precision[] (src) to vector / halfvec rows (elem), as (float) of the int32 or
+ * double (round to nearest even) and, for halfvec, Float4ToHalf of that float.  typmod is the target's dimension, or -1.
+ * Before any work, in the reference's order: CheckDim(dim) ("vector must have at least 1 dimension", "vector cannot
+ * have more than 16000 dimensions"), then CheckExpectedDim ("expected %d dimensions, not %d").  Data errors, from the
+ * lowest failing row:
+ *   vector:  the whole row is converted, then the first NaN or infinite element gives "NaN not allowed in vector" or
+ *            "infinite value not allowed in vector" (so {4e38} from double precision[] is an infinite value);
+ *   halfvec: first the conversion pass: the first element whose float is finite but whose half is infinite gives
+ *            "\"<float>\" is out of range for type halfvec"; only when there is none, the check pass: "NaN not allowed
+ *            in halfvec" / "infinite value not allowed in halfvec".  So in one row a range error beats an earlier NaN.
+ * On a data error out is unspecified.  The array structure checks ("array must be 1-D", "array must not contain
+ * nulls", "unsupported array type") and numeric[] stay with the caller, which unpacks the ArrayType.
+ */
+#define VB_ARRAY_INT4 0			/* integer[]          : (float) int32  */
+#define VB_ARRAY_FLOAT4 1		/* real[]             : as is          */
+#define VB_ARRAY_FLOAT8 2		/* double precision[] : (float) double */
+int			vb_array_to_rows_batch(int elem, int src, int dim, int32_t typmod, const void *in, int64_t n, void *out);
+/*
+ * The same on device rows.  Each result equals its host variant's bit for bit.  Refused before any launch (VB_EINVAL):
+ * a bad elem, op or src, a dimension <= 0, a negative count, a NULL pointer for work that exists, rows or output not
+ * aligned to their elements, and input and output that overlap, except that vb_arith_batch_dev may write in place
+ * (out_dev == a_dev or b_dev) over an operand that is not broadcast.  Calls with 0 result rows launch nothing.
+ * vb_concat_batch_dev is fully asynchronous on vb_stream() and uses no workspace (it can be captured into a CUDA graph).
+ * vb_arith_batch_dev and vb_array_to_rows_batch_dev read back the 8-byte key of the first offender and synchronise;
+ * a halfvec range error also reads the offending source element (at most 8 bytes) for its text.
+ */
+int			vb_arith_batch_dev(int elem, int op, int dim_a, const void *a_dev, int64_t na, int dim_b, const void *b_dev,
+							   int64_t nb, void *out_dev);
+int			vb_concat_batch_dev(int elem, int dim_a, const void *a_dev, int64_t na, int dim_b, const void *b_dev, int64_t nb,
+								void *out_dev, int *out_dim);
+int			vb_array_to_rows_batch_dev(int elem, int src, int dim, int32_t typmod, const void *in_dev, int64_t n,
+									   void *out_dev);
 
 /* ------------------------------------------------------ resident row tables */
 

@@ -1470,3 +1470,139 @@ def subvector(rows, start, count, elem=VECTOR):
         out = np.empty((n, d.value), dtype=_NP[elem])
         call(_ptr(r2), n, _ptr(out))
     return out[0] if single else out
+
+
+# --------------------------------------------------------------------- + - * || and the array casts
+#
+# Both operands are numpy arrays (host variants) or both torch CUDA tensors (_dev variants); a 1-d operand is one row,
+# used with every row of the other.  The result is one row when both operands are 1-d.
+
+ADD, SUB, MUL = 0, 1, 2
+ARRAY_INT4, ARRAY_FLOAT4, ARRAY_FLOAT8 = 0, 1, 2
+
+
+def _check_reference(rc):
+    """the reference's errors as Python ones: "value out of range: ..." raises OverflowError, its other texts
+    (dimensions, NaN / infinite elements, halfvec range) ValueError; argument refusals name the entry point."""
+    if rc == _lib.EINVAL:
+        msg = load().vb_last_error().decode()
+        if msg.startswith("value out of range: "):
+            raise OverflowError(msg)
+        if not msg.startswith("vb_"):
+            raise ValueError(msg)
+    _lib.check(rc)
+
+
+def _operands(a, b, elem):
+    """(a rows, b rows, whether the result is one row, whether on the device)"""
+    dev = _is_cuda(a)
+    if dev != _is_cuda(b):
+        raise TypeError("both operands must be numpy arrays or both torch CUDA tensors")
+    out = []
+    for x in (a, b):
+        if dev:
+            out.append(_dev_rows(x, elem))
+        else:
+            x = _host(elem, x)
+            out.append((np.ascontiguousarray(x.reshape(1, -1) if x.ndim == 1 else x), x.ndim == 1))
+    (a2, sa), (b2, sb) = out
+    return a2, b2, sa and sb, dev
+
+
+def _result_rows(a2, b2):
+    na, nb = a2.shape[0], b2.shape[0]
+    return na if nb == 1 else nb
+
+
+def _arith(op, a, b, elem):
+    lib = load()
+    a2, b2, single, dev = _operands(a, b, elem)
+    m, dim = _result_rows(a2, b2), a2.shape[1]
+    args = (elem, op, a2.shape[1], _ptr(a2), a2.shape[0], b2.shape[1], _ptr(b2), b2.shape[0])
+    if dev:
+        import torch
+        out = torch.empty((m, dim), dtype=a2.dtype if elem == VECTOR else torch.float16, device=a2.device)
+        _after_torch(a2, b2)
+        _check_reference(lib.vb_arith_batch_dev(*args, _ptr(out)))
+        synchronize()
+    else:
+        out = np.empty((m, dim), dtype=_NP[elem])
+        _check_reference(lib.vb_arith_batch(*args, _ptr(out)))
+    return out[0] if single else out
+
+
+def vector_add(a, b, elem=VECTOR):
+    """a + b (vector_add, src/vector.c:826-852; halfvec_add, src/halfvec.c:766-798); overflow raises OverflowError."""
+    return _arith(ADD, a, b, elem)
+
+
+def vector_sub(a, b, elem=VECTOR):
+    """a - b (vector_sub, src/vector.c:859-885; halfvec_sub, src/halfvec.c:805-837); overflow raises OverflowError."""
+    return _arith(SUB, a, b, elem)
+
+
+def vector_mul(a, b, elem=VECTOR):
+    """a * b (vector_mul, src/vector.c:892-921; halfvec_mul, src/halfvec.c:844-879); overflow and underflow raise
+    OverflowError."""
+    return _arith(MUL, a, b, elem)
+
+
+def vector_concat(a, b, elem=VECTOR):
+    """a || b (vector_concat, src/vector.c:928-947; halfvec_concat, src/halfvec.c:886-903)."""
+    lib = load()
+    a2, b2, single, dev = _operands(a, b, elem)
+    m, da, db = _result_rows(a2, b2), a2.shape[1], b2.shape[1]
+    fn = lib.vb_concat_batch_dev if dev else lib.vb_concat_batch
+    d = C.c_int(0)
+    _check_reference(fn(elem, da, None, 0, db, None, 0, None, C.byref(d)))   # 0 rows size the output
+    if dev:
+        import torch
+        out = torch.empty((m, d.value), dtype=a2.dtype if elem == VECTOR else torch.float16, device=a2.device)
+        _after_torch(a2, b2)
+    else:
+        out = np.empty((m, d.value), dtype=_NP[elem])
+    _check_reference(fn(elem, da, _ptr(a2), a2.shape[0], db, _ptr(b2), b2.shape[0], _ptr(out), C.byref(d)))
+    if dev:
+        synchronize()
+    return out[0] if single else out
+
+
+def _array_cast(elem, rows, typmod):
+    lib = load()
+    dev = _is_cuda(rows)
+    if dev:
+        import torch
+        src = {torch.int32: ARRAY_INT4, torch.float32: ARRAY_FLOAT4, torch.float64: ARRAY_FLOAT8}.get(rows.dtype)
+    else:
+        rows = np.asarray(rows)
+        src = {np.dtype(np.int32): ARRAY_INT4, np.dtype(np.float32): ARRAY_FLOAT4, np.dtype(np.float64): ARRAY_FLOAT8}.get(rows.dtype)
+    if src is None:
+        raise ValueError("unsupported array type")
+    single = rows.ndim == 1
+    r2 = rows.reshape(1, -1) if single else rows
+    if r2.ndim != 2:
+        raise ValueError("array must be 1-D")
+    n, dim = r2.shape
+    if dev:
+        r2 = r2.contiguous()
+        out = torch.empty((n, dim), dtype=torch.float32 if elem == VECTOR else torch.float16, device=r2.device)
+        _after_torch(r2)
+        _check_reference(lib.vb_array_to_rows_batch_dev(elem, src, dim, int(typmod), _ptr(r2), n, _ptr(out)))
+        synchronize()
+    else:
+        r2 = np.ascontiguousarray(r2)
+        out = np.empty((n, dim), dtype=_NP[elem])
+        _check_reference(lib.vb_array_to_rows_batch(elem, src, dim, int(typmod), _ptr(r2), n, _ptr(out)))
+    return out[0] if single else out
+
+
+def array_to_vector(rows, typmod=-1):
+    """integer[] / real[] / double precision[] :: vector(typmod) of every row (src/vector.c:443-512): the dtype (int32,
+    float32, float64) is the array type.  The reference's errors raise ValueError."""
+    return _array_cast(VECTOR, rows, typmod)
+
+
+def array_to_halfvec(rows, typmod=-1):
+    """the same to halfvec (src/halfvec.c:442-509): binary16 bit patterns (uint16) from numpy rows, float16 on the
+    device.  The reference's errors, including "<float>" is out of range for type halfvec, raise ValueError."""
+    return _array_cast(HALFVEC, rows, typmod)

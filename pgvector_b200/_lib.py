@@ -42,6 +42,12 @@ SIGNATURES = {
     "vb_vector_to_halfvec_batch_dev": (_i, [_i, _vp, _i64, _vp]),
     "vb_halfvec_to_vector_batch_dev": (_i, [_i, _vp, _i64, _vp]),
     "vb_subvector_batch_dev": (_i, [_i, _i, _vp, _i64, C.c_int32, C.c_int32, _vp, C.POINTER(_i)]),
+    "vb_arith_batch": (_i, [_i, _i, _i, _vp, _i64, _i, _vp, _i64, _vp]),
+    "vb_arith_batch_dev": (_i, [_i, _i, _i, _vp, _i64, _i, _vp, _i64, _vp]),
+    "vb_concat_batch": (_i, [_i, _i, _vp, _i64, _i, _vp, _i64, _vp, C.POINTER(_i)]),
+    "vb_concat_batch_dev": (_i, [_i, _i, _vp, _i64, _i, _vp, _i64, _vp, C.POINTER(_i)]),
+    "vb_array_to_rows_batch": (_i, [_i, _i, _i, C.c_int32, _vp, _i64, _vp]),
+    "vb_array_to_rows_batch_dev": (_i, [_i, _i, _i, C.c_int32, _vp, _i64, _vp]),
     "vb_sparsevec_distance_batch": (_i, [_i, _i, _i, C.c_int32, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "vb_sparsevec_norm_batch": (_i, [_i64, _vp, _vp, _vp]),
     "vb_sparsevec_l2_normalize_batch": (_i, [_i64, _vp, _vp, _vp, _vp, _vp, _vp]),

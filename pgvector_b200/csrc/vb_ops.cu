@@ -4,6 +4,10 @@
 //   vb_binary_quantize_batch  binary_quantize                  (src/vector.c:952-978, src/halfvec.c twin)
 //   vb_subvector_batch     subvector                           (src/vector.c:983-1025, src/halfvec.c:939-981)
 //   vb_vector_to_halfvec_batch / vb_halfvec_to_vector_batch     the casts between the two
+//   vb_arith_batch         + - * (src/vector.c:824-921, src/halfvec.c:766-879)
+//   vb_concat_batch        ||    (src/vector.c:928-947, src/halfvec.c:886-903), two column copies
+//   vb_array_to_rows_batch integer[] / real[] / double precision[] -> vector / halfvec (src/vector.c:443-512,
+//                          src/halfvec.c:442-509)
 // The cosine opclasses normalise every indexed row and the query (src/ivfbuild.c:174-180,
 // src/ivfscan.c:222-229, src/hnswutils.c:417-423); norms accumulate in fp64 like the reference.
 // One warp per row; HBM bound (row read once, written once).
@@ -16,6 +20,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 namespace vb {
 
@@ -96,22 +101,176 @@ __global__ void to_float_kernel(const __half* __restrict__ in, int64_t total, fl
     if (i < total) out[i] = __half2float(in[i]);
 }
 
-// subvector: `words` words of T from word `first` of every input row (`pitch` words apart) into packed output rows.
+// subvector and ||: `words` words of T from word `first` of every input row (`pitch` words apart; 0 repeats one row)
+// to word `out_first` of every output row (`out_pitch` words apart).
 // 2^lg lanes per row (lg <= 5), so short rows share a warp; consecutive lanes move consecutive words of a row, so a
-// warp's loads and stores are contiguous runs.  T is the widest word (2 to 16 bytes) that the row pitch, the offset,
-// the output row and both base addresses allow.
+// warp's loads and stores are contiguous runs.  T is the widest word (2 to 16 bytes) that the row pitches, the offsets,
+// the run and both base addresses allow.
 template <typename T>
 __global__ void subvector_kernel(const T* __restrict__ in, int64_t pitch, int64_t first, int64_t n, int words, int lg,
-                                 T* __restrict__ out) {
+                                 T* __restrict__ out, int64_t out_pitch, int64_t out_first) {
     const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     const int64_t r = t >> lg;
     if (r >= n) return;
     const T* src = in + r * pitch + first;
-    T* dst = out + r * (int64_t)words;
+    T* dst = out + r * out_pitch + out_first;
     for (int j = (int)(t & ((1 << lg) - 1)); j < words; j += 1 << lg) dst[j] = src[j];
 }
 
-enum { WSO_IN = 17, WSO_OUT = 18, WSO_FLAG = 19 };
+// ---------------------------------------------------------------- + - * and the array casts
+// The first data error of a batch is the one the reference's row-by-row execution raises: the lowest row, then within
+// the row the first check its loops reach.  Every offender lowers one 64-bit key with atomicMin:
+//   key = ((row * 2 + pass) * dim + element) * 4 + kind
+// pass 0 / 1 are the two checking loops of array_to_halfvec (conversion, then CheckElement); the other functions have
+// one.  A batch with no offender leaves the key at ~0.
+enum { ERR_OVERFLOW = 0, ERR_UNDERFLOW = 1 };             // + - *: float_overflow_error / float_underflow_error
+enum { ERR_RANGE = 0, ERR_NAN = 1, ERR_INF = 2 };         // casts: Float4ToHalf, CheckElement
+constexpr unsigned long long NO_ERROR = ~0ull;
+
+__device__ __forceinline__ unsigned long long error_key(int64_t row, int pass, int64_t dim, int64_t elem, int kind) {
+    return (unsigned long long)(((row * 2 + pass) * dim + elem) * 4 + kind);
+}
+
+// element bits of a word: fp32 as uint32_t, binary16 as uint16_t
+template <typename W, int ES>
+union Elems {
+    W w;
+    typename std::conditional<ES == 4, uint32_t, uint16_t>::type e[sizeof(W) / ES];
+};
+
+// a op b of one element as the reference computes it; *kind = the error its checking loop raises there, or -1.
+// vector: fp32 (src/vector.c:824-921); halfvec: Float4ToHalfUnchecked(HalfToFloat4(a) op HalfToFloat4(b))
+// (src/halfvec.c:766-879).  _rn intrinsics: one correctly rounded operation, never contracted.
+template <int ELEM, int OP>
+__device__ __forceinline__ uint32_t arith_elem(uint32_t a, uint32_t b, int* kind) {
+    const float x = ELEM == VB_VECTOR ? __uint_as_float(a) : __half2float(__ushort_as_half((unsigned short)a));
+    const float y = ELEM == VB_VECTOR ? __uint_as_float(b) : __half2float(__ushort_as_half((unsigned short)b));
+    const float r = OP == VB_ADD ? __fadd_rn(x, y) : OP == VB_SUB ? __fsub_rn(x, y) : __fmul_rn(x, y);
+    *kind = -1;
+    // A NaN result takes the bits the reference gets on x86 (SSE, and F16C for the half conversions), where the GPU would
+    // give its one canonical NaN: the first NaN operand, quieted, or the default NaN 0xFFC00000 for an invalid operation
+    // such as inf - inf.  The half <-> float conversions keep the payload, so for halfvec that is the half operand | 0x200.
+    if (ELEM == VB_VECTOR) {
+        if (isnan(r)) return isnan(x) ? a | 0x400000u : isnan(y) ? b | 0x400000u : 0xFFC00000u;
+        if (isinf(r)) *kind = ERR_OVERFLOW;
+        else if (OP == VB_MUL && r == 0.f && !(x == 0.f || y == 0.f)) *kind = ERR_UNDERFLOW;
+        return __float_as_uint(r);
+    }
+    if (isnan(r)) return isnan(x) ? a | 0x200u : isnan(y) ? b | 0x200u : 0xFE00u;
+    const uint32_t h = __half_as_ushort(__float2half_rn(r));
+    // HalfIsInf / HalfIsZero (src/halfutils.h:37-57) on the bits, so -0 is zero
+    if ((h & 0x7FFF) == 0x7C00) *kind = ERR_OVERFLOW;
+    else if (OP == VB_MUL && (h & 0x7FFF) == 0 && !((a & 0x7FFF) == 0 || (b & 0x7FFF) == 0)) *kind = ERR_UNDERFLOW;
+    return h;
+}
+
+// out row r = a row r op b row r, in words of W; a broadcast operand has a row pitch of 0.  Lanes per row as in
+// subvector_kernel.  out may be a or b (in place): every word is read by the thread that writes it, before it writes it,
+// so no pointer is __restrict__.
+template <typename W, int ELEM, int OP>
+__global__ void arith_kernel(const W* a, int64_t pitch_a, const W* b, int64_t pitch_b, int64_t n, int dim, int words, int lg,
+                             W* out, unsigned long long* __restrict__ first_bad) {
+    constexpr int ES = ELEM == VB_VECTOR ? 4 : 2;
+    constexpr int V = sizeof(W) / ES;
+    const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int64_t r = t >> lg;
+    if (r >= n) return;
+    const W* ra = a + r * pitch_a;
+    const W* rb = b + r * pitch_b;
+    W* ro = out + r * (int64_t)words;
+    int bad = -1, bad_kind = 0;   // the first offending element this thread sees (its words ascend)
+    for (int j = (int)(t & ((1 << lg) - 1)); j < words; j += 1 << lg) {
+        Elems<W, ES> x, y, z;
+        x.w = ra[j];
+        y.w = rb[j];
+#pragma unroll
+        for (int v = 0; v < V; ++v) {
+            int kind;
+            z.e[v] = arith_elem<ELEM, OP>(x.e[v], y.e[v], &kind);
+            if (kind >= 0 && bad < 0) {
+                bad = j * V + v;
+                bad_kind = kind;
+            }
+        }
+        ro[j] = z.w;
+    }
+    if (bad >= 0) atomicMin(first_bad, error_key(r, 0, dim, bad, bad_kind));
+}
+
+// four consecutive source elements, 16-byte aligned
+__device__ __forceinline__ void load4(const int32_t* p, int32_t s[4]) {
+    const int4 u = *reinterpret_cast<const int4*>(p);
+    s[0] = u.x, s[1] = u.y, s[2] = u.z, s[3] = u.w;
+}
+__device__ __forceinline__ void load4(const float* p, float s[4]) {
+    const float4 u = *reinterpret_cast<const float4*>(p);
+    s[0] = u.x, s[1] = u.y, s[2] = u.z, s[3] = u.w;
+}
+__device__ __forceinline__ void load4(const double* p, double s[4]) {
+    const double2 u = reinterpret_cast<const double2*>(p)[0], w = reinterpret_cast<const double2*>(p)[1];
+    s[0] = u.x, s[1] = u.y, s[2] = w.x, s[3] = w.y;
+}
+__device__ __forceinline__ float to_float4(int32_t x) { return __int2float_rn(x); }
+__device__ __forceinline__ float to_float4(float x) { return x; }
+__device__ __forceinline__ float to_float4(double x) { return __double2float_rn(x); }
+
+// array_to_vector / array_to_halfvec of packed source rows (src/vector.c:443-512, src/halfvec.c:442-509): (float) of the
+// int32 or double (round to nearest even), as is for float4; halfvec then Float4ToHalf.  V consecutive elements of the
+// flattened rows per thread (V = 4 where both base addresses allow whole words, else 1); the last thread takes the
+// tail.  A thread's elements may belong to two rows, so each offender makes its own key.
+template <typename S, int ELEM, int V>
+__global__ void array_cast_kernel(const S* __restrict__ in, int64_t total, int dim, void* __restrict__ out,
+                                  unsigned long long* __restrict__ first_bad) {
+    const int64_t i0 = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) * V;
+    if (i0 >= total) return;
+    const bool whole = total - i0 >= V;
+    S s[V];
+    if (V == 4 && whole) {
+        load4(in + i0, s);
+    } else {
+#pragma unroll
+        for (int v = 0; v < V; ++v) s[v] = i0 + v < total ? in[i0 + v] : S(0);
+    }
+    unsigned long long key = NO_ERROR;
+    uint32_t o[V];   // result bits
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+        const float f = to_float4(s[v]);
+        const int64_t i = i0 + v;
+        int pass = 0, kind = -1;
+        if (ELEM == VB_VECTOR) {
+            o[v] = __float_as_uint(f);
+            // CheckElement (src/vector.c:112-123), after the whole row is converted
+            if (isnan(f)) kind = ERR_NAN;
+            else if (isinf(f)) kind = ERR_INF;
+        } else {
+            bool over;
+            o[v] = __half_as_ushort(float_to_half_checked(f, &over));
+            // pass 0: Float4ToHalf; pass 1: CheckElement (src/halfvec.c:113-126), HalfIsNan, then HalfIsInf
+            if (over) kind = ERR_RANGE;
+            else if ((o[v] & 0x7C00) == 0x7C00) pass = 1, kind = (o[v] & 0x7FFF) != 0x7C00 ? ERR_NAN : ERR_INF;
+        }
+        if (kind >= 0 && i < total) key = min(key, error_key(i / dim, pass, dim, i % dim, kind));
+    }
+    if (ELEM == VB_VECTOR) {
+        float* dst = (float*)out + i0;
+        if (V == 4 && whole) *reinterpret_cast<uint4*>(dst) = make_uint4(o[0], o[1], o[2], o[3]);
+        else
+#pragma unroll
+            for (int v = 0; v < V; ++v)
+                if (i0 + v < total) dst[v] = __uint_as_float(o[v]);
+    } else {
+        __half* dst = (__half*)out + i0;
+        if (V == 4 && whole) *reinterpret_cast<uint2*>(dst) = make_uint2(o[0] | o[1] << 16, o[2] | o[3] << 16);
+        else
+#pragma unroll
+            for (int v = 0; v < V; ++v)
+                if (i0 + v < total) dst[v] = __ushort_as_half((unsigned short)o[v]);
+    }
+    if (key != NO_ERROR) atomicMin(first_bad, key);
+}
+
+enum { WSO_IN = 17, WSO_OUT = 18, WSO_FLAG = 19, WSO_IN2 = 20 };
 
 // the shortest decimal that reads back as the same float, in PostgreSQL's float4 output style
 // (float_to_shortest_decimal_buf: fixed notation for exponents -4 .. 14, scientific otherwise)
@@ -215,26 +374,122 @@ static int to_float_rows(int dim, const void* in, int64_t n, void* out) {
     return VB_OK;
 }
 
-template <typename T>
-static void launch_subvector(const void* in, int64_t pitch_b, int64_t first_b, int64_t n, int64_t row_b, void* out, cudaStream_t s) {
-    const int words = (int)(row_b / (int64_t)sizeof(T));
+// 2^lg lanes per row of `words` words: up to a warp
+static int lanes_lg(int words) {
     int lg = 0;
     while (lg < 5 && (1 << lg) < words) ++lg;
+    return lg;
+}
+
+template <typename T>
+static void launch_subvector(const void* in, int64_t pitch_b, int64_t first_b, int64_t n, int64_t row_b, void* out, int64_t out_pitch_b,
+                             int64_t out_first_b, cudaStream_t s) {
+    const int64_t w = (int64_t)sizeof(T);
+    const int words = (int)(row_b / w);
+    const int lg = lanes_lg(words);
     const unsigned grid = (unsigned)(((n << lg) + 255) / 256);
-    subvector_kernel<T><<<grid, 256, 0, s>>>((const T*)in, pitch_b / (int64_t)sizeof(T), first_b / (int64_t)sizeof(T), n, words, lg, (T*)out);
+    subvector_kernel<T><<<grid, 256, 0, s>>>((const T*)in, pitch_b / w, first_b / w, n, words, lg, (T*)out, out_pitch_b / w, out_first_b / w);
+}
+
+// row_b bytes from byte first_b of every input row (pitch_b apart, 0: one row repeated) to byte out_first_b of every
+// output row (out_pitch_b apart), n rows, in the widest word that every pitch, offset, the run and both base addresses
+// are aligned to
+static int copy_columns(const void* in, int64_t pitch_b, int64_t first_b, int64_t n, int64_t row_b, void* out, int64_t out_pitch_b,
+                        int64_t out_first_b) {
+    cudaStream_t s = ctx().stream;
+    const uint64_t a = (uint64_t)pitch_b | (uint64_t)first_b | (uint64_t)row_b | (uint64_t)out_pitch_b | (uint64_t)out_first_b |
+                       (uint64_t)(uintptr_t)in | (uint64_t)(uintptr_t)out;
+    if (a % 16 == 0) launch_subvector<uint4>(in, pitch_b, first_b, n, row_b, out, out_pitch_b, out_first_b, s);
+    else if (a % 8 == 0) launch_subvector<uint2>(in, pitch_b, first_b, n, row_b, out, out_pitch_b, out_first_b, s);
+    else if (a % 4 == 0) launch_subvector<uint32_t>(in, pitch_b, first_b, n, row_b, out, out_pitch_b, out_first_b, s);
+    else launch_subvector<uint16_t>(in, pitch_b, first_b, n, row_b, out, out_pitch_b, out_first_b, s);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
 }
 
 // elements [first, first + out_dim) of every row
 static int subvector_rows(int elem, int dim, const void* in, int64_t n, int first, int out_dim, void* out) {
-    cudaStream_t s = ctx().stream;
     const int64_t es = elem == VB_VECTOR ? 4 : 2;
-    const int64_t pitch_b = es * dim, first_b = es * first, row_b = es * out_dim;
-    // the widest word every row start, the offset, every output row and both base addresses are aligned to
-    const uint64_t a = (uint64_t)pitch_b | (uint64_t)first_b | (uint64_t)row_b | (uint64_t)(uintptr_t)in | (uint64_t)(uintptr_t)out;
-    if (a % 16 == 0) launch_subvector<uint4>(in, pitch_b, first_b, n, row_b, out, s);
-    else if (a % 8 == 0) launch_subvector<uint2>(in, pitch_b, first_b, n, row_b, out, s);
-    else if (a % 4 == 0) launch_subvector<uint32_t>(in, pitch_b, first_b, n, row_b, out, s);
-    else launch_subvector<uint16_t>(in, pitch_b, first_b, n, row_b, out, s);
+    return copy_columns(in, es * dim, es * first, n, es * out_dim, out, es * out_dim, 0);
+}
+
+// a || b: the m result rows (m = max(na, nb) where one count is 1); an operand of one row is repeated (pitch 0)
+static int concat_rows(int elem, int dim_a, const void* a, int64_t na, int dim_b, const void* b, int64_t nb, int64_t m, void* out) {
+    const int64_t es = elem == VB_VECTOR ? 4 : 2, pitch_o = es * (dim_a + dim_b);
+    VB_TRY(copy_columns(a, na == 1 ? 0 : es * dim_a, 0, m, es * dim_a, out, pitch_o, 0));
+    return copy_columns(b, nb == 1 ? 0 : es * dim_b, 0, m, es * dim_b, out, pitch_o, es * dim_a);
+}
+
+template <typename W, int ELEM, int OP>
+static void launch_arith(const void* a, int64_t pitch_a_b, const void* b, int64_t pitch_b_b, int64_t m, int dim, void* out,
+                         unsigned long long* first_bad, cudaStream_t s) {
+    const int64_t w = (int64_t)sizeof(W);
+    const int words = (int)(raw_row_bytes(ELEM, dim) / w);
+    const int lg = lanes_lg(words);
+    const unsigned grid = (unsigned)(((m << lg) + 255) / 256);
+    arith_kernel<W, ELEM, OP><<<grid, 256, 0, s>>>((const W*)a, pitch_a_b / w, (const W*)b, pitch_b_b / w, m, dim, words, lg, (W*)out,
+                                                   first_bad);
+}
+
+template <int ELEM, int OP>
+static void launch_arith_words(const void* a, int64_t pitch_a_b, const void* b, int64_t pitch_b_b, int64_t m, int dim, void* out,
+                               unsigned long long* first_bad, cudaStream_t s) {
+    // the widest word every row start and the three base addresses are aligned to
+    const uint64_t al = (uint64_t)raw_row_bytes(ELEM, dim) | (uint64_t)(uintptr_t)a | (uint64_t)(uintptr_t)b | (uint64_t)(uintptr_t)out;
+    if (al % 16 == 0) launch_arith<uint4, ELEM, OP>(a, pitch_a_b, b, pitch_b_b, m, dim, out, first_bad, s);
+    else if (al % 8 == 0) launch_arith<uint2, ELEM, OP>(a, pitch_a_b, b, pitch_b_b, m, dim, out, first_bad, s);
+    else if constexpr (ELEM == VB_VECTOR) launch_arith<uint32_t, ELEM, OP>(a, pitch_a_b, b, pitch_b_b, m, dim, out, first_bad, s);
+    else if (al % 4 == 0) launch_arith<uint32_t, ELEM, OP>(a, pitch_a_b, b, pitch_b_b, m, dim, out, first_bad, s);
+    else launch_arith<uint16_t, ELEM, OP>(a, pitch_a_b, b, pitch_b_b, m, dim, out, first_bad, s);
+}
+
+// out = a op b over m result rows; *first_bad (device) is set to ~0 here and lowered to the key of every offender
+static int arith_rows(int elem, int op, int dim, const void* a, int64_t na, const void* b, int64_t nb, int64_t m, void* out,
+                      unsigned long long* first_bad) {
+    cudaStream_t s = ctx().stream;
+    VB_CUDA(cudaMemsetAsync(first_bad, 0xFF, sizeof(unsigned long long), s));
+    const int64_t row_b = (int64_t)raw_row_bytes(elem, dim);
+    const int64_t pa = na == 1 ? 0 : row_b, pb = nb == 1 ? 0 : row_b;
+#define VB_ARITH_CASE(E, O) \
+    if (elem == E && op == O) launch_arith_words<E, O>(a, pa, b, pb, m, dim, out, first_bad, s);
+    VB_ARITH_CASE(VB_VECTOR, VB_ADD)
+    VB_ARITH_CASE(VB_VECTOR, VB_SUB)
+    VB_ARITH_CASE(VB_VECTOR, VB_MUL)
+    VB_ARITH_CASE(VB_HALFVEC, VB_ADD)
+    VB_ARITH_CASE(VB_HALFVEC, VB_SUB)
+    VB_ARITH_CASE(VB_HALFVEC, VB_MUL)
+#undef VB_ARITH_CASE
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
+}
+
+template <typename S, int ELEM>
+static void launch_array_cast(const void* in, int64_t total, int dim, void* out, unsigned long long* first_bad, cudaStream_t s) {
+    // four elements per thread where the source and the result base addresses allow whole words
+    if ((uintptr_t)in % (4 * sizeof(S)) == 0 && (uintptr_t)out % (ELEM == VB_VECTOR ? 16 : 8) == 0)
+        array_cast_kernel<S, ELEM, 4><<<(unsigned)(((total + 3) / 4 + 255) / 256), 256, 0, s>>>((const S*)in, total, dim, out, first_bad);
+    else
+        array_cast_kernel<S, ELEM, 1><<<(unsigned)((total + 255) / 256), 256, 0, s>>>((const S*)in, total, dim, out, first_bad);
+}
+
+static size_t array_elem_bytes(int src) { return src == VB_ARRAY_FLOAT8 ? 8 : 4; }
+
+// n source rows of dim elements to vector / halfvec rows; *first_bad as in arith_rows
+static int array_cast_rows(int elem, int src, int dim, const void* in, int64_t n, void* out, unsigned long long* first_bad) {
+    cudaStream_t s = ctx().stream;
+    VB_CUDA(cudaMemsetAsync(first_bad, 0xFF, sizeof(unsigned long long), s));
+    const int64_t total = n * dim;
+#define VB_CAST_CASE(SRC, S, E) \
+    if (src == SRC && elem == E) launch_array_cast<S, E>(in, total, dim, out, first_bad, s);
+    VB_CAST_CASE(VB_ARRAY_INT4, int32_t, VB_VECTOR)
+    VB_CAST_CASE(VB_ARRAY_FLOAT4, float, VB_VECTOR)
+    VB_CAST_CASE(VB_ARRAY_FLOAT8, double, VB_VECTOR)
+    VB_CAST_CASE(VB_ARRAY_INT4, int32_t, VB_HALFVEC)
+    VB_CAST_CASE(VB_ARRAY_FLOAT4, float, VB_HALFVEC)
+    VB_CAST_CASE(VB_ARRAY_FLOAT8, double, VB_HALFVEC)
+#undef VB_CAST_CASE
     VB_CUDA(cudaGetLastError());
     count_launch();
     return VB_OK;
@@ -275,6 +530,65 @@ static int check_disjoint(const char* fn, const void* in, size_t in_bytes, const
 }
 
 static size_t dense_bytes(int elem, int dim, int64_t n) { return raw_row_bytes(elem, dim) * (size_t)n; }
+
+static const char* type_name(int elem) { return elem == VB_VECTOR ? "vector" : "halfvec"; }
+
+// the argument checks of + - * and ||: *m = the result rows (nb, or na when nb == 1)
+static int check_pair(const char* fn, int elem, int dim_a, const void* a, int64_t na, int dim_b, const void* b, int64_t nb, const void* out,
+                      int64_t* m) {
+    VB_REQUIRE(elem == VB_VECTOR || elem == VB_HALFVEC, "%s: elem must be VB_VECTOR or VB_HALFVEC, got %d", fn, elem);
+    VB_REQUIRE(dim_a > 0 && dim_b > 0, "%s: dimensions must be positive, got %d and %d", fn, dim_a, dim_b);
+    VB_REQUIRE(na >= 0 && nb >= 0, "%s: bad row counts %lld and %lld", fn, (long long)na, (long long)nb);
+    VB_REQUIRE(na == nb || na == 1 || nb == 1, "%s: row counts %lld and %lld neither match nor broadcast", fn, (long long)na,
+               (long long)nb);
+    *m = nb == 1 ? na : nb;
+    VB_REQUIRE(*m == 0 || (a && b && out), "%s: null rows or output", fn);
+    const uintptr_t es = elem == VB_VECTOR ? 4 : 2;
+    VB_REQUIRE(((uintptr_t)a | (uintptr_t)b | (uintptr_t)out) % es == 0, "%s: rows and output must be %d-byte aligned", fn, (int)es);
+    return VB_OK;
+}
+
+// the result of a batch from its first-offender key (host): VB_OK, or the reference's error for that offender.  For a
+// halfvec range error, range_value(row-major element index) gives the float the text shows.
+template <typename RangeValue>
+static int batch_error(unsigned long long key, bool arith, int elem, int dim, RangeValue range_value) {
+    if (key == NO_ERROR) return VB_OK;
+    const int kind = (int)(key & 3);
+    const unsigned long long rest = key >> 2, rp = rest / (unsigned)dim;
+    if (arith) {
+        // float_overflow_error / float_underflow_error
+        set_error("value out of range: %s", kind == ERR_UNDERFLOW ? "underflow" : "overflow");
+    } else if (kind == ERR_RANGE && elem == VB_HALFVEC) {
+        float v;
+        VB_TRY(range_value((int64_t)((rp >> 1) * (unsigned)dim + rest % (unsigned)dim), &v));
+        return half_range_error(v);
+    } else {
+        set_error(kind == ERR_NAN ? "NaN not allowed in %s" : "infinite value not allowed in %s", type_name(elem));
+    }
+    return VB_EINVAL;
+}
+
+// (float) of source element i of an array cast, as the kernel forms it (host C casts round to nearest even too)
+static float source_float(int src, const void* p, int64_t i) {
+    if (src == VB_ARRAY_INT4) return (float)((const int32_t*)p)[i];
+    if (src == VB_ARRAY_FLOAT8) return (float)((const double*)p)[i];
+    return ((const float*)p)[i];
+}
+
+// the scalar checks of array_to_vector / array_to_halfvec, before any work
+static int check_array_cast(const char* fn, int elem, int src, int dim, int32_t typmod, const void* in, int64_t n, const void* out) {
+    VB_REQUIRE(elem == VB_VECTOR || elem == VB_HALFVEC, "%s: elem must be VB_VECTOR or VB_HALFVEC, got %d", fn, elem);
+    VB_REQUIRE(src == VB_ARRAY_INT4 || src == VB_ARRAY_FLOAT4 || src == VB_ARRAY_FLOAT8, "%s: bad source type %d", fn, src);
+    VB_REQUIRE(n >= 0, "%s: bad row count %lld", fn, (long long)n);
+    // CheckDim, then CheckExpectedDim (src/vector.c:80-106, src/halfvec.c twins)
+    VB_REQUIRE(dim >= 1, "%s must have at least 1 dimension", type_name(elem));
+    VB_REQUIRE(dim <= 16000, "%s cannot have more than %d dimensions", type_name(elem), 16000);
+    VB_REQUIRE(typmod == -1 || typmod == dim, "expected %d dimensions, not %d", typmod, dim);
+    VB_REQUIRE(n == 0 || (in && out), "%s: null rows or output", fn);
+    VB_REQUIRE((uintptr_t)in % array_elem_bytes(src) == 0 && (uintptr_t)out % (elem == VB_VECTOR ? 4 : 2) == 0,
+               "%s: rows and output must be aligned to their elements", fn);
+    return VB_OK;
+}
 
 }  // namespace vb
 
@@ -464,6 +778,151 @@ int vb_subvector_batch_dev(int elem, int dim, const void* rows_dev, int64_t n, i
     *out_dim = d;
     if (n == 0) return VB_OK;
     return subvector_rows(elem, dim, rows_dev, n, first, d, out_dev);
+}
+
+// ---------------------------------------------------------------- + - * ||, array casts
+
+int vb_arith_batch(int elem, int op, int dim_a, const void* a, int64_t na, int dim_b, const void* b, int64_t nb, void* out) {
+    const char* fn = "vb_arith_batch";
+    VB_TRY(require_init());
+    int64_t m;
+    VB_TRY(check_pair(fn, elem, dim_a, a, na, dim_b, b, nb, out, &m));
+    VB_REQUIRE(op == VB_ADD || op == VB_SUB || op == VB_MUL, "%s: bad op %d", fn, op);
+    // CheckDims (src/vector.c:71-77, src/halfvec.c:74-81)
+    VB_REQUIRE(dim_a == dim_b, "different %s dimensions %d and %d", type_name(elem), dim_a, dim_b);
+    if (m == 0) return VB_OK;
+    cudaStream_t s = ctx().stream;
+    void *d_a, *d_b, *d_out, *d_flag;
+    const size_t raw = raw_row_bytes(elem, dim_a);
+    VB_TRY(stage_in(elem, dim_a, a, na, &d_a));
+    VB_TRY(workspace(WSO_IN2, raw * (size_t)nb, &d_b));
+    VB_CUDA(cudaMemcpyAsync(d_b, b, raw * (size_t)nb, cudaMemcpyHostToDevice, s));
+    VB_TRY(workspace(WSO_OUT, raw * (size_t)m, &d_out));
+    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(arith_rows(elem, op, dim_a, d_a, na, d_b, nb, m, d_out, (unsigned long long*)d_flag));
+    unsigned long long key = NO_ERROR;
+    VB_CUDA(cudaMemcpyAsync(out, d_out, raw * (size_t)m, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaMemcpyAsync(&key, d_flag, sizeof(key), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    return batch_error(key, true, elem, dim_a, [](int64_t, float*) { return VB_OK; });
+}
+
+int vb_arith_batch_dev(int elem, int op, int dim_a, const void* a_dev, int64_t na, int dim_b, const void* b_dev, int64_t nb, void* out_dev) {
+    const char* fn = "vb_arith_batch_dev";
+    VB_TRY(require_init());
+    int64_t m;
+    VB_TRY(check_pair(fn, elem, dim_a, a_dev, na, dim_b, b_dev, nb, out_dev, &m));
+    VB_REQUIRE(op == VB_ADD || op == VB_SUB || op == VB_MUL, "%s: bad op %d", fn, op);
+    VB_REQUIRE(dim_a == dim_b, "different %s dimensions %d and %d", type_name(elem), dim_a, dim_b);
+    if (m == 0) return VB_OK;
+    // in place is allowed on an operand that is not broadcast; any other overlap is refused
+    const size_t raw = raw_row_bytes(elem, dim_a);
+    if (!(out_dev == a_dev && na == m)) VB_TRY(check_disjoint(fn, a_dev, raw * (size_t)na, out_dev, raw * (size_t)m));
+    if (!(out_dev == b_dev && nb == m)) VB_TRY(check_disjoint(fn, b_dev, raw * (size_t)nb, out_dev, raw * (size_t)m));
+    cudaStream_t s = ctx().stream;
+    void* d_flag;
+    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(arith_rows(elem, op, dim_a, a_dev, na, b_dev, nb, m, out_dev, (unsigned long long*)d_flag));
+    unsigned long long key = NO_ERROR;
+    VB_CUDA(cudaMemcpyAsync(&key, d_flag, sizeof(key), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    return batch_error(key, true, elem, dim_a, [](int64_t, float*) { return VB_OK; });
+}
+
+// CheckDim of the concatenated dimension (src/vector.c:935, src/halfvec.c:893): both dimensions are positive, so only
+// the upper bound can fail
+static int concat_dim(int elem, int dim_a, int dim_b, int* d) {
+    const int64_t sum = (int64_t)dim_a + dim_b;
+    VB_REQUIRE(sum <= 16000, "%s cannot have more than %d dimensions", type_name(elem), 16000);
+    *d = (int)sum;
+    return VB_OK;
+}
+
+int vb_concat_batch(int elem, int dim_a, const void* a, int64_t na, int dim_b, const void* b, int64_t nb, void* out, int* out_dim) {
+    const char* fn = "vb_concat_batch";
+    VB_TRY(require_init());
+    int64_t m;
+    VB_TRY(check_pair(fn, elem, dim_a, a, na, dim_b, b, nb, out, &m));
+    VB_REQUIRE(out_dim, "%s: null out_dim", fn);
+    int d;
+    VB_TRY(concat_dim(elem, dim_a, dim_b, &d));
+    *out_dim = d;
+    if (m == 0) return VB_OK;
+    cudaStream_t s = ctx().stream;
+    void *d_a, *d_b, *d_out;
+    VB_TRY(stage_in(elem, dim_a, a, na, &d_a));
+    VB_TRY(workspace(WSO_IN2, dense_bytes(elem, dim_b, nb), &d_b));
+    VB_CUDA(cudaMemcpyAsync(d_b, b, dense_bytes(elem, dim_b, nb), cudaMemcpyHostToDevice, s));
+    VB_TRY(workspace(WSO_OUT, dense_bytes(elem, d, m), &d_out));
+    VB_TRY(concat_rows(elem, dim_a, d_a, na, dim_b, d_b, nb, m, d_out));
+    VB_CUDA(cudaMemcpyAsync(out, d_out, dense_bytes(elem, d, m), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    return VB_OK;
+}
+
+int vb_concat_batch_dev(int elem, int dim_a, const void* a_dev, int64_t na, int dim_b, const void* b_dev, int64_t nb, void* out_dev,
+                        int* out_dim) {
+    const char* fn = "vb_concat_batch_dev";
+    VB_TRY(require_init());
+    int64_t m;
+    VB_TRY(check_pair(fn, elem, dim_a, a_dev, na, dim_b, b_dev, nb, out_dev, &m));
+    VB_REQUIRE(out_dim, "%s: null out_dim", fn);
+    int d;
+    VB_TRY(concat_dim(elem, dim_a, dim_b, &d));
+    if (m > 0) {
+        VB_TRY(check_disjoint(fn, a_dev, dense_bytes(elem, dim_a, na), out_dev, dense_bytes(elem, d, m)));
+        VB_TRY(check_disjoint(fn, b_dev, dense_bytes(elem, dim_b, nb), out_dev, dense_bytes(elem, d, m)));
+    }
+    *out_dim = d;
+    if (m == 0) return VB_OK;
+    return concat_rows(elem, dim_a, a_dev, na, dim_b, b_dev, nb, m, out_dev);
+}
+
+int vb_array_to_rows_batch(int elem, int src, int dim, int32_t typmod, const void* in, int64_t n, void* out) {
+    const char* fn = "vb_array_to_rows_batch";
+    VB_TRY(require_init());
+    VB_TRY(check_array_cast(fn, elem, src, dim, typmod, in, n, out));
+    if (n == 0) return VB_OK;
+    cudaStream_t s = ctx().stream;
+    const size_t in_bytes = array_elem_bytes(src) * (size_t)dim * (size_t)n;
+    void *d_in, *d_out, *d_flag;
+    VB_TRY(workspace(WSO_IN, in_bytes, &d_in));
+    VB_CUDA(cudaMemcpyAsync(d_in, in, in_bytes, cudaMemcpyHostToDevice, s));
+    VB_TRY(workspace(WSO_OUT, dense_bytes(elem, dim, n), &d_out));
+    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(array_cast_rows(elem, src, dim, d_in, n, d_out, (unsigned long long*)d_flag));
+    unsigned long long key = NO_ERROR;
+    VB_CUDA(cudaMemcpyAsync(out, d_out, dense_bytes(elem, dim, n), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaMemcpyAsync(&key, d_flag, sizeof(key), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    return batch_error(key, false, elem, dim, [&](int64_t i, float* v) {
+        *v = source_float(src, in, i);
+        return VB_OK;
+    });
+}
+
+int vb_array_to_rows_batch_dev(int elem, int src, int dim, int32_t typmod, const void* in_dev, int64_t n, void* out_dev) {
+    const char* fn = "vb_array_to_rows_batch_dev";
+    VB_TRY(require_init());
+    VB_TRY(check_array_cast(fn, elem, src, dim, typmod, in_dev, n, out_dev));
+    if (n == 0) return VB_OK;
+    VB_TRY(check_disjoint(fn, in_dev, array_elem_bytes(src) * (size_t)dim * (size_t)n, out_dev, dense_bytes(elem, dim, n)));
+    cudaStream_t s = ctx().stream;
+    void* d_flag;
+    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(array_cast_rows(elem, src, dim, in_dev, n, out_dev, (unsigned long long*)d_flag));
+    unsigned long long key = NO_ERROR;
+    VB_CUDA(cudaMemcpyAsync(&key, d_flag, sizeof(key), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    return batch_error(key, false, elem, dim, [&](int64_t i, float* v) {
+        // only the error reads the offending source element, for the reference's text
+        double raw = 0;
+        VB_CUDA(cudaMemcpyAsync(&raw, (const uint8_t*)in_dev + array_elem_bytes(src) * (size_t)i, array_elem_bytes(src),
+                                cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaStreamSynchronize(s));
+        *v = source_float(src, &raw, 0);
+        return VB_OK;
+    });
 }
 
 }  // extern "C"
