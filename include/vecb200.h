@@ -86,6 +86,8 @@ int			vb_init(int device);
 /* Release every device allocation made by the library in this process. */
 int			vb_shutdown(void);
 const char *vb_last_error(void);
+/* The reference's errdetail of the last error, "" when it has none (the type input errors below have one). */
+const char *vb_last_error_detail(void);
 int			vb_abi_version(void);
 /* cudaStream_t the library launches on (as void*), for event timing / graph capture by the host. */
 void	   *vb_stream(void);
@@ -120,6 +122,8 @@ int			vb_stream_wait_event(void *cuda_event);
 #define VB_PROF_BUILD_DEST 11	/* list numbers -> list offsets, image order and per-row destinations */
 #define VB_PROF_BUILD_PLACE 12	/* the placement kernel alone (one bracket per launch) */
 #define VB_PROF_BUILD_ASSIGN 13	/* pass one: the list of every row (per chunk: padding / normalisation, assign) */
+#define VB_PROF_TEXT_PARSE 14	/* the type input parse kernels (text_parse_dense_kernel, text_parse_sparse_kernel) */
+#define VB_PROF_TEXT_FORMAT 15	/* the type output kernels (text_format_kernel, length and write passes) */
 int			vb_prof_enable(int on);
 /* Synchronises, then returns accumulated milliseconds and bracketed launches since the last read of `kernel`. */
 int			vb_prof_read(int kernel, double *total_ms, int64_t *launches);
@@ -514,6 +518,68 @@ int			vb_sparsevec_to_dense_batch(int elem, int dim, int64_t n, const int64_t *r
 										void *out);
 int			vb_sparsevec_to_dense_batch_dev(int elem, int dim, int64_t n, const int64_t *row_off_dev, const int32_t *idx_dev,
 											const float *val_dev, void *out_dev);
+
+/* ------------------------------------------------------------ text input and output */
+
+/*
+ * The type I/O over a column: vector_in / halfvec_in (src/vector.c:174-281, src/halfvec.c:178-286, elem = VB_VECTOR /
+ * VB_HALFVEC), sparsevec_in (src/sparsevec.c:203-409) and vector_out / halfvec_out / sparsevec_out (src/vector.c:289-326,
+ * src/halfvec.c:294-335, src/sparsevec.c:428-476).  Values, bytes and error texts are the reference's.
+ *
+ * Input literals.  Literal i is text[off[i] .. off[i + 1]), ending earlier at its first NUL byte as the cstring the fmgr
+ * passes would; no terminator is needed.  Tokens are what glibc strtof / strtol (base 10) accept in the C locale,
+ * correctly rounded to nearest even (decimal of any length, hex floats, inf / infinity / nan / nan(chars), any case).
+ * Rows: dense values packed at out[out_row_off[i] ..) (float, or IEEE half bits); sparsevec as the CSR the sparse table
+ * calls take (ascending 0-based indices, no zeros: vb_sparse_table_append_dev takes it unchanged) and the dimension of
+ * each literal in out_dim.
+ *
+ * Sizes.  The bound of a literal is its commas before the first NUL + 1 (the dimension of every valid dense literal,
+ * and sparsevec_in's maxNnz); typmod >= 1 makes the dense offsets i * typmod.  out_row_off [n + 1] is always written:
+ * dense, the bound's (or typmod's) offsets; sparsevec, the stored entries' offsets on success and the bound's when
+ * the call fails on cap.  A bound total above cap fails with VB_EINVAL naming the total and writes nothing else.
+ * Output: text without terminators, out_off [n + 1] byte offsets, always written; cap is bytes, and a total above it
+ * fails with VB_EINVAL naming the total (out = NULL sizes: offsets only, no cap check).  The reference's own buffer bound always suffices:
+ * dim * 16 + 2 bytes per dense row, (12 + 16) * nnz + 15 per sparsevec row.
+ *
+ * Errors.  A call fails (VB_EINVAL) with the error the reference's row-by-row execution raises first: the lowest failing
+ * literal, within it the first error its left-to-right scan reaches, the end-of-literal checks (CheckDim,
+ * CheckExpectedDim, and after the sort CheckIndex) last.  vb_last_error() is the reference's errmsg (the literal echoed
+ * in "invalid input syntax for type vector: \"...\"", the strtof token in "\"4e38\" is out of range for type vector"),
+ * vb_last_error_detail() its errdetail.  *out_bad (may be NULL) is the failing literal's index, -1 otherwise.  On an
+ * error the rows are unspecified.
+ *
+ * Host variants stream the text through pinned staging in chunks of literals of at most 64 MiB of text (one longer
+ * literal makes a chunk of its own); chunks run in order and the first chunk with an error stops the call.  The dense
+ * input overlaps the host's staging of the next chunk (and its copy of the previous chunk's rows) with the parse of
+ * the current one through two pinned slots; sparsevec input runs chunks one after another, since each reads back its
+ * stored total and sort flag before the next can start.  The bound is counted on the host first (commas before the
+ * first NUL, with the C library's memchr).  Output host variants take chunks of rows whose text is at most 64 MiB by
+ * the reference's bound; a length pass over all chunks sizes the text before any is written, and the write pass
+ * reuses those offsets.  sparsevec output first checks the rows as the sparse table calls do (offsets from 0, indices
+ * ascending inside [0, dim)), with their texts ("sparsevec index out of bounds (row r)").  _dev variants take device
+ * pointers (text, off, outputs; out_bad and cap stay host values), run on vb_stream() and synchronise.  They read
+ * back: dense input, the bound total (8 bytes) and a 64-byte status; sparsevec input, the bound total, the stored total
+ * and the sort flag (8 bytes each) and the status (more than 2^31 - 1 bound entries in one call are refused);
+ * output, the text total (8 bytes), and for sparsevec the 24-byte row check.  On an error they also read the failing
+ * literal (at most its length in bytes).
+ */
+int			vb_text_to_rows_batch(int elem, int32_t typmod, int64_t n, const char *text, const int64_t *off, int64_t cap,
+								  int64_t *out_row_off, void *out, int64_t *out_bad);
+int			vb_text_to_rows_batch_dev(int elem, int32_t typmod, int64_t n, const char *text_dev, const int64_t *off_dev,
+									  int64_t cap, int64_t *out_row_off_dev, void *out_dev, int64_t *out_bad);
+int			vb_text_to_sparsevec_batch(int32_t typmod, int64_t n, const char *text, const int64_t *off, int64_t cap,
+									   int32_t *out_dim, int64_t *out_row_off, int32_t *out_idx, float *out_val,
+									   int64_t *out_bad);
+int			vb_text_to_sparsevec_batch_dev(int32_t typmod, int64_t n, const char *text_dev, const int64_t *off_dev,
+										   int64_t cap, int32_t *out_dim_dev, int64_t *out_row_off_dev, int32_t *out_idx_dev,
+										   float *out_val_dev, int64_t *out_bad);
+int			vb_rows_to_text_batch(int elem, int dim, const void *rows, int64_t n, int64_t cap, int64_t *out_off, char *out);
+int			vb_rows_to_text_batch_dev(int elem, int dim, const void *rows_dev, int64_t n, int64_t cap, int64_t *out_off_dev,
+									  char *out_dev);
+int			vb_sparsevec_to_text_batch(int dim, int64_t n, const int64_t *row_off, const int32_t *idx, const float *val,
+									   int64_t cap, int64_t *out_off, char *out);
+int			vb_sparsevec_to_text_batch_dev(int dim, int64_t n, const int64_t *row_off_dev, const int32_t *idx_dev,
+										   const float *val_dev, int64_t cap, int64_t *out_off_dev, char *out_dev);
 
 /* ------------------------------------------------------------ ordering by value */
 

@@ -1606,3 +1606,108 @@ def array_to_halfvec(rows, typmod=-1):
     """the same to halfvec (src/halfvec.c:442-509): binary16 bit patterns (uint16) from numpy rows, float16 on the
     device.  The reference's errors, including "<float>" is out of range for type halfvec, raise ValueError."""
     return _array_cast(HALFVEC, rows, typmod)
+
+
+# ------------------------------------------------------------------------- type I/O: text in, text out
+
+def _text_input(texts):
+    """(text, off, n, on the device) of a list of str, or of a (CUDA uint8 tensor, CUDA int64 offsets) pair"""
+    if isinstance(texts, (tuple, list)) and len(texts) == 2 and all(_is_cuda(t) for t in texts):
+        import torch
+        text, off = texts
+        if text.dtype != torch.uint8 or off.dtype != torch.int64 or text.dim() != 1 or off.dim() != 1 or off.numel() < 1:
+            raise ValueError("device text: a 1-d uint8 tensor and 1-d int64 offsets [n + 1]")
+        return text.contiguous(), off.contiguous(), off.numel() - 1, True
+    blobs = [t.encode() if isinstance(t, str) else bytes(t) for t in texts]
+    off = np.zeros(len(blobs) + 1, dtype=np.int64)
+    off[1:] = np.cumsum([len(b) for b in blobs])
+    text = np.frombuffer(b"".join(blobs) or b"\0", dtype=np.uint8)
+    return text, off, len(blobs), False
+
+
+def _raise_text(rc, bad):
+    if rc == _lib.EINVAL:
+        lib = load()
+        msg = lib.vb_last_error().decode()
+        if bad.value >= 0:
+            raise _lib.TextInputError(msg, lib.vb_last_error_detail().decode(), int(bad.value))
+    _lib.check(rc)
+
+
+def _text_to_rows(elem, texts, typmod):
+    lib = load()
+    text, off, n, dev = _text_input(texts)
+    bad = C.c_int64(-1)
+    if dev:
+        import torch
+        row_off = torch.zeros(n + 1, dtype=torch.int64, device=text.device)   # a refused argument writes none
+        fn = lib.vb_text_to_rows_batch_dev
+        _after_torch(text, off)
+    else:
+        row_off = np.zeros(n + 1, dtype=np.int64)
+        fn = lib.vb_text_to_rows_batch
+    rc = fn(elem, typmod, n, _ptr(text), _ptr(off), 0, _ptr(row_off), None, C.byref(bad))
+    total = int(row_off[-1])
+    if dev:
+        out = torch.empty(0, dtype=torch.float32 if elem == VECTOR else torch.float16, device=text.device)
+    else:
+        out = np.empty(0, dtype=_NP[elem])
+    if rc == _lib.EINVAL and total > 0 and bad.value < 0:
+        if dev:
+            out = torch.empty(total, dtype=torch.float32 if elem == VECTOR else torch.float16, device=text.device)
+        else:
+            out = np.empty(total, dtype=_NP[elem])
+        rc = fn(elem, typmod, n, _ptr(text), _ptr(off), total, _ptr(row_off), _ptr(out), C.byref(bad))
+    _raise_text(rc, bad)
+    if dev:
+        return out, row_off
+    return [out[row_off[i]:row_off[i + 1]] for i in range(n)]
+
+
+def vector_in(texts, typmod=-1):
+    """vector_in (src/vector.c:174-281) of every literal: a list of str gives a list of float32 arrays; a (CUDA uint8
+    text, CUDA int64 offsets) pair gives device (values, row offsets).  The reference's errors raise
+    TextInputError (a ValueError) with .detail and .row."""
+    return _text_to_rows(VECTOR, texts, typmod)
+
+
+def halfvec_in(texts, typmod=-1):
+    """halfvec_in (src/halfvec.c:178-286): rows as binary16 bit patterns (uint16) on the host, float16 on the device."""
+    return _text_to_rows(HALFVEC, texts, typmod)
+
+
+def _rows_to_text(elem, rows):
+    lib = load()
+    if _is_cuda(rows):
+        import torch
+        x, _ = _dev_rows(rows, elem)
+        n, dim = int(x.shape[0]), int(x.shape[1])
+        off = torch.empty(n + 1, dtype=torch.int64, device=x.device)
+        _after_torch(x)
+        _lib.check(lib.vb_rows_to_text_batch_dev(elem, dim, _ptr(x), n, 0, _ptr(off), None))
+        out = torch.empty(max(int(off[-1]), 1), dtype=torch.uint8, device=x.device)
+        _lib.check(lib.vb_rows_to_text_batch_dev(elem, dim, _ptr(x), n, int(off[-1]), _ptr(off), _ptr(out)))
+        return out[:int(off[-1])], off
+    x = _host(elem, rows)
+    x = x.reshape(1, -1) if x.ndim == 1 else x
+    n, dim = x.shape
+    # the reference's own bound: 15 bytes per element, separators and brackets
+    cap = n * (dim * 16 + 2)
+    off = np.empty(n + 1, dtype=np.int64)
+    out = np.empty(max(cap, 1), dtype=np.uint8)
+    _lib.check(lib.vb_rows_to_text_batch(elem, dim, _ptr(x), n, cap, _ptr(off), _ptr(out)))
+    blob = out.tobytes()
+    return [blob[off[i]:off[i + 1]].decode() for i in range(n)]
+
+
+def vector_out(rows):
+    """vector_out (src/vector.c:289-326) of every row: numpy rows give a list of str, CUDA rows device (text, offsets)."""
+    return _rows_to_text(VECTOR, rows)
+
+
+def halfvec_out(rows):
+    """halfvec_out (src/halfvec.c:294-335): numpy rows are binary16 bit patterns (uint16) or floats rounded to half."""
+    return _rows_to_text(HALFVEC, rows)
+
+
+from .sparsevec import sparsevec_in, sparsevec_out  # noqa: E402,F401

@@ -22,6 +22,7 @@ SIGNATURES = {
     "vb_init": (_i, [_i]),
     "vb_shutdown": (_i, []),
     "vb_last_error": (C.c_char_p, []),
+    "vb_last_error_detail": (C.c_char_p, []),
     "vb_abi_version": (_i, []),
     "vb_stream": (_vp, []),
     "vb_launch_count": (_i64, []),
@@ -69,6 +70,14 @@ SIGNATURES = {
     "vb_dense_to_sparsevec_batch_dev": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp, _vp]),
     "vb_sparsevec_to_dense_batch": (_i, [_i, _i, _i64, _vp, _vp, _vp, _vp]),
     "vb_sparsevec_to_dense_batch_dev": (_i, [_i, _i, _i64, _vp, _vp, _vp, _vp]),
+    "vb_text_to_rows_batch": (_i, [_i, C.c_int32, _i64, _vp, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
+    "vb_text_to_rows_batch_dev": (_i, [_i, C.c_int32, _i64, _vp, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
+    "vb_text_to_sparsevec_batch": (_i, [C.c_int32, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp, C.POINTER(_i64)]),
+    "vb_text_to_sparsevec_batch_dev": (_i, [C.c_int32, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp, C.POINTER(_i64)]),
+    "vb_rows_to_text_batch": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp]),
+    "vb_rows_to_text_batch_dev": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp]),
+    "vb_sparsevec_to_text_batch": (_i, [_i, _i64, _vp, _vp, _vp, _i64, _vp, _vp]),
+    "vb_sparsevec_to_text_batch_dev": (_i, [_i, _i64, _vp, _vp, _vp, _i64, _vp, _vp]),
     "vb_table_create": (_i, [_i, _i, C.POINTER(_vp)]),
     "vb_table_append": (_i, [_vp, _vp, _i64]),
     "vb_table_append_dev": (_i, [_vp, _vp, _i64]),
@@ -185,6 +194,16 @@ class IvfBuildOpts(C.Structure):
     """vb_ivf_build_opts"""
     _fields_ = [("seed", _u64), ("max_iter", _i), ("sample_rows", _vp), ("n_samples", _i64), ("first_row", _i64), ("u", _vp),
                 ("chunk_rows", _i64)]
+
+
+class TextInputError(ValueError):
+    """a type input error: the reference's errmsg, with its errdetail (.detail, "" when none) and the failing
+    literal's index (.row)"""
+
+    def __init__(self, msg, detail, row):
+        super().__init__(msg)
+        self.detail = detail
+        self.row = row
 
 
 class VecB200Error(RuntimeError):

@@ -10,16 +10,27 @@
 
 namespace vb {
 
-static thread_local char g_err[512] = "";
+// grows to hold the longest message: the type input errors echo their whole literal (16000 elements, ~250 kB)
+static thread_local std::string g_err;
+static thread_local std::string g_err_detail;
 thread_local int g_last_status = 0;
 
 void set_error(const char* fmt, ...) {
-    va_list ap;
+    va_list ap, ap2;
     va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
+    va_copy(ap2, ap);
+    const int len = vsnprintf(nullptr, 0, fmt, ap);
     va_end(ap);
+    std::string msg(len > 0 ? (size_t)len : 0, '\0');   // formatted apart: an argument may be the old message
+    if (len > 0) vsnprintf(&msg[0], (size_t)len + 1, fmt, ap2);
+    va_end(ap2);
+    g_err.swap(msg);
+    g_err_detail.clear();
 }
-const char* last_error() { return g_err; }
+// the errdetail of the error just set (the type input errors have one)
+void set_error_detail(const char* detail) { g_err_detail = detail; }
+const char* last_error() { return g_err.c_str(); }
+const char* last_error_detail() { return g_err_detail.c_str(); }
 int prof_read(int which, double* total_ms, int64_t* launches);
 void prof_set(bool on);
 
@@ -304,6 +315,7 @@ extern "C" {
 int vb_abi_version(void) { return VB_ABI_VERSION; }
 
 const char* vb_last_error(void) { return vb::last_error(); }
+const char* vb_last_error_detail(void) { return vb::last_error_detail(); }
 
 int vb_init(int device) {
     vb::Context& c = vb::ctx();

@@ -515,6 +515,10 @@ static int check_csr_dev(const char* what, int dim, int64_t n, const int64_t* of
     return VB_OK;
 }
 
+int sparse_csr_check_dev(const char* what, int dim, int64_t n, const int64_t* off, const int32_t* idx) {
+    return check_csr_dev(what, dim, n, off, idx, nullptr, nullptr);
+}
+
 static bool sparse_metric_ok(int metric) {
     return metric == VB_L2_SQUARED || metric == VB_L2 || metric == VB_IP || metric == VB_NEG_IP || metric == VB_COSINE || metric == VB_L1;
 }

@@ -526,3 +526,70 @@ class SparseTable:
             self.free()
         except Exception:
             pass
+
+
+# ------------------------------------------------------------------------- type I/O
+
+def sparsevec_in(texts, typmod=-1):
+    """sparsevec_in (src/sparsevec.c:203-409) of every literal -> (SparseRows, dims): ascending indices, no zeros;
+    SparseRows.dim is the literals' common dimension (0 when they differ).  A (CUDA uint8 text, CUDA int64 offsets)
+    pair gives ((row_off, idx, val), dims) as CUDA tensors.  The reference's errors raise TextInputError."""
+    from . import _after_torch, _ptr, _raise_text, _text_input
+    lib = load()
+    text, off, n, dev = _text_input(texts)
+    bad = C.c_int64(-1)
+    if dev:
+        import torch
+        new = lambda k, dt: torch.empty(max(k, 1), dtype=dt, device=text.device)  # noqa: E731
+        i32, i64, f32 = torch.int32, torch.int64, torch.float32
+        fn = lib.vb_text_to_sparsevec_batch_dev
+        _after_torch(text, off)
+    else:
+        new = lambda k, dt: np.empty(max(k, 1), dtype=dt)  # noqa: E731
+        i32, i64, f32 = np.int32, np.int64, np.float32
+        fn = lib.vb_text_to_sparsevec_batch
+    row_off, dims = new(n + 1, i64), new(n, i32)
+    row_off[:] = 0      # a refused argument writes no offsets
+    rc = fn(typmod, n, _ptr(text), _ptr(off), 0, _ptr(dims), _ptr(row_off), None, None, C.byref(bad))
+    bound = int(row_off[n])
+    idx, val = new(bound, i32), new(bound, f32)
+    if rc == _lib.EINVAL and bound > 0 and bad.value < 0:
+        rc = fn(typmod, n, _ptr(text), _ptr(off), bound, _ptr(dims), _ptr(row_off), _ptr(idx), _ptr(val), C.byref(bad))
+    _raise_text(rc, bad)
+    tot = int(row_off[n])
+    dims = dims[:n]
+    if dev:
+        return (row_off, idx[:tot], val[:tot]), dims
+    common = int(dims[0]) if n and (dims == dims[0]).all() else 0
+    return SparseRows(common, row_off, idx[:tot], val[:tot]), dims
+
+
+def sparsevec_out(rows):
+    """sparsevec_out (src/sparsevec.c:428-476) of every row: SparseRows give a list of str; device CSR
+    ((row_off, idx, val) CUDA tensors, or a torch sparse CSR tensor) with rows.dim given as ((...), dim) gives device
+    (text, offsets)."""
+    from . import _after_torch
+    lib = load()
+    if isinstance(rows, tuple) and len(rows) == 2 and isinstance(rows[1], int):
+        got = _device_csr(rows[0], rows[1])
+        if got is not None:
+            import torch
+            n, dim, roff, idx, val = got
+            out_off = torch.empty(n + 1, dtype=torch.int64, device=roff.device)
+            _after_torch(roff, idx, val)
+            _lib.check(lib.vb_sparsevec_to_text_batch_dev(dim, n, _tp(roff), _tp(idx), _tp(val), 0, _tp(out_off), None))
+            out = torch.empty(max(int(out_off[-1]), 1), dtype=torch.uint8, device=roff.device)
+            _lib.check(lib.vb_sparsevec_to_text_batch_dev(dim, n, _tp(roff), _tp(idx), _tp(val), int(out_off[-1]),
+                                                          _tp(out_off), _tp(out)))
+            return out[:int(out_off[-1])], out_off
+    rows = _rows(rows)
+    n = rows.n
+    nnz = int(rows.row_off[-1] - rows.row_off[0])
+    cap = 28 * nnz + 15 * n
+    off = np.empty(n + 1, dtype=np.int64)
+    out = np.empty(max(cap, 1), dtype=np.uint8)
+    roff = np.ascontiguousarray(rows.row_off - rows.row_off[0])
+    _lib.check(lib.vb_sparsevec_to_text_batch(rows.dim, n, _p(roff), _p(rows.idx[rows.row_off[0]:]),
+                                              _p(rows.val[rows.row_off[0]:]), cap, _p(off), _p(out)))
+    blob = out.tobytes()
+    return [blob[off[i]:off[i + 1]].decode() for i in range(n)]
