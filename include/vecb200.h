@@ -36,6 +36,9 @@
  *     sparsevec _dev calls, and vb_arith_batch_dev and vb_array_to_rows_batch_dev read the
  *     8-byte key of the first value that fails the reference's checks, plus, for a halfvec
  *     range error only, that source element (at most 8 bytes, for the error text).
+ *     The binary receive calls read the bound total (8 bytes) and a 24-byte status;
+ *     vb_sparsevec_to_binary_batch_dev reads its 24-byte CSR check; vb_rows_to_binary_batch_dev
+ *     reads nothing (it can be captured into a CUDA graph).
  *   - rows are row-major and contiguous in the caller's buffers (vector: dim
  *     fp32; halfvec: dim IEEE binary16; bit: (dim+7)/8 bytes, MSB first, tail
  *     bits zero -- exactly the payload of Vector.x (src/vector.h:18-24),
@@ -124,6 +127,8 @@ int			vb_stream_wait_event(void *cuda_event);
 #define VB_PROF_BUILD_ASSIGN 13	/* pass one: the list of every row (per chunk: padding / normalisation, assign) */
 #define VB_PROF_TEXT_PARSE 14	/* the type input parse kernels (text_parse_dense_kernel, text_parse_sparse_kernel) */
 #define VB_PROF_TEXT_FORMAT 15	/* the type output kernels (text_format_kernel, length and write passes) */
+#define VB_PROF_BINARY_RECV 16	/* the binary receive kernels (recv_dense_kernel, recv_sparse_kernel) */
+#define VB_PROF_BINARY_SEND 17	/* the binary send kernels (send_dense_kernel, send_sparse_kernel) */
 int			vb_prof_enable(int on);
 /* Synchronises, then returns accumulated milliseconds and bracketed launches since the last read of `kernel`. */
 int			vb_prof_read(int kernel, double *total_ms, int64_t *launches);
@@ -580,6 +585,62 @@ int			vb_sparsevec_to_text_batch(int dim, int64_t n, const int64_t *row_off, con
 									   int64_t cap, int64_t *out_off, char *out);
 int			vb_sparsevec_to_text_batch_dev(int dim, int64_t n, const int64_t *row_off_dev, const int32_t *idx_dev,
 										   const float *val_dev, int64_t cap, int64_t *out_off_dev, char *out_dev);
+
+/* ------------------------------------------------------------ binary input and output */
+
+/*
+ * The binary type I/O over a column, what COPY ... (FORMAT binary) and binary bind parameters run: vector_recv /
+ * vector_send (src/vector.c:376-422), halfvec_recv / halfvec_send (src/halfvec.c:43-72, 373-419, elem = VB_HALFVEC),
+ * sparsevec_recv / sparsevec_send (src/sparsevec.c:514-585).  Values, bytes and error texts are the reference's.
+ *
+ * Payloads.  Field i is bytes[off[i] .. off[i + 1]), the bytes the server hands the receive function (no length word;
+ * a zero byte is data; any alignment; NULL fields are not in the batch).  vector / halfvec: uint16 dim, uint16 unused,
+ * then dim big-endian float4 (halfvec: binary16 bits); sparsevec: int32 dim, nnz and unused, nnz 0-based int32
+ * indices, then nnz float4 values.
+ *
+ * Receive.  Each field is decoded in the reference's order: the header reads, CheckDim, (sparsevec: CheckNnz),
+ * CheckExpectedDim, unused != 0, then element by element the read and CheckElement (sparsevec: every index read and
+ * CheckIndex, then every value read, CheckElement and the zero check).  A read past the end of the field fails where it
+ * happens with PostgreSQL's "insufficient data left in message"; bytes left over after a good decode fail with COPY's
+ * "incorrect binary data format".  A failing call (VB_EINVAL) raises the error row-by-row execution raises first: the
+ * lowest failing field, within it the first step above.  vb_last_error() is the errmsg, vb_last_error_detail() is "",
+ * *out_bad (may be NULL) the failing field's index (-1 otherwise); the rows are then unspecified.
+ *
+ * Sizes.  The bound of a field is max(0, (len - 4) / esz) elements (esz 4 or 2), sparsevec max(0, (len - 12) / 8)
+ * entries; a field that decodes has exactly its bound, so out_row_off [n + 1], always written, is final from the
+ * offsets alone.  A bound total above cap fails naming the total and writes nothing else; out = NULL (sparsevec: idx and
+ * val) with cap 0 sizes.  Dense rows are packed at out_row_off (with a typmod, the n x typmod block
+ * vb_table_append_dev takes); sparsevec gives the CSR the sparse table calls take and every field's dim in out_dim [n].
+ *
+ * Send.  Rows are written byte for byte as the reference's send writes them, bits unchanged (-0, subnormals, inf and
+ * NaN payloads: send checks nothing); dense rows are n x dim, dim <= 65535.  out_off [n + 1] is always written; a total
+ * above cap fails naming it, out = NULL sizes.  sparsevec rows (offsets from 0) are first checked as
+ * vb_sparsevec_to_text_batch checks them, with the same texts and "(row r)".
+ *
+ * Host variants stream through the pinned staging of the text calls in chunks of at most 64 MiB of payload (one larger
+ * field or row makes a chunk of its own).  Since sizes follow from the offsets, receive and dense send pipeline: the
+ * host stages chunk c + 1 and copies out chunk c - 1 while chunk c runs.  sparsevec send runs its chunks one after
+ * another (each reads back its CSR check).  _dev variants take device pointers (out_bad and cap stay host values) and
+ * run on vb_stream(); what they read back is listed in the conventions above.  Receive and sparsevec send synchronise;
+ * vb_rows_to_binary_batch_dev only enqueues.
+ */
+int			vb_binary_to_rows_batch(int elem, int32_t typmod, int64_t n, const void *bytes, const int64_t *off, int64_t cap,
+									int64_t *out_row_off, void *out, int64_t *out_bad);
+int			vb_binary_to_rows_batch_dev(int elem, int32_t typmod, int64_t n, const void *bytes_dev, const int64_t *off_dev,
+										int64_t cap, int64_t *out_row_off_dev, void *out_dev, int64_t *out_bad);
+int			vb_binary_to_sparsevec_batch(int32_t typmod, int64_t n, const void *bytes, const int64_t *off, int64_t cap,
+										 int32_t *out_dim, int64_t *out_row_off, int32_t *out_idx, float *out_val,
+										 int64_t *out_bad);
+int			vb_binary_to_sparsevec_batch_dev(int32_t typmod, int64_t n, const void *bytes_dev, const int64_t *off_dev,
+											 int64_t cap, int32_t *out_dim_dev, int64_t *out_row_off_dev,
+											 int32_t *out_idx_dev, float *out_val_dev, int64_t *out_bad);
+int			vb_rows_to_binary_batch(int elem, int dim, const void *rows, int64_t n, int64_t cap, int64_t *out_off, void *out);
+int			vb_rows_to_binary_batch_dev(int elem, int dim, const void *rows_dev, int64_t n, int64_t cap,
+										int64_t *out_off_dev, void *out_dev);
+int			vb_sparsevec_to_binary_batch(int dim, int64_t n, const int64_t *row_off, const int32_t *idx, const float *val,
+										 int64_t cap, int64_t *out_off, void *out);
+int			vb_sparsevec_to_binary_batch_dev(int dim, int64_t n, const int64_t *row_off_dev, const int32_t *idx_dev,
+											 const float *val_dev, int64_t cap, int64_t *out_off_dev, void *out_dev);
 
 /* ------------------------------------------------------------ ordering by value */
 

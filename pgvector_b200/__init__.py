@@ -1611,7 +1611,8 @@ def array_to_halfvec(rows, typmod=-1):
 # ------------------------------------------------------------------------- type I/O: text in, text out
 
 def _text_input(texts):
-    """(text, off, n, on the device) of a list of str, or of a (CUDA uint8 tensor, CUDA int64 offsets) pair"""
+    """(bytes, off, n, on the device) of a list of str (text literals) or bytes (binary payloads), or of a (CUDA uint8
+    tensor, CUDA int64 offsets) pair"""
     if isinstance(texts, (tuple, list)) and len(texts) == 2 and all(_is_cuda(t) for t in texts):
         import torch
         text, off = texts
@@ -1710,4 +1711,81 @@ def halfvec_out(rows):
     return _rows_to_text(HALFVEC, rows)
 
 
-from .sparsevec import sparsevec_in, sparsevec_out  # noqa: E402,F401
+# ------------------------------------------------------------------------- type I/O: binary in, binary out
+
+def _binary_to_rows(elem, payloads, typmod):
+    lib = load()
+    data, off, n, dev = _text_input(payloads)
+    bad = C.c_int64(-1)
+    if dev:
+        import torch
+        torch_dt = torch.float32 if elem == VECTOR else torch.float16
+        row_off = torch.zeros(n + 1, dtype=torch.int64, device=data.device)   # a refused argument writes none
+        fn = lib.vb_binary_to_rows_batch_dev
+        _after_torch(data, off)
+    else:
+        row_off = np.zeros(n + 1, dtype=np.int64)
+        fn = lib.vb_binary_to_rows_batch
+    rc = fn(elem, typmod, n, _ptr(data), _ptr(off), 0, _ptr(row_off), None, C.byref(bad))
+    total = int(row_off[-1])
+    if dev:
+        out = torch.empty(max(total, 1), dtype=torch_dt, device=data.device)
+    else:
+        out = np.empty(max(total, 1), dtype=_NP[elem])
+    if rc == _lib.EINVAL and bad.value < 0 and total > 0:
+        rc = fn(elem, typmod, n, _ptr(data), _ptr(off), total, _ptr(row_off), _ptr(out), C.byref(bad))
+    _raise_text(rc, bad)
+    out = out[:total]
+    if dev:
+        return out, row_off
+    return [out[row_off[i]:row_off[i + 1]] for i in range(n)]
+
+
+def vector_recv(payloads, typmod=-1):
+    """vector_recv (src/vector.c:376-400) of every field: a list of bytes gives a list of float32 arrays; a (CUDA uint8
+    payloads, CUDA int64 offsets) pair gives device (values, row offsets), as vector_in does.  The reference's errors,
+    and PostgreSQL's for a short or overlong field, raise TextInputError (a ValueError) with .row."""
+    return _binary_to_rows(VECTOR, payloads, typmod)
+
+
+def halfvec_recv(payloads, typmod=-1):
+    """halfvec_recv (src/halfvec.c:373-401): rows as binary16 bit patterns (uint16) on the host, float16 on the device."""
+    return _binary_to_rows(HALFVEC, payloads, typmod)
+
+
+def _rows_to_binary(elem, rows):
+    lib = load()
+    if _is_cuda(rows):
+        import torch
+        x, _ = _dev_rows(rows, elem)
+        n, dim = int(x.shape[0]), int(x.shape[1])
+        off = torch.empty(n + 1, dtype=torch.int64, device=x.device)
+        total = n * (4 + dim * x.element_size())
+        out = torch.empty(max(total, 1), dtype=torch.uint8, device=x.device)
+        _after_torch(x)
+        _lib.check(lib.vb_rows_to_binary_batch_dev(elem, dim, _ptr(x), n, total, _ptr(off), _ptr(out)))
+        synchronize()
+        return out[:total], off
+    x = _host(elem, rows)
+    x = x.reshape(1, -1) if x.ndim == 1 else x
+    n, dim = x.shape
+    cap = n * (4 + dim * x.itemsize)
+    off = np.empty(n + 1, dtype=np.int64)
+    out = np.empty(max(cap, 1), dtype=np.uint8)
+    _lib.check(lib.vb_rows_to_binary_batch(elem, dim, _ptr(x), n, cap, _ptr(off), _ptr(out)))
+    blob = out.tobytes()
+    return [blob[off[i]:off[i + 1]] for i in range(n)]
+
+
+def vector_send(rows):
+    """vector_send (src/vector.c:405-422) of every row: numpy rows give a list of bytes, CUDA rows device (payloads,
+    offsets).  The bits go out unchanged."""
+    return _rows_to_binary(VECTOR, rows)
+
+
+def halfvec_send(rows):
+    """halfvec_send (src/halfvec.c:406-419): numpy rows are binary16 bit patterns (uint16) or floats rounded to half."""
+    return _rows_to_binary(HALFVEC, rows)
+
+
+from .sparsevec import sparsevec_in, sparsevec_out, sparsevec_recv, sparsevec_send  # noqa: E402,F401

@@ -78,6 +78,14 @@ SIGNATURES = {
     "vb_rows_to_text_batch_dev": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp]),
     "vb_sparsevec_to_text_batch": (_i, [_i, _i64, _vp, _vp, _vp, _i64, _vp, _vp]),
     "vb_sparsevec_to_text_batch_dev": (_i, [_i, _i64, _vp, _vp, _vp, _i64, _vp, _vp]),
+    "vb_binary_to_rows_batch": (_i, [_i, C.c_int32, _i64, _vp, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
+    "vb_binary_to_rows_batch_dev": (_i, [_i, C.c_int32, _i64, _vp, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
+    "vb_binary_to_sparsevec_batch": (_i, [C.c_int32, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp, C.POINTER(_i64)]),
+    "vb_binary_to_sparsevec_batch_dev": (_i, [C.c_int32, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp, C.POINTER(_i64)]),
+    "vb_rows_to_binary_batch": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp]),
+    "vb_rows_to_binary_batch_dev": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp]),
+    "vb_sparsevec_to_binary_batch": (_i, [_i, _i64, _vp, _vp, _vp, _i64, _vp, _vp]),
+    "vb_sparsevec_to_binary_batch_dev": (_i, [_i, _i64, _vp, _vp, _vp, _i64, _vp, _vp]),
     "vb_table_create": (_i, [_i, _i, C.POINTER(_vp)]),
     "vb_table_append": (_i, [_vp, _vp, _i64]),
     "vb_table_append_dev": (_i, [_vp, _vp, _i64]),

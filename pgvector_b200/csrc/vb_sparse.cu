@@ -515,8 +515,8 @@ static int check_csr_dev(const char* what, int dim, int64_t n, const int64_t* of
     return VB_OK;
 }
 
-int sparse_csr_check_dev(const char* what, int dim, int64_t n, const int64_t* off, const int32_t* idx) {
-    return check_csr_dev(what, dim, n, off, idx, nullptr, nullptr);
+int sparse_csr_check_dev(const char* what, int dim, int64_t n, const int64_t* off, const int32_t* idx, int64_t* total) {
+    return check_csr_dev(what, dim, n, off, idx, nullptr, total);
 }
 
 static bool sparse_metric_ok(int metric) {

@@ -3,6 +3,7 @@
 // (src/vector.c:289-326, src/halfvec.c:294-335, src/sparsevec.c:428-476), one warp per literal or row.
 #include "vb_common.cuh"
 #include "vb_text.cuh"
+#include "vb_typio.cuh"
 
 #include <cub/cub.cuh>
 
@@ -11,9 +12,38 @@
 #include <vector>
 
 namespace vb {
+int offsets_from_counts(const int64_t* count, int64_t n, int64_t* row_off) {
+    cudaStream_t s = ctx().stream;
+    VB_CUDA(cudaMemsetAsync(row_off, 0, sizeof(int64_t), s));
+    if (n == 0) return VB_OK;
+    size_t tb = 0;
+    VB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, count, row_off + 1, n, s));
+    DevBuf tmp;
+    VB_TRY(tmp.alloc(tb));
+    VB_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, count, row_off + 1, n, s));
+    count_launch();
+    return VB_OK;
+}
+
+Staging& staging() {
+    static Staging st;
+    return st;
+}
+
+int pinned_grow(void** buf, size_t* have, size_t bytes) {
+    if (*have >= bytes) return VB_OK;
+    if (*buf) VB_CUDA(cudaFreeHost(*buf));
+    *buf = nullptr;
+    *have = 0;
+    if (cudaMallocHost(buf, bytes) != cudaSuccess) {
+        set_error("cudaMallocHost(%zu) for type I/O staging failed", bytes);
+        return VB_ENOMEM;
+    }
+    *have = bytes;
+    return VB_OK;
+}
+
 void set_error_detail(const char* detail);
-// the sparse table calls' check of device CSR rows, with their texts (vb_sparse.cu)
-int sparse_csr_check_dev(const char* what, int dim, int64_t n, const int64_t* off, const int32_t* idx);
 
 namespace {
 using namespace text;
@@ -452,33 +482,6 @@ int grid_for(int64_t n) {
     return (int)std::max<int64_t>(1, std::min(want, cap));
 }
 
-// device buffer freed at scope exit (stream-ordered)
-struct DevBuf {
-    void* p = nullptr;
-    ~DevBuf() { if (p) cudaFreeAsync(p, ctx().stream); }
-    int alloc(size_t bytes) {
-        if (cudaMallocAsync(&p, bytes ? bytes : 16, ctx().stream) != cudaSuccess) {
-            set_error("cudaMallocAsync(%zu) for the text call failed", bytes);
-            return VB_ENOMEM;
-        }
-        return VB_OK;
-    }
-};
-
-// row_off[0] = 0, row_off[1 + i] = sum of count[0 .. i]
-int offsets_from_counts(const int64_t* count, int64_t n, int64_t* row_off) {
-    cudaStream_t s = ctx().stream;
-    VB_CUDA(cudaMemsetAsync(row_off, 0, sizeof(int64_t), s));
-    if (n == 0) return VB_OK;
-    size_t tb = 0;
-    VB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, count, row_off + 1, n, s));
-    DevBuf tmp;
-    VB_TRY(tmp.alloc(tb));
-    VB_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, count, row_off + 1, n, s));
-    count_launch();
-    return VB_OK;
-}
-
 const char* type_name(int kind) { return kind == 0 ? "vector" : kind == 1 ? "halfvec" : "sparsevec"; }
 
 // the reference's error for a recorded failure; lit is the literal up to its first NUL
@@ -604,30 +607,6 @@ int64_t host_count(const char* t, int64_t len) {
     int64_t c = 1;
     for (const char* p = t; (p = static_cast<const char*>(std::memchr(p, ',', (size_t)(end - p)))) != nullptr; ++p) ++c;
     return c;
-}
-
-// pinned staging of the pipelined host input: two slots, each text + offsets in and rows + status out
-struct Staging {
-    void* in[2] = {nullptr, nullptr};
-    void* out[2] = {nullptr, nullptr};
-    size_t in_bytes[2] = {0, 0}, out_bytes[2] = {0, 0};
-    cudaEvent_t done[2] = {nullptr, nullptr};
-};
-Staging& staging() {
-    static Staging st;
-    return st;
-}
-int pinned_grow(void** buf, size_t* have, size_t bytes) {
-    if (*have >= bytes) return VB_OK;
-    if (*buf) VB_CUDA(cudaFreeHost(*buf));
-    *buf = nullptr;
-    *have = 0;
-    if (cudaMallocHost(buf, bytes) != cudaSuccess) {
-        set_error("cudaMallocHost(%zu) for text staging failed", bytes);
-        return VB_ENOMEM;
-    }
-    *have = bytes;
-    return VB_OK;
 }
 
 
@@ -835,31 +814,14 @@ int vb_text_to_rows_batch(int elem, int32_t typmod, int64_t n, const char* text,
     for (int k = 0; k < 2 && k < nch; ++k) {
         VB_TRY(pinned_grow(&sg.in[k], &sg.in_bytes[k], in_bytes));
         VB_TRY(pinned_grow(&sg.out[k], &sg.out_bytes[k], out_bytes));
-        if (!sg.done[k]) VB_CUDA(cudaEventCreateWithFlags(&sg.done[k], cudaEventDisableTiming));
         VB_TRY(dtext[k].alloc((size_t)max_tb));
         VB_TRY(doff[k].alloc(sizeof(int64_t) * 2 * (size_t)(max_nr + 1)));
         VB_TRY(dout[k].alloc(esz * (size_t)max_ne));
         VB_TRY(dst[k].alloc(sizeof(Status)));
     }
-    auto finish_chunk = [&](int64_t c) -> int {
-        const int k = (int)(c & 1);
-        const int64_t r0 = cuts[c], r1 = cuts[c + 1];
-        VB_CUDA(cudaEventSynchronize(sg.done[k]));
-        const Status& st = *static_cast<const Status*>(sg.out[k]);
-        if (st.first_bad != ~0ull) {
-            if (out_bad) *out_bad = r0 + (int64_t)st.first_bad;
-            return text_error(elem == VB_VECTOR ? 0 : 1, typmod, st,
-                              std::string(text + off[r0] + st.lit_begin, (size_t)st.lit_len));
-        }
-        std::memcpy(static_cast<char*>(out) + esz * (size_t)out_row_off[r0], static_cast<char*>(sg.out[k]) + sizeof(Status),
-                    esz * (size_t)(out_row_off[r1] - out_row_off[r0]));
-        return VB_OK;
-    };
-    for (int64_t c = 0; c < nch; ++c) {
-        const int k = (int)(c & 1);
+    auto enqueue = [&](int64_t c, int k) -> int {
         const int64_t r0 = cuts[c], r1 = cuts[c + 1];
         const int64_t tb = off[r1] - off[r0], nr = r1 - r0, ne = out_row_off[r1] - out_row_off[r0];
-        // slot k's last user, chunk c - 2, was finished (its event waited for) in the previous iteration
         char* ptext = static_cast<char*>(sg.in[k]);
         int64_t* poff = reinterpret_cast<int64_t*>(ptext + tb_al);
         std::memcpy(ptext, text + off[r0], (size_t)tb);
@@ -875,17 +837,21 @@ int vb_text_to_rows_batch(int elem, int32_t typmod, int64_t n, const char* text,
         VB_CUDA(cudaMemcpyAsync(sg.out[k], sp, sizeof(Status), cudaMemcpyDeviceToHost, s));
         VB_CUDA(cudaMemcpyAsync(static_cast<char*>(sg.out[k]) + sizeof(Status), dout[k].p, esz * (size_t)ne,
                                 cudaMemcpyDeviceToHost, s));
-        VB_CUDA(cudaEventRecord(sg.done[k], s));
-        if (c >= 1) {
-            const int rc = finish_chunk(c - 1);
-            if (rc != VB_OK) {
-                cudaStreamSynchronize(s);   // chunk c is still in flight: let it land before the buffers go
-                return rc;
-            }
+        return VB_OK;
+    };
+    auto finish_chunk = [&](int64_t c, int k) -> int {
+        const int64_t r0 = cuts[c], r1 = cuts[c + 1];
+        const Status& st = *static_cast<const Status*>(sg.out[k]);
+        if (st.first_bad != ~0ull) {
+            if (out_bad) *out_bad = r0 + (int64_t)st.first_bad;
+            return text_error(elem == VB_VECTOR ? 0 : 1, typmod, st,
+                              std::string(text + off[r0] + st.lit_begin, (size_t)st.lit_len));
         }
-    }
-    VB_TRY(finish_chunk(nch - 1));
-    return VB_OK;
+        std::memcpy(static_cast<char*>(out) + esz * (size_t)out_row_off[r0], static_cast<char*>(sg.out[k]) + sizeof(Status),
+                    esz * (size_t)(out_row_off[r1] - out_row_off[r0]));
+        return VB_OK;
+    };
+    return pipeline_chunks(nch, enqueue, finish_chunk);
 }
 
 int vb_text_to_sparsevec_batch_dev(int32_t typmod, int64_t n, const char* text, const int64_t* off, int64_t cap,

@@ -593,3 +593,70 @@ def sparsevec_out(rows):
                                               _p(rows.val[rows.row_off[0]:]), cap, _p(off), _p(out)))
     blob = out.tobytes()
     return [blob[off[i]:off[i + 1]].decode() for i in range(n)]
+
+
+def sparsevec_recv(payloads, typmod=-1):
+    """sparsevec_recv (src/sparsevec.c:514-562) of every field (a list of bytes, or a (CUDA uint8 payloads, CUDA int64
+    offsets) pair), with sparsevec_in's return shapes.  The reference's errors, and PostgreSQL's for a short or
+    overlong field, raise TextInputError (a ValueError) with .row."""
+    from . import _after_torch, _ptr, _raise_text, _text_input
+    lib = load()
+    data, off, n, dev = _text_input(payloads)
+    bad = C.c_int64(-1)
+    if dev:
+        import torch
+        new = lambda k, dt: torch.empty(max(k, 1), dtype=dt, device=data.device)  # noqa: E731
+        i32, i64, f32 = torch.int32, torch.int64, torch.float32
+        fn = lib.vb_binary_to_sparsevec_batch_dev
+        _after_torch(data, off)
+    else:
+        new = lambda k, dt: np.empty(max(k, 1), dtype=dt)  # noqa: E731
+        i32, i64, f32 = np.int32, np.int64, np.float32
+        fn = lib.vb_binary_to_sparsevec_batch
+    row_off, dims = new(n + 1, i64), new(n, i32)
+    row_off[:] = 0      # a refused argument writes no offsets
+    rc = fn(typmod, n, _ptr(data), _ptr(off), 0, _ptr(dims), _ptr(row_off), None, None, C.byref(bad))
+    tot = int(row_off[n])
+    idx, val = new(tot, i32), new(tot, f32)
+    if rc == _lib.EINVAL and tot > 0 and bad.value < 0:
+        rc = fn(typmod, n, _ptr(data), _ptr(off), tot, _ptr(dims), _ptr(row_off), _ptr(idx), _ptr(val), C.byref(bad))
+    _raise_text(rc, bad)
+    dims = dims[:n]
+    if dev:
+        return (row_off, idx[:tot], val[:tot]), dims
+    common = int(dims[0]) if n and (dims == dims[0]).all() else 0
+    return SparseRows(common, row_off, idx[:tot], val[:tot]), dims
+
+
+def sparsevec_send(rows):
+    """sparsevec_send (src/sparsevec.c:567-585) of every row: SparseRows give a list of bytes; device CSR given as
+    ((row_off, idx, val), dim) gives device (payloads, offsets).  Rows that break the CSR rules raise with the texts
+    of sparsevec_out."""
+    from . import _after_torch, synchronize
+    lib = load()
+    if isinstance(rows, tuple) and len(rows) == 2 and isinstance(rows[1], int):
+        got = _device_csr(rows[0], rows[1])
+        if got is not None:
+            import torch
+            n, dim, roff, idx, val = got
+            out_off = torch.empty(n + 1, dtype=torch.int64, device=roff.device)
+            _after_torch(roff, idx, val)
+            _lib.check(lib.vb_sparsevec_to_binary_batch_dev(dim, n, _tp(roff), _tp(idx), _tp(val), 0, _tp(out_off), None))
+            synchronize()
+            total = int(out_off[-1])
+            out = torch.empty(max(total, 1), dtype=torch.uint8, device=roff.device)
+            _lib.check(lib.vb_sparsevec_to_binary_batch_dev(dim, n, _tp(roff), _tp(idx), _tp(val), total, _tp(out_off),
+                                                            _tp(out)))
+            synchronize()
+            return out[:total], out_off
+    rows = _rows(rows)
+    n = rows.n
+    nnz = int(rows.row_off[-1] - rows.row_off[0])
+    cap = 12 * n + 8 * nnz
+    off = np.empty(n + 1, dtype=np.int64)
+    out = np.empty(max(cap, 1), dtype=np.uint8)
+    roff = np.ascontiguousarray(rows.row_off - rows.row_off[0])
+    _lib.check(lib.vb_sparsevec_to_binary_batch(rows.dim, n, _p(roff), _p(rows.idx[rows.row_off[0]:]),
+                                                _p(rows.val[rows.row_off[0]:]), cap, _p(off), _p(out)))
+    blob = out.tobytes()
+    return [blob[off[i]:off[i + 1]] for i in range(n)]
