@@ -280,14 +280,6 @@ int dispatch_agg(int elem, int agg, const Table& tb, const RunPlan& p, void* sta
 
 static inline size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-// one stream-ordered allocation for the call's scratch, released on every return path (asynchronously)
-struct AggScratch {
-    void* mem = nullptr;
-    ~AggScratch() {
-        if (mem) cudaFreeAsync(mem, ctx().stream);
-    }
-};
-
 static int aggregate_impl(vb_table* t, int agg, const int32_t* group_of_row, int ngroups, int64_t run_rows, void* out,
                    int64_t* out_counts, double* out_state, bool host) {
     const char* fn = host ? "vb_table_aggregate" : "vb_table_aggregate_dev";
@@ -351,15 +343,14 @@ static int aggregate_impl(vb_table* t, int agg, const int32_t* group_of_row, int
                   fn, total, list_bytes + group_bytes + tmp_bytes, run_state_bytes, stage_bytes, free_b);
         return VB_ENOMEM;
     }
-    AggScratch scratch;
-    if (cudaMallocAsync(&scratch.mem, total, c.stream) != cudaSuccess) {
-        cudaGetLastError();
-        scratch.mem = nullptr;
+    Scratch scratch;
+    void* mem;
+    if (scratch.own(total, &mem) != VB_OK) {
         set_error("%s: allocation of %zu bytes (row list and sort space %zu, run states %zu, staged results %zu) failed", fn, total,
                   list_bytes + group_bytes + tmp_bytes, run_state_bytes, stage_bytes);
         return VB_ENOMEM;
     }
-    uint8_t* cur = (uint8_t*)scratch.mem;
+    uint8_t* cur = (uint8_t*)mem;
     auto take = [&](size_t b) {
         uint8_t* r = cur;
         cur += al256(b);

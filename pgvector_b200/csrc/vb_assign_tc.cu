@@ -190,11 +190,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) assign_tc_kernel(TcArgs a) {
 
 // ----------------------------------------------------------------------------- host side
 
-enum { WST_A = 14, WST_B = 15, WST_N = 13, WST_F = 12 };
-
 static bool g_tc_enabled = true;
 
 int launch_assign_tc(const Table& X, int metric, const Table& Cn, int k, int32_t* out_idx) {
+    Scratch sc;
     Context& c = ctx();
     cudaStream_t s = c.stream;
     const int km = key_metric(metric);
@@ -208,17 +207,17 @@ int launch_assign_tc(const Table& X, int metric, const Table& Cn, int k, int32_t
     // centres: packed planes + norms
     const size_t b_bytes = (size_t)n_ntiles * n_kblocks * B_STAGE_BYTES;
     void *d_B, *d_norms, *d_A, *d_flag;
-    VB_TRY(workspace(WST_B, b_bytes, &d_B));
+    VB_TRY(sc.take(b_bytes, &d_B));
     const int64_t kpad = (int64_t)n_ntiles * TC_N;
     // slab of rows: a few tiles per SM
     const int64_t slab_tiles = (int64_t)c.sm_count * 4;
     const int64_t slab_rows = slab_tiles * TC_M;
     const size_t a_bytes = (size_t)slab_tiles * n_kblocks * A_STAGE_BYTES;
-    VB_TRY(workspace(WST_A, a_bytes, &d_A));
-    VB_TRY(workspace(WST_N, sizeof(float) * (size_t)(kpad + slab_rows) + 64, &d_norms));
+    VB_TRY(sc.take(a_bytes, &d_A));
+    VB_TRY(sc.take(sizeof(float) * (size_t)(kpad + slab_rows) + 64, &d_norms));
     float* d_cn = (float*)d_norms;
     float* d_xn = d_cn + kpad;
-    VB_TRY(workspace(WST_F, sizeof(int32_t) * (size_t)n + 64, &d_flag));
+    VB_TRY(sc.take(sizeof(int32_t) * (size_t)n + 64, &d_flag));
     int* d_nflag = (int*)d_flag;
     int32_t* d_flagged = (int32_t*)d_flag + 16;
     VB_CUDA(cudaMemsetAsync(d_nflag, 0, sizeof(int), s));

@@ -463,12 +463,13 @@ int recv_dev(int kind, int32_t typmod, int64_t n, const uint8_t* bytes, const in
     int hdr, per;
     field_shape(kind, &hdr, &per);
     {
-        DevBuf cnt;
-        VB_TRY(cnt.alloc(sizeof(int64_t) * (size_t)n));
-        if (n) bound_kernel<<<grid_for(n, 0), kThreads, 0, s>>>(off, n, hdr, per, static_cast<int64_t*>(cnt.p));
+        Scratch sc("type I/O");
+        void* cnt = nullptr;
+        VB_TRY(sc.own(sizeof(int64_t) * (size_t)n, &cnt));
+        if (n) bound_kernel<<<grid_for(n, 0), kThreads, 0, s>>>(off, n, hdr, per, static_cast<int64_t*>(cnt));
         VB_CUDA(cudaGetLastError());
         count_launch();
-        VB_TRY(offsets_from_counts(static_cast<int64_t*>(cnt.p), n, out_row_off));
+        VB_TRY(offsets_from_counts(static_cast<int64_t*>(cnt), n, out_row_off));
     }
     int64_t total = 0;
     VB_CUDA(cudaMemcpyAsync(&total, out_row_off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
@@ -478,9 +479,10 @@ int recv_dev(int kind, int32_t typmod, int64_t n, const uint8_t* bytes, const in
     if (n == 0) return VB_OK;
     VB_REQUIRE(kind == 2 ? (out_dim && (total == 0 || (out_idx && out_val))) : (total == 0 || out != nullptr),
                "%s: the outputs are required", fn);
-    DevBuf st;
-    VB_TRY(st.alloc(sizeof(Status)));
-    Status* sp = static_cast<Status*>(st.p);
+    Scratch sc("type I/O");
+    void* st = nullptr;
+    VB_TRY(sc.own(sizeof(Status), &st));
+    Status* sp = static_cast<Status*>(st);
     VB_TRY(recv_enqueue(kind, typmod, n, bytes, off, out_row_off, out, out_dim, out_idx, out_val,
                         (total * per / n + 15) / 16, sp));
     Status h;
@@ -531,14 +533,15 @@ int recv_host(int kind, int32_t typmod, int64_t n, const uint8_t* bytes, const i
     const size_t ne_al = (esz * (size_t)max_ne + 15) & ~(size_t)15;
     const size_t in_bytes = tb_al + sizeof(int64_t) * 2 * (size_t)(max_nr + 1);
     const size_t out_bytes = sizeof(Status) + dims_al + (size_t)planes * ne_al;
-    DevBuf dbytes[2], doff[2], dout[2], dst[2];
+    Scratch sc("type I/O");
+    void *dbytes[2] = {}, *doff[2] = {}, *dout[2] = {}, *dst[2] = {};
     for (int k = 0; k < 2 && k < nch; ++k) {
         VB_TRY(pinned_grow(&sg.in[k], &sg.in_bytes[k], in_bytes));
         VB_TRY(pinned_grow(&sg.out[k], &sg.out_bytes[k], out_bytes));
-        VB_TRY(dbytes[k].alloc((size_t)max_tb));
-        VB_TRY(doff[k].alloc(sizeof(int64_t) * 2 * (size_t)(max_nr + 1)));
-        VB_TRY(dout[k].alloc(dims_al + (size_t)planes * ne_al));
-        VB_TRY(dst[k].alloc(sizeof(Status)));
+        VB_TRY(sc.own((size_t)max_tb, &dbytes[k]));
+        VB_TRY(sc.own(sizeof(int64_t) * 2 * (size_t)(max_nr + 1), &doff[k]));
+        VB_TRY(sc.own(dims_al + (size_t)planes * ne_al, &dout[k]));
+        VB_TRY(sc.own(sizeof(Status), &dst[k]));
     }
     cudaStream_t s = ctx().stream;
     auto enqueue = [&](int64_t c, int k) -> int {
@@ -551,12 +554,12 @@ int recv_host(int kind, int32_t typmod, int64_t n, const uint8_t* bytes, const i
             poff[i] = off[r0 + i] - off[r0];
             poff[nr + 1 + i] = out_row_off[r0 + i] - out_row_off[r0];
         }
-        VB_CUDA(cudaMemcpyAsync(dbytes[k].p, pin, (size_t)tb, cudaMemcpyHostToDevice, s));
-        VB_CUDA(cudaMemcpyAsync(doff[k].p, poff, sizeof(int64_t) * 2 * (size_t)(nr + 1), cudaMemcpyHostToDevice, s));
-        const int64_t* doffp = static_cast<int64_t*>(doff[k].p);
-        uint8_t* o = static_cast<uint8_t*>(dout[k].p);
-        Status* sp = static_cast<Status*>(dst[k].p);
-        VB_TRY(recv_enqueue(kind, typmod, nr, static_cast<uint8_t*>(dbytes[k].p), doffp, doffp + nr + 1, o,
+        VB_CUDA(cudaMemcpyAsync(dbytes[k], pin, (size_t)tb, cudaMemcpyHostToDevice, s));
+        VB_CUDA(cudaMemcpyAsync(doff[k], poff, sizeof(int64_t) * 2 * (size_t)(nr + 1), cudaMemcpyHostToDevice, s));
+        const int64_t* doffp = static_cast<int64_t*>(doff[k]);
+        uint8_t* o = static_cast<uint8_t*>(dout[k]);
+        Status* sp = static_cast<Status*>(dst[k]);
+        VB_TRY(recv_enqueue(kind, typmod, nr, static_cast<uint8_t*>(dbytes[k]), doffp, doffp + nr + 1, o,
                             reinterpret_cast<int32_t*>(o), reinterpret_cast<int32_t*>(o + dims_al),
                             reinterpret_cast<float*>(o + dims_al + ne_al), (ne * per / nr + 15) / 16, sp));
         uint8_t* po = static_cast<uint8_t*>(sg.out[k]);
@@ -718,21 +721,22 @@ int vb_rows_to_binary_batch(int elem, int dim, const void* rows, int64_t n, int6
     const int64_t nch = (n + per - 1) / per;
     const int64_t max_nr = std::min(n, per);
     Staging& sg = staging();
-    DevBuf drows[2], dout[2], doff[2];
+    Scratch sc("type I/O");
+    void *drows[2] = {}, *dout[2] = {}, *doff[2] = {};
     for (int k = 0; k < 2 && k < nch; ++k) {
         VB_TRY(pinned_grow(&sg.in[k], &sg.in_bytes[k], (size_t)(max_nr * dim * esz)));
         VB_TRY(pinned_grow(&sg.out[k], &sg.out_bytes[k], (size_t)(max_nr * rb)));
-        VB_TRY(drows[k].alloc((size_t)(max_nr * dim * esz)));
-        VB_TRY(dout[k].alloc((size_t)(max_nr * rb)));
-        VB_TRY(doff[k].alloc(sizeof(int64_t) * (size_t)(max_nr + 1)));
+        VB_TRY(sc.own((size_t)(max_nr * dim * esz), &drows[k]));
+        VB_TRY(sc.own((size_t)(max_nr * rb), &dout[k]));
+        VB_TRY(sc.own(sizeof(int64_t) * (size_t)(max_nr + 1), &doff[k]));
     }
     cudaStream_t s = ctx().stream;
     auto enqueue = [&](int64_t c, int k) -> int {
         const int64_t r0 = c * per, nr = std::min(per, n - r0);
         std::memcpy(sg.in[k], static_cast<const uint8_t*>(rows) + r0 * dim * esz, (size_t)(nr * dim * esz));
-        VB_CUDA(cudaMemcpyAsync(drows[k].p, sg.in[k], (size_t)(nr * dim * esz), cudaMemcpyHostToDevice, s));
-        VB_TRY(send_dense_enqueue(elem, dim, drows[k].p, nr, static_cast<int64_t*>(doff[k].p), dout[k].p));
-        VB_CUDA(cudaMemcpyAsync(sg.out[k], dout[k].p, (size_t)(nr * rb), cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaMemcpyAsync(drows[k], sg.in[k], (size_t)(nr * dim * esz), cudaMemcpyHostToDevice, s));
+        VB_TRY(send_dense_enqueue(elem, dim, drows[k], nr, static_cast<int64_t*>(doff[k]), dout[k]));
+        VB_CUDA(cudaMemcpyAsync(sg.out[k], dout[k], (size_t)(nr * rb), cudaMemcpyDeviceToHost, s));
         return VB_OK;
     };
     auto finish = [&](int64_t c, int k) -> int {
@@ -777,25 +781,26 @@ int vb_sparsevec_to_binary_batch(int dim, int64_t n, const int64_t* row_off, con
         const int64_t r0 = cuts[c], r1 = cuts[c + 1], nr = r1 - r0;
         const int64_t e0 = row_off[r0], ne = row_off[r1] - e0;
         VB_REQUIRE(ne >= 0, "sparsevec_send: offsets must not decrease");
-        DevBuf droff, didx, dval, doff, dout;
-        VB_TRY(droff.alloc(sizeof(int64_t) * (size_t)(nr + 1)));
-        VB_TRY(didx.alloc(sizeof(int32_t) * (size_t)ne));
-        VB_TRY(dval.alloc(sizeof(float) * (size_t)ne));
-        VB_TRY(doff.alloc(sizeof(int64_t) * (size_t)(nr + 1)));
-        VB_TRY(dout.alloc((size_t)(12 * nr + 8 * ne)));
+        Scratch sc("type I/O");
+        void *droff = nullptr, *didx = nullptr, *dval = nullptr, *doff = nullptr, *dout = nullptr;
+        VB_TRY(sc.own(sizeof(int64_t) * (size_t)(nr + 1), &droff));
+        VB_TRY(sc.own(sizeof(int32_t) * (size_t)ne, &didx));
+        VB_TRY(sc.own(sizeof(float) * (size_t)ne, &dval));
+        VB_TRY(sc.own(sizeof(int64_t) * (size_t)(nr + 1), &doff));
+        VB_TRY(sc.own((size_t)(12 * nr + 8 * ne), &dout));
         std::vector<int64_t> ro((size_t)nr + 1);
         for (int64_t i = 0; i <= nr; ++i) ro[(size_t)i] = row_off[r0 + i] - e0;
-        VB_CUDA(cudaMemcpyAsync(droff.p, ro.data(), sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyHostToDevice, s));
-        if (ne) VB_CUDA(cudaMemcpyAsync(didx.p, idx + e0, sizeof(int32_t) * (size_t)ne, cudaMemcpyHostToDevice, s));
-        if (ne && write) VB_CUDA(cudaMemcpyAsync(dval.p, val + e0, sizeof(float) * (size_t)ne, cudaMemcpyHostToDevice, s));
-        VB_TRY(send_sparse_dev(dim, nr, static_cast<int64_t*>(droff.p), static_cast<int32_t*>(didx.p),
-                               static_cast<float*>(dval.p), INT64_MAX, static_cast<int64_t*>(doff.p),
-                               write ? dout.p : nullptr, "vb_sparsevec_to_binary_batch"));
+        VB_CUDA(cudaMemcpyAsync(droff, ro.data(), sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyHostToDevice, s));
+        if (ne) VB_CUDA(cudaMemcpyAsync(didx, idx + e0, sizeof(int32_t) * (size_t)ne, cudaMemcpyHostToDevice, s));
+        if (ne && write) VB_CUDA(cudaMemcpyAsync(dval, val + e0, sizeof(float) * (size_t)ne, cudaMemcpyHostToDevice, s));
+        VB_TRY(send_sparse_dev(dim, nr, static_cast<int64_t*>(droff), static_cast<int32_t*>(didx),
+                               static_cast<float*>(dval), INT64_MAX, static_cast<int64_t*>(doff),
+                               write ? dout : nullptr, "vb_sparsevec_to_binary_batch"));
         for (int64_t i = 1; i <= nr; ++i) out_off[r0 + i] = 12 * (r0 + i) + 8 * row_off[r0 + i];
         if (write) {
             void* pin;
             VB_TRY(pinned_buffer2((size_t)(12 * nr + 8 * ne) + 16, &pin));
-            VB_CUDA(cudaMemcpyAsync(pin, dout.p, (size_t)(12 * nr + 8 * ne), cudaMemcpyDeviceToHost, s));
+            VB_CUDA(cudaMemcpyAsync(pin, dout, (size_t)(12 * nr + 8 * ne), cudaMemcpyDeviceToHost, s));
             VB_CUDA(cudaStreamSynchronize(s));
             std::memcpy(static_cast<uint8_t*>(out) + out_off[r0], pin, (size_t)(12 * nr + 8 * ne));
         }

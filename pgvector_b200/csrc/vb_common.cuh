@@ -40,6 +40,7 @@ extern thread_local int g_last_status;
     } while (0)
 
 // ---------------------------------------------------------------- context
+struct Scratch;
 struct Context {
     bool inited = false;
     int device = -1;
@@ -48,7 +49,6 @@ struct Context {
     cudaStream_t copy_stream = nullptr;
     int64_t launches = 0;
     int slab_select = 1;               // selection from the filter's slab minima (0: full radix selection of every run)
-    uint64_t query_epoch = 0;          // bumped by every upload_queries(): caches keyed on a query image are valid for one batch only
     int tc_level1 = 1;                 // batched list scan: try the hi-plane-only filter first (vb_set_option "tc_level1")
     int tc_level0 = 1;                 // ... and in front of it the int8 filter, where tc_level1 is on (vb_set_option "tc_level0")
     int pp_filter = 1;                 // k-means++ on large fp32 sample tables: triangle-inequality + bf16 filters in front of the exact distances
@@ -59,9 +59,11 @@ struct Context {
     int hnsw_build_batch = 16384;      // ... and at most this many elements
     int hnsw_l2_persist = 1;           // HNSW scans: keep the visited tables in the persisting part of L2
     int64_t last_assign_flagged = -1;  // rows re-checked by the exact kernel in the last tensor-core assign (-1: exact path)
-    // grow-only device workspace arenas (index = slot)
-    void* ws[32] = {nullptr};
-    size_t ws_bytes[32] = {0};
+    // the grow-only scratch arena (Scratch)
+    uint8_t* arena = nullptr;
+    size_t arena_bytes = 0;
+    size_t arena_peak = 0;             // the most of it any call has needed
+    Scratch* scratch = nullptr;        // the innermost live Scratch
     // pinned staging
     void* pinned = nullptr;
     size_t pinned_bytes = 0;
@@ -70,8 +72,28 @@ struct Context {
 };
 Context& ctx();
 int require_init();
-// returns device pointer of at least `bytes` in slot (contents preserved only if not grown)
-int workspace(int slot, size_t bytes, void** out);
+
+// Device scratch of one library call.  Scratch objects nest like the calls that own them: take() hands out a
+// 256-byte-aligned range of the library's grow-only arena above everything the enclosing calls hold; own() a
+// one-off allocation for build-sized temporaries the library must not keep.  Both are released with the Scratch.
+// A function whose device pointers outlive its return takes its caller's Scratch; every other one opens its own.
+// Only the innermost live Scratch may take (anything else is refused with VB_ESTATE).  A range that does not fit the
+// arena is a one-off allocation, and the arena grows to the call's peak when the outermost Scratch closes, so a
+// repeated call allocates nothing.  fn (optional) names the call in the allocation errors.
+struct Scratch {
+    explicit Scratch(const char* fn = nullptr);
+    ~Scratch();
+    Scratch(const Scratch&) = delete;
+    Scratch& operator=(const Scratch&) = delete;
+    int take(size_t bytes, void** out);
+    int own(size_t bytes, void** out);
+
+  private:
+    const char* fn_;
+    Scratch* outer_;
+    size_t top_;                 // arena offset of the next range (past the arena's end: one-off allocations)
+    std::vector<void*> owned_;
+};
 int pinned_buffer(size_t bytes, void** out);
 int pinned_buffer2(size_t bytes, void** out);
 
@@ -142,7 +164,7 @@ int half_range_error(float v);
 
 // Pad + (for halfvec) widen queries into the fp32 query image the kernels read.
 // vector/halfvec: float[nq][qstride/4]; bit: bytes[nq][qstride]. host==true: `queries` is host memory.
-int upload_queries(int elem, int dim, const void* queries, int64_t nq, bool host, int ws_slot, void** out_dev, size_t* qstride);
+int upload_queries(Scratch& sc, int elem, int dim, const void* queries, int64_t nq, bool host, void** out_dev, size_t* qstride);
 
 // ---------------------------------------------------------------- scan primitives (vb_scan.cu)
 struct Chunk {           // one unit of scan work: a run of rows against one query
@@ -237,7 +259,7 @@ __host__ __device__ inline int64_t slab_cap(int64_t cap, int probes) { return (c
 __host__ __device__ inline int64_t slab_base(int64_t q, int64_t cap_s, int32_t cand_off, int p) {
     return q * cap_s + (cand_off >> 5) + 2 * p;
 }
-int build_query_groups(const int32_t* d_lists, int64_t nq, int probes, const int32_t* cand_off, int64_t cap, int n_lists, int gt_rows,
+int build_query_groups(Scratch& sc, const int32_t* d_lists, int64_t nq, int probes, const int32_t* cand_off, int64_t cap, int n_lists, int gt_rows,
                        QueryGroups* g, int64_t cap_s = 0);
 // tensor-core filter of the batched list scan (vb_list_tc.cu)
 struct ListUnit {
@@ -262,6 +284,10 @@ struct ListTcImage {
     bool l0_tried = false;       // the int8 plane was built or found not to fit
 };
 bool list_tc_supported(int elem, int key_metric, int k);
+// The per-query inputs of the filter's and the refine's error bounds for one batch of query images, owned by the batch so
+// that its probe selection and list scan compute |q|^2 once: *qn = a range of sc holding |q|^2 of the batch, with room for
+// what launch_list_tc adds at level 0 (t_q, eps(q)^2, per-row bound coefficients)
+int list_tc_query_norms(Scratch& sc, const void* qimg, size_t qstride, int64_t nq, float** qn);
 int list_tc_kp(int k, int level = 2);
 int list_tc_prepare(const Table& rows, ListTcImage* im);
 // the int8 plane, row scales and rmax of level 0 (rows must already be prepared)
@@ -278,7 +304,7 @@ bool list_tc_reserve(ListTcImage* im, int64_t nt, int64_t* cap_tiles, int64_t* c
 int list_tc_repack(const Table& rows, ListTcImage* im, int64_t first_tile, int64_t first_tile8, unsigned* d_stats);
 int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                    const int32_t* d_lists, int probes, const int32_t* cand_off, int64_t cap, const int64_t* d_list_off, int n_lists,
-                   float* out, const float** qn_out, bool one_list_all_queries = false, int level = 2, float* smin = nullptr,
+                   float* out, float* qn, bool one_list_all_queries = false, int level = 2, float* smin = nullptr,
                    int64_t cap_s = 0);
 // the k' nearest of every query's candidate run from the slab minima (same output as launch_segment_topk_v)
 int launch_slab_select(const float* dist, const float* smin, int64_t nq, int probes, const int32_t* probe_lists, const int32_t* cand_off,
@@ -293,7 +319,7 @@ int list_tc_level0_rescored(int64_t* out3);
 // per query.  The k' are selected in the kernel from the slab minima (smin), taken as selected (pre_pos / pre_key
 // [nq][kp], sorted, -1 padded: launch_slab_select / launch_segment_topk_v), or else selected in the kernel from the whole
 // run dist[q * cap ..) of seg_len[q] <= CR_RUN_MAX entries.  The number of uncertified queries is ADDED to *fail_dev
-// (level 0: and they are listed in fail_list).
+// (level 0: and they are listed in fail_list).  qn: the batch's bound inputs the filter used (list_tc_query_norms).
 constexpr int CR_RUN_MAX = 4096;
 // has_nan (vb_ivf_search_filtered): the runs were masked (FILTER_REJECTED marks rejected entries): marked candidates are
 // not candidates, and a query with an allowed NaN d~ (has_nan[q]) counts as uncertified.
@@ -384,8 +410,8 @@ struct FilterBatch {
     int64_t max_chunks = 0;
 };
 // The positions of the filters side by side: fbase [nfilters + 1] (host), *rows = the device array (a single filter is
-// read in place, several are copied into workspace slot ws_slot)
-int filter_concat_positions(const vb_filter* const* filters, int nfilters, int ws_slot, std::vector<int64_t>* fbase, const int64_t** rows);
+// read in place, several are copied into a range of sc)
+int filter_concat_positions(Scratch& sc, const vb_filter* const* filters, int nfilters, std::vector<int64_t>* fbase, const int64_t** rows);
 // The next sub-batch from query q0 on: as many queries as keep its distances under ~1 GiB (at least one), at most max_q.
 // A filter's queries get one block of chunks; each block gets a scan launch of its own once it fills grid_chunks chunks
 // (the whole grid then reads one filter's rows, which stay in L2 for its other queries), smaller blocks share one.
@@ -412,8 +438,8 @@ SparseCsr sparse_table_csr(const vb_sparse_table* h);
 uint64_t sparse_table_uid(const vb_sparse_table* h);
 // nq >= 1 sparse queries of a call on a table of dimension dim, checked with the sparse calls' rules and texts (CheckDims,
 // then the CSR: host variant on the host, device CSR by the one checked read-back) and on the device: host CSR uploaded
-// to the queries' workspace, device CSR used in place
-int sparse_queries_on_device(int dim, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, const float* q_val, bool host,
+// to a range of sc, device CSR used in place
+int sparse_queries_on_device(Scratch& sc, int dim, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, const float* q_val, bool host,
                              SparseCsr* out);
 
 int list_tile_rows();

@@ -39,9 +39,6 @@ uint64_t next_owner_uid() {
     return next.fetch_add(1);
 }
 
-// the slots of vb_exact_topk / vb_table_rerank: whole calls on the library stream that never overlap
-enum { WSF_QIMG = 0, WSF_DIST = 1, WSF_POSCAT = 2, WSF_QARGS = 3, WSF_CHUNKS = 4, WSF_POS = 6, WSF_OUT = 7 };
-
 constexpr int FILTER_MAX_K = 2048;   // as the re-rank: segment_topk_kernel selects without host-side segment sizes
 constexpr int FB_THREADS = 256;      // compaction: one bitset word per thread, 8192 rows per block
 
@@ -157,14 +154,6 @@ void filter_release(Filter* f) {
     f->bits = nullptr;
 }
 
-// Temporaries of a build: one allocation, freed before returning (construction is off the scan's hot path).
-struct FilterTmp {
-    void* mem = nullptr;
-    ~FilterTmp() {
-        if (mem) cudaFree(mem);
-    }
-};
-
 // bits (nwords words, set) -> f->pos / f->ids / f->off, f->n.  The buffers are sized by the count of set bits, read back
 // after the scan of the block sums: an IVFFlat image may hold one heap id on several rows, so the allowed rows are not
 // bounded by the number of ids given (only by the image's rows).
@@ -211,12 +200,13 @@ int filter_build_table(int64_t n_rows, const int64_t* rows, int64_t n, bool host
     Context& c = ctx();
     const int64_t nwords = (n_rows + 31) / 32;
     const int64_t nb = std::max<int64_t>(1, (nwords + FB_THREADS - 1) / FB_THREADS);
-    FilterTmp tmp;
+    Scratch sc("row filter");
+    void* tmp;
     const size_t bits_bytes = (4 * (size_t)std::max<int64_t>(nwords, 1) + 15) & ~(size_t)15;
     const size_t bytes = bits_bytes + 8 * ((size_t)nb + 1) + (host ? 8 * (size_t)n : 0);
-    VB_CUDA(cudaMalloc(&tmp.mem, bytes));
-    uint32_t* bits = (uint32_t*)tmp.mem;
-    int64_t* block_sum = (int64_t*)((uint8_t*)tmp.mem + bits_bytes);
+    VB_TRY(sc.own(bytes, &tmp));
+    uint32_t* bits = (uint32_t*)tmp;
+    int64_t* block_sum = (int64_t*)((uint8_t*)tmp + bits_bytes);
     const int64_t* d_rows = rows;
     if (host && n) {
         int64_t* up = block_sum + nb + 1;
@@ -241,12 +231,13 @@ int filter_build_ivf(int64_t n_rows, const int64_t* image_ids, const int64_t* li
     const int64_t nb = std::max<int64_t>(1, (nwords + FB_THREADS - 1) / FB_THREADS);
     size_t sort_bytes = 0;
     if (n) VB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, (const int64_t*)nullptr, (int64_t*)nullptr, (int)n, 0, 64, c.stream));
-    FilterTmp tmp;
+    Scratch sc("row filter");
+    void* tmp;
     const size_t bits_bytes = (4 * (size_t)std::max<int64_t>(nwords, 1) + 15) & ~(size_t)15;
     const size_t bytes = bits_bytes + 8 * ((size_t)nb + 1) + 8 * (size_t)n * (host ? 2 : 1) + sort_bytes + 256;
-    VB_CUDA(cudaMalloc(&tmp.mem, bytes));
-    uint32_t* bits = (uint32_t*)tmp.mem;
-    int64_t* block_sum = (int64_t*)((uint8_t*)tmp.mem + bits_bytes);
+    VB_TRY(sc.own(bytes, &tmp));
+    uint32_t* bits = (uint32_t*)tmp;
+    int64_t* block_sum = (int64_t*)((uint8_t*)tmp + bits_bytes);
     int64_t* sorted = block_sum + nb + 1;
     int64_t* up = sorted + n;
     void* sort_tmp = (void*)(((uintptr_t)(up + (host ? n : 0)) + 255) & ~(uintptr_t)255);
@@ -283,9 +274,10 @@ int filter_build_hnsw(int64_t n_elems, const int64_t* elems, int64_t n, bool hos
         return VB_ENOMEM;
     }
     f->bits = (uint32_t*)f->mem;
-    FilterTmp tmp;
-    VB_CUDA(cudaMalloc(&tmp.mem, 8 * ((size_t)nb + 1) + (host ? 8 * (size_t)n : 0)));
-    int64_t* block_sum = (int64_t*)tmp.mem;
+    Scratch sc("row filter");
+    void* tmp;
+    VB_TRY(sc.own(8 * ((size_t)nb + 1) + (host ? 8 * (size_t)n : 0), &tmp));
+    int64_t* block_sum = (int64_t*)tmp;
     const int64_t* d_elems = elems;
     if (host && n) {
         int64_t* up = block_sum + nb + 1;
@@ -341,14 +333,14 @@ int launch_filter_chunks(const FilterQuery* qa_dev, int64_t nq, int rows_per_chu
     return VB_OK;
 }
 
-int filter_concat_positions(const vb_filter* const* filters, int nfilters, int ws_slot, std::vector<int64_t>* fbase, const int64_t** rows) {
+int filter_concat_positions(Scratch& sc, const vb_filter* const* filters, int nfilters, std::vector<int64_t>* fbase, const int64_t** rows) {
     Context& cx = ctx();
     fbase->assign((size_t)nfilters + 1, 0);
     for (int i = 0; i < nfilters; ++i) (*fbase)[(size_t)i + 1] = (*fbase)[(size_t)i] + filters[i]->f.n;
     *rows = filters[0]->f.pos;
     if (nfilters > 1) {
         void* d_cat;
-        VB_TRY(workspace(ws_slot, 8 * (size_t)std::max<int64_t>(fbase->back(), 1), &d_cat));
+        VB_TRY(sc.take(8 * (size_t)std::max<int64_t>(fbase->back(), 1), &d_cat));
         for (int i = 0; i < nfilters; ++i)
             if (filters[i]->f.n)
                 VB_CUDA(cudaMemcpyAsync((int64_t*)d_cat + (*fbase)[(size_t)i], filters[i]->f.pos, 8 * (size_t)filters[i]->f.n,
@@ -428,9 +420,10 @@ static int exact_topk_filtered_impl(vb_table* t, int metric, const void* queries
     Context& cx = ctx();
     Table& T = t->t;
     // the filters' positions side by side (one device copy per filter; a single filter is read in place)
+    Scratch sc;
     std::vector<int64_t> fbase;
     const int64_t* rows;
-    VB_TRY(filter_concat_positions(filters, nfilters, WSF_POSCAT, &fbase, &rows));
+    VB_TRY(filter_concat_positions(sc, filters, nfilters, &fbase, &rows));
     const size_t rawq = raw_row_bytes(T.elem, T.dim);
     const int rpc = scan_chunk_rows(T);
     const int km = key_metric(metric);
@@ -440,6 +433,7 @@ static int exact_topk_filtered_impl(vb_table* t, int metric, const void* queries
     const int64_t grid_chunks = 8 * (int64_t)cx.sm_count;
     FilterBatch b;
     for (int64_t q0 = 0; q0 < nq;) {
+        Scratch batch;
         VB_TRY(filter_batch_plan(filters, nfilters, filter_of_query, fbase.data(), q0, nq, INT64_MAX, rpc, grid_chunks, &b));
         const std::vector<FilterQuery>& qa = b.qa;
         const std::vector<int64_t>& launch_begin = b.launch_begin;
@@ -447,22 +441,22 @@ static int exact_topk_filtered_impl(vb_table* t, int metric, const void* queries
         const int64_t m = (int64_t)qa.size(), run = b.run, max_chunks = b.max_chunks;
         void *qimg, *d_qa, *d_chunks, *d_dist, *d_pos;
         size_t qstride;
-        VB_TRY(upload_queries(T.elem, T.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, host, WSF_QIMG, &qimg, &qstride));
+        VB_TRY(upload_queries(batch, T.elem, T.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, host, &qimg, &qstride));
         const size_t qa_bytes = (sizeof(FilterQuery) * (size_t)m + 255) & ~(size_t)255;
         const size_t nl = launch_count.size();
-        VB_TRY(workspace(WSF_QARGS, qa_bytes + (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + sizeof(int32_t) * nl + 64, &d_qa));
+        VB_TRY(batch.take(qa_bytes + (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + sizeof(int32_t) * nl + 64, &d_qa));
         int64_t* seg_begin = (int64_t*)((uint8_t*)d_qa + qa_bytes);
         int32_t* seg_len = (int32_t*)(seg_begin + m);
         int32_t* d_count = seg_len + m;   // chunks of each scan launch
         VB_CUDA(cudaMemcpyAsync(d_qa, qa.data(), sizeof(FilterQuery) * (size_t)m, cudaMemcpyHostToDevice, cx.stream));
         if (nl) VB_CUDA(cudaMemcpyAsync(d_count, launch_count.data(), sizeof(int32_t) * nl, cudaMemcpyHostToDevice, cx.stream));
-        VB_TRY(workspace(WSF_CHUNKS, sizeof(Chunk) * (size_t)max_chunks + 64, &d_chunks));
+        VB_TRY(batch.take(sizeof(Chunk) * (size_t)max_chunks + 64, &d_chunks));
         VB_TRY(launch_filter_chunks((const FilterQuery*)d_qa, m, rpc, seg_begin, seg_len, (Chunk*)d_chunks));
-        VB_TRY(workspace(WSF_DIST, sizeof(float) * (size_t)std::max<int64_t>(run, 1), &d_dist));
+        VB_TRY(batch.take(sizeof(float) * (size_t)std::max<int64_t>(run, 1), &d_dist));
         for (size_t l = 0; l < nl; ++l)
             VB_TRY(launch_scan_gather(T, km, qimg, qstride, rows, (const Chunk*)d_chunks + launch_begin[l], d_count + l, launch_count[l],
                                       (float*)d_dist));
-        VB_TRY(workspace(WSF_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
+        VB_TRY(batch.take((sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
         int32_t* pos = (int32_t*)d_pos;
         float* key = (float*)(pos + (size_t)m * k);
         VB_TRY(launch_segment_topk_v((const float*)d_dist, seg_begin, seg_len, nullptr, nullptr, m, k, pos, key));
@@ -471,7 +465,7 @@ static int exact_topk_filtered_impl(vb_table* t, int metric, const void* queries
         double* o_d = nullptr;
         if (host) {
             void* d_out;
-            VB_TRY(workspace(WSF_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
+            VB_TRY(batch.take((sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
             o_ids = (int64_t*)d_out;
             o_d = (double*)(o_ids + (size_t)m * k);
         } else {

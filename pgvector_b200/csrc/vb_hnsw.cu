@@ -180,8 +180,6 @@ static int hnsw_launch(const Hnsw& h, const HnswDev& g, const void* qimg, size_t
     return VB_EINVAL;
 }
 
-enum { WSH_QIMG = 0, WSH_OUT = 7, WSH_FLAG = 12 };
-
 // The visited tables are the only data of a graph walk that is re-used (32 probes per expansion, every one a random
 // 32-byte sector); rows and neighbour lists stream past once.  Marking the tables' range persisting in L2 keeps the
 // probes out of DRAM.
@@ -215,6 +213,7 @@ static void hnsw_l2_window(cudaStream_t s, void* base, size_t bytes, bool on) {
 
 static int hnsw_search_impl(Hnsw& h, const void* queries, int64_t nq, int ef, int k, bool host, int64_t* out_ids, float* out_f,
                             double* out_d, int64_t* out_nd) {
+    Scratch sc;
     VB_REQUIRE(h.loaded, "hnsw index not loaded");
     VB_REQUIRE(ef >= 1 && ef <= 1000, "ef_search must be 1..1000 (src/hnsw.h:60-62)");
     VB_REQUIRE(k >= 1 && k <= ef, "k must be 1..ef_search");
@@ -246,7 +245,7 @@ static int hnsw_search_impl(Hnsw& h, const void* queries, int64_t nq, int ef, in
 
     void* qimg;
     size_t qstride;
-    VB_TRY(upload_queries(h.elem, h.dim, queries, nq, host, WSH_QIMG, &qimg, &qstride));
+    VB_TRY(upload_queries(sc, h.elem, h.dim, queries, nq, host, &qimg, &qstride));
 
     int64_t* d_ids = out_ids;
     float* d_f = out_f;
@@ -254,14 +253,14 @@ static int hnsw_search_impl(Hnsw& h, const void* queries, int64_t nq, int ef, in
     int64_t* d_nd = out_nd;
     if (host) {
         void* d_out;
-        VB_TRY(workspace(WSH_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)nq * k + sizeof(int64_t) * (size_t)nq, &d_out));
+        VB_TRY(sc.take((sizeof(int64_t) + sizeof(double)) * (size_t)nq * k + sizeof(int64_t) * (size_t)nq, &d_out));
         d_ids = (int64_t*)d_out;
         d_d = (double*)(d_ids + (size_t)nq * k);
         d_nd = (int64_t*)(d_d + (size_t)nq * k);
         d_f = nullptr;
     }
     void* d_flag;
-    VB_TRY(workspace(WSH_FLAG, 64, &d_flag));
+    VB_TRY(sc.take(64, &d_flag));
 
     // resident warps: a few CTAs per SM; every warp owns one visited table
     const int64_t want_ctas = (nq + HN_WARPS - 1) / HN_WARPS;

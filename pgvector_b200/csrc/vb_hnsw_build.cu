@@ -683,9 +683,6 @@ __global__ void fill_i32_kernel(int32_t* p, int64_t n, int32_t v) {
 
 // ----------------------------------------------------------------------------- host side
 
-enum { WSB_KEYS = 14, WSB_KEYS2 = 15, WSB_VALS = 16, WSB_VALS2 = 17, WSB_TMP = 18, WSB_FLAGS = 19, WSB_KEEP = 20 };
-enum { WSB_VSEL = 21, WSB_VOLD0 = 22, WSB_VOLDUP = 23, WSB_VSTAGE0 = 24, WSB_VSTAGEUP = 25 };
-
 struct BuildLaunch {
     int (*insert)(const BuildDev&, const VacDev&, uint32_t*, uint32_t, uint32_t, int, size_t, int*);
     int (*update)(const BuildDev&, const VacDev&, const uint64_t*, const float*, int, const InsertRec&, int, size_t, int*);
@@ -764,6 +761,7 @@ static double build_uniform(uint64_t* st) {   // (0, 1]: -log() stays finite
 }
 
 static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t n, int efc, uint64_t seed, const int32_t* levels_in) {
+    Scratch sc;
     VB_REQUIRE(efc >= 4 && efc <= 1000, "ef_construction must be 4..1000 (src/hnsw.h:57-59)");
     VB_REQUIRE(efc >= 2 * h.m, "ef_construction must be greater than or equal to 2 * m (src/hnswbuild.c:713-716)");
     VB_REQUIRE(n >= 0 && n < (int64_t)0x7fffffff, "bad row count");
@@ -857,7 +855,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
     const int max_grid_upd = c.sm_count * std::max(1, occ_upd) * 4;
 
     void* d_flags;
-    VB_TRY(workspace(WSB_FLAGS, 64, &d_flags));
+    VB_TRY(sc.take(64, &d_flags));
     b.n_edges = (int*)d_flags;
     b.overflow = b.n_edges + 1;
 
@@ -873,6 +871,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
     h.entry = 0;
     h.entry_level = levels[0];
     while (done < n) {
+        Scratch batch;
         int64_t B = std::min<int64_t>(std::min<int64_t>(b_max, std::max<int64_t>(1, done / frac)), n - done);
         // a batch ends at the first element that rises above the entry point: it becomes the entry point of the next batch
         int64_t promote = -1;
@@ -892,10 +891,10 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
         b.b0 = (int)done;
         b.B = (int)B;
         void *d_k1, *d_k2, *d_v1, *d_v2;
-        VB_TRY(workspace(WSB_KEYS, sizeof(uint64_t) * (size_t)max_edges, &d_k1));
-        VB_TRY(workspace(WSB_KEYS2, sizeof(uint64_t) * (size_t)max_edges, &d_k2));
-        VB_TRY(workspace(WSB_VALS, sizeof(float) * (size_t)max_edges, &d_v1));
-        VB_TRY(workspace(WSB_VALS2, sizeof(float) * (size_t)max_edges, &d_v2));
+        VB_TRY(batch.take(sizeof(uint64_t) * (size_t)max_edges, &d_k1));
+        VB_TRY(batch.take(sizeof(uint64_t) * (size_t)max_edges, &d_k2));
+        VB_TRY(batch.take(sizeof(float) * (size_t)max_edges, &d_v1));
+        VB_TRY(batch.take(sizeof(float) * (size_t)max_edges, &d_v2));
         b.edge_key = (uint64_t*)d_k1;
         b.edge_val = (float*)d_v1;
         const int grid_ins = (int)std::min<int64_t>((B + HN_WARPS - 1) / HN_WARPS, max_grid_ins);
@@ -934,8 +933,9 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
             size_t tmp_bytes = 0;
             VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1,
                                                     (float*)d_v2, n_edges, 0, 57, s));
+            Scratch sort;
             void* d_tmp;
-            VB_TRY(workspace(WSB_TMP, tmp_bytes, &d_tmp));
+            VB_TRY(sort.take(tmp_bytes, &d_tmp));
             VB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1,
                                                     (float*)d_v2, n_edges, 0, 57, s));
             count_launch();
@@ -996,6 +996,7 @@ static int hnsw_ensure_counts(Hnsw& h) {
 // the last record of each slot.  Everything the call needs is reserved before the first kernel.
 static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t n, int efc, uint64_t seed, const int32_t* levels_in,
                             int32_t* out_dup_of, int64_t* out_nchanges) {
+    Scratch sc;
     VB_REQUIRE(h.loaded, "hnsw index not loaded");
     VB_REQUIRE(efc >= 4 && efc <= 1000, "ef_construction must be 4..1000 (src/hnsw.h:57-59)");
     VB_REQUIRE(efc >= 2 * h.m, "ef_construction must be greater than or equal to 2 * m (src/hnswbuild.c:713-716)");
@@ -1080,12 +1081,13 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
         h.rec_cap = recs;
     }
     void *d_k1, *d_k2, *d_v1, *d_v2, *d_keep, *d_flags, *d_tmp;
-    VB_TRY(workspace(WSB_KEYS, sizeof(uint64_t) * (size_t)total_edges, &d_k1));
-    VB_TRY(workspace(WSB_KEYS2, sizeof(uint64_t) * (size_t)recs, &d_k2));
-    VB_TRY(workspace(WSB_VALS, sizeof(float) * (size_t)total_edges, &d_v1));
-    VB_TRY(workspace(WSB_VALS2, sizeof(float) * (size_t)recs, &d_v2));
-    VB_TRY(workspace(WSB_KEEP, (size_t)recs, &d_keep));
-    VB_TRY(workspace(WSB_FLAGS, 64, &d_flags));
+    VB_TRY(sc.take(sizeof(uint64_t) * (size_t)total_edges, &d_k1));
+    VB_TRY(sc.take(sizeof(uint64_t) * (size_t)recs, &d_k2));
+    VB_TRY(sc.take(sizeof(float) * (size_t)total_edges, &d_v1));
+    VB_TRY(sc.take(sizeof(float) * (size_t)recs, &d_v2));
+    VB_TRY(sc.take((size_t)recs, &d_keep));
+    VB_TRY(sc.take(64, &d_flags));
+    // one CUB temporary for every sort and select below, sized for their largest counts
     size_t tmp_bytes = 0;
     {
         size_t t1 = 0, t2 = 0, t3 = 0, t4 = 0;
@@ -1096,7 +1098,7 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
         VB_CUDA(cub::DeviceSelect::Flagged(nullptr, t3, (const uint64_t*)d_k2, (const uint8_t*)d_keep, h.rec_key, (int*)d_flags, (int)recs, s));
         VB_CUDA(cub::DeviceSelect::Flagged(nullptr, t4, (const int32_t*)d_v2, (const uint8_t*)d_keep, h.rec_val, (int*)d_flags, (int)recs, s));
         tmp_bytes = std::max(std::max(t1, t2), std::max(t3, t4));
-        VB_TRY(workspace(WSB_TMP, tmp_bytes, &d_tmp));
+        VB_TRY(sc.take(tmp_bytes, &d_tmp));
     }
     int occ_ins = 1, occ_upd = 1;
     VB_TRY(K.insert(BuildDev{}, VacDev{}, nullptr, 0, 0, 0, smem_ins, &occ_ins));
@@ -1207,10 +1209,7 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
         const int n_edges = flags[0];
         VB_REQUIRE(n_edges <= total_edges, "hnsw insert: record overflow (%d > %lld)", n_edges, (long long)total_edges);
         if (n_edges > 0) {
-            size_t tb = 0;
-            VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
-                                                    n_edges, 0, 57, s));
-            VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+            size_t tb = tmp_bytes;
             VB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
                                                     n_edges, 0, 57, s));
             count_launch();
@@ -1240,21 +1239,12 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
     VB_REQUIRE(n_rec <= recs, "hnsw insert: change record overflow (%d > %lld)", n_rec, (long long)recs);
     if (n_rec > 0) {
         int* d_nsel = b.n_edges + 3;
-        size_t tb = 0;
-        VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)h.rec_key, (uint64_t*)d_k2, (const int32_t*)h.rec_val,
-                                                (int32_t*)d_v2, n_rec, 0, 45, s));
-        VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+        size_t tb = tmp_bytes;
         VB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)h.rec_key, (uint64_t*)d_k2, (const int32_t*)h.rec_val,
                                                 (int32_t*)d_v2, n_rec, 0, 45, s));
         hnsw_last_of_key_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, s>>>((const uint64_t*)d_k2, n_rec, (uint8_t*)d_keep);
         VB_CUDA(cudaGetLastError());
-        tb = 0;
-        VB_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, (const uint64_t*)d_k2, (const uint8_t*)d_keep, h.rec_key, d_nsel, n_rec, s));
-        VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
         VB_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, (const uint64_t*)d_k2, (const uint8_t*)d_keep, h.rec_key, d_nsel, n_rec, s));
-        tb = 0;
-        VB_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, (const int32_t*)d_v2, (const uint8_t*)d_keep, h.rec_val, d_nsel, n_rec, s));
-        VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
         VB_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, (const int32_t*)d_v2, (const uint8_t*)d_keep, h.rec_val, d_nsel, n_rec, s));
         count_launch(4);
         VB_CUDA(cudaMemcpyAsync(&n_sel, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -1365,6 +1355,7 @@ __global__ void hnsw_slot_diff_kernel(HnswDev g, const int32_t* __restrict__ old
 // taken from the candidates in element order), MarkDeleted, then the change records as the diff against a snapshot of the
 // neighbour arrays.  Everything the call needs is reserved before the first kernel.
 static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* out_nrepaired, int64_t* out_nchanges) {
+    Scratch sc;
     VB_REQUIRE(h.loaded, "hnsw index not loaded");
     VB_REQUIRE(efc >= 4 && efc <= 1000, "ef_construction must be 4..1000 (src/hnsw.h:57-59)");
     VB_REQUIRE(efc >= 2 * h.m, "ef_construction must be greater than or equal to 2 * m (src/hnswbuild.c:713-716)");
@@ -1432,17 +1423,19 @@ static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* ou
         h.rec_cap = recs;
     }
     void *d_k1, *d_k2, *d_v1, *d_v2, *d_flags, *d_tmp, *d_need, *d_sel, *d_old0, *d_oldup, *d_stage0, *d_stageup;
-    VB_TRY(workspace(WSB_KEYS, sizeof(uint64_t) * (size_t)std::max<int64_t>(max_edges, 1), &d_k1));
-    VB_TRY(workspace(WSB_KEYS2, sizeof(uint64_t) * (size_t)std::max(max_edges, recs), &d_k2));
-    VB_TRY(workspace(WSB_VALS, sizeof(float) * (size_t)std::max<int64_t>(max_edges, 1), &d_v1));
-    VB_TRY(workspace(WSB_VALS2, sizeof(float) * (size_t)std::max(max_edges, recs), &d_v2));
-    VB_TRY(workspace(WSB_KEEP, (size_t)n, &d_need));
-    VB_TRY(workspace(WSB_FLAGS, 64, &d_flags));
-    VB_TRY(workspace(WSB_VSEL, sizeof(int32_t) * (size_t)(n + 1), &d_sel));
-    VB_TRY(workspace(WSB_VOLD0, sizeof(int32_t) * (size_t)n * lm0, &d_old0));
-    VB_TRY(workspace(WSB_VOLDUP, sizeof(int32_t) * (size_t)std::max<int64_t>(slots, 1) * m, &d_oldup));
-    VB_TRY(workspace(WSB_VSTAGE0, sizeof(int32_t) * (size_t)b_max * lm0, &d_stage0));
-    VB_TRY(workspace(WSB_VSTAGEUP, sizeof(int32_t) * (size_t)std::max<int64_t>(slots, 1) * m, &d_stageup));
+    VB_TRY(sc.take(sizeof(uint64_t) * (size_t)std::max<int64_t>(max_edges, 1), &d_k1));
+    VB_TRY(sc.take(sizeof(uint64_t) * (size_t)std::max(max_edges, recs), &d_k2));
+    VB_TRY(sc.take(sizeof(float) * (size_t)std::max<int64_t>(max_edges, 1), &d_v1));
+    VB_TRY(sc.take(sizeof(float) * (size_t)std::max(max_edges, recs), &d_v2));
+    VB_TRY(sc.take((size_t)n, &d_need));
+    VB_TRY(sc.take(64, &d_flags));
+    VB_TRY(sc.take(sizeof(int32_t) * (size_t)(n + 1), &d_sel));
+    VB_TRY(sc.take(sizeof(int32_t) * (size_t)n * lm0, &d_old0));
+    VB_TRY(sc.take(sizeof(int32_t) * (size_t)std::max<int64_t>(slots, 1) * m, &d_oldup));
+    VB_TRY(sc.take(sizeof(int32_t) * (size_t)b_max * lm0, &d_stage0));
+    VB_TRY(sc.take(sizeof(int32_t) * (size_t)std::max<int64_t>(slots, 1) * m, &d_stageup));
+    // one CUB temporary for every sort and select below, sized for their largest counts
+    size_t tmp_bytes = 0;
     {
         size_t t1 = 0, t2 = 0, t3 = 0;
         VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
@@ -1451,7 +1444,8 @@ static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* ou
                                                 45, s));
         VB_CUDA(cub::DeviceSelect::Flagged(nullptr, t3, cub::CountingInputIterator<int32_t>(0), (const uint8_t*)d_need, (int32_t*)d_sel,
                                            (int*)d_flags, (int)n, s));
-        VB_TRY(workspace(WSB_TMP, std::max(t1, std::max(t2, t3)), &d_tmp));
+        tmp_bytes = std::max(t1, std::max(t2, t3));
+        VB_TRY(sc.take(tmp_bytes, &d_tmp));
     }
     int occ_ins = 1, occ_glob = 1, occ_upd = 1;
     VB_TRY(K.insert(BuildDev{}, VacDev{}, nullptr, 0, 0, 0, smem_ins, &occ_ins));
@@ -1585,10 +1579,7 @@ static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* ou
         VB_CUDA(cudaStreamSynchronize(s));
         VB_REQUIRE(n_edges <= max_edges, "hnsw vacuum: record overflow (%d > %lld)", n_edges, (long long)max_edges);
         if (n_edges > 0) {
-            size_t tb = 0;
-            VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
-                                                    n_edges, 0, 57, s));
-            VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+            size_t tb = tmp_bytes;
             VB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)d_k1, (uint64_t*)d_k2, (const float*)d_v1, (float*)d_v2,
                                                     n_edges, 0, 57, s));
             count_launch();
@@ -1654,10 +1645,7 @@ static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* ou
         int64_t from = 0;
         while (h.entry >= 0 && from < n) {
             VB_TRY(needs(from, (int)h.entry));
-            size_t tb = 0;
-            VB_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, cub::CountingInputIterator<int32_t>((int32_t)from), (const uint8_t*)d_need,
-                                               (int32_t*)d_sel, d_nsel, (int)(n - from), s));
-            VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+            size_t tb = tmp_bytes;
             VB_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, cub::CountingInputIterator<int32_t>((int32_t)from), (const uint8_t*)d_need,
                                                (int32_t*)d_sel, d_nsel, (int)(n - from), s));
             count_launch();
@@ -1685,10 +1673,7 @@ static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* ou
         VB_CUDA(cudaMemcpyAsync(&n_rec, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, s));
         VB_CUDA(cudaStreamSynchronize(s));
         if (n_rec > 0) {
-            size_t tb = 0;
-            VB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)d_k2, h.rec_key, (const int32_t*)d_v2, h.rec_val, n_rec, 0, 45,
-                                                    s));
-            VB_TRY(workspace(WSB_TMP, tb, &d_tmp));
+            size_t tb = tmp_bytes;
             VB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)d_k2, h.rec_key, (const int32_t*)d_v2, h.rec_val, n_rec, 0, 45,
                                                     s));
             count_launch();

@@ -590,8 +590,9 @@ static int hnsw_scan_begin_impl(const char* fn, vb_hnsw* ix, const void* queries
                   (long long)nq, per_query, filters ? " plus the filters and carries" : "");
         return VB_ENOMEM;
     }
+    Scratch scratch;
     void* qimg;
-    int rc = upload_queries(h.elem, h.dim, queries, nq, true, 0, &qimg, &sc->qstride);
+    int rc = upload_queries(scratch, h.elem, h.dim, queries, nq, true, &qimg, &sc->qstride);
     if (rc != VB_OK) {
         delete sc;
         return rc;

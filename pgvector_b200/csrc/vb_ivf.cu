@@ -12,11 +12,6 @@
 
 namespace vb {
 
-// workspace slots
-enum { WS_QIMG = 0, WS_DIST = 1, WS_CDIST = 2, WS_PROBES = 3, WS_CHUNKS = 4, WS_SEG = 5, WS_POS = 6, WS_OUT = 7 };
-// 8..11 are used by the CUB sort path in vb_scan.cu
-enum { WS_MISC = 12, WS_OUT2 = 13, WS_SMIN = 31 };
-
 __global__ void regular_segments_kernel(int64_t nseg, int64_t stride, int32_t len, int64_t* begin, int32_t* lens) {
     int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i < nseg) {
@@ -346,12 +341,13 @@ static int ivf_ensure_centre_tc(Ivf& ix) {
     return VB_OK;
 }
 
-// probe selection for a batch of query images: d_probe_lists [nq x probes] ascending by (distance, list)
-static int ivf_select_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, int probes, int32_t** d_lists,
+// probe selection for a batch of query images: d_probe_lists [nq x probes] ascending by (distance, list), in sc.  *qn: the
+// batch's |q|^2 (list_tc_query_norms), computed here where the tensor-core filter first needs it
+static int ivf_select_probes(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride, int64_t nq, float** qn, int probes, int32_t** d_lists,
                              float** d_ldist) {
     Context& c = ctx();
     void *d_cdist, *d_seg, *d_probe;
-    VB_TRY(workspace(WS_CDIST, sizeof(float) * (size_t)nq * ix.lists, &d_cdist));
+    VB_TRY(sc.take(sizeof(float) * (size_t)nq * ix.lists, &d_cdist));
     // Query batches: the same tensor-core filter as the list scan, with the centre table as ONE list probed by every
     // query -- approximate distances to all centres, the k' nearest re-scored exactly, order (distance, list number)
     // certified; any uncertified query sends the batch through the exact tiles below.
@@ -369,13 +365,13 @@ static int ivf_select_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t 
     if (tc) {
         const int kp = list_tc_kp(probes);
         void *d_pairs, *d_seg2, *d_probe2;
-        VB_TRY(workspace(WS_MISC, sizeof(int32_t) * (size_t)nq * 3 + 64, &d_pairs));
+        VB_TRY(sc.take(sizeof(int32_t) * (size_t)nq * 3 + 64, &d_pairs));
         int32_t* zero_lists = (int32_t*)d_pairs;
         int32_t* pair_off = zero_lists + nq;
-        VB_TRY(workspace(WS_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)nq * 2 + 64, &d_seg2));
+        VB_TRY(sc.take((sizeof(int64_t) + sizeof(int32_t)) * (size_t)nq * 2 + 64, &d_seg2));
         int64_t* sb = (int64_t*)d_seg2;
         int32_t* sl = (int32_t*)(sb + nq);
-        VB_TRY(workspace(WS_PROBES, (sizeof(int32_t) + sizeof(float)) * (size_t)nq * (probes + kp), &d_probe2));
+        VB_TRY(sc.take((sizeof(int32_t) + sizeof(float)) * (size_t)nq * (probes + kp), &d_probe2));
         int32_t* lists = (int32_t*)d_probe2;
         float* ldist = (float*)(lists + (size_t)nq * probes);
         int32_t* pos_kp = (int32_t*)(ldist + (size_t)nq * probes);
@@ -385,9 +381,9 @@ static int ivf_select_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t 
         regular_segments_kernel<<<(unsigned)((nq + 255) / 256), 256, 0, c.stream>>>(nq, ix.lists, ix.lists, sb, sl);
         VB_CUDA(cudaGetLastError());
         count_launch(2);
-        const float* qn = nullptr;
+        if (!*qn) VB_TRY(list_tc_query_norms(sc, qimg, qstride, nq, qn));
         VB_TRY(launch_list_tc(ix.centers, ix.ctc, km, qimg, qstride, nq, zero_lists, 1, pair_off, ix.lists, ix.d_centre_off, 1,
-                              (float*)d_cdist, &qn, true));
+                              (float*)d_cdist, *qn, true));
         int n_failed = 0;
         if (!ix.defer_tc_check) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, sizeof(int), c.stream));
         // a run of at most CR_RUN_MAX centre distances is selected inside the refine kernel, a longer one by a launch of its own
@@ -395,7 +391,7 @@ static int ivf_select_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t 
         if (pre) VB_TRY(launch_segment_topk_v((const float*)d_cdist, sb, sl, nullptr, nullptr, nq, kp, pos_kp, key_kp));
         VB_TRY(launch_list_tc_cta_refine(ix.centers, ix.ctc, km, qimg, qstride, nq, probes, kp, 1, zero_lists, pair_off, ix.d_centre_off,
                                          (const float*)d_cdist, nullptr, pre ? pos_kp : nullptr, pre ? key_kp : nullptr, ix.lists, 0, sl,
-                                         qn, lists, ldist, ix.d_tc_fail, 2));
+                                         *qn, lists, ldist, ix.d_tc_fail, 2));
         if (!ix.defer_tc_check) {
             VB_CUDA(cudaMemcpyAsync(&n_failed, ix.d_tc_fail, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
             VB_CUDA(cudaStreamSynchronize(c.stream));
@@ -426,13 +422,13 @@ static int ivf_select_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t 
         VB_TRY(launch_scan_regular(ix.centers, key_metric(ix.metric), qimg, qstride, nq, ix.lists, (float*)d_cdist, ix.lists));
     }
     prof_end(VB_PROF_SCAN_LISTS);
-    VB_TRY(workspace(WS_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)nq * 2 + 64, &d_seg));
+    VB_TRY(sc.take((sizeof(int64_t) + sizeof(int32_t)) * (size_t)nq * 2 + 64, &d_seg));
     int64_t* seg_begin = (int64_t*)d_seg;
     int32_t* seg_len = (int32_t*)(seg_begin + nq);
     regular_segments_kernel<<<(unsigned)((nq + 255) / 256), 256, 0, c.stream>>>(nq, ix.lists, ix.lists, seg_begin, seg_len);
     VB_CUDA(cudaGetLastError());
     count_launch();
-    VB_TRY(workspace(WS_PROBES, (sizeof(int32_t) + sizeof(float)) * (size_t)nq * probes, &d_probe));
+    VB_TRY(sc.take((sizeof(int32_t) + sizeof(float)) * (size_t)nq * probes, &d_probe));
     int32_t* lists = (int32_t*)d_probe;
     float* ldist = (float*)(lists + (size_t)nq * probes);
     std::vector<int64_t> hb;
@@ -502,8 +498,8 @@ static int ivf_ensure_l0_image(Ivf& ix) {
 }
 
 // scan the given probe lists for a batch of queries and keep the k nearest per query (mask: of the rows each query's
-// row filter allows)
-static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, const int32_t* d_lists, int probes, int k,
+// row filter allows); *cand_total_dev is in sc, *qn as in ivf_select_probes
+static int ivf_scan_topk(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride, int64_t nq, float** qn, const int32_t* d_lists, int probes, int k,
                          int64_t* out_ids_dev, float* out_f_dev, double* out_d_dev, int32_t** cand_total_dev, const IvfMask* mask = nullptr) {
     Context& c = ctx();
     const int rpc = scan_chunk_rows(ix.rows);
@@ -511,11 +507,10 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
     const int64_t max_chunks = nq * (cap / rpc + probes + 1);
     VB_REQUIRE(max_chunks < (int64_t)INT32_MAX, "too many scan chunks (%lld)", (long long)max_chunks);
     void *d_chunks, *d_seg, *d_dist, *d_pos;
-    VB_TRY(workspace(WS_CHUNKS, sizeof(Chunk) * (size_t)max_chunks + sizeof(int32_t) * (size_t)nq * (probes + 1) + 64, &d_chunks));
+    VB_TRY(sc.take(sizeof(Chunk) * (size_t)max_chunks + sizeof(int32_t) * (size_t)nq * (probes + 1) + 64, &d_chunks));
     Chunk* chunks = (Chunk*)d_chunks;
     int32_t* cand_off = (int32_t*)(chunks + max_chunks);
-    VB_TRY(workspace(WS_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)nq * 2 + 64, &d_seg));
-    // second half of WS_SEG (first half may still hold the probe-selection segments)
+    VB_TRY(sc.take((sizeof(int64_t) + sizeof(int32_t)) * (size_t)nq * 2 + 64, &d_seg));
     int64_t* seg_begin = (int64_t*)d_seg;
     int32_t* seg_len = (int32_t*)(seg_begin + nq);
     int* n_chunks = (int*)(seg_len + nq);
@@ -532,7 +527,7 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
                                                                                       ix.d_cand_sum, nullptr);
     VB_CUDA(cudaGetLastError());
     count_launch();
-    VB_TRY(workspace(WS_DIST, sizeof(float) * (size_t)nq * cap, &d_dist));
+    VB_TRY(sc.take(sizeof(float) * (size_t)nq * cap, &d_dist));
     prof_begin(VB_PROF_SCAN_ITEMS);
     // scan_impl: 0 = per-query LDG scan, 1 = per-query bulk-copy scan, 2 = automatic, 3 = list-major fp32 wherever it
     // applies, 4 = tensor-core filter + exact re-score wherever it applies.
@@ -578,17 +573,17 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
         ix.last_list_level = level;
         ix.last_level0 = level == 0;
         const int kp = list_tc_kp(k, level);
-        const float* qn = nullptr;
         const bool slabs = slabs_fit && kp <= 128;
         void* d_smin = nullptr;
-        if (slabs) VB_TRY(workspace(WS_SMIN, sizeof(float) * (size_t)nq * cap_s, &d_smin));
+        if (slabs) VB_TRY(sc.take(sizeof(float) * (size_t)nq * cap_s, &d_smin));
+        if (!*qn) VB_TRY(list_tc_query_norms(sc, qimg, qstride, nq, qn));
         VB_TRY(launch_list_tc(ix.rows, ix.tc, km, qimg, qstride, nq, d_lists, probes, cand_off, cap, ix.d_list_off, ix.lists,
-                              (float*)d_dist, &qn, false, level, (float*)d_smin, cap_s));
+                              (float*)d_dist, *qn, false, level, (float*)d_smin, cap_s));
         prof_end(VB_PROF_SCAN_ITEMS);
         if (mask)
             VB_TRY(ivf_mask_runs(*mask, nq, d_lists, probes, cand_off, ix.d_list_off, cap, (float*)d_dist, (float*)d_smin, cap_s));
         const int32_t* has_nan = mask ? mask->has_nan : nullptr;
-        VB_TRY(workspace(WS_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)nq * (k + kp), &d_pos));
+        VB_TRY(sc.take((sizeof(int32_t) + sizeof(float)) * (size_t)nq * (k + kp), &d_pos));
         int32_t* pos = (int32_t*)d_pos;
         float* key = (float*)(pos + (size_t)nq * k);
         int32_t* pos_kp = (int32_t*)(key + (size_t)nq * k);
@@ -604,7 +599,7 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
             // one CTA per query: slab selection, re-score on eight warps, ranking, certificate (a selection that overflows
             // counts as uncertified: the repeat of the batch selects below)
             VB_TRY(launch_list_tc_cta_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
-                                             (const float*)d_dist, (const float*)d_smin, nullptr, nullptr, cap, cap_s, seg_len, qn, pos, key,
+                                             (const float*)d_dist, (const float*)d_smin, nullptr, nullptr, cap, cap_s, seg_len, *qn, pos, key,
                                              ix.d_tc_fail + 1, level, level == 0 ? ix.d_l0_fail : nullptr, has_nan));
         } else {
             // the k' selected by a launch of their own (slab_select_kernel hands what overflows it to the full selection)
@@ -614,7 +609,7 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
             else
                 VB_TRY(launch_segment_topk_v((const float*)d_dist, seg_begin, seg_len, nullptr, nullptr, nq, kp, pos_kp, key_kp));
             VB_TRY(launch_list_tc_cta_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
-                                             (const float*)d_dist, nullptr, pos_kp, key_kp, cap, cap_s, seg_len, qn, pos, key,
+                                             (const float*)d_dist, nullptr, pos_kp, key_kp, cap, cap_s, seg_len, *qn, pos, key,
                                              ix.d_tc_fail + 1, level, nullptr, has_nan));
         }
         if (!ix.defer_tc_check) {
@@ -648,7 +643,7 @@ static int ivf_scan_topk(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
     }
     prof_end(VB_PROF_SCAN_ITEMS);
     if (mask) VB_TRY(ivf_mask_runs(*mask, nq, d_lists, probes, cand_off, ix.d_list_off, cap, (float*)d_dist, nullptr, 0));
-    VB_TRY(workspace(WS_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)nq * k, &d_pos));
+    VB_TRY(sc.take((sizeof(int32_t) + sizeof(float)) * (size_t)nq * k, &d_pos));
     int32_t* pos = (int32_t*)d_pos;
     float* key = (float*)(pos + (size_t)nq * k);
     std::vector<int64_t> hb;
@@ -765,11 +760,11 @@ static bool ivf_one_applies(const Ivf& ix, int64_t nq, int probes, int64_t k, in
     return one_probe_fits(ix.lists, qs, probes) && one_scan_fits(one_cap(cap), qs, probes, k);
 }
 
-// GetScanLists for nq <= ONE_MAX_Q query images: one launch
-static int ivf_one_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, int probes, int32_t** d_lists, float** d_ldist) {
+// GetScanLists for nq <= ONE_MAX_Q query images: one launch (the lists in sc)
+static int ivf_one_probes(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride, int64_t nq, int probes, int32_t** d_lists, float** d_ldist) {
     void *d_cdist, *d_probe;
-    VB_TRY(workspace(WS_CDIST, sizeof(float) * (size_t)nq * ix.lists, &d_cdist));
-    VB_TRY(workspace(WS_PROBES, (sizeof(int32_t) + sizeof(float)) * (size_t)nq * probes, &d_probe));
+    VB_TRY(sc.take(sizeof(float) * (size_t)nq * ix.lists, &d_cdist));
+    VB_TRY(sc.take((sizeof(int32_t) + sizeof(float)) * (size_t)nq * probes, &d_probe));
     int32_t* lists = (int32_t*)d_probe;
     float* ldist = (float*)(lists + (size_t)nq * probes);
     unsigned *tp, *ts;
@@ -787,8 +782,9 @@ static int ivf_one_probes(Ivf& ix, const void* qimg, size_t qstride, int64_t nq,
 static int ivf_one_items(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, const int32_t* d_lists, int probes, int k, int64_t cap,
                          int64_t* out_ids_dev, float* out_f_dev, double* out_d_dev, bool cand_store) {
     cap = one_cap(cap);
+    Scratch sc;
     void* d_dist;
-    VB_TRY(workspace(WS_DIST, sizeof(float) * (size_t)nq * cap, &d_dist));
+    VB_TRY(sc.take(sizeof(float) * (size_t)nq * cap, &d_dist));
     unsigned *tp, *ts;
     VB_TRY(ivf_tickets(ix, &tp, &ts));
     if (!ix.d_cand_sum) VB_CUDA(cudaMalloc(&ix.d_cand_sum, sizeof(int64_t)));
@@ -799,7 +795,7 @@ static int ivf_one_items(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
     return VB_OK;
 }
 
-// results of a fused scan to host memory: ONE copy (ids and float8 distances are adjacent in the workspace) into the pinned
+// results of a fused scan to host memory: ONE copy (ids and float8 distances are adjacent in the scratch) into the pinned
 // staging buffer, one synchronisation
 static int ivf_one_fetch(const void* d_out, int64_t n, int64_t* out_ids, double* out_d) {
     void* pin;
@@ -821,7 +817,7 @@ struct vb_ivf {
 };
 
 // ivfflat.iterative_scan for a batch of queries (vb_ivf_iter.cu).  Everything kept between calls lives in `mem`, one
-// allocation the handle owns: the shared workspaces only carry data within a call.
+// allocation the handle owns: scratch only carries data within a call.
 struct vb_ivf_scan {
     Ivf* ix = nullptr;
     uint64_t generation = 0;   // ix->generation at begin
@@ -919,18 +915,20 @@ static int ivf_scan_setup(vb_ivf_scan& s, const void* queries) {
     const int64_t bq = std::min<int64_t>(s.nq, 65535);
     for (int64_t q0 = 0; q0 < s.nq; q0 += bq) {
         const int64_t m = std::min(bq, s.nq - q0);
+        Scratch sc;
         void* qimg;
         size_t qstride;
-        VB_TRY(upload_queries(ix.elem, ix.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, true, WS_QIMG, &qimg, &qstride));
+        VB_TRY(upload_queries(sc, ix.elem, ix.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, true, &qimg, &qstride));
         VB_REQUIRE(qstride == s.qstride, "query image stride %zu, expected %zu", qstride, s.qstride);
         uint8_t* mine = s.qimg + (size_t)q0 * s.qstride;
         VB_CUDA(cudaMemcpyAsync(mine, qimg, (size_t)m * s.qstride, cudaMemcpyDeviceToDevice, c.stream));
         int32_t* d_lists;
         float* d_ldist;
+        float* qn = nullptr;
         if (c.one_query && m <= ONE_MAX_Q && one_probe_fits(ix.lists, s.qstride, s.max_probes))
-            VB_TRY(ivf_one_probes(ix, mine, s.qstride, m, s.max_probes, &d_lists, &d_ldist));
+            VB_TRY(ivf_one_probes(sc, ix, mine, s.qstride, m, s.max_probes, &d_lists, &d_ldist));
         else
-            VB_TRY(ivf_select_probes(ix, mine, s.qstride, m, s.max_probes, &d_lists, &d_ldist));
+            VB_TRY(ivf_select_probes(sc, ix, mine, s.qstride, m, &qn, s.max_probes, &d_lists, &d_ldist));
         VB_CUDA(cudaMemcpyAsync(s.probe + (size_t)q0 * s.max_probes, d_lists, sizeof(int32_t) * (size_t)m * s.max_probes,
                                 cudaMemcpyDeviceToDevice, c.stream));
     }
@@ -973,11 +971,12 @@ int vb_distance_batch(int elem, int metric, int dim, const void* q, const void* 
         table_free(t);
         return rc;
     }
+    Scratch sc;
     void* qimg;
     size_t qstride;
     void* d_out;
-    rc = upload_queries(elem, dim, q, 1, true, WS_QIMG, &qimg, &qstride);
-    if (rc == VB_OK) rc = workspace(WS_OUT, sizeof(double) * (size_t)n, &d_out);
+    rc = upload_queries(sc, elem, dim, q, 1, true, &qimg, &qstride);
+    if (rc == VB_OK) rc = sc.take(sizeof(double) * (size_t)n, &d_out);
     if (rc == VB_OK) rc = launch_scan_regular_f64(t, key_metric(metric), qimg, qstride, 1, n, (double*)d_out, n);
     if (rc == VB_OK) {
         cudaError_t e = cudaMemcpyAsync(out, d_out, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, c.stream);
@@ -1055,11 +1054,12 @@ static int exact_topk_impl(vb_table* t, int metric, const void* queries, int64_t
     // sub-batch so the distance matrix stays under ~1 GiB
     int64_t bq = std::max<int64_t>(1, std::min<int64_t>(nq, (int64_t)(1ull << 30) / (4 * std::max<int64_t>(n, 1))));
     for (int64_t q0 = 0; q0 < nq; q0 += bq) {
+        Scratch sc;
         int64_t m = std::min(bq, nq - q0);
         void *qimg, *d_dist, *d_seg, *d_pos, *d_ids, *d_of;
         size_t qstride;
-        VB_TRY(upload_queries(T.elem, T.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, host, WS_QIMG, &qimg, &qstride));
-        VB_TRY(workspace(WS_DIST, sizeof(float) * (size_t)m * std::max<int64_t>(n, 1), &d_dist));
+        VB_TRY(upload_queries(sc, T.elem, T.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, host, &qimg, &qstride));
+        VB_TRY(sc.take(sizeof(float) * (size_t)m * std::max<int64_t>(n, 1), &d_dist));
         // A batch of queries against the whole table is a distance matrix: tile it (table rows read once per 128
         // queries instead of once per query) when the query image has the table's row layout.  One query at a
         // time, or a metric with a per-row epilogue, streams the table through the scan kernel instead.
@@ -1077,13 +1077,13 @@ static int exact_topk_impl(vb_table* t, int metric, const void* queries, int64_t
         } else {
             VB_TRY(launch_scan_regular(T, km, qimg, qstride, m, n, (float*)d_dist, n));
         }
-        VB_TRY(workspace(WS_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
+        VB_TRY(sc.take((sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
         int64_t* seg_begin = (int64_t*)d_seg;
         int32_t* seg_len = (int32_t*)(seg_begin + m);
         regular_segments_kernel<<<(unsigned)((m + 255) / 256), 256, 0, c.stream>>>(m, n, (int32_t)n, seg_begin, seg_len);
         VB_CUDA(cudaGetLastError());
         count_launch();
-        VB_TRY(workspace(WS_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
+        VB_TRY(sc.take((sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
         int32_t* pos = (int32_t*)d_pos;
         float* key = (float*)(pos + (size_t)m * k);
         std::vector<int64_t> hb;
@@ -1099,7 +1099,7 @@ static int exact_topk_impl(vb_table* t, int metric, const void* queries, int64_t
         float* o_f = nullptr;
         double* o_d = nullptr;
         if (host) {
-            VB_TRY(workspace(WS_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_ids));
+            VB_TRY(sc.take((sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_ids));
             o_ids = (int64_t*)d_ids;
             o_d = (double*)(o_ids + (size_t)m * k);
         } else {
@@ -1425,20 +1425,22 @@ static int ivf_insert_lists(Ivf& ix, const void* rows, int64_t n, bool host, int
     const int64_t bq = 65535;
     std::vector<float> d0;
     for (int64_t q0 = 0; q0 < n; q0 += bq) {
+        Scratch sc;
         const int64_t m = std::min(bq, n - q0);
         void* qimg;
         size_t qstride;
-        VB_TRY(upload_queries(ix.elem, ix.dim, (const uint8_t*)rows + (size_t)q0 * raw, m, host, WS_QIMG, &qimg, &qstride));
+        VB_TRY(upload_queries(sc, ix.elem, ix.dim, (const uint8_t*)rows + (size_t)q0 * raw, m, host, &qimg, &qstride));
         int32_t* d_lists;
         float* d_ldist;
+        float* qn = nullptr;
         if (c.one_query && m <= ONE_MAX_Q && one_probe_fits(ix.lists, qstride, 1))
-            VB_TRY(ivf_one_probes(ix, qimg, qstride, m, 1, &d_lists, &d_ldist));
+            VB_TRY(ivf_one_probes(sc, ix, qimg, qstride, m, 1, &d_lists, &d_ldist));
         else
-            VB_TRY(ivf_select_probes(ix, qimg, qstride, m, 1, &d_lists, &d_ldist));
+            VB_TRY(ivf_select_probes(sc, ix, qimg, qstride, m, &qn, 1, &d_lists, &d_ldist));
         VB_CUDA(cudaMemcpyAsync(out + q0, d_lists, sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c.stream));
         if (ix.elem != VB_BIT) {   // (Hamming distances are never NaN)
             void* d_d0;
-            VB_TRY(workspace(WS_DIST, sizeof(float) * (size_t)m, &d_d0));
+            VB_TRY(sc.take(sizeof(float) * (size_t)m, &d_d0));
             VB_TRY(launch_scan_regular(ix.centers, key_metric(ix.metric), qimg, qstride, m, 1, (float*)d_d0, 1));
             d0.resize((size_t)m);
             VB_CUDA(cudaMemcpyAsync(d0.data(), d_d0, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c.stream));
@@ -1447,27 +1449,6 @@ static int ivf_insert_lists(Ivf& ix, const void* rows, int64_t n, bool host, int
         if (ix.elem != VB_BIT)
             for (int64_t i = 0; i < m; ++i)
                 if (std::isnan(d0[(size_t)i])) out[q0 + i] = 0;
-    }
-    return VB_OK;
-}
-
-// Temporaries of one insert or delete: one device allocation, freed on every exit
-struct IvfTmp {
-    void* mem = nullptr;
-    ~IvfTmp() {
-        if (mem) {
-            cudaStreamSynchronize(ctx().stream);
-            cudaFree(mem);
-        }
-    }
-};
-
-static int ivf_alloc_tmp(const char* fn, IvfTmp& tmp, size_t bytes) {
-    if (cudaMalloc(&tmp.mem, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        tmp.mem = nullptr;
-        set_error("%s: allocation of %zu bytes of device memory failed", fn, bytes);
-        return VB_ENOMEM;
     }
     return VB_OK;
 }
@@ -1561,9 +1542,10 @@ static int ivf_insert_impl(const char* fn, vb_ivf* h, const void* rows, const in
         ix.d_ids = nid;
         ix.ids_cap = ix.rows.cap;
     }
-    IvfTmp tmp;
-    VB_TRY(ivf_alloc_tmp(fn, tmp, tmp_bytes));
-    uint8_t* p = (uint8_t*)tmp.mem;
+    Scratch sc(fn);
+    void* tmp;
+    VB_TRY(sc.own(tmp_bytes, &tmp));
+    uint8_t* p = (uint8_t*)tmp;
     auto take = [&](size_t b) {
         uint8_t* q = p;
         p += align256(b);
@@ -1653,10 +1635,11 @@ int vb_ivf_delete(vb_ivf* h, const int64_t* ids, int64_t n, int64_t* out_removed
     const int64_t suffix = n_old - first;
     const size_t stride = ix.rows.stride;
     const int64_t window = std::max<int64_t>(1, std::min<int64_t>(suffix, (int64_t)(IVF_MOVE_WINDOW_BYTES / stride)));
-    IvfTmp tmp;
-    VB_TRY(ivf_alloc_tmp(fn, tmp, align256(8 * (size_t)suffix) + align256(16) + align256((size_t)window * stride) + align256(8 * (size_t)window)));
-    int64_t* d_dst = (int64_t*)tmp.mem;
-    unsigned* d_stats = (unsigned*)((uint8_t*)tmp.mem + align256(8 * (size_t)suffix));
+    Scratch sc(fn);
+    void* tmp;
+    VB_TRY(sc.own(align256(8 * (size_t)suffix) + align256(16) + align256((size_t)window * stride) + align256(8 * (size_t)window), &tmp));
+    int64_t* d_dst = (int64_t*)tmp;
+    unsigned* d_stats = (unsigned*)((uint8_t*)tmp + align256(8 * (size_t)suffix));
     uint8_t* stage = (uint8_t*)d_stats + align256(16);
     int64_t* stage_ids = (int64_t*)(stage + align256((size_t)window * stride));
     ++ix.generation;
@@ -1708,7 +1691,7 @@ struct IvfBuildSource {
     bool host;
     int64_t chunk;
     void* pin[2] = {nullptr, nullptr};
-    IvfTmp dev[2];
+    void* dev[2] = {nullptr, nullptr};   // owned by the caller's Scratch, released after the destructor drained the copy stream
     cudaEvent_t copied[2] = {nullptr, nullptr}, done[2] = {nullptr, nullptr};
     bool rows_pinned = false;
     ~IvfBuildSource() {
@@ -1720,13 +1703,14 @@ struct IvfBuildSource {
     }
     size_t ids_at() const { return align256((size_t)chunk * raw + 16); }   // offset of a chunk's ids in its buffers
     size_t buffer_bytes() const { return ids_at() + 8 * (size_t)chunk; }
-    int prepare(const char* fn) {
+    int prepare(Scratch& sc) {
         if (!host) return VB_OK;
         for (int b = 0; b < 2; ++b) {
-            VB_TRY(ivf_alloc_tmp(fn, dev[b], buffer_bytes()));
+            VB_TRY(sc.own(buffer_bytes(), &dev[b]));
             VB_CUDA(cudaEventCreateWithFlags(&copied[b], cudaEventDisableTiming));
             VB_CUDA(cudaEventCreateWithFlags(&done[b], cudaEventDisableTiming));
         }
+        VB_CUDA(cudaStreamSynchronize(ctx().stream));   // the buffers' stream-ordered allocations precede their copy-stream use
         cudaPointerAttributes attr;
         rows_pinned = cudaPointerGetAttributes(&attr, rows) == cudaSuccess && attr.type == cudaMemoryTypeHost;
         cudaGetLastError();   // (older drivers report an unregistered pointer as an error)
@@ -1746,10 +1730,10 @@ struct IvfBuildSource {
             src = (const uint8_t*)pin[b];
         }
         VB_CUDA(cudaStreamWaitEvent(cx.copy_stream, done[b], 0));   // the device buffer's last chunk has been worked on
-        VB_CUDA(cudaMemcpyAsync(dev[b].mem, src, (size_t)m * raw, cudaMemcpyHostToDevice, cx.copy_stream));
+        VB_CUDA(cudaMemcpyAsync(dev[b], src, (size_t)m * raw, cudaMemcpyHostToDevice, cx.copy_stream));
         if (with_ids) {
             memcpy((uint8_t*)pin[b] + ids_at(), ids + r0, 8 * (size_t)m);
-            VB_CUDA(cudaMemcpyAsync((uint8_t*)dev[b].mem + ids_at(), (uint8_t*)pin[b] + ids_at(), 8 * (size_t)m, cudaMemcpyHostToDevice,
+            VB_CUDA(cudaMemcpyAsync((uint8_t*)dev[b] + ids_at(), (uint8_t*)pin[b] + ids_at(), 8 * (size_t)m, cudaMemcpyHostToDevice,
                                     cx.copy_stream));
         }
         VB_CUDA(cudaEventRecord(copied[b], cx.copy_stream));
@@ -1773,8 +1757,8 @@ struct IvfBuildSource {
             const int b = (int)(c & 1);
             if (c + 1 < nc) VB_TRY(issue(c + 1, pick, total, with_ids));
             VB_CUDA(cudaStreamWaitEvent(cx.stream, copied[b], 0));
-            VB_TRY(work(c * chunk, std::min(chunk, total - c * chunk), (const uint8_t*)dev[b].mem,
-                        (const int64_t*)((const uint8_t*)dev[b].mem + ids_at())));
+            VB_TRY(work(c * chunk, std::min(chunk, total - c * chunk), (const uint8_t*)dev[b],
+                        (const int64_t*)((const uint8_t*)dev[b] + ids_at())));
             VB_CUDA(cudaEventRecord(done[b], cx.stream));
         }
         return VB_OK;
@@ -1828,19 +1812,21 @@ static int ivf_build_impl(const char* fn, vb_ivf* h, const void* rows, const int
     VB_REQUIRE(ns >= L, "%s: %lld samples are fewer than %d lists", fn, (long long)ns, L);
     VB_REQUIRE(!o.u || o.first_row >= 0, "%s: first_row must not be negative", fn);
 
+    Scratch sc(fn);
     IvfBuildSource src{(const uint8_t*)rows, ids, n, raw, host, 0};
     const int64_t auto_chunk = std::min<int64_t>((int64_t)1 << 20, std::max<int64_t>(1024, (int64_t)(IVF_BUILD_CHUNK_BYTES / raw)));
     src.chunk = std::min<int64_t>(n, o.chunk_rows > 0 ? o.chunk_rows : auto_chunk);
-    VB_TRY(src.prepare(fn));
+    VB_TRY(src.prepare(sc));
 
     // centres: samples (spherical: the usable ones, normalised), seeding, Lloyd -- through the host, as vb_kmeans hands
     // them over (lists x dim elements)
     std::vector<uint8_t> cent(raw * (size_t)L);
     int iters = 0;
     {
-        IvfTmp t_pick, t_raw, t_unit;
-        VB_TRY(ivf_alloc_tmp(fn, t_pick, 8 * (size_t)ns));
-        int64_t* d_pick = (int64_t*)t_pick.mem;
+        Scratch sample(fn);
+        void *t_pick, *t_raw, *t_unit;
+        VB_TRY(sample.own(8 * (size_t)ns, &t_pick));
+        int64_t* d_pick = (int64_t*)t_pick;
         Table S = ix.rows;   // (element type, dimensions, stride)
         {
             ProfScope span(VB_PROF_BUILD_SAMPLE);
@@ -1854,8 +1840,8 @@ static int ivf_build_impl(const char* fn, vb_ivf* h, const void* rows, const int
                     VB_CUDA(cudaStreamSynchronize(c.stream));
                 }
             }
-            VB_TRY(ivf_alloc_tmp(fn, t_raw, (size_t)ns * stride + 16));
-            S.d = (uint8_t*)t_raw.mem;
+            VB_TRY(sample.own((size_t)ns * stride + 16, &t_raw));
+            S.d = (uint8_t*)t_raw;
             S.n = S.cap = ns;
             if (host)
                 VB_TRY(src.stream(pick.data(), ns, false, [&](int64_t r0, int64_t m, const uint8_t* d_rows, const int64_t*) {
@@ -1867,15 +1853,15 @@ static int ivf_build_impl(const char* fn, vb_ivf* h, const void* rows, const int
             if (km == VB_SPHERICAL) {
                 // AddSample: a sample that cannot be normalised is dropped, the others are stored as unit vectors
                 const size_t b_rows = align256((size_t)ns * stride + 16), b_zero = align256(4 * (size_t)ns);
-                VB_TRY(ivf_alloc_tmp(fn, t_unit, b_rows + b_zero + 8 * (size_t)ns));
-                int32_t* d_zero = (int32_t*)((uint8_t*)t_unit.mem + b_rows);
-                int64_t* d_to = (int64_t*)((uint8_t*)t_unit.mem + b_rows + b_zero);
+                VB_TRY(sample.own(b_rows + b_zero + 8 * (size_t)ns, &t_unit));
+                int32_t* d_zero = (int32_t*)((uint8_t*)t_unit + b_rows);
+                int64_t* d_to = (int64_t*)((uint8_t*)t_unit + b_rows + b_zero);
                 int64_t kept = 0;
                 VB_TRY(launch_place_rows(ix.elem, ix.dim, true, S.d, stride, nullptr, nullptr, nullptr, ns, nullptr, stride, nullptr, d_zero));
                 VB_TRY(build_compact_map(d_zero, ns, d_to, &kept));
-                VB_TRY(launch_place_rows(ix.elem, ix.dim, true, S.d, stride, nullptr, nullptr, d_to, ns, (uint8_t*)t_unit.mem, stride, nullptr,
+                VB_TRY(launch_place_rows(ix.elem, ix.dim, true, S.d, stride, nullptr, nullptr, d_to, ns, (uint8_t*)t_unit, stride, nullptr,
                                          nullptr));
-                S.d = (uint8_t*)t_unit.mem;
+                S.d = (uint8_t*)t_unit;
                 S.n = kept;
             }
         }
@@ -1898,9 +1884,9 @@ static int ivf_build_impl(const char* fn, vb_ivf* h, const void* rows, const int
     VB_TRY(table_append_host(Cn.t, cent.data(), L));
 
     // pass one: the list of every row (4 bytes per row stay); cosine: of the normalised row, -1 for a row of norm 0
-    IvfTmp t_lists, t_prep, t_dst;
-    VB_TRY(ivf_alloc_tmp(fn, t_lists, 4 * (size_t)n));
-    int32_t* d_lists = (int32_t*)t_lists.mem;
+    void *t_lists, *t_prep, *t_dst;
+    VB_TRY(sc.own(4 * (size_t)n, &t_lists));
+    int32_t* d_lists = (int32_t*)t_lists;
     // A chunk is a table as it lies when its rows need no padding or normalisation and start 16-byte aligned.  Tables the
     // library allocates carry 16 spare bytes behind the last row; the caller's device rows carry none, so of those the
     // last row goes through the padded buffer like a chunk that needs preparing, and the row behind every row read in
@@ -1909,8 +1895,8 @@ static int ivf_build_impl(const char* fn, vb_ivf* h, const void* rows, const int
     if (!host) src.chunk = prep ? std::min(n, auto_chunk) : std::max<int64_t>(n - 1, 1);
     const int64_t prep_rows = prep ? src.chunk : 1;
     const size_t b_prep = align256((size_t)prep_rows * stride + 16);
-    VB_TRY(ivf_alloc_tmp(fn, t_prep, b_prep + 4 * (size_t)prep_rows));
-    uint8_t* d_prep = (uint8_t*)t_prep.mem;
+    VB_TRY(sc.own(b_prep + 4 * (size_t)prep_rows, &t_prep));
+    uint8_t* d_prep = (uint8_t*)t_prep;
     int32_t* d_zero = norm_rows ? (int32_t*)(d_prep + b_prep) : nullptr;
     VB_TRY(src.stream(nullptr, n, false, [&](int64_t r0, int64_t m, const uint8_t* d_rows, const int64_t*) {
         ProfScope span(VB_PROF_BUILD_ASSIGN);
@@ -1926,9 +1912,9 @@ static int ivf_build_impl(const char* fn, vb_ivf* h, const void* rows, const int
     }));
 
     // destinations: list offsets, the image order, and the image row of every row
-    VB_TRY(ivf_alloc_tmp(fn, t_dst, 2 * align256(8 * (size_t)n)));
-    int64_t* d_order = (int64_t*)t_dst.mem;
-    int64_t* d_dst = (int64_t*)((uint8_t*)t_dst.mem + align256(8 * (size_t)n));
+    VB_TRY(sc.own(2 * align256(8 * (size_t)n), &t_dst));
+    int64_t* d_order = (int64_t*)t_dst;
+    int64_t* d_dst = (int64_t*)((uint8_t*)t_dst + align256(8 * (size_t)n));
     std::vector<int64_t> off((size_t)L + 1);
     VB_TRY(build_destinations(d_lists, n, L, d_order, d_dst, off.data()));
     const int64_t n_idx = off[(size_t)L];
@@ -2046,15 +2032,16 @@ int vb_ivf_scan_lists(vb_ivf* h, const void* queries, int64_t nq, int max_probes
             }
         return VB_OK;
     }
+    Scratch sc;
     void* qimg;
     size_t qstride;
-    VB_TRY(upload_queries(ix.elem, ix.dim, queries, nq, true, WS_QIMG, &qimg, &qstride));
+    VB_TRY(upload_queries(sc, ix.elem, ix.dim, queries, nq, true, &qimg, &qstride));
     int32_t* d_lists;
     float* d_ldist;
     if (c.one_query && nq <= ONE_MAX_Q && one_probe_fits(ix.lists, qstride, probes)) {
         // one backend, one scan: distances to the centres and the selection in a single launch; list numbers and
-        // distances (adjacent in the workspace) come back with one copy
-        VB_TRY(ivf_one_probes(ix, qimg, qstride, nq, probes, &d_lists, &d_ldist));
+        // distances (adjacent in the scratch) come back with one copy
+        VB_TRY(ivf_one_probes(sc, ix, qimg, qstride, nq, probes, &d_lists, &d_ldist));
         void* pin;
         const size_t np = (size_t)nq * probes;
         VB_TRY(pinned_buffer2(8 * np, &pin));
@@ -2070,7 +2057,8 @@ int vb_ivf_scan_lists(vb_ivf* h, const void* queries, int64_t nq, int max_probes
             }
         return VB_OK;
     }
-    VB_TRY(ivf_select_probes(ix, qimg, qstride, nq, probes, &d_lists, &d_ldist));
+    float* qn = nullptr;
+    VB_TRY(ivf_select_probes(sc, ix, qimg, qstride, nq, &qn, probes, &d_lists, &d_ldist));
     std::vector<int32_t> hl((size_t)nq * probes);
     std::vector<float> hd((size_t)nq * probes);
     VB_CUDA(cudaMemcpyAsync(hl.data(), d_lists, sizeof(int32_t) * hl.size(), cudaMemcpyDeviceToHost, c.stream));
@@ -2116,13 +2104,14 @@ int vb_ivf_scan_items(vb_ivf* h, const void* q, const int32_t* lists, int nlists
         return VB_OK;
     }
     VB_REQUIRE(k < (int64_t)INT32_MAX, "too many candidates");
+    Scratch sc;
     void* qimg;
     size_t qstride;
-    VB_TRY(upload_queries(ix.elem, ix.dim, q, 1, true, WS_QIMG, &qimg, &qstride));
+    VB_TRY(upload_queries(sc, ix.elem, ix.dim, q, 1, true, &qimg, &qstride));
     void* d_misc;
-    VB_TRY(workspace(WS_MISC, sizeof(int32_t) * (size_t)nlists, &d_misc));
+    VB_TRY(sc.take(sizeof(int32_t) * (size_t)nlists, &d_misc));
     void* d_out;
-    VB_TRY(workspace(WS_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)k, &d_out));
+    VB_TRY(sc.take((sizeof(int64_t) + sizeof(double)) * (size_t)k, &d_out));
     int64_t* o_ids = (int64_t*)d_out;
     double* o_d = (double*)(o_ids + k);
     if (ivf_one_applies(ix, 1, nlists, k, total)) {
@@ -2142,7 +2131,8 @@ int vb_ivf_scan_items(vb_ivf* h, const void* q, const int32_t* lists, int nlists
     // capacity bound must cover these particular lists
     std::vector<int64_t> saved = ix.sorted_len;
     ix.sorted_len.assign(1, total);
-    int rc = ivf_scan_topk(ix, qimg, qstride, 1, (const int32_t*)d_misc, nlists, (int)k, o_ids, nullptr, o_d, nullptr);
+    float* qn = nullptr;
+    int rc = ivf_scan_topk(sc, ix, qimg, qstride, 1, &qn, (const int32_t*)d_misc, nlists, (int)k, o_ids, nullptr, o_d, nullptr);
     ix.sorted_len = saved;
     VB_TRY(rc);
     VB_CUDA(cudaMemcpyAsync(out_ids, o_ids, sizeof(int64_t) * (size_t)k, cudaMemcpyDeviceToHost, c.stream));
@@ -2176,14 +2166,12 @@ struct IvfFilterSpec {
 static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, bool host, bool q_host, int64_t* out_ids,
                            float* out_f, double* out_d, bool level0 = true, const IvfFilterSpec* filt = nullptr);
 
-enum { WS_FILT = 23 };   // the mask arguments of a sub-batch (the sparsevec calls' slot: they never run inside a search)
-
-// the mask arguments of queries [q0, q0 + m) of a filtered call: the filters' positions and runs, in place
-static int ivf_upload_mask(const IvfFilterSpec& filt, int64_t q0, int64_t m, IvfMask* mk) {
+// the mask arguments of queries [q0, q0 + m) of a filtered call (in sc): the filters' positions and runs, in place
+static int ivf_upload_mask(Scratch& sc, const IvfFilterSpec& filt, int64_t q0, int64_t m, IvfMask* mk) {
     Context& c = ctx();
     const size_t tab = ((sizeof(MaskFilter) * (size_t)filt.nfilters) + 15) & ~(size_t)15;
     void* d;
-    VB_TRY(workspace(WS_FILT, tab + 2 * sizeof(int32_t) * (size_t)m, &d));
+    VB_TRY(sc.take(tab + 2 * sizeof(int32_t) * (size_t)m, &d));
     std::vector<MaskFilter> h((size_t)filt.nfilters);
     for (int i = 0; i < filt.nfilters; ++i) h[(size_t)i] = MaskFilter{filt.filters[i]->f.pos, filt.filters[i]->f.off};
     VB_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(MaskFilter) * h.size(), cudaMemcpyHostToDevice, c.stream));
@@ -2286,15 +2274,16 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
     if (!ix.repairing && !filt && ivf_one_applies(ix, nq, probes, k, ivf_cap(ix, probes))) {
         // a handful of queries (one backend's scan): two fused launches, no memsets, one copy back
         const int64_t cap = ivf_cap(ix, probes);
+        Scratch sc;
         void* qimg;
         size_t qstride;
-        VB_TRY(upload_queries(ix.elem, ix.dim, queries, nq, q_host, WS_QIMG, &qimg, &qstride));
+        VB_TRY(upload_queries(sc, ix.elem, ix.dim, queries, nq, q_host, &qimg, &qstride));
         int32_t* d_lists;
         float* d_ldist;
-        VB_TRY(ivf_one_probes(ix, qimg, qstride, nq, probes, &d_lists, &d_ldist));
+        VB_TRY(ivf_one_probes(sc, ix, qimg, qstride, nq, probes, &d_lists, &d_ldist));
         if (host) {
             void* d_out;
-            VB_TRY(workspace(WS_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)nq * k, &d_out));
+            VB_TRY(sc.take((sizeof(int64_t) + sizeof(double)) * (size_t)nq * k, &d_out));
             int64_t* o_ids = (int64_t*)d_out;
             double* o_d = (double*)(o_ids + (size_t)nq * k);
             VB_TRY(ivf_one_items(ix, qimg, qstride, nq, d_lists, probes, k, cap, o_ids, nullptr, o_d, false));
@@ -2323,25 +2312,27 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
         ResetFlag reset{ix.allow_level0};
         ix.allow_level0 = level0 && mode == 0;
         if (ix.d_tc_fail) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), c.stream));
+        Scratch sc;
         void* qimg;
         size_t qstride;
-        VB_TRY(upload_queries(ix.elem, ix.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, q_host, WS_QIMG, &qimg, &qstride));
+        VB_TRY(upload_queries(sc, ix.elem, ix.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, q_host, &qimg, &qstride));
         IvfMask mk{};
-        if (filt) VB_TRY(ivf_upload_mask(*filt, q0, m, &mk));
+        if (filt) VB_TRY(ivf_upload_mask(sc, *filt, q0, m, &mk));
         const IvfMask* mask = filt ? &mk : nullptr;
         int32_t* d_lists;
         float* d_ldist;
-        VB_TRY(ivf_select_probes(ix, qimg, qstride, m, probes, &d_lists, &d_ldist));
+        float* qn = nullptr;   // |q|^2 of the sub-batch, shared by its probe selection and its list scan
+        VB_TRY(ivf_select_probes(sc, ix, qimg, qstride, m, &qn, probes, &d_lists, &d_ldist));
         if (host) {
             void* d_out;
-            VB_TRY(workspace(WS_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
+            VB_TRY(sc.take((sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
             int64_t* o_ids = (int64_t*)d_out;
             double* o_d = (double*)(o_ids + (size_t)m * k);
-            VB_TRY(ivf_scan_topk(ix, qimg, qstride, m, d_lists, probes, k, o_ids, nullptr, o_d, nullptr, mask));
+            VB_TRY(ivf_scan_topk(sc, ix, qimg, qstride, m, &qn, d_lists, probes, k, o_ids, nullptr, o_d, nullptr, mask));
             VB_CUDA(cudaMemcpyAsync(out_ids + q0 * k, o_ids, sizeof(int64_t) * (size_t)m * k, cudaMemcpyDeviceToHost, c.stream));
             VB_CUDA(cudaMemcpyAsync(out_d + q0 * k, o_d, sizeof(double) * (size_t)m * k, cudaMemcpyDeviceToHost, c.stream));
         } else {
-            VB_TRY(ivf_scan_topk(ix, qimg, qstride, m, d_lists, probes, k, out_ids + q0 * k, out_f + q0 * k, nullptr, nullptr, mask));
+            VB_TRY(ivf_scan_topk(sc, ix, qimg, qstride, m, &qn, d_lists, probes, k, out_ids + q0 * k, out_f + q0 * k, nullptr, nullptr, mask));
         }
         fails[0] = fails[1] = 0;
         const bool check = !exact && ix.d_tc_fail != nullptr;
@@ -2527,13 +2518,13 @@ int vb_ivf_search_sharded_dev(vb_ivf* h, const void* queries_dev, int64_t nq, in
     VB_REQUIRE(P <= 4096, "sharded search: world * k must not exceed 4096");
     const int64_t chunk = (nq + world - 1) / world;
     const int64_t q0 = std::min<int64_t>(nq, (int64_t)rank * chunk), m = std::min<int64_t>(chunk, nq - q0);
-    enum { WS_SH_LISTS = 24, WS_SH_RES = 25 };
+    Scratch sc;
     void *d_sh, *d_res;
-    VB_TRY(workspace(WS_SH_LISTS, sizeof(int32_t) * (size_t)chunk * probes * (world + 1) + 64, &d_sh));
+    VB_TRY(sc.take(sizeof(int32_t) * (size_t)chunk * probes * (world + 1) + 64, &d_sh));
     int32_t* my_lists = (int32_t*)d_sh;                          // [chunk x probes]
     int32_t* all_lists = my_lists + (size_t)chunk * probes;      // [world x chunk x probes] = [nq' x probes]
     const size_t res_ids = sizeof(int64_t) * (size_t)nq * k, res_dist = sizeof(float) * (size_t)nq * k;
-    VB_TRY(workspace(WS_SH_RES, (res_ids + res_dist) * (size_t)(world + 1) + 256, &d_res));
+    VB_TRY(sc.take((res_ids + res_dist) * (size_t)(world + 1) + 256, &d_res));
     int64_t* my_ids = (int64_t*)d_res;
     float* my_dist = (float*)((uint8_t*)d_res + res_ids);
     int64_t* all_ids = (int64_t*)((uint8_t*)d_res + res_ids + res_dist);
@@ -2548,19 +2539,23 @@ int vb_ivf_search_sharded_dev(vb_ivf* h, const void* queries_dev, int64_t nq, in
         ix.force_level2 = mode == 1;
         ix.defer_tc_check = !exact;
         VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), c.stream));
+        Scratch batch;
         void* qimg;
         size_t qstride;
-        VB_TRY(upload_queries(ix.elem, ix.dim, queries_dev, nq, false, WS_QIMG, &qimg, &qstride));
+        VB_TRY(upload_queries(batch, ix.elem, ix.dim, queries_dev, nq, false, &qimg, &qstride));
         VB_CUDA(cudaMemsetAsync(my_lists, 0xFF, sizeof(int32_t) * (size_t)chunk * probes, c.stream));
         if (m > 0) {
             int32_t* d_lists;
             float* d_ldist;
-            VB_TRY(ivf_select_probes(ix, (const uint8_t*)qimg + (size_t)q0 * qstride, qstride, m, probes, &d_lists, &d_ldist));
+            float* qn_mine = nullptr;
+            VB_TRY(ivf_select_probes(batch, ix, (const uint8_t*)qimg + (size_t)q0 * qstride, qstride, m, &qn_mine, probes, &d_lists,
+                                     &d_ldist));
             VB_CUDA(cudaMemcpyAsync(my_lists, d_lists, sizeof(int32_t) * (size_t)m * probes, cudaMemcpyDeviceToDevice, c.stream));
         }
         VB_TRY(comm_allgather(my_lists, all_lists, (int64_t)sizeof(int32_t) * chunk * probes));
         // (ranks hold `chunk` queries each, the last one possibly fewer: the gathered array is query-major for q < nq)
-        VB_TRY(ivf_scan_topk(ix, qimg, qstride, nq, all_lists, probes, k, my_ids, my_dist, nullptr, nullptr));
+        float* qn = nullptr;
+        VB_TRY(ivf_scan_topk(batch, ix, qimg, qstride, nq, &qn, all_lists, probes, k, my_ids, my_dist, nullptr, nullptr));
         // one buffer per rank: [ids | distances]; gathered rank-major, so view it as two strided arrays
         VB_TRY(comm_allgather(my_ids, all_ids, (int64_t)res_ids));
         VB_TRY(comm_allgather(my_dist, all_dist, (int64_t)res_dist));
@@ -2612,10 +2607,10 @@ int vb_exact_topk_sharded_dev(vb_table* t, int metric, const void* queries_dev, 
     int P = 2;
     while (P < world * k) P <<= 1;
     VB_REQUIRE(P <= 4096, "sharded exact scan: world * k must not exceed 4096");
-    enum { WS_SH_RES = 25 };
+    Scratch sc;
     void* d_res;
     const size_t res_ids = sizeof(int64_t) * (size_t)nq * k, res_dist = sizeof(float) * (size_t)nq * k;
-    VB_TRY(workspace(WS_SH_RES, (res_ids + res_dist) * (size_t)(world + 1) + 256, &d_res));
+    VB_TRY(sc.take((res_ids + res_dist) * (size_t)(world + 1) + 256, &d_res));
     int64_t* my_ids = (int64_t*)d_res;
     float* my_dist = (float*)((uint8_t*)d_res + res_ids);
     int64_t* all_ids = (int64_t*)((uint8_t*)d_res + res_ids + res_dist);
@@ -2637,9 +2632,9 @@ int vb_ivf_search_sharded(vb_ivf* h, const void* queries, int64_t nq, int probes
     Ivf& ix = h->ix;
     Context& c = ctx();
     const size_t raw = raw_row_bytes(ix.elem, ix.dim);
-    enum { WS_SH_Q = 26 };
+    Scratch sc;
     void* d_q;
-    VB_TRY(workspace(WS_SH_Q, raw * (size_t)nq + (sizeof(int64_t) + sizeof(float)) * (size_t)nq * k + 64, &d_q));
+    VB_TRY(sc.take(raw * (size_t)nq + (sizeof(int64_t) + sizeof(float)) * (size_t)nq * k + 64, &d_q));
     int64_t* d_ids = (int64_t*)((uint8_t*)d_q + ((raw * (size_t)nq + 15) & ~(size_t)15));
     float* d_dist = (float*)(d_ids + (size_t)nq * k);
     VB_CUDA(cudaMemcpyAsync(d_q, queries, raw * (size_t)nq, cudaMemcpyHostToDevice, c.stream));
@@ -2678,8 +2673,9 @@ static int ivf_scan_copy_filters(vb_ivf_scan& s, const vb_filter* const* filters
     foff.back() = base;
     VB_CUDA(cudaMemcpyAsync(s.foff, foff.data(), 8 * foff.size(), cudaMemcpyHostToDevice, c.stream));
     if (filter_of_query && s.nfilters > 1) {
+        Scratch sc;
         void* d_fq;
-        VB_TRY(workspace(WS_MISC, sizeof(int32_t) * (size_t)s.nq, &d_fq));
+        VB_TRY(sc.take(sizeof(int32_t) * (size_t)s.nq, &d_fq));
         VB_CUDA(cudaMemcpyAsync(d_fq, filter_of_query, sizeof(int32_t) * (size_t)s.nq, cudaMemcpyHostToDevice, c.stream));
         VB_TRY(launch_ivf_filter_lists(s.nq, s.max_probes, lists, (const int32_t*)d_fq, s.probe));
     }

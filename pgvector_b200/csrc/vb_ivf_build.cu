@@ -37,26 +37,6 @@ __global__ void build_draw_kernel(int64_t n, int64_t ns, uint64_t seed, int half
     rows_out[j] = (int64_t)x;
 }
 
-// scratch of one call: one allocation, freed (after the stream drained) on every exit
-struct BuildScratch {
-    void* mem = nullptr;
-    ~BuildScratch() {
-        if (mem) {
-            cudaStreamSynchronize(ctx().stream);
-            cudaFree(mem);
-        }
-    }
-    int alloc(const char* what, size_t bytes) {
-        if (cudaMalloc(&mem, bytes) != cudaSuccess) {
-            cudaGetLastError();
-            mem = nullptr;
-            set_error("ivfflat build: allocation of %zu bytes of device memory for %s failed", bytes, what);
-            return VB_ENOMEM;
-        }
-        return VB_OK;
-    }
-};
-
 static size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 int build_draw_samples(int64_t n, int64_t ns, uint64_t seed, int64_t* rows_out) {
@@ -65,12 +45,13 @@ int build_draw_samples(int64_t n, int64_t ns, uint64_t seed, int64_t* rows_out) 
     while (((int64_t)1 << (2 * half)) < n) ++half;
     size_t tmp_bytes = 0;
     VB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, (int64_t*)nullptr, (int64_t*)nullptr, ns, 0, 2 * half, s));
-    BuildScratch sc;
-    VB_TRY(sc.alloc("the sample draw", up256(8 * (size_t)ns) + tmp_bytes));
-    int64_t* drawn = (int64_t*)sc.mem;
+    Scratch sc("ivfflat build");
+    void* mem;
+    VB_TRY(sc.own(up256(8 * (size_t)ns) + tmp_bytes, &mem));
+    int64_t* drawn = (int64_t*)mem;
     build_draw_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, s>>>(n, ns, seed, half, drawn);
     VB_CUDA(cudaGetLastError());
-    VB_CUDA(cub::DeviceRadixSort::SortKeys((uint8_t*)sc.mem + up256(8 * (size_t)ns), tmp_bytes, drawn, rows_out, ns, 0, 2 * half, s));
+    VB_CUDA(cub::DeviceRadixSort::SortKeys((uint8_t*)mem + up256(8 * (size_t)ns), tmp_bytes, drawn, rows_out, ns, 0, 2 * half, s));
     count_launch(2);
     return VB_OK;
 }
@@ -212,10 +193,11 @@ int build_compact_map(const int32_t* zero, int64_t m, int64_t* dst, int64_t* kep
     cudaStream_t s = ctx().stream;
     size_t tmp_bytes = 0;
     VB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, (const int32_t*)nullptr, (int64_t*)nullptr, m, s));
-    BuildScratch sc;
-    VB_TRY(sc.alloc("the sample compaction", up256(8 * (size_t)m) + up256(8) + tmp_bytes));
-    int64_t* before = (int64_t*)sc.mem;
-    int64_t* d_kept = (int64_t*)((uint8_t*)sc.mem + up256(8 * (size_t)m));
+    Scratch sc("ivfflat build");
+    void* mem;
+    VB_TRY(sc.own(up256(8 * (size_t)m) + up256(8) + tmp_bytes, &mem));
+    int64_t* before = (int64_t*)mem;
+    int64_t* d_kept = (int64_t*)((uint8_t*)mem + up256(8 * (size_t)m));
     VB_CUDA(cub::DeviceScan::ExclusiveSum((uint8_t*)d_kept + up256(8), tmp_bytes, zero, before, m, s));
     build_compact_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(zero, before, m, dst, d_kept);
     VB_CUDA(cudaGetLastError());
@@ -263,9 +245,10 @@ int build_destinations(const int32_t* lists_of_row, int64_t n, int lists, int64_
                                             (int64_t*)nullptr, n, 0, end_bit, s));
     // the radix sort is stable: rows of one list stay in call order
     const size_t b_key = up256(4 * (size_t)n), b_row = up256(8 * (size_t)n), b_off = up256(8 * ((size_t)lists + 1));
-    BuildScratch sc;
-    VB_TRY(sc.alloc("the destinations", 2 * b_key + b_row + b_off + tmp_bytes));
-    uint8_t* p = (uint8_t*)sc.mem;
+    Scratch sc("ivfflat build");
+    void* mem;
+    VB_TRY(sc.own(2 * b_key + b_row + b_off + tmp_bytes, &mem));
+    uint8_t* p = (uint8_t*)mem;
     uint32_t* key = (uint32_t*)p;
     uint32_t* sorted_key = (uint32_t*)(p + b_key);
     int64_t* row = (int64_t*)(p + 2 * b_key);

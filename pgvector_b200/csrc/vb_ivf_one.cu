@@ -199,7 +199,7 @@ __global__ void __launch_bounds__(ONE_THREADS) one_scan_kernel(OneScanArgs a) {
     }
     if (!one_last_cta(a.ticket + q)) return;
     {
-        // (cap is a multiple of 4 and the workspace 256-byte aligned: every query's run starts on a 16-byte boundary)
+        // (cap is a multiple of 4 and the scratch 256-byte aligned: every query's run starts on a 16-byte boundary)
         const int t4 = total >> 2;
         const uint4* d4 = reinterpret_cast<const uint4*>(dq);
         for (int i = threadIdx.x; i < t4; i += ONE_THREADS) {

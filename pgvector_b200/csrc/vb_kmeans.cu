@@ -20,9 +20,6 @@
 
 namespace vb {
 
-enum { WSK_STATE = 26 };   // Lloyd state arena (kmeans_run)
-enum { WSK_QIMG = 0, WSK_DIST = 1, WSK_A = 2, WSK_B = 3, WSK_C = 4, WSK_D = 5, WSK_E = 6, WSK_F = 7, WSK_G = 12, WSK_H = 13, WSK_I = 14, WSK_J = 16 };
-
 // ----------------------------------------------------------------------------- exact assign
 
 constexpr int AT_M = 128, AT_N = 128, AT_K = 16, AT_THREADS = 256;
@@ -228,6 +225,7 @@ static int assign_kind(int metric) {
 // exact assign of all rows of X (or of the rows listed in row_sel) against k centres
 int launch_assign_exact(const Table& X, int metric, const Table& Cn, int k, const int32_t* row_sel_dev, int64_t n_sel,
                         int32_t* out_idx, float* out_val) {
+    Scratch sc;
     const int kind = assign_kind(metric);
     VB_REQUIRE(kind >= 0, "assign: unsupported metric %d", metric);
     const int64_t total = row_sel_dev ? n_sel : X.n;
@@ -244,7 +242,7 @@ int launch_assign_exact(const Table& X, int metric, const Table& Cn, int k, cons
     unsigned long long* packed = nullptr;
     if (splits > 1) {
         void* p;
-        VB_TRY(workspace(WSK_J, sizeof(unsigned long long) * (size_t)total, &p));
+        VB_TRY(sc.take(sizeof(unsigned long long) * (size_t)total, &p));
         packed = (unsigned long long*)p;
         VB_CUDA(cudaMemsetAsync(packed, 0xFF, sizeof(unsigned long long) * (size_t)total, s));
     }
@@ -571,6 +569,7 @@ static int kmeans_update_centers(const Table& X, KmeansState& st, int k, bool sp
 
 int kmeans_run(const Table& X, int kmeans_metric, void* centers_host, int k, int max_iter, uint64_t seed,
                vb_allreduce_fn allreduce, void* actx, int* iters_out) {
+    Scratch sc;
     Context& c = ctx();
     cudaStream_t s = c.stream;
     const bool spherical = kmeans_metric == VB_SPHERICAL;
@@ -587,9 +586,9 @@ int kmeans_run(const Table& X, int kmeans_metric, void* centers_host, int k, int
     st.centers.dim = X.dim;
     st.centers.stride = X.stride;
     const int64_t n = X.n;
-    // The state of a run lives in ONE grow-only arena (slot WSK_STATE; the sharded-scan / sparsevec slots it shares
-    // never run beside a k-means): nine cudaMalloc + cudaFree pairs per call cost more than the five Lloyd iterations of
-    // config D on a context that holds a large table, and cudaFree synchronises the device.
+    // The state of a run lives in ONE range of the scratch arena: nine cudaMalloc + cudaFree pairs per call cost more
+    // than the five Lloyd iterations of config D on a context that holds a large table, and cudaFree synchronises the
+    // device.
     size_t scan_tmp_bytes = 0;
     VB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp_bytes, (int32_t*)nullptr, (int32_t*)nullptr, k, s));
     st.scan_tmp_bytes = scan_tmp_bytes;
@@ -597,7 +596,7 @@ int kmeans_run(const Table& X, int kmeans_metric, void* centers_host, int k, int
     const size_t b_cent = up(X.stride * (size_t)k + 16), b_n = up(sizeof(int32_t) * (size_t)std::max<int64_t>(n, 1)),
                  b_k = up(sizeof(int32_t) * (size_t)k), b_agg = up(sizeof(float) * (size_t)k * X.dim), b_tmp = up(std::max<size_t>(scan_tmp_bytes, 16));
     void* arena;
-    VB_TRY(workspace(WSK_STATE, b_cent + 3 * b_n + 2 * b_k + b_agg + 256 + b_tmp, &arena));
+    VB_TRY(sc.take(b_cent + 3 * b_n + 2 * b_k + b_agg + 256 + b_tmp, &arena));
     {
         uint8_t* p = (uint8_t*)arena;
         st.centers.d = p;                       // (table_append_host copies into it: capacity k, nothing to reserve)
@@ -929,23 +928,20 @@ __global__ void pp_fill_f64_kernel(double* p, int64_t n, double v) {
     if (i < n) p[i] = v;
 }
 
-enum { WSK_XB = 27, WSK_FLT = 28, WSK_CENT = 29 };
-
-
 static bool pp_filter_applies(const Table& X, int kmeans_metric, int k) {
     // the filters pay off once the sample table is much larger than L2 and there are enough rounds to amortise the bf16 copy
     if (!ctx().pp_filter || X.elem != VB_VECTOR || kmeans_metric != VB_L2 || X.stride % 32 != 0) return false;
     return ctx().pp_filter == 2 || (k >= 64 && (size_t)X.n * X.stride >= ((size_t)256 << 20));   // 2 = forced (tests)
 }
 
-static int pp_filter_prepare(const Table& X, int k, double* d_wd, PpFilter* f) {
+static int pp_filter_prepare(Scratch& sc, const Table& X, int k, double* d_wd, PpFilter* f) {
     cudaStream_t s = ctx().stream;
     const int64_t n = X.n;
     f->words = (int)(X.stride / 4);
     void *p_xb, *p_flt, *p_cent;
-    VB_TRY(workspace(WSK_XB, sizeof(__nv_bfloat16) * (size_t)n * f->words, &p_xb));
-    VB_TRY(workspace(WSK_FLT, (sizeof(float) + sizeof(int32_t)) * (size_t)n + sizeof(float) * (size_t)k + 64, &p_flt));
-    VB_TRY(workspace(WSK_CENT, X.stride * (size_t)k, &p_cent));
+    VB_TRY(sc.take(sizeof(__nv_bfloat16) * (size_t)n * f->words, &p_xb));
+    VB_TRY(sc.take((sizeof(float) + sizeof(int32_t)) * (size_t)n + sizeof(float) * (size_t)k + 64, &p_flt));
+    VB_TRY(sc.take(X.stride * (size_t)k, &p_cent));
     f->xb = (__nv_bfloat16*)p_xb;
     f->ex = (float*)p_flt;
     f->near = (int32_t*)(f->ex + n);
@@ -1001,6 +997,7 @@ static double host_uniform(uint64_t* st) {
 // oracle the same ones); otherwise they come from the seed.  picked_out (optional, host): the chosen sample rows.
 int kmeans_pp(const Table& X, int kmeans_metric, void* centers_host, int k, uint64_t seed, int64_t first_row, const double* u_in,
               int64_t* picked_out) {
+    Scratch sc;
     Context& c = ctx();
     cudaStream_t s = c.stream;
     const int64_t n = X.n;
@@ -1009,17 +1006,17 @@ int kmeans_pp(const Table& X, int kmeans_metric, void* centers_host, int k, uint
     const int km = kmeans_metric == VB_L2 ? VB_L2_SQUARED : kmeans_metric == VB_SPHERICAL ? VB_NEG_IP : VB_HAMMING;
     const size_t raw = raw_row_bytes(X.elem, X.dim);
     void *d_key, *d_w, *d_wd, *d_cum, *d_picks, *d_u, *d_tmp, *d_q, *d_qraw, *d_out;
-    VB_TRY(workspace(WSK_DIST, sizeof(float) * (size_t)n, &d_key));
-    VB_TRY(workspace(WSK_A, sizeof(float) * (size_t)n, &d_w));
-    VB_TRY(workspace(WSK_B, sizeof(double) * (size_t)n, &d_wd));
-    VB_TRY(workspace(WSK_C, sizeof(double) * (size_t)n, &d_cum));
-    VB_TRY(workspace(WSK_G, sizeof(int64_t) * (size_t)k, &d_picks));
-    VB_TRY(workspace(WSK_F, sizeof(double) * (size_t)k, &d_u));
-    VB_TRY(workspace(WSK_H, X.stride, &d_qraw));
-    VB_TRY(workspace(WSK_I, raw * (size_t)k, &d_out));
+    VB_TRY(sc.take(sizeof(float) * (size_t)n, &d_key));
+    VB_TRY(sc.take(sizeof(float) * (size_t)n, &d_w));
+    VB_TRY(sc.take(sizeof(double) * (size_t)n, &d_wd));
+    VB_TRY(sc.take(sizeof(double) * (size_t)n, &d_cum));
+    VB_TRY(sc.take(sizeof(int64_t) * (size_t)k, &d_picks));
+    VB_TRY(sc.take(sizeof(double) * (size_t)k, &d_u));
+    VB_TRY(sc.take(X.stride, &d_qraw));
+    VB_TRY(sc.take(raw * (size_t)k, &d_out));
     size_t tmp_bytes = 0;
     VB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, (double*)d_wd, (double*)d_cum, (int)n, s));
-    VB_TRY(workspace(WSK_E, tmp_bytes, &d_tmp));
+    VB_TRY(sc.take(tmp_bytes, &d_tmp));
     // FLT_MAX start (src/ivfkmeans.c:39-40); every uniform draw is made up front, in the order the rounds consume them
     std::vector<float> w0((size_t)n, 3.402823466e+38f);
     uint64_t rs = seed ^ 0x5851f42d4c957f2dULL;
@@ -1036,7 +1033,7 @@ int kmeans_pp(const Table& X, int kmeans_metric, void* centers_host, int k, uint
     VB_CUDA(cudaStreamSynchronize(s));  // the host vectors above go out of use here
     const bool filtered = pp_filter_applies(X, kmeans_metric, k);
     PpFilter flt;
-    if (filtered) VB_TRY(pp_filter_prepare(X, k, (double*)d_wd, &flt));
+    if (filtered) VB_TRY(pp_filter_prepare(sc, X, k, (double*)d_wd, &flt));
     pp_gather_rows_kernel<<<1, 256, 0, s>>>(X.d, X.stride, (const int64_t*)d_picks, X.stride, X.stride, (uint8_t*)d_qraw);
     count_launch(1);
     for (int i = 0; i + 1 < k; ++i) {
@@ -1044,8 +1041,9 @@ int kmeans_pp(const Table& X, int kmeans_metric, void* centers_host, int k, uint
         if (filtered) {
             VB_TRY(pp_filter_round(X, flt, (const uint8_t*)d_qraw, i, (float*)d_w, (double*)d_wd));
         } else {
+            Scratch query;
             size_t qstride;
-            VB_TRY(upload_queries(X.elem, X.dim, d_qraw, 1, false, WSK_QIMG, &d_q, &qstride));
+            VB_TRY(upload_queries(query, X.elem, X.dim, d_qraw, 1, false, &d_q, &qstride));
             VB_TRY(launch_scan_regular(X, km, d_q, qstride, 1, n, (float*)d_key, n));
             pp_weight_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const float*)d_key, kmeans_metric, n, (float*)d_w, (double*)d_wd);
         }
@@ -1123,6 +1121,7 @@ __global__ void pp_store_centre_kernel(const uint8_t* __restrict__ row, size_t r
 }
 
 static int kmeans_pp_sharded(const Table& X, int kmeans_metric, void* centers_host, int k, uint64_t seed, int64_t* picked_out) {
+    Scratch sc;
     Context& c = ctx();
     cudaStream_t s = c.stream;
     const int world = comm_world(), rank = comm_rank();
@@ -1133,15 +1132,15 @@ static int kmeans_pp_sharded(const Table& X, int kmeans_metric, void* centers_ho
     const size_t raw = raw_row_bytes(X.elem, X.dim);
     const int words = (int)(X.stride / 4);
     void *d_key, *d_w, *d_wd, *d_cum, *d_u, *d_tmp = nullptr, *d_q, *d_row, *d_out, *d_misc;
-    VB_TRY(workspace(WSK_DIST, sizeof(float) * (size_t)std::max<int64_t>(n, 1), &d_key));
-    VB_TRY(workspace(WSK_A, sizeof(float) * (size_t)std::max<int64_t>(n, 1), &d_w));
-    VB_TRY(workspace(WSK_B, sizeof(double) * (size_t)std::max<int64_t>(n, 1), &d_wd));
-    VB_TRY(workspace(WSK_C, sizeof(double) * (size_t)std::max<int64_t>(n, 1), &d_cum));
-    VB_TRY(workspace(WSK_F, sizeof(double) * (size_t)k, &d_u));
-    VB_TRY(workspace(WSK_H, X.stride, &d_row));
-    VB_TRY(workspace(WSK_I, raw * (size_t)k, &d_out));
+    VB_TRY(sc.take(sizeof(float) * (size_t)std::max<int64_t>(n, 1), &d_key));
+    VB_TRY(sc.take(sizeof(float) * (size_t)std::max<int64_t>(n, 1), &d_w));
+    VB_TRY(sc.take(sizeof(double) * (size_t)std::max<int64_t>(n, 1), &d_wd));
+    VB_TRY(sc.take(sizeof(double) * (size_t)std::max<int64_t>(n, 1), &d_cum));
+    VB_TRY(sc.take(sizeof(double) * (size_t)k, &d_u));
+    VB_TRY(sc.take(X.stride, &d_row));
+    VB_TRY(sc.take(raw * (size_t)k, &d_out));
     // misc: sums[world] doubles | local sum | row_base[world] | picked_local | picked_global[k]
-    VB_TRY(workspace(WSK_G, sizeof(double) * (size_t)(world + 1) + sizeof(int64_t) * (size_t)(world + 1 + k) + 64, &d_misc));
+    VB_TRY(sc.take(sizeof(double) * (size_t)(world + 1) + sizeof(int64_t) * (size_t)(world + 1 + k) + 64, &d_misc));
     double* d_sums = (double*)d_misc;
     double* d_lsum = d_sums + world;
     int64_t* d_base = (int64_t*)(d_lsum + 1);
@@ -1150,7 +1149,7 @@ static int kmeans_pp_sharded(const Table& X, int kmeans_metric, void* centers_ho
     size_t tmp_bytes = 0;
     if (n > 0) {
         VB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, (double*)d_wd, (double*)d_cum, (int)n, s));
-        VB_TRY(workspace(WSK_E, tmp_bytes, &d_tmp));
+        VB_TRY(sc.take(tmp_bytes, &d_tmp));
     }
     // global row numbering: every rank learns every slice length (one exchange at the start)
     std::vector<int64_t> lens((size_t)world, 0), base((size_t)world, 0);
@@ -1186,7 +1185,7 @@ static int kmeans_pp_sharded(const Table& X, int kmeans_metric, void* centers_ho
     const bool filtered = n > 0 && ctx().pp_filter && X.elem == VB_VECTOR && kmeans_metric == VB_L2 && X.stride % 32 == 0 &&
                           (ctx().pp_filter == 2 || (k >= 64 && (size_t)n_total * X.stride >= ((size_t)256 << 20)));
     PpFilter flt;
-    if (filtered) VB_TRY(pp_filter_prepare(X, k, (double*)d_wd, &flt));
+    if (filtered) VB_TRY(pp_filter_prepare(sc, X, k, (double*)d_wd, &flt));
     for (int i = 0; i < k; ++i) {
         // centre i: the owner's row reaches every rank
         pp_contribute_row_kernel<<<4, 256, 0, s>>>(X.d, X.stride, d_pick, (uint32_t*)d_row, words);
@@ -1199,8 +1198,9 @@ static int kmeans_pp_sharded(const Table& X, int kmeans_metric, void* centers_ho
             if (filtered) {
                 VB_TRY(pp_filter_round(X, flt, (const uint8_t*)d_row, i, (float*)d_w, (double*)d_wd));
             } else {
+                Scratch query;
                 size_t qstride;
-                VB_TRY(upload_queries(X.elem, X.dim, d_row, 1, false, WSK_QIMG, &d_q, &qstride));
+                VB_TRY(upload_queries(query, X.elem, X.dim, d_row, 1, false, &d_q, &qstride));
                 VB_TRY(launch_scan_regular(X, km, d_q, qstride, 1, n, (float*)d_key, n));
                 pp_weight_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const float*)d_key, kmeans_metric, n, (float*)d_w, (double*)d_wd);
             }
@@ -1271,9 +1271,10 @@ static int assign_impl(vb_table* rows, int metric, const void* centers, int k, b
     Cn.stride = X.stride;
     int rc = host ? table_append_host(Cn, centers, k) : table_append_dev(Cn, centers, k);
     int32_t* d_out = out;
+    Scratch sc;
     void* ws = nullptr;
     if (rc == VB_OK && host) {
-        rc = workspace(WSK_F, sizeof(int32_t) * (size_t)std::max<int64_t>(X.n, 1), &ws);
+        rc = sc.take(sizeof(int32_t) * (size_t)std::max<int64_t>(X.n, 1), &ws);
         d_out = (int32_t*)ws;
     }
     if (rc == VB_OK) {

@@ -1003,15 +1003,26 @@ __global__ void lc_traffic_kernel(LcArgs a, uint32_t a_bytes, unsigned long long
 
 // ----------------------------------------------------------------------------- host side
 
-enum { WSC_B = 21, WSC_N = 22 };
-
 // c_sum of lc_make_bound: the fp32 norms, the final sum and the exact distance, relative to |x|^2 + |q|^2
 static float lc_c_sum(int dim) { return std::max(1.0f / 65536.0f, 3.0f * ((float)dim / 32.0f + 8.0f) / 16777216.0f); }
 
-// level 0's per-row bound coefficients: the float4 array after eps(q)^2 in launch_list_tc's WSC_N workspace, which hands
-// the refine kernels eps(q)^2 (qe2) for the batch's nq queries
+// the batch's bound inputs (list_tc_query_norms): [|q|^2 | level 0: t_q | level 0: eps(q)^2 | level 0: per-row bound
+// coefficients]; the refine kernels read |q|^2, or at level 0 eps(q)^2 and the coefficients
+static const float* l0_qe2(const float* qn, int64_t nq) { return qn + 2 * nq; }
 static float4* l0_row_coef(const float* qe2, int64_t nq) {
     return reinterpret_cast<float4*>(((uintptr_t)(qe2 + nq) + 15) & ~(uintptr_t)15);
+}
+
+int list_tc_query_norms(Scratch& sc, const void* qimg, size_t qstride, int64_t nq, float** qn) {
+    void* p;
+    VB_TRY(sc.take(sizeof(float) * (size_t)nq * 3 + 16 + sizeof(float4) * (size_t)nq + 64, &p));
+    *qn = (float*)p;
+    // the query image is fp32 with the rows' padded dimension count for both element types
+    row_sqnorm_kernel<VB_VECTOR><<<(unsigned)((nq * 32 + 255) / 256), 256, 0, ctx().stream>>>((const uint8_t*)qimg, qstride, nq,
+                                                                                            (int)(qstride / 4), *qn, nq, 0.f);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
 }
 
 // device accumulators: [0..3] / [4..7] lc_traffic_kernel per filter use (lists / centres), [8..10] the level-0 refine's
@@ -1226,39 +1237,21 @@ int list_tc_repack(const Table& rows, ListTcImage* im, int64_t first_tile, int64
 // approximate pass: fills `out` (the per-query candidate runs) with d~
 int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, const void* qimg, size_t qstride, int64_t nq,
                    const int32_t* d_lists, int probes, const int32_t* cand_off, int64_t cap, const int64_t* d_list_off, int n_lists,
-                   float* out, const float** qn_out, bool one_list_all_queries, int level, float* smin, int64_t cap_s) {
+                   float* out, float* qn, bool one_list_all_queries, int level, float* smin, int64_t cap_s) {
     Context& c = ctx();
     cudaStream_t s = c.stream;
+    Scratch sc;
     QueryGroups g{};
-    VB_TRY(build_query_groups(d_lists, nq, probes, cand_off, cap, n_lists, LC_N, &g, smin ? cap_s : 0));
+    VB_TRY(build_query_groups(sc, d_lists, nq, probes, cand_off, cap, n_lists, LC_N, &g, smin ? cap_s : 0));
     const int64_t max_gtiles = g.n_pairs / LC_N + n_lists + 1;
-    void *d_B, *d_qn;
+    void* d_B;
     // (level 0: the B tiles take half of this, the packed queries q8 follow them)
     const size_t q8_bytes = level == 0 ? (size_t)nq * 2 * im.n_kblocks8 * 128 : 0;
-    VB_TRY(workspace(WSC_B, (size_t)max_gtiles * im.n_kblocks * LC_B_STAGE + q8_bytes, &d_B));
-    // [|q|^2 | level 0: t_q | level 0: eps(q)^2 | level 0: per-row bound coefficients (l0_row_coef)], one size for every
-    // level so that the |q|^2 cache below stays put
-    VB_TRY(workspace(WSC_N, sizeof(float) * (size_t)nq * 3 + 16 + sizeof(float4) * (size_t)nq + 64, &d_qn));
-    float* d_tq = (float*)d_qn + nq;
+    VB_TRY(sc.take((size_t)max_gtiles * im.n_kblocks * LC_B_STAGE + q8_bytes, &d_B));
+    float* d_tq = qn + nq;
     float* d_qe2 = d_tq + nq;
     // the query image is fp32 with the rows' padded dimension count for both element types
     const int qdim = (int)(qstride / 4);
-    {
-        // |q|^2 of the batch: the probe selection and the list scan of one batch see the same query image -- compute once
-        static const void* qn_img = nullptr;
-        static int64_t qn_nq = 0;
-        static uint64_t qn_epoch = ~0ull;
-        static void* qn_buf = nullptr;
-        if (!(qn_img == qimg && qn_nq == nq && qn_epoch == c.query_epoch && qn_buf == d_qn)) {
-            row_sqnorm_kernel<VB_VECTOR><<<(unsigned)((nq * 32 + 255) / 256), 256, 0, s>>>((const uint8_t*)qimg, qstride, nq, qdim, (float*)d_qn,
-                                                                                          nq, 0.f);
-            count_launch();
-            qn_img = qimg;
-            qn_nq = nq;
-            qn_epoch = c.query_epoch;
-            qn_buf = d_qn;
-        }
-    }
     const bool l0 = level == 0;
     const int n_kblocks = l0 ? im.n_kblocks8 : im.n_kblocks;
     const int64_t chunks = g.n_pairs * n_kblocks * 8;
@@ -1296,7 +1289,7 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
     a.pair_q = g.pair_q;
     a.pair_out = g.pair_out;
     a.xn = im.xn;
-    a.qn = (const float*)d_qn;
+    a.qn = qn;
     a.out = out;
     a.smin = smin;
     a.pair_sbase = g.pair_sbase;
@@ -1317,8 +1310,6 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
         lc_traffic_kernel<<<32, 256, 0, s>>>(a, level <= 1 ? LC_A_PLANE : LC_A_STAGE, g_traffic + (one_list_all_queries ? 4 : 0));
         VB_CUDA(cudaGetLastError());
     }
-    // the refine kernels take the bound's per-query input: |q|^2, or at level 0 eps(q)^2 (lc_make_bound)
-    *qn_out = l0 ? d_qe2 : (const float*)d_qn;
     return VB_OK;
 }
 
@@ -1417,6 +1408,8 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
     Context& c = ctx();
     cudaStream_t s = c.stream;
     const LcBound bound = lc_make_bound(rows, im, key_metric, level);
+    // the bound's per-query input: |q|^2, or at level 0 eps(q)^2 (lc_make_bound)
+    if (level == 0) qn = l0_qe2(qn, nq);
     const int V = (int)(rows.stride / 16);
     const size_t smem = (size_t)SS_CAND * 8 + (size_t)kp * 16 + qstride + cr_work_bytes(smin, pre_pos, cap, cap_s, probes) + (size_t)kp * 4 + 16;
     VB_REQUIRE(kp <= SS_THREADS && smem <= 200 * 1024 && (smin || pre_pos || cap <= CR_RUN_MAX),

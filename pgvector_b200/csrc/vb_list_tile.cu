@@ -373,11 +373,9 @@ bool list_major_supported(int elem, int key_metric) {
     return (elem == VB_VECTOR || elem == VB_HALFVEC) && (key_metric == VB_L2_SQUARED || key_metric == VB_NEG_IP);
 }
 
-enum { WSL_GROUPS = 20 };
-
 // Group the (query, probe) pairs of a batch by list.  gt_rows > 0 additionally numbers the query tiles of
 // gt_rows queries over all lists (tensor-core path: one packed B tile per query tile).
-int build_query_groups(const int32_t* d_lists, int64_t nq, int probes, const int32_t* cand_off, int64_t cap, int n_lists, int gt_rows,
+int build_query_groups(Scratch& sc, const int32_t* d_lists, int64_t nq, int probes, const int32_t* cand_off, int64_t cap, int n_lists, int gt_rows,
                        QueryGroups* g, int64_t cap_s) {
     Context& c = ctx();
     cudaStream_t s = c.stream;
@@ -386,7 +384,7 @@ int build_query_groups(const int32_t* d_lists, int64_t nq, int probes, const int
     void* d_ws;
     VB_REQUIRE(nq * cap_s < (int64_t)INT32_MAX, "slab-minimum array too large (%lld queries)", (long long)nq);
     const size_t ints = (size_t)n_lists * 5 + (size_t)n_pairs * 3;
-    VB_TRY(workspace(WSL_GROUPS, sizeof(int64_t) * (size_t)n_pairs + sizeof(int32_t) * ints + 64, &d_ws));
+    VB_TRY(sc.take(sizeof(int64_t) * (size_t)n_pairs + sizeof(int32_t) * ints + 64, &d_ws));
     g->pair_out = (int64_t*)d_ws;
     g->pair_q = (int32_t*)(g->pair_out + n_pairs);
     g->pair_list = g->pair_q + n_pairs;
@@ -433,8 +431,9 @@ int launch_list_major(const Table& rows, int key_metric, const void* qimg, size_
     VB_REQUIRE(list_major_supported(rows.elem, key_metric), "list-major scan: unsupported element type / metric");
     if (nq <= 0 || n_tiles <= 0) return VB_OK;
     cudaStream_t s = ctx().stream;
+    Scratch sc;
     QueryGroups g{};
-    VB_TRY(build_query_groups(d_lists, nq, probes, cand_off, cap, n_lists, 0, &g));
+    VB_TRY(build_query_groups(sc, d_lists, nq, probes, cand_off, cap, n_lists, 0, &g));
     int32_t* begin = g.begin;
     int32_t* cnt = g.cnt;
     int32_t* pair_q = g.pair_q;

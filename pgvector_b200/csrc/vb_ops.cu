@@ -12,7 +12,7 @@
 // src/ivfscan.c:222-229, src/hnswutils.c:417-423); norms accumulate in fp64 like the reference.
 // One warp per row; HBM bound (row read once, written once).
 // Every transform is one launcher over device rows (the *_rows functions); the _dev entry points call it on the
-// caller's buffers, the host variants stage the rows in a workspace, call it and copy the result back, so both give
+// caller's buffers, the host variants stage the rows in device scratch, call it and copy the result back, so both give
 // the same bits.
 #include "vb_common.cuh"
 
@@ -270,8 +270,6 @@ __global__ void array_cast_kernel(const S* __restrict__ in, int64_t total, int d
     if (key != NO_ERROR) atomicMin(first_bad, key);
 }
 
-enum { WSO_IN = 17, WSO_OUT = 18, WSO_FLAG = 19, WSO_IN2 = 20 };
-
 // the shortest decimal that reads back as the same float, in PostgreSQL's float4 output style
 // (float_to_shortest_decimal_buf: fixed notation for exponents -4 .. 14, scientific otherwise)
 static void shortest_float(float v, char* buf, size_t cap) {
@@ -306,9 +304,9 @@ int half_range_error(float v) {
     return VB_EINVAL;
 }
 
-static int stage_in(int elem, int dim, const void* rows, int64_t n, void** d_in) {
+static int stage_in(Scratch& sc, int elem, int dim, const void* rows, int64_t n, void** d_in) {
     const size_t raw = raw_row_bytes(elem, dim);
-    VB_TRY(workspace(WSO_IN, raw * (size_t)n, d_in));
+    VB_TRY(sc.take(raw * (size_t)n, d_in));
     VB_CUDA(cudaMemcpyAsync(*d_in, rows, raw * (size_t)n, cudaMemcpyHostToDevice, ctx().stream));
     return VB_OK;
 }
@@ -599,13 +597,14 @@ extern "C" {
 // ---------------------------------------------------------------- host buffers
 
 int vb_norm_batch(int elem, int dim, const void* rows, int64_t n, double* out) {
+    Scratch sc;
     VB_TRY(require_init());
     VB_REQUIRE((elem == VB_VECTOR || elem == VB_HALFVEC) && dim > 0 && (rows || n == 0) && out, "bad norm arguments");
     if (n <= 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     void *d_in, *d_out;
-    VB_TRY(stage_in(elem, dim, rows, n, &d_in));
-    VB_TRY(workspace(WSO_OUT, sizeof(double) * (size_t)n, &d_out));
+    VB_TRY(stage_in(sc, elem, dim, rows, n, &d_in));
+    VB_TRY(sc.take(sizeof(double) * (size_t)n, &d_out));
     VB_TRY(norm_rows(elem, dim, d_in, n, (double*)d_out));
     VB_CUDA(cudaMemcpyAsync(out, d_out, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, s));
     VB_CUDA(cudaStreamSynchronize(s));
@@ -613,15 +612,16 @@ int vb_norm_batch(int elem, int dim, const void* rows, int64_t n, double* out) {
 }
 
 int vb_l2_normalize_batch(int elem, int dim, const void* rows, int64_t n, void* out) {
+    Scratch sc;
     VB_TRY(require_init());
     VB_REQUIRE((elem == VB_VECTOR || elem == VB_HALFVEC) && dim > 0 && (rows || n == 0) && out, "bad normalize arguments");
     if (n <= 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     void *d_in, *d_out, *d_flag;
     const size_t raw = raw_row_bytes(elem, dim);
-    VB_TRY(stage_in(elem, dim, rows, n, &d_in));
-    VB_TRY(workspace(WSO_OUT, raw * (size_t)n, &d_out));
-    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(stage_in(sc, elem, dim, rows, n, &d_in));
+    VB_TRY(sc.take(raw * (size_t)n, &d_out));
+    VB_TRY(sc.take(64, &d_flag));
     VB_TRY(normalize_rows(elem, dim, d_in, n, d_out, (int*)d_flag));
     int flag = 0;
     VB_CUDA(cudaMemcpyAsync(out, d_out, raw * (size_t)n, cudaMemcpyDeviceToHost, s));
@@ -633,14 +633,15 @@ int vb_l2_normalize_batch(int elem, int dim, const void* rows, int64_t n, void* 
 }
 
 int vb_binary_quantize_batch(int elem, int dim, const void* rows, int64_t n, uint8_t* out) {
+    Scratch sc;
     VB_TRY(require_init());
     VB_REQUIRE((elem == VB_VECTOR || elem == VB_HALFVEC) && dim > 0 && (rows || n == 0) && out, "bad binary_quantize arguments");
     if (n <= 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     void *d_in, *d_out;
     const size_t nb = ((size_t)dim + 7) / 8;
-    VB_TRY(stage_in(elem, dim, rows, n, &d_in));
-    VB_TRY(workspace(WSO_OUT, nb * (size_t)n, &d_out));
+    VB_TRY(stage_in(sc, elem, dim, rows, n, &d_in));
+    VB_TRY(sc.take(nb * (size_t)n, &d_out));
     VB_TRY(quantize_rows(elem, dim, d_in, n, (uint8_t*)d_out));
     VB_CUDA(cudaMemcpyAsync(out, d_out, nb * (size_t)n, cudaMemcpyDeviceToHost, s));
     VB_CUDA(cudaStreamSynchronize(s));
@@ -648,15 +649,16 @@ int vb_binary_quantize_batch(int elem, int dim, const void* rows, int64_t n, uin
 }
 
 int vb_vector_to_halfvec_batch(int dim, const void* rows, int64_t n, void* out) {
+    Scratch sc;
     VB_TRY(require_init());
     VB_REQUIRE(dim > 0 && (rows || n == 0) && out, "bad cast arguments");
     if (n <= 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     const int64_t total = n * dim;
     void *d_in, *d_out, *d_flag;
-    VB_TRY(stage_in(VB_VECTOR, dim, rows, n, &d_in));
-    VB_TRY(workspace(WSO_OUT, sizeof(__half) * (size_t)total, &d_out));
-    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(stage_in(sc, VB_VECTOR, dim, rows, n, &d_in));
+    VB_TRY(sc.take(sizeof(__half) * (size_t)total, &d_out));
+    VB_TRY(sc.take(64, &d_flag));
     VB_TRY(to_half_rows(dim, d_in, n, d_out, (unsigned long long*)d_flag));
     unsigned long long bad = ~0ull;
     VB_CUDA(cudaMemcpyAsync(out, d_out, sizeof(__half) * (size_t)total, cudaMemcpyDeviceToHost, s));
@@ -667,14 +669,15 @@ int vb_vector_to_halfvec_batch(int dim, const void* rows, int64_t n, void* out) 
 }
 
 int vb_halfvec_to_vector_batch(int dim, const void* rows, int64_t n, void* out) {
+    Scratch sc;
     VB_TRY(require_init());
     VB_REQUIRE(dim > 0 && (rows || n == 0) && out, "bad cast arguments");
     if (n <= 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     const int64_t total = n * dim;
     void *d_in, *d_out;
-    VB_TRY(stage_in(VB_HALFVEC, dim, rows, n, &d_in));
-    VB_TRY(workspace(WSO_OUT, sizeof(float) * (size_t)total, &d_out));
+    VB_TRY(stage_in(sc, VB_HALFVEC, dim, rows, n, &d_in));
+    VB_TRY(sc.take(sizeof(float) * (size_t)total, &d_out));
     VB_TRY(to_float_rows(dim, d_in, n, d_out));
     VB_CUDA(cudaMemcpyAsync(out, d_out, sizeof(float) * (size_t)total, cudaMemcpyDeviceToHost, s));
     VB_CUDA(cudaStreamSynchronize(s));
@@ -682,6 +685,7 @@ int vb_halfvec_to_vector_batch(int dim, const void* rows, int64_t n, void* out) 
 }
 
 int vb_subvector_batch(int elem, int dim, const void* rows, int64_t n, int32_t start, int32_t count, void* out, int* out_dim) {
+    Scratch sc;
     const char* fn = "vb_subvector_batch";
     VB_TRY(require_init());
     VB_TRY(check_rows(fn, elem, dim, n, rows, out));
@@ -692,8 +696,8 @@ int vb_subvector_batch(int elem, int dim, const void* rows, int64_t n, int32_t s
     if (n == 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     void *d_in, *d_out;
-    VB_TRY(stage_in(elem, dim, rows, n, &d_in));
-    VB_TRY(workspace(WSO_OUT, dense_bytes(elem, d, n), &d_out));
+    VB_TRY(stage_in(sc, elem, dim, rows, n, &d_in));
+    VB_TRY(sc.take(dense_bytes(elem, d, n), &d_out));
     VB_TRY(subvector_rows(elem, dim, d_in, n, first, d, d_out));
     VB_CUDA(cudaMemcpyAsync(out, d_out, dense_bytes(elem, d, n), cudaMemcpyDeviceToHost, s));
     VB_CUDA(cudaStreamSynchronize(s));
@@ -712,6 +716,7 @@ int vb_norm_batch_dev(int elem, int dim, const void* rows_dev, int64_t n, double
 }
 
 int vb_l2_normalize_batch_dev(int elem, int dim, const void* rows_dev, int64_t n, void* out_dev) {
+    Scratch sc;
     VB_TRY(require_init());
     const char* fn = "vb_l2_normalize_batch_dev";
     VB_TRY(check_rows(fn, elem, dim, n, rows_dev, out_dev));
@@ -720,7 +725,7 @@ int vb_l2_normalize_batch_dev(int elem, int dim, const void* rows_dev, int64_t n
     if (rows_dev != out_dev) VB_TRY(check_disjoint(fn, rows_dev, bytes, out_dev, bytes));   // in place is allowed
     cudaStream_t s = ctx().stream;
     void* d_flag;
-    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(sc.take(64, &d_flag));
     VB_TRY(normalize_rows(elem, dim, rows_dev, n, out_dev, (int*)d_flag));
     int flag = 0;
     VB_CUDA(cudaMemcpyAsync(&flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -739,6 +744,7 @@ int vb_binary_quantize_batch_dev(int elem, int dim, const void* rows_dev, int64_
 }
 
 int vb_vector_to_halfvec_batch_dev(int dim, const void* rows_dev, int64_t n, void* out_dev) {
+    Scratch sc;
     VB_TRY(require_init());
     const char* fn = "vb_vector_to_halfvec_batch_dev";
     VB_TRY(check_rows(fn, VB_VECTOR, dim, n, rows_dev, out_dev));
@@ -746,7 +752,7 @@ int vb_vector_to_halfvec_batch_dev(int dim, const void* rows_dev, int64_t n, voi
     VB_TRY(check_disjoint(fn, rows_dev, dense_bytes(VB_VECTOR, dim, n), out_dev, dense_bytes(VB_HALFVEC, dim, n)));
     cudaStream_t s = ctx().stream;
     void* d_flag;
-    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(sc.take(64, &d_flag));
     VB_TRY(to_half_rows(dim, rows_dev, n, out_dev, (unsigned long long*)d_flag));
     unsigned long long bad = ~0ull;
     VB_CUDA(cudaMemcpyAsync(&bad, d_flag, sizeof(bad), cudaMemcpyDeviceToHost, s));
@@ -783,6 +789,7 @@ int vb_subvector_batch_dev(int elem, int dim, const void* rows_dev, int64_t n, i
 // ---------------------------------------------------------------- + - * ||, array casts
 
 int vb_arith_batch(int elem, int op, int dim_a, const void* a, int64_t na, int dim_b, const void* b, int64_t nb, void* out) {
+    Scratch sc;
     const char* fn = "vb_arith_batch";
     VB_TRY(require_init());
     int64_t m;
@@ -794,11 +801,11 @@ int vb_arith_batch(int elem, int op, int dim_a, const void* a, int64_t na, int d
     cudaStream_t s = ctx().stream;
     void *d_a, *d_b, *d_out, *d_flag;
     const size_t raw = raw_row_bytes(elem, dim_a);
-    VB_TRY(stage_in(elem, dim_a, a, na, &d_a));
-    VB_TRY(workspace(WSO_IN2, raw * (size_t)nb, &d_b));
+    VB_TRY(stage_in(sc, elem, dim_a, a, na, &d_a));
+    VB_TRY(sc.take(raw * (size_t)nb, &d_b));
     VB_CUDA(cudaMemcpyAsync(d_b, b, raw * (size_t)nb, cudaMemcpyHostToDevice, s));
-    VB_TRY(workspace(WSO_OUT, raw * (size_t)m, &d_out));
-    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(sc.take(raw * (size_t)m, &d_out));
+    VB_TRY(sc.take(64, &d_flag));
     VB_TRY(arith_rows(elem, op, dim_a, d_a, na, d_b, nb, m, d_out, (unsigned long long*)d_flag));
     unsigned long long key = NO_ERROR;
     VB_CUDA(cudaMemcpyAsync(out, d_out, raw * (size_t)m, cudaMemcpyDeviceToHost, s));
@@ -808,6 +815,7 @@ int vb_arith_batch(int elem, int op, int dim_a, const void* a, int64_t na, int d
 }
 
 int vb_arith_batch_dev(int elem, int op, int dim_a, const void* a_dev, int64_t na, int dim_b, const void* b_dev, int64_t nb, void* out_dev) {
+    Scratch sc;
     const char* fn = "vb_arith_batch_dev";
     VB_TRY(require_init());
     int64_t m;
@@ -821,7 +829,7 @@ int vb_arith_batch_dev(int elem, int op, int dim_a, const void* a_dev, int64_t n
     if (!(out_dev == b_dev && nb == m)) VB_TRY(check_disjoint(fn, b_dev, raw * (size_t)nb, out_dev, raw * (size_t)m));
     cudaStream_t s = ctx().stream;
     void* d_flag;
-    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(sc.take(64, &d_flag));
     VB_TRY(arith_rows(elem, op, dim_a, a_dev, na, b_dev, nb, m, out_dev, (unsigned long long*)d_flag));
     unsigned long long key = NO_ERROR;
     VB_CUDA(cudaMemcpyAsync(&key, d_flag, sizeof(key), cudaMemcpyDeviceToHost, s));
@@ -839,6 +847,7 @@ static int concat_dim(int elem, int dim_a, int dim_b, int* d) {
 }
 
 int vb_concat_batch(int elem, int dim_a, const void* a, int64_t na, int dim_b, const void* b, int64_t nb, void* out, int* out_dim) {
+    Scratch sc;
     const char* fn = "vb_concat_batch";
     VB_TRY(require_init());
     int64_t m;
@@ -850,10 +859,10 @@ int vb_concat_batch(int elem, int dim_a, const void* a, int64_t na, int dim_b, c
     if (m == 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     void *d_a, *d_b, *d_out;
-    VB_TRY(stage_in(elem, dim_a, a, na, &d_a));
-    VB_TRY(workspace(WSO_IN2, dense_bytes(elem, dim_b, nb), &d_b));
+    VB_TRY(stage_in(sc, elem, dim_a, a, na, &d_a));
+    VB_TRY(sc.take(dense_bytes(elem, dim_b, nb), &d_b));
     VB_CUDA(cudaMemcpyAsync(d_b, b, dense_bytes(elem, dim_b, nb), cudaMemcpyHostToDevice, s));
-    VB_TRY(workspace(WSO_OUT, dense_bytes(elem, d, m), &d_out));
+    VB_TRY(sc.take(dense_bytes(elem, d, m), &d_out));
     VB_TRY(concat_rows(elem, dim_a, d_a, na, dim_b, d_b, nb, m, d_out));
     VB_CUDA(cudaMemcpyAsync(out, d_out, dense_bytes(elem, d, m), cudaMemcpyDeviceToHost, s));
     VB_CUDA(cudaStreamSynchronize(s));
@@ -879,6 +888,7 @@ int vb_concat_batch_dev(int elem, int dim_a, const void* a_dev, int64_t na, int 
 }
 
 int vb_array_to_rows_batch(int elem, int src, int dim, int32_t typmod, const void* in, int64_t n, void* out) {
+    Scratch sc;
     const char* fn = "vb_array_to_rows_batch";
     VB_TRY(require_init());
     VB_TRY(check_array_cast(fn, elem, src, dim, typmod, in, n, out));
@@ -886,10 +896,10 @@ int vb_array_to_rows_batch(int elem, int src, int dim, int32_t typmod, const voi
     cudaStream_t s = ctx().stream;
     const size_t in_bytes = array_elem_bytes(src) * (size_t)dim * (size_t)n;
     void *d_in, *d_out, *d_flag;
-    VB_TRY(workspace(WSO_IN, in_bytes, &d_in));
+    VB_TRY(sc.take(in_bytes, &d_in));
     VB_CUDA(cudaMemcpyAsync(d_in, in, in_bytes, cudaMemcpyHostToDevice, s));
-    VB_TRY(workspace(WSO_OUT, dense_bytes(elem, dim, n), &d_out));
-    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(sc.take(dense_bytes(elem, dim, n), &d_out));
+    VB_TRY(sc.take(64, &d_flag));
     VB_TRY(array_cast_rows(elem, src, dim, d_in, n, d_out, (unsigned long long*)d_flag));
     unsigned long long key = NO_ERROR;
     VB_CUDA(cudaMemcpyAsync(out, d_out, dense_bytes(elem, dim, n), cudaMemcpyDeviceToHost, s));
@@ -902,6 +912,7 @@ int vb_array_to_rows_batch(int elem, int src, int dim, int32_t typmod, const voi
 }
 
 int vb_array_to_rows_batch_dev(int elem, int src, int dim, int32_t typmod, const void* in_dev, int64_t n, void* out_dev) {
+    Scratch sc;
     const char* fn = "vb_array_to_rows_batch_dev";
     VB_TRY(require_init());
     VB_TRY(check_array_cast(fn, elem, src, dim, typmod, in_dev, n, out_dev));
@@ -909,7 +920,7 @@ int vb_array_to_rows_batch_dev(int elem, int src, int dim, int32_t typmod, const
     VB_TRY(check_disjoint(fn, in_dev, array_elem_bytes(src) * (size_t)dim * (size_t)n, out_dev, dense_bytes(elem, dim, n)));
     cudaStream_t s = ctx().stream;
     void* d_flag;
-    VB_TRY(workspace(WSO_FLAG, 64, &d_flag));
+    VB_TRY(sc.take(64, &d_flag));
     VB_TRY(array_cast_rows(elem, src, dim, in_dev, n, out_dev, (unsigned long long*)d_flag));
     unsigned long long key = NO_ERROR;
     VB_CUDA(cudaMemcpyAsync(&key, d_flag, sizeof(key), cudaMemcpyDeviceToHost, s));

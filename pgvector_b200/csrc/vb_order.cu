@@ -367,14 +367,6 @@ struct vb_order {
 
 namespace vb {
 
-// Temporaries of a creation: one allocation, freed before returning.
-struct OrderTmp {
-    void* mem = nullptr;
-    ~OrderTmp() {
-        if (mem) cudaFree(mem);
-    }
-};
-
 static inline unsigned grid_of(int64_t threads) { return (unsigned)((threads + 255) / 256); }
 
 // The sort of n rows (DenseSrc or SparseSrc, by SPARSE) into o: perm, group_of_row, group_start, groups, passes.
@@ -410,10 +402,9 @@ static int order_build(const char* fn, const DenseSrc& D, const SparseSrc& S, in
         set_error("%s: allocation of %zu bytes for the order (and %zu bytes of temporaries) failed", fn, out_bytes, tmp_bytes);
         return VB_ENOMEM;
     }
-    OrderTmp tmp;
-    if (cudaMalloc(&tmp.mem, tmp_bytes) != cudaSuccess) {
-        cudaGetLastError();
-        tmp.mem = nullptr;
+    Scratch sc;
+    void* tmp;
+    if (sc.own(tmp_bytes, &tmp) != VB_OK) {
         cudaFree(o->mem);
         o->mem = nullptr;
         set_error("%s: allocation of %zu bytes of temporaries (beside %zu bytes for the order) failed", fn, tmp_bytes, out_bytes);
@@ -433,7 +424,7 @@ static int order_build(const char* fn, const DenseSrc& D, const SparseSrc& S, in
         VB_CUDA(cudaStreamSynchronize(st));
         return VB_OK;
     }
-    uint8_t* t = (uint8_t*)tmp.mem;
+    uint8_t* t = (uint8_t*)tmp;
     auto take = [&](size_t b) {
         uint8_t* r = t;
         t += al(b);
@@ -559,8 +550,6 @@ static int launch_bounds(const vb_order* o, bool sparse, const DenseSrc& D, cons
     return VB_OK;
 }
 
-enum { WSO_QUERIES = 0, WSO_BOUNDS = 1 };   // per-call scratch of the host bounds (whole calls on the library stream)
-
 static DenseSrc dense_src(const Table& T) { return DenseSrc{T.d, T.stride, T.elem, T.dim, dense_words(T.elem, T.dim)}; }
 
 static int dense_bounds(vb_order* o, const void* queries, int64_t nq, bool host, int64_t* out_lo, int64_t* out_hi) {
@@ -575,9 +564,10 @@ static int dense_bounds(vb_order* o, const void* queries, int64_t nq, bool host,
     const size_t qbytes = raw_row_bytes(T.elem, T.dim);
     if (!host) return launch_bounds(o, false, D, SparseSrc{}, (const uint8_t*)queries, qbytes, SparseSrc{}, nq, out_lo, out_hi);
     Context& c = ctx();
+    Scratch sc;
     void *d_q, *d_out;
-    VB_TRY(workspace(WSO_QUERIES, qbytes * (size_t)nq, &d_q));
-    VB_TRY(workspace(WSO_BOUNDS, 16 * (size_t)nq, &d_out));
+    VB_TRY(sc.take(qbytes * (size_t)nq, &d_q));
+    VB_TRY(sc.take(16 * (size_t)nq, &d_out));
     int64_t* lo = (int64_t*)d_out;
     int64_t* hi = lo + nq;
     VB_CUDA(cudaMemcpyAsync(d_q, queries, qbytes * (size_t)nq, cudaMemcpyHostToDevice, c.stream));
@@ -597,13 +587,14 @@ static int sparse_bounds(vb_order* o, int q_dim, int64_t nq, const int64_t* q_of
     if (nq == 0) return VB_OK;
     VB_REQUIRE(out_lo && out_hi, "%s: null query / output buffers", fn);
     const SparseCsr T = sparse_table_csr(static_cast<const vb_sparse_table*>(o->owner));
+    Scratch sc;
     SparseCsr Q;
-    VB_TRY(sparse_queries_on_device(T.dim, q_dim, nq, q_off, q_idx, q_val, host, &Q));
+    VB_TRY(sparse_queries_on_device(sc, T.dim, q_dim, nq, q_off, q_idx, q_val, host, &Q));
     const SparseSrc S{T.off, T.idx, T.val}, QS{Q.off, Q.idx, Q.val};
     if (!host) return launch_bounds(o, true, DenseSrc{}, S, nullptr, 0, QS, nq, out_lo, out_hi);
     Context& c = ctx();
     void* d_out;
-    VB_TRY(workspace(WSO_BOUNDS, 16 * (size_t)nq, &d_out));
+    VB_TRY(sc.take(16 * (size_t)nq, &d_out));
     int64_t* lo = (int64_t*)d_out;
     int64_t* hi = lo + nq;
     VB_TRY(launch_bounds(o, true, DenseSrc{}, S, nullptr, 0, QS, nq, lo, hi));

@@ -20,9 +20,6 @@
 
 namespace vb {
 
-// the slots of vb_exact_topk (vb_ivf.cu): both are whole calls on the library stream and never overlap
-enum { WSR_QIMG = 0, WSR_DIST = 1, WSR_CAND = 2, WSR_IDS = 3, WSR_CHUNKS = 4, WSR_SEG = 5, WSR_POS = 6, WSR_OUT = 7 };
-
 constexpr int RERANK_MAX_K = 2048;   // the largest k segment_topk_kernel selects without host-side segment sizes
 
 // One warp per query: ids[q c + j], j < valid_q = the candidates in [0, n), in candidate order.
@@ -107,30 +104,31 @@ static int rerank_impl(vb_table* t, int metric, const void* queries, int64_t nq,
     // sub-batch so the distance array stays under ~1 GiB
     const int64_t bq = std::max<int64_t>(1, std::min<int64_t>(nq, (int64_t)(1ull << 30) / (4 * std::max(c, 1))));
     for (int64_t q0 = 0; q0 < nq; q0 += bq) {
+        Scratch sc;
         const int64_t m = std::min(bq, nq - q0);
         const size_t mc = (size_t)m * c;
         void *qimg, *d_cand, *d_ids, *d_chunks, *d_seg, *d_dist, *d_pos;
         size_t qstride;
-        VB_TRY(upload_queries(T.elem, T.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, host, WSR_QIMG, &qimg, &qstride));
+        VB_TRY(upload_queries(sc, T.elem, T.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, host, &qimg, &qstride));
         if (host) {
-            VB_TRY(workspace(WSR_CAND, sizeof(int64_t) * mc, &d_cand));
+            VB_TRY(sc.take(sizeof(int64_t) * mc, &d_cand));
             if (mc) VB_CUDA(cudaMemcpyAsync(d_cand, cand + (size_t)q0 * c, sizeof(int64_t) * mc, cudaMemcpyHostToDevice, cx.stream));
         } else {
             d_cand = const_cast<int64_t*>(cand) + (size_t)q0 * c;
         }
-        VB_TRY(workspace(WSR_IDS, sizeof(int64_t) * mc, &d_ids));
+        VB_TRY(sc.take(sizeof(int64_t) * mc, &d_ids));
         const int64_t max_chunks = m * ((c + rpc - 1) / rpc);
-        VB_TRY(workspace(WSR_CHUNKS, sizeof(Chunk) * (size_t)max_chunks + 64, &d_chunks));
+        VB_TRY(sc.take(sizeof(Chunk) * (size_t)max_chunks + 64, &d_chunks));
         int* n_chunks = (int*)((Chunk*)d_chunks + max_chunks);
-        VB_TRY(workspace(WSR_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
+        VB_TRY(sc.take((sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
         int64_t* seg_begin = (int64_t*)d_seg;
         int32_t* seg_len = (int32_t*)(seg_begin + m);
         VB_CUDA(cudaMemsetAsync(n_chunks, 0, sizeof(int), cx.stream));
         VB_TRY(launch_rerank_prepare((const int64_t*)d_cand, m, c, n, rpc, (int64_t*)d_ids, seg_begin, seg_len, (Chunk*)d_chunks, n_chunks));
-        VB_TRY(workspace(WSR_DIST, sizeof(float) * mc, &d_dist));
+        VB_TRY(sc.take(sizeof(float) * mc, &d_dist));
         VB_TRY(launch_scan_gather(T, km, qimg, qstride, (const int64_t*)d_ids, (const Chunk*)d_chunks, n_chunks, (int)max_chunks,
                                   (float*)d_dist));
-        VB_TRY(workspace(WSR_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
+        VB_TRY(sc.take((sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
         int32_t* pos = (int32_t*)d_pos;
         float* key = (float*)(pos + (size_t)m * k);
         VB_TRY(launch_segment_topk_v((const float*)d_dist, seg_begin, seg_len, nullptr, nullptr, m, k, pos, key));
@@ -139,7 +137,7 @@ static int rerank_impl(vb_table* t, int metric, const void* queries, int64_t nq,
         double* o_d = nullptr;
         if (host) {
             void* d_out;
-            VB_TRY(workspace(WSR_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
+            VB_TRY(sc.take((sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
             o_ids = (int64_t*)d_out;
             o_d = (double*)(o_ids + (size_t)m * k);
         } else {

@@ -1,5 +1,5 @@
 // vb_runtime.cu -- process-wide runtime of libvecb200: device binding, streams,
-// workspaces, pinned staging, resident row tables, query image upload.
+// scratch, pinned staging, resident row tables, query image upload.
 #include "vb_common.cuh"
 
 #include <cstdarg>
@@ -48,25 +48,55 @@ int require_init() {
     return VB_OK;
 }
 
-int workspace(int slot, size_t bytes, void** out) {
+Scratch::Scratch(const char* fn) : fn_(fn), outer_(ctx().scratch), top_(outer_ ? outer_->top_ : 0) { ctx().scratch = this; }
+
+Scratch::~Scratch() {
     Context& c = ctx();
-    if (bytes == 0) bytes = 16;
-    if (c.ws_bytes[slot] < bytes) {
-        if (c.ws[slot]) {
-            VB_CUDA(cudaStreamSynchronize(c.stream));
-            VB_CUDA(cudaFree(c.ws[slot]));
-            c.ws[slot] = nullptr;
-            c.ws_bytes[slot] = 0;
-        }
-        size_t want = bytes + bytes / 4;  // head-room so steady-state calls stop reallocating
-        cudaError_t e = cudaMalloc(&c.ws[slot], want);
-        if (e != cudaSuccess) {
-            set_error("cudaMalloc(%zu) for workspace %d failed: %s", want, slot, cudaGetErrorString(e));
-            return VB_ENOMEM;
-        }
-        c.ws_bytes[slot] = want;
+    for (void* p : owned_) cudaFreeAsync(p, c.stream);
+    c.scratch = outer_;
+    if (outer_ || c.arena_peak <= c.arena_bytes) return;
+    // the call needed more than the arena holds: grow it to the peak, with head-room so steady-state calls stop
+    // reallocating (after the work that still reads the old arena)
+    cudaStreamSynchronize(c.stream);
+    cudaFree(c.arena);
+    c.arena = nullptr;
+    c.arena_bytes = 0;
+    const size_t want = c.arena_peak + c.arena_peak / 4;
+    if (cudaMalloc(&c.arena, want) == cudaSuccess) {
+        c.arena_bytes = want;
+    } else {
+        // the arena stays empty and forgets the peak: the next call takes one-off allocations and grows the arena to
+        // its own peak, so one oversized call does not make every later one allocate
+        cudaGetLastError();
+        c.arena = nullptr;
+        c.arena_peak = 0;
     }
-    *out = c.ws[slot];
+}
+
+int Scratch::take(size_t bytes, void** out) {
+    Context& c = ctx();
+    if (c.scratch != this) {
+        set_error("%s: scratch taken from an enclosing call while an inner call's scratch is live", fn_ ? fn_ : "libvecb200");
+        return VB_ESTATE;
+    }
+    const size_t end = top_ + ((std::max<size_t>(bytes, 16) + 255) & ~(size_t)255);
+    if (end <= c.arena_bytes) *out = c.arena + top_;
+    else VB_TRY(own(bytes, out));   // (a range that could not be had does not raise the peak)
+    top_ = end;
+    c.arena_peak = std::max(c.arena_peak, end);
+    return VB_OK;
+}
+
+int Scratch::own(size_t bytes, void** out) {
+    void* p = nullptr;
+    const cudaError_t e = cudaMallocAsync(&p, bytes ? bytes : 16, ctx().stream);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        set_error("%s: allocation of %zu bytes of device memory failed: %s", fn_ ? fn_ : "libvecb200", bytes, cudaGetErrorString(e));
+        return VB_ENOMEM;
+    }
+    owned_.push_back(p);
+    *out = p;
     return VB_OK;
 }
 
@@ -201,10 +231,9 @@ __global__ void query_image_kernel(int elem, int dim, const uint8_t* __restrict_
     }
 }
 
-int upload_queries(int elem, int dim, const void* queries, int64_t nq, bool host, int ws_slot, void** out_dev,
+int upload_queries(Scratch& sc, int elem, int dim, const void* queries, int64_t nq, bool host, void** out_dev,
                    size_t* qstride) {
     Context& c = ctx();
-    ++c.query_epoch;
     const size_t raw = raw_row_bytes(elem, dim);
     const size_t pad = padded_row_bytes(elem, dim);
     // image stride: fp32 per element for vector/halfvec (halfvec padded to 8 elements -> 32 B of floats)
@@ -215,7 +244,7 @@ int upload_queries(int elem, int dim, const void* queries, int64_t nq, bool host
         return VB_OK;
     }
     void* d_img;
-    VB_TRY(workspace(ws_slot, img * (size_t)nq + raw * (size_t)nq + 32, &d_img));
+    VB_TRY(sc.take(img * (size_t)nq + raw * (size_t)nq + 32, &d_img));
     uint8_t* d_raw = (uint8_t*)d_img + ((img * (size_t)nq + 15) & ~(size_t)15);
     const uint8_t* src_dev = (const uint8_t*)queries;
     if (host) {
@@ -355,11 +384,9 @@ int vb_shutdown(void) {
     vb::Context& c = vb::ctx();
     if (!c.inited) return VB_OK;
     cudaDeviceSynchronize();
-    for (int i = 0; i < 32; ++i) {
-        if (c.ws[i]) cudaFree(c.ws[i]);
-        c.ws[i] = nullptr;
-        c.ws_bytes[i] = 0;
-    }
+    if (c.arena) cudaFree(c.arena);
+    c.arena = nullptr;
+    c.arena_bytes = c.arena_peak = 0;
     if (c.pinned) cudaFreeHost(c.pinned);
     if (c.pinned2) cudaFreeHost(c.pinned2);
     c.pinned = c.pinned2 = nullptr;

@@ -490,16 +490,15 @@ __global__ void __launch_bounds__(SS_THREADS) slab_select_kernel(const float* __
     }
 }
 
-enum { WSS_FLAG = 30 };
-
 int launch_slab_select(const float* dist, const float* smin, int64_t nq, int probes, const int32_t* probe_lists, const int32_t* cand_off,
                        const int64_t* list_off, int64_t cap, int64_t cap_s, const int64_t* seg_begin, const int32_t* seg_len, int kp,
                        int32_t* out_pos, float* out_key) {
+    Scratch sc;
     if (nq == 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     VB_REQUIRE(kp <= TOPK_MAX_K, "slab selection: k' too large");
     void* d_flag;
-    VB_TRY(workspace(WSS_FLAG, sizeof(int32_t) * (size_t)nq, &d_flag));
+    VB_TRY(sc.take(sizeof(int32_t) * (size_t)nq, &d_flag));
     const size_t smem = (size_t)SS_CAND * 8 + ss_select_smem_bytes(cap_s, probes);
     VB_REQUIRE(smem <= 200 * 1024, "slab selection: %zu bytes of shared memory", smem);
     static size_t attr = 0;
@@ -553,6 +552,7 @@ __global__ void emit_sorted_kernel(const uint64_t* __restrict__ sorted, const in
 int launch_segment_topk_v(const float* keys, const int64_t* seg_begin_dev, const int32_t* seg_len_dev,
                           const int64_t* seg_begin_host, const int32_t* seg_len_host, int64_t nseg, int k,
                           int32_t* out_pos, float* out_key) {
+    Scratch sc;
     if (nseg == 0 || k <= 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     if (k <= TOPK_MAX_K) {
@@ -578,9 +578,9 @@ int launch_segment_topk_v(const float* keys, const int64_t* seg_begin_dev, const
     }
     off[(size_t)nseg] = total;
     void *d_off, *d_in, *d_out, *d_tmp;
-    VB_TRY(workspace(8, sizeof(int64_t) * ((size_t)nseg + 1), &d_off));
-    VB_TRY(workspace(9, sizeof(uint64_t) * (size_t)std::max<int64_t>(total, 1), &d_in));
-    VB_TRY(workspace(10, sizeof(uint64_t) * (size_t)std::max<int64_t>(total, 1), &d_out));
+    VB_TRY(sc.take(sizeof(int64_t) * ((size_t)nseg + 1), &d_off));
+    VB_TRY(sc.take(sizeof(uint64_t) * (size_t)std::max<int64_t>(total, 1), &d_in));
+    VB_TRY(sc.take(sizeof(uint64_t) * (size_t)std::max<int64_t>(total, 1), &d_out));
     VB_CUDA(cudaMemcpyAsync(d_off, off.data(), sizeof(int64_t) * ((size_t)nseg + 1), cudaMemcpyHostToDevice, s));
     VB_CUDA(cudaStreamSynchronize(s));  // off is a stack-owned vector
     int32_t maxlen = 0;
@@ -594,7 +594,7 @@ int launch_segment_topk_v(const float* keys, const int64_t* seg_begin_dev, const
         VB_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_bytes, (const uint64_t*)d_in, (uint64_t*)d_out,
                                                         (int)total, (int)nseg, (const int64_t*)d_off,
                                                         (const int64_t*)d_off + 1, 0, 64, s));
-        VB_TRY(workspace(11, tmp_bytes, &d_tmp));
+        VB_TRY(sc.take(tmp_bytes, &d_tmp));
         VB_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(d_tmp, tmp_bytes, (const uint64_t*)d_in, (uint64_t*)d_out,
                                                         (int)total, (int)nseg, (const int64_t*)d_off,
                                                         (const int64_t*)d_off + 1, 0, 64, s));

@@ -409,9 +409,6 @@ __global__ void sparse_pad_kernel(int64_t total, int64_t* __restrict__ out_ids, 
     out_f[i] = INFINITY;
 }
 
-// workspace slots of this file
-enum { WSP_Q = 20, WSP_ROWS = 21, WSP_OUT = 22, WSP_TMP = 23, WSP_SEG = 24, WSP_POS = 25, WSP_SCAN = 26, WSP_CHECK = 27 };
-
 // ----------------------------------------------------------------------------- CSR validation on the device
 
 // What sparse_check_kernel finds in n device CSR rows, read back in one copy by check_csr_dev.  bad: the first defect as
@@ -485,11 +482,11 @@ static int sparse_check_error(const char* what, unsigned long long bad) {
     return VB_EINVAL;
 }
 
-// Launch the initialisation and the check of n >= 1 device CSR rows into *chk (workspace slot WSP_CHECK); no read.
-static int launch_sparse_check(int dim, int64_t n, const int64_t* off, const int32_t* idx, SparseCheck** chk) {
+// Launch the initialisation and the check of n >= 1 device CSR rows into *chk (a range of sc); no read.
+static int launch_sparse_check(Scratch& sc, int dim, int64_t n, const int64_t* off, const int32_t* idx, SparseCheck** chk) {
     cudaStream_t s = ctx().stream;
     void* d;
-    VB_TRY(workspace(WSP_CHECK, sizeof(SparseCheck), &d));
+    VB_TRY(sc.take(sizeof(SparseCheck), &d));
     *chk = (SparseCheck*)d;
     sparse_check_init_kernel<<<1, 1, 0, s>>>(*chk);
     sparse_check_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(n, off, idx, dim, *chk);
@@ -501,11 +498,12 @@ static int launch_sparse_check(int dim, int64_t n, const int64_t* off, const int
 // check_csr for n >= 1 device CSR rows: one sparse_check_kernel pass and one read of its 24-byte result (which
 // synchronises).  *max_nnz / *total (optional): the largest row nnz and off[n].
 static int check_csr_dev(const char* what, int dim, int64_t n, const int64_t* off, const int32_t* idx, int* max_nnz, int64_t* total) {
+    Scratch sc;
     VB_REQUIRE(dim >= 1 && dim <= SP_MAX_DIM, "sparsevec must have between 1 and %d dimensions", SP_MAX_DIM);
     VB_REQUIRE(off, "%s: offsets must start at 0", what);
     SparseCheck h{~0ull, 0, 0, 0};
     SparseCheck* d;
-    VB_TRY(launch_sparse_check(dim, n, off, idx, &d));
+    VB_TRY(launch_sparse_check(sc, dim, n, off, idx, &d));
     cudaStream_t s = ctx().stream;
     VB_CUDA(cudaMemcpyAsync(&h, d, SPC_READ, cudaMemcpyDeviceToHost, s));
     VB_CUDA(cudaStreamSynchronize(s));
@@ -544,13 +542,13 @@ static int check_csr(const char* what, int dim, int64_t n, const int64_t* off, c
     return VB_OK;
 }
 
-// queries to the device: [off (nq + 1) | idx | val] in one workspace block
-static int upload_sparse_queries(int64_t nq, const int64_t* off, const int32_t* idx, const float* val, SparseQueries* Q) {
+// queries to the device: [off (nq + 1) | idx | val] in one range of sc
+static int upload_sparse_queries(Scratch& sc, int64_t nq, const int64_t* off, const int32_t* idx, const float* val, SparseQueries* Q) {
     const int64_t tot = off[nq];
     const size_t b_off = sizeof(int64_t) * (size_t)(nq + 1);
     const size_t b_idx = (sizeof(int32_t) * (size_t)tot + 15) & ~(size_t)15;
     void* d;
-    VB_TRY(workspace(WSP_Q, b_off + b_idx + sizeof(float) * (size_t)tot + 64, &d));
+    VB_TRY(sc.take(b_off + b_idx + sizeof(float) * (size_t)tot + 64, &d));
     cudaStream_t s = ctx().stream;
     uint8_t* p = (uint8_t*)d;
     VB_CUDA(cudaMemcpyAsync(p, off, b_off, cudaMemcpyHostToDevice, s));
@@ -616,19 +614,19 @@ __global__ void sparse_shift_offsets_kernel(int64_t* off, int64_t n, int64_t add
 }
 
 // queries q0 .. q0 + m of a call's CSR batch to the device, offsets rebased to 0
-static int upload_query_range(int64_t q0, int64_t m, const int64_t* q_off, const int32_t* q_idx, const float* q_val, SparseQueries* Q) {
+static int upload_query_range(Scratch& sc, int64_t q0, int64_t m, const int64_t* q_off, const int32_t* q_idx, const float* q_val, SparseQueries* Q) {
     std::vector<int64_t> off((size_t)m + 1);
     for (int64_t i = 0; i <= m; ++i) off[(size_t)i] = q_off[q0 + i] - q_off[q0];
-    VB_TRY(upload_sparse_queries(m, off.data(), q_idx + q_off[q0], q_val + q_off[q0], Q));
+    VB_TRY(upload_sparse_queries(sc, m, off.data(), q_idx + q_off[q0], q_val + q_off[q0], Q));
     VB_CUDA(cudaStreamSynchronize(ctx().stream));   // `off` is a local vector
     return VB_OK;
 }
 
 // The queries q0 .. q0 + m of a call: host CSR is uploaded (upload_query_range); device CSR is read in place, its
 // offsets absolute into the call's q_idx / q_val (sp_stage reads Q.off[q] .. Q.off[q + 1]), so nothing is copied.
-static int sub_batch_queries(bool host, int64_t q0, int64_t m, const int64_t* q_off, const int32_t* q_idx, const float* q_val,
+static int sub_batch_queries(Scratch& sc, bool host, int64_t q0, int64_t m, const int64_t* q_off, const int32_t* q_idx, const float* q_val,
                              SparseQueries* Q) {
-    if (host) return upload_query_range(q0, m, q_off, q_idx, q_val, Q);
+    if (host) return upload_query_range(sc, q0, m, q_off, q_idx, q_val, Q);
     *Q = SparseQueries{q_off + q0, q_idx, q_val};
     return VB_OK;
 }
@@ -646,9 +644,10 @@ static int sparse_topk_args(vb_sparse_table* h, int metric, int q_dim, int64_t n
 static int sparse_select_finish(int metric, int64_t m, int k, const float* key_runs, const int64_t* seg_begin, const int32_t* seg_len,
                                 const int64_t* rows, const int64_t* seg_rows, int seg_rows_stride, int64_t* out_ids, double* out_dist,
                                 float* out_f = nullptr) {
+    Scratch sc;
     cudaStream_t s = ctx().stream;
     void *d_pos, *d_out;
-    VB_TRY(workspace(WSP_POS, (sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
+    VB_TRY(sc.take((sizeof(int32_t) + sizeof(float)) * (size_t)m * k, &d_pos));
     int32_t* pos = (int32_t*)d_pos;
     float* key = (float*)(pos + (size_t)m * k);
     VB_TRY(launch_segment_topk_v(key_runs, seg_begin, seg_len, nullptr, nullptr, m, k, pos, key));
@@ -659,7 +658,7 @@ static int sparse_select_finish(int metric, int64_t m, int k, const float* key_r
         count_launch();
         return VB_OK;
     }
-    VB_TRY(workspace(WSP_OUT, (sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
+    VB_TRY(sc.take((sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
     int64_t* o_ids = (int64_t*)d_out;
     double* o_d = (double*)(o_ids + (size_t)m * k);
     sparse_finish_kernel<<<(unsigned)((m * k + 255) / 256), 256, 0, s>>>(metric, m * k, k, pos, key, rows, seg_rows, seg_rows_stride, o_ids,
@@ -703,7 +702,7 @@ SparseCsr sparse_table_csr(const vb_sparse_table* h) { return SparseCsr{h->t.dim
 
 uint64_t sparse_table_uid(const vb_sparse_table* h) { return h->uid; }
 
-int sparse_queries_on_device(int dim, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, const float* q_val, bool host,
+int sparse_queries_on_device(Scratch& sc, int dim, int q_dim, int64_t nq, const int64_t* q_off, const int32_t* q_idx, const float* q_val, bool host,
                              SparseCsr* out) {
     VB_REQUIRE(dim == q_dim, "different sparsevec dimensions %d and %d", dim, q_dim);
     VB_REQUIRE(q_off, "null query / output buffers");
@@ -711,7 +710,7 @@ int sparse_queries_on_device(int dim, int q_dim, int64_t nq, const int64_t* q_of
         VB_TRY(check_csr("queries", dim, nq, q_off, q_idx, nullptr));
         VB_REQUIRE(q_off[nq] == 0 || q_val, "null query / output buffers");
         SparseQueries Q;
-        VB_TRY(upload_query_range(0, nq, q_off, q_idx, q_val, &Q));
+        VB_TRY(upload_query_range(sc, 0, nq, q_off, q_idx, q_val, &Q));
         *out = SparseCsr{dim, nq, Q.off, Q.idx, Q.val};
         return VB_OK;
     }
@@ -749,33 +748,35 @@ static int sparse_topk_filtered(vb_sparse_table* h, int metric, int q_dim, int64
                    filter_of_query[q], nfilters - 1);
     Context& c = ctx();
     const SparseTable& t = h->t;
+    Scratch pos;
     std::vector<int64_t> fbase;
     const int64_t* rows;
-    VB_TRY(filter_concat_positions(filters, nfilters, WSP_ROWS, &fbase, &rows));
+    VB_TRY(filter_concat_positions(pos, filters, nfilters, &fbase, &rows));
     const int km = key_metric(metric);
     // host results are staged on the host so that a failing sub-batch leaves the caller's buffers untouched
     std::vector<int64_t> ids(host ? (size_t)(nq * k) : 0);
     std::vector<double> dist(host ? (size_t)(nq * k) : 0);
     FilterBatch b;
     for (int64_t q0 = 0; q0 < nq;) {
+        Scratch sc;
         VB_TRY(filter_batch_plan(filters, nfilters, filter_of_query, fbase.data(), q0, nq, SP_MAX_BATCH, SP_CHUNK_ROWS, 8 * (int64_t)c.sm_count,
                                  &b));
         const int64_t m = (int64_t)b.qa.size();
         const size_t nl = b.launch_count.size();
         SparseQueries Q;
-        VB_TRY(sub_batch_queries(host, q0, m, q_off, q_idx, q_val, &Q));
+        VB_TRY(sub_batch_queries(sc, host, q0, m, q_off, q_idx, q_val, &Q));
         // per-query arguments | segments | chunks of each gather launch
         void *d_qa, *d_chunks, *d_keys;
         const size_t qa_bytes = (sizeof(FilterQuery) * (size_t)m + 255) & ~(size_t)255;
-        VB_TRY(workspace(WSP_SEG, qa_bytes + (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + sizeof(int32_t) * nl + 64, &d_qa));
+        VB_TRY(sc.take(qa_bytes + (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + sizeof(int32_t) * nl + 64, &d_qa));
         int64_t* seg_begin = (int64_t*)((uint8_t*)d_qa + qa_bytes);
         int32_t* seg_len = (int32_t*)(seg_begin + m);
         int32_t* d_count = seg_len + m;
         VB_CUDA(cudaMemcpyAsync(d_qa, b.qa.data(), sizeof(FilterQuery) * (size_t)m, cudaMemcpyHostToDevice, c.stream));
         if (nl) VB_CUDA(cudaMemcpyAsync(d_count, b.launch_count.data(), sizeof(int32_t) * nl, cudaMemcpyHostToDevice, c.stream));
-        VB_TRY(workspace(WSP_SCAN, sizeof(Chunk) * (size_t)b.max_chunks + 64, &d_chunks));
+        VB_TRY(sc.take(sizeof(Chunk) * (size_t)b.max_chunks + 64, &d_chunks));
         VB_TRY(launch_filter_chunks((const FilterQuery*)d_qa, m, SP_CHUNK_ROWS, seg_begin, seg_len, (Chunk*)d_chunks));
-        VB_TRY(workspace(WSP_TMP, sizeof(float) * (size_t)std::max<int64_t>(b.run, 1), &d_keys));
+        VB_TRY(sc.take(sizeof(float) * (size_t)std::max<int64_t>(b.run, 1), &d_keys));
         for (size_t l = 0; l < nl; ++l)
             VB_TRY(launch_sparse_gather(km, t.dim, Q, max_q, t, rows, (const Chunk*)d_chunks + b.launch_begin[l], d_count + l, b.launch_count[l],
                                         (float*)d_keys));
@@ -822,25 +823,26 @@ static int sparse_rerank(vb_sparse_table* h, int metric, int q_dim, int64_t nq, 
     // sub-batches keep the keys under ~1 GiB
     const int64_t bq = std::max<int64_t>(1, std::min<int64_t>(std::min(nq, SP_MAX_BATCH), (int64_t)(1ull << 28) / std::max(c, 1)));
     for (int64_t q0 = 0; q0 < nq; q0 += bq) {
+        Scratch sc;
         const int64_t m = std::min(bq, nq - q0);
         const size_t mc = (size_t)m * c;
         SparseQueries Q;
-        VB_TRY(sub_batch_queries(host, q0, m, q_off, q_idx, q_val, &Q));
+        VB_TRY(sub_batch_queries(sc, host, q0, m, q_off, q_idx, q_val, &Q));
         // candidates (host variant: their copy) | their compaction
         void *d_cand, *d_chunks, *d_seg, *d_keys;
-        VB_TRY(workspace(WSP_ROWS, 2 * sizeof(int64_t) * mc, &d_cand));
+        VB_TRY(sc.take(2 * sizeof(int64_t) * mc, &d_cand));
         int64_t* d_ids = (int64_t*)d_cand + mc;
         if (!host) d_cand = const_cast<int64_t*>(cand) + (size_t)q0 * c;
         else if (mc) VB_CUDA(cudaMemcpyAsync(d_cand, cand + (size_t)q0 * c, sizeof(int64_t) * mc, cudaMemcpyHostToDevice, cx.stream));
         const int64_t max_chunks = m * ((c + SP_CHUNK_ROWS - 1) / SP_CHUNK_ROWS);
-        VB_TRY(workspace(WSP_SCAN, sizeof(Chunk) * (size_t)max_chunks + 64, &d_chunks));
+        VB_TRY(sc.take(sizeof(Chunk) * (size_t)max_chunks + 64, &d_chunks));
         int* n_chunks = (int*)((Chunk*)d_chunks + max_chunks);
-        VB_TRY(workspace(WSP_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
+        VB_TRY(sc.take((sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
         int64_t* seg_begin = (int64_t*)d_seg;
         int32_t* seg_len = (int32_t*)(seg_begin + m);
         VB_CUDA(cudaMemsetAsync(n_chunks, 0, sizeof(int), cx.stream));
         VB_TRY(launch_rerank_prepare((const int64_t*)d_cand, m, c, n, SP_CHUNK_ROWS, d_ids, seg_begin, seg_len, (Chunk*)d_chunks, n_chunks));
-        VB_TRY(workspace(WSP_TMP, sizeof(float) * mc, &d_keys));
+        VB_TRY(sc.take(sizeof(float) * mc, &d_keys));
         VB_TRY(launch_sparse_gather(km, t.dim, Q, max_q, t, d_ids, (const Chunk*)d_chunks, n_chunks, (int)max_chunks, (float*)d_keys));
         // entry p of query j's segment is d_ids[seg_begin[j] + p] (seg_begin[j] = j c)
         VB_TRY(sparse_select_finish(metric, m, k, (const float*)d_keys, seg_begin, seg_len, d_ids, seg_begin, 1,
@@ -885,13 +887,14 @@ static int sparse_exact_topk(vb_sparse_table* h, int metric, int q_dim, int64_t 
     // sub-batches keep the key matrix under ~1 GiB
     const int64_t bq = std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(nq, 65535), (int64_t)(1ull << 30) / (4 * n)));
     for (int64_t q0 = 0; q0 < nq; q0 += bq) {
+        Scratch sc;
         const int64_t m = std::min(bq, nq - q0);
         SparseQueries Q;
-        VB_TRY(sub_batch_queries(host, q0, m, q_off, q_idx, q_val, &Q));
+        VB_TRY(sub_batch_queries(sc, host, q0, m, q_off, q_idx, q_val, &Q));
         void *d_key, *d_seg;
-        VB_TRY(workspace(WSP_TMP, sizeof(float) * (size_t)m * (size_t)n, &d_key));
+        VB_TRY(sc.take(sizeof(float) * (size_t)m * (size_t)n, &d_key));
         VB_TRY(launch_sparse_scan(key_metric(metric), t.dim, Q, m, max_q, t.row_off, t.idx, t.val, n, nullptr, (float*)d_key));
-        VB_TRY(workspace(WSP_SEG, (sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
+        VB_TRY(sc.take((sizeof(int64_t) + sizeof(int32_t)) * (size_t)m + 64, &d_seg));
         int64_t* seg_begin = (int64_t*)d_seg;
         int32_t* seg_len = (int32_t*)(seg_begin + m);
         sparse_segments_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(m, n, seg_begin, seg_len);
@@ -1047,6 +1050,7 @@ static const char* dense_name(int elem) { return elem == VB_VECTOR ? "vector" : 
 // vb_dense_to_sparsevec_batch[_dev]
 static int dense_to_sparse(int elem, int dim, const void* rows, int64_t n, int64_t cap, bool host, int64_t* out_row_off, int32_t* out_idx,
                            float* out_val) {
+    Scratch sc;
     const char* fn = host ? "vb_dense_to_sparsevec_batch" : "vb_dense_to_sparsevec_batch_dev";
     VB_TRY(require_init());
     VB_REQUIRE(elem == VB_VECTOR || elem == VB_HALFVEC, "%s: elem must be VB_VECTOR or VB_HALFVEC, got %d", fn, elem);
@@ -1066,12 +1070,12 @@ static int dense_to_sparse(int elem, int dim, const void* rows, int64_t n, int64
     const size_t b_off = sizeof(int64_t) * (size_t)(n + 1);
     void *d_in = const_cast<void*>(rows), *d_cnt, *d_off = out_row_off, *d_scan, *d_chk;
     if (host) {
-        VB_TRY(workspace(WSP_ROWS, raw * (size_t)n, &d_in));
+        VB_TRY(sc.take(raw * (size_t)n, &d_in));
         VB_CUDA(cudaMemcpyAsync(d_in, rows, raw * (size_t)n, cudaMemcpyHostToDevice, s));
-        VB_TRY(workspace(WSP_SEG, b_off, &d_off));
+        VB_TRY(sc.take(b_off, &d_off));
     }
-    VB_TRY(workspace(WSP_TMP, b_off, &d_cnt));
-    VB_TRY(workspace(WSP_CHECK, sizeof(SparseCheck), &d_chk));
+    VB_TRY(sc.take(b_off, &d_cnt));
+    VB_TRY(sc.take(sizeof(SparseCheck), &d_chk));
     SparseCheck* chk = (SparseCheck*)d_chk;
     int64_t* cnt = (int64_t*)d_cnt;
     int64_t* off = (int64_t*)d_off;
@@ -1083,7 +1087,7 @@ static int dense_to_sparse(int elem, int dim, const void* rows, int64_t n, int64
     VB_CUDA(cudaMemsetAsync(cnt + n, 0, sizeof(int64_t), s));
     size_t scan_bytes = 0;
     VB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, cnt, off, (int)(n + 1), s));
-    VB_TRY(workspace(WSP_SCAN, scan_bytes + 64, &d_scan));
+    VB_TRY(sc.take(scan_bytes + 64, &d_scan));
     VB_CUDA(cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, cnt, off, (int)(n + 1), s));
     count_launch(3);
     VB_CUDA(cudaMemcpyAsync(&chk->total, off + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
@@ -1101,7 +1105,7 @@ static int dense_to_sparse(int elem, int dim, const void* rows, int64_t n, int64
     const size_t b_idx = (sizeof(int32_t) * (size_t)total + 15) & ~(size_t)15;
     if (host) {
         void* d_out;
-        VB_TRY(workspace(WSP_OUT, b_idx + sizeof(float) * (size_t)total, &d_out));
+        VB_TRY(sc.take(b_idx + sizeof(float) * (size_t)total, &d_out));
         o_idx = (int32_t*)d_out;
         o_val = (float*)((uint8_t*)d_out + b_idx);
     }
@@ -1119,6 +1123,7 @@ static int dense_to_sparse(int elem, int dim, const void* rows, int64_t n, int64
 
 // vb_sparsevec_to_dense_batch[_dev]
 static int sparse_to_dense(int elem, int dim, int64_t n, const int64_t* row_off, const int32_t* idx, const float* val, void* out, bool host) {
+    Scratch sc;
     const char* fn = host ? "vb_sparsevec_to_dense_batch" : "vb_sparsevec_to_dense_batch_dev";
     VB_TRY(require_init());
     VB_REQUIRE(elem == VB_VECTOR || elem == VB_HALFVEC, "%s: elem must be VB_VECTOR or VB_HALFVEC, got %d", fn, elem);
@@ -1140,7 +1145,7 @@ static int sparse_to_dense(int elem, int dim, int64_t n, const int64_t* row_off,
         const size_t b_off = sizeof(int64_t) * (size_t)(n + 1);
         const size_t b_idx = (sizeof(int32_t) * (size_t)total + 15) & ~(size_t)15;
         void* d_rows;
-        VB_TRY(workspace(WSP_ROWS, b_off + b_idx + sizeof(float) * (size_t)total + 64, &d_rows));
+        VB_TRY(sc.take(b_off + b_idx + sizeof(float) * (size_t)total + 64, &d_rows));
         uint8_t* p = (uint8_t*)d_rows;
         VB_CUDA(cudaMemcpyAsync(p, row_off, b_off, cudaMemcpyHostToDevice, s));
         if (total > 0) {
@@ -1153,16 +1158,16 @@ static int sparse_to_dense(int elem, int dim, int64_t n, const int64_t* row_off,
     }
     const size_t out_bytes = (elem == VB_VECTOR ? sizeof(float) : sizeof(__half)) * (size_t)n * (size_t)dim;
     void* d_out = out;
-    if (host) VB_TRY(workspace(WSP_OUT, out_bytes, &d_out));
+    if (host) VB_TRY(sc.take(out_bytes, &d_out));
     SparseCheck* chk;
     if (host) {   // validated above: only the overflow word is needed
         void* d;
-        VB_TRY(workspace(WSP_CHECK, sizeof(SparseCheck), &d));
+        VB_TRY(sc.take(sizeof(SparseCheck), &d));
         chk = (SparseCheck*)d;
         sparse_check_init_kernel<<<1, 1, 0, s>>>(chk);
         count_launch();
     } else {
-        VB_TRY(launch_sparse_check(dim, n, d_off, d_idx, &chk));
+        VB_TRY(launch_sparse_check(sc, dim, n, d_off, d_idx, &chk));
     }
     const unsigned grid = (unsigned)((n * 32 + 255) / 256);
     if (elem == VB_VECTOR) sparse_to_dense_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(n, d_off, d_idx, d_val, dim, d_out, chk);
@@ -1197,6 +1202,7 @@ extern "C" {
 
 int vb_sparsevec_distance_batch(int metric, int dim, int q_dim, int32_t q_nnz, const int32_t* q_idx, const float* q_val, int64_t n,
                                 const int64_t* row_off, const int32_t* idx, const float* val, double* out) {
+    Scratch sc;
     VB_TRY(require_init());
     VB_REQUIRE(sparse_metric_ok(metric), "metric %d is not defined for sparsevec", metric);
     VB_REQUIRE(n >= 0 && (n == 0 || (row_off && out)), "bad sparsevec batch arguments");
@@ -1213,13 +1219,13 @@ int vb_sparsevec_distance_batch(int metric, int dim, int q_dim, int32_t q_nnz, c
     VB_TRY(check_csr("query", dim, 1, qoff, q_idx, &max_q));
     Context& c = ctx();
     SparseQueries Q;
-    VB_TRY(upload_sparse_queries(1, qoff, q_idx, q_val, &Q));
+    VB_TRY(upload_sparse_queries(sc, 1, qoff, q_idx, q_val, &Q));
     const int64_t tot = row_off[n];
     const size_t b_off = sizeof(int64_t) * (size_t)(n + 1);
     const size_t b_idx = (sizeof(int32_t) * (size_t)tot + 15) & ~(size_t)15;
     void *d_rows, *d_out;
-    VB_TRY(workspace(WSP_ROWS, b_off + b_idx + sizeof(float) * (size_t)tot + 64, &d_rows));
-    VB_TRY(workspace(WSP_OUT, sizeof(double) * (size_t)n, &d_out));
+    VB_TRY(sc.take(b_off + b_idx + sizeof(float) * (size_t)tot + 64, &d_rows));
+    VB_TRY(sc.take(sizeof(double) * (size_t)n, &d_out));
     uint8_t* p = (uint8_t*)d_rows;
     VB_CUDA(cudaMemcpyAsync(p, row_off, b_off, cudaMemcpyHostToDevice, c.stream));
     if (tot > 0) {
@@ -1234,6 +1240,7 @@ int vb_sparsevec_distance_batch(int metric, int dim, int q_dim, int32_t q_nnz, c
 }
 
 int vb_sparsevec_norm_batch(int64_t n, const int64_t* row_off, const float* val, double* out) {
+    Scratch sc;
     VB_TRY(require_init());
     VB_REQUIRE(n >= 0 && (n == 0 || (row_off && out && row_off[0] == 0)), "bad sparsevec norm arguments");
     if (n == 0) return VB_OK;
@@ -1242,8 +1249,8 @@ int vb_sparsevec_norm_batch(int64_t n, const int64_t* row_off, const float* val,
     const int64_t tot = row_off[n];
     const size_t b_off = sizeof(int64_t) * (size_t)(n + 1);
     void *d_rows, *d_out;
-    VB_TRY(workspace(WSP_ROWS, b_off + sizeof(float) * (size_t)tot + 64, &d_rows));
-    VB_TRY(workspace(WSP_OUT, sizeof(double) * (size_t)n, &d_out));
+    VB_TRY(sc.take(b_off + sizeof(float) * (size_t)tot + 64, &d_rows));
+    VB_TRY(sc.take(sizeof(double) * (size_t)n, &d_out));
     uint8_t* p = (uint8_t*)d_rows;
     VB_CUDA(cudaMemcpyAsync(p, row_off, b_off, cudaMemcpyHostToDevice, c.stream));
     if (tot > 0) VB_CUDA(cudaMemcpyAsync(p + b_off, val, sizeof(float) * (size_t)tot, cudaMemcpyHostToDevice, c.stream));
@@ -1258,6 +1265,7 @@ int vb_sparsevec_norm_batch(int64_t n, const int64_t* row_off, const float* val,
 
 int vb_sparsevec_l2_normalize_batch(int64_t n, const int64_t* row_off, const int32_t* idx, const float* val, int64_t* out_row_off,
                                     int32_t* out_idx, float* out_val) {
+    Scratch sc;
     VB_TRY(require_init());
     VB_REQUIRE(n >= 0 && (n == 0 || (row_off && out_row_off && row_off[0] == 0)), "bad sparsevec normalize arguments");
     if (n == 0) {
@@ -1273,10 +1281,10 @@ int vb_sparsevec_l2_normalize_batch(int64_t n, const int64_t* row_off, const int
     const size_t b_idx = (sizeof(int32_t) * (size_t)tot + 15) & ~(size_t)15;
     const size_t b_val = (sizeof(float) * (size_t)tot + 15) & ~(size_t)15;
     void *d_rows, *d_tmp, *d_outb, *d_scan;
-    VB_TRY(workspace(WSP_ROWS, b_off + b_idx + b_val + 64, &d_rows));
+    VB_TRY(sc.take(b_off + b_idx + b_val + 64, &d_rows));
     // tmp: quotients | kept[n + 1] | out_off[n + 1] | overflow flag
-    VB_TRY(workspace(WSP_TMP, b_val + 2 * b_off + 64, &d_tmp));
-    VB_TRY(workspace(WSP_OUT, b_idx + b_val + 64, &d_outb));
+    VB_TRY(sc.take(b_val + 2 * b_off + 64, &d_tmp));
+    VB_TRY(sc.take(b_idx + b_val + 64, &d_outb));
     uint8_t* p = (uint8_t*)d_rows;
     uint8_t* t = (uint8_t*)d_tmp;
     float* d_q = (float*)t;
@@ -1296,7 +1304,7 @@ int vb_sparsevec_l2_normalize_batch(int64_t n, const int64_t* row_off, const int
     count_launch();
     size_t scan_bytes = 0;
     VB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_kept, d_ooff, (int)(n + 1), s));
-    VB_TRY(workspace(WSP_SCAN, scan_bytes + 64, &d_scan));
+    VB_TRY(sc.take(scan_bytes + 64, &d_scan));
     VB_CUDA(cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, d_kept, d_ooff, (int)(n + 1), s));
     count_launch();
     uint8_t* o = (uint8_t*)d_outb;

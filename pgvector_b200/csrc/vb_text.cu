@@ -18,9 +18,10 @@ int offsets_from_counts(const int64_t* count, int64_t n, int64_t* row_off) {
     if (n == 0) return VB_OK;
     size_t tb = 0;
     VB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, count, row_off + 1, n, s));
-    DevBuf tmp;
-    VB_TRY(tmp.alloc(tb));
-    VB_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, count, row_off + 1, n, s));
+    Scratch sc("type I/O");
+    void* tmp = nullptr;
+    VB_TRY(sc.own(tb, &tmp));
+    VB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tb, count, row_off + 1, n, s));
     count_launch();
     return VB_OK;
 }
@@ -587,9 +588,10 @@ int dense_parse_enqueue(int elem, int32_t typmod, int64_t n, const char* text, c
 
 int dense_parse_dev(int elem, int32_t typmod, int64_t n, const char* text, const int64_t* off, const int64_t* row_off,
                     void* out, int64_t* out_bad, int64_t bad_base) {
-    DevBuf st;
-    VB_TRY(st.alloc(sizeof(Status)));
-    Status* sp = static_cast<Status*>(st.p);
+    Scratch sc("type I/O");
+    void* st = nullptr;
+    VB_TRY(sc.own(sizeof(Status), &st));
+    Status* sp = static_cast<Status*>(st);
     VB_TRY(dense_parse_enqueue(elem, typmod, n, text, off, row_off, out, sp));
     return finish(elem == VB_VECTOR ? 0 : 1, typmod, text, sp, out_bad, bad_base);
 }
@@ -615,13 +617,14 @@ int sparse_parse_dev(int32_t typmod, int64_t n, const char* text, const int64_t*
                      int64_t* out_row_off, int32_t* out_idx, float* out_val, int64_t* out_bad, int64_t bad_base,
                      int64_t* total_out) {
     cudaStream_t s = ctx().stream;
-    DevBuf cnt, slot_off, st;
-    VB_TRY(cnt.alloc(sizeof(int64_t) * (size_t)n));
-    VB_TRY(slot_off.alloc(sizeof(int64_t) * (size_t)(n + 1)));
-    VB_TRY(st.alloc(sizeof(Status)));
-    int64_t* cp = static_cast<int64_t*>(cnt.p);
-    int64_t* so = static_cast<int64_t*>(slot_off.p);
-    Status* sp = static_cast<Status*>(st.p);
+    Scratch sc("type I/O");
+    void *cnt = nullptr, *slot_off = nullptr, *st = nullptr;
+    VB_TRY(sc.own(sizeof(int64_t) * (size_t)n, &cnt));
+    VB_TRY(sc.own(sizeof(int64_t) * (size_t)(n + 1), &slot_off));
+    VB_TRY(sc.own(sizeof(Status), &st));
+    int64_t* cp = static_cast<int64_t*>(cnt);
+    int64_t* so = static_cast<int64_t*>(slot_off);
+    Status* sp = static_cast<Status*>(st);
     if (n) text_count_kernel<<<grid_for(n), kWarps * 32, 0, s>>>(text, off, n, cp);
     VB_CUDA(cudaGetLastError());
     VB_TRY(offsets_from_counts(cp, n, so));
@@ -642,11 +645,11 @@ int sparse_parse_dev(int32_t typmod, int64_t n, const char* text, const int64_t*
     // the segmented sort counts entries in int
     VB_REQUIRE(bound <= INT32_MAX, "sparsevec_in: the literals need up to %lld entries, more than %d in one call",
                (long long)bound, INT32_MAX);
-    DevBuf sidx, sval;
-    VB_TRY(sidx.alloc(sizeof(int32_t) * (size_t)bound));
-    VB_TRY(sval.alloc(sizeof(float) * (size_t)bound));
-    int32_t* si = static_cast<int32_t*>(sidx.p);
-    float* sv = static_cast<float*>(sval.p);
+    void *sidx = nullptr, *sval = nullptr;
+    VB_TRY(sc.own(sizeof(int32_t) * (size_t)bound, &sidx));
+    VB_TRY(sc.own(sizeof(float) * (size_t)bound, &sval));
+    int32_t* si = static_cast<int32_t*>(sidx);
+    float* sv = static_cast<float*>(sval);
     const Status init = fresh_status();
     VB_CUDA(cudaMemcpyAsync(sp, &init, sizeof(Status), cudaMemcpyHostToDevice, s));
     {
@@ -671,9 +674,10 @@ int sparse_parse_dev(int32_t typmod, int64_t n, const char* text, const int64_t*
         size_t tb = 0;
         VB_CUDA(cub::DeviceSegmentedSort::StableSortPairs(nullptr, tb, si, out_idx, sv, out_val, (int)nnz, (int)n,
                                                           out_row_off, out_row_off + 1, s));
-        DevBuf tmp;
-        VB_TRY(tmp.alloc(tb));
-        VB_CUDA(cub::DeviceSegmentedSort::StableSortPairs(tmp.p, tb, si, out_idx, sv, out_val, (int)nnz, (int)n,
+        Scratch sc("type I/O");
+        void* tmp = nullptr;
+        VB_TRY(sc.own(tb, &tmp));
+        VB_CUDA(cub::DeviceSegmentedSort::StableSortPairs(tmp, tb, si, out_idx, sv, out_val, (int)nnz, (int)n,
                                                           out_row_off, out_row_off + 1, s));
         sparse_check_kernel<<<grid_for(n), kWarps * 32, 0, s>>>(n, out_row_off, out_idx, out_dim, true, sp);
         VB_CUDA(cudaGetLastError());
@@ -707,9 +711,10 @@ int format_dev(bool sparse, int elem, int dim, const void* rows, int64_t n, cons
                int64_t cap, int64_t* out_off, char* out, int64_t* total_out) {
     cudaStream_t s = ctx().stream;
     if (sparse && n) VB_TRY(sparse_csr_check_dev("sparsevec_out", dim, n, row_off, idx));
-    DevBuf len;
-    VB_TRY(len.alloc(sizeof(int64_t) * (size_t)n));
-    int64_t* lp = static_cast<int64_t*>(len.p);
+    Scratch sc("type I/O");
+    void* len = nullptr;
+    VB_TRY(sc.own(sizeof(int64_t) * (size_t)n, &len));
+    int64_t* lp = static_cast<int64_t*>(len);
     {
         ProfScope prof(VB_PROF_TEXT_FORMAT);
         if (n) {
@@ -755,11 +760,12 @@ int vb_text_to_rows_batch_dev(int elem, int32_t typmod, int64_t n, const char* t
     if (typmod >= 1) {
         typmod_offsets_kernel<<<grid_for(n + 1), 256, 0, s>>>(n, typmod, out_row_off);
     } else {
-        DevBuf cnt;
-        VB_TRY(cnt.alloc(sizeof(int64_t) * (size_t)n));
-        if (n) text_count_kernel<<<grid_for(n), kWarps * 32, 0, s>>>(text, off, n, static_cast<int64_t*>(cnt.p));
+        Scratch sc("type I/O");
+        void* cnt = nullptr;
+        VB_TRY(sc.own(sizeof(int64_t) * (size_t)n, &cnt));
+        if (n) text_count_kernel<<<grid_for(n), kWarps * 32, 0, s>>>(text, off, n, static_cast<int64_t*>(cnt));
         VB_CUDA(cudaGetLastError());
-        VB_TRY(offsets_from_counts(static_cast<int64_t*>(cnt.p), n, out_row_off));
+        VB_TRY(offsets_from_counts(static_cast<int64_t*>(cnt), n, out_row_off));
     }
     VB_CUDA(cudaGetLastError());
     count_launch();
@@ -810,14 +816,15 @@ int vb_text_to_rows_batch(int elem, int32_t typmod, int64_t n, const char* text,
     const size_t tb_al = ((size_t)max_tb + 15) & ~(size_t)15;
     const size_t in_bytes = tb_al + sizeof(int64_t) * 2 * (size_t)(max_nr + 1);
     const size_t out_bytes = sizeof(Status) + esz * (size_t)max_ne;
-    DevBuf dtext[2], doff[2], dout[2], dst[2];
+    Scratch sc("type I/O");
+    void *dtext[2] = {}, *doff[2] = {}, *dout[2] = {}, *dst[2] = {};
     for (int k = 0; k < 2 && k < nch; ++k) {
         VB_TRY(pinned_grow(&sg.in[k], &sg.in_bytes[k], in_bytes));
         VB_TRY(pinned_grow(&sg.out[k], &sg.out_bytes[k], out_bytes));
-        VB_TRY(dtext[k].alloc((size_t)max_tb));
-        VB_TRY(doff[k].alloc(sizeof(int64_t) * 2 * (size_t)(max_nr + 1)));
-        VB_TRY(dout[k].alloc(esz * (size_t)max_ne));
-        VB_TRY(dst[k].alloc(sizeof(Status)));
+        VB_TRY(sc.own((size_t)max_tb, &dtext[k]));
+        VB_TRY(sc.own(sizeof(int64_t) * 2 * (size_t)(max_nr + 1), &doff[k]));
+        VB_TRY(sc.own(esz * (size_t)max_ne, &dout[k]));
+        VB_TRY(sc.own(sizeof(Status), &dst[k]));
     }
     auto enqueue = [&](int64_t c, int k) -> int {
         const int64_t r0 = cuts[c], r1 = cuts[c + 1];
@@ -829,13 +836,13 @@ int vb_text_to_rows_batch(int elem, int32_t typmod, int64_t n, const char* text,
             poff[i] = off[r0 + i] - off[r0];
             poff[nr + 1 + i] = out_row_off[r0 + i] - out_row_off[r0];
         }
-        VB_CUDA(cudaMemcpyAsync(dtext[k].p, ptext, (size_t)tb, cudaMemcpyHostToDevice, s));
-        VB_CUDA(cudaMemcpyAsync(doff[k].p, poff, sizeof(int64_t) * 2 * (size_t)(nr + 1), cudaMemcpyHostToDevice, s));
-        const int64_t* doffp = static_cast<int64_t*>(doff[k].p);
-        Status* sp = static_cast<Status*>(dst[k].p);
-        VB_TRY(dense_parse_enqueue(elem, typmod, nr, static_cast<char*>(dtext[k].p), doffp, doffp + nr + 1, dout[k].p, sp));
+        VB_CUDA(cudaMemcpyAsync(dtext[k], ptext, (size_t)tb, cudaMemcpyHostToDevice, s));
+        VB_CUDA(cudaMemcpyAsync(doff[k], poff, sizeof(int64_t) * 2 * (size_t)(nr + 1), cudaMemcpyHostToDevice, s));
+        const int64_t* doffp = static_cast<int64_t*>(doff[k]);
+        Status* sp = static_cast<Status*>(dst[k]);
+        VB_TRY(dense_parse_enqueue(elem, typmod, nr, static_cast<char*>(dtext[k]), doffp, doffp + nr + 1, dout[k], sp));
         VB_CUDA(cudaMemcpyAsync(sg.out[k], sp, sizeof(Status), cudaMemcpyDeviceToHost, s));
-        VB_CUDA(cudaMemcpyAsync(static_cast<char*>(sg.out[k]) + sizeof(Status), dout[k].p, esz * (size_t)ne,
+        VB_CUDA(cudaMemcpyAsync(static_cast<char*>(sg.out[k]) + sizeof(Status), dout[k], esz * (size_t)ne,
                                 cudaMemcpyDeviceToHost, s));
         return VB_OK;
     };
@@ -892,24 +899,25 @@ int vb_text_to_sparsevec_batch(int32_t typmod, int64_t n, const char* text, cons
         int64_t* poff = reinterpret_cast<int64_t*>(ptext + ((tb + 15) & ~(int64_t)15));
         std::memcpy(ptext, text + off[r0], (size_t)tb);
         for (int64_t i = 0; i <= nr; ++i) poff[i] = off[r0 + i] - off[r0];
-        DevBuf dtext, doff, ddim, drow, didx, dval;
-        VB_TRY(dtext.alloc((size_t)tb));
-        VB_TRY(doff.alloc(sizeof(int64_t) * (size_t)(nr + 1)));
-        VB_TRY(ddim.alloc(sizeof(int32_t) * (size_t)nr));
-        VB_TRY(drow.alloc(sizeof(int64_t) * (size_t)(nr + 1)));
-        VB_TRY(didx.alloc(sizeof(int32_t) * (size_t)bound));
-        VB_TRY(dval.alloc(sizeof(float) * (size_t)bound));
-        VB_CUDA(cudaMemcpyAsync(dtext.p, ptext, (size_t)tb, cudaMemcpyHostToDevice, s));
-        VB_CUDA(cudaMemcpyAsync(doff.p, poff, sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyHostToDevice, s));
-        VB_TRY(sparse_parse_dev(typmod, nr, static_cast<char*>(dtext.p), static_cast<int64_t*>(doff.p), bound,
-                                static_cast<int32_t*>(ddim.p), static_cast<int64_t*>(drow.p), static_cast<int32_t*>(didx.p),
-                                static_cast<float*>(dval.p), out_bad, r0, nullptr));
+        Scratch sc("type I/O");
+        void *dtext = nullptr, *doff = nullptr, *ddim = nullptr, *drow = nullptr, *didx = nullptr, *dval = nullptr;
+        VB_TRY(sc.own((size_t)tb, &dtext));
+        VB_TRY(sc.own(sizeof(int64_t) * (size_t)(nr + 1), &doff));
+        VB_TRY(sc.own(sizeof(int32_t) * (size_t)nr, &ddim));
+        VB_TRY(sc.own(sizeof(int64_t) * (size_t)(nr + 1), &drow));
+        VB_TRY(sc.own(sizeof(int32_t) * (size_t)bound, &didx));
+        VB_TRY(sc.own(sizeof(float) * (size_t)bound, &dval));
+        VB_CUDA(cudaMemcpyAsync(dtext, ptext, (size_t)tb, cudaMemcpyHostToDevice, s));
+        VB_CUDA(cudaMemcpyAsync(doff, poff, sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyHostToDevice, s));
+        VB_TRY(sparse_parse_dev(typmod, nr, static_cast<char*>(dtext), static_cast<int64_t*>(doff), bound,
+                                static_cast<int32_t*>(ddim), static_cast<int64_t*>(drow), static_cast<int32_t*>(didx),
+                                static_cast<float*>(dval), out_bad, r0, nullptr));
         std::vector<int64_t> rows((size_t)nr + 1);
-        VB_CUDA(cudaMemcpy(rows.data(), drow.p, sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyDeviceToHost));
+        VB_CUDA(cudaMemcpy(rows.data(), drow, sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyDeviceToHost));
         const int64_t nz = rows[(size_t)nr];
-        VB_CUDA(cudaMemcpy(out_dim + r0, ddim.p, sizeof(int32_t) * (size_t)nr, cudaMemcpyDeviceToHost));
-        VB_CUDA(cudaMemcpy(out_idx + done_nnz, didx.p, sizeof(int32_t) * (size_t)nz, cudaMemcpyDeviceToHost));
-        VB_CUDA(cudaMemcpy(out_val + done_nnz, dval.p, sizeof(float) * (size_t)nz, cudaMemcpyDeviceToHost));
+        VB_CUDA(cudaMemcpy(out_dim + r0, ddim, sizeof(int32_t) * (size_t)nr, cudaMemcpyDeviceToHost));
+        VB_CUDA(cudaMemcpy(out_idx + done_nnz, didx, sizeof(int32_t) * (size_t)nz, cudaMemcpyDeviceToHost));
+        VB_CUDA(cudaMemcpy(out_val + done_nnz, dval, sizeof(float) * (size_t)nz, cudaMemcpyDeviceToHost));
         // out_row_off[r0] is already final (earlier chunks); the bound offsets past it become the stored ones
         for (int64_t i = 1; i <= nr; ++i) out_row_off[r0 + i] = done_nnz + rows[(size_t)i];
         done_nnz += nz;
@@ -961,37 +969,38 @@ static int rows_to_text_host(bool sparse, int elem, int dim, const void* rows, i
         for (size_t c = 0; c + 1 < cuts.size(); ++c) {
             const int64_t r0 = cuts[c], r1 = cuts[c + 1];
             const int64_t nr = r1 - r0, ne = first(r1) - first(r0);
-            DevBuf drows, didx, droff, doff, dtext;
-            VB_TRY(drows.alloc(esz * (size_t)ne));
-            VB_CUDA(cudaMemcpyAsync(drows.p, static_cast<const char*>(rows) + esz * (size_t)first(r0), esz * (size_t)ne,
+            Scratch sc("type I/O");
+            void *drows = nullptr, *didx = nullptr, *droff = nullptr, *doff = nullptr, *dtext = nullptr;
+            VB_TRY(sc.own(esz * (size_t)ne, &drows));
+            VB_CUDA(cudaMemcpyAsync(drows, static_cast<const char*>(rows) + esz * (size_t)first(r0), esz * (size_t)ne,
                                     cudaMemcpyHostToDevice, s));
             const int64_t* rp = nullptr;
             if (sparse) {
-                VB_TRY(didx.alloc(sizeof(int32_t) * (size_t)ne));
-                VB_TRY(droff.alloc(sizeof(int64_t) * (size_t)(nr + 1)));
+                VB_TRY(sc.own(sizeof(int32_t) * (size_t)ne, &didx));
+                VB_TRY(sc.own(sizeof(int64_t) * (size_t)(nr + 1), &droff));
                 std::vector<int64_t> ro((size_t)nr + 1);
                 for (int64_t i = 0; i <= nr; ++i) ro[(size_t)i] = row_off[r0 + i] - row_off[r0];
-                VB_CUDA(cudaMemcpyAsync(didx.p, idx + row_off[r0], sizeof(int32_t) * (size_t)ne, cudaMemcpyHostToDevice, s));
-                VB_CUDA(cudaMemcpy(droff.p, ro.data(), sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyHostToDevice));
-                rp = static_cast<int64_t*>(droff.p);
+                VB_CUDA(cudaMemcpyAsync(didx, idx + row_off[r0], sizeof(int32_t) * (size_t)ne, cudaMemcpyHostToDevice, s));
+                VB_CUDA(cudaMemcpy(droff, ro.data(), sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyHostToDevice));
+                rp = static_cast<int64_t*>(droff);
             }
-            VB_TRY(doff.alloc(sizeof(int64_t) * (size_t)(nr + 1)));
-            int64_t* dop = static_cast<int64_t*>(doff.p);
+            VB_TRY(sc.own(sizeof(int64_t) * (size_t)(nr + 1), &doff));
+            int64_t* dop = static_cast<int64_t*>(doff);
             std::vector<int64_t> o((size_t)nr + 1);
             if (pass == 0) {
-                VB_TRY(format_dev(sparse, elem, dim, drows.p, nr, rp, static_cast<int32_t*>(didx.p), INT64_MAX, dop, nullptr, nullptr));
+                VB_TRY(format_dev(sparse, elem, dim, drows, nr, rp, static_cast<int32_t*>(didx), INT64_MAX, dop, nullptr, nullptr));
                 VB_CUDA(cudaMemcpy(o.data(), dop, sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyDeviceToHost));
                 for (int64_t i = 1; i <= nr; ++i) out_off[r0 + i] = out_off[r0] + o[(size_t)i];
             } else {
                 const int64_t tb = out_off[r1] - out_off[r0];
                 for (int64_t i = 0; i <= nr; ++i) o[(size_t)i] = out_off[r0 + i] - out_off[r0];
                 VB_CUDA(cudaMemcpy(dop, o.data(), sizeof(int64_t) * (size_t)(nr + 1), cudaMemcpyHostToDevice));
-                VB_TRY(dtext.alloc((size_t)tb));
-                VB_TRY(format_write(sparse, elem, dim, drows.p, nr, rp, static_cast<int32_t*>(didx.p), dop,
-                                    static_cast<char*>(dtext.p)));
+                VB_TRY(sc.own((size_t)tb, &dtext));
+                VB_TRY(format_write(sparse, elem, dim, drows, nr, rp, static_cast<int32_t*>(didx), dop,
+                                    static_cast<char*>(dtext)));
                 void* pin;
                 VB_TRY(pinned_buffer2((size_t)tb + 16, &pin));
-                VB_CUDA(cudaMemcpyAsync(pin, dtext.p, (size_t)tb, cudaMemcpyDeviceToHost, s));
+                VB_CUDA(cudaMemcpyAsync(pin, dtext, (size_t)tb, cudaMemcpyDeviceToHost, s));
                 VB_CUDA(cudaStreamSynchronize(s));
                 std::memcpy(out + out_off[r0], pin, (size_t)tb);
             }

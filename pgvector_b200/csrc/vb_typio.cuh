@@ -1,23 +1,10 @@
-// vb_typio.cuh -- host machinery the type I/O calls share (vb_text.cu, vb_binary.cu): stream-ordered scratch buffers,
-// offsets from per-row counts, and the two-slot pinned staging that pipelines the host variants.
+// vb_typio.cuh -- host machinery the type I/O calls share (vb_text.cu, vb_binary.cu): offsets from per-row
+// counts, and the two-slot pinned staging that pipelines the host variants.
 #pragma once
 
 #include "vb_common.cuh"
 
 namespace vb {
-
-// device buffer freed at scope exit (stream-ordered)
-struct DevBuf {
-    void* p = nullptr;
-    ~DevBuf() { if (p) cudaFreeAsync(p, ctx().stream); }
-    int alloc(size_t bytes) {
-        if (cudaMallocAsync(&p, bytes ? bytes : 16, ctx().stream) != cudaSuccess) {
-            set_error("cudaMallocAsync(%zu) for the type I/O call failed", bytes);
-            return VB_ENOMEM;
-        }
-        return VB_OK;
-    }
-};
 
 // row_off[0] = 0, row_off[1 + i] = sum of count[0 .. i] (device arrays, on the library stream)
 int offsets_from_counts(const int64_t* count, int64_t n, int64_t* row_off);
