@@ -239,12 +239,40 @@ int			vb_concat_batch(int elem, int dim_a, const void *a, int64_t na, int dim_b,
  *            "\"<float>\" is out of range for type halfvec"; only when there is none, the check pass: "NaN not allowed
  *            in halfvec" / "infinite value not allowed in halfvec".  So in one row a range error beats an earlier NaN.
  * On a data error out is unspecified.  The array structure checks ("array must be 1-D", "array must not contain
- * nulls", "unsupported array type") and numeric[] stay with the caller, which unpacks the ArrayType.
+ * nulls", "unsupported array type") stay with the caller, which unpacks the ArrayType; numeric[] sources go to
+ * vb_numeric_array_to_rows_batch.
  */
 #define VB_ARRAY_INT4 0			/* integer[]          : (float) int32  */
 #define VB_ARRAY_FLOAT4 1		/* real[]             : as is          */
 #define VB_ARRAY_FLOAT8 2		/* double precision[] : (float) double */
+#define VB_ARRAY_NUMERIC 3		/* numeric[]: one numeric_send field per element (vb_numeric_array_to_rows_batch,
+								 * vb_array_to_sparsevec_batch; vb_array_to_rows_batch refuses it) */
 int			vb_array_to_rows_batch(int elem, int src, int dim, int32_t typmod, const void *in, int64_t n, void *out);
+/*
+ * The numeric[] branch of array_to_vector / array_to_halfvec: n rows of dim numeric elements, element i of row r the
+ * field e = r * dim + i at bytes[off[e] .. off[e + 1]) (any alignment; off[n * dim + 1], 8-byte aligned).  A field is
+ * what PostgreSQL's numeric_send writes: big-endian int16 ndigits, int16 weight, uint16 sign, uint16 dscale, then
+ * ndigits base-10000 int16 digits.  These rules are PostgreSQL core's (numeric.c, float.c), not pgvector's:
+ *   - a field is first checked as numeric_recv reads it; a malformed one is refused with VB_EINVAL before any data
+ *     error, naming the field: "insufficient data left in message" (a read past its end), "invalid sign in external
+ *     "numeric" value", "invalid scale in external "numeric" value" (dscale > 0x3FFF), "invalid digit in external
+ *     "numeric" value" (a digit >= 10000), "incorrect binary data format" (bytes left over, as COPY reports them);
+ *   - each element becomes numeric_float4 of it: NaN and +-Infinity as themselves; a finite value is float4in of the
+ *     decimal numeric_out prints (digits past dscale fraction digits truncated, zero as "0", so +0), which is glibc
+ *     strtof, correctly rounded; when strtof's result is 0 or infinite from a value that is not, float4in fails with
+ *     ""<numeric_out text>" is out of range for type real" (a subnormal result is kept);
+ *   - vector converts the whole row, then CheckElement: a range error at element 9 beats a NaN at element 2;
+ *     halfvec runs numeric_float4 and then Float4ToHalf on each element in turn (""65520" is out of range for type
+ *     halfvec"), then CheckElement.
+ * The dimension checks and the lowest-failing-row rule are vb_array_to_rows_batch's.  *out_bad (optional) is the failing
+ * row, or -1.  The host variant streams chunks of whole rows (about 32 MB of fields and offsets; a longer row alone)
+ * through pinned staging.  The _dev variant reads back 16 bytes (the first-offender key and the first malformed field)
+ * and, on an error only, the offending field for its text.
+ */
+int			vb_numeric_array_to_rows_batch(int elem, int dim, int32_t typmod, const void *bytes, const int64_t *off, int64_t n,
+										   void *out, int64_t *out_bad);
+int			vb_numeric_array_to_rows_batch_dev(int elem, int dim, int32_t typmod, const void *bytes_dev, const int64_t *off_dev,
+											   int64_t n, void *out_dev, int64_t *out_bad);
 /*
  * The same on device rows.  Each result equals its host variant's bit for bit.  Refused before any launch (VB_EINVAL):
  * a bad elem, op or src, a dimension <= 0, a negative count, a NULL pointer for work that exists, rows or output not
@@ -515,6 +543,34 @@ int			vb_sparse_table_rerank_dev(vb_sparse_table *t, int metric, int q_dim, int6
  * Host variants synchronise.  _dev variants read back one result of at most 24 bytes (to sparsevec: the nnz check and
  * the total) or 32 bytes (to dense: the CSR check and the first overflowing entry; on that error 4 more bytes, the value).
  */
+/*
+ * array_to_sparsevec (src/sparsevec.c:694-821), batched: n rows of dim elements of integer[], real[], double precision[]
+ * (src = VB_ARRAY_INT4 / FLOAT4 / FLOAT8, rows packed and aligned to their elements, in_off NULL) or numeric[]
+ * (VB_ARRAY_NUMERIC: in holds numeric_send fields at in_off, as in vb_numeric_array_to_rows_batch) to CSR, with the
+ * output conventions of vb_dense_to_sparsevec_batch (out_row_off [n + 1] always written, cap = 0 sizes the output, a
+ * total above cap fails with VB_EINVAL naming the total and writes no entries).  Each element becomes (float) of the
+ * int32 or double (round to nearest even), a real as is, or numeric_float4 of the numeric, and is kept when v != 0: -0
+ * and a double that rounds to 0 (1e-46) are dropped, NaN and the infinities are kept.  Rows may have up to 10^9
+ * elements.
+ * Before any work, in the reference's order: CheckDim ("sparsevec must have at least 1 dimension", "sparsevec cannot
+ * have more than 1000000000 dimensions"), then CheckExpectedDim ("expected %d dimensions, not %d"; typmod -1: none).
+ * numeric[]: malformed fields are refused first, as in vb_numeric_array_to_rows_batch.  Data errors, as row-by-row
+ * execution raises them (the lowest failing row, then the first check its loops reach): numeric_float4's range error in
+ * the count loop (the first failing element), CheckNnz after it ("sparsevec cannot have more than 16000 non-zero
+ * elements"), then CheckElement over the kept values in index order ("NaN not allowed in sparsevec", "infinite value not
+ * allowed in sparsevec").  A data error wins over the cap check, so a sizing call already fails with the error the full
+ * call would raise.  *out_bad (optional) is the failing row, or -1.  On an error the outputs are unspecified.  The array
+ * structure checks ("array must be 1-D", "array must not contain nulls", "unsupported array type") stay with the caller.
+ * The host variant streams chunks of whole rows (about 32 MB of source each; a longer row is a chunk of its own)
+ * through pinned staging, so the input is not bound by device memory.  The _dev variant reads back one 24-byte check
+ * result, like vb_dense_to_sparsevec_batch_dev (numeric[]: 16 bytes more, and the offending field on an error).  Calls
+ * with n = 0 launch nothing.
+ */
+int			vb_array_to_sparsevec_batch(int src, int dim, int32_t typmod, const void *in, const int64_t *in_off, int64_t n,
+										int64_t cap, int64_t *out_row_off, int32_t *out_idx, float *out_val, int64_t *out_bad);
+int			vb_array_to_sparsevec_batch_dev(int src, int dim, int32_t typmod, const void *in_dev, const int64_t *in_off_dev,
+											int64_t n, int64_t cap, int64_t *out_row_off_dev, int32_t *out_idx_dev,
+											float *out_val_dev, int64_t *out_bad);
 int			vb_dense_to_sparsevec_batch(int elem, int dim, const void *rows, int64_t n, int64_t cap, int64_t *out_row_off,
 										int32_t *out_idx, float *out_val);
 int			vb_dense_to_sparsevec_batch_dev(int elem, int dim, const void *rows_dev, int64_t n, int64_t cap,

@@ -20,6 +20,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
+from . import numeric as _numeric
 from . import sparsevec  # noqa: F401  (sparsevec functions, CSR tables and the exact scan over them)
 from ._lib import VecB200Error, load  # noqa: F401
 from .sparsevec import SparseRows, SparseTable, SparseVector  # noqa: F401
@@ -1567,7 +1568,28 @@ def vector_concat(a, b, elem=VECTOR):
     return out[0] if single else out
 
 
+def _numeric_cast(elem, rows, typmod):
+    """numeric[] rows (Decimal values or NumericArrays) through vb_numeric_array_to_rows_batch[_dev]"""
+    lib = load()
+    A, single = _numeric.as_numeric_arrays(rows)
+    bad = C.c_int64(-1)
+    if A.is_cuda:
+        import torch
+        out = torch.empty((A.n, A.dim), dtype=torch.float32 if elem == VECTOR else torch.float16, device=A.data.device)
+        _after_torch(A.data, A.off)
+        _check_reference(lib.vb_numeric_array_to_rows_batch_dev(elem, A.dim, int(typmod), _ptr(A.data), _ptr(A.off), A.n, _ptr(out),
+                                                                C.byref(bad)))
+        synchronize()
+    else:
+        out = np.empty((A.n, A.dim), dtype=_NP[elem])
+        _check_reference(lib.vb_numeric_array_to_rows_batch(elem, A.dim, int(typmod), _ptr(np.ascontiguousarray(A.data)),
+                                                            _ptr(np.ascontiguousarray(A.off, dtype=np.int64)), A.n, _ptr(out), C.byref(bad)))
+    return out[0] if single else out
+
+
 def _array_cast(elem, rows, typmod):
+    if _numeric.is_numeric_rows(rows):
+        return _numeric_cast(elem, rows, typmod)
     lib = load()
     dev = _is_cuda(rows)
     if dev:
@@ -1597,8 +1619,9 @@ def _array_cast(elem, rows, typmod):
 
 
 def array_to_vector(rows, typmod=-1):
-    """integer[] / real[] / double precision[] :: vector(typmod) of every row (src/vector.c:443-512): the dtype (int32,
-    float32, float64) is the array type.  The reference's errors raise ValueError."""
+    """integer[] / real[] / double precision[] / numeric[] :: vector(typmod) of every row (src/vector.c:443-512): the
+    dtype (int32, float32, float64) is the array type; rows of decimal.Decimal values, or numeric.NumericArrays of
+    numeric_send fields (host or CUDA), are numeric[].  The reference's errors raise ValueError."""
     return _array_cast(VECTOR, rows, typmod)
 
 

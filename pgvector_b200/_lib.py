@@ -49,6 +49,8 @@ SIGNATURES = {
     "vb_concat_batch_dev": (_i, [_i, _i, _vp, _i64, _i, _vp, _i64, _vp, C.POINTER(_i)]),
     "vb_array_to_rows_batch": (_i, [_i, _i, _i, C.c_int32, _vp, _i64, _vp]),
     "vb_array_to_rows_batch_dev": (_i, [_i, _i, _i, C.c_int32, _vp, _i64, _vp]),
+    "vb_numeric_array_to_rows_batch": (_i, [_i, _i, C.c_int32, _vp, _vp, _i64, _vp, C.POINTER(_i64)]),
+    "vb_numeric_array_to_rows_batch_dev": (_i, [_i, _i, C.c_int32, _vp, _vp, _i64, _vp, C.POINTER(_i64)]),
     "vb_sparsevec_distance_batch": (_i, [_i, _i, _i, C.c_int32, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "vb_sparsevec_norm_batch": (_i, [_i64, _vp, _vp, _vp]),
     "vb_sparsevec_l2_normalize_batch": (_i, [_i64, _vp, _vp, _vp, _vp, _vp, _vp]),
@@ -66,6 +68,8 @@ SIGNATURES = {
     "vb_sparse_table_filter_create_dev": (_i, [_vp, _vp, _i64, C.POINTER(_vp)]),
     "vb_sparse_exact_topk_filtered_dev": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
     "vb_sparse_table_rerank_dev": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),
+    "vb_array_to_sparsevec_batch": (_i, [_i, _i, C.c_int32, _vp, _vp, _i64, _i64, _vp, _vp, _vp, C.POINTER(_i64)]),
+    "vb_array_to_sparsevec_batch_dev": (_i, [_i, _i, C.c_int32, _vp, _vp, _i64, _i64, _vp, _vp, _vp, C.POINTER(_i64)]),
     "vb_dense_to_sparsevec_batch": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp, _vp]),
     "vb_dense_to_sparsevec_batch_dev": (_i, [_i, _i, _vp, _i64, _i64, _vp, _vp, _vp]),
     "vb_sparsevec_to_dense_batch": (_i, [_i, _i, _i64, _vp, _vp, _vp, _vp]),

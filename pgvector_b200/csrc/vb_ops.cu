@@ -8,6 +8,7 @@
 //   vb_concat_batch        ||    (src/vector.c:928-947, src/halfvec.c:886-903), two column copies
 //   vb_array_to_rows_batch integer[] / real[] / double precision[] -> vector / halfvec (src/vector.c:443-512,
 //                          src/halfvec.c:442-509)
+//   vb_numeric_array_to_rows_batch  numeric[] -> vector / halfvec, the same functions' numeric_float4 branch
 // The cosine opclasses normalise every indexed row and the query (src/ivfbuild.c:174-180,
 // src/ivfscan.c:222-229, src/hnswutils.c:417-423); norms accumulate in fp64 like the reference.
 // One warp per row; HBM bound (row read once, written once).
@@ -15,6 +16,8 @@
 // caller's buffers, the host variants stage the rows in device scratch, call it and copy the result back, so both give
 // the same bits.
 #include "vb_common.cuh"
+#include "vb_numeric.cuh"
+#include "vb_typio.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -124,7 +127,7 @@ __global__ void subvector_kernel(const T* __restrict__ in, int64_t pitch, int64_
 // pass 0 / 1 are the two checking loops of array_to_halfvec (conversion, then CheckElement); the other functions have
 // one.  A batch with no offender leaves the key at ~0.
 enum { ERR_OVERFLOW = 0, ERR_UNDERFLOW = 1 };             // + - *: float_overflow_error / float_underflow_error
-enum { ERR_RANGE = 0, ERR_NAN = 1, ERR_INF = 2 };         // casts: Float4ToHalf, CheckElement
+enum { ERR_RANGE = 0, ERR_NAN = 1, ERR_INF = 2, ERR_REAL = 3 };   // casts: Float4ToHalf, CheckElement, float4in
 constexpr unsigned long long NO_ERROR = ~0ull;
 
 __device__ __forceinline__ unsigned long long error_key(int64_t row, int pass, int64_t dim, int64_t elem, int kind) {
@@ -268,6 +271,51 @@ __global__ void array_cast_kernel(const S* __restrict__ in, int64_t total, int d
                 if (i0 + v < total) dst[v] = __ushort_as_half((unsigned short)o[v]);
     }
     if (key != NO_ERROR) atomicMin(first_bad, key);
+}
+
+// numeric[] -> vector / halfvec (numeric_cast_kernel's sink): vector stores numeric_float4's value, and its checking
+// loop (CheckElement) runs after the whole row is converted, so float4in's range error is pass 0 and NaN / infinity
+// pass 1.  halfvec runs numeric_float4 and then Float4ToHalf on each element in turn (pass 0: float4in's range error,
+// or the half overflow), then CheckElement (pass 1).
+template <int ELEM>
+struct NumericRowSink {
+    void* out;
+    int dim;
+    unsigned long long* first_bad;
+    __device__ __forceinline__ void put(int64_t e, float f, bool real_range) const {
+        const int64_t r = e / dim, i = e - r * dim;
+        int pass = 0, kind = -1;
+        if (real_range) {
+            kind = ERR_REAL;
+        } else if (ELEM == VB_VECTOR) {
+            reinterpret_cast<float*>(out)[e] = f;
+            if (isnan(f)) pass = 1, kind = ERR_NAN;
+            else if (isinf(f)) pass = 1, kind = ERR_INF;
+        } else {
+            bool over;
+            const uint32_t h = __half_as_ushort(float_to_half_checked(f, &over));
+            reinterpret_cast<__half*>(out)[e] = __ushort_as_half((unsigned short)h);
+            if (over) kind = ERR_RANGE;
+            else if ((h & 0x7C00) == 0x7C00) pass = 1, kind = (h & 0x7FFF) != 0x7C00 ? ERR_NAN : ERR_INF;
+        }
+        if (kind >= 0) atomicMin(first_bad, error_key(r, pass, dim, i, kind));
+    }
+};
+
+// total fields (total > 0) to rows; status[0] = the first-offender key, status[1] = the first malformed field (both set
+// to ~0 here)
+static int numeric_cast_rows(int elem, int dim, const uint8_t* bytes, const int64_t* off, int64_t base, int64_t total, void* out,
+                             unsigned long long* status) {
+    cudaStream_t s = ctx().stream;
+    VB_CUDA(cudaMemsetAsync(status, 0xFF, 2 * sizeof(unsigned long long), s));
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    if (elem == VB_VECTOR)
+        numeric_cast_kernel<<<grid, 256, 0, s>>>(bytes, off, base, total, NumericRowSink<VB_VECTOR>{out, dim, status}, status + 1);
+    else
+        numeric_cast_kernel<<<grid, 256, 0, s>>>(bytes, off, base, total, NumericRowSink<VB_HALFVEC>{out, dim, status}, status + 1);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
 }
 
 // the shortest decimal that reads back as the same float, in PostgreSQL's float4 output style
@@ -586,6 +634,36 @@ static int check_array_cast(const char* fn, int elem, int src, int dim, int32_t 
     VB_REQUIRE((uintptr_t)in % array_elem_bytes(src) == 0 && (uintptr_t)out % (elem == VB_VECTOR ? 4 : 2) == 0,
                "%s: rows and output must be aligned to their elements", fn);
     return VB_OK;
+}
+
+// the scalar checks of numeric[] -> vector / halfvec, before any work
+static int check_numeric_cast(const char* fn, int elem, int dim, int32_t typmod, const void* bytes, const int64_t* off, int64_t n,
+                              const void* out) {
+    VB_REQUIRE(elem == VB_VECTOR || elem == VB_HALFVEC, "%s: elem must be VB_VECTOR or VB_HALFVEC, got %d", fn, elem);
+    VB_REQUIRE(n >= 0, "%s: bad row count %lld", fn, (long long)n);
+    VB_REQUIRE(dim >= 1, "%s must have at least 1 dimension", type_name(elem));
+    VB_REQUIRE(dim <= 16000, "%s cannot have more than %d dimensions", type_name(elem), 16000);
+    VB_REQUIRE(typmod == -1 || typmod == dim, "expected %d dimensions, not %d", typmod, dim);
+    VB_REQUIRE(n == 0 || (bytes && off && out), "%s: null fields, offsets or output", fn);
+    VB_REQUIRE((uintptr_t)off % 8 == 0 && (uintptr_t)out % (elem == VB_VECTOR ? 4 : 2) == 0,
+               "%s: offsets and output must be aligned to their elements", fn);
+    return VB_OK;
+}
+
+// the numeric cast's error from its first-offender key; field(e) gives a host copy of field e's bytes
+template <typename Field>
+static int numeric_batch_error(unsigned long long key, int elem, int dim, int64_t* out_bad, Field field) {
+    const int kind = (int)(key & 3);
+    const unsigned long long rest = key >> 2, rp = rest / (unsigned)dim;
+    const int64_t row = (int64_t)(rp >> 1), e = row * dim + (int64_t)(rest % (unsigned)dim);
+    if (out_bad) *out_bad = row;
+    if (kind == ERR_NAN || kind == ERR_INF) {
+        set_error(kind == ERR_NAN ? "NaN not allowed in %s" : "infinite value not allowed in %s", type_name(elem));
+        return VB_EINVAL;
+    }
+    std::vector<uint8_t> f;
+    VB_TRY(field(e, f));
+    return kind == ERR_REAL ? numeric_range_error(f.data()) : half_range_error(numeric_float4_host(f.data()));
 }
 
 }  // namespace vb
@@ -934,6 +1012,127 @@ int vb_array_to_rows_batch_dev(int elem, int src, int dim, int32_t typmod, const
         *v = source_float(src, &raw, 0);
         return VB_OK;
     });
+}
+
+// numeric[] -> vector / halfvec.  Host: chunks of whole rows through the two staging slots; every chunk is converted
+// and checked, so a malformed field anywhere wins over a data error, and the first chunk with a data error has the
+// lowest failing row.
+int vb_numeric_array_to_rows_batch(int elem, int dim, int32_t typmod, const void* bytes, const int64_t* off, int64_t n, void* out,
+                                   int64_t* out_bad) {
+    Scratch sc;
+    const char* fn = "vb_numeric_array_to_rows_batch";
+    if (out_bad) *out_bad = -1;
+    VB_TRY(require_init());
+    VB_TRY(check_numeric_cast(fn, elem, dim, typmod, bytes, off, n, out));
+    if (n == 0) return VB_OK;
+    const int64_t total = n * dim;
+    VB_TRY(numeric_offsets_check(fn, off, total, out_bad, dim));
+    std::vector<int64_t> starts;
+    numeric_chunks(off, n, dim, (size_t)32 << 20, starts);
+    const int64_t nch = (int64_t)starts.size() - 1;
+    int64_t max_rows = 0, max_bytes = 0;
+    for (int64_t c = 0; c < nch; ++c) {
+        max_rows = std::max(max_rows, starts[c + 1] - starts[c]);
+        max_bytes = std::max(max_bytes, off[starts[c + 1] * dim] - off[starts[c] * dim]);
+    }
+    const size_t esz = elem == VB_VECTOR ? 4 : 2;
+    const size_t b_off = sizeof(int64_t) * (size_t)(max_rows * dim + 1), b_out = esz * (size_t)(max_rows * dim);
+    Staging& st = staging();
+    struct Slot {
+        int64_t* off;
+        uint8_t* bytes;
+        void* out;
+        unsigned long long* status;
+    } slot[2];
+    for (int k = 0; k < 2 && k < nch; ++k) {
+        void *a, *b, *c, *d;
+        VB_TRY(sc.take(b_off, &a));
+        VB_TRY(sc.take((size_t)max_bytes + 16, &b));
+        VB_TRY(sc.take(b_out, &c));
+        VB_TRY(sc.take(16, &d));
+        slot[k] = Slot{(int64_t*)a, (uint8_t*)b, c, (unsigned long long*)d};
+        VB_TRY(pinned_grow(&st.in[k], &st.in_bytes[k], b_off + (size_t)max_bytes));
+        VB_TRY(pinned_grow(&st.out[k], &st.out_bytes[k], b_out + 16));
+    }
+    cudaStream_t s = ctx().stream;
+    const uint8_t* src = (const uint8_t*)bytes;
+    int64_t malformed = -1, bad_chunk = -1;
+    unsigned long long bad_key = NO_ERROR;
+    auto enqueue = [&](int64_t c, int k) -> int {
+        const int64_t e0 = starts[c] * dim, ne = (starts[c + 1] - starts[c]) * dim, b0 = off[e0], nb = off[e0 + ne] - b0;
+        uint8_t* in = (uint8_t*)st.in[k];
+        memcpy(in, off + e0, sizeof(int64_t) * (size_t)(ne + 1));
+        memcpy(in + b_off, src + b0, (size_t)nb);
+        VB_CUDA(cudaMemcpyAsync(slot[k].off, in, sizeof(int64_t) * (size_t)(ne + 1), cudaMemcpyHostToDevice, s));
+        VB_CUDA(cudaMemcpyAsync(slot[k].bytes, in + b_off, (size_t)nb, cudaMemcpyHostToDevice, s));
+        VB_TRY(numeric_cast_rows(elem, dim, slot[k].bytes, slot[k].off, b0, ne, slot[k].out, slot[k].status));
+        uint8_t* o = (uint8_t*)st.out[k];
+        VB_CUDA(cudaMemcpyAsync(o, slot[k].out, esz * (size_t)ne, cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaMemcpyAsync(o + b_out, slot[k].status, 16, cudaMemcpyDeviceToHost, s));
+        return VB_OK;
+    };
+    auto finish = [&](int64_t c, int k) -> int {
+        const int64_t e0 = starts[c] * dim, ne = (starts[c + 1] - starts[c]) * dim;
+        const uint8_t* o = (const uint8_t*)st.out[k];
+        unsigned long long status[2];
+        memcpy(status, o + b_out, 16);
+        if (malformed < 0 && status[1] != NO_ERROR) malformed = e0 + (int64_t)status[1];
+        if (bad_chunk < 0 && status[0] != NO_ERROR) bad_chunk = c, bad_key = status[0];
+        memcpy((uint8_t*)out + esz * (size_t)e0, o, esz * (size_t)ne);
+        return VB_OK;
+    };
+    VB_TRY(pipeline_chunks(nch, enqueue, finish));
+    if (malformed >= 0) {
+        if (out_bad) *out_bad = malformed / dim;
+        return numeric_field_error(fn, malformed, src + off[malformed], off[malformed + 1] - off[malformed]);
+    }
+    if (bad_chunk < 0) return VB_OK;
+    const int64_t r0 = starts[bad_chunk];
+    const int rc = numeric_batch_error(bad_key, elem, dim, out_bad, [&](int64_t e, std::vector<uint8_t>& f) {
+        const int64_t g = r0 * dim + e;
+        f.assign(src + off[g], src + off[g + 1]);
+        return VB_OK;
+    });
+    if (out_bad) *out_bad += r0;
+    return rc;
+}
+
+int vb_numeric_array_to_rows_batch_dev(int elem, int dim, int32_t typmod, const void* bytes_dev, const int64_t* off_dev, int64_t n,
+                                       void* out_dev, int64_t* out_bad) {
+    Scratch sc;
+    const char* fn = "vb_numeric_array_to_rows_batch_dev";
+    if (out_bad) *out_bad = -1;
+    VB_TRY(require_init());
+    VB_TRY(check_numeric_cast(fn, elem, dim, typmod, bytes_dev, off_dev, n, out_dev));
+    if (n == 0) return VB_OK;
+    cudaStream_t s = ctx().stream;
+    void* d_status;
+    VB_TRY(sc.take(16, &d_status));
+    VB_TRY(numeric_cast_rows(elem, dim, (const uint8_t*)bytes_dev, off_dev, 0, n * dim, out_dev, (unsigned long long*)d_status));
+    unsigned long long status[2];
+    VB_CUDA(cudaMemcpyAsync(status, d_status, 16, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    if (status[0] == NO_ERROR && status[1] == NO_ERROR) return VB_OK;
+    // only an error reads a field back, for its text
+    auto field = [&](int64_t e, std::vector<uint8_t>& f) {
+        int64_t o[2];
+        VB_CUDA(cudaMemcpy(o, off_dev + e, sizeof(o), cudaMemcpyDeviceToHost));
+        const int64_t len = std::max<int64_t>(0, std::min<int64_t>(o[1] - o[0], 8 + 2 * 65535 + 1));
+        f.resize((size_t)len + 8);
+        if (len > 0) VB_CUDA(cudaMemcpy(f.data(), (const uint8_t*)bytes_dev + o[0], (size_t)len, cudaMemcpyDeviceToHost));
+        f.resize((size_t)len);   // past the longest valid field only the count of bytes left over matters
+        return VB_OK;
+    };
+    if (status[1] != NO_ERROR) {
+        const int64_t e = (int64_t)status[1];
+        if (out_bad) *out_bad = e / dim;
+        int64_t o[2];
+        VB_CUDA(cudaMemcpy(o, off_dev + e, sizeof(o), cudaMemcpyDeviceToHost));
+        std::vector<uint8_t> f;
+        VB_TRY(field(e, f));
+        return numeric_field_error(fn, e, f.data(), o[1] < o[0] ? o[1] - o[0] : (int64_t)f.size());
+    }
+    return numeric_batch_error(status[0], elem, dim, out_bad, field);
 }
 
 }  // extern "C"

@@ -1,7 +1,8 @@
 // vb_sparse.cu -- sparsevec on the device (SURVEY 8 f4): the distance functions of src/sparsevec.c:826-1057
 // (l2_distance / l2_squared_distance / inner_product / negative_inner_product / cosine_distance / l1_distance),
 // l2_norm / l2_normalize (src/sparsevec.c:1062-1150), a resident CSR row table and the exact (no index) top-k
-// over it, filtered (row filters of vb_filter.cu) or over per-query candidate rows (re-rank).
+// over it, filtered (row filters of vb_filter.cu) or over per-query candidate rows (re-rank), and the casts to and from
+// sparsevec: vector / halfvec rows and integer[] / real[] / double precision[] / numeric[] arrays (array_to_sparsevec).
 //
 // A sparsevec is (dim, nnz, indices[nnz] ascending 0-based, values[nnz]) -- src/sparsevec.h:21-32; a batch of rows is
 // CSR: row r = entries row_off[r] .. row_off[r+1] of idx[] / val[].
@@ -17,11 +18,15 @@
 // of index order: within 1e-5 relative of the fp64 truth, tested against the oracle).
 #include "vb_common.cuh"
 #include "vb_distance.cuh"
+#include "vb_numeric.cuh"
+#include "vb_typio.cuh"
 
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
+#include <type_traits>
 #include <vector>
 
 namespace vb {
@@ -943,71 +948,153 @@ static int sparse_append(vb_sparse_table* h, int64_t n, const int64_t* row_off, 
 
 // ----------------------------------------------------------------------------- casts between the dense types and sparsevec
 
-// element i of packed dense rows as the cast sees it: kept (vector: x != 0; halfvec: !HalfIsZero, so -0 is dropped in
-// both) and its float value (halfvec: HalfToFloat4, exact)
+// The element sources of the casts to sparsevec.  keep(i, &v): element i of the packed rows is kept, v its float value.
+// nnz_key(r): the SparseCheck::bad key of CheckNnz's error in row r; elem_key(r, i, v): the key of CheckElement's error
+// at kept element i (kCheck sources only).
+//
+// vector / halfvec rows (vector_to_sparsevec / halfvec_to_sparsevec): kept when x != 0 (halfvec: !HalfIsZero, so -0 is
+// dropped in both), halfvec widened exactly; CheckNnz as check_csr reports it, (row << 8) | SPC_NNZ.
 template <int ELEM>
-__device__ __forceinline__ bool dense_elem(const void* __restrict__ rows, size_t i, float* v) {
-    if (ELEM == VB_VECTOR) {
-        *v = __ldg(reinterpret_cast<const float*>(rows) + i);
+struct DenseSource {
+    const void* rows;
+    static constexpr bool kCheck = false;
+    __device__ __forceinline__ bool keep(size_t i, float* v) const {
+        if (ELEM == VB_VECTOR) {
+            *v = __ldg(reinterpret_cast<const float*>(rows) + i);
+            return *v != 0.f;
+        }
+        const unsigned short b = __ldg(reinterpret_cast<const unsigned short*>(rows) + i);
+        *v = __half2float(__ushort_as_half(b));
+        return (b & 0x7FFFu) != 0;
+    }
+    __device__ __forceinline__ unsigned long long nnz_key(int64_t r) const { return ((unsigned long long)r << 8) | SPC_NNZ; }
+    __device__ __forceinline__ unsigned long long elem_key(int64_t, int, float) const { return ~0ull; }
+};
+
+// array_to_sparsevec's first-offender key (src/sparsevec.c:694-821): (row, pass, element, kind) in 31 + 2 + 30 + 1 bits,
+// so the lowest row wins, then the first pass its loops reach, then the element.  Pass 0 is numeric_float4's range
+// error in the count loop (numeric[] only), pass 1 CheckNnz after it, pass 2 CheckElement over the kept values (kind 0:
+// NaN, 1: infinite).  n < 2^31 rows and dim <= 10^9 < 2^30 fit.
+enum { ASP_PASS_REAL = 0, ASP_PASS_NNZ = 1, ASP_PASS_ELEMENT = 2 };
+__host__ __device__ __forceinline__ unsigned long long array_sparse_key(int64_t r, int pass, int64_t i, int kind) {
+    return ((unsigned long long)r << 33) | ((unsigned long long)pass << 31) | ((unsigned long long)i << 1) | (unsigned)kind;
+}
+
+// numeric[] -> sparsevec, first step (numeric_cast_kernel's sink): numeric_float4 of every element into a float
+// buffer that the count and write passes then read as real[]; float4in's range error lowers *first_bad
+struct NumericFloatSink {
+    float* out;
+    int dim;
+    unsigned long long* first_bad;
+    __device__ __forceinline__ void put(int64_t e, float f, bool real_range) const {
+        out[e] = real_range ? 0.f : f;
+        if (real_range) atomicMin(first_bad, array_sparse_key(e / dim, ASP_PASS_REAL, e % dim, 0));
+    }
+};
+
+__device__ __forceinline__ float array_float(int32_t x) { return __int2float_rn(x); }
+__device__ __forceinline__ float array_float(float x) { return x; }
+__device__ __forceinline__ float array_float(double x) { return __double2float_rn(x); }
+
+// integer[] / real[] / double precision[] rows: (float) of the int32 or double (round to nearest even), real as is;
+// kept when v != 0, so -0 and a double that rounds to 0 are dropped and NaN and the infinities are kept
+template <typename S>
+struct ArraySource {
+    const S* rows;
+    static constexpr bool kCheck = !std::is_same<S, int32_t>::value;   // an int32 is always finite
+    __device__ __forceinline__ bool keep(size_t i, float* v) const {
+        *v = array_float(__ldg(rows + i));
         return *v != 0.f;
     }
-    const unsigned short b = __ldg(reinterpret_cast<const unsigned short*>(rows) + i);
-    *v = __half2float(__ushort_as_half(b));
-    return (b & 0x7FFFu) != 0;
-}
+    __device__ __forceinline__ unsigned long long nnz_key(int64_t r) const { return array_sparse_key(r, ASP_PASS_NNZ, 0, 0); }
+    __device__ __forceinline__ unsigned long long elem_key(int64_t r, int i, float v) const {
+        return isnan(v) ? array_sparse_key(r, ASP_PASS_ELEMENT, i, 0) : isinf(v) ? array_sparse_key(r, ASP_PASS_ELEMENT, i, 1) : ~0ull;
+    }
+};
 
 constexpr int SP_CAST_UNROLL = 4;   // elements per lane in flight: each lane loads 4 before the warp's ballots
 
-// Count pass of vector_to_sparsevec / halfvec_to_sparsevec (src/sparsevec.c:606-689): one warp per row, the kept
-// elements ballot-counted.  cnt[r] = the row's nnz; a row above SP_MAX_NNZ is CheckNnz's error (the first such row wins).
-template <int ELEM>
-__global__ void __launch_bounds__(256) dense_count_kernel(const void* __restrict__ rows, int dim, int64_t n, int64_t* __restrict__ cnt,
+// The work of the casts to sparsevec: one warp per segment of seg_len elements, nseg segments per row (row r's
+// segment j is warp r * nseg + j), so a batch of a few long rows still fills the device.  With nseg == 1 a warp takes
+// a whole row and the segment offsets are the row offsets.
+struct SparseSegs {
+    int nseg;
+    int seg_len;   // a multiple of 32 * SP_CAST_UNROLL
+};
+
+// Count pass of the casts to sparsevec (vector_to_sparsevec / halfvec_to_sparsevec, src/sparsevec.c:606-689, and
+// array_to_sparsevec, src/sparsevec.c:694-821): the kept elements of each segment ballot-counted into cnt[w].  With one
+// segment per row a row above SP_MAX_NNZ is CheckNnz's error here (else segment_rows_kernel checks the row sums).  A
+// kCheck source also lowers the key of each lane's first kept NaN or infinity.
+template <typename Src>
+__global__ void __launch_bounds__(256) dense_count_kernel(Src src, int dim, int64_t n, SparseSegs sg, int64_t* __restrict__ cnt,
                                                           SparseCheck* __restrict__ chk) {
-    const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
-    if (r >= n) return;   // whole warps
+    if (w >= n * sg.nseg) return;   // whole warps
+    const int64_t r = w / sg.nseg;
+    const int lo = (int)(w - r * sg.nseg) * sg.seg_len;
+    const int hi = min(dim, lo + sg.seg_len);
     const size_t base = (size_t)r * (size_t)dim;
     int64_t c = 0;
-    for (int i0 = 0; i0 < dim; i0 += 32 * SP_CAST_UNROLL) {
+    unsigned long long key = ~0ull;
+    for (int i0 = lo; i0 < hi; i0 += 32 * SP_CAST_UNROLL) {
         bool keep[SP_CAST_UNROLL];
 #pragma unroll
         for (int u = 0; u < SP_CAST_UNROLL; ++u) {
             const int i = i0 + u * 32 + lane;
             float v;
-            keep[u] = i < dim && dense_elem<ELEM>(rows, base + i, &v);
+            keep[u] = i < hi && src.keep(base + i, &v);
+            if (Src::kCheck && keep[u] && key == ~0ull) key = src.elem_key(r, i, v);
         }
 #pragma unroll
         for (int u = 0; u < SP_CAST_UNROLL; ++u) c += __popc(__ballot_sync(0xffffffffu, keep[u]));
     }
+    if (Src::kCheck && key != ~0ull) atomicMin(&chk->bad, key);
     if (lane == 0) {
-        cnt[r] = c;
-        if (c > SP_MAX_NNZ) atomicMin(&chk->bad, ((unsigned long long)r << 8) | SPC_NNZ);
+        cnt[w] = c;
+        if (sg.nseg == 1 && c > SP_MAX_NNZ) atomicMin(&chk->bad, src.nnz_key(r));
     }
 }
 
-// Write pass: the kept elements of row r at off[r] .. in ascending index order (ballot + the warp prefix of each step)
-template <int ELEM>
-__global__ void __launch_bounds__(256) dense_write_kernel(const void* __restrict__ rows, int dim, int64_t n, const int64_t* __restrict__ off,
-                                                          int32_t* __restrict__ out_idx, float* __restrict__ out_val) {
-    const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+// Rows split into segments: row_off[r] = seg_off[r * nseg] for r in [0, n], and CheckNnz over each row's sum
+template <typename Src>
+__global__ void segment_rows_kernel(Src src, int64_t n, int nseg, const int64_t* __restrict__ seg_off, int64_t* __restrict__ row_off,
+                                    SparseCheck* __restrict__ chk) {
+    const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (r > n) return;
+    const int64_t b = seg_off[r * nseg];
+    row_off[r] = b;
+    if (r < n && seg_off[(r + 1) * nseg] - b > SP_MAX_NNZ) atomicMin(&chk->bad, src.nnz_key(r));
+}
+
+// Write pass: the kept elements of segment w at off[w] .. in ascending index order (ballot + the warp prefix of each
+// step).  Entries at lim and above are not written: a buffer of lim entries is too small only for rows CheckNnz refuses.
+template <typename Src>
+__global__ void __launch_bounds__(256) dense_write_kernel(Src src, int dim, int64_t n, SparseSegs sg, const int64_t* __restrict__ off,
+                                                          int64_t lim, int32_t* __restrict__ out_idx, float* __restrict__ out_val) {
+    const int64_t ws = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
-    if (r >= n) return;   // whole warps
+    if (ws >= n * sg.nseg) return;   // whole warps
+    const int64_t r = ws / sg.nseg;
+    const int lo = (int)(ws - r * sg.nseg) * sg.seg_len;
+    const int hi = min(dim, lo + sg.seg_len);
     const size_t base = (size_t)r * (size_t)dim;
     const unsigned below = (1u << lane) - 1u;
-    int64_t w = off[r];
-    for (int i0 = 0; i0 < dim; i0 += 32 * SP_CAST_UNROLL) {
+    int64_t w = off[ws];
+    for (int i0 = lo; i0 < hi; i0 += 32 * SP_CAST_UNROLL) {
         bool keep[SP_CAST_UNROLL];
         float v[SP_CAST_UNROLL];
 #pragma unroll
         for (int u = 0; u < SP_CAST_UNROLL; ++u) {
             const int i = i0 + u * 32 + lane;
-            keep[u] = i < dim && dense_elem<ELEM>(rows, base + i, &v[u]);
+            keep[u] = i < hi && src.keep(base + i, &v[u]);
         }
 #pragma unroll
         for (int u = 0; u < SP_CAST_UNROLL; ++u) {
             const unsigned m = __ballot_sync(0xffffffffu, keep[u]);
-            if (keep[u]) {
-                const int64_t at = w + __popc(m & below);
+            const int64_t at = w + __popc(m & below);
+            if (keep[u] && at < lim) {
                 out_idx[at] = i0 + u * 32 + lane;
                 out_val[at] = v[u];
             }
@@ -1047,6 +1134,71 @@ __global__ void __launch_bounds__(256) sparse_to_dense_kernel(int64_t n, const i
 
 static const char* dense_name(int elem) { return elem == VB_VECTOR ? "vector" : "halfvec"; }
 
+// The segments of n rows of dim elements: one per row when the rows alone give every SM 64 warps or are short, else
+// enough to do so, none shorter than 2048 elements
+static SparseSegs sparse_segs(int dim, int64_t n) {
+    const int64_t unit = 32 * SP_CAST_UNROLL, want = (int64_t)ctx().sm_count * 64;
+    int64_t nseg = 1;
+    if (n < want && dim > 2048) nseg = std::min<int64_t>((dim + 2047) / 2048, (want + n - 1) / n);
+    const int64_t len = ((dim + nseg - 1) / nseg + unit - 1) / unit * unit;
+    return SparseSegs{(int)((dim + len - 1) / len), (int)len};
+}
+
+// device buffers of a count pass over up to m segments
+struct SparseCountBufs {
+    int64_t* cnt;   // [m + 1]
+    int64_t* seg;   // [m + 1], the segment offsets when a row has several
+    void* scan;
+    size_t scan_bytes;
+};
+static int sparse_count_bufs(Scratch& sc, int64_t m, SparseCountBufs* b) {
+    void *c, *g;
+    VB_TRY(sc.take(sizeof(int64_t) * (size_t)(m + 1), &c));
+    VB_TRY(sc.take(sizeof(int64_t) * (size_t)(m + 1), &g));
+    b->cnt = (int64_t*)c;
+    b->seg = (int64_t*)g;
+    b->scan_bytes = 0;
+    VB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b->scan_bytes, b->cnt, b->seg, (int)(m + 1), ctx().stream));
+    return sc.take(b->scan_bytes + 64, &b->scan);
+}
+
+// Enqueues the count pass of a cast to sparsevec over n >= 1 device rows: chk initialised, then lowered to the first
+// error; row_off[0 .. n] (device) the row offsets and chk->total = row_off[n]; *seg_off the offsets the write pass
+// takes (row_off itself when each row is one segment).  Reads nothing back.
+template <typename Src>
+static int sparse_cast_count(Src src, int dim, int64_t n, const SparseSegs& sg, const SparseCountBufs& b, int64_t* row_off,
+                             SparseCheck* chk, const int64_t** seg_off) {
+    cudaStream_t s = ctx().stream;
+    const int64_t m = n * sg.nseg;
+    int64_t* so = sg.nseg == 1 ? row_off : b.seg;
+    sparse_check_init_kernel<<<1, 1, 0, s>>>(chk);
+    dense_count_kernel<Src><<<(unsigned)((m * 32 + 255) / 256), 256, 0, s>>>(src, dim, n, sg, b.cnt, chk);
+    VB_CUDA(cudaGetLastError());
+    VB_CUDA(cudaMemsetAsync(b.cnt + m, 0, sizeof(int64_t), s));
+    size_t scan_bytes = b.scan_bytes;
+    VB_CUDA(cub::DeviceScan::ExclusiveSum(b.scan, scan_bytes, b.cnt, so, (int)(m + 1), s));
+    count_launch(3);
+    if (sg.nseg > 1) {
+        segment_rows_kernel<Src><<<(unsigned)((n + 1 + 255) / 256), 256, 0, s>>>(src, n, sg.nseg, so, row_off, chk);
+        VB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    VB_CUDA(cudaMemcpyAsync(&chk->total, row_off + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
+    *seg_off = so;
+    return VB_OK;
+}
+
+// Enqueues the write pass after sparse_cast_count: at most lim entries into idx / val (device)
+template <typename Src>
+static int sparse_cast_write(Src src, int dim, int64_t n, const SparseSegs& sg, const int64_t* seg_off, int64_t lim, int32_t* idx,
+                             float* val) {
+    const int64_t m = n * sg.nseg;
+    dense_write_kernel<Src><<<(unsigned)((m * 32 + 255) / 256), 256, 0, ctx().stream>>>(src, dim, n, sg, seg_off, lim, idx, val);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
+}
+
 // vb_dense_to_sparsevec_batch[_dev]
 static int dense_to_sparse(int elem, int dim, const void* rows, int64_t n, int64_t cap, bool host, int64_t* out_row_off, int32_t* out_idx,
                            float* out_val) {
@@ -1068,29 +1220,21 @@ static int dense_to_sparse(int elem, int dim, const void* rows, int64_t n, int64
     }
     const size_t raw = raw_row_bytes(elem, dim);
     const size_t b_off = sizeof(int64_t) * (size_t)(n + 1);
-    void *d_in = const_cast<void*>(rows), *d_cnt, *d_off = out_row_off, *d_scan, *d_chk;
+    void *d_in = const_cast<void*>(rows), *d_off = out_row_off, *d_chk;
     if (host) {
         VB_TRY(sc.take(raw * (size_t)n, &d_in));
         VB_CUDA(cudaMemcpyAsync(d_in, rows, raw * (size_t)n, cudaMemcpyHostToDevice, s));
         VB_TRY(sc.take(b_off, &d_off));
     }
-    VB_TRY(sc.take(b_off, &d_cnt));
     VB_TRY(sc.take(sizeof(SparseCheck), &d_chk));
     SparseCheck* chk = (SparseCheck*)d_chk;
-    int64_t* cnt = (int64_t*)d_cnt;
     int64_t* off = (int64_t*)d_off;
-    const unsigned grid = (unsigned)((n * 32 + 255) / 256);
-    sparse_check_init_kernel<<<1, 1, 0, s>>>(chk);
-    if (elem == VB_VECTOR) dense_count_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(d_in, dim, n, cnt, chk);
-    else dense_count_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(d_in, dim, n, cnt, chk);
-    VB_CUDA(cudaGetLastError());
-    VB_CUDA(cudaMemsetAsync(cnt + n, 0, sizeof(int64_t), s));
-    size_t scan_bytes = 0;
-    VB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, cnt, off, (int)(n + 1), s));
-    VB_TRY(sc.take(scan_bytes + 64, &d_scan));
-    VB_CUDA(cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, cnt, off, (int)(n + 1), s));
-    count_launch(3);
-    VB_CUDA(cudaMemcpyAsync(&chk->total, off + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
+    const SparseSegs sg = sparse_segs(dim, n);
+    SparseCountBufs cb;
+    VB_TRY(sparse_count_bufs(sc, n * sg.nseg, &cb));
+    const int64_t* seg_off;
+    if (elem == VB_VECTOR) VB_TRY(sparse_cast_count(DenseSource<VB_VECTOR>{d_in}, dim, n, sg, cb, off, chk, &seg_off));
+    else VB_TRY(sparse_cast_count(DenseSource<VB_HALFVEC>{d_in}, dim, n, sg, cb, off, chk, &seg_off));
     SparseCheck hc;
     if (host) VB_CUDA(cudaMemcpyAsync(out_row_off, off, b_off, cudaMemcpyDeviceToHost, s));
     VB_CUDA(cudaMemcpyAsync(&hc, chk, SPC_READ, cudaMemcpyDeviceToHost, s));
@@ -1109,16 +1253,271 @@ static int dense_to_sparse(int elem, int dim, const void* rows, int64_t n, int64
         o_idx = (int32_t*)d_out;
         o_val = (float*)((uint8_t*)d_out + b_idx);
     }
-    if (elem == VB_VECTOR) dense_write_kernel<VB_VECTOR><<<grid, 256, 0, s>>>(d_in, dim, n, off, o_idx, o_val);
-    else dense_write_kernel<VB_HALFVEC><<<grid, 256, 0, s>>>(d_in, dim, n, off, o_idx, o_val);
-    VB_CUDA(cudaGetLastError());
-    count_launch();
+    if (elem == VB_VECTOR) VB_TRY(sparse_cast_write(DenseSource<VB_VECTOR>{d_in}, dim, n, sg, seg_off, total, o_idx, o_val));
+    else VB_TRY(sparse_cast_write(DenseSource<VB_HALFVEC>{d_in}, dim, n, sg, seg_off, total, o_idx, o_val));
     if (host) {
         VB_CUDA(cudaMemcpyAsync(out_idx, o_idx, sizeof(int32_t) * (size_t)total, cudaMemcpyDeviceToHost, s));
         VB_CUDA(cudaMemcpyAsync(out_val, o_val, sizeof(float) * (size_t)total, cudaMemcpyDeviceToHost, s));
         VB_CUDA(cudaStreamSynchronize(s));
     }
     return VB_OK;
+}
+
+// array_to_sparsevec's error from a first-offender key; *out_bad = the failing row (plus first_row).  field(e) gives a
+// host copy of numeric field e of the rows the key counts in, for float4in's range error.
+template <typename Field>
+static int array_sparse_error(unsigned long long key, int dim, int64_t first_row, int64_t* out_bad, Field field) {
+    const int64_t row = (int64_t)(key >> 33);
+    if (out_bad) *out_bad = first_row + row;
+    const int pass = (int)((key >> 31) & 3);
+    if (pass == ASP_PASS_REAL) {
+        std::vector<uint8_t> f;
+        VB_TRY(field(row * dim + (int64_t)((key >> 1) & 0x3FFFFFFF), f));
+        return numeric_range_error(f.data());
+    }
+    if (pass == ASP_PASS_NNZ) set_error("sparsevec cannot have more than %d non-zero elements", SP_MAX_NNZ);
+    else set_error((key & 1) ? "infinite value not allowed in sparsevec" : "NaN not allowed in sparsevec");
+    return VB_EINVAL;
+}
+
+constexpr size_t ASP_CHUNK_BYTES = (size_t)32 << 20;   // source bytes (numeric: fields and offsets) per host chunk
+
+// numeric_float4 of fields [0, total) into vals (device); status[0] / [1]: float4in's first range error (key) and the
+// first malformed field, both set to ~0 here
+static int numeric_to_floats(const uint8_t* bytes, const int64_t* off, int64_t base, int64_t total, int dim, float* vals,
+                             unsigned long long* status) {
+    cudaStream_t s = ctx().stream;
+    VB_CUDA(cudaMemsetAsync(status, 0xFF, 2 * sizeof(unsigned long long), s));
+    numeric_cast_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(bytes, off, base, total, NumericFloatSink{vals, dim, status},
+                                                                        status + 1);
+    VB_CUDA(cudaGetLastError());
+    count_launch();
+    return VB_OK;
+}
+
+// vb_array_to_sparsevec_batch_dev (the arguments checked); NUM: numeric[] fields in[off[e] .. off[e + 1]), S = float
+template <typename S, bool NUM>
+static int array_to_sparse_dev(int dim, const void* in, const int64_t* in_off, int64_t n, int64_t cap, int64_t* out_row_off, int32_t* out_idx,
+                               float* out_val, int64_t* out_bad) {
+    Scratch sc;
+    const char* fn = "vb_array_to_sparsevec_batch_dev";
+    cudaStream_t s = ctx().stream;
+    void *d_chk, *d_status = nullptr, *d_vals = nullptr;
+    VB_TRY(sc.take(sizeof(SparseCheck), &d_chk));
+    SparseCheck* chk = (SparseCheck*)d_chk;
+    const S* rows = (const S*)in;
+    unsigned long long status[2] = {~0ull, ~0ull};
+    if (NUM) {
+        VB_TRY(sc.take(16, &d_status));
+        VB_TRY(sc.take(sizeof(float) * (size_t)(n * dim), &d_vals));
+        VB_TRY(numeric_to_floats((const uint8_t*)in, in_off, 0, n * dim, dim, (float*)d_vals, (unsigned long long*)d_status));
+        rows = (const S*)d_vals;
+    }
+    const SparseSegs sg = sparse_segs(dim, n);
+    SparseCountBufs cb;
+    VB_TRY(sparse_count_bufs(sc, n * sg.nseg, &cb));
+    const int64_t* seg_off;
+    VB_TRY(sparse_cast_count(ArraySource<S>{rows}, dim, n, sg, cb, out_row_off, chk, &seg_off));
+    SparseCheck hc;
+    VB_CUDA(cudaMemcpyAsync(&hc, chk, SPC_READ, cudaMemcpyDeviceToHost, s));
+    if (NUM) VB_CUDA(cudaMemcpyAsync(status, d_status, 16, cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+    // only an error reads a field back, for its text
+    auto field = [&](int64_t e, std::vector<uint8_t>& f) {
+        int64_t o[2];
+        VB_CUDA(cudaMemcpy(o, in_off + e, sizeof(o), cudaMemcpyDeviceToHost));
+        const int64_t len = std::max<int64_t>(0, std::min<int64_t>(o[1] - o[0], 8 + 2 * 65535 + 1));
+        f.resize((size_t)len + 8);
+        if (len > 0) VB_CUDA(cudaMemcpy(f.data(), (const uint8_t*)in + o[0], (size_t)len, cudaMemcpyDeviceToHost));
+        f.resize((size_t)len);   // past the longest valid field only the count of bytes left over matters
+        return o[1] < o[0] ? VB_EINVAL : VB_OK;
+    };
+    if (status[1] != ~0ull) {
+        const int64_t e = (int64_t)status[1];
+        if (out_bad) *out_bad = e / dim;
+        std::vector<uint8_t> f;
+        if (field(e, f) != VB_OK) return numeric_field_error(fn, e, f.data(), -1);
+        return numeric_field_error(fn, e, f.data(), (int64_t)f.size());
+    }
+    const unsigned long long key = std::min(hc.bad, status[0]);
+    if (key != ~0ull) return array_sparse_error(key, dim, 0, out_bad, field);
+    const int64_t total = hc.total;
+    VB_REQUIRE(total <= cap, "%s: the rows have %lld non-zero elements, more than cap = %lld", fn, (long long)total, (long long)cap);
+    if (total == 0) return VB_OK;
+    VB_REQUIRE(out_idx && out_val, "%s: null output indices or values", fn);
+    return sparse_cast_write(ArraySource<S>{rows}, dim, n, sg, seg_off, total, out_idx, out_val);
+}
+
+// vb_array_to_sparsevec_batch (the arguments checked): chunks of whole rows through the two staging slots.  Each slot
+// has its device input (numeric: offsets, fields and their floats), offsets, entries (at most min(dim, SP_MAX_NNZ) per
+// row: more is CheckNnz's error) and check.  A chunk's entries are copied out once its check is read, while the next
+// chunk is on the device.  The chunks run in row order, so the first failing chunk has the lowest failing row; past cap
+// the chunks are still counted and checked, so a data error still wins over the cap error.  numeric[]: every chunk is
+// converted and checked, so a malformed field anywhere wins over a data error.
+template <typename S, bool NUM>
+static int array_to_sparse_host(int dim, const void* in, const int64_t* in_off, int64_t n, int64_t cap, int64_t* out_row_off,
+                                int32_t* out_idx, float* out_val, int64_t* out_bad) {
+    Scratch sc;
+    const char* fn = "vb_array_to_sparsevec_batch";
+    cudaStream_t s = ctx().stream;
+    const uint8_t* src = (const uint8_t*)in;
+    std::vector<int64_t> starts;
+    if (NUM) {
+        VB_TRY(numeric_offsets_check(fn, in_off, n * dim, out_bad, dim));
+        numeric_chunks(in_off, n, dim, ASP_CHUNK_BYTES, starts);
+    } else {
+        const int64_t rc = std::min<int64_t>(n, std::max<int64_t>(1, (int64_t)(ASP_CHUNK_BYTES / (sizeof(S) * (size_t)dim))));
+        for (int64_t r = 0; r < n; r += rc) starts.push_back(r);
+        starts.push_back(n);
+    }
+    const int64_t nch = (int64_t)starts.size() - 1;
+    // chunk c: rows [starts[c], starts[c + 1]), its source bytes at src_at(c) .. + src_bytes(c)
+    auto src_at = [&](int64_t c) { return NUM ? in_off[starts[c] * dim] : (int64_t)sizeof(S) * starts[c] * dim; };
+    auto src_bytes = [&](int64_t c) { return NUM ? in_off[starts[c + 1] * dim] - src_at(c) : (int64_t)sizeof(S) * (starts[c + 1] - starts[c]) * dim; };
+    int64_t rc = 0, segs = 0, max_src = 0;
+    for (int64_t c = 0; c < nch; ++c) {
+        const int64_t m = starts[c + 1] - starts[c];
+        rc = std::max(rc, m);
+        segs = std::max(segs, m * sparse_segs(dim, m).nseg);
+        max_src = std::max(max_src, src_bytes(c));
+    }
+    const int64_t ent = rc * std::min(dim, SP_MAX_NNZ);
+    const size_t b_off = sizeof(int64_t) * (size_t)(rc + 1), b_in_off = NUM ? sizeof(int64_t) * (size_t)(rc * dim + 1) : 0;
+    Staging& st = staging();
+    struct Slot {
+        uint8_t* in;
+        int64_t* in_off;
+        float* vals;
+        unsigned long long* status;
+        int64_t* off;
+        int32_t* idx;
+        float* val;
+        SparseCheck* chk;
+        SparseCountBufs cb;
+        const int64_t* seg_off;
+    } slot[2];
+    for (int k = 0; k < 2 && k < nch; ++k) {
+        void *a, *b = nullptr, *v = nullptr, *w = nullptr, *c, *d, *e, *f;
+        VB_TRY(sc.take((size_t)max_src + 16, &a));
+        if (NUM) {
+            VB_TRY(sc.take(b_in_off, &b));
+            VB_TRY(sc.take(sizeof(float) * (size_t)(rc * dim), &v));
+            VB_TRY(sc.take(16, &w));
+        }
+        VB_TRY(sc.take(b_off, &c));
+        VB_TRY(sc.take(sizeof(int32_t) * (size_t)ent, &d));
+        VB_TRY(sc.take(sizeof(float) * (size_t)ent, &e));
+        VB_TRY(sc.take(sizeof(SparseCheck), &f));
+        slot[k] = Slot{(uint8_t*)a, (int64_t*)b, (float*)v, (unsigned long long*)w, (int64_t*)c, (int32_t*)d, (float*)e, (SparseCheck*)f, {}, nullptr};
+        VB_TRY(sparse_count_bufs(sc, segs, &slot[k].cb));
+        VB_TRY(pinned_grow(&st.in[k], &st.in_bytes[k], b_in_off + (size_t)max_src));
+        VB_TRY(pinned_grow(&st.out[k], &st.out_bytes[k], b_off + sizeof(SparseCheck) + 16));
+    }
+    int64_t base = 0;   // entries of the rows finished so far
+    int64_t malformed = -1, bad_chunk = -1;
+    unsigned long long bad_key = ~0ull;
+    out_row_off[0] = 0;
+    auto enqueue = [&](int64_t c, int k) -> int {
+        const int64_t r0 = starts[c], m = starts[c + 1] - r0, nb = src_bytes(c);
+        Slot& sl = slot[k];
+        uint8_t* pin = (uint8_t*)st.in[k];
+        const S* rows = (const S*)sl.in;
+        if (NUM) {
+            memcpy(pin, in_off + r0 * dim, sizeof(int64_t) * (size_t)(m * dim + 1));
+            VB_CUDA(cudaMemcpyAsync(sl.in_off, pin, sizeof(int64_t) * (size_t)(m * dim + 1), cudaMemcpyHostToDevice, s));
+        }
+        memcpy(pin + b_in_off, src + src_at(c), (size_t)nb);
+        VB_CUDA(cudaMemcpyAsync(sl.in, pin + b_in_off, (size_t)nb, cudaMemcpyHostToDevice, s));
+        if (NUM) {
+            VB_TRY(numeric_to_floats(sl.in, sl.in_off, src_at(c), m * dim, dim, sl.vals, sl.status));
+            rows = (const S*)sl.vals;
+        }
+        const SparseSegs sg = sparse_segs(dim, m);
+        VB_TRY(sparse_cast_count(ArraySource<S>{rows}, dim, m, sg, sl.cb, sl.off, sl.chk, &sl.seg_off));
+        VB_TRY(sparse_cast_write(ArraySource<S>{rows}, dim, m, sg, sl.seg_off, ent, sl.idx, sl.val));
+        uint8_t* o = (uint8_t*)st.out[k];
+        VB_CUDA(cudaMemcpyAsync(o, sl.off, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyDeviceToHost, s));
+        VB_CUDA(cudaMemcpyAsync(o + b_off, sl.chk, SPC_READ, cudaMemcpyDeviceToHost, s));
+        if (NUM) VB_CUDA(cudaMemcpyAsync(o + b_off + sizeof(SparseCheck), sl.status, 16, cudaMemcpyDeviceToHost, s));
+        return VB_OK;
+    };
+    auto finish = [&](int64_t c, int k) -> int {
+        const int64_t r0 = starts[c], m = starts[c + 1] - r0;
+        const uint8_t* o = (const uint8_t*)st.out[k];
+        SparseCheck hc;
+        memcpy(&hc, o + b_off, SPC_READ);
+        unsigned long long status[2] = {~0ull, ~0ull};
+        if (NUM) memcpy(status, o + b_off + sizeof(SparseCheck), 16);
+        if (malformed < 0 && status[1] != ~0ull) malformed = r0 * dim + (int64_t)status[1];
+        const unsigned long long key = std::min(hc.bad, status[0]);
+        if (bad_chunk < 0 && key != ~0ull) {
+            bad_chunk = c, bad_key = key;
+            if (!NUM) return VB_EINVAL;   // reported below
+        }
+        if (bad_chunk >= 0 || malformed >= 0) return VB_OK;   // numeric[]: the later chunks are only checked
+        const int64_t* off = (const int64_t*)o;
+        for (int64_t j = 1; j <= m; ++j) out_row_off[r0 + j] = base + off[j];
+        const int64_t t = off[m];
+        if (t > 0 && base + t <= cap) {
+            VB_CUDA(cudaMemcpyAsync(out_idx + base, slot[k].idx, sizeof(int32_t) * (size_t)t, cudaMemcpyDeviceToHost, s));
+            VB_CUDA(cudaMemcpyAsync(out_val + base, slot[k].val, sizeof(float) * (size_t)t, cudaMemcpyDeviceToHost, s));
+            VB_CUDA(cudaStreamSynchronize(s));
+        }
+        base += t;
+        return VB_OK;
+    };
+    const int rc_pipe = pipeline_chunks(nch, enqueue, finish);
+    if (rc_pipe != VB_OK && bad_chunk < 0) return rc_pipe;
+    if (malformed >= 0) {
+        if (out_bad) *out_bad = malformed / dim;
+        return numeric_field_error(fn, malformed, src + in_off[malformed], in_off[malformed + 1] - in_off[malformed]);
+    }
+    if (bad_chunk >= 0) {
+        const int64_t r0 = starts[bad_chunk];
+        return array_sparse_error(bad_key, dim, r0, out_bad, [&](int64_t e, std::vector<uint8_t>& f) {
+            const int64_t g = r0 * dim + e;
+            f.assign(src + in_off[g], src + in_off[g + 1]);
+            return VB_OK;
+        });
+    }
+    VB_REQUIRE(base <= cap, "%s: the rows have %lld non-zero elements, more than cap = %lld", fn, (long long)base, (long long)cap);
+    return VB_OK;
+}
+
+// vb_array_to_sparsevec_batch[_dev]
+static int array_to_sparse(int src, int dim, int32_t typmod, const void* in, const int64_t* in_off, int64_t n, int64_t cap, bool host,
+                           int64_t* out_row_off, int32_t* out_idx, float* out_val, int64_t* out_bad) {
+    const char* fn = host ? "vb_array_to_sparsevec_batch" : "vb_array_to_sparsevec_batch_dev";
+    if (out_bad) *out_bad = -1;
+    VB_TRY(require_init());
+    VB_REQUIRE(src == VB_ARRAY_INT4 || src == VB_ARRAY_FLOAT4 || src == VB_ARRAY_FLOAT8 || src == VB_ARRAY_NUMERIC,
+               "%s: bad source type %d", fn, src);
+    VB_REQUIRE(n >= 0 && n < (int64_t)INT32_MAX && cap >= 0, "%s: bad row count %lld or cap %lld", fn, (long long)n, (long long)cap);
+    // CheckDim, then CheckExpectedDim (src/sparsevec.c:68-94)
+    VB_REQUIRE(dim >= 1, "sparsevec must have at least 1 dimension");
+    VB_REQUIRE(dim <= SP_MAX_DIM, "sparsevec cannot have more than %d dimensions", SP_MAX_DIM);
+    VB_REQUIRE(typmod == -1 || typmod == dim, "expected %d dimensions, not %d", typmod, dim);
+    VB_REQUIRE(out_row_off && (in || n == 0), "%s: null rows or offsets", fn);
+    const bool num = src == VB_ARRAY_NUMERIC;
+    VB_REQUIRE(num == (in_off != nullptr || (num && n == 0)), "%s: in_off is required for numeric[] and only there", fn);
+    const size_t es = src == VB_ARRAY_FLOAT8 ? 8 : num ? 1 : 4;
+    VB_REQUIRE((uintptr_t)in % es == 0 && (uintptr_t)in_off % 8 == 0, "%s: rows must be aligned to their elements", fn);
+    if (host) VB_REQUIRE(cap == 0 || (out_idx && out_val), "%s: null output indices or values", fn);
+    if (n == 0) {
+        if (host) out_row_off[0] = 0;
+        else VB_CUDA(cudaMemsetAsync(out_row_off, 0, sizeof(int64_t), ctx().stream));
+        return VB_OK;
+    }
+#define VB_ASP_CASE(SRC, S, NUM)                                                                                        \
+    if (src == SRC)                                                                                                     \
+        return host ? array_to_sparse_host<S, NUM>(dim, in, in_off, n, cap, out_row_off, out_idx, out_val, out_bad) \
+                    : array_to_sparse_dev<S, NUM>(dim, in, in_off, n, cap, out_row_off, out_idx, out_val, out_bad);
+    VB_ASP_CASE(VB_ARRAY_INT4, int32_t, false)
+    VB_ASP_CASE(VB_ARRAY_FLOAT4, float, false)
+    VB_ASP_CASE(VB_ARRAY_FLOAT8, double, false)
+    VB_ASP_CASE(VB_ARRAY_NUMERIC, float, true)
+#undef VB_ASP_CASE
+    return VB_EINVAL;
 }
 
 // vb_sparsevec_to_dense_batch[_dev]
@@ -1411,6 +1810,16 @@ int vb_dense_to_sparsevec_batch(int elem, int dim, const void* rows, int64_t n, 
 int vb_dense_to_sparsevec_batch_dev(int elem, int dim, const void* rows_dev, int64_t n, int64_t cap, int64_t* out_row_off_dev,
                                     int32_t* out_idx_dev, float* out_val_dev) {
     return dense_to_sparse(elem, dim, rows_dev, n, cap, false, out_row_off_dev, out_idx_dev, out_val_dev);
+}
+
+int vb_array_to_sparsevec_batch(int src, int dim, int32_t typmod, const void* in, const int64_t* in_off, int64_t n, int64_t cap,
+                                int64_t* out_row_off, int32_t* out_idx, float* out_val, int64_t* out_bad) {
+    return array_to_sparse(src, dim, typmod, in, in_off, n, cap, true, out_row_off, out_idx, out_val, out_bad);
+}
+
+int vb_array_to_sparsevec_batch_dev(int src, int dim, int32_t typmod, const void* in_dev, const int64_t* in_off_dev, int64_t n, int64_t cap,
+                                    int64_t* out_row_off_dev, int32_t* out_idx_dev, float* out_val_dev, int64_t* out_bad) {
+    return array_to_sparse(src, dim, typmod, in_dev, in_off_dev, n, cap, false, out_row_off_dev, out_idx_dev, out_val_dev, out_bad);
 }
 
 int vb_sparsevec_to_dense_batch(int elem, int dim, int64_t n, const int64_t* row_off, const int32_t* idx, const float* val, void* out) {

@@ -231,31 +231,96 @@ __device__ __forceinline__ FloatParse round_binary(uint64_t m, int e2, bool stic
     return r;
 }
 
-// The exact decision of a decimal token between two adjacent floats: digits from `d0` (the first significant digit,
-// `point` the position of '.', or -1), `nd` digits in all, value = digits * 10^q10 where q10 is the exponent of the
-// last digit.  Returns the sign of value - (2c + 1) * 2^(h2).  Only the first 120 significant digits are exact; any
-// non-zero digit after them is a sticky excess (a float32 halfway point has at most 113).
-__device__ __noinline__ int decimal_vs_halfway(Lit L, int64_t d0, int64_t nd, int64_t q10, uint64_t c, int h2) {
-    Big<16> D, H;
-    D.set(0);
-    int64_t taken = 0, p = d0;
+// The significant digits of a decimal literal from its first one (at p), skipping the decimal point
+struct TextDigits {
+    Lit L;
+    int64_t p;
+    __device__ __forceinline__ uint32_t next() {
+        while (!is_digit(L.at(p))) ++p;
+        return L.at(p++) - '0';
+    }
+};
+
+// The exact decision of a decimal between two adjacent floats: its nd significant digits from D (D.next() yields them
+// in order), value = digits * 10^q10 where q10 is the exponent of the last digit.  Returns the sign of
+// value - (2c + 1) * 2^(h2).  Only the first 120 significant digits are exact; any non-zero digit after them is a
+// sticky excess (a float32 halfway point has at most 113).
+template <class Digits>
+__device__ __noinline__ int decimal_vs_halfway(Digits D, int64_t nd, int64_t q10, uint64_t c, int h2) {
+    Big<16> A, H;
+    A.set(0);
+    int64_t taken = 0;
     bool sticky = false;
-    for (int64_t i = 0; i < nd; ++p) {
-        const uint32_t ch = L.at(p);
-        if (!is_digit(ch)) continue;       // the decimal point
-        if (taken < 120) { D.mul_add(10, ch - '0'); ++taken; }
-        else if (ch != '0') sticky = true;
-        ++i;
+    for (int64_t i = 0; i < nd; ++i) {
+        const uint32_t v = D.next();
+        if (taken < 120) { A.mul_add(10, v); ++taken; }
+        else if (v != 0) sticky = true;
     }
     const int q = (int)(q10 + (nd - taken));   // within [-190, 40] for a value near a float32
     H.set(2 * c + 1);
-    int s = scaled_cmp(D, q > 0 ? q : 0, q, H, q < 0 ? -q : 0, h2);
+    int s = scaled_cmp(A, q > 0 ? q : 0, q, H, q < 0 ? -q : 0, h2);
     if (s == 0 && sticky) s = 1;
     return s;
 }
 
+// The float32 nearest a decimal (ties to even), with glibc strtof's ERANGE: w = its first `kept` (<= 19) significant
+// digits, value ~ w * 10^scale, trunc = a non-zero digit after them; nd = its significant digits in all, which D yields
+// in order for the exact decision near a halfway point.  w == 0 is a zero.  end is not set.  The one copy of the
+// decimal -> float32 decision: strtof of a literal (parse_float4) and numeric_float4 (vb_numeric.cuh).
+template <class Digits>
+__device__ __forceinline__ FloatParse decimal_to_float(uint64_t w, int kept, int64_t nd, int64_t scale, bool trunc, bool neg,
+                                                       Digits D) {
+    FloatParse r{0.f, 0, false};
+    if (w == 0) { r.v = neg ? -0.f : 0.f; return r; }
+    if (scale > 38) {
+        r.v = neg ? -__int_as_float(0x7f800000) : __int_as_float(0x7f800000);
+        r.erange = true;
+        return r;
+    }
+    if (scale < -64) { r.v = neg ? -0.f : 0.f; r.erange = true; return r; }
+    // exact fast path: w and 10^|scale| both exact in float, one rounding
+    if (!trunc && w <= (1u << 24) && scale >= -10 && scale <= 10) {
+        const float fw = (float)w;
+        r.v = scale >= 0 ? __fmul_rn(fw, kTens[scale]) : __fdiv_rn(fw, kTens[-scale]);
+        if (neg) r.v = -r.v;
+        return r;
+    }
+    // one 64 x 64-bit product against the truncated power: the high word is at most 19 units below the exact value
+    // (a truncated power, a truncated mantissa), so only a product within that distance of a halfway point is undecided
+    const int lz = __clzll((long long)w);
+    const uint64_t W = w << lz;
+    const uint64_t T = kPow10Mant[scale + 64];
+    uint64_t hi = __umul64hi(W, T);
+    const int e2 = kPow10Exp2[scale + 64] + 64 - lz;        // value ~ hi * 2^e2
+    const int msb = 63 - __clzll((long long)hi);
+    const int E = msb + e2;
+    const int keep = E >= -126 ? 24 : E + 150;
+    if (keep == -1) {
+        // within a factor of two below 2^-150, half the least subnormal (or at it, when hi fell short of a power
+        // of two): decided exactly between 0 and 2^-149
+        const int s = decimal_vs_halfway(D, nd, scale - (nd - kept), 0, -150);
+        if (s <= 0) { r.v = neg ? -0.f : 0.f; r.erange = true; return r; }
+        r.v = __int_as_float((int)(1u | (neg ? 0x80000000u : 0u)));
+        return r;
+    }
+    if (keep >= 0) {
+        const int shift = msb + 1 - keep;                   // >= 39
+        const uint64_t rem = shift >= 64 ? hi : hi & ((1ull << shift) - 1);
+        const uint64_t half = 1ull << (shift - 1);
+        if (rem + 64 >= half && rem <= half + 1) {
+            const uint64_t c = shift >= 64 ? 0 : hi >> shift;
+            const int s = decimal_vs_halfway(D, nd, scale - (nd - kept), c, e2 + shift - 1);
+            // decide exactly: c below, c + 1 above, the even one on a tie
+            const bool up = s > 0 || (s == 0 && (c & 1));
+            if (c == 0 && !up) { r.v = neg ? -0.f : 0.f; r.erange = true; return r; }
+            return round_binary((c + (up ? 1 : 0)) << 1, e2 + shift - 1, false, neg);   // exact: kept as is
+        }
+    }
+    return round_binary(hi, e2, true, neg);
+}
+
 // glibc strtof from position p of L in the C locale
-__device__ FloatParse parse_float4(Lit L, int64_t p0) {
+static __device__ FloatParse parse_float4(Lit L, int64_t p0) {
     FloatParse r{0.f, p0, false};
     int64_t p = p0;
     while (is_space(L.at(p))) ++p;
@@ -364,56 +429,7 @@ __device__ FloatParse parse_float4(Lit L, int64_t p0) {
             q = t;
         }
     }
-    r.end = q;
-    if (w == 0) { r.v = neg ? -0.f : 0.f; return r; }
-    if (scale > 38) {
-        r.v = neg ? -__int_as_float(0x7f800000) : __int_as_float(0x7f800000);
-        r.erange = true;
-        return r;
-    }
-    if (scale < -64) { r.v = neg ? -0.f : 0.f; r.erange = true; return r; }
-    // exact fast path: w and 10^|scale| both exact in float, one rounding
-    if (!trunc && w <= (1u << 24) && scale >= -10 && scale <= 10) {
-        const float fw = (float)w;
-        r.v = scale >= 0 ? __fmul_rn(fw, kTens[scale]) : __fdiv_rn(fw, kTens[-scale]);
-        if (neg) r.v = -r.v;
-        return r;
-    }
-    // one 64 x 64-bit product against the truncated power: the high word is at most 19 units below the exact value
-    // (a truncated power, a truncated mantissa), so only a product within that distance of a halfway point is undecided
-    const int lz = __clzll((long long)w);
-    const uint64_t W = w << lz;
-    const uint64_t T = kPow10Mant[scale + 64];
-    uint64_t hi = __umul64hi(W, T);
-    const int e2 = kPow10Exp2[scale + 64] + 64 - lz;        // value ~ hi * 2^e2
-    const int msb = 63 - __clzll((long long)hi);
-    const int E = msb + e2;
-    const int keep = E >= -126 ? 24 : E + 150;
-    if (keep == -1) {
-        // within a factor of two below 2^-150, half the least subnormal (or at it, when hi fell short of a power
-        // of two): decided exactly between 0 and 2^-149
-        const int s = decimal_vs_halfway(L, d0, nd, scale - (nd - kept), 0, -150);
-        if (s <= 0) { r.v = neg ? -0.f : 0.f; r.erange = true; r.end = q; return r; }
-        r.v = __int_as_float((int)(1u | (neg ? 0x80000000u : 0u)));
-        r.end = q;
-        return r;
-    }
-    if (keep >= 0) {
-        const int shift = msb + 1 - keep;                   // >= 39
-        const uint64_t rem = shift >= 64 ? hi : hi & ((1ull << shift) - 1);
-        const uint64_t half = 1ull << (shift - 1);
-        if (rem + 64 >= half && rem <= half + 1) {
-            const uint64_t c = shift >= 64 ? 0 : hi >> shift;
-            const int s = decimal_vs_halfway(L, d0, nd, scale - (nd - kept), c, e2 + shift - 1);
-            // decide exactly: c below, c + 1 above, the even one on a tie
-            const bool up = s > 0 || (s == 0 && (c & 1));
-            if (c == 0 && !up) { r.v = neg ? -0.f : 0.f; r.erange = true; return r; }
-            FloatParse f = round_binary((c + (up ? 1 : 0)) << 1, e2 + shift - 1, false, neg);   // exact: kept as is
-            f.end = q;
-            return f;
-        }
-    }
-    FloatParse f = round_binary(hi, e2, true, neg);
+    FloatParse f = decimal_to_float(w, kept, nd, scale, trunc, neg, TextDigits{L, d0});
     f.end = q;
     return f;
 }
@@ -440,7 +456,7 @@ __device__ __forceinline__ IntParse parse_long(Lit L, int64_t p0, int64_t lo, in
 
 // ------------------------------------------------------------------ float_to_shortest_decimal_bufn
 // sign of c * 10^t - n * 2^s (c, n < 2^40)
-__device__ __noinline__ int dec_vs_bin(uint64_t c, int t, uint64_t n, int s) {
+static __device__ __noinline__ int dec_vs_bin(uint64_t c, int t, uint64_t n, int s) {
     Big<8> A, B;
     A.set(c);
     B.set(n);
@@ -457,7 +473,7 @@ __device__ __forceinline__ int put_uint(char* o, uint64_t v) {
 
 // The shortest decimal that strtof reads back as f, the nearest to f among those (the even digit on a tie); fixed notation when the first
 // digit's exponent X is in [-4, 6), else d[.ddd]e+-XX.  Writes at most 15 bytes to o, returns the count.
-__device__ int format_float4(float f, char* o) {
+static __device__ int format_float4(float f, char* o) {
     const uint32_t u = (uint32_t)__float_as_int(f);
     int n = 0;
     const uint32_t ex = (u >> 23) & 0xff, fr = u & 0x7fffff;

@@ -17,6 +17,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
+from . import numeric as _numeric
 from ._lib import load
 
 VECTOR, HALFVEC = 0, 1
@@ -342,6 +343,89 @@ def halfvec_to_sparsevec(rows, cap=None):
     """halfvec -> sparsevec (src/sparsevec.c:650-689): numpy float16 (or uint16 bit patterns) [n, dim] -> SparseRows; a
     float16 CUDA tensor -> (row_off, idx, val) CUDA tensors; values widened exactly, zeros of either sign dropped"""
     return _to_sparsevec(HALFVEC, rows, cap)
+
+
+ARRAY_INT4, ARRAY_FLOAT4, ARRAY_FLOAT8, ARRAY_NUMERIC = 0, 1, 2, 3   # VB_ARRAY_*: integer[], real[], double precision[], numeric[]
+
+
+class ArrayCastError(ValueError):
+    """an error of array_to_sparsevec: the reference's errmsg, with the failing row (.row)"""
+
+    def __init__(self, msg, row):
+        super().__init__(msg)
+        self.row = row
+
+
+def _array_check(rc, bad):
+    if rc == _lib.EINVAL:
+        msg = load().vb_last_error().decode()
+        if not msg.startswith("vb_"):   # the reference's texts; argument refusals name the entry point
+            raise ArrayCastError(msg, int(bad.value))
+    _lib.check(rc)
+
+
+def array_to_sparsevec(rows, typmod=-1, cap=None):
+    """integer[] / real[] / double precision[] / numeric[] :: sparsevec(typmod) of every row (array_to_sparsevec,
+    src/sparsevec.c:694-821): the dtype (int32, float32, float64) is the array type, each row one array of dim
+    elements, up to 10^9; rows of decimal.Decimal values, or numeric.NumericArrays of numeric_send fields, are
+    numeric[].  An element is (float) of the value (numeric: numeric_float4) and is kept when it is not zero (-0 and
+    doubles that round to 0 are dropped).  Host rows -> SparseRows; CUDA rows -> (row_off, idx, val) CUDA tensors, as
+    vector_to_sparsevec.  cap: an upper bound of the total nnz, if known (one pass); else a first pass sizes the output.
+    The reference's errors raise ArrayCastError (a ValueError) with the failing row."""
+    bad = C.c_int64(-1)
+    in_off = None
+    if _numeric.is_numeric_rows(rows):
+        A, _ = _numeric.as_numeric_arrays(rows)
+        src, n, dim, dev = ARRAY_NUMERIC, A.n, A.dim, A.is_cuda
+        x, in_off = A.data, A.off
+        if not dev:
+            x, in_off = np.ascontiguousarray(x), np.ascontiguousarray(in_off, dtype=np.int64)
+    elif _is_cuda(rows):
+        import torch
+        src, dev = {torch.int32: ARRAY_INT4, torch.float32: ARRAY_FLOAT4, torch.float64: ARRAY_FLOAT8}.get(rows.dtype), True
+        if src is None:
+            raise ValueError("unsupported array type")
+        x = rows.reshape(1, -1) if rows.dim() == 1 else rows
+        if x.dim() != 2:
+            raise ValueError("array must be 1-D")
+        x = x.contiguous()
+        n, dim = int(x.shape[0]), int(x.shape[1])
+    else:
+        x = np.asarray(rows)
+        src, dev = {np.dtype(np.int32): ARRAY_INT4, np.dtype(np.float32): ARRAY_FLOAT4, np.dtype(np.float64): ARRAY_FLOAT8}.get(x.dtype), False
+        if src is None:
+            raise ValueError("unsupported array type")
+        x = x.reshape(1, -1) if x.ndim == 1 else x
+        if x.ndim != 2:
+            raise ValueError("array must be 1-D")
+        x = np.ascontiguousarray(x)
+        n, dim = x.shape
+    if dev:
+        import torch
+        off = torch.empty(n + 1, dtype=torch.int64, device=x.device)
+
+        def run(cap):
+            idx = torch.empty(max(cap, 1), dtype=torch.int32, device=x.device)
+            val = torch.empty(max(cap, 1), dtype=torch.float32, device=x.device)
+            rc = _run_dev("vb_array_to_sparsevec_batch_dev", src, dim, int(typmod), _tp(x), _tp(in_off), n, cap, _tp(off), _tp(idx),
+                          _tp(val), C.byref(bad), tensors=(x,) if in_off is None else (x, in_off))
+            return rc, idx, val
+        total = lambda: int(off[-1].item())   # noqa: E731
+    else:
+        off = np.empty(n + 1, dtype=np.int64)
+
+        def run(cap):
+            idx = np.empty(max(cap, 1), dtype=np.int32)
+            val = np.empty(max(cap, 1), dtype=np.float32)
+            rc = load().vb_array_to_sparsevec_batch(src, dim, int(typmod), _p(x), _p(in_off), n, cap, _p(off), _p(idx), _p(val), C.byref(bad))
+            return rc, idx, val
+        total = lambda: int(off[-1])   # noqa: E731
+    rc, idx, val = run(0 if cap is None else int(cap))
+    if cap is None and rc == _lib.EINVAL and _CAP_ERROR in load().vb_last_error().decode():
+        rc, idx, val = run(total())   # the offsets were written: they size the output
+    _array_check(rc, bad)
+    tot = total()
+    return (off, idx[:tot], val[:tot]) if dev else SparseRows(dim, off, idx[:tot], val[:tot])
 
 
 def _to_dense(elem, rows, dim):
