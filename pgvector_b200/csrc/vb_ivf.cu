@@ -41,7 +41,7 @@ struct Ivf {
     std::vector<int64_t> h_list_off;
     std::vector<int64_t> sorted_len;  // list lengths, descending (bounds candidates per query)
     int64_t last_bytes = 0, last_cand = 0;
-    int64_t* d_cand_sum = nullptr;    // device accumulator of candidates scanned
+    int64_t* d_cand_sum = nullptr;    // device accumulator of candidates scanned (allocated and zeroed with the image)
     ListTile* d_tiles = nullptr;      // static row tiles of the lists (list-major batched scan)
     int n_tiles = 0;
     ListTcImage tc;                   // packed bf16 planes + norms + (list, tile) units, built on first tensor-core scan
@@ -53,21 +53,14 @@ struct Ivf {
     size_t q_bytes[2] = {0, 0};
     int64_t q_nq[2] = {0, 0};
     unsigned* d_ticket = nullptr;     // 2 x ONE_MAX_Q arrival counters of the fused one-query kernels (zero between launches)
-    int* d_tc_fail = nullptr;         // device counters of uncertified queries: [0] probe selection, [1] list scan
-    bool defer_tc_check = false;      // batched search: counters are read once, with the results
-    bool force_exact = false;         // re-run of a batch whose certificate failed
-    bool force_level2 = false;        // re-run of a batch whose level-1 (hi plane only) certificate failed
-    int last_list_level = 0;          // filter level the last batched list scan ran at (0 = exact kernels)
+    int* d_tc_fail = nullptr;         // device counters of uncertified queries: [0] probe selection, [1] list scan (ivf_tc_fail_zero)
     int l1_cooldown = 0;              // batches left before level 1 is tried again after it failed
     int l0_cooldown = 0;              // the same for level 0 (after a batch where it failed often)
-    bool allow_level0 = false;        // set by the batched search, which runs level 0's uncertified queries again on their own
-    bool repairing = false;           // that re-run: it takes the batched filter chain whatever its size
-    bool last_level0 = false;         // the last batched list scan ran at level 0 (last_list_level 0 means the exact kernels)
     int32_t* d_l0_fail = nullptr;     // the queries level 0 could not certify ([d_tc_fail[1]] of them)
     int64_t l0_fail_cap = 0;
-    void* d_repair = nullptr;         // gathered queries and results of such a re-run (device queries / results)
+    void* d_repair = nullptr;         // gathered queries and results of their re-run (device queries / results)
     size_t repair_bytes = 0;
-    int64_t last_tc_failed = 0, total_tc_failed = 0, total_l1_failed = 0, total_l0_failed = 0;
+    int64_t total_tc_failed = 0, total_l1_failed = 0, total_l0_failed = 0;
     bool loaded = false;
     uint64_t generation = 0;          // bumped whenever rows or lists change: an iterative scan handle refuses a changed image
     bool has_ids = false;             // loaded with heap ids (vb_ivf_insert / vb_ivf_delete need them)
@@ -341,10 +334,29 @@ static int ivf_ensure_centre_tc(Ivf& ix) {
     return VB_OK;
 }
 
+// What one pass of probe selection and list scan may do.  A default-constructed pass is a plain one: the filter level is
+// chosen automatically (never level 0), and each tensor-core certificate is read back by the pass itself.
+struct IvfPass {
+    enum Mode { AUTO, LEVEL2, EXACT };
+    Mode mode = AUTO;           // LEVEL2: the repeat of a batch whose level-1 certificate failed; EXACT: no tensor-core filter
+    bool defer_check = false;   // the caller reads the certificate counters (d_tc_fail) at its own synchronisation
+    bool level0 = false;        // the list scan may start at level 0: the caller runs the queries it cannot certify again
+    bool repair = false;        // that re-run: it takes the batched filter chain whatever its size
+};
+constexpr int IVF_LEVEL_EXACT = -1;   // list level of a scan that ran on the exact kernels
+
+// zero the certificate counters, allocating them first.  They are allocated by the first pass that needs them: until then
+// the batched search neither clears nor reads them back.
+static int ivf_tc_fail_zero(Ivf& ix) {
+    if (!ix.d_tc_fail) VB_CUDA(cudaMalloc(&ix.d_tc_fail, 2 * sizeof(int)));
+    VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), ctx().stream));
+    return VB_OK;
+}
+
 // probe selection for a batch of query images: d_probe_lists [nq x probes] ascending by (distance, list), in sc.  *qn: the
 // batch's |q|^2 (list_tc_query_norms), computed here where the tensor-core filter first needs it
-static int ivf_select_probes(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride, int64_t nq, float** qn, int probes, int32_t** d_lists,
-                             float** d_ldist) {
+static int ivf_select_probes(Scratch& sc, Ivf& ix, const IvfPass& pass, const void* qimg, size_t qstride, int64_t nq, float** qn, int probes,
+                             int32_t** d_lists, float** d_ldist) {
     Context& c = ctx();
     void *d_cdist, *d_seg, *d_probe;
     VB_TRY(sc.take(sizeof(float) * (size_t)nq * ix.lists, &d_cdist));
@@ -352,16 +364,13 @@ static int ivf_select_probes(Scratch& sc, Ivf& ix, const void* qimg, size_t qstr
     // query -- approximate distances to all centres, the k' nearest re-scored exactly, order (distance, list number)
     // certified; any uncertified query sends the batch through the exact tiles below.
     const int km = key_metric(ix.metric);
-    bool tc = (c.scan_impl == 2 || c.scan_impl == 4) && !ix.force_exact && nq >= 256 && ix.lists >= 128 &&
+    bool tc = (c.scan_impl == 2 || c.scan_impl == 4) && pass.mode != IvfPass::EXACT && nq >= 256 && ix.lists >= 128 &&
               list_tc_supported(ix.elem, km, probes);
     if (tc) {
         VB_TRY(ivf_ensure_centre_tc(ix));
         tc = ix.ctc.finite && ix.ctc.planes != nullptr;
     }
-    if (tc && !ix.d_tc_fail) {
-        VB_CUDA(cudaMalloc(&ix.d_tc_fail, 2 * sizeof(int)));
-        VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), c.stream));
-    }
+    if (tc && !ix.d_tc_fail) VB_TRY(ivf_tc_fail_zero(ix));
     if (tc) {
         const int kp = list_tc_kp(probes);
         void *d_pairs, *d_seg2, *d_probe2;
@@ -385,14 +394,14 @@ static int ivf_select_probes(Scratch& sc, Ivf& ix, const void* qimg, size_t qstr
         VB_TRY(launch_list_tc(ix.centers, ix.ctc, km, qimg, qstride, nq, zero_lists, 1, pair_off, ix.lists, ix.d_centre_off, 1,
                               (float*)d_cdist, *qn, true));
         int n_failed = 0;
-        if (!ix.defer_tc_check) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, sizeof(int), c.stream));
+        if (!pass.defer_check) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, sizeof(int), c.stream));
         // a run of at most CR_RUN_MAX centre distances is selected inside the refine kernel, a longer one by a launch of its own
         const bool pre = ix.lists > CR_RUN_MAX;
         if (pre) VB_TRY(launch_segment_topk_v((const float*)d_cdist, sb, sl, nullptr, nullptr, nq, kp, pos_kp, key_kp));
         VB_TRY(launch_list_tc_cta_refine(ix.centers, ix.ctc, km, qimg, qstride, nq, probes, kp, 1, zero_lists, pair_off, ix.d_centre_off,
                                          (const float*)d_cdist, nullptr, pre ? pos_kp : nullptr, pre ? key_kp : nullptr, ix.lists, 0, sl,
                                          *qn, lists, ldist, ix.d_tc_fail, 2));
-        if (!ix.defer_tc_check) {
+        if (!pass.defer_check) {
             VB_CUDA(cudaMemcpyAsync(&n_failed, ix.d_tc_fail, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
             VB_CUDA(cudaStreamSynchronize(c.stream));
         }
@@ -498,12 +507,13 @@ static int ivf_ensure_l0_image(Ivf& ix) {
 }
 
 // scan the given probe lists for a batch of queries and keep the k nearest per query (mask: of the rows each query's
-// row filter allows); *cand_total_dev is in sc, *qn as in ivf_select_probes
-static int ivf_scan_topk(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride, int64_t nq, float** qn, const int32_t* d_lists, int probes, int k,
-                         int64_t* out_ids_dev, float* out_f_dev, double* out_d_dev, int32_t** cand_total_dev, const IvfMask* mask = nullptr) {
+// row filter allows).  cap bounds the candidates of one query; *qn as in ivf_select_probes; *level: the filter level
+// the scan ran at, or IVF_LEVEL_EXACT
+static int ivf_scan_topk(Scratch& sc, Ivf& ix, const IvfPass& pass, const void* qimg, size_t qstride, int64_t nq, float** qn,
+                         const int32_t* d_lists, int probes, int64_t cap, int k, int64_t* out_ids_dev, float* out_f_dev, double* out_d_dev,
+                         int* level_out = nullptr, const IvfMask* mask = nullptr) {
     Context& c = ctx();
     const int rpc = scan_chunk_rows(ix.rows);
-    const int64_t cap = ivf_cap(ix, probes);
     const int64_t max_chunks = nq * (cap / rpc + probes + 1);
     VB_REQUIRE(max_chunks < (int64_t)INT32_MAX, "too many scan chunks (%lld)", (long long)max_chunks);
     void *d_chunks, *d_seg, *d_dist, *d_pos;
@@ -515,10 +525,6 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride,
     int32_t* seg_len = (int32_t*)(seg_begin + nq);
     int* n_chunks = (int*)(seg_len + nq);
     VB_CUDA(cudaMemsetAsync(n_chunks, 0, sizeof(int), c.stream));
-    if (!ix.d_cand_sum) {
-        VB_CUDA(cudaMalloc(&ix.d_cand_sum, sizeof(int64_t)));
-        VB_CUDA(cudaMemsetAsync(ix.d_cand_sum, 0, sizeof(int64_t), c.stream));
-    }
     // chunk descriptors are for the per-query scan kernels only; batched scans (tensor-core filter, list-major) skip them
     const bool per_query_scan = !(list_major_supported(ix.elem, key_metric(ix.metric)) && ix.n_tiles > 0 &&
                                   (c.scan_impl >= 3 || (c.scan_impl == 2 && nq * probes >= 256)));
@@ -535,29 +541,30 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride,
     // so each probed list is read once per batch instead of once per query; small k goes through the tensor-core
     // filter (HBM-bound), larger k through the fp32 list-major kernel (FMA-pipe bound).
     const int km = key_metric(ix.metric);
-    const bool batched = nq * probes >= 256 || ix.repairing;
-    bool tc = (c.scan_impl == 4 || c.scan_impl == 2) && !ix.force_exact && batched && list_tc_supported(ix.elem, km, k) && ix.rows.n > 0;
+    const bool batched = nq * probes >= 256 || pass.repair;
+    bool tc = (c.scan_impl == 4 || c.scan_impl == 2) && pass.mode != IvfPass::EXACT && batched && list_tc_supported(ix.elem, km, k) &&
+              ix.rows.n > 0;
     if (tc) {
         VB_TRY(ivf_ensure_tc_image(ix));
         tc = ix.tc.finite;   // rows with Inf / NaN norms have no error bound: exact path
     }
-    ix.last_list_level = 0;
-    ix.last_level0 = false;
+    if (level_out) *level_out = IVF_LEVEL_EXACT;
     if (tc) {
         // level 1 reads only the hi plane of the rows (half the HBM traffic, error bound 2^-7 |x||q|): it certifies
         // whenever the neighbours are separated by more than that, otherwise the batch is repeated at level 2 (both
         // planes, 2^-12) and level 1 rests for a while
-        int level = (c.tc_level1 && !ix.force_level2 && ix.l1_cooldown == 0 && list_tc_kp(k, 1) <= 128) ? 1 : 2;
-        if (ix.l1_cooldown > 0 && !ix.force_level2) --ix.l1_cooldown;
+        const bool level2 = pass.mode == IvfPass::LEVEL2;
+        int level = (c.tc_level1 && !level2 && ix.l1_cooldown == 0 && list_tc_kp(k, 1) <= 128) ? 1 : 2;
+        if (ix.l1_cooldown > 0 && !level2) --ix.l1_cooldown;
         // slab minima for the selection (vb_common.cuh slab_base): with them the k' nearest are found from 32 k' candidates
         // per query instead of the whole run
         const int64_t cap_s = slab_cap(cap, probes);
         const bool slabs_fit = c.slab_select && nq * cap_s < (int64_t)INT32_MAX &&
                                (size_t)cap_s * 4 + 20 * 1024 <= 160 * 1024;
         // level 0 in front of level 1: int8 rows (1 byte per element, bound ~R_max |q|, k' = 128).  Its uncertified queries
-        // are listed by the one-CTA-per-query refine and searched again on their own by the batched search
-        // (ivf_search_impl), the only caller that allows it.
-        if (level == 1 && c.tc_level0 && ix.allow_level0 && slabs_fit && list_tc_kp(k, 0) <= 128) {
+        // are listed by the one-CTA-per-query refine, and a pass allows it only where its caller searches them again on
+        // their own.
+        if (level == 1 && c.tc_level0 && pass.level0 && slabs_fit && list_tc_kp(k, 0) <= 128) {
             if (ix.l0_cooldown > 0) {
                 --ix.l0_cooldown;
             } else {
@@ -570,8 +577,7 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride,
             VB_CUDA(cudaMalloc(&ix.d_l0_fail, sizeof(int32_t) * (size_t)nq));
             ix.l0_fail_cap = nq;
         }
-        ix.last_list_level = level;
-        ix.last_level0 = level == 0;
+        if (level_out) *level_out = level;
         const int kp = list_tc_kp(k, level);
         const bool slabs = slabs_fit && kp <= 128;
         void* d_smin = nullptr;
@@ -590,12 +596,9 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride,
         float* key_kp = (float*)(pos_kp + (size_t)nq * kp);
         prof_begin(VB_PROF_TOPK);
         int n_failed = 0;
-        if (!ix.d_tc_fail) {
-            VB_CUDA(cudaMalloc(&ix.d_tc_fail, 2 * sizeof(int)));
-            VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), c.stream));
-        }
-        if (!ix.defer_tc_check) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail + 1, 0, sizeof(int), c.stream));
-        if (slabs && !ix.force_level2) {
+        if (!ix.d_tc_fail) VB_TRY(ivf_tc_fail_zero(ix));
+        if (!pass.defer_check) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail + 1, 0, sizeof(int), c.stream));
+        if (slabs && !level2) {
             // one CTA per query: slab selection, re-score on eight warps, ranking, certificate (a selection that overflows
             // counts as uncertified: the repeat of the batch selects below)
             VB_TRY(launch_list_tc_cta_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
@@ -612,12 +615,11 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride,
                                              (const float*)d_dist, nullptr, pos_kp, key_kp, cap, cap_s, seg_len, *qn, pos, key,
                                              ix.d_tc_fail + 1, level, nullptr, has_nan));
         }
-        if (!ix.defer_tc_check) {
+        if (!pass.defer_check) {
             VB_CUDA(cudaMemcpyAsync(&n_failed, ix.d_tc_fail + 1, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
             VB_CUDA(cudaStreamSynchronize(c.stream));
         }
         prof_end(VB_PROF_TOPK);
-        ix.last_tc_failed = n_failed;
         ix.total_tc_failed += n_failed;
         if (n_failed == 0) {
             ivf_finish_kernel<<<(unsigned)((nq * k + 255) / 256), 256, 0, c.stream>>>(ix.metric, nq, k, probes, pos, key, d_lists, cand_off,
@@ -628,7 +630,6 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride,
             if (mask)
                 VB_TRY(ivf_unmask(ix, *mask, nq, k, probes, pos, key, (const float*)d_dist, cap, d_lists, cand_off, out_ids_dev, out_f_dev,
                                   out_d_dev));
-            if (cand_total_dev) *cand_total_dev = seg_len;
             return VB_OK;
         }
         // some certificate failed: the whole batch goes through the exact kernel below (rare by construction)
@@ -667,7 +668,6 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride,
     count_launch();
     if (mask)
         VB_TRY(ivf_unmask(ix, *mask, nq, k, probes, pos, key, (const float*)d_dist, cap, d_lists, cand_off, out_ids_dev, out_f_dev, out_d_dev));
-    if (cand_total_dev) *cand_total_dev = seg_len;
     return VB_OK;
 }
 
@@ -769,7 +769,6 @@ static int ivf_one_probes(Scratch& sc, Ivf& ix, const void* qimg, size_t qstride
     float* ldist = (float*)(lists + (size_t)nq * probes);
     unsigned *tp, *ts;
     VB_TRY(ivf_tickets(ix, &tp, &ts));
-    if (!ix.d_cand_sum) VB_CUDA(cudaMalloc(&ix.d_cand_sum, sizeof(int64_t)));
     prof_begin(VB_PROF_SCAN_LISTS);
     VB_TRY(launch_one_probe(ix.centers, key_metric(ix.metric), qimg, qstride, nq, probes, (float*)d_cdist, tp, lists, ldist, ix.d_cand_sum));
     prof_end(VB_PROF_SCAN_LISTS);
@@ -787,7 +786,6 @@ static int ivf_one_items(Ivf& ix, const void* qimg, size_t qstride, int64_t nq, 
     VB_TRY(sc.take(sizeof(float) * (size_t)nq * cap, &d_dist));
     unsigned *tp, *ts;
     VB_TRY(ivf_tickets(ix, &tp, &ts));
-    if (!ix.d_cand_sum) VB_CUDA(cudaMalloc(&ix.d_cand_sum, sizeof(int64_t)));
     prof_begin(VB_PROF_SCAN_ITEMS);
     VB_TRY(launch_one_scan(ix.rows, key_metric(ix.metric), ix.metric, ix.d_list_off, ix.d_ids, d_lists, probes, qimg, qstride, nq, k, cap,
                            (float*)d_dist, ts, out_ids_dev, out_f_dev, out_d_dev, nullptr, ix.d_cand_sum, cand_store));
@@ -928,7 +926,7 @@ static int ivf_scan_setup(vb_ivf_scan& s, const void* queries) {
         if (c.one_query && m <= ONE_MAX_Q && one_probe_fits(ix.lists, s.qstride, s.max_probes))
             VB_TRY(ivf_one_probes(sc, ix, mine, s.qstride, m, s.max_probes, &d_lists, &d_ldist));
         else
-            VB_TRY(ivf_select_probes(sc, ix, mine, s.qstride, m, &qn, s.max_probes, &d_lists, &d_ldist));
+            VB_TRY(ivf_select_probes(sc, ix, IvfPass{}, mine, s.qstride, m, &qn, s.max_probes, &d_lists, &d_ldist));
         VB_CUDA(cudaMemcpyAsync(s.probe + (size_t)q0 * s.max_probes, d_lists, sizeof(int32_t) * (size_t)m * s.max_probes,
                                 cudaMemcpyDeviceToDevice, c.stream));
     }
@@ -1134,8 +1132,12 @@ int vb_ivf_create(int elem, int metric, int dim, int lists, vb_ivf** out) {
     VB_REQUIRE(out && elem >= 0 && elem <= 2 && dim > 0 && lists >= 1 && lists <= 32768, "bad ivfflat arguments (lists 1..32768, src/ivfflat.h:56-57)");
     bool ok = elem == VB_BIT ? metric == VB_HAMMING : (metric == VB_L2_SQUARED || metric == VB_NEG_IP);
     VB_REQUIRE(ok, "ivfflat opclass proc 1 must be L2 squared / negative inner product (vector, halfvec) or Hamming (bit)");
+    int64_t* d_cand_sum;
+    VB_CUDA(cudaMalloc(&d_cand_sum, sizeof(int64_t)));
+    VB_CUDA(cudaMemsetAsync(d_cand_sum, 0, sizeof(int64_t), ctx().stream));
     vb_ivf* h = new vb_ivf();
     Ivf& ix = h->ix;
+    ix.d_cand_sum = d_cand_sum;
     ix.elem = elem;
     ix.metric = metric;
     ix.dim = dim;
@@ -1436,7 +1438,7 @@ static int ivf_insert_lists(Ivf& ix, const void* rows, int64_t n, bool host, int
         if (c.one_query && m <= ONE_MAX_Q && one_probe_fits(ix.lists, qstride, 1))
             VB_TRY(ivf_one_probes(sc, ix, qimg, qstride, m, 1, &d_lists, &d_ldist));
         else
-            VB_TRY(ivf_select_probes(sc, ix, qimg, qstride, m, &qn, 1, &d_lists, &d_ldist));
+            VB_TRY(ivf_select_probes(sc, ix, IvfPass{}, qimg, qstride, m, &qn, 1, &d_lists, &d_ldist));
         VB_CUDA(cudaMemcpyAsync(out + q0, d_lists, sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c.stream));
         if (ix.elem != VB_BIT) {   // (Hamming distances are never NaN)
             void* d_d0;
@@ -2058,7 +2060,7 @@ int vb_ivf_scan_lists(vb_ivf* h, const void* queries, int64_t nq, int max_probes
         return VB_OK;
     }
     float* qn = nullptr;
-    VB_TRY(ivf_select_probes(sc, ix, qimg, qstride, nq, &qn, probes, &d_lists, &d_ldist));
+    VB_TRY(ivf_select_probes(sc, ix, IvfPass{}, qimg, qstride, nq, &qn, probes, &d_lists, &d_ldist));
     std::vector<int32_t> hl((size_t)nq * probes);
     std::vector<float> hd((size_t)nq * probes);
     VB_CUDA(cudaMemcpyAsync(hl.data(), d_lists, sizeof(int32_t) * hl.size(), cudaMemcpyDeviceToHost, c.stream));
@@ -2128,13 +2130,10 @@ int vb_ivf_scan_items(vb_ivf* h, const void* q, const int32_t* lists, int nlists
     }
     VB_CUDA(cudaMemcpyAsync(d_misc, lists, sizeof(int32_t) * (size_t)nlists, cudaMemcpyHostToDevice, c.stream));
     VB_CUDA(cudaStreamSynchronize(c.stream));
-    // capacity bound must cover these particular lists
-    std::vector<int64_t> saved = ix.sorted_len;
-    ix.sorted_len.assign(1, total);
     float* qn = nullptr;
-    int rc = ivf_scan_topk(sc, ix, qimg, qstride, 1, &qn, (const int32_t*)d_misc, nlists, (int)k, o_ids, nullptr, o_d, nullptr);
-    ix.sorted_len = saved;
-    VB_TRY(rc);
+    // capacity bound: these particular lists
+    VB_TRY(ivf_scan_topk(sc, ix, IvfPass{}, qimg, qstride, 1, &qn, (const int32_t*)d_misc, nlists, std::max<int64_t>(total, 1), (int)k, o_ids,
+                         nullptr, o_d));
     VB_CUDA(cudaMemcpyAsync(out_ids, o_ids, sizeof(int64_t) * (size_t)k, cudaMemcpyDeviceToHost, c.stream));
     VB_CUDA(cudaMemcpyAsync(out_dist, o_d, sizeof(double) * (size_t)k, cudaMemcpyDeviceToHost, c.stream));
     VB_CUDA(cudaStreamSynchronize(c.stream));
@@ -2164,7 +2163,7 @@ struct IvfFilterSpec {
 };
 
 static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, bool host, bool q_host, int64_t* out_ids,
-                           float* out_f, double* out_d, bool level0 = true, const IvfFilterSpec* filt = nullptr);
+                           float* out_f, double* out_d, bool repair = false, const IvfFilterSpec* filt = nullptr);
 
 // the mask arguments of queries [q0, q0 + m) of a filtered call (in sc): the filters' positions and runs, in place
 static int ivf_upload_mask(Scratch& sc, const IvfFilterSpec& filt, int64_t q0, int64_t m, IvfMask* mk) {
@@ -2182,11 +2181,6 @@ static int ivf_upload_mask(Scratch& sc, const IvfFilterSpec& filt, int64_t q0, i
     mk->has_nan = fq + m;
     return VB_OK;
 }
-
-struct ResetFlag {   // clears a flag on every exit of a scope
-    bool& f;
-    ~ResetFlag() { f = false; }
-};
 
 // The queries `fail` (numbers within `queries`, nf of them) that level 0 could not certify are searched again on their own,
 // from level 1 on, and their rows of the outputs overwritten.  The re-run takes the batched filter chain whatever its size
@@ -2237,12 +2231,10 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
         count_launch();
     }
     VB_CUDA(cudaMemcpyAsync(d_cand_saved, ix.d_cand_sum, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
-    ResetFlag flag{ix.repairing};
-    ix.repairing = true;
     if (host) {
         std::vector<int64_t> ti((size_t)nf * k);
         std::vector<double> td((size_t)nf * k);
-        VB_TRY(ivf_search_impl(h, sub, nf, probes, k, true, q_host, ti.data(), nullptr, td.data(), false, filt));
+        VB_TRY(ivf_search_impl(h, sub, nf, probes, k, true, q_host, ti.data(), nullptr, td.data(), true, filt));
         VB_CUDA(cudaMemcpyAsync(ix.d_cand_sum, d_cand_saved, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
         for (int64_t i = 0; i < nf; ++i) {
             memcpy(out_ids + (size_t)fail[(size_t)i] * k, ti.data() + (size_t)i * k, sizeof(int64_t) * k);
@@ -2250,7 +2242,7 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
         }
         return VB_OK;
     }
-    VB_TRY(ivf_search_impl(h, sub, nf, probes, k, false, false, d_ids, d_f, nullptr, false, filt));
+    VB_TRY(ivf_search_impl(h, sub, nf, probes, k, false, false, d_ids, d_f, nullptr, true, filt));
     VB_CUDA(cudaMemcpyAsync(ix.d_cand_sum, d_cand_saved, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
     scatter_results_kernel<<<(unsigned)((nf * k + 255) / 256), 256, 0, c.stream>>>(d_ids, d_f, d_idx, nf, k, out_ids, out_f);
     VB_CUDA(cudaGetLastError());
@@ -2258,10 +2250,55 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
     return VB_OK;
 }
 
-// host: results go to host memory (int64 ids + float8 distances); q_host: the queries are host memory.  level0: the list
-// scan may start at filter level 0 (false for the re-run of the queries it could not certify)
+// The certificate repeat policy of one sub-batch of the batched search.  run(pass, fails, &level) computes the sub-batch
+// once: the queries its probe selection (fails[0]) and list scan (fails[1]) could not certify, and the list level it ran
+// at.  The tensor-core filter runs optimistically: the counters are read back together with the results (one
+// synchronisation per pass).  pass is the first, automatic pass: where its level0 lets the list scan start at level 0,
+// repair(n) searches the n queries level 0 could not certify again on their own.  Otherwise a sub-batch with an
+// uncertified query is run again at level 2 when level 1 failed, then on the exact kernels.
+static int ivf_certified_batch(Ivf& ix, int probes, IvfPass pass, const std::function<int(const IvfPass&, int*, int*)>& run,
+                               const std::function<int(int)>& repair) {
+    int fails[2], level;
+    pass.defer_check = true;
+    VB_TRY(run(pass, fails, &level));
+    pass.level0 = false;   // (a repeat never starts at level 0)
+    auto exact = [&] {
+        pass.mode = IvfPass::EXACT;
+        pass.defer_check = false;
+        return run(pass, fails, &level);
+    };
+    if (fails[0] == 0 && fails[1] > 0 && level == 0) {
+        // level 0 could not separate the neighbours of some queries: only those go on, from level 1.  Their re-run
+        // streams the lists they probe at level 1: with n failed queries, about 1 - (1 - probes / lists)^n of what a
+        // level-1 pass over the batch streams, while level 0 saved half of that pass.  Past a quarter (the re-run also
+        // selects probes and synchronises again) level 0 no longer pays, and it rests for the next 64 batches (the data
+        // decides this, not the batch).  At 1000 lists and probes 10 that is 29 failed queries.
+        ix.total_l0_failed += fails[1];
+        if (1.0 - std::pow(1.0 - (double)probes / ix.lists, (double)fails[1]) > 0.25) ix.l0_cooldown = 64;
+        const int64_t exact0 = ix.total_tc_failed;
+        VB_TRY(repair(fails[1]));
+        return ix.total_tc_failed > exact0 ? exact() : VB_OK;   // neither level 1 nor 2 certified them
+    }
+    if (fails[0] == 0 && fails[1] > 0 && level == 1) {
+        // the hi-plane filter could not separate the neighbours of some query: both planes, and leave level 1 alone
+        // for the next batches (the data decides this, not the batch)
+        ix.total_l1_failed += fails[1];
+        ix.l1_cooldown = 64;
+        pass.mode = IvfPass::LEVEL2;
+        VB_TRY(run(pass, fails, &level));
+    }
+    if (fails[0] + fails[1] > 0) {
+        ix.total_tc_failed += fails[0] + fails[1];
+        return exact();
+    }
+    return VB_OK;
+}
+
+// host: results go to host memory (int64 ids + float8 distances); q_host: the queries are host memory.  repair: the re-run
+// of the queries level 0 could not certify (ivf_repair_level0), which never starts at level 0 and adds to its caller's
+// candidate count
 static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, bool host, bool q_host, int64_t* out_ids,
-                           float* out_f, double* out_d, bool level0, const IvfFilterSpec* filt) {
+                           float* out_f, double* out_d, bool repair, const IvfFilterSpec* filt) {
     VB_TRY(require_init());
     VB_REQUIRE(h && h->ix.loaded, "index not loaded");
     VB_REQUIRE(queries && probes >= 1 && k >= 1, "bad search arguments");
@@ -2270,10 +2307,10 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
     probes = std::min(probes, ix.lists);
     if (nq <= 0) return VB_OK;
     const size_t rawq = raw_row_bytes(ix.elem, ix.dim);
+    const int64_t cap = ivf_cap(ix, probes);
     // (the fused one-query kernels select inside the scan: a filtered call takes the general path and its mask)
-    if (!ix.repairing && !filt && ivf_one_applies(ix, nq, probes, k, ivf_cap(ix, probes))) {
+    if (!repair && !filt && ivf_one_applies(ix, nq, probes, k, cap)) {
         // a handful of queries (one backend's scan): two fused launches, no memsets, one copy back
-        const int64_t cap = ivf_cap(ix, probes);
         Scratch sc;
         void* qimg;
         size_t qstride;
@@ -2296,98 +2333,64 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
         return VB_OK;
     }
     const int64_t bq = ivf_batch_limit(ix, probes);
-    if (!ix.d_cand_sum) VB_CUDA(cudaMalloc(&ix.d_cand_sum, sizeof(int64_t)));
-    if (level0) VB_CUDA(cudaMemsetAsync(ix.d_cand_sum, 0, sizeof(int64_t), c.stream));   // (a re-run adds to its caller's count)
-    // One pass of a sub-batch.  The tensor-core filter runs optimistically: its certificate counters are read back
-    // together with the results (one synchronisation per sub-batch).  Queries level 0 could not certify are listed and
-    // searched again on their own; otherwise a sub-batch with an uncertified query is run again at level 2, then on the
-    // exact kernels.
+    if (!repair) VB_CUDA(cudaMemsetAsync(ix.d_cand_sum, 0, sizeof(int64_t), c.stream));
     constexpr int L0_LIST_READ = 64;   // failed queries read back with the counters (more take a second copy)
     int32_t l0_list[L0_LIST_READ];
-    auto run = [&](int64_t q0, int64_t m, int mode, int* fails) -> int {   // mode 0: automatic, 1: filter level 2, 2: exact
-        const bool exact = mode == 2;
-        ix.force_exact = exact;
-        ix.force_level2 = mode == 1;
-        ix.defer_tc_check = !exact;
-        ResetFlag reset{ix.allow_level0};
-        ix.allow_level0 = level0 && mode == 0;
-        if (ix.d_tc_fail) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), c.stream));
-        Scratch sc;
-        void* qimg;
-        size_t qstride;
-        VB_TRY(upload_queries(sc, ix.elem, ix.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, q_host, &qimg, &qstride));
-        IvfMask mk{};
-        if (filt) VB_TRY(ivf_upload_mask(sc, *filt, q0, m, &mk));
-        const IvfMask* mask = filt ? &mk : nullptr;
-        int32_t* d_lists;
-        float* d_ldist;
-        float* qn = nullptr;   // |q|^2 of the sub-batch, shared by its probe selection and its list scan
-        VB_TRY(ivf_select_probes(sc, ix, qimg, qstride, m, &qn, probes, &d_lists, &d_ldist));
-        if (host) {
-            void* d_out;
-            VB_TRY(sc.take((sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
-            int64_t* o_ids = (int64_t*)d_out;
-            double* o_d = (double*)(o_ids + (size_t)m * k);
-            VB_TRY(ivf_scan_topk(sc, ix, qimg, qstride, m, &qn, d_lists, probes, k, o_ids, nullptr, o_d, nullptr, mask));
-            VB_CUDA(cudaMemcpyAsync(out_ids + q0 * k, o_ids, sizeof(int64_t) * (size_t)m * k, cudaMemcpyDeviceToHost, c.stream));
-            VB_CUDA(cudaMemcpyAsync(out_d + q0 * k, o_d, sizeof(double) * (size_t)m * k, cudaMemcpyDeviceToHost, c.stream));
-        } else {
-            VB_TRY(ivf_scan_topk(sc, ix, qimg, qstride, m, &qn, d_lists, probes, k, out_ids + q0 * k, out_f + q0 * k, nullptr, nullptr, mask));
-        }
-        fails[0] = fails[1] = 0;
-        const bool check = !exact && ix.d_tc_fail != nullptr;
-        if (check) VB_CUDA(cudaMemcpyAsync(fails, ix.d_tc_fail, 2 * sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-        if (check && ix.last_level0)
-            VB_CUDA(cudaMemcpyAsync(l0_list, ix.d_l0_fail, sizeof(int32_t) * (size_t)std::min<int64_t>(m, L0_LIST_READ),
-                                    cudaMemcpyDeviceToHost, c.stream));
-        if (host || check) VB_CUDA(cudaStreamSynchronize(c.stream));
-        return VB_OK;
-    };
-    int rc = VB_OK;
-    for (int64_t q0 = 0; q0 < nq && rc == VB_OK; q0 += bq) {
+    IvfPass first;
+    first.level0 = !repair;
+    first.repair = repair;
+    for (int64_t q0 = 0; q0 < nq; q0 += bq) {
         const int64_t m = std::min(bq, nq - q0);
-        int fails[2];
-        rc = run(q0, m, 0, fails);
-        if (rc == VB_OK && fails[0] == 0 && fails[1] > 0 && ix.last_level0) {
-            // level 0 could not separate the neighbours of some queries: only those go on, from level 1.  Their re-run
-            // streams the lists they probe at level 1: with n failed queries, about 1 - (1 - probes / lists)^n of what a
-            // level-1 pass over the batch streams, while level 0 saved half of that pass.  Past a quarter (the re-run also
-            // selects probes and synchronises again) level 0 no longer pays, and it rests for the next 64 batches (the data
-            // decides this, not the batch).  At 1000 lists and probes 10 that is 29 failed queries.
-            ix.total_l0_failed += fails[1];
-            if (1.0 - std::pow(1.0 - (double)probes / ix.lists, (double)fails[1]) > 0.25) ix.l0_cooldown = 64;
-            std::vector<int32_t> fail(l0_list, l0_list + std::min(fails[1], L0_LIST_READ));
-            if (fails[1] > L0_LIST_READ) {
-                fail.resize((size_t)fails[1]);
-                VB_CUDA(cudaMemcpy(fail.data(), ix.d_l0_fail, sizeof(int32_t) * (size_t)fails[1], cudaMemcpyDeviceToHost));
+        auto run = [&](const IvfPass& pass, int* fails, int* level) -> int {
+            if (ix.d_tc_fail) VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), c.stream));
+            Scratch sc;
+            void* qimg;
+            size_t qstride;
+            VB_TRY(upload_queries(sc, ix.elem, ix.dim, (const uint8_t*)queries + (size_t)q0 * rawq, m, q_host, &qimg, &qstride));
+            IvfMask mk{};
+            if (filt) VB_TRY(ivf_upload_mask(sc, *filt, q0, m, &mk));
+            const IvfMask* mask = filt ? &mk : nullptr;
+            int32_t* d_lists;
+            float* d_ldist;
+            float* qn = nullptr;   // |q|^2 of the sub-batch, shared by its probe selection and its list scan
+            VB_TRY(ivf_select_probes(sc, ix, pass, qimg, qstride, m, &qn, probes, &d_lists, &d_ldist));
+            if (host) {
+                void* d_out;
+                VB_TRY(sc.take((sizeof(int64_t) + sizeof(double)) * (size_t)m * k, &d_out));
+                int64_t* o_ids = (int64_t*)d_out;
+                double* o_d = (double*)(o_ids + (size_t)m * k);
+                VB_TRY(ivf_scan_topk(sc, ix, pass, qimg, qstride, m, &qn, d_lists, probes, cap, k, o_ids, nullptr, o_d, level, mask));
+                VB_CUDA(cudaMemcpyAsync(out_ids + q0 * k, o_ids, sizeof(int64_t) * (size_t)m * k, cudaMemcpyDeviceToHost, c.stream));
+                VB_CUDA(cudaMemcpyAsync(out_d + q0 * k, o_d, sizeof(double) * (size_t)m * k, cudaMemcpyDeviceToHost, c.stream));
+            } else {
+                VB_TRY(ivf_scan_topk(sc, ix, pass, qimg, qstride, m, &qn, d_lists, probes, cap, k, out_ids + q0 * k, out_f + q0 * k, nullptr,
+                                     level, mask));
             }
-            const int64_t exact0 = ix.total_tc_failed;
+            fails[0] = fails[1] = 0;
+            const bool check = pass.defer_check && ix.d_tc_fail != nullptr;
+            if (check) VB_CUDA(cudaMemcpyAsync(fails, ix.d_tc_fail, 2 * sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+            if (check && *level == 0)
+                VB_CUDA(cudaMemcpyAsync(l0_list, ix.d_l0_fail, sizeof(int32_t) * (size_t)std::min<int64_t>(m, L0_LIST_READ),
+                                        cudaMemcpyDeviceToHost, c.stream));
+            if (host || check) VB_CUDA(cudaStreamSynchronize(c.stream));
+            return VB_OK;
+        };
+        auto repair_level0 = [&](int n_failed) -> int {
+            std::vector<int32_t> fail(l0_list, l0_list + std::min(n_failed, L0_LIST_READ));
+            if (n_failed > L0_LIST_READ) {
+                fail.resize((size_t)n_failed);
+                VB_CUDA(cudaMemcpy(fail.data(), ix.d_l0_fail, sizeof(int32_t) * (size_t)n_failed, cudaMemcpyDeviceToHost));
+            }
             IvfFilterSpec sub_filt;
             if (filt) {
                 sub_filt = *filt;
                 if (filt->fq) sub_filt.fq = filt->fq + q0;
             }
-            rc = ivf_repair_level0(h, (const uint8_t*)queries + (size_t)q0 * rawq, fail, probes, k, host, q_host, out_ids + q0 * k,
-                                   out_f ? out_f + q0 * k : nullptr, out_d ? out_d + q0 * k : nullptr, filt ? &sub_filt : nullptr);
-            if (rc == VB_OK && ix.total_tc_failed > exact0) rc = run(q0, m, 2, fails);   // neither level 1 nor 2 certified them
-            continue;
-        }
-        if (rc == VB_OK && fails[0] == 0 && fails[1] > 0 && ix.last_list_level == 1) {
-            // the hi-plane filter could not separate the neighbours of some query: both planes, and leave level 1 alone
-            // for the next batches (the data decides this, not the batch)
-            ix.total_l1_failed += fails[1];
-            ix.l1_cooldown = 64;
-            rc = run(q0, m, 1, fails);
-        }
-        if (rc == VB_OK && fails[0] + fails[1] > 0) {
-            ix.total_tc_failed += fails[0] + fails[1];
-            rc = run(q0, m, 2, fails);
-        }
+            return ivf_repair_level0(h, (const uint8_t*)queries + (size_t)q0 * rawq, fail, probes, k, host, q_host, out_ids + q0 * k,
+                                     out_f ? out_f + q0 * k : nullptr, out_d ? out_d + q0 * k : nullptr, filt ? &sub_filt : nullptr);
+        };
+        VB_TRY(ivf_certified_batch(ix, probes, first, run, repair_level0));
     }
-    ix.force_exact = false;
-    ix.force_level2 = false;
-    ix.defer_tc_check = false;
-    VB_TRY(rc);
     ix.last_cand = -1;  // fetched lazily
     ix.last_bytes = nq;
     return VB_OK;
@@ -2433,10 +2436,10 @@ static int ivf_search_filtered_impl(const char* fn, vb_ivf* h, const void* queri
     if (nq <= 0) return VB_OK;
     VB_REQUIRE(out_ids && (out_f || out_d), "%s: null output", fn);
     const IvfFilterSpec filt{filters, nfilters, nfilters > 1 ? filter_of_query : nullptr};
-    if (!host) return ivf_search_impl(h, queries, nq, probes, k, false, false, out_ids, out_f, nullptr, true, &filt);
+    if (!host) return ivf_search_impl(h, queries, nq, probes, k, false, false, out_ids, out_f, nullptr, false, &filt);
     std::vector<int64_t> ids((size_t)nq * k);
     std::vector<double> dist((size_t)nq * k);
-    VB_TRY(ivf_search_impl(h, queries, nq, probes, k, true, true, ids.data(), nullptr, dist.data(), true, &filt));
+    VB_TRY(ivf_search_impl(h, queries, nq, probes, k, true, true, ids.data(), nullptr, dist.data(), false, &filt));
     memcpy(out_ids, ids.data(), sizeof(int64_t) * ids.size());
     memcpy(out_d, dist.data(), sizeof(double) * dist.size());
     return VB_OK;
@@ -2529,16 +2532,11 @@ int vb_ivf_search_sharded_dev(vb_ivf* h, const void* queries_dev, int64_t nq, in
     float* my_dist = (float*)((uint8_t*)d_res + res_ids);
     int64_t* all_ids = (int64_t*)((uint8_t*)d_res + res_ids + res_dist);
     float* all_dist = (float*)((uint8_t*)all_ids + res_ids * (size_t)world);
-    if (!ix.d_cand_sum) VB_CUDA(cudaMalloc(&ix.d_cand_sum, sizeof(int64_t)));
     VB_CUDA(cudaMemsetAsync(ix.d_cand_sum, 0, sizeof(int64_t), c.stream));
-    if (!ix.d_tc_fail) VB_CUDA(cudaMalloc(&ix.d_tc_fail, 2 * sizeof(int)));
+    const int64_t cap = ivf_cap(ix, probes);
 
-    auto run = [&](int mode, int* fails) -> int {   // mode 0: automatic, 1: filter level 2, 2: exact
-        const bool exact = mode == 2;
-        ix.force_exact = exact;
-        ix.force_level2 = mode == 1;
-        ix.defer_tc_check = !exact;
-        VB_CUDA(cudaMemsetAsync(ix.d_tc_fail, 0, 2 * sizeof(int), c.stream));
+    auto run = [&](const IvfPass& pass, int* fails, int* level) -> int {
+        VB_TRY(ivf_tc_fail_zero(ix));
         Scratch batch;
         void* qimg;
         size_t qstride;
@@ -2548,14 +2546,14 @@ int vb_ivf_search_sharded_dev(vb_ivf* h, const void* queries_dev, int64_t nq, in
             int32_t* d_lists;
             float* d_ldist;
             float* qn_mine = nullptr;
-            VB_TRY(ivf_select_probes(batch, ix, (const uint8_t*)qimg + (size_t)q0 * qstride, qstride, m, &qn_mine, probes, &d_lists,
-                                     &d_ldist));
+            VB_TRY(ivf_select_probes(batch, ix, pass, (const uint8_t*)qimg + (size_t)q0 * qstride, qstride, m, &qn_mine, probes,
+                                     &d_lists, &d_ldist));
             VB_CUDA(cudaMemcpyAsync(my_lists, d_lists, sizeof(int32_t) * (size_t)m * probes, cudaMemcpyDeviceToDevice, c.stream));
         }
         VB_TRY(comm_allgather(my_lists, all_lists, (int64_t)sizeof(int32_t) * chunk * probes));
         // (ranks hold `chunk` queries each, the last one possibly fewer: the gathered array is query-major for q < nq)
         float* qn = nullptr;
-        VB_TRY(ivf_scan_topk(batch, ix, qimg, qstride, nq, &qn, all_lists, probes, k, my_ids, my_dist, nullptr, nullptr));
+        VB_TRY(ivf_scan_topk(batch, ix, pass, qimg, qstride, nq, &qn, all_lists, probes, cap, k, my_ids, my_dist, nullptr, level));
         // one buffer per rank: [ids | distances]; gathered rank-major, so view it as two strided arrays
         VB_TRY(comm_allgather(my_ids, all_ids, (int64_t)res_ids));
         VB_TRY(comm_allgather(my_dist, all_dist, (int64_t)res_dist));
@@ -2563,28 +2561,15 @@ int vb_ivf_search_sharded_dev(vb_ivf* h, const void* queries_dev, int64_t nq, in
         VB_CUDA(cudaGetLastError());
         count_launch();
         fails[0] = fails[1] = 0;
-        if (!exact) {
+        if (pass.defer_check) {
             VB_TRY(comm_allreduce(ix.d_tc_fail, 2, 1));
             VB_CUDA(cudaMemcpyAsync(fails, ix.d_tc_fail, 2 * sizeof(int), cudaMemcpyDeviceToHost, c.stream));
             VB_CUDA(cudaStreamSynchronize(c.stream));
         }
         return VB_OK;
     };
-    int fails[2];
-    int rc = run(0, fails);
-    if (rc == VB_OK && fails[0] == 0 && fails[1] > 0 && ix.last_list_level == 1) {
-        ix.total_l1_failed += fails[1];
-        ix.l1_cooldown = 64;
-        rc = run(1, fails);
-    }
-    if (rc == VB_OK && fails[0] + fails[1] > 0) {
-        ix.total_tc_failed += fails[0] + fails[1];
-        rc = run(2, fails);
-    }
-    ix.force_exact = false;
-    ix.force_level2 = false;
-    ix.defer_tc_check = false;
-    VB_TRY(rc);
+    // no level 0: the sharded search keeps the batch-wide repeats, which every rank makes together
+    VB_TRY(ivf_certified_batch(ix, probes, IvfPass{}, run, nullptr));
     ix.last_cand = -1;
     ix.last_bytes = nq;
     return VB_OK;
