@@ -289,6 +289,9 @@ bool list_tc_supported(int elem, int key_metric, int k);
 // what launch_list_tc adds at level 0 (t_q, eps(q)^2, per-row bound coefficients)
 int list_tc_query_norms(Scratch& sc, const void* qimg, size_t qstride, int64_t nq, float** qn);
 int list_tc_kp(int k, int level = 2);
+// dynamic shared memory of a launch_list_tc_cta_refine launch that selects its k' nearest from the slab minima (slabs), takes
+// them preselected (pre) or selects them from the whole run (neither)
+size_t cta_refine_smem_bytes(int kp, size_t qstride, bool slabs, bool pre, int64_t cap, int64_t cap_s, int probes);
 int list_tc_prepare(const Table& rows, ListTcImage* im);
 // the int8 plane, row scales and rmax of level 0 (rows must already be prepared)
 int list_tc_prepare_l0(const Table& rows, ListTcImage* im);

@@ -2,6 +2,7 @@
 // top-k and the IVFFlat scan path (GetScanLists + GetScanItems, src/ivfscan.c:47-187).
 #include "vb_common.cuh"
 #include "vb_distance.cuh"
+#include "vb_slab_select.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -557,14 +558,19 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const IvfPass& pass, const void* 
         int level = (c.tc_level1 && !level2 && ix.l1_cooldown == 0 && list_tc_kp(k, 1) <= 128) ? 1 : 2;
         if (ix.l1_cooldown > 0 && !level2) --ix.l1_cooldown;
         // slab minima for the selection (vb_common.cuh slab_base): with them the k' nearest are found from 32 k' candidates
-        // per query instead of the whole run
+        // per query instead of the whole run.  They hold a run's slab keys in shared memory, so they are taken only where
+        // the launch that reads them fits: the refine at the level's k', or in a repeat at level 2 slab_select_kernel.
+        // Elsewhere the k' are selected from the whole run (launch_segment_topk_v).
         const int64_t cap_s = slab_cap(cap, probes);
-        const bool slabs_fit = c.slab_select && nq * cap_s < (int64_t)INT32_MAX &&
-                               (size_t)cap_s * 4 + 20 * 1024 <= 160 * 1024;
+        auto slabs_fit = [&](int lvl) {
+            const int kp = list_tc_kp(k, lvl);
+            const size_t smem = level2 ? slab_select_launch_smem(cap_s, probes) : cta_refine_smem_bytes(kp, qstride, true, false, cap, cap_s, probes);
+            return c.slab_select && nq * cap_s < (int64_t)INT32_MAX && kp <= 128 && smem <= SS_SMEM_MAX;
+        };
         // level 0 in front of level 1: int8 rows (1 byte per element, bound ~R_max |q|, k' = 128).  Its uncertified queries
         // are listed by the one-CTA-per-query refine, and a pass allows it only where its caller searches them again on
         // their own.
-        if (level == 1 && c.tc_level0 && pass.level0 && slabs_fit && list_tc_kp(k, 0) <= 128) {
+        if (level == 1 && c.tc_level0 && pass.level0 && slabs_fit(0)) {
             if (ix.l0_cooldown > 0) {
                 --ix.l0_cooldown;
             } else {
@@ -579,7 +585,7 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const IvfPass& pass, const void* 
         }
         if (level_out) *level_out = level;
         const int kp = list_tc_kp(k, level);
-        const bool slabs = slabs_fit && kp <= 128;
+        const bool slabs = slabs_fit(level);
         void* d_smin = nullptr;
         if (slabs) VB_TRY(sc.take(sizeof(float) * (size_t)nq * cap_s, &d_smin));
         if (!*qn) VB_TRY(list_tc_query_norms(sc, qimg, qstride, nq, qn));

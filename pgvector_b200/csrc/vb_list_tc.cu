@@ -700,6 +700,10 @@ __device__ __forceinline__ float lc_eps(const LcBound& b, float qn) {
 __host__ __device__ inline size_t cr_work_bytes(bool slabs, bool pre, int64_t cap, int64_t cap_s, int probes) {
     return slabs ? ss_select_smem_bytes(cap_s, probes) : pre ? 0 : (size_t)cap * 4;
 }
+// dynamic shared memory of one cta_refine_body CTA: cand, fin, rowp, the query image, the selection's work area, exact
+size_t cta_refine_smem_bytes(int kp, size_t qstride, bool slabs, bool pre, int64_t cap, int64_t cap_s, int probes) {
+    return (size_t)SS_CAND * 8 + (size_t)kp * 16 + qstride + cr_work_bytes(slabs, pre, cap, cap_s, probes) + (size_t)kp * 4 + 16;
+}
 
 // Steps 2 + 3 + 4 with ONE CTA per query (cta_refine_kernel): the k' nearest by (d~, position) come from one of three
 // sources -- a CTA-wide selection from the slab minima (smin), the k' preselected by launch_slab_select /
@@ -1411,8 +1415,8 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
     // the bound's per-query input: |q|^2, or at level 0 eps(q)^2 (lc_make_bound)
     if (level == 0) qn = l0_qe2(qn, nq);
     const int V = (int)(rows.stride / 16);
-    const size_t smem = (size_t)SS_CAND * 8 + (size_t)kp * 16 + qstride + cr_work_bytes(smin, pre_pos, cap, cap_s, probes) + (size_t)kp * 4 + 16;
-    VB_REQUIRE(kp <= SS_THREADS && smem <= 200 * 1024 && (smin || pre_pos || cap <= CR_RUN_MAX),
+    const size_t smem = cta_refine_smem_bytes(kp, qstride, smin, pre_pos, cap, cap_s, probes);
+    VB_REQUIRE(kp <= SS_THREADS && smem <= SS_SMEM_MAX && (smin || pre_pos || cap <= CR_RUN_MAX),
                "cta_refine: k' = %d / %zu bytes of shared memory not supported", kp, smem);
     VB_REQUIRE(!fail_list || (level == 0 && im.r8 && smin), "cta_refine: the listing kernel is level 0's and needs its int8 image and slab minima");
 #define VB_CR(E, M)                                                                                                              \

@@ -499,8 +499,8 @@ int launch_slab_select(const float* dist, const float* smin, int64_t nq, int pro
     VB_REQUIRE(kp <= TOPK_MAX_K, "slab selection: k' too large");
     void* d_flag;
     VB_TRY(sc.take(sizeof(int32_t) * (size_t)nq, &d_flag));
-    const size_t smem = (size_t)SS_CAND * 8 + ss_select_smem_bytes(cap_s, probes);
-    VB_REQUIRE(smem <= 200 * 1024, "slab selection: %zu bytes of shared memory", smem);
+    const size_t smem = slab_select_launch_smem(cap_s, probes);
+    VB_REQUIRE(smem <= SS_SMEM_MAX, "slab selection: %zu bytes of shared memory", smem);
     static size_t attr = 0;
     if (smem > 48 * 1024 && smem > attr) {
         VB_CUDA(cudaFuncSetAttribute(slab_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -132,6 +132,13 @@ __host__ __device__ inline size_t ss_select_smem_bytes(int64_t cap_s, int probes
     return (size_t)cap_s * 8 + (size_t)(2 * probes + 2) * 4 + (size_t)probes * 16 + 16;
 }
 
+// dynamic shared memory of one CTA of launch_slab_select and of launch_list_tc_cta_refine, at most.  The batched search
+// takes slab minima only where the launch that reads them stays under it (ivf_scan_topk).
+constexpr size_t SS_SMEM_MAX = 200 * 1024;
+
+// dynamic shared memory of slab_select_kernel (launch_slab_select): cand[SS_CAND] and the selection's work area
+inline size_t slab_select_launch_smem(int64_t cap_s, int probes) { return (size_t)SS_CAND * 8 + ss_select_smem_bytes(cap_s, probes); }
+
 // The candidates of query q that can be among its k nearest by d~: (1) the run's slab minima into shared memory,
 // (2) radix-select tau, (3) list the qualifying slabs, then gather their candidates <= tau with every load independent
 // (one candidate per thread and step), (4) sort.  Returns their number n (cand[0 .. n) sorted, n >= min(k, run length)),
