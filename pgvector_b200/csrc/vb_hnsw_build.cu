@@ -101,6 +101,18 @@ __host__ __device__ inline size_t hb_update_smem(int qvec) {
     return (b + 15) & ~(size_t)15;
 }
 
+// dynamic shared memory one CTA of the build kernels may take: the one limit both the launches and the choice of where
+// hnsw_insert_kernel keeps R are checked against
+constexpr size_t HB_SMEM_MAX = 200 * 1024;
+
+// the largest capacity of R in [lo, hi] whose hnsw_insert_kernel CTA fits in shared memory, or 0 when none does: R then lives
+// in global memory (VacDev::wk, capacity hi) and only the row images stay in shared memory
+static int hb_insert_shared_cap(int qvec, int lm0, int lo, int hi) {
+    for (int cap = hi; cap >= lo; --cap)
+        if (hb_insert_smem(qvec, cap, lm0) * HN_WARPS <= HB_SMEM_MAX) return cap;
+    return 0;
+}
+
 // candidates cand[from..n) that are still unpruned are scored against the image `img` (the row of the candidate
 // just accepted); those with d(e, r) <= d(e, q) are pruned (CheckElementCloser, src/hnswutils.c:1040-1060)
 template <int ELEM, int METRIC, int LPR, typename IdOf, typename DistOf>
@@ -134,6 +146,8 @@ __device__ __forceinline__ void prune_against(const HnswDev& g, const uint4* img
 // HnswFindElementNeighbors with existing = true: elements being deleted do not count towards ef (R holds v.wcap
 // entries), ef_construction + 1 (b.efc already is), the element itself is removed too, and the whole new tuple goes to
 // the staging area (the layers above the entry point's level are left empty, as the reference's are).
+// R and the candidate arrays live in shared memory, or in global memory when v.wk is set (rows too wide for R of this
+// capacity to fit beside the two row images, or a repair that outgrew the shared R).
 template <int ELEM, int METRIC, int LPR, bool INS = false, bool VAC = false>
 __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_insert_kernel(BuildDev b, uint32_t* __restrict__ vis_all, uint32_t vis_cap,
                                                                     uint32_t vis_upper, VacDev v) {
@@ -142,32 +156,30 @@ __global__ void __launch_bounds__(HN_WARPS * 32) hnsw_insert_kernel(BuildDev b, 
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
     const int efc = b.efc, lm0 = 2 * g.m;
     const int wc = VAC ? v.wcap : efc;   // capacity of R and of the candidate arrays
-    uint8_t* base = reinterpret_cast<uint8_t*>(smem) + (size_t)warp * hb_insert_smem(b.qvec, VAC && v.wk ? 0 : wc, lm0);
+    uint8_t* base = reinterpret_cast<uint8_t*>(smem) + (size_t)warp * hb_insert_smem(b.qvec, v.wk ? 0 : wc, lm0);
     uint4* sq = reinterpret_cast<uint4*>(base);
     uint4* img = sq + b.qvec;
     uint64_t* keyA = reinterpret_cast<uint64_t*>(img + b.qvec);
-    uint64_t* keyB = keyA + (VAC && v.wk ? 0 : wc);
-    uint64_t* bkey = keyB + (VAC && v.wk ? 0 : wc);
+    uint64_t* keyB = keyA + (v.wk ? 0 : wc);
+    uint64_t* bkey = keyB + (v.wk ? 0 : wc);
     uint32_t* idA = reinterpret_cast<uint32_t*>(bkey + 32);
-    uint32_t* idB = idA + (VAC && v.wk ? 0 : wc);
-    uint32_t* bid = idB + (VAC && v.wk ? 0 : wc);
+    uint32_t* idB = idA + (v.wk ? 0 : wc);
+    uint32_t* bid = idB + (v.wk ? 0 : wc);
     int32_t* bj = reinterpret_cast<int32_t*>(bid + 32);
     int32_t* sel = bj + 32;
     uint16_t* wd = reinterpret_cast<uint16_t*>(sel + lm0);
-    uint8_t* dead = reinterpret_cast<uint8_t*>(wd + (VAC && v.wk ? 0 : wc));
+    uint8_t* dead = reinterpret_cast<uint8_t*>(wd + (v.wk ? 0 : wc));
 
     const int gwarp = blockIdx.x * HN_WARPS + warp;
     const int nwarps = gridDim.x * HN_WARPS;
     uint32_t* vis = vis_all + (size_t)gwarp * vis_cap;
-    if constexpr (VAC) {
-        if (v.wk) {
-            keyA = v.wk + (size_t)gwarp * 2 * wc;
-            keyB = keyA + wc;
-            idA = v.wi + (size_t)gwarp * 2 * wc;
-            idB = idA + wc;
-            wd = v.wd + (size_t)gwarp * wc;
-            dead = v.dead + (size_t)gwarp * wc;
-        }
+    if (v.wk) {
+        keyA = v.wk + (size_t)gwarp * 2 * wc;
+        keyB = keyA + wc;
+        idA = v.wi + (size_t)gwarp * 2 * wc;
+        idB = idA + wc;
+        wd = v.wd + (size_t)gwarp * wc;
+        dead = v.dead + (size_t)gwarp * wc;
     }
 
     for (int w = gwarp; w < b.B; w += nwarps) {
@@ -696,6 +708,7 @@ template <int ELEM, int METRIC, int LPR, int MODE>
 static int launch_insert(const BuildDev& b, const VacDev& v, uint32_t* vis, uint32_t vis_cap, uint32_t vis_upper, int grid, size_t smem,
                          int* occ) {
     auto kern = hnsw_insert_kernel<ELEM, METRIC, LPR, MODE != HB_BUILD, MODE == HB_VACUUM>;
+    VB_REQUIRE(smem <= HB_SMEM_MAX, "hnsw: %zu bytes of shared memory per CTA do not fit", smem);
     if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (occ) {
         VB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, HN_WARPS * 32, smem));
@@ -712,6 +725,7 @@ static int launch_update(const BuildDev& b, const VacDev& v, const uint64_t* key
     auto kern = hnsw_update_kernel<ELEM, METRIC, LPR>;
     auto kern_disk = hnsw_update_disk_kernel<ELEM, METRIC, LPR, MODE == HB_VACUUM>;
     const void* k = MODE != HB_BUILD ? (const void*)kern_disk : (const void*)kern;
+    VB_REQUIRE(smem <= HB_SMEM_MAX, "hnsw: %zu bytes of shared memory per CTA do not fit", smem);
     if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (occ) {
         VB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, k, HN_WARPS * 32, smem));
@@ -750,6 +764,23 @@ static bool pick_kernels(const Hnsw& h, int V, BuildLaunch* out) {
         else return false;
     }
     return true;
+}
+
+// R and the candidate arrays of hnsw_insert_kernel in global memory: `wcap` entries for each of `warps` warps
+static void hb_point_global_r(void* buf, size_t warps, int wcap, VacDev* v) {
+    const size_t nw = warps * (size_t)wcap;
+    v->wcap = wcap;
+    v->wk = (uint64_t*)buf;
+    v->wi = (uint32_t*)(v->wk + 2 * nw);
+    v->wd = (uint16_t*)(v->wi + 2 * nw);
+    v->dead = (uint8_t*)(v->wd + nw);
+}
+static size_t hb_global_r_bytes(size_t warps, int wcap) { return warps * (size_t)wcap * (2 * 8 + 2 * 4 + 2 + 1); }
+static int hb_take_global_r(Scratch& sc, size_t warps, int wcap, VacDev* v) {
+    void* p;
+    VB_TRY(sc.take(hb_global_r_bytes(warps, wcap), &p));
+    hb_point_global_r(p, warps, wcap, v);
+    return VB_OK;
 }
 
 static double build_uniform(uint64_t* st) {   // (0, 1]: -log() stays finite
@@ -824,10 +855,10 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
         return VB_EINVAL;
     }
     const int qvec = h.elem == VB_HALFVEC ? 2 * V : V;
-    const size_t smem_ins = hb_insert_smem(qvec, efc, lm0) * HN_WARPS;
+    // R of ef_construction entries: in shared memory where it fits beside the row images, in global memory otherwise
+    const bool r_shared = hb_insert_shared_cap(qvec, lm0, efc, efc) > 0;
+    const size_t smem_ins = hb_insert_smem(qvec, r_shared ? efc : 0, lm0) * HN_WARPS;
     const size_t smem_upd = hb_update_smem(qvec) * HN_WARPS;
-    VB_REQUIRE(smem_ins <= 200 * 1024 && smem_upd <= 200 * 1024,
-               "ef_construction %d / m %d with this dimension need %zu bytes of shared memory per CTA", efc, m, smem_ins);
 
     BuildDev b{};
     b.g.rows = h.rows.d;
@@ -853,6 +884,8 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
     VB_TRY(K.update(b, VacDev{}, nullptr, nullptr, 0, InsertRec{}, 0, smem_upd, &occ_upd));
     const int max_grid_ins = c.sm_count * std::max(1, occ_ins);
     const int max_grid_upd = c.sm_count * std::max(1, occ_upd) * 4;
+    VacDev vr{};
+    if (!r_shared) VB_TRY(hb_take_global_r(sc, (size_t)max_grid_ins * HN_WARPS, efc, &vr));
 
     void* d_flags;
     VB_TRY(sc.take(64, &d_flags));
@@ -917,7 +950,7 @@ static int hnsw_build_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_t
                 h.vis_bytes = need;
             }
             VB_CUDA(cudaMemsetAsync(d_flags, 0, 2 * sizeof(int), s));
-            VB_TRY(K.insert(b, VacDev{}, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
+            VB_TRY(K.insert(b, vr, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
             hnsw_finalize_kernel<false><<<(unsigned)std::min<int64_t>((B * 32 + 127) / 128, (int64_t)c.sm_count * 16), 128, 0, s>>>(b);
             VB_CUDA(cudaGetLastError());
             count_launch();
@@ -1011,10 +1044,9 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
     }
     const int m = h.m, lm0 = 2 * m;
     const int qvec = h.elem == VB_HALFVEC ? 2 * V : V;
-    const size_t smem_ins = hb_insert_smem(qvec, efc, lm0) * HN_WARPS;
+    const bool r_shared = hb_insert_shared_cap(qvec, lm0, efc, efc) > 0;   // (as the build's)
+    const size_t smem_ins = hb_insert_smem(qvec, r_shared ? efc : 0, lm0) * HN_WARPS;
     const size_t smem_upd = hb_update_disk_smem(qvec) * HN_WARPS;
-    VB_REQUIRE(smem_ins <= 200 * 1024 && smem_upd <= 200 * 1024,
-               "ef_construction %d / m %d with this dimension need %zu bytes of shared memory per CTA", efc, m, smem_ins);
 
     // levels (HnswInitElement, src/hnswutils.c:248-254), capped at HnswGetMaxLevel(m), and the new upper slots
     const double ml = 1.0 / std::log((double)m);
@@ -1105,6 +1137,8 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
     VB_TRY(K.update(BuildDev{}, VacDev{}, nullptr, nullptr, 0, InsertRec{}, 0, smem_upd, &occ_upd));
     const int max_grid_ins = c.sm_count * std::max(1, occ_ins);
     const int max_grid_upd = c.sm_count * std::max(1, occ_upd) * 4;
+    VacDev vr{};
+    if (!r_shared) VB_TRY(hb_take_global_r(sc, (size_t)max_grid_ins * HN_WARPS, efc, &vr));
     uint32_t cap = 1u << 14;
     while (cap < (uint32_t)(efc * m * 16) && cap < (1u << 22)) cap <<= 1;
     auto reserve_vis = [&](uint32_t vis_cap) -> int {
@@ -1196,7 +1230,7 @@ static int hnsw_insert_impl(Hnsw& h, const void* rows, bool rows_on_host, int64_
             const uint32_t vis_cap = cap + vis_upper;
             VB_TRY(reserve_vis(vis_cap));
             VB_CUDA(cudaMemsetAsync(d_flags, 0, 2 * sizeof(int), s));
-            VB_TRY(K.insert(b, VacDev{}, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
+            VB_TRY(K.insert(b, vr, h.vis, vis_cap, vis_upper, grid_ins, smem_ins, nullptr));
             hnsw_finalize_kernel<true><<<(unsigned)std::min<int64_t>((B * 32 + 127) / 128, (int64_t)c.sm_count * 16), 128, 0, s>>>(b);
             VB_CUDA(cudaGetLastError());
             count_launch();
@@ -1375,14 +1409,12 @@ static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* ou
     const int m = h.m, lm0 = 2 * m;
     const int qvec = h.elem == VB_HALFVEC ? 2 * V : V;
     const int efv = efc + 1;   // "Add one for existing element" (src/hnswutils.c:1315-1317)
-    // R in shared memory holds a few times ef: elements being deleted do not count towards ef
-    int wcap_s = 4 * efv;
-    while (wcap_s > efv && hb_insert_smem(qvec, wcap_s, lm0) * HN_WARPS > 160 * 1024) wcap_s -= efv / 2 + 1;
-    const size_t smem_ins = hb_insert_smem(qvec, wcap_s, lm0) * HN_WARPS;
+    // R holds up to four times ef (elements being deleted do not count towards ef): the largest such capacity that fits in
+    // shared memory, or four times ef in global memory when not even ef fits
+    const int wcap_s = hb_insert_shared_cap(qvec, lm0, efv, 4 * efv);
     const size_t smem_glob = hb_insert_smem(qvec, 0, lm0) * HN_WARPS;
+    const size_t smem_ins = wcap_s > 0 ? hb_insert_smem(qvec, wcap_s, lm0) * HN_WARPS : smem_glob;
     const size_t smem_upd = hb_update_disk_smem(qvec) * HN_WARPS;
-    VB_REQUIRE(wcap_s >= efv && smem_ins <= 200 * 1024 && smem_upd <= 200 * 1024,
-               "ef_construction %d / m %d with this dimension need %zu bytes of shared memory per CTA", efc, m, smem_ins);
     if (n == 0) {
         ++h.generation;
         h.n_changes = 0;
@@ -1473,6 +1505,9 @@ static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* ou
         return VB_OK;
     };
     VB_TRY(reserve_vis(cap + std::max<uint32_t>(2048u, cap / 8)));
+    VacDev v{};
+    v.wcap = wcap_s;
+    if (wcap_s == 0) VB_TRY(hb_take_global_r(sc, (size_t)max_grid_ins * HN_WARPS, 4 * efv, &v));
 
     // ---- the image changes from here on
     ++h.generation;
@@ -1503,16 +1538,34 @@ static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* ou
     b.overflow = b.n_edges + 1;
     b.edge_key = (uint64_t*)d_k1;
     b.edge_val = (float*)d_v1;
-    VacDev v{};
     v.stage0 = (int32_t*)d_stage0;
     v.stage_up = (int32_t*)d_stageup;
     v.counts = h.n_heaptids;
-    v.wcap = wcap_s;
     v.wfull = b.n_edges + 2;
     int* d_nsel = b.n_edges + 3;
-    void* wbuf = nullptr;   // R in global memory, after a repair overflowed the shared one
+    void* wbuf = nullptr;   // R in global memory after a repair overflowed the one it started on
     size_t wbuf_bytes = 0;
     int64_t nrep = 0;
+    // R of wcap entries per warp in global memory
+    auto global_r = [&](int wcap) -> int {
+        const size_t need = hb_global_r_bytes((size_t)max_grid_ins * HN_WARPS, wcap);
+        if (wbuf_bytes < need) {
+            if (wbuf) {
+                VB_CUDA(cudaStreamSynchronize(s));
+                cudaFree(wbuf);
+                wbuf = nullptr;
+                wbuf_bytes = 0;
+            }
+            if (cudaMalloc(&wbuf, need) != cudaSuccess) {
+                cudaGetLastError();
+                set_error("hnsw vacuum: candidate buffers (%zu bytes) do not fit", need);
+                return VB_ENOMEM;
+            }
+            wbuf_bytes = need;
+        }
+        hb_point_global_r(wbuf, (size_t)max_grid_ins * HN_WARPS, wcap, &v);
+        return VB_OK;
+    };
 
     // NeedsUpdated of the elements [from, n) (skip: the entry point) into d_need
     auto needs = [&](int64_t from, int skip) -> int {
@@ -1541,28 +1594,7 @@ static int hnsw_vacuum_impl(Hnsw& h, const int32_t* counts, int efc, int64_t* ou
                 // a repair's R overflowed: repeat the batch's searches with R in global memory, four times as large (nothing
                 // was published)
                 VB_REQUIRE(v.wcap < 65535, "hnsw vacuum: a repair keeps more than 65535 candidates");
-                v.wcap = (int)std::min<int64_t>(65535, (int64_t)v.wcap * 4);
-                const size_t per = (size_t)v.wcap * (2 * 8 + 2 * 4 + 2 + 1);
-                const size_t need = per * (size_t)max_grid_ins * HN_WARPS;
-                if (wbuf_bytes < need) {
-                    if (wbuf) {
-                        VB_CUDA(cudaStreamSynchronize(s));
-                        cudaFree(wbuf);
-                        wbuf = nullptr;
-                        wbuf_bytes = 0;
-                    }
-                    if (cudaMalloc(&wbuf, need) != cudaSuccess) {
-                        cudaGetLastError();
-                        set_error("hnsw vacuum: candidate buffers (%zu bytes) do not fit", need);
-                        return VB_ENOMEM;
-                    }
-                    wbuf_bytes = need;
-                }
-                const size_t nw = (size_t)max_grid_ins * HN_WARPS * v.wcap;
-                v.wk = (uint64_t*)wbuf;
-                v.wi = (uint32_t*)(v.wk + 2 * nw);
-                v.wd = (uint16_t*)(v.wi + 2 * nw);
-                v.dead = (uint8_t*)(v.wd + nw);
+                VB_TRY(global_r((int)std::min<int64_t>(65535, (int64_t)v.wcap * 4)));
                 continue;
             }
             if (!flags[1]) break;

@@ -52,45 +52,60 @@ def check_records(before, after, recs):
     assert np.all(np.diff(keys) > 0)
 
 
-def make_rows(kind, n, seed):
+def make_rows(kind, n, seed, dim=None):
+    """mixture rows of a vector_l2_ops or a halfvec opclass (24 and 32 dimensions unless given)"""
     if kind == "vector_l2_ops":
-        x, _ = mixture(n, 24, 16, seed=seed)
-        return O.VECTOR, O.L2_SQUARED, x, 24
-    x, _ = mixture(n, 32, 16, seed=seed)
-    return O.HALFVEC, O.NEG_IP, f32_to_half_bits(x), 32
+        dim = dim or 24
+        x, _ = mixture(n, dim, 16, seed=seed)
+        return O.VECTOR, O.L2_SQUARED, x, dim
+    dim = dim or 32
+    x, _ = mixture(n, dim, 16, seed=seed)
+    return O.HALFVEC, O.NEG_IP, f32_to_half_bits(x), dim
 
 
-@pytest.mark.parametrize("opclass", ["vector_l2_ops", "halfvec_ip_ops"])
-def test_one_row_batches_are_the_serial_on_disk_insert(pv, opclass):
+# (opclass, dim, m, ef_construction, rows before the insert): the insert kernel at m = 100 / ef_construction = 1000, on both
+# sides of its lanes-per-row split at 32 words (vector(123) and (125)), and on halfvec(4000) rows, whose R of 1000 entries
+# lives in global memory
+SERIAL_INSERT_CASES = [
+    pytest.param("vector_l2_ops", 24, 8, 40, 1500, id="vector_l2_ops"),
+    pytest.param("halfvec_ip_ops", 32, 8, 40, 1500, id="halfvec_ip_ops"),
+    pytest.param("vector_l2_ops", 24, 100, 1000, 800, id="vector_l2_ops-m100-efc1000"),
+    pytest.param("vector_l2_ops", 123, 8, 40, 1500, id="vector_l2_ops-dim123"),
+    pytest.param("vector_l2_ops", 125, 8, 40, 1500, id="vector_l2_ops-dim125"),
+    pytest.param("halfvec_ip_ops", 4000, 16, 1000, 400, id="halfvec_ip_ops-dim4000-efc1000"),
+]
+
+
+@pytest.mark.parametrize("opclass,dim,m,efc,n0", SERIAL_INSERT_CASES)
+def test_one_row_batches_are_the_serial_on_disk_insert(pv, opclass, dim, m, efc, n0):
     """batches of one row and the oracle's level draws: the GPU insert is the serial on-disk insert (tests/hnsw_ondisk_oracle.c), including elements
     being deleted (heap TID count 0).  (Bit Hamming is not compared list for list: its integer distances tie almost
     everywhere, the oracle's search breaks ties in pairing-heap order and the GPU's by element number, and one different
     tie sends the serial inserts apart; measured on an H100, 26 % of the lists were identical and 63 % had the same
     distances.  Its inserts are held to the 021 recall floors instead.)"""
-    elem, metric, x, dim = make_rows(opclass, 3000, 31)
-    m, efc = 8, 40
-    og = DiskHnsw(elem, metric, x[:1500], m=m, ef_construction=efc, seed=3, dim=dim)
+    elem, metric, x, dim = make_rows(opclass, 2 * n0, 31, dim=dim)
+    og = DiskHnsw(elem, metric, x[:n0], m=m, ef_construction=efc, seed=3, dim=dim)
     ge = og.export()
-    assert len(ge["levels"]) == 1500
-    counts = np.ones(1500, np.int32)
-    counts[np.random.default_rng(1).choice(1500, 75, replace=False)] = 0
+    assert len(ge["levels"]) == n0
+    counts = np.ones(n0, np.int32)
+    counts[np.random.default_rng(1).choice(n0, n0 // 20, replace=False)] = 0
     og.set_heaptid_counts(counts)
-    gi = pv.HnswIndex(opclass, dim, m=m).load(x[:1500], ge["levels"], ge["nbr0"], ge["upper_off"], ge["upper"], ge["entry"])
+    gi = pv.HnswIndex(opclass, dim, m=m).load(x[:n0], ge["levels"], ge["nbr0"], ge["upper_off"], ge["upper"], ge["entry"])
     gi.set_heaptid_counts(counts)
-    lv = draw_levels(1500, m, 8)
+    lv = draw_levels(n0, m, 8)
     try:
         pv.set_option("hnsw_build_fraction", 1 << 30)
-        dup, recs = gi.insert(x[1500:], ef_construction=efc, levels=lv)
+        dup, recs = gi.insert(x[n0:], ef_construction=efc, levels=lv)
     finally:
         pv.set_option("hnsw_build_fraction", 64)
-    odup, orecs = og.insert_on_disk(x[1500:], levels=lv)
+    odup, orecs = og.insert_on_disk(x[n0:], levels=lv)
     g, oe = gi.export(), og.export()
     assert g["entry"] == oe["entry"]
     assert np.array_equal(dup, odup)
     touched = np.union1d(recs["element"][recs["layer"] == 0], orecs["element"][orecs["layer"] == 0])
     same = np.all(g["nbr0"][touched] == oe["nbr0"][touched], axis=1)
-    assert len(touched) > 1500 and same.mean() > 0.98, same.mean()
-    assert not np.isin(g["nbr0"][1500:], np.nonzero(counts == 0)[0]).any()
+    assert len(touched) > n0 and same.mean() > 0.98, same.mean()
+    assert not np.isin(g["nbr0"][n0:], np.nonzero(counts == 0)[0]).any()
 
 
 @pytest.mark.parametrize("fraction", [64, 1 << 30])

@@ -37,18 +37,56 @@ def vacuum(pv, gi, counts, efc=64, fraction=64):
         pv.set_option("hnsw_build_fraction", 64)
 
 
-@pytest.mark.parametrize("deleted", [0.10, 0.75, 0.99])
-@pytest.mark.parametrize("opclass", ["vector_l2_ops", "halfvec_ip_ops"])
-def test_one_element_batches_are_the_serial_vacuum(pv, opclass, deleted):
+# (opclass, dim, m, ef_construction, rows): besides m = 8 / ef_construction = 40, the repair kernel at m = 100 /
+# ef_construction = 1000, on both sides of its lanes-per-row split at 32 words (vector(123) and (125)), where R of
+# ef_construction + 1 entries fits in shared memory but four times that does not (vector(3) at ef_construction 1000,
+# vector(2000) at 620, halfvec(4000) at 300: a shared R between the two), and where not even ef_construction + 1 entries
+# fit (halfvec(4000) at 1000: R in global memory from the start)
+SERIAL_VACUUM_SHAPES = [("vector_l2_ops", 24, 8, 40, 3000, "vector_l2_ops"), ("halfvec_ip_ops", 32, 8, 40, 3000, "halfvec_ip_ops"),
+                        ("vector_l2_ops", 24, 100, 1000, 1500, "vector_l2_ops-m100-efc1000"),
+                        ("vector_l2_ops", 123, 8, 40, 3000, "vector_l2_ops-dim123"),
+                        ("vector_l2_ops", 125, 8, 40, 3000, "vector_l2_ops-dim125"),
+                        ("vector_l2_ops", 3, 16, 1000, 2000, "vector_l2_ops-dim3-efc1000"),
+                        ("vector_l2_ops", 2000, 16, 620, 800, "vector_l2_ops-dim2000-efc620"),
+                        ("halfvec_ip_ops", 4000, 16, 300, 600, "halfvec_ip_ops-dim4000-efc300"),
+                        ("halfvec_ip_ops", 4000, 16, 1000, 600, "halfvec_ip_ops-dim4000-efc1000")]
+
+
+def repair_shared_cap(opclass, dim, m, efc):
+    """R's capacity in shared memory as vb_hnsw_vacuum picks it (hb_insert_smem / hb_insert_shared_cap, vb_hnsw_build.cu):
+    the largest in [ef + 1, 4 (ef + 1)] whose 4-warp CTA fits in 200 KiB, or 0: R in global memory"""
+    words = ((4 if opclass.startswith("vector") else 2) * dim + 15) // 16
+    qvec = 2 * words if opclass.startswith("halfvec") else words   # (a halfvec row image is widened to fp32)
+
+    def cta(cap):
+        b = qvec * 16 * 2 + cap * 2 * 8 + 32 * 8 + cap * 2 * 4 + 32 * 4 * 2 + 2 * m * 4 + cap * 2 + cap
+        return ((b + 15) & ~15) * 4
+    efv = efc + 1
+    return next((c for c in range(4 * efv, efv - 1, -1) if cta(c) <= 200 * 1024), 0)
+
+
+def test_vacuum_shapes_take_the_routes_they_name():
+    cap = {i: (repair_shared_cap(o, d, m, efc), efc + 1) for o, d, m, efc, n, i in SERIAL_VACUUM_SHAPES}
+    for i in ("vector_l2_ops-dim3-efc1000", "vector_l2_ops-dim2000-efc620", "halfvec_ip_ops-dim4000-efc300"):
+        c, efv = cap[i]
+        assert efv <= c < 4 * efv, (i, c)
+    assert cap["vector_l2_ops"][0] == 4 * 41 and cap["halfvec_ip_ops-dim4000-efc1000"][0] == 0
+
+
+SERIAL_VACUUM_CASES = [pytest.param(o, d, m, efc, n, dl, id=f"{i}-{dl}") for o, d, m, efc, n, i in SERIAL_VACUUM_SHAPES
+                       for dl in (0.10, 0.75, 0.99)]
+
+
+@pytest.mark.parametrize("opclass,dim,m,efc,n,deleted", SERIAL_VACUUM_CASES)
+def test_one_element_batches_are_the_serial_vacuum(pv, opclass, dim, m, efc, n, deleted):
     """batches of one element: the GPU vacuum is the oracle's serial vacuum (tests/hnsw_vacuum_oracle.c).  At 99 %
     deleted a repair's candidate list outgrows the shared-memory one and is rerun in global memory."""
-    elem, metric, x, dim = make_rows(opclass, 3000, 41)
-    m, efc = 8, 40
+    elem, metric, x, dim = make_rows(opclass, n, 41, dim=dim)
     og = VacuumHnsw(elem, metric, x, m=m, ef_construction=efc, seed=3, dim=dim)
     ge = og.export()
     gi = pv.HnswIndex(opclass, dim, m=m).load(x, ge["levels"], ge["nbr0"], ge["upper_off"], ge["upper"], ge["entry"])
-    counts = np.ones(3000, np.int32)
-    counts[np.random.default_rng(int(deleted * 100)).choice(3000, int(3000 * deleted), replace=False)] = 0
+    counts = np.ones(n, np.int32)
+    counts[np.random.default_rng(int(deleted * 100)).choice(n, int(n * deleted), replace=False)] = 0
     recs, nrep = vacuum(pv, gi, counts, efc=efc, fraction=1 << 30)
     orecs, onrep = og.vacuum(counts)
     g, oe = gi.export(), og.export()
