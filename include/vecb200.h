@@ -293,6 +293,11 @@ int			vb_array_to_rows_batch_dev(int elem, int src, int dim, int32_t typmod, con
 
 typedef struct vb_table vb_table;	/* [n x dim] rows resident in HBM (exact scan, HNSW vectors, k-means samples) */
 
+/*
+ * Rows whose query image (the padded row, halfvec widened to fp32) is over the 227 KiB of shared memory the scan holds
+ * it in -- vector or halfvec past 58112 dimensions, bit past 1859584 bits -- are refused with VB_EINVAL, as they are by
+ * vb_distance_batch.
+ */
 int			vb_table_create(int elem, int dim, vb_table **out);
 /* Append n rows from host memory (pinned staging + async copy inside). */
 int			vb_table_append(vb_table *t, const void *rows, int64_t n);

@@ -123,6 +123,19 @@ inline size_t raw_row_bytes(int elem, int dim) {
 }
 // device rows are padded to 16-byte multiples so every row starts 128-bit aligned
 inline size_t padded_row_bytes(int elem, int dim) { return (raw_row_bytes(elem, dim) + 15) & ~(size_t)15; }
+// The LDG scan (vb_scan.cu) holds one query's image -- the padded row, halfvec widened to fp32 -- in shared memory, and
+// an sm_90 CTA can opt into at most 227 KiB of it: wider rows (vector or halfvec past 58112 dimensions, bit past
+// 1859584 bits) cannot be scanned, so tables and distance batches of them are refused before anything runs.
+constexpr size_t SCAN_QUERY_SMEM_MAX = 227 * 1024;
+inline size_t query_image_bytes(int elem, int dim) {
+    return elem == VB_HALFVEC ? 2 * padded_row_bytes(elem, dim) : padded_row_bytes(elem, dim);
+}
+inline int require_scannable_rows(int elem, int dim) {
+    VB_REQUIRE(query_image_bytes(elem, dim) <= SCAN_QUERY_SMEM_MAX,
+               "rows of %d %s take a %zu-byte query image; the scan holds it in shared memory, at most %zu bytes (227 KiB)",
+               dim, elem == VB_BIT ? "bits" : "dimensions", query_image_bytes(elem, dim), SCAN_QUERY_SMEM_MAX);
+    return VB_OK;
+}
 
 inline bool metric_valid_for(int elem, int metric) {
     if (elem == VB_BIT) return metric == VB_HAMMING || metric == VB_JACCARD;

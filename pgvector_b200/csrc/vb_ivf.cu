@@ -950,6 +950,7 @@ int vb_distance_batch(int elem, int metric, int dim, const void* q, const void* 
     VB_TRY(require_init());
     VB_REQUIRE(elem >= 0 && elem <= 2 && (dim > 0 || (elem == VB_BIT && dim == 0)) && metric_valid_for(elem, metric),
                "bad element type/metric/dim (%d, %d, %d)", elem, metric, dim);
+    VB_TRY(require_scannable_rows(elem, dim));
     if (n <= 0) return VB_OK;
     // a zero-length bit string ('' :: bit) has no set bits: Hamming 0 and Jaccard 1 (ab == 0, src/bitvec.c:60-70), the
     // counts of eight zero bits -- scored as such by the same kernel
@@ -1012,6 +1013,7 @@ int vb_distance_batch(int elem, int metric, int dim, const void* q, const void* 
 int vb_table_create(int elem, int dim, vb_table** out) {
     VB_TRY(require_init());
     VB_REQUIRE(elem >= 0 && elem <= 2 && dim > 0 && out, "bad table arguments");
+    VB_TRY(require_scannable_rows(elem, dim));
     vb_table* t = new vb_table();
     t->t.elem = elem;
     t->t.dim = dim;
