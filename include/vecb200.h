@@ -983,6 +983,10 @@ int64_t		vb_ivf_tc_level1_fallbacks(const vb_ivf *ix);
  * searched again, from level 1 on; level 0 rests for 64 batches after one whose failed queries probe, in expectation,
  * more than a quarter of the lists (1 - (1 - probes / lists)^failed > 1/4), where the re-run costs more than level 0 saved. */
 int64_t		vb_ivf_tc_level0_fallbacks(const vb_ivf *ix);
+/* Queries (cumulative) filter level P (a lower bound from the rows' projection on their principal directions, option
+ * "tc_levelp") could not certify.  Only those queries were searched again, from level 0 on; level P rests for 64 batches
+ * after one whose failed queries probe, in expectation, more than half of the lists. */
+int64_t		vb_ivf_tc_levelp_fallbacks(const vb_ivf *ix);
 
 /*
  * Traffic accounting of the tensor-core filter kernel (profiling, off by default): with on != 0 every launch also
@@ -1101,7 +1105,12 @@ int64_t		vb_last_assign_rechecked(void);
  * hi plane of the rows (half the HBM traffic, 2^-7 relative error bound) and repeats a batch with both planes when a
  * certificate fails.  "tc_level0" (default 1, effective where "tc_level1" is on): batched searches (vb_ivf_search*,
  * not the sharded one) start one level lower, at int8 rows (a quarter of the bf16 planes' bytes, bound ~ max |x - x^| |q|,
- * k' = 128); only the queries it cannot certify are searched again, from level 1 on.  "tensor_cores" as vb_set_tensor_cores.  "one_query" (default 1): calls with at most 16 queries --
+ * k' = 128); only the queries it cannot certify are searched again, from level 1 on.  "tc_levelp" (default 1, effective
+ * where "tc_level0" is on, fp32 rows with L2 distance): in front of level 0, the bound |x - q|^2 >= |P(x - q)|^2 / sigma^2
+ * with P the top principal directions of a row sample (r of them, a multiple of 16 holding 90 % of its energy, at most
+ * dim / 8; no level P where none does) reads 4 r bytes a row; only the queries it cannot certify are searched again, from
+ * level 0 on.  It is taken with scan_impl 2, for batches of at least 256 queries over at least 128 lists, where the int8
+ * bytes it saves exceed the fp32 rows its looser bound adds to the refine.  "tensor_cores" as vb_set_tensor_cores.  "one_query" (default 1): calls with at most 16 queries --
  * one backend's scan: vb_ivf_scan_lists, vb_ivf_scan_items, vb_ivf_search -- run as two fused distance + select
  * kernels (the last CTA to finish selects; csrc/vb_ivf_one.cu) instead of the general launch sequence; 0 = general path.
  */

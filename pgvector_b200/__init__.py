@@ -708,6 +708,10 @@ class IvfflatIndex:
         """queries the int8 filter level could not certify (only they were searched again, from level 1 on)"""
         return int(load().vb_ivf_tc_level0_fallbacks(self.h))
 
+    def tc_levelp_fallbacks(self):
+        """queries the projection lower-bound level could not certify (only they were searched again, from level 0 on)"""
+        return int(load().vb_ivf_tc_levelp_fallbacks(self.h))
+
     def tc_level1_fallbacks(self):
         """queries the hi-plane-only filter level could not certify (their batches were repeated with both planes)"""
         return int(load().vb_ivf_tc_level1_fallbacks(self.h))

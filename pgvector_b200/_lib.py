@@ -168,6 +168,7 @@ SIGNATURES = {
     "vb_comm_allgather": (_i, [_vp, _vp, _i64]),
     "vb_ivf_tc_level1_fallbacks": (_i64, [_vp]),
     "vb_ivf_tc_level0_fallbacks": (_i64, [_vp]),
+    "vb_ivf_tc_levelp_fallbacks": (_i64, [_vp]),
     "vb_kmeans": (_i, [_vp, _i, _vp, _i, _i, _u64, _vp, _vp, _vp]),
     "vb_kmeans_pp_init": (_i, [_vp, _i, _vp, _i, _u64]),
     "vb_kmeans_pp_stats": (_i, [_vp]),

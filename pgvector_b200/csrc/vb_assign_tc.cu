@@ -335,6 +335,10 @@ int vb_set_option(const char* name, int64_t value) {
         vb::ctx().tc_level0 = value != 0;
         return VB_OK;
     }
+    if (!strcmp(name, "tc_levelp")) {
+        vb::ctx().tc_levelp = value != 0;
+        return VB_OK;
+    }
     if (!strcmp(name, "pp_filter")) {
         vb::ctx().pp_filter = (int)value;
         return VB_OK;

@@ -51,6 +51,7 @@ struct Context {
     int slab_select = 1;               // selection from the filter's slab minima (0: full radix selection of every run)
     int tc_level1 = 1;                 // batched list scan: try the hi-plane-only filter first (vb_set_option "tc_level1")
     int tc_level0 = 1;                 // ... and in front of it the int8 filter, where tc_level1 is on (vb_set_option "tc_level0")
+    int tc_levelp = 1;                 // ... and in front of that the projection lower bound, where tc_level0 is on (vb_set_option "tc_levelp")
     int pp_filter = 1;                 // k-means++ on large fp32 sample tables: triangle-inequality + bf16 filters in front of the exact distances
     unsigned long long pp_stats[3] = {0, 0, 0};   // last seeding: samples skipped by the triangle rule / stopped by the bf16 bound / re-scored exactly
     int one_query = 1;                 // scans of at most 16 queries: two fused distance + select kernels (vb_ivf_one.cu); 0 = the general path
@@ -322,6 +323,29 @@ int launch_list_tc(const Table& rows, const ListTcImage& im, int key_metric, con
                    const int32_t* d_lists, int probes, const int32_t* cand_off, int64_t cap, const int64_t* d_list_off, int n_lists,
                    float* out, float* qn, bool one_list_all_queries = false, int level = 2, float* smin = nullptr,
                    int64_t cap_s = 0);
+// Level P of the batched list scan (vb_list_proj.cu): a projection lower bound |x - q|^2 >= |P(x - q)|^2 / sigma^2 with the
+// top principal directions of the rows as P, in front of level 0.  Its runs hold rigorous lower bounds of the fp32 distance
+// and go through level 0's listing refine with zero per-row terms.
+constexpr int LIST_LEVEL_P = 3;
+struct ListProj {
+    float* P = nullptr;          // [r][dim] fp32 basis
+    float* y = nullptr;          // [cap_rows][r] fp32 projections of the rows, list order
+    int r = 0;                   // 0: no level P (not built, or no r <= dim / 8 holds 90 % of the sample's energy)
+    int64_t cap_rows = 0;
+    double sigma2 = 0.0;         // >= ||P||_2^2
+    float c1 = 0.f, c2 = 0.f, ce = 0.f;   // the bound's constants (lp_bound_kernel)
+    bool tried = false;          // the basis was built or found not to apply
+};
+// the basis and the projected plane, once per image (fp32 rows only; lp->r stays 0 where no basis applies)
+int list_proj_prepare(const Table& rows, int n_lists, ListProj* lp);
+void list_proj_release(ListProj* lp);
+// after an in-place change: the projections re-computed from first_row on (the basis stays), the plane grown when needed
+int list_proj_update(const Table& rows, ListProj* lp, int64_t first_row);
+// the filter pass: the queries projected, fl(|y_x - y_q|^2) by the list-major kernel into the runs, turned into lower bounds
+// of the fp32 distance in place, and the slab minima (smin) taken.  qn: |q|^2 of the batch; xmax: max |x| over the rows.
+int launch_list_proj(Scratch& sc, const Table& rows, const ListProj& lp, float xmax, const void* qimg, size_t qstride, int64_t nq,
+                     const int32_t* d_lists, int probes, const int32_t* cand_off, int64_t cap, const int64_t* d_list_off, int n_lists,
+                     const ListTile* d_tiles, int n_tiles, float* out, const float* qn, float* smin, int64_t cap_s);
 // the k' nearest of every query's candidate run from the slab minima (same output as launch_segment_topk_v)
 int launch_slab_select(const float* dist, const float* smin, int64_t nq, int probes, const int32_t* probe_lists, const int32_t* cand_off,
                        const int64_t* list_off, int64_t cap, int64_t cap_s, const int64_t* seg_begin, const int32_t* seg_len, int kp,

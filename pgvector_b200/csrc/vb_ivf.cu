@@ -57,11 +57,13 @@ struct Ivf {
     int* d_tc_fail = nullptr;         // device counters of uncertified queries: [0] probe selection, [1] list scan (ivf_tc_fail_zero)
     int l1_cooldown = 0;              // batches left before level 1 is tried again after it failed
     int l0_cooldown = 0;              // the same for level 0 (after a batch where it failed often)
+    int lp_cooldown = 0;              // the same for level P
+    ListProj lp;                      // level P's basis and projected rows, built with level 0's image (vb_list_proj.cu)
     int32_t* d_l0_fail = nullptr;     // the queries level 0 could not certify ([d_tc_fail[1]] of them)
     int64_t l0_fail_cap = 0;
-    void* d_repair = nullptr;         // gathered queries and results of their re-run (device queries / results)
-    size_t repair_bytes = 0;
-    int64_t total_tc_failed = 0, total_l1_failed = 0, total_l0_failed = 0;
+    void* d_repair[2] = {nullptr, nullptr};   // gathered queries and results of their re-run (device queries / results), by the
+    size_t repair_bytes[2] = {0, 0};          // level it starts at (0: after level P; 1: after level 0, which a re-run from 0 may need)
+    int64_t total_tc_failed = 0, total_l1_failed = 0, total_l0_failed = 0, total_lp_failed = 0;
     bool loaded = false;
     uint64_t generation = 0;          // bumped whenever rows or lists change: an iterative scan handle refuses a changed image
     bool has_ids = false;             // loaded with heap ids (vb_ivf_insert / vb_ivf_delete need them)
@@ -342,6 +344,7 @@ struct IvfPass {
     Mode mode = AUTO;           // LEVEL2: the repeat of a batch whose level-1 certificate failed; EXACT: no tensor-core filter
     bool defer_check = false;   // the caller reads the certificate counters (d_tc_fail) at its own synchronisation
     bool level0 = false;        // the list scan may start at level 0: the caller runs the queries it cannot certify again
+    bool levelp = false;        // ... and at level P in front of it (the caller runs those queries again from level 0)
     bool repair = false;        // that re-run: it takes the batched filter chain whatever its size
 };
 constexpr int IVF_LEVEL_EXACT = -1;   // list level of a scan that ran on the exact kernels
@@ -507,6 +510,33 @@ static int ivf_ensure_l0_image(Ivf& ix) {
     return list_tc_prepare_l0(ix.rows, &ix.tc);
 }
 
+// level P's basis and projected plane (4 r bytes a row, r <= dim / 8), built on first use where it fits with 4 GiB to spare
+static int ivf_ensure_lp_image(Ivf& ix) {
+    if (ix.lp.tried) return VB_OK;
+    const size_t need = (size_t)std::max(ix.rows.cap, ix.rows.n) * (size_t)(ix.rows.dim / 8) * 4 + (size_t)ix.rows.dim * ix.rows.dim * 10;
+    size_t free_b = 0, total_b = 0;
+    VB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    if (free_b < need + ((size_t)4 << 30)) {
+        ix.lp.tried = true;
+        return VB_OK;
+    }
+    return list_proj_prepare(ix.rows, ix.lists, &ix.lp);
+}
+
+// Whether level P pays for a batch: it reads 4 r bytes of every probed row instead of level 0's dim, and its looser bound
+// re-scores about LP_EXTRA_ROWS more rows per query than level 0's (44.7 against 13.7 on bench.py's rank16 law, DESIGN
+// section 4), 4 dim bytes each.  The batch probes about n (1 - (1 - probes / lists)^nq) distinct rows.  Before the basis
+// is built r is taken at its cap, dim / 8.  Those figures hold for batches of thousands of queries over an index of a
+// thousand lists; as for the tensor-core probe selection, a batch of fewer than 256 queries or an index of fewer than 128
+// lists keeps level 0.
+constexpr double LP_EXTRA_ROWS = 32.0;
+static bool ivf_levelp_pays(const Ivf& ix, int64_t nq, int probes) {
+    if (nq < 256 || ix.lists < 128) return false;
+    const int r = ix.lp.tried ? ix.lp.r : ix.rows.dim / 8 / 16 * 16;
+    const double rows = (double)ix.rows.n * (1.0 - std::pow(1.0 - (double)probes / ix.lists, (double)nq));
+    return rows * (ix.rows.dim - 4.0 * r) > (double)nq * LP_EXTRA_ROWS * 4.0 * ix.rows.dim;
+}
+
 // scan the given probe lists for a batch of queries and keep the k nearest per query (mask: of the rows each query's
 // row filter allows).  cap bounds the candidates of one query; *qn as in ivf_select_probes; *level: the filter level
 // the scan ran at, or IVF_LEVEL_EXACT
@@ -578,7 +608,21 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const IvfPass& pass, const void* 
                 if (ix.tc.planes8) level = 0;
             }
         }
-        if (level == 0 && ix.l0_fail_cap < nq) {
+        // level P in front of level 0: lower bounds from the rows' projection on their principal directions (fp32 rows,
+        // L2, where the rows' spectrum allows a basis: vb_list_proj.cu), where the scan is chosen automatically (scan_impl
+        // 4 asks for the tensor-core filter) and the batch is large enough for it to pay.  Its uncertified queries are
+        // listed by the same refine and searched again from level 0.
+        if (level == 0 && c.tc_levelp && c.scan_impl == 2 && pass.levelp && km == VB_L2_SQUARED && ix.elem == VB_VECTOR && ix.n_tiles > 0 &&
+            ivf_levelp_pays(ix, nq, probes)) {
+            if (ix.lp_cooldown > 0) {
+                --ix.lp_cooldown;
+            } else {
+                VB_TRY(ivf_ensure_lp_image(ix));
+                if (ix.lp.r > 0) level = LIST_LEVEL_P;
+            }
+        }
+        const bool listed = level == 0 || level == LIST_LEVEL_P;
+        if (listed && ix.l0_fail_cap < nq) {
             if (ix.d_l0_fail) VB_CUDA(cudaFree(ix.d_l0_fail));
             VB_CUDA(cudaMalloc(&ix.d_l0_fail, sizeof(int32_t) * (size_t)nq));
             ix.l0_fail_cap = nq;
@@ -589,8 +633,12 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const IvfPass& pass, const void* 
         void* d_smin = nullptr;
         if (slabs) VB_TRY(sc.take(sizeof(float) * (size_t)nq * cap_s, &d_smin));
         if (!*qn) VB_TRY(list_tc_query_norms(sc, qimg, qstride, nq, qn));
-        VB_TRY(launch_list_tc(ix.rows, ix.tc, km, qimg, qstride, nq, d_lists, probes, cand_off, cap, ix.d_list_off, ix.lists,
-                              (float*)d_dist, *qn, false, level, (float*)d_smin, cap_s));
+        if (level == LIST_LEVEL_P)
+            VB_TRY(launch_list_proj(sc, ix.rows, ix.lp, ix.tc.xmax, qimg, qstride, nq, d_lists, probes, cand_off, cap, ix.d_list_off, ix.lists,
+                                    ix.d_tiles, ix.n_tiles, (float*)d_dist, *qn, (float*)d_smin, cap_s));
+        else
+            VB_TRY(launch_list_tc(ix.rows, ix.tc, km, qimg, qstride, nq, d_lists, probes, cand_off, cap, ix.d_list_off, ix.lists,
+                                  (float*)d_dist, *qn, false, level, (float*)d_smin, cap_s));
         prof_end(VB_PROF_SCAN_ITEMS);
         if (mask)
             VB_TRY(ivf_mask_runs(*mask, nq, d_lists, probes, cand_off, ix.d_list_off, cap, (float*)d_dist, (float*)d_smin, cap_s));
@@ -609,7 +657,7 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const IvfPass& pass, const void* 
             // counts as uncertified: the repeat of the batch selects below)
             VB_TRY(launch_list_tc_cta_refine(ix.rows, ix.tc, km, qimg, qstride, nq, k, kp, probes, d_lists, cand_off, ix.d_list_off,
                                              (const float*)d_dist, (const float*)d_smin, nullptr, nullptr, cap, cap_s, seg_len, *qn, pos, key,
-                                             ix.d_tc_fail + 1, level, level == 0 ? ix.d_l0_fail : nullptr, has_nan));
+                                             ix.d_tc_fail + 1, level, listed ? ix.d_l0_fail : nullptr, has_nan));
         } else {
             // the k' selected by a launch of their own (slab_select_kernel hands what overflows it to the full selection)
             if (slabs)
@@ -1184,6 +1232,7 @@ static int ivf_set_layout(Ivf& ix, const int64_t* list_offsets, bool release) {
     if (release) {
         list_tc_release(&ix.tc);   // rows are about to change: planes are rebuilt on the next tensor-core scan
         list_tc_release(&ix.ctc);
+        list_proj_release(&ix.lp);
         ix.ids_cap = -1;
     }
     ix.n_tiles = (int)tiles.size();
@@ -1472,6 +1521,10 @@ static int ivf_finish_update(Ivf& ix, const std::vector<int64_t>& new_off, int64
     if (ix.tc.planes) {
         VB_TRY(list_tc_repack(ix.rows, &ix.tc, whole ? 0 : first / 128, whole8 ? 0 : first / 128, d_stats));
         VB_TRY(ivf_build_units(ix));
+        // level P's projections from the first changed row on; the basis stays (any basis is valid, a stale one looser)
+        VB_TRY(list_proj_update(ix.rows, &ix.lp, first));
+    } else {
+        list_proj_release(&ix.lp);   // built again with the planes
     }
     VB_CUDA(cudaStreamSynchronize(ctx().stream));
     return VB_OK;
@@ -1940,6 +1993,7 @@ static int ivf_build_impl(const char* fn, vb_ivf* h, const void* rows, const int
     ix.has_ids = false;
     list_tc_release(&ix.tc);
     list_tc_release(&ix.ctc);
+    list_proj_release(&ix.lp);
     table_free(ix.centers);
     ix.centers = Cn.t;
     Cn.t.d = nullptr;
@@ -2014,7 +2068,9 @@ int vb_ivf_free(vb_ivf* h) {
     if (h->ix.d_centre_off) cudaFree(h->ix.d_centre_off);
     if (h->ix.d_tc_fail) cudaFree(h->ix.d_tc_fail);
     if (h->ix.d_l0_fail) cudaFree(h->ix.d_l0_fail);
-    if (h->ix.d_repair) cudaFree(h->ix.d_repair);
+    for (void* b : h->ix.d_repair)
+        if (b) cudaFree(b);
+    list_proj_release(&h->ix.lp);
     if (h->ix.d_ticket) cudaFree(h->ix.d_ticket);
     for (int i = 0; i < 2; ++i) {
         if (h->ix.q_buf[i]) cudaFree(h->ix.q_buf[i]);
@@ -2171,7 +2227,7 @@ struct IvfFilterSpec {
 };
 
 static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, bool host, bool q_host, int64_t* out_ids,
-                           float* out_f, double* out_d, bool repair = false, const IvfFilterSpec* filt = nullptr);
+                           float* out_f, double* out_d, bool repair = false, const IvfFilterSpec* filt = nullptr, int repair_from = 1);
 
 // the mask arguments of queries [q0, q0 + m) of a filtered call (in sc): the filters' positions and runs, in place
 static int ivf_upload_mask(Scratch& sc, const IvfFilterSpec& filt, int64_t q0, int64_t m, IvfMask* mk) {
@@ -2190,14 +2246,14 @@ static int ivf_upload_mask(Scratch& sc, const IvfFilterSpec& filt, int64_t q0, i
     return VB_OK;
 }
 
-// The queries `fail` (numbers within `queries`, nf of them) that level 0 could not certify are searched again on their own,
-// from level 1 on, and their rows of the outputs overwritten.  The re-run takes the batched filter chain whatever its size
+// The queries `fail` (numbers within `queries`, nf of them) that level 0 (level P) could not certify are searched again on
+// their own, from level 1 (level 0) on -- `from` -- and their rows of the outputs overwritten.  The re-run takes the batched filter chain whatever its size
 // (not the fused one-query kernels): a query certified at level 1 or 2 carries the filter's exact re-score, as it would in
 // a batch-wide repeat.  When the re-run needs the exact kernels, the caller computes the whole sub-batch there instead,
 // as it does without level 0 (the list-major kernel's sums may differ from the re-score's in the last bit).
 // (filt: the row filters of `queries`, whose failed queries' entries of filter_of_query go along)
 static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t>& fail, int probes, int k, bool host, bool q_host,
-                             int64_t* out_ids, float* out_f, double* out_d, const IvfFilterSpec* filt) {
+                             int64_t* out_ids, float* out_f, double* out_d, const IvfFilterSpec* filt, int from) {
     Ivf& ix = h->ix;
     Context& c = ctx();
     std::sort(fail.begin(), fail.end());
@@ -2216,12 +2272,14 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
     const size_t rawq = raw_row_bytes(ix.elem, ix.dim);
     const size_t q_bytes = (rawq * (size_t)nf + 15) & ~(size_t)15;
     const size_t need = q_bytes + (sizeof(int64_t) + sizeof(float)) * (size_t)nf * k + sizeof(int64_t) + sizeof(int32_t) * (size_t)nf;
-    if (ix.repair_bytes < need) {
-        if (ix.d_repair) VB_CUDA(cudaFree(ix.d_repair));
-        VB_CUDA(cudaMalloc(&ix.d_repair, need));
-        ix.repair_bytes = need;
+    // (a re-run from level 0 may repair its own level-0 failures from level 1 while its buffer is in use: one buffer per level)
+    const int slot = from == 0 ? 0 : 1;
+    if (ix.repair_bytes[slot] < need) {
+        if (ix.d_repair[slot]) VB_CUDA(cudaFree(ix.d_repair[slot]));
+        VB_CUDA(cudaMalloc(&ix.d_repair[slot], need));
+        ix.repair_bytes[slot] = need;
     }
-    uint8_t* d_q = (uint8_t*)ix.d_repair;
+    uint8_t* d_q = (uint8_t*)ix.d_repair[slot];
     int64_t* d_ids = (int64_t*)(d_q + q_bytes);
     int64_t* d_cand_saved = d_ids + (size_t)nf * k;   // the caller's candidate count: the re-run's scans do not add to it
     float* d_f = (float*)(d_cand_saved + 1);
@@ -2242,7 +2300,7 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
     if (host) {
         std::vector<int64_t> ti((size_t)nf * k);
         std::vector<double> td((size_t)nf * k);
-        VB_TRY(ivf_search_impl(h, sub, nf, probes, k, true, q_host, ti.data(), nullptr, td.data(), true, filt));
+        VB_TRY(ivf_search_impl(h, sub, nf, probes, k, true, q_host, ti.data(), nullptr, td.data(), true, filt, from));
         VB_CUDA(cudaMemcpyAsync(ix.d_cand_sum, d_cand_saved, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
         for (int64_t i = 0; i < nf; ++i) {
             memcpy(out_ids + (size_t)fail[(size_t)i] * k, ti.data() + (size_t)i * k, sizeof(int64_t) * k);
@@ -2250,7 +2308,7 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
         }
         return VB_OK;
     }
-    VB_TRY(ivf_search_impl(h, sub, nf, probes, k, false, false, d_ids, d_f, nullptr, true, filt));
+    VB_TRY(ivf_search_impl(h, sub, nf, probes, k, false, false, d_ids, d_f, nullptr, true, filt, from));
     VB_CUDA(cudaMemcpyAsync(ix.d_cand_sum, d_cand_saved, sizeof(int64_t), cudaMemcpyDeviceToDevice, c.stream));
     scatter_results_kernel<<<(unsigned)((nf * k + 255) / 256), 256, 0, c.stream>>>(d_ids, d_f, d_idx, nf, k, out_ids, out_f);
     VB_CUDA(cudaGetLastError());
@@ -2261,20 +2319,30 @@ static int ivf_repair_level0(vb_ivf* h, const void* queries, std::vector<int32_t
 // The certificate repeat policy of one sub-batch of the batched search.  run(pass, fails, &level) computes the sub-batch
 // once: the queries its probe selection (fails[0]) and list scan (fails[1]) could not certify, and the list level it ran
 // at.  The tensor-core filter runs optimistically: the counters are read back together with the results (one
-// synchronisation per pass).  pass is the first, automatic pass: where its level0 lets the list scan start at level 0,
-// repair(n) searches the n queries level 0 could not certify again on their own.  Otherwise a sub-batch with an
+// synchronisation per pass).  pass is the first, automatic pass: where its level0 (levelp) lets the list scan start at
+// level 0 (P), repair(n, from) searches the n queries that level could not certify again on their own, from level `from`.  Otherwise a sub-batch with an
 // uncertified query is run again at level 2 when level 1 failed, then on the exact kernels.
 static int ivf_certified_batch(Ivf& ix, int probes, IvfPass pass, const std::function<int(const IvfPass&, int*, int*)>& run,
-                               const std::function<int(int)>& repair) {
+                               const std::function<int(int, int)>& repair) {
     int fails[2], level;
     pass.defer_check = true;
     VB_TRY(run(pass, fails, &level));
-    pass.level0 = false;   // (a repeat never starts at level 0)
+    pass.level0 = pass.levelp = false;   // (a repeat never starts at level 0 or P)
     auto exact = [&] {
         pass.mode = IvfPass::EXACT;
         pass.defer_check = false;
         return run(pass, fails, &level);
     };
+    if (fails[0] == 0 && fails[1] > 0 && level == LIST_LEVEL_P) {
+        // level P could not certify some queries: only those go on, from level 0.  The rule is level 0's: their re-run
+        // streams about 1 - (1 - probes / lists)^n of a level-0 pass, and level P saved most of one (it reads 4 r bytes a
+        // row instead of dim); past half of it level P no longer pays and rests for the next 64 batches.
+        ix.total_lp_failed += fails[1];
+        if (1.0 - std::pow(1.0 - (double)probes / ix.lists, (double)fails[1]) > 0.5) ix.lp_cooldown = 64;
+        const int64_t exact0 = ix.total_tc_failed;
+        VB_TRY(repair(fails[1], 0));
+        return ix.total_tc_failed > exact0 ? exact() : VB_OK;   // the re-run needed the exact kernels
+    }
     if (fails[0] == 0 && fails[1] > 0 && level == 0) {
         // level 0 could not separate the neighbours of some queries: only those go on, from level 1.  Their re-run
         // streams the lists they probe at level 1: with n failed queries, about 1 - (1 - probes / lists)^n of what a
@@ -2284,7 +2352,7 @@ static int ivf_certified_batch(Ivf& ix, int probes, IvfPass pass, const std::fun
         ix.total_l0_failed += fails[1];
         if (1.0 - std::pow(1.0 - (double)probes / ix.lists, (double)fails[1]) > 0.25) ix.l0_cooldown = 64;
         const int64_t exact0 = ix.total_tc_failed;
-        VB_TRY(repair(fails[1]));
+        VB_TRY(repair(fails[1], 1));
         return ix.total_tc_failed > exact0 ? exact() : VB_OK;   // neither level 1 nor 2 certified them
     }
     if (fails[0] == 0 && fails[1] > 0 && level == 1) {
@@ -2303,10 +2371,10 @@ static int ivf_certified_batch(Ivf& ix, int probes, IvfPass pass, const std::fun
 }
 
 // host: results go to host memory (int64 ids + float8 distances); q_host: the queries are host memory.  repair: the re-run
-// of the queries level 0 could not certify (ivf_repair_level0), which never starts at level 0 and adds to its caller's
-// candidate count
+// of the queries level 0 or P could not certify (ivf_repair_level0), which starts at level repair_from (0 or 1), never at
+// level P, and adds to its caller's candidate count
 static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probes, int k, bool host, bool q_host, int64_t* out_ids,
-                           float* out_f, double* out_d, bool repair, const IvfFilterSpec* filt) {
+                           float* out_f, double* out_d, bool repair, const IvfFilterSpec* filt, int repair_from) {
     VB_TRY(require_init());
     VB_REQUIRE(h && h->ix.loaded, "index not loaded");
     VB_REQUIRE(queries && probes >= 1 && k >= 1, "bad search arguments");
@@ -2345,7 +2413,8 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
     constexpr int L0_LIST_READ = 64;   // failed queries read back with the counters (more take a second copy)
     int32_t l0_list[L0_LIST_READ];
     IvfPass first;
-    first.level0 = !repair;
+    first.level0 = !repair || repair_from == 0;
+    first.levelp = !repair;
     first.repair = repair;
     for (int64_t q0 = 0; q0 < nq; q0 += bq) {
         const int64_t m = std::min(bq, nq - q0);
@@ -2377,13 +2446,13 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
             fails[0] = fails[1] = 0;
             const bool check = pass.defer_check && ix.d_tc_fail != nullptr;
             if (check) VB_CUDA(cudaMemcpyAsync(fails, ix.d_tc_fail, 2 * sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-            if (check && *level == 0)
+            if (check && (*level == 0 || *level == LIST_LEVEL_P))
                 VB_CUDA(cudaMemcpyAsync(l0_list, ix.d_l0_fail, sizeof(int32_t) * (size_t)std::min<int64_t>(m, L0_LIST_READ),
                                         cudaMemcpyDeviceToHost, c.stream));
             if (host || check) VB_CUDA(cudaStreamSynchronize(c.stream));
             return VB_OK;
         };
-        auto repair_level0 = [&](int n_failed) -> int {
+        auto repair_level0 = [&](int n_failed, int from) -> int {
             std::vector<int32_t> fail(l0_list, l0_list + std::min(n_failed, L0_LIST_READ));
             if (n_failed > L0_LIST_READ) {
                 fail.resize((size_t)n_failed);
@@ -2395,7 +2464,7 @@ static int ivf_search_impl(vb_ivf* h, const void* queries, int64_t nq, int probe
                 if (filt->fq) sub_filt.fq = filt->fq + q0;
             }
             return ivf_repair_level0(h, (const uint8_t*)queries + (size_t)q0 * rawq, fail, probes, k, host, q_host, out_ids + q0 * k,
-                                     out_f ? out_f + q0 * k : nullptr, out_d ? out_d + q0 * k : nullptr, filt ? &sub_filt : nullptr);
+                                     out_f ? out_f + q0 * k : nullptr, out_d ? out_d + q0 * k : nullptr, filt ? &sub_filt : nullptr, from);
         };
         VB_TRY(ivf_certified_batch(ix, probes, first, run, repair_level0));
     }
@@ -2884,6 +2953,7 @@ int vb_ivf_tc_level0_rescored(int64_t* out3) {
 int64_t vb_ivf_tc_fallbacks(const vb_ivf* h) { return h ? h->ix.total_tc_failed : 0; }
 int64_t vb_ivf_tc_level1_fallbacks(const vb_ivf* h) { return h ? h->ix.total_l1_failed : 0; }
 int64_t vb_ivf_tc_level0_fallbacks(const vb_ivf* h) { return h ? h->ix.total_l0_failed : 0; }
+int64_t vb_ivf_tc_levelp_fallbacks(const vb_ivf* h) { return h ? h->ix.total_lp_failed : 0; }
 
 int64_t vb_ivf_last_candidates(const vb_ivf* h) {
     if (!h || !h->ix.d_cand_sum) return 0;

@@ -1042,7 +1042,7 @@ bool list_tc_supported(int elem, int key_metric, int k) {
 int list_tc_kp(int k, int level) {
     // candidates kept per query.  Only those under the threshold are re-scored, so a generous k' costs a slightly
     // larger selection, not more exact distances; the certificate fails only when ALL k' are under the threshold.
-    if (level == 0) return k <= 10 ? 128 : 1 << 20;   // level 0's bound is ~4x level 1's: twice the candidates
+    if (level == 0 || level == LIST_LEVEL_P) return k <= 10 ? 128 : 1 << 20;   // level 0's bound is ~4x level 1's: twice the candidates
     if (level == 1) return k <= 10 ? 64 : k <= 40 ? 128 : 1 << 20;
     return k <= 10 ? 32 : k <= 24 ? 48 : k <= 40 ? 64 : 1 << 20;
 }
@@ -1411,14 +1411,23 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
     if (nq == 0) return VB_OK;
     Context& c = ctx();
     cudaStream_t s = c.stream;
-    const LcBound bound = lc_make_bound(rows, im, key_metric, level);
+    // level P: the runs hold lower bounds of the fp32 distance (vb_list_proj.cu), refined as level 0's with zero per-row
+    // terms and eps(q) = 0: the coefficients and eps(q)^2 are zeroed, and |x|^2 stands in for R_x (0 R_x = 0 on finite rows)
+    const bool lp = level == LIST_LEVEL_P;
+    if (lp) {
+        VB_CUDA(cudaMemsetAsync(const_cast<float*>(l0_qe2(qn, nq)), 0, sizeof(float) * (size_t)nq, s));
+        VB_CUDA(cudaMemsetAsync(l0_row_coef(l0_qe2(qn, nq), nq), 0, sizeof(float4) * (size_t)nq, s));
+    }
+    const LcBound bound = lc_make_bound(rows, im, key_metric, lp ? 0 : level);
+    const float* r8 = lp ? im.xn : im.r8;
     // the bound's per-query input: |q|^2, or at level 0 eps(q)^2 (lc_make_bound)
-    if (level == 0) qn = l0_qe2(qn, nq);
+    if (level == 0 || lp) qn = l0_qe2(qn, nq);
     const int V = (int)(rows.stride / 16);
     const size_t smem = cta_refine_smem_bytes(kp, qstride, smin, pre_pos, cap, cap_s, probes);
     VB_REQUIRE(kp <= SS_THREADS && smem <= SS_SMEM_MAX && (smin || pre_pos || cap <= CR_RUN_MAX),
                "cta_refine: k' = %d / %zu bytes of shared memory not supported", kp, smem);
-    VB_REQUIRE(!fail_list || (level == 0 && im.r8 && smin), "cta_refine: the listing kernel is level 0's and needs its int8 image and slab minima");
+    VB_REQUIRE(!fail_list || (((level == 0 && im.r8) || lp) && smin),
+               "cta_refine: the listing kernel is level 0's and P's and needs level 0's int8 image and slab minima");
 #define VB_CR(E, M)                                                                                                              \
     do {                                                                                                                         \
         if (fail_list && has_nan) {                                                                                              \
@@ -1426,7 +1435,7 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
             if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
             kern<<<(unsigned)nq, SS_THREADS, smem, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, k, kp, probes, bound, qn, dist, \
                                                        smin, cap, cap_s, seg_len, d_lists, cand_off, d_list_off, out_pos, out_key, fail_dev, \
-                                                       fail_list, im.xn, im.r8, l0_row_coef(qn, nq),                             \
+                                                       fail_list, im.xn, r8, l0_row_coef(qn, nq),                                     \
                                                        g_traffic_on ? g_traffic + 8 : nullptr, has_nan);                        \
             break;                                                                                                               \
         }                                                                                                                        \
@@ -1443,7 +1452,7 @@ int launch_list_tc_cta_refine(const Table& rows, const ListTcImage& im, int key_
             if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
             kern<<<(unsigned)nq, SS_THREADS, smem, s>>>(rows.d, rows.stride, V, (const uint8_t*)qimg, qstride, k, kp, probes, bound, qn, dist, \
                                                        smin, cap, cap_s, seg_len, d_lists, cand_off, d_list_off, out_pos, out_key, fail_dev, \
-                                                       fail_list, im.xn, im.r8, l0_row_coef(qn, nq),                             \
+                                                       fail_list, im.xn, r8, l0_row_coef(qn, nq),                                     \
                                                        g_traffic_on ? g_traffic + 8 : nullptr);                                 \
             break;                                                                                                               \
         }                                                                                                                        \

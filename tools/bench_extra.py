@@ -12,6 +12,7 @@ does not cover: k-means assign on the tensor cores (config D shape, one GPU's sh
     python tools/bench_extra.py filter   [--rows N --dim D --lists L --probes P --max-probes M --page K --queries Q]
                                           (row filters on the device: filtered iterative scan and exact top-k vs host filtering)
     python tools/bench_extra.py level0   [--rows N --dim D --lists L --probes P --rounds R --law rank16|mixture --load S]
+    python tools/bench_extra.py levelp   [the same]
                                           (the batched list scan with filter level 0 (int8 rows) on and off, alternating)
     python tools/bench_extra.py hnsw-filter [--rows N --dim D --ef EF --queries Q]
                                           (element filters on the device for hnsw.iterative_scan vs host filtering)
@@ -338,11 +339,12 @@ def bench_ivf(args):
                                    "bytes_per_launch": cand * rb, "avg_launch_ms": scan_ms / scan_n, "share_of_step": scan_ms / scan_n / ms, "peak_source": src}}))
 
 
-def bench_level0(args):
+def bench_level0(args, level="0"):
     """config B (IVFFlat L2, 2048-query batches, k 10) on bench.py's own data and index -- its law, its queries (the first
-    four batches of 2048) and its index recipe, through its functions -- with "tc_level0" 1 and 0 in alternating rounds in
-    one process: step time, list_tc_kernel time and bytes, refine time, level-0 fallbacks per batch, and whether the two
-    arms return identical ids and distances for every batch."""
+    four batches of 2048) and its index recipe, through its functions -- with "tc_level0" (level "p": "tc_levelp") 1 and 0
+    in alternating rounds in one process: step time, list scan time (the filter pass with its grouping), list_tc_kernel
+    time and bytes, refine time and rows it re-scored per query, the level's fallbacks per batch, and whether the two arms
+    return identical ids and distances for every batch."""
     import argparse as ap_
     import torch
     import bench
@@ -376,44 +378,50 @@ def bench_level0(args):
         return got
 
     rounds, ref = [], {}
+    pv.set_option("scan_impl", 2)
     for r in range(args.rounds):
         for arm in (1, 0):
-            pv.set_option("tc_level0", arm)
+            pv.set_option("tc_level" + level, arm)
             n = 16 * len(batches)
-            f0 = ix.tc_level0_fallbacks()
+            fallbacks = ix.tc_levelp_fallbacks if level == "p" else ix.tc_level0_fallbacks
+            f0 = fallbacks()
             # bench.py's conditions: the timed steps follow `--load` untimed ones (its clock-sampler load, 600 steps), so
             # a power-limited card is at its sustained clock; the SM clock is sampled over both (bench.ClockSampler)
             sampler = bench.ClockSampler(0)
             sampler.start()
             ms = timed(pv, torch, stream, one, warmup=args.load, steps=n)
             clocks = sampler.stop()
-            fails = (ix.tc_level0_fallbacks() - f0) / (n + args.load)
+            fails = (fallbacks() - f0) / (n + args.load)
             pv.prof_enable(True)
-            for p in (pv.PROF_LIST_TC, pv.PROF_TOPK):
+            for p in (pv.PROF_LIST_TC, pv.PROF_TOPK, pv.PROF_SCAN_ITEMS):
                 pv.prof_read(p)
             ms_prof = timed(pv, torch, stream, one, warmup=0, steps=2 * len(batches))   # as bench.py times: kernel brackets on
             tc_ms, tc_n = pv.prof_read(pv.PROF_LIST_TC)
             rf_ms, rf_n = pv.prof_read(pv.PROF_TOPK)
+            sc_ms, sc_n = pv.prof_read(pv.PROF_SCAN_ITEMS)
             pv.prof_enable(False)
             pv.tc_traffic(True, read=True)
+            pv.tc_level0_rescored()
             one()
             pv.synchronize()
             t = pv.tc_traffic(False, read=True)
+            rs = pv.tc_level0_rescored()
             got = outputs()
             if arm not in ref:
                 ref[arm] = got
-            rounds.append({"round": r, "tc_level0": arm, "ms_per_step": ms, "queries_per_s": B / (ms / 1000.0),
+            rounds.append({"round": r, "tc_level" + level: arm, "ms_per_step": ms, "queries_per_s": B / (ms / 1000.0),
                            "ms_per_step_with_kernel_brackets": ms_prof, "sm_mhz": clocks.get("sm_mhz"),
                            "clock_reasons": clocks.get("reasons"),
                            "list_tc_ms": tc_ms / max(tc_n, 1), "list_tc_launches_per_step": tc_n / (2 * len(batches)),
                            "list_tc_bytes_per_launch": int((t[1] + t[2]) / max(t[3], 1)), "refine_ms": rf_ms / max(rf_n, 1),
-                           "level0_fallback_queries_per_batch": fails})
+                           "list_scan_ms": sc_ms / max(sc_n, 1), "listing_refine_rows_rescored_per_query": int(rs[0]) / max(int(rs[2]), 1),
+                           "level%s_fallback_queries_per_batch" % level: fails})
     same = all(np.array_equal(a[0], b_[0]) and np.array_equal(a[1], b_[1]) for a, b_ in zip(ref[1], ref[0]))
     ratio = [rounds[i + 1]["ms_per_step"] / rounds[i]["ms_per_step"] for i in range(0, len(rounds), 2)]   # off / on
-    print(json.dumps({"bench": "level0", "card": card(),
+    print(json.dumps({"bench": "level" + level, "card": card(),
                       "workload": f"IVFFlat vector_l2_ops {args.rows}x{args.dim}, lists={args.lists}, probes={args.probes}, k={k}, "
                                   f"{len(batches)} batches of {B} queries, bench.py's {args.law} law and index ({how})",
-                      "rounds": rounds, "speedup_level0_per_round": ratio, "outputs_identical": bool(same)}))
+                      "rounds": rounds, "speedup_level%s_per_round" % level: ratio, "outputs_identical": bool(same)}))
 
 
 def bench_ivf_iter(args):
@@ -853,7 +861,7 @@ def bench_sparse(args):
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("what", choices=["assign", "hnsw", "exact", "ivf", "ivf-iter", "filter", "kmeans", "sparse", "rerank", "level0",
-                                        "hnsw-filter"])
+                                        "levelp", "hnsw-filter"])
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--lists", type=int, default=1000)
     ap.add_argument("--probes", type=int, default=10)
@@ -875,7 +883,7 @@ if __name__ == "__main__":
         a.queries, a.ef = a.queries or 2048, a.ef or 200
     if a.what in ("ivf-iter", "filter", "hnsw-filter"):
         a.queries = a.queries or 2048
-    if a.what == "level0":
+    if a.what in ("level0", "levelp"):
         a.queries = a.queries or 4 * 2048
     a.queries, a.ef = a.queries or 4096, a.ef or 100
     if a.what == "sparse":
@@ -907,11 +915,11 @@ if __name__ == "__main__":
         a.dim = a.dim or 1536
         a.elem = "vector" if a.elem == "halfvec" and "--elem" not in sys.argv else a.elem
         (bench_ivf_iter if a.what == "ivf-iter" else bench_filter)(a)
-    elif a.what == "level0":
+    elif a.what in ("level0", "levelp"):
         a.rows = a.rows or 1_000_000
         a.dim = a.dim or 1536
         a.elem = "vector" if "--elem" not in sys.argv else a.elem
-        bench_level0(a)
+        bench_level0(a, a.what[5:])
     elif a.what == "ivf":
         a.rows = a.rows or 1_000_000
         a.dim = a.dim or (1536 if a.elem == "halfvec" else 1024)
