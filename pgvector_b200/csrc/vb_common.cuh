@@ -333,7 +333,7 @@ struct ListProj {
     int r = 0;                   // 0: no level P (not built, or no r <= dim / 8 holds 90 % of the sample's energy)
     int64_t cap_rows = 0;
     double sigma2 = 0.0;         // >= ||P||_2^2
-    float c1 = 0.f, c2 = 0.f, ce = 0.f;   // the bound's constants (lp_bound_kernel)
+    float c1 = 0.f, c2 = 0.f, ce = 0.f;   // the bound's constants (lp_scan_kernel)
     bool tried = false;          // the basis was built or found not to apply
 };
 // the basis and the projected plane, once per image (fp32 rows only; lp->r stays 0 where no basis applies)
@@ -341,11 +341,12 @@ int list_proj_prepare(const Table& rows, int n_lists, ListProj* lp);
 void list_proj_release(ListProj* lp);
 // after an in-place change: the projections re-computed from first_row on (the basis stays), the plane grown when needed
 int list_proj_update(const Table& rows, ListProj* lp, int64_t first_row);
-// the filter pass: the queries projected, fl(|y_x - y_q|^2) by the list-major kernel into the runs, turned into lower bounds
-// of the fp32 distance in place, and the slab minima (smin) taken.  qn: |q|^2 of the batch; xmax: max |x| over the rows.
-int launch_list_proj(Scratch& sc, const Table& rows, const ListProj& lp, float xmax, const void* qimg, size_t qstride, int64_t nq,
+// the filter pass: the queries projected, then one pass over the (list, table tile) units of im (im.units) writes the lower
+// bounds of the fp32 distance from fl(|y_x - y_q|^2) into the runs and takes the slab minima (smin, required).
+// qn: |q|^2 of the batch; im.xmax: max |x| over the rows.
+int launch_list_proj(Scratch& sc, const Table& rows, const ListProj& lp, const ListTcImage& im, const void* qimg, size_t qstride, int64_t nq,
                      const int32_t* d_lists, int probes, const int32_t* cand_off, int64_t cap, const int64_t* d_list_off, int n_lists,
-                     const ListTile* d_tiles, int n_tiles, float* out, const float* qn, float* smin, int64_t cap_s);
+                     float* out, const float* qn, float* smin, int64_t cap_s);
 // the k' nearest of every query's candidate run from the slab minima (same output as launch_segment_topk_v)
 int launch_slab_select(const float* dist, const float* smin, int64_t nq, int probes, const int32_t* probe_lists, const int32_t* cand_off,
                        const int64_t* list_off, int64_t cap, int64_t cap_s, const int64_t* seg_begin, const int32_t* seg_len, int kp,

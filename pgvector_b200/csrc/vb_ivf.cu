@@ -634,8 +634,8 @@ static int ivf_scan_topk(Scratch& sc, Ivf& ix, const IvfPass& pass, const void* 
         if (slabs) VB_TRY(sc.take(sizeof(float) * (size_t)nq * cap_s, &d_smin));
         if (!*qn) VB_TRY(list_tc_query_norms(sc, qimg, qstride, nq, qn));
         if (level == LIST_LEVEL_P)
-            VB_TRY(launch_list_proj(sc, ix.rows, ix.lp, ix.tc.xmax, qimg, qstride, nq, d_lists, probes, cand_off, cap, ix.d_list_off, ix.lists,
-                                    ix.d_tiles, ix.n_tiles, (float*)d_dist, *qn, (float*)d_smin, cap_s));
+            VB_TRY(launch_list_proj(sc, ix.rows, ix.lp, ix.tc, qimg, qstride, nq, d_lists, probes, cand_off, cap, ix.d_list_off, ix.lists,
+                                    (float*)d_dist, *qn, (float*)d_smin, cap_s));
         else
             VB_TRY(launch_list_tc(ix.rows, ix.tc, km, qimg, qstride, nq, d_lists, probes, cand_off, cap, ix.d_list_off, ix.lists,
                                   (float*)d_dist, *qn, false, level, (float*)d_smin, cap_s));

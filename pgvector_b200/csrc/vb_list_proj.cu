@@ -10,9 +10,9 @@
 // the device in double, QR on the host in double), r = the smallest multiple of 16 holding at least 90 % of the sample's
 // energy about the origin, at most dim / 8; none (no level P) when no such r exists.  sigma^2 >= ||P||_2^2 comes from a
 // Gershgorin bound on P P^T in double, so P need not be orthonormal.  Each row's y_x = P x (accumulated in double,
-// rounded to fp32) is stored in list order; the queries are projected the same way per batch, and the list-major fp32
-// kernel (launch_list_major) computes fl(sum_j (y_x,j - y_q,j)^2) over the projected plane as a table of dimension r.
-// lp_bound_kernel turns those sums into rigorous lower bounds and takes the slab minima the refine selects from.
+// rounded to fp32) is stored in list order; the queries are projected the same way per batch, and one pass over the
+// projected plane (lp_scan_kernel) computes fl(sum_j (y_x,j - y_q,j)^2) for every probed (row, query) pair, turns it into a
+// rigorous lower bound and takes the slab minima the refine selects from.
 #include "vb_common.cuh"
 
 #include <algorithm>
@@ -45,41 +45,59 @@ __global__ void lp_gemm_tn_kernel(const T* __restrict__ A, int64_t lda, const T*
     if (m < M && n < N) C[(int64_t)m * N + n] = acc;
 }
 
-// y[row][c 16 + j] = fl32(sum_i P[c 16 + j][i] x[row][i]), the sum in double: one warp per (row, 16 components).  Rows past
-// n (up to n_out) are zero.
+// y[row][c LP_PC + j] = fl32(sum_i P[c LP_PC + j][i] x[row][i]), the sum in double: one warp per (row, LP_PC components),
+// lane l summing i = l, l + 32, ... in order, then an xor-shuffle tree.  The loads of LP_PU consecutive steps are issued
+// before their FMAs.  (With a warp per 16 components and one step at a time, a batch's queries -- a warp each -- took 79 us
+// at config B: 48 round trips in a row on 15 warps per SM.)  Rows past n (up to n_out) are zero.
+constexpr int LP_PC = 4;
+constexpr int LP_PU = 8;
 __global__ void lp_project_kernel(const uint8_t* __restrict__ rows, size_t stride, int64_t n, int dim, const float* __restrict__ P, int r,
                                   float* __restrict__ y, int64_t n_out) {
     const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32;
     const int lane = threadIdx.x % 32;
-    const int chunks = r / 16;
+    const int chunks = r / LP_PC;
     const int64_t row = w / chunks;
     const int c = (int)(w % chunks);
     if (row >= n_out) return;
-    double acc[16];
+    double acc[LP_PC];
 #pragma unroll
-    for (int j = 0; j < 16; ++j) acc[j] = 0.0;
+    for (int j = 0; j < LP_PC; ++j) acc[j] = 0.0;
     if (row < n) {
         const float* x = reinterpret_cast<const float*>(rows + (size_t)row * stride);
-        const float* p = P + (size_t)c * 16 * dim;
-        for (int i = lane; i < dim; i += 32) {
+        const float* p = P + (size_t)c * LP_PC * dim;
+        int i = lane;
+        for (; i + 32 * (LP_PU - 1) < dim; i += 32 * LP_PU) {
+            float xv[LP_PU], pv[LP_PU][LP_PC];
+#pragma unroll
+            for (int u = 0; u < LP_PU; ++u) {
+                xv[u] = x[i + 32 * u];
+#pragma unroll
+                for (int j = 0; j < LP_PC; ++j) pv[u][j] = __ldg(p + (size_t)j * dim + i + 32 * u);
+            }
+#pragma unroll
+            for (int u = 0; u < LP_PU; ++u)
+#pragma unroll
+                for (int j = 0; j < LP_PC; ++j) acc[j] = fma((double)pv[u][j], (double)xv[u], acc[j]);
+        }
+        for (; i < dim; i += 32) {
             const double xv = x[i];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) acc[j] = fma((double)__ldg(p + (size_t)j * dim + i), xv, acc[j]);
+            for (int j = 0; j < LP_PC; ++j) acc[j] = fma((double)__ldg(p + (size_t)j * dim + i), xv, acc[j]);
         }
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
+        for (int j = 0; j < LP_PC; ++j)
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
     }
     float v = 0.f;
 #pragma unroll
-    for (int j = 0; j < 16; ++j)
+    for (int j = 0; j < LP_PC; ++j)
         if (lane == j) v = (float)acc[j];
-    if (lane < 16) y[(size_t)row * r + c * 16 + lane] = v;
+    if (lane < LP_PC) y[(size_t)row * r + c * LP_PC + lane] = v;
 }
 
-// The bound, from s = fl(sum_j fl(y^x_j - y^q_j)^2) (list_tile_kernel: a sequential fmaf chain over the r components) with
-// y^ the stored fp32 projections, u = 2^-24:
+// The bound, from s = fl(sum_j fl(y^x_j - y^q_j)^2) (a sequential fmaf chain over the r components, as the list-major
+// fp32 kernel list_tile_kernel computes it) with y^ the stored fp32 projections, u = 2^-24:
 //   the sum: each difference rounds once (factor (1 + u)^2 on its square) and the chain of r fmaf rounds r times on
 //     non-negative terms, so a = |y^x - y^q| satisfies a^2 >= s / ((1 + u)^(r + 2)) >= s c1, c1 = 1 - (r + 4) u;
 //   the projections: y^ = fl32(y~) with y~ the double sum, |y^_j - y~_j| <= u |y~_j| and |y~_j - (P x)_j| <= dim 2^-53
@@ -95,37 +113,150 @@ struct LpBound {
     float c1, c2, ce, xmax;
 };
 
-// one warp per (query, probe): the pair's run, slab by slab (32 table-aligned rows of its list), sums -> bounds in place,
-// and the slab minima (vb_common.cuh slab_base) the refine selects from
-__global__ void lp_bound_kernel(float* __restrict__ dist, float* __restrict__ smin, int64_t cap, int64_t cap_s, const int32_t* __restrict__ probe_lists,
-                                int probes, const int32_t* __restrict__ cand_off, const int64_t* __restrict__ list_off, const float* __restrict__ qn,
-                                int64_t nq, LpBound b) {
-    const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32;
-    const int lane = threadIdx.x % 32;
-    if (w >= nq * probes) return;
-    const int64_t q = w / probes;
-    const int p = (int)(w % probes);
-    const int l = probe_lists[w];
-    if (l < 0) return;
-    const int64_t lo = list_off[l], hi = list_off[l + 1];
-    const int32_t co = cand_off[q * (probes + 1) + p];
-    float* run = dist + q * cap + co;
-    const float delta = __fmul_ru(b.ce, __fadd_ru(b.xmax, __fmul_ru(__fsqrt_ru(qn[q]), 1.0f + 1.0f / 1024.0f)));
-    const int64_t sb = slab_base(q, cap_s, co, p);
-    for (int64_t s0 = lo & ~(int64_t)31; s0 < hi; s0 += 32) {
-        const int64_t r = s0 + lane;
-        float v = __int_as_float(0x7F800000);
-        if (r >= lo && r < hi) {
-            float s = run[r - lo];
-            if (s > FLT_MAX) s = FLT_MAX;
-            float t = __fsub_rd(__fsqrt_rd(__fmul_rd(s, b.c1)), delta);
-            if (t < 0.f) t = 0.f;
-            v = __fmul_rd(__fmul_rd(t, t), b.c2);
-            run[r - lo] = v;
-        }
+constexpr int LP_ROWS = 128;             // one table tile (a ListUnit): 4 warps, each one table-aligned 32-row slab
+constexpr int LP_XP = LP_ROWS + 2;       // line of one component across the tile; +2 words make the transposing stores conflict-free
+constexpr int LP_QC = 32;                // queries staged per chunk
+
+struct LpScanArgs {
+    const float* y;              // [rows][r] projections of the rows, list order
+    const float* yq;             // [nq][r] projections of the queries
+    const ListUnit* units;
+    const int64_t* list_off;
+    const int32_t* grp_begin;
+    const int32_t* grp_cnt;
+    const int32_t* pair_q;
+    const int64_t* pair_out;
+    const int32_t* pair_sbase;
+    const float* qn;             // |q|^2
+    float* out;                  // the per-query candidate runs
+    float* smin;                 // slab minima (slab_base(), vb_common.cuh)
+    LpBound b;
+    int r;
+};
+
+static size_t lp_scan_smem(int r) { return sizeof(float) * (size_t)r * (LP_XP + LP_QC); }
+
+// NQ queries (columns j0 .. j0 + NQ - 1 of the staged chunk; all of them real when FULL, else the first nqt - j0) against
+// the thread's row: the distance chains, then per query the bound and its store, and the slab minima, which lane j
+// collects for query j0 + j and stores once.  The minimum is taken on the bit patterns: every bound is +0, positive, +inf
+// or NaN (mapped to the canonical 0x7FFFFFFF, above +inf), whose unsigned order is fminf's, NaN ignored unless the whole
+// slab is NaN -- and min is exact, so any reduction order gives the bits of fminf's butterfly.
+template <int NQ, bool FULL>
+__device__ __forceinline__ void lp_block(const float* __restrict__ Xs, const float* __restrict__ Qs, int r, int j0, int nqt, int tid,
+                                         bool valid, float* const* s_outp, const float* s_delta, float* __restrict__ smin,
+                                         const int32_t* s_sb, int64_t slab, const LpBound& b) {
+    float s[NQ];
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
-        if (smin && lane == 0) smin[sb + ((s0 >> 5) - (lo >> 5))] = v;
+    for (int j = 0; j < NQ; ++j) s[j] = 0.f;
+    for (int d0 = 0; d0 < r; d0 += 16) {
+#pragma unroll
+        for (int dd = 0; dd < 16; ++dd) {
+            const int d = d0 + dd;
+            const float x = Xs[d * LP_XP + tid];
+            float nq[NQ];
+#pragma unroll
+            for (int j = 0; j < NQ; j += 4) {
+                const float4 q4 = *reinterpret_cast<const float4*>(&Qs[d * LP_QC + j0 + j]);
+                nq[j] = q4.x;
+                nq[j + 1] = q4.y;
+                nq[j + 2] = q4.z;
+                nq[j + 3] = q4.w;
+            }
+#pragma unroll
+            for (int j = 0; j < NQ; ++j) {
+                const float e = __fadd_rn(x, nq[j]);
+                s[j] = __fmaf_rn(e, e, s[j]);
+            }
+        }
+    }
+    const int lane = tid % 32;
+    const int nv = FULL ? NQ : nqt - j0;
+    unsigned mine = 0u;
+#pragma unroll
+    for (int j = 0; j < NQ; ++j) {
+        if (!FULL && j >= nv) break;   // block-uniform
+        float sj = s[j];
+        if (sj > FLT_MAX) sj = FLT_MAX;
+        float t = __fsub_rd(__fsqrt_rd(__fmul_rd(sj, b.c1)), s_delta[j0 + j]);
+        if (t < 0.f) t = 0.f;
+        const float v = __fmul_rd(__fmul_rd(t, t), b.c2);
+        if (valid) s_outp[j0 + j][tid] = v;
+        const unsigned key = !valid ? 0x7F800000u : v != v ? 0x7FFFFFFFu : __float_as_uint(v);
+        const unsigned m = __reduce_min_sync(0xffffffffu, key);
+        if (lane == j) mine = m;
+    }
+    if (lane < nv) smin[s_sb[j0 + lane] + slab] = __uint_as_float(mine);
+}
+
+// One CTA per (list, 128-row table tile) unit against every query probing the list: the tile's projected rows are read
+// once, coalesced, into a transposed shared tile, the queries' projections follow in chunks of LP_QC, and each thread
+// (one row) runs up to 8 queries at a time.  Per (row, query): s = fmaf(d, d, s) over j = 0 .. r - 1 from 0 with
+// d = y_x,j + (-y_q,j) (list_tile_kernel's chain, bit for bit), then the bound above stored at pair_out + (row - lo), one
+// coalesced 128-byte store per (warp, query), and the minimum over the warp's slab (rows outside the list: +inf, nothing
+// stored).
+__global__ void __launch_bounds__(LP_ROWS) lp_scan_kernel(LpScanArgs a) {
+    const ListUnit un = a.units[blockIdx.x];
+    const int cnt = a.grp_cnt[un.list];
+    if (cnt == 0) return;   // list not probed by this batch
+
+    extern __shared__ __align__(16) float lp_smem[];
+    const int r = a.r, r4 = a.r / 4;
+    float* Xs = lp_smem;                 // [r][LP_XP] the tile's rows, transposed
+    float* Qs = lp_smem + r * LP_XP;     // [r][LP_QC] the chunk's queries, negated, transposed
+    __shared__ int32_t s_q[LP_QC];
+    __shared__ int32_t s_sb[LP_QC];
+    __shared__ float* s_outp[LP_QC];     // the run entry of the tile's row t0 (thread 0's)
+    __shared__ float s_delta[LP_QC];
+
+    const int tid = threadIdx.x, warp = tid / 32;
+    const int64_t lo = a.list_off[un.list], hi = a.list_off[un.list + 1];
+    const int64_t t0 = (int64_t)un.tile * LP_ROWS, row = t0 + tid, s0 = t0 + 32 * warp;
+    const bool valid = row >= lo && row < hi;
+    const bool warp_rows = s0 < hi && s0 + 32 > lo;   // warp-uniform
+    const int64_t slab = (s0 >> 5) - (lo >> 5);
+    const int gb = a.grp_begin[un.list];
+    const LpBound b = a.b;
+
+    {
+        const float4* src = reinterpret_cast<const float4*>(a.y + (size_t)t0 * r);
+        for (int i = tid; i < LP_ROWS * r4; i += LP_ROWS) {
+            const int rr = i / r4, c = 4 * (i - rr * r4);
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (t0 + rr >= lo && t0 + rr < hi) v = __ldg(src + i);
+            Xs[(c + 0) * LP_XP + rr] = v.x;
+            Xs[(c + 1) * LP_XP + rr] = v.y;
+            Xs[(c + 2) * LP_XP + rr] = v.z;
+            Xs[(c + 3) * LP_XP + rr] = v.w;
+        }
+    }
+
+    for (int c0 = 0; c0 < cnt; c0 += LP_QC) {
+        const int nqt = min(LP_QC, cnt - c0);
+        __syncthreads();   // the previous chunk is done with Qs and the pair arrays
+        if (tid < LP_QC) {
+            const int sl = gb + c0 + min(tid, nqt - 1);   // the chunk's last query fills the unused columns
+            const int q = a.pair_q[sl];
+            s_q[tid] = q;
+            s_outp[tid] = a.out + a.pair_out[sl] + (t0 - lo);
+            s_sb[tid] = a.pair_sbase[sl];
+            s_delta[tid] = __fmul_ru(b.ce, __fadd_ru(b.xmax, __fmul_ru(__fsqrt_ru(a.qn[q]), 1.0f + 1.0f / 1024.0f)));
+        }
+        __syncthreads();
+        for (int i = tid; i < LP_QC * r4; i += LP_ROWS) {
+            const int j = i / r4, c4 = i - j * r4;
+            const float4 v = __ldg(reinterpret_cast<const float4*>(a.yq + (size_t)s_q[j] * r) + c4);
+            Qs[(4 * c4 + 0) * LP_QC + j] = -v.x;
+            Qs[(4 * c4 + 1) * LP_QC + j] = -v.y;
+            Qs[(4 * c4 + 2) * LP_QC + j] = -v.z;
+            Qs[(4 * c4 + 3) * LP_QC + j] = -v.w;
+        }
+        __syncthreads();
+        if (!warp_rows) continue;
+        int j0 = 0;
+        for (; j0 + 8 <= nqt; j0 += 8) lp_block<8, true>(Xs, Qs, r, j0, nqt, tid, valid, s_outp, s_delta, a.smin, s_sb, slab, b);
+        if (nqt - j0 > 4) lp_block<8, false>(Xs, Qs, r, j0, nqt, tid, valid, s_outp, s_delta, a.smin, s_sb, slab, b);
+        else if (nqt - j0 == 4) lp_block<4, true>(Xs, Qs, r, j0, nqt, tid, valid, s_outp, s_delta, a.smin, s_sb, slab, b);
+        else if (nqt > j0) lp_block<4, false>(Xs, Qs, r, j0, nqt, tid, valid, s_outp, s_delta, a.smin, s_sb, slab, b);
     }
 }
 
@@ -165,7 +296,7 @@ static void lp_orthonormalise(std::vector<double>& b, int dim, int c) {
 int list_proj_project(const Table& rows, const ListProj& lp, int64_t first_row, int64_t n_out) {
     if (n_out <= first_row) return VB_OK;
     const int64_t m = n_out - first_row;
-    const int64_t warps = m * (lp.r / 16);
+    const int64_t warps = m * (lp.r / LP_PC);
     lp_project_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, ctx().stream>>>(rows.d + (size_t)first_row * rows.stride, rows.stride,
                                                                                   std::max<int64_t>(rows.n - first_row, 0), rows.dim, lp.P, lp.r,
                                                                                   lp.y + (size_t)first_row * lp.r, m);
@@ -288,27 +419,42 @@ int list_proj_update(const Table& rows, ListProj* lp, int64_t first_row) {
     return list_proj_project(rows, *lp, std::min(first_row, rows.n), rows.n);
 }
 
-int launch_list_proj(Scratch& sc, const Table& rows, const ListProj& lp, float xmax, const void* qimg, size_t qstride, int64_t nq,
+int launch_list_proj(Scratch& sc, const Table& rows, const ListProj& lp, const ListTcImage& im, const void* qimg, size_t qstride, int64_t nq,
                      const int32_t* d_lists, int probes, const int32_t* cand_off, int64_t cap, const int64_t* d_list_off, int n_lists,
-                     const ListTile* d_tiles, int n_tiles, float* out, const float* qn, float* smin, int64_t cap_s) {
+                     float* out, const float* qn, float* smin, int64_t cap_s) {
+    VB_REQUIRE(lp.r > 0 && lp.r % 16 == 0 && lp.y != nullptr, "list scan level P without its projected plane");
+    // (level P's k' is level 0's, and level 0 runs only where the refine takes the slab minima at that k': ivf_scan_topk)
+    VB_REQUIRE(smin != nullptr, "list scan level P without slab minima");
+    if (nq <= 0 || im.n_units <= 0) return VB_OK;
     cudaStream_t s = ctx().stream;
     void* d_yq;
     VB_TRY(sc.take(sizeof(float) * (size_t)nq * lp.r, &d_yq));
-    const int64_t warps = nq * (lp.r / 16);
+    const int64_t warps = nq * (lp.r / LP_PC);
     lp_project_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, s>>>((const uint8_t*)qimg, qstride, nq, rows.dim, lp.P, lp.r,
                                                                          (float*)d_yq, nq);
     VB_CUDA(cudaGetLastError());
     count_launch();
-    Table yt;
-    yt.elem = VB_VECTOR;
-    yt.dim = lp.r;
-    yt.stride = sizeof(float) * (size_t)lp.r;
-    yt.n = yt.cap = rows.n;
-    yt.d = (uint8_t*)lp.y;
-    VB_TRY(launch_list_major(yt, VB_L2_SQUARED, d_yq, yt.stride, nq, d_lists, probes, cand_off, cap, d_list_off, n_lists, d_tiles, n_tiles, out));
-    LpBound b{lp.c1, lp.c2, lp.ce, __builtin_nextafterf(xmax * (1.0f + 1.0f / 1024.0f), FLT_MAX)};
-    lp_bound_kernel<<<(unsigned)((nq * probes * 32 + 255) / 256), 256, 0, s>>>(out, smin, cap, cap_s, d_lists, probes, cand_off, d_list_off, qn,
-                                                                             nq, b);
+    QueryGroups g{};
+    VB_TRY(build_query_groups(sc, d_lists, nq, probes, cand_off, cap, n_lists, 0, &g, cap_s));
+    const size_t smem = lp_scan_smem(lp.r);
+    VB_REQUIRE(smem <= 227 * 1024, "level P: r = %d needs %zu bytes of shared memory", lp.r, smem);
+    if (smem > 48 * 1024) VB_CUDA(cudaFuncSetAttribute(lp_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LpScanArgs a{};
+    a.y = lp.y;
+    a.yq = (const float*)d_yq;
+    a.units = im.units;
+    a.list_off = d_list_off;
+    a.grp_begin = g.begin;
+    a.grp_cnt = g.cnt;
+    a.pair_q = g.pair_q;
+    a.pair_out = g.pair_out;
+    a.pair_sbase = g.pair_sbase;
+    a.qn = qn;
+    a.out = out;
+    a.smin = smin;
+    a.b = LpBound{lp.c1, lp.c2, lp.ce, __builtin_nextafterf(im.xmax * (1.0f + 1.0f / 1024.0f), FLT_MAX)};
+    a.r = lp.r;
+    lp_scan_kernel<<<(unsigned)im.n_units, LP_ROWS, smem, s>>>(a);
     VB_CUDA(cudaGetLastError());
     count_launch();
     return VB_OK;
